@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
-"""bench.py -- CT entries/sec through the B200-native map/reduce hot path.
+"""bench.py -- CT entries/sec through the H100-native map/reduce hot path.
 
     python bench.py --gpus N --steps K --warmup W            # this repository's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU algorithm (Go engine if `go` exists, else the oracle port)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one pass of the hot path over one batch of synthetic CT entries resident in HBM (BASELINE.json
 configs[1] at N=1: 10 M x ~1.5 KB DER, SHA-256 fingerprint + KnownCertificates dedup, per-issuer counts).  At N>1
@@ -74,15 +75,19 @@ def parse_args():
     ap.add_argument("--no-secondary", action="store_true", help="skip the BASELINE configs[2..4] streaming runs")
     ap.add_argument("--secondary-entries", type=int, default=0, help="entries per GPU of each streaming run (default: as written)")
     ap.add_argument("--cpu-sample", type=int, default=0, help="entries in the CPU sample (default: auto)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write rank 0's outputs of the last timed step as DIR/<name>.npy (float32/float64; a fixed, seeded "
+                         "sample of entries when the batch is large)")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks, power limit and throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,"
+         "power.limit,name")
 
     def __init__(self, gpu_index: int):
         self.rows = []
@@ -111,35 +116,27 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons, power = [], [], set(), []
+        sm, mx, reasons, power, limit, gpu_name = [], [], set(), [], [], None
         for r in self.rows:
             f = [x.strip() for x in r.split(",")]
-            if len(f) < 9:
+            if len(f) < 11:
                 continue
             try:
                 sm.append(float(f[1])); mx.append(float(f[2])); power.append(float(f[3]))
             except ValueError:
                 continue
+            try:
+                limit.append(float(f[9]))
+            except ValueError:
+                pass
+            gpu_name = f[10]
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "power_w_max": max(power) if power else None, "samples": len(sm), "reasons": sorted(reasons)}
-
-
-def measured_traffic(kernel, entries_per_launch):
-    """dram__bytes_read+write of a kernel from the committed ncu --set full capture (profiles/), scaled from the
-    captured launch size to this run's entries per launch; None when no capture is committed."""
-    for name in (f"r2_{kernel}_traffic.json", "r1_map_traffic.json" if kernel == "map_stream" else ""):
-        p = os.path.join(ROOT, "profiles", name)
-        try:
-            t = json.load(open(p))
-            per_entry = (t["dram_bytes_read"] + t["dram_bytes_write"]) / t["entries"]
-            return per_entry * entries_per_launch, t["source"]
-        except Exception:
-            continue
-    return None, None
+                "power_w_max": max(power) if power else None, "power_limit_w": min(limit) if limit else None, "gpu": gpu_name,
+                "samples": len(sm), "reasons": sorted(reasons)}
 
 
 def measured_peaks():
@@ -149,7 +146,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback: H100 SXM data sheet, 3.35 TB/s (not measured)"
 
 
 # ---------------------------------------------------------------------------------------------- reference arm
@@ -161,8 +158,8 @@ def host_threads():
 
 
 def go_probe():
-    """BASELINE.md §3 Variant A / SURVEY §8(c): use the Go engine when the box has a Go toolchain AND the reference's
-    module dependencies are resolvable offline.  Returns (usable, one-line description)."""
+    """BASELINE.md §3 Variant A / SURVEY §8(c): what the box offers for running the Go engine.  The reference's Go
+    sources are not part of this repository, so it is never usable from here.  Returns (usable, one-line description)."""
     go = shutil.which("go")
     if not go:
         return False, "`go version`: command not found on this box"
@@ -170,14 +167,7 @@ def go_probe():
         ver = subprocess.run([go, "version"], capture_output=True, text=True, timeout=20).stdout.strip()
     except Exception as e:  # noqa: BLE001
         return False, f"`go version` failed: {e}"
-    ref = "/root/reference"
-    if not os.path.isdir(ref):
-        return False, f"{ver}; the reference sources (/root/reference) are not on this box"
-    env = dict(os.environ, GOFLAGS="-mod=mod", GOPROXY="off")
-    r = subprocess.run([go, "list", "./storage"], cwd=ref, capture_output=True, text=True, env=env, timeout=120)
-    if r.returncode != 0:
-        return False, f"{ver}; `go list ./storage` fails offline (certificate-transparency-go v1.1.0 not in the module cache)"
-    return True, ver
+    return False, f"{ver}; the reference's Go sources are not part of this repository"
 
 
 def cpu_arm(n_sample, workload, steps, warmup, make_sample, map_only_too=False):
@@ -249,6 +239,32 @@ def run_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------- our arm
+DUMP_SAMPLE = 131072   # entries dumped when the batch is larger: 131072 x (32 fingerprint bytes + 4 fields) in float32 = 18.9 MB
+
+
+def dump_outputs(out_dir, per_entry, counts, stat):
+    """The last timed step's outputs as float32 / float64 .npy files: per-entry arrays at a fixed, seeded sample of
+    entry indices (every entry when the batch is small enough), the per-issuer counts and status counters whole."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    n = per_entry["status"].shape[0]
+    if n <= DUMP_SAMPLE:
+        pick = np.arange(n, dtype=np.int64)
+    else:
+        pick = np.sort(np.random.default_rng(SEED).choice(n, DUMP_SAMPLE, replace=False))
+    sel = torch.from_numpy(pick).to(per_entry["status"].device)
+    np.save(os.path.join(out_dir, "entry_index.npy"), pick.astype(np.float64))
+    for name, t in per_entry.items():
+        if t is None:
+            continue
+        v = t[sel].cpu().numpy()
+        # exp_hour (int64 hours since the epoch) is exact in float64; bytes and bits are exact in float32
+        np.save(os.path.join(out_dir, name + ".npy"), v.astype(np.float64 if v.dtype == np.int64 else np.float32))
+    np.save(os.path.join(out_dir, "issuer_counts.npy"), counts.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "status_counters.npy"), stat.cpu().numpy().astype(np.float64))
+
+
 def main():
     args = parse_args()
     if args.impl == "reference":
@@ -274,7 +290,7 @@ def main():
     dev = torch.device("cuda", local)
     build.build()
     lib = capi.load()
-    # pinned buffers allocated from here on are local to the GPU's NUMA node (8 ranks x 56 GB/s of host reads)
+    # pinned buffers allocated from here on are local to the GPU's NUMA node (every rank reads its own host buffers)
     numa_node = lib.ctmr_bind_host_to_device(local) if os.environ.get("CTMR_BENCH_NUMA", "1") == "1" else -2
     if world > 1:
         if same_gpu:
@@ -381,6 +397,9 @@ def main():
     map_ms = allmax(db.profile_last()[0])   # K_map's CUDA-event duration (sum over the step's 4 launches) in the LAST timed step
     db.check_device(stream.cuda_stream)
     counts, stat = hist[: cfg.n_issuers].clone(), hist[cfg.n_issuers:].clone()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(status=status, sha256=None if args.no_fingerprint else sha, exp_hour=exp_hour,
+                                             was_unknown=was_unknown, first_issuer_hour=first), counts, stat)
 
     # ---- the timed result is the real thing: size-independent checks on the LAST timed step's outputs ----------
     truth_id = torch.empty(n, dtype=torch.int64, device=dev)
@@ -460,8 +479,6 @@ def main():
     # per round: len_order (3 kernels) + K_map + resolve + pairs; N>1 adds 2 barrier kernels per round, 2 around the reset,
     # and barrier + sum + barrier for the histogram all-reduce
     launches_per_step = map_launches * 6 + (map_launches * 2 + 2 + 3 if world > 1 else 0)
-    kname = "map_light" if args.no_fingerprint else "map_stream"
-    traffic, traffic_src = measured_traffic(kname, n / map_launches)
 
     # ---- e2e through the host-buffer C ABI (pinned host memory -> results on the host); at N>1 the same exact
     # multi-GPU path: a collective ctmr_process_batch per rank, keys inserted at their owners over NVLink
@@ -592,10 +609,9 @@ def main():
                 total_entries = world * chunks * nc
                 algb = tot_bytes + w2["out_bytes"] * chunks * nc
                 nofp = bool(fl & capi.F_NO_FINGERPRINT)
-                tr, trs = measured_traffic("map_light" if nofp else "map_stream", nc / R)
                 rl = {"bound": "hbm" if nofp else "int_alu", "kernel": "map_light_kernel" if nofp else "map_stream_kernel",
                       "hbm": {"achieved": algb / (mms / 1e3) / 1e9, "peak": peak, "unit": "GB/s", "frac": algb / (mms / 1e3) / 1e9 / peak},
-                      "kernel_ms_total": mms, "traffic_per_launch": tr, "traffic_source": trs}
+                      "kernel_ms_total": mms}
                 if not nofp and int_ceiling_gbs:
                     rl.update(achieved=tot_bytes / (mms / 1e3) / 1e9, peak=int_ceiling_gbs, unit="GB/s of message bytes",
                               frac=tot_bytes / (mms / 1e3) / 1e9 / int_ceiling_gbs)
@@ -696,7 +712,6 @@ def main():
                     "kernel": "map_light_kernel" if args.no_fingerprint else "map_stream_kernel<8,128,0,1>",
                     "hbm": {"achieved": hbm_achieved, "peak": peak, "unit": "GB/s", "frac": hbm_achieved / peak, "peak_source": peak_src,
                             "algorithmic_bytes_per_step": int(alg_bytes), "algorithmic_bytes_per_launch": int(alg_bytes / map_launches)},
-                    "traffic": traffic, "traffic_source": traffic_src,
                     "kernel_ms_per_step": map_ms, "kernel_ms": map_ms / map_launches, "launches_per_step": map_launches}
         if args.no_fingerprint:
             roofline.update(achieved=hbm_achieved, peak=peak, unit="GB/s", frac=hbm_achieved / peak)
@@ -713,7 +728,7 @@ def main():
             "dtype": "u32", "data": "synthetic",
             "config": {"workload": wl["desc"] + (" [fingerprint OFF: reference-faithful path]" if args.no_fingerprint else ""),
                        "entries_per_gpu_per_step": n, "bytes_per_gpu_per_step": int(total_bytes),
-                       "issuers": cfg.n_issuers, "l2": "inputs (>=7 GB per step) far exceed the 126 MB L2; no explicit flush",
+                       "issuers": cfg.n_issuers, "l2": "inputs (>=7 GB per step) far exceed the 50 MB L2; no explicit flush",
                        "parallelism": (f"entry-index shards x{world}; every set serials::<expDate>::<issuer> owned by one GPU, K_map inserts "
                                        f"into the owner's table over NVLink (peer atomics), {2 * map_launches} peer-memory barriers + 1 "
                                        "histogram all-reduce per step; no NCCL on the data path") if world > 1 else "single GPU",

@@ -1,9 +1,9 @@
-"""Builds libctmr.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc.
+"""Builds libctmr.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc.
 
     python -m ct_mapreduce_b200.build [--force] [--verbose]
 
-nvcc cross-compiles for sm_100a without a GPU; the .so lands next to this file so that it
-travels to the GPU box with the repository snapshot.
+nvcc cross-compiles for sm_90a without a GPU; the .so lands next to this file, where capi.load()
+looks for it.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ DEPS = SOURCES + EXPERIMENT_SOURCES + ["ctmr_ctx.cuh", "ctmr_kernels.cuh", "ctmr
                   os.path.join("..", "..", "include", "ctmr.h"), os.path.join("..", "..", "include", "ctmr_frontend.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

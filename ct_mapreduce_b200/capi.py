@@ -1,6 +1,6 @@
 """ctypes binding of libctmr.so (include/ctmr.h) -- the same C ABI a Go host binds with cgo.
 
-The library is hand-written CUDA for sm_100a; there is no Python or CPU implementation of the path
+The library is hand-written CUDA for sm_90a; there is no Python or CPU implementation of the path
 behind these calls.  `load()` raises if the shared object is missing instead of falling back.
 """
 from __future__ import annotations

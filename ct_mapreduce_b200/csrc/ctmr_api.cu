@@ -496,8 +496,8 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
     CUC(cudaSetDevice(c->device));
     cudaDeviceProp prop;
     CUC(cudaGetDeviceProperties(&prop, c->device));
-    if (prop.major < 10) {
-        c->err = "libctmr is built for sm_100a (B200) only";
+    if (prop.major != 9 || prop.minor != 0) {
+        c->err = "libctmr is built for sm_90a (H100) only";
         return bail(CTMR_E_NO_DEVICE);
     }
     c->sm_count = prop.multiProcessorCount;
@@ -772,7 +772,7 @@ int ctmr_map_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o,
             c->order_cap = b->n;
         }
         if (!c->len_hist) CU(c, cudaMalloc(&c->len_hist, 256 * sizeof(unsigned int)));
-        CU(c, launch_len_order(b->offsets, b->lens, b->n, b->blob_bytes, c->len_hist, c->order_scratch, s));
+        CU(c, launch_len_order(b->offsets, b->lens, b->n, b->blob_bytes, c->len_hist, c->order_scratch, c->sm_count, s));
         p.order = c->order_scratch;
     }
     CU(c, launch_map(p, c->sm_count, s));
@@ -881,7 +881,7 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
         rc = round_begin(c, parity, sa);
         if (rc) return rc;
         if (c->bucket_by_length && cnt > 64 && p.sha256) {
-            CU(c, launch_len_order(sb.offsets, sb.lens, cnt, sb.blob_bytes, c->len_hist_sub[k], c->order_scratch + lo, sa));
+            CU(c, launch_len_order(sb.offsets, sb.lens, cnt, sb.blob_bytes, c->len_hist_sub[k], c->order_scratch + lo, c->sm_count, sa));
             p.order = c->order_scratch + lo;
         }
         CU(c, launch_map(p, c->sm_count, sa));
@@ -1263,7 +1263,7 @@ int ctmr_table_stats(ctmr_ctx* c, uint64_t* used, uint64_t* capacity) {
     CU(c, cudaSetDevice(c->device));
     unsigned long long u = 0;
     CU(c, cudaMemsetAsync(c->small_dev + 81, 0, sizeof(unsigned long long), c->stream));
-    CU(c, launch_table_count(c->st, c->small_dev + 81, c->stream));
+    CU(c, launch_table_count(c->st, c->small_dev + 81, c->sm_count, c->stream));
     CU(c, cudaMemcpyAsync(&u, c->small_dev + 81, sizeof u, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     if (used) *used = u;
@@ -1280,17 +1280,17 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     unsigned long long counters[2] = {0, 0};
     unsigned long long* dev = c->small_dev + 92;  // [92] live, [93] expired, [94] compaction cursor
     CU(c, cudaMemsetAsync(dev, 0, 3 * sizeof(unsigned long long), c->stream));
-    CU(c, launch_evict_count(c->st, now_unix_sec, dev, c->stream));
+    CU(c, launch_evict_count(c->st, now_unix_sec, dev, c->sm_count, c->stream));
     CU(c, cudaMemcpyAsync(counters, dev, sizeof counters, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     if (evicted_out) *evicted_out = counters[1];
     if (counters[1] == 0) return CTMR_OK;
-    CU(c, launch_evict_pairs(c->st, now_unix_sec, c->stream));  // the expired sets' cardinalities are 0 again
+    CU(c, launch_evict_pairs(c->st, now_unix_sec, c->sm_count, c->stream));  // the expired sets' cardinalities are 0 again
     // open addressing with linear probing: taking slots out would cut probe chains, so the survivors are
     // compacted aside, the table is cleared and they are inserted again (first-seen indices preserved)
     KnownSlot* keep = nullptr;
     if (counters[0]) CU(c, cudaMalloc(&keep, counters[0] * sizeof(KnownSlot)));
-    if (counters[0]) CU(c, launch_evict_compact(c->st, now_unix_sec, keep, dev + 2, c->stream));
+    if (counters[0]) CU(c, launch_evict_compact(c->st, now_unix_sec, keep, dev + 2, c->sm_count, c->stream));
     CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), c->stream));
     CU(c, launch_evict_reinsert(c->st, keep, counters[0], c->stream));
     CU(c, cudaStreamSynchronize(c->stream));

@@ -141,7 +141,7 @@ enum : uint32_t {
 
 struct ctmr_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     uint32_t flags = 0;
     cudaStream_t stream = nullptr;
     DeviceState st{};

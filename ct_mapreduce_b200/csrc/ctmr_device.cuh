@@ -1,4 +1,4 @@
-// ctmr_device.cuh -- device-side building blocks of the CT map path (sm_100a).
+// ctmr_device.cuh -- device-side building blocks of the CT map path (sm_90a).
 //
 //   * SHA-256 compression held entirely in registers (8 state + 16 rolling schedule words);
 //     rotations are funnel shifts (SHF.R.W), Ch/Maj/xor3 fold into LOP3, round constants are
@@ -34,11 +34,11 @@ struct Sha256State {
 };
 
 // Additions are steered onto the FMA pipe.  Rotations (SHF) and the boolean functions (LOP3) can
-// only issue on the ALU datapath, and ncu showed that datapath as the binding unit (ALU 61-74 %
-// busy, FMA 4-6 %) because ptxas turns every add into IADD3 -- including `mad.lo x, 1, y`, which
-// it folds back.  Multiplying by a run-time 1 (a kernel parameter it cannot fold) keeps a genuine
-// IMAD, which issues on the otherwise idle FMA datapath: per 64-byte block ~1090 ALU + ~460 FMA
-// instructions instead of ~1290 ALU + 160 FMA (profiles/, DESIGN.md "K_map").
+// only issue on the ALU datapath, and that datapath is the binding unit while the FMA datapath
+// idles, because ptxas turns every add into IADD3 -- including `mad.lo x, 1, y`, which it folds
+// back.  Multiplying by a run-time 1 (a kernel parameter it cannot fold) keeps a genuine IMAD,
+// which issues on the otherwise idle FMA datapath and takes the adds off the ALU pipe
+// (DESIGN.md §3, K_map).
 __device__ __forceinline__ uint32_t fadd(uint32_t a, uint32_t b, uint32_t one) {
     uint32_t d;
     asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(one), "r"(b));
@@ -98,9 +98,8 @@ __device__ __forceinline__ void sha256_compress(Sha256State& s, uint32_t (&w)[16
 }
 
 // Same compression with the 64 rounds rolled into 4 passes of 16 (round constants from the constant
-// bank instead of immediates).  ~7 KB of code instead of ~26 KB: ncu charged 20 % of warp time to
-// "no_instruction" (instruction-cache misses) on the fully unrolled body once 8-16 desynchronised
-// warps per SM walk it at different offsets.
+// bank instead of immediates).  ~7 KB of code instead of ~26 KB: the fully unrolled body misses in
+// the instruction cache once 8-16 desynchronised warps per SM walk it at different offsets.
 static __constant__ uint32_t kSha256K[64] = {
     0x428a2f98u, 0x71374491u, 0xb5c0fbcfu, 0xe9b5dba5u, 0x3956c25bu, 0x59f111f1u, 0x923f82a4u, 0xab1c5ed5u,
     0xd807aa98u, 0x12835b01u, 0x243185beu, 0x550c7dc3u, 0x72be5d74u, 0x80deb1feu, 0x9bdc06a7u, 0xc19bf174u,

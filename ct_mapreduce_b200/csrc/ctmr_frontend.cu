@@ -19,9 +19,9 @@ namespace ctmr {
 namespace {
 
 // ASCII -> 6-bit value, 0xFF = not in the standard alphabet ('=' included: padding is handled by position).
-// One 256-byte table per CTA.  A per-lane replicated table (32 KB, conflict-free look-ups) was measured and
-// rejected: 246 vs 195 us per 60 k entries -- the kernel is bound by loads in flight, and the larger table
-// costs two resident CTAs per SM.
+// One 256-byte table per CTA.  A per-lane replicated table (32 KB, conflict-free look-ups) was measured before
+// the port and rejected as slower: the kernel is bound by loads in flight, and the larger table costs two
+// resident CTAs per SM.
 __device__ __forceinline__ void fill_b64_lut(uint8_t* lut) {
     for (uint32_t c = threadIdx.x; c < 256u; c += blockDim.x) {
         uint32_t v = 0xFFu;

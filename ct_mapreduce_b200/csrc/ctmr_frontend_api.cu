@@ -350,7 +350,7 @@ int group_round(ctmr_group* g, RawChunk* ch, int parity, ctmr_ctx** failed) {
                     c->order_cap = cnt;
                 }
                 if (!c->len_hist) CU(c, cudaMalloc(&c->len_hist, 256 * sizeof(unsigned int)));
-                CU(c, launch_len_order(ch[r].db.offsets, ch[r].db.lens, cnt, ch[r].db.blob_bytes, c->len_hist, c->order_scratch, s));
+                CU(c, launch_len_order(ch[r].db.offsets, ch[r].db.lens, cnt, ch[r].db.blob_bytes, c->len_hist, c->order_scratch, c->sm_count, s));
                 p.order = c->order_scratch;
             }
             CU(c, launch_map(p, c->sm_count, s));

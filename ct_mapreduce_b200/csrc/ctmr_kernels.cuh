@@ -45,8 +45,8 @@ struct __align__(16) MetaSlot {      // IssuerMetadata string sets: identity = t
 
 // Multi-GPU (SURVEY.md §8(e)): every set "serials::<expDate>::<issuer>" has ONE owner GPU
 // (key_owner(exp_hour, issuer, world)), which holds its serials and its (issuer, hour) slot, and does every table
-// operation on them with device-scope atomics in its own HBM.  What crosses NVLink is BULK traffic only (measured:
-// fine-grained remote atomics run at ~0.4 G ops/s per GPU and made K_map 4x slower, profiles/r2_peer_atomics_2gpu.json):
+// operation on them with device-scope atomics in its own HBM.  What crosses NVLink is BULK traffic only (measured before
+// the port: fine-grained remote atomics are limited by the rate of remote operations and made K_map several times slower):
 // K_map appends the 64-byte key record of an entry owned elsewhere to a per-source region of the owner's INBOX
 // (coalesced posted writes, cursors in local memory), the owner inserts / resolves its inbox after a barrier, and the
 // source pulls the result bits back as contiguous arrays.  The peers' memory is mapped into every rank (peer access
@@ -171,7 +171,7 @@ cudaError_t launch_map_v1(const MapParams& p, int sm_count, cudaStream_t s);  //
 cudaError_t launch_map_v3(const MapParams& p, int sm_count, cudaStream_t s);  // ctmr_map_alt.cu
 cudaError_t launch_sha_ceiling(uint32_t iters, int rolled, int ctas_per_sm, int sm_count, uint32_t* sink, cudaStream_t s);
 cudaError_t launch_len_order(const uint64_t* offsets, const uint32_t* lens, uint64_t n, uint64_t blob_bytes, unsigned int* hist256, uint32_t* order,
-                             cudaStream_t s);
+                             int sm_count, cudaStream_t s);
 cudaError_t launch_insert(const DeviceState& st, const ctmr_key* keys, uint64_t m, uint32_t* slot_of, cudaStream_t s);
 cudaError_t launch_resolve(const DeviceState& st, const ctmr_key* keys, uint64_t m, const uint32_t* slot_of,
                            uint32_t* pair_slot, uint8_t* was_unknown, cudaStream_t s);
@@ -197,7 +197,7 @@ cudaError_t launch_meta_insert(const DeviceState& st, const uint8_t* blob, const
                                const uint32_t* crl_len, uint32_t* meta_slots, cudaStream_t s);
 cudaError_t launch_meta_resolve(const DeviceState& st, const ctmr_key* keys, uint64_t m, const uint32_t* meta_slots, uint8_t* first_dn,
                                 uint8_t* first_crl, cudaStream_t s);
-cudaError_t launch_evict_pairs(const DeviceState& st, int64_t now_sec, cudaStream_t s);
+cudaError_t launch_evict_pairs(const DeviceState& st, int64_t now_sec, int sm_count, cudaStream_t s);
 cudaError_t launch_issuer_registry(const IssuerRegistry& reg, const uint8_t* digests, const uint8_t* ok, uint32_t n, uint32_t* idx_out,
                                    int* error_flag, cudaStream_t s);
 cudaError_t launch_peer_post(const PeerFlags& pf, unsigned long long value, cudaStream_t s);
@@ -206,9 +206,10 @@ cudaError_t launch_hist_sum(const PeerFlags& pf, uint32_t n_slots, unsigned long
                             cudaStream_t s);
 cudaError_t launch_issuer_prepare(const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint8_t* digests,
                                   uint8_t* ok, cudaStream_t s);
-cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, cudaStream_t s);
-cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters /* [2] */, cudaStream_t s);
-cudaError_t launch_evict_compact(const DeviceState& st, int64_t now_sec, KnownSlot* keep, unsigned long long* cursor, cudaStream_t s);
+cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, int sm_count, cudaStream_t s);
+cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters /* [2] */, int sm_count, cudaStream_t s);
+cudaError_t launch_evict_compact(const DeviceState& st, int64_t now_sec, KnownSlot* keep, unsigned long long* cursor, int sm_count,
+                                 cudaStream_t s);
 cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, cudaStream_t s);
 cudaError_t launch_cardinality(const DeviceState& st, int32_t exp_hour, uint32_t issuer, unsigned long long* out,
                                cudaStream_t s);

@@ -1,4 +1,4 @@
-// ctmr_map.cu -- the map half of the CT-entry hot path: hand-written sm_100a kernels.
+// ctmr_map.cu -- the map half of the CT-entry hot path: hand-written sm_90a kernels.
 //
 // K_map        (map_stream_kernel<8,128,0,1>) lane-per-certificate map: DER walk + certIsFilteredOut + SHA-256(leaf DER).
 //              Each lane streams ITS certificate through a private double-buffered shared-memory window filled by
@@ -49,10 +49,10 @@ __device__ __forceinline__ void route_append(const RouteOut& r, bool remote, uin
 // names, validity, the extension headers, the trailing signature header) and skips the key,
 // the padding and the signature.  So: no shared memory, one thread per certificate, byte loads
 // through L1 (the full 256 KB is available as cache), 32 resident warps per SM to hide the pointer
-// chase.  The streaming kernel, which must stage every byte, tops out at ~2.0 TB/s here.
+// chase.  The streaming kernel, which must stage every byte, is slower on this path.
 // ------------------------------------------------------------------------------------------------
-// 6 resident CTAs per SM (40 registers, 60 bytes of spills): +9 % over 4 CTAs (56 registers), 8 CTAs (32 registers) spill too much
-// (profiles/r2_ab_light_occupancy.log)
+// 6 resident CTAs per SM (40 registers, a few bytes of spills) ran faster than 4 CTAs (56 registers) when measured before the
+// port; 8 CTAs (32 registers) spill too much
 __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant__ MapParams p) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool act = e < p.n;
@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant
         const uint32_t L = bad_span ? 0u : (uint32_t)(end - off);
         const uint8_t* d = p.blob + off;
         if (p.light_prefetch && L) {
-            // The walk is a pointer chase (ncu: 19 long-scoreboard stalls per issue, DRAM 25 % busy): start the lines it is
+            // The walk is a pointer chase (latency bound, not bandwidth bound): start the lines it is
             // going to need -- header, serial, names, validity at the front; signatureAlgorithm + signature header at the
             // back -- before the first dependent load, so that they arrive in parallel
             const uint8_t* base = reinterpret_cast<const uint8_t*>(reinterpret_cast<uint64_t>(d) & ~127ull);
@@ -414,7 +414,7 @@ static cudaError_t launch_stream_t(const MapParams& p, int sm_count, int ctas_pe
 // ------------------------------------------------------------------------------------------------
 // Length bucketing: a counting sort of the batch's entries by their number of streaming chunks,
 // longest first.  K_map then gives each warp 32 records of (nearly) equal length, so a warp no
-// longer waits for its longest record (mixed 512 B..8 KB input: 292 -> see DESIGN.md GB/s), and the
+// longer waits for its longest record (this matters on mixed 512 B..8 KB input), and the
 // longest records are started first (LPT order) so the grid drains evenly.  Three tiny kernels:
 // histogram over 256 buckets, 256-entry scan, scatter.
 // ------------------------------------------------------------------------------------------------
@@ -441,7 +441,7 @@ __global__ void __launch_bounds__(256) len_hist_kernel(const uint64_t* __restric
 }
 
 // exclusive scan of the 256 bucket counts by ONE WARP (8 buckets per lane + a shuffle scan): this tiny kernel sits on
-// K_map's stream in front of every launch, where a single-thread loop cost 33 us (profiles/r2_launches_10M.csv)
+// K_map's stream in front of every launch, where a single-thread loop sat on the critical path
 __global__ void len_scan_kernel(unsigned int* hist_then_cursor) {
     const uint32_t lane = threadIdx.x;
     unsigned int v[8], sum = 0;
@@ -480,12 +480,13 @@ __global__ void __launch_bounds__(256) len_scatter_kernel(const uint64_t* __rest
 }
 
 cudaError_t launch_len_order(const uint64_t* offsets, const uint32_t* lens, uint64_t n, uint64_t blob_bytes, unsigned int* hist256, uint32_t* order,
-                             cudaStream_t s) {
+                             int sm_count, cudaStream_t s) {
     if (!n) return cudaSuccess;
     cudaError_t err = cudaMemsetAsync(hist256, 0, kLenBuckets * sizeof(unsigned int), s);
     if (err != cudaSuccess) return err;
     const unsigned hb = (unsigned)((n + 256 * 8 - 1) / (256 * 8));
-    len_hist_kernel<<<hb < 148u * 8u ? (hb ? hb : 1u) : 148u * 8u, 256, 0, s>>>(offsets, lens, n, blob_bytes, hist256);
+    const unsigned cap = (unsigned)sm_count * 8u;
+    len_hist_kernel<<<hb < cap ? (hb ? hb : 1u) : cap, 256, 0, s>>>(offsets, lens, n, blob_bytes, hist256);
     len_scan_kernel<<<1, 32, 0, s>>>(hist256);
     len_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(offsets, lens, n, blob_bytes, hist256, order);
     return cudaGetLastError();
@@ -528,8 +529,8 @@ cudaError_t launch_sha_ceiling(uint32_t iters, int rolled, int ctas_per_sm, int 
     return cudaGetLastError();
 }
 
-// Shape of the persistent grid = the measured best (DESIGN.md "K_map tuning").  A build with
-// CTMR_EXPERIMENTS=1 adds the environment overrides used for the A/B runs recorded under profiles/.
+// Shape of the persistent grid = the best measured before the port (DESIGN.md §3, K_map).  A build with
+// CTMR_EXPERIMENTS=1 adds the environment overrides used for the A/B runs (tools/ab_*.sh).
 cudaError_t launch_map(const MapParams& p, int sm_count, cudaStream_t s) {
     if (p.n == 0) return cudaSuccess;
     static const int light = env_int("CTMR_MAP_LIGHT", 1);

@@ -1,5 +1,5 @@
 // ctmr_map_alt.cu -- MEASURED ALTERNATIVES of K_map, kept selectable (CTMR_MAP_VARIANT=1|3) because the
-// numbers in DESIGN.md "Measured and rejected" come from them and they pass the same parity suite:
+// verdicts in DESIGN.md "Measured and rejected" come from them and they pass the same parity suite:
 //   v1  DER walk on global memory (LDG.U8) + per-lane TMA bulk copies for the SHA-256 stream
 //   v3  streaming kernel with per-lane dynamic scheduling (loader cursor two slots ahead)
 #include "ctmr_common.cuh"
@@ -226,7 +226,7 @@ cudaError_t launch_map_v1(const MapParams& p, int sm_count, cudaStream_t s) {
 //
 // In v2 a warp takes 32 consecutive records and runs until its longest record is done, so on
 // mixed-size input (BASELINE configs[4]: 512 B..8 KB) lanes idle for most of the time (measured
-// 294 GB/s vs 626 GB/s on uniform sizes).  Here every lane owns an endless stream of "slots"
+// before the port at less than half the uniform-size rate).  Here every lane owns an endless stream of "slots"
 // (one slot = one CHUNK of one record); a loader cursor runs exactly two slots ahead of the consumer
 // cursor and crosses record boundaries on its own, so the first chunks of a lane's NEXT record are
 // already in flight while it finishes the current one.  Records are handed out from a warp-local

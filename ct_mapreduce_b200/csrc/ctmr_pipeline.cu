@@ -223,7 +223,7 @@ int issue_map(ctmr_ctx* c, Stage& s, int sidx, const BatchArgs& a, const Slice& 
         MapParams p;
         fill_map_params(c, &db, &dout, p, sidx, fused ? s.slot_of : nullptr, sidx);
         if (c->bucket_by_length && cnt > 64 && p.sha256) {
-            CU(c, launch_len_order(s.offsets, nullptr, cnt, db.blob_bytes, s.len_hist, s.order, s.stream));
+            CU(c, launch_len_order(s.offsets, nullptr, cnt, db.blob_bytes, s.len_hist, s.order, c->sm_count, s.stream));
             p.order = s.order;
         }
         CU(c, launch_map(p, c->sm_count, s.stream));
@@ -481,7 +481,7 @@ int ctmr_group_create(const ctmr_config* cfg, const int32_t* devices, uint32_t n
         c->group = g;
         g->m.push_back(c);
     }
-    // peer access between the distinct devices (NVLink through NVSwitch on a B200 box)
+    // peer access between the distinct devices (NVLink through NVSwitch on an H100 box)
     for (uint32_t r = 0; r < n_devices; ++r)
         for (uint32_t q = 0; q < n_devices; ++q) {
             if (devices[r] == devices[q]) continue;

@@ -428,12 +428,13 @@ __global__ void __launch_bounds__(256) evict_reinsert_kernel(DeviceState st, con
     known_insert<false>(st.table, st.table_mask, st.error_flag, body, keep[i].inv_first);  // a rank only ever holds keys it owns
 }
 
-cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters, cudaStream_t s) {
-    evict_count_kernel<<<148 * 8, 256, 0, s>>>(st, now_sec, counters);
+cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters, int sm_count, cudaStream_t s) {
+    evict_count_kernel<<<sm_count * 8, 256, 0, s>>>(st, now_sec, counters);
     return cudaGetLastError();
 }
-cudaError_t launch_evict_compact(const DeviceState& st, int64_t now_sec, KnownSlot* keep, unsigned long long* cursor, cudaStream_t s) {
-    evict_compact_kernel<<<148 * 8, 256, 0, s>>>(st, now_sec, keep, cursor);
+cudaError_t launch_evict_compact(const DeviceState& st, int64_t now_sec, KnownSlot* keep, unsigned long long* cursor, int sm_count,
+                                 cudaStream_t s) {
+    evict_compact_kernel<<<sm_count * 8, 256, 0, s>>>(st, now_sec, keep, cursor);
     return cudaGetLastError();
 }
 cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, cudaStream_t s) {
@@ -442,8 +443,8 @@ cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, 
     return cudaGetLastError();
 }
 
-cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, cudaStream_t s) {
-    table_count_kernel<<<148 * 8, 256, 0, s>>>(st, out);
+cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, int sm_count, cudaStream_t s) {
+    table_count_kernel<<<sm_count * 8, 256, 0, s>>>(st, out);
     return cudaGetLastError();
 }
 
@@ -463,8 +464,8 @@ __global__ void __launch_bounds__(256) evict_pairs_kernel(DeviceState st, int64_
         if (hour * 3600 <= now_sec) st.pairs[i].count = 0ull;
     }
 }
-cudaError_t launch_evict_pairs(const DeviceState& st, int64_t now_sec, cudaStream_t s) {
-    evict_pairs_kernel<<<148 * 4, 256, 0, s>>>(st, now_sec);
+cudaError_t launch_evict_pairs(const DeviceState& st, int64_t now_sec, int sm_count, cudaStream_t s) {
+    evict_pairs_kernel<<<sm_count * 4, 256, 0, s>>>(st, now_sec);
     return cudaGetLastError();
 }
 

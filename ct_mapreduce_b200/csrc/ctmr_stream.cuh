@@ -1,8 +1,8 @@
 // ctmr_stream.cuh -- resumable DER walker for the streaming map kernel.
 //
-// The v1 kernel walked the TLV tree with byte loads from global memory; ncu showed that with
-// ~210 KB of shared memory carved out per SM the remaining L1 (~45 KB) thrashes under 384 lanes
-// each touching its own lines (25 % miss, 21 % of warp time in long-scoreboard stalls).  This walker
+// The v1 kernel walked the TLV tree with byte loads from global memory; with ~210 KB of shared
+// memory carved out per SM the remaining L1 (~45 KB) thrashes under 384 lanes each touching its
+// own lines, and the walk stalls on global loads.  This walker
 // instead consumes the certificate from the SAME shared-memory chunks the SHA-256 loop streams
 // through, so every certificate byte crosses L2->SM exactly once, by an asynchronous copy.
 //

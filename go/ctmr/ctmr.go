@@ -1,4 +1,4 @@
-// Package ctmr binds libctmr.so (include/ctmr.h) with cgo: the B200-native replacement for the
+// Package ctmr binds libctmr.so (include/ctmr.h) with cgo: the H100-native replacement for the
 // loop body of insertCTWorker (cmd/ct-fetch/ct-fetch.go:191-245) and FilesystemDatabase.Store
 // (storage/filesystemdatabase.go:158-211).
 //

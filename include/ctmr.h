@@ -1,5 +1,5 @@
 /*
- * ctmr.h -- C ABI of the B200-native CT-entry map/reduce hot path (libctmr.so).
+ * ctmr.h -- C ABI of the H100-native CT-entry map/reduce hot path (libctmr.so).
  *
  * This is the drop-in boundary for ONE path of jcjones/ct-mapreduce (@739eda2): the per-entry
  * worker and its two reducers.  A Go host binds these entry points with cgo (INTEGRATION.md shows

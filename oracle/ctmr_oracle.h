@@ -7,7 +7,7 @@
  * raw serial, hour truncation), storage/knowncertificates.go:28-63 (set key, first-insert-true),
  * storage/issuermetadata.go:92-138 (first-seen expDate memo), storage/mockcache.go:38-61,120-122
  * (set semantics) and cmd/storage-statistics/storage-statistics.go:36-82 (per-issuer counts).
- * The X.509 parse itself lives in a third-party dependency that is NOT under /root/reference:
+ * The X.509 parse itself lives in a third-party dependency that is NOT in the reference repository:
  * github.com/google/certificate-transparency-go v1.1.0 (go.mod:10), packages x509/asn1/pkix; it
  * is restated here from RFC 5280 §4.1 / X.690 DER plus the Go behaviours the call sites rely on.
  *

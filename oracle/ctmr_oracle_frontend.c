@@ -13,7 +13,7 @@
  *   - insertCTWorker's entry-type switch (ct-fetch.go:198-204) picks the certificate to process and
  *     Chain[0] is the issuer (ct-fetch.go:215-221).
  *
- * github.com/google/certificate-transparency-go v1.1.0 (go.mod:10) is NOT under /root/reference, so the
+ * github.com/google/certificate-transparency-go v1.1.0 (go.mod:10) is NOT in the reference repository, so the
  * structures are restated from RFC 6962 §3.4 / §4.6 and RFC 5246 §4 (TLS presentation language) with the
  * struct tags that release publishes in types.go:
  *     MerkleTreeLeaf   { Version tls.Enum `maxval:255`; LeafType tls.Enum `maxval:255`;

@@ -17,7 +17,7 @@ README_FILTER = b"Let's Encrypt, ISRG"  # reference README.md:29, split without 
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 box)")
 
 
 def pem_to_der(path):

@@ -1,7 +1,7 @@
 """What the path does NOT model of ct-go's x509 fork -- as tests, not prose (VERDICT r1, next-round item 7).
 
 The reference parses with github.com/google/certificate-transparency-go v1.1.0 (go.mod:10), a fork of Go's crypto/x509
-+ encoding/asn1 whose source is NOT under /root/reference, so none of this can be pinned against the reference here
++ encoding/asn1 whose source is NOT in the reference repository, so none of this can be pinned against the reference here
 ("parity unpinned", SURVEY.md §8(c)).  What CAN be stated is (i) what the oracle and the CUDA walker do today -- asserted
 below, so a change is noticed -- and (ii) what Go's own encoding/asn1 / crypto/x509 (1.13, the base of the fork) is
 documented to do with the same bytes -- recorded as a strict xfail: the test "fails as expected" for as long as the

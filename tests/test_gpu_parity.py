@@ -1,6 +1,6 @@
 """Parity tests proper: the CUDA path, called through the C ABI, against the oracle on the same
 seeded inputs -- bit-exact for every output (fingerprints, membership bits, per-issuer counts).
-Marked gpu: they run on the B200 box."""
+Marked gpu: they run on the H100 box."""
 import hashlib
 
 import numpy as np

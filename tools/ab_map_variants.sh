@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B of K_map variants on one B200 (run under gpurun): builds the EXPERIMENTS library on the box (the product build
+# A/B of K_map variants on one GPU: builds the EXPERIMENTS library on the GPU machine (the product build
 # ships one instantiation only), then times each variant alone with bench.py.  Usage: tools/ab_map_variants.sh [entries] [workload]
 N=${1:-4000000}
 W=${2:-cfg2}

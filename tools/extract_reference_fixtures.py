@@ -5,7 +5,7 @@ The reference's Go tests embed three PEM certificates -- the only real-world DER
     storage/types_test.go:21-39               kLeadingZeroes (serial 0x00AA, GeneralizedTime)
     storage/filesystemdatabase_test.go:17-33  kEmptySPKI     (CA:TRUE, UTF8 CN "ca")
     storage/filesystemdatabase_test.go:35-64  kRealSPKI      (UTCTime, 5-RDN PrintableString issuer, CRL-DP)
-/root/reference does not exist on the GPU box, so the PEMs (public certificates, test data) are copied
+The reference is not part of this repository, so the PEMs (public certificates, test data) are copied
 to tests/golden/*.pem and the values an independent implementation derives from them -- Python
 hashlib + `cryptography`, NOT this repository's oracle -- are written to tests/golden/fixtures.json.
 The Go tests' literal expectations (types_test.go:50,93,98 ...) are cited in tests/test_oracle_kat.py.
@@ -17,7 +17,7 @@ from cryptography.hazmat.primitives import serialization
 from cryptography.x509.oid import ExtensionOID, NameOID
 
 warnings.filterwarnings("ignore")
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else sys.exit("usage: extract_reference_fixtures.py <reference checkout>")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 SRC = {
     "kLeadingZeroes": "storage/types_test.go",

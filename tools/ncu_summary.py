@@ -1,7 +1,7 @@
-"""Turns `ncu -i <rep> --page raw --csv` output into the short metric list kept under profiles/.
+"""Turns `ncu -i <rep> --page raw --csv` output into a short metric list.
 
-    ncu -i gpurun_out/x.ncu-rep --page raw --csv > gpurun_out/x_raw.csv
-    python tools/ncu_summary.py gpurun_out/x_raw.csv [kernel-name-substring] > profiles/<name>_summary.txt
+    ncu -i profile_out/x.ncu-rep --page raw --csv > profile_out/x_raw.csv
+    python tools/ncu_summary.py profile_out/x_raw.csv [kernel-name-substring] > profile_out/x_summary.txt
 """
 import csv
 import sys

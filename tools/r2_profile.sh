@@ -1,8 +1,9 @@
 #!/bin/bash
-# Round-2 profiling pass on ONE B200 (run under gpurun): launch list of the default bench, ncu --set full of the two map
-# kernels (fingerprint on / off), compute-sanitizer over a parity subset.  Everything lands in gpurun_out/.
+# Profiling pass on ONE GPU: launch list of the default bench, ncu --set full of the two map kernels (fingerprint
+# on / off), compute-sanitizer over a parity subset.  Everything lands in the directory given as $1 (default profile_out/).
 set -u
-O=gpurun_out
+O=${1:-profile_out}
+mkdir -p "$O"
 NCU="ncu --clock-control none"
 BENCH="python bench.py --steps 2 --warmup 1 --no-e2e --no-cpu-baseline --no-secondary"
 # 1. launch list (per-launch times are cold-cache and serialised: shares, not absolutes)

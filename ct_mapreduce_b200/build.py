@@ -16,9 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libctmr.so")
 SOURCES = ["ctmr_map.cu", "ctmr_reduce.cu", "ctmr_api.cu", "ctmr_pipeline.cu", "ctmr_frontend.cu", "ctmr_frontend_api.cu", "ctmr_synth_kernels.cu", "ctmr_synth_pages.cu"]
-# measured-and-rejected K_map variants (v1 global-memory walk, dynamic scheduling, TMA bulk loader): only with CTMR_EXPERIMENTS=1
-EXPERIMENT_SOURCES = ["ctmr_map_alt.cu"]
-DEPS = SOURCES + EXPERIMENT_SOURCES + ["ctmr_ctx.cuh", "ctmr_kernels.cuh", "ctmr_common.cuh", "ctmr_stream.cuh", "ctmr_device.cuh", "ctmr_synth.h",
+DEPS = SOURCES + ["ctmr_ctx.cuh", "ctmr_kernels.cuh", "ctmr_common.cuh", "ctmr_stream.cuh", "ctmr_device.cuh", "ctmr_synth.h",
                   "ctmr_synth_ecpoints.inc",
                   os.path.join("..", "..", "include", "ctmr.h"), os.path.join("..", "..", "include", "ctmr_frontend.h")]
 
@@ -48,9 +46,8 @@ def needs_build() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return LIB
-    exp = os.environ.get("CTMR_EXPERIMENTS", "0") == "1"
-    cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + (["-DCTMR_EXPERIMENTS=1"] if exp else []) + \
-          [os.path.join(CSRC, s) for s in SOURCES + (EXPERIMENT_SOURCES if exp else [])] + ["-o", LIB + ".tmp", "-lcudart"]
+    cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
+          [os.path.join(CSRC, s) for s in SOURCES] + ["-o", LIB + ".tmp", "-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or r.returncode:
         sys.stderr.write(r.stdout + r.stderr)

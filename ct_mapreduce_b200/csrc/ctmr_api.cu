@@ -90,8 +90,8 @@ int ensure_scratch(ctmr_ctx* c, uint64_t n) {
     return CTMR_OK;
 }
 
-void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, MapParams& p, int counter_slot,
-                     uint32_t* fused_slot_of, int parity) {
+static void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, MapParams& p, uint32_t* fused_slot_of,
+                            int parity) {
     std::memset(&p, 0, sizeof p);
     p.blob = b->blob;
     p.blob_bytes = b->blob_bytes;
@@ -108,14 +108,6 @@ void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o
     p.now_sec = sec;
     p.now_frac_nonzero = (ns - sec * 1000000000LL) != 0;
     p.one = 1;
-    {
-        static const bool skip = getenv("CTMR_DEBUG_SKIP_WALK") && atoi(getenv("CTMR_DEBUG_SKIP_WALK"));
-        p.debug_skip_walk = skip;
-    }
-    {
-        static const int sh[12] = {2, 13, 22, 6, 11, 25, 7, 18, 3, 17, 19, 10};
-        for (int i = 0; i < 12; ++i) p.rot_mul[i] = 1u << (32 - sh[i]);
-    }
     p.status = o->status;
     p.sha256 = (c->flags & CTMR_F_NO_FINGERPRINT) ? nullptr : o->sha256;
     p.exp_hour = o->exp_hour;
@@ -128,12 +120,7 @@ void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o
         p.crldp_off = o->crldp_off;
         p.crldp_len = o->crldp_len;
     }
-    {
-        static const int lp = env_int("CTMR_LIGHT_PREFETCH", 2);
-        p.light_prefetch = (uint32_t)lp;
-    }
     p.status_counts = c->st.status_counts;
-    p.work_counter = c->small_dev + 84 + counter_slot;  // one per pipeline stage + one for the device entry points
     p.filter = c->filter;
     p.route.world = 1;
     if (fused_slot_of && p.keys) {  // K_insert fused into K_map: own keys into the own table, the others to their owners' inboxes
@@ -151,6 +138,31 @@ void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o
         p.error_flag = c->st.error_flag;
         p.slot_of = fused_slot_of;
     }
+}
+
+int map_slice(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, uint32_t* fused_slot_of, int parity, uint32_t* order,
+              unsigned int* len_hist, cudaStream_t s) {
+    MapParams p;
+    fill_map_params(c, b, o, p, fused_slot_of, parity);
+    if (b->n > 64 && p.sha256) {  // the light (no-fingerprint) kernel has no lock-step loop to balance
+        CU(c, launch_len_order(b->offsets, b->lens, b->n, b->blob_bytes, len_hist, order, c->sm_count, s));
+        p.order = order;
+    }
+    CU(c, launch_map(p, c->sm_count, s));
+    return CTMR_OK;
+}
+
+int ensure_order(ctmr_ctx* c, uint64_t n) {
+    if (n > c->order_cap) {
+        CU(c, cudaDeviceSynchronize());  // the old buffer may still be in use
+        cudaFree(c->order_scratch);
+        c->order_scratch = nullptr;
+        c->order_cap = 0;
+        CU(c, cudaMalloc(&c->order_scratch, n * sizeof(uint32_t)));
+        c->order_cap = n;
+    }
+    if (!c->len_hist) CU(c, cudaMalloc(&c->len_hist, 256 * sizeof(unsigned int)));
+    return CTMR_OK;
 }
 
 // views of every rank's shared region: the tables K_map / K_resolve address, the flags and histograms of the
@@ -246,6 +258,14 @@ int round_pull(ctmr_ctx* c, int parity, uint64_t maxr, uint8_t* was_unknown, uin
     CU(c, launch_pull_bits(c->px, (uint32_t)parity, c->cursors + (size_t)parity * kMaxWorld,
                            c->rev + (uint64_t)parity * c->px.world * c->px.X, maxr, was_unknown, first, s));
     return CTMR_OK;
+}
+int round_resolve(ctmr_ctx* c, int parity, uint64_t maxr, const ctmr_key* keys, uint64_t cnt, const uint32_t* slot_of,
+                  uint32_t* pair_slot, uint8_t* was_unknown, uint8_t* first, cudaStream_t s) {
+    CU(c, launch_resolve(c->st, keys, cnt, slot_of, pair_slot, was_unknown, s));
+    int rc = round_owner_resolve(c, parity, maxr, s);
+    if (rc) return rc;
+    CU(c, launch_resolve_pairs(c->st, keys, cnt, pair_slot, was_unknown, first, s));
+    return round_owner_pairs(c, parity, maxr, s);
 }
 
 // Rounds of E entries with a SHORT last round (a quarter of E): what a call exposes at its end is the reduce chain of its
@@ -541,9 +561,6 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
     c->stage_bytes = want_bytes < kStageBytes ? want_bytes : kStageBytes;
     c->cfg_round_entries = cfg->max_round_entries;
     c->px.world = 1;
-    if (const char* ev = getenv("CTMR_BUCKET_BY_LENGTH")) c->bucket_by_length = atoi(ev) != 0;
-    if (const char* ev = getenv("CTMR_FUSE_INSERT")) c->fuse_insert = atoi(ev) != 0;
-    if (const char* ev = getenv("CTMR_MAP_VARIANT")) if (atoi(ev) != 2) c->fuse_insert = false;  // only the streaming kernel fuses
     CUC(cudaStreamSynchronize(c->stream));
 #undef CUC
     *out = c;
@@ -759,24 +776,9 @@ int ctmr_map_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o,
     if (!c || !b || !o) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n && (!b->blob || !b->offsets)) return fail(c, CTMR_E_INVALID, "null batch buffers");
     CU(c, cudaSetDevice(c->device));
-    MapParams p;
-    fill_map_params(c, b, o, p);
-    cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
-    if (c->bucket_by_length && b->n > 64 && p.sha256) {  // the light (no-fingerprint) kernel has no lock-step loop to balance
-        if (b->n > c->order_cap) {
-            CU(c, cudaDeviceSynchronize());
-            cudaFree(c->order_scratch);
-            c->order_scratch = nullptr;
-            c->order_cap = 0;
-            CU(c, cudaMalloc(&c->order_scratch, b->n * sizeof(uint32_t)));
-            c->order_cap = b->n;
-        }
-        if (!c->len_hist) CU(c, cudaMalloc(&c->len_hist, 256 * sizeof(unsigned int)));
-        CU(c, launch_len_order(b->offsets, b->lens, b->n, b->blob_bytes, c->len_hist, c->order_scratch, c->sm_count, s));
-        p.order = c->order_scratch;
-    }
-    CU(c, launch_map(p, c->sm_count, s));
-    return CTMR_OK;
+    int rc = ensure_order(c, b->n);
+    if (rc) return rc;
+    return map_slice(c, b, o, nullptr, 0, c->order_scratch, c->len_hist, stream ? (cudaStream_t)stream : c->stream);
 }
 
 int ctmr_reduce_device(ctmr_ctx* c, const ctmr_key* keys, uint64_t m, uint8_t* was_unknown, uint8_t* first, void* stream) {
@@ -795,14 +797,8 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     CU(c, cudaSetDevice(c->device));
     int rc = ensure_scratch(c, b->n);
     if (rc) return rc;
-    if (c->bucket_by_length && b->n > c->order_cap) {
-        CU(c, cudaDeviceSynchronize());
-        cudaFree(c->order_scratch);
-        c->order_scratch = nullptr;
-        c->order_cap = 0;
-        CU(c, cudaMalloc(&c->order_scratch, b->n * sizeof(uint32_t)));
-        c->order_cap = b->n;
-    }
+    rc = ensure_order(c, b->n);
+    if (rc) return rc;
     if (!c->stream_a) {
         CU(c, cudaStreamCreateWithFlags(&c->stream_a, cudaStreamNonBlocking));
         CU(c, cudaStreamCreateWithFlags(&c->stream_a2, cudaStreamNonBlocking));
@@ -833,10 +829,7 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     const bool coll = c->peer_mode == PEER_IPC && world > 1;
     if (c->peer_mode == PEER_GROUP && world > 1)
         return fail(c, CTMR_E_INVALID, "members of an in-process group are driven through ctmr_group_process_batch");
-    static const int rounds_env = env_int("CTMR_DEVICE_ROUNDS", 0);   // experiments: rounds of the single-GPU call
-    static const int map_streams = env_int("CTMR_MAP_STREAMS", 2);    // K_map launches alternate between two streams
-    int nsub = coll ? (int)peer_rounds() : (b->n >= (1u << 21) ? 8 : (b->n >= (1u << 18) ? 2 : 1));
-    if (!coll && rounds_env > 0 && b->n >= (1u << 18)) nsub = rounds_env > kMaxRounds ? kMaxRounds : rounds_env;
+    const int nsub = coll ? (int)peer_rounds() : (b->n >= (1u << 21) ? 8 : (b->n >= (1u << 18) ? 2 : 1));
     const uint64_t per_round = device_round_entries(b->n, (uint32_t)nsub);
     if (coll && per_round > c->px.X)
         return fail(c, CTMR_E_BATCH_TOO_LARGE, "entries per round exceed the key-exchange regions: raise config.max_round_entries to ceil(n / ctmr_peer_rounds())");
@@ -872,35 +865,24 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
         const int parity = k % (int)kParities;
         // consecutive K_map launches on alternating streams: the next launch's CTAs fill the SMs the previous one's
         // draining tail leaves idle (a persistent grid ends with its slowest warps)
-        cudaStream_t sa = (map_streams > 1 && (k & 1)) ? c->stream_a2 : c->stream_a;
-        const bool fused = c->fuse_insert || world > 1;   // a group always fuses: the routing happens in K_map's epilogue
-        MapParams p;
-        fill_map_params(c, &sb, &so, p, 3, fused ? c->slot_scratch + lo : nullptr, parity);
+        cudaStream_t sa = (k & 1) ? c->stream_a2 : c->stream_a;
         if (world > 1 && k >= (int)kParities) CU(c, cudaStreamWaitEvent(sa, c->ev_pulled[parity], 0));  // the parity's regions are free again
         CU(c, cudaEventRecord(c->ev_map0[k], sa));
         rc = round_begin(c, parity, sa);
         if (rc) return rc;
-        if (c->bucket_by_length && cnt > 64 && p.sha256) {
-            CU(c, launch_len_order(sb.offsets, sb.lens, cnt, sb.blob_bytes, c->len_hist_sub[k], c->order_scratch + lo, c->sm_count, sa));
-            p.order = c->order_scratch + lo;
-        }
-        CU(c, launch_map(p, c->sm_count, sa));
+        rc = map_slice(c, &sb, &so, c->slot_scratch + lo, parity, c->order_scratch + lo, c->len_hist_sub[k], sa);
+        if (rc) return rc;
         CU(c, cudaEventRecord(c->ev_map1[k], sa));
         rc = round_publish(c, parity, sa);  // region sizes to the owners (outside K_map's timed bracket)
         if (rc) return rc;
         CU(c, cudaEventRecord(c->ev_tok[k], sa));   // ordering token: K_map + the published sizes
         CU(c, cudaStreamWaitEvent(c->stream_b, c->ev_tok[k], 0));
         cudaStream_t sbm = c->stream_b;
-        if (!fused) CU(c, launch_insert(c->st, keys + lo, cnt, c->slot_scratch + lo, sbm));
         rc = peer_barrier(c, CH_DEV_MAP, sbm);  // every rank's appends of rounds <= k have landed in the owners' inboxes
         if (rc) return rc;
         rc = round_owner_insert(c, parity, per_round, sbm);
         if (rc) return rc;
-        CU(c, launch_resolve(c->st, keys + lo, cnt, c->slot_scratch + lo, c->pair_scratch + lo, wu + lo, sbm));
-        rc = round_owner_resolve(c, parity, per_round, sbm);
-        if (rc) return rc;
-        CU(c, launch_resolve_pairs(c->st, keys + lo, cnt, c->pair_scratch + lo, wu + lo, fi + lo, sbm));
-        rc = round_owner_pairs(c, parity, per_round, sbm);
+        rc = round_resolve(c, parity, per_round, keys + lo, cnt, c->slot_scratch + lo, c->pair_scratch + lo, wu + lo, fi + lo, sbm);
         if (rc) return rc;
         rc = peer_barrier(c, CH_DEV_RESOLVE, sbm);  // every owner has the result bits of this round's records ready
         if (rc) return rc;
@@ -916,7 +898,6 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
         CU(c, cudaEventRecord(c->ev_red1[k], c->stream_b));
     }
     c->last_sub = nsub;
-    c->last_map_streams = map_streams > 1 ? 2 : 1;
     CU(c, cudaEventRecord(c->ev_join_a2, c->stream_a2));
     CU(c, cudaStreamWaitEvent(user, c->ev_join_a2, 0));
     CU(c, cudaEventRecord(c->ev_join_a, c->stream_a));
@@ -926,31 +907,21 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     return CTMR_OK;
 }
 
-/* CUDA-event timings of the last ctmr_process_device call (after the caller synchronised):
- * map_ms = sum of the K_map stage durations on their stream, total_ms = first map start -> last reduce end */
 uint32_t ctmr_peer_rounds(void) { return peer_rounds(); }
 uint64_t ctmr_peer_round_entries(uint64_t n) { return device_round_entries(n, peer_rounds()); }
 
+/* CUDA-event timings of the last ctmr_process_device call (after the caller synchronised):
+ * map_ms = first K_map start -> last K_map end, total_ms = first map start -> last reduce end */
 int ctmr_profile_last(ctmr_ctx* c, float* map_ms, float* total_ms) {
     if (!c || c->last_sub <= 0) return fail(c, CTMR_E_INVALID, "no ctmr_process_device call to report");
     CU(c, cudaSetDevice(c->device));
+    // launches overlap (alternating streams): K_map's time is the span from the first launch's start to the last one's end,
+    // during which some K_map CTA is always resident
     float m = 0.f, t = 0.f;
-    if (c->last_map_streams > 1) {
-        // launches overlap (alternating streams): K_map's time is the span from the first launch's start to the last one's end,
-        // during which some K_map CTA is always resident
-        float best = 0.f;
-        for (int k = 0; k < c->last_sub; ++k) {
-            float d = 0.f;
-            CU(c, cudaEventElapsedTime(&d, c->ev_map0[0], c->ev_map1[k]));
-            best = d > best ? d : best;
-        }
-        m = best;
-    } else {
-        for (int k = 0; k < c->last_sub; ++k) {
-            float d = 0.f;
-            CU(c, cudaEventElapsedTime(&d, c->ev_map0[k], c->ev_map1[k]));
-            m += d;
-        }
+    for (int k = 0; k < c->last_sub; ++k) {
+        float d = 0.f;
+        CU(c, cudaEventElapsedTime(&d, c->ev_map0[0], c->ev_map1[k]));
+        m = d > m ? d : m;
     }
     CU(c, cudaEventElapsedTime(&t, c->ev_map0[0], c->ev_red1[c->last_sub - 1]));
     if (map_ms) *map_ms = m;

@@ -1,53 +1,12 @@
 // ctmr_common.cuh -- device helpers shared by the map and reduce translation units: PTX wrappers
-// (mbarrier, TMA bulk copy, cp.async), the known-certificate table probe, streaming geometry.
+// (cp.async), the known-certificate table probe, streaming geometry.
 #pragma once
-#include <cstdlib>
-
 #include "ctmr_device.cuh"
 #include "ctmr_kernels.cuh"
 
 namespace ctmr {
 
-static inline int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return v && *v ? atoi(v) : dflt;
-}
-
-// ------------------------------------------------------------------------------------------------
-// PTX wrappers: mbarrier + bulk async copy (TMA, non-tensor form)
-// ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    while (!mbar_try_wait(bar, parity)) {
-    }
-}
-// global -> shared::cta bulk copy; src and dst 16-byte aligned, bytes a multiple of 16
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
-}
 
 __device__ __forceinline__ uint32_t warp_max_u32(uint32_t v) { return __reduce_max_sync(0xffffffffu, v); }
 
@@ -150,23 +109,21 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-#ifndef CTMR_SLOT_PAD
-#define CTMR_SLOT_PAD 16
-#endif
-
-template <int WARPS, int CHUNK, int LOADER, int ROLLED = 0>
+// Shape of the streaming map (K_map): the best measured before the port (DESIGN.md §3, K_map).
 struct StreamCfg {
+    static constexpr int kWarps = 8;       // warps per CTA, one certificate per lane
+    static constexpr int kChunk = 128;     // record bytes staged per lane and step
+    static constexpr int kCtasPerSm = 2;   // resident CTAs per SM of the persistent grid
     static constexpr int kOverlap = 48;  // >= kWalkNeed, multiple of 16
     // Lane slots are kSlot bytes apart and every lane reads the same word of its own slot, so the stride
     // decides the bank pattern: 16-byte granules (cp.async) allow at best 8 distinct bank groups; an odd
     // number of granules per slot reaches that (4-way worst case), an even one collapses to 2 groups (16-way).
-    static constexpr int kSlotRaw = kOverlap + CHUNK + 16;
-    static constexpr int kSlot = kSlotRaw + (((kSlotRaw / 16) % 2 == 0) ? CTMR_SLOT_PAD : 0);
+    static constexpr int kSlotRaw = kOverlap + kChunk + 16;
+    static constexpr int kSlot = kSlotRaw + (((kSlotRaw / 16) % 2 == 0) ? 16 : 0);
     static constexpr int kWarpBytes = 2 * 32 * kSlot;
-    static constexpr int kBlocksPerChunk = CHUNK / 64;
-    static constexpr int kPieces = kSlot / 16;
+    static constexpr int kBlocksPerChunk = kChunk / 64;
     // +16: the walker's word-wise header read may touch the word after the last staged byte
-    static constexpr size_t kSmem = (size_t)WARPS * kWarpBytes + 16 + (LOADER == 1 ? (size_t)WARPS * 2 * sizeof(uint64_t) : 0);
+    static constexpr size_t kSmem = (size_t)kWarps * kWarpBytes + 16;
 };
 
 struct GlobalBytes {

@@ -183,18 +183,16 @@ struct ctmr_ctx {
     uint8_t* bits_scratch = nullptr;
     uint32_t* meta_scratch = nullptr;  // [2*cap]
     uint64_t scratch_cap = 0;
-    uint32_t* order_scratch = nullptr;  // length-bucketed order of the device entry points
+    uint32_t* order_scratch = nullptr;  // length-bucketed order of the device entry points (ensure_order)
     uint64_t order_cap = 0;
     unsigned int* len_hist = nullptr;
-    bool bucket_by_length = true;
-    bool fuse_insert = true;
     // ctmr_process_device pipelines map (stream A) against reduce (stream B) over kSub sub-batches
     cudaStream_t stream_a = nullptr, stream_a2 = nullptr, stream_b = nullptr;  // K_map alternates between a and a2
     cudaEvent_t ev_fork = nullptr, ev_join_a = nullptr, ev_join_a2 = nullptr, ev_join_b = nullptr;
     cudaEvent_t ev_map0[kMaxRounds] = {}, ev_map1[kMaxRounds] = {}, ev_red1[kMaxRounds] = {}, ev_tok[kMaxRounds] = {};
-    int last_sub = 0, last_map_streams = 1;
+    int last_sub = 0;
     unsigned int* len_hist_sub[kMaxRounds] = {};
-    unsigned long long* small_dev = nullptr;  // [128] private counters / cursors / results (error flag at +73)
+    unsigned long long* small_dev = nullptr;  // [128] private counters / cursors / results (error flag at +73; words 84..87 unused)
     FrontEnd* fe = nullptr;
     std::string err;
 };
@@ -220,8 +218,13 @@ int fail(ctmr_ctx* ctx, int code, const std::string& msg);
     } while (0)
 
 uint64_t pow2_at_least(uint64_t v);
-void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, MapParams& p, int counter_slot = 3,
-                     uint32_t* fused_slot_of = nullptr, int parity = 0);
+// K_map over one slice on stream s.  fused_slot_of != NULL: the keys go straight into the table (this rank's) or to
+// their owners' inboxes of exchange `parity`, slot -> fused_slot_of.  The fingerprint path of more than 64 entries first
+// orders the slice by length into order[0..n), with len_hist (256 counters) as scratch: rounds that may run concurrently
+// pass separate histograms.
+int map_slice(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, uint32_t* fused_slot_of, int parity, uint32_t* order,
+              unsigned int* len_hist, cudaStream_t s);
+int ensure_order(ctmr_ctx* c, uint64_t n);   // c->order_scratch holds >= n entries, c->len_hist exists
 // key exchange: allocation for a group of `world` ranks, views of every rank's area
 size_t exchange_bytes(uint32_t world, uint64_t X);
 int alloc_exchange(ctmr_ctx* c, uint32_t world);
@@ -233,6 +236,10 @@ int round_owner_insert(ctmr_ctx* c, int parity, uint64_t max_per_region, cudaStr
 int round_owner_resolve(ctmr_ctx* c, int parity, uint64_t max_per_region, cudaStream_t s);  // ... their was_unknown, counts, pair slots
 int round_owner_pairs(ctmr_ctx* c, int parity, uint64_t max_per_region, cudaStream_t s);    // ... their first_issuer_hour
 int round_pull(ctmr_ctx* c, int parity, uint64_t max_per_region, uint8_t* was_unknown, uint8_t* first, cudaStream_t s);
+// the owner passes of a round after every insert of it (own keys and inbox records) has landed, in the order
+// lowest-index-wins needs: K_resolve, inbox resolve, K_pairs, inbox pairs
+int round_resolve(ctmr_ctx* c, int parity, uint64_t max_per_region, const ctmr_key* keys, uint64_t cnt, const uint32_t* slot_of,
+                  uint32_t* pair_slot, uint8_t* was_unknown, uint8_t* first, cudaStream_t s);
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise

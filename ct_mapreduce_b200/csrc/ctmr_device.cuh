@@ -134,85 +134,6 @@ __device__ __forceinline__ void sha256_compress_rolled(Sha256State& s, uint32_t 
     s.h[0] += a; s.h[1] += b; s.h[2] += c; s.h[3] += d; s.h[4] += e; s.h[5] += f; s.h[6] += g; s.h[7] += h;
 }
 
-// ------------------------------------------------------------------------------------------------
-// Variant of the rolled compression that also moves ROTATIONS off the ALU pipe: rotr(x, n) is the
-// OR of the two halves of the 64-bit product x * 2^(32-n), and x >> n is the high half alone, so a
-// sigma function becomes IMAD.WIDE / IMAD.HI (FMA pipe) plus two LOP3 instead of three SHF plus one
-// LOP3.  The multipliers come from kernel parameters so that ptxas cannot turn them back into
-// shifts.  WIDE = 1: message schedule only; 2: schedule + Sigma1; 3: schedule + Sigma1 + Sigma0.
-// ------------------------------------------------------------------------------------------------
-struct RotMul {  // 2^(32-n) for the rotation / shift amounts SHA-256 uses
-    uint32_t r2, r13, r22, r6, r11, r25, r7, r18, s3, r17, r19, s10;
-};
-
-__device__ __forceinline__ void mulwide(uint32_t x, uint32_t m, uint32_t& lo, uint32_t& hi) {
-    asm("{\n\t.reg .u64 t;\n\tmul.wide.u32 t, %2, %3;\n\tmov.b64 {%0, %1}, t;\n\t}" : "=r"(lo), "=r"(hi) : "r"(x), "r"(m));
-}
-__device__ __forceinline__ uint32_t mulhi(uint32_t x, uint32_t m) {
-    uint32_t d;
-    asm("mul.hi.u32 %0, %1, %2;" : "=r"(d) : "r"(x), "r"(m));
-    return d;
-}
-__device__ __forceinline__ uint32_t ssig0_w(uint32_t x, const RotMul& r) {
-    uint32_t a, b, c, d;
-    mulwide(x, r.r7, a, b);
-    mulwide(x, r.r18, c, d);
-    return (a ^ b ^ c) ^ d ^ mulhi(x, r.s3);
-}
-__device__ __forceinline__ uint32_t ssig1_w(uint32_t x, const RotMul& r) {
-    uint32_t a, b, c, d;
-    mulwide(x, r.r17, a, b);
-    mulwide(x, r.r19, c, d);
-    return (a ^ b ^ c) ^ d ^ mulhi(x, r.s10);
-}
-__device__ __forceinline__ uint32_t bsig1_w(uint32_t x, const RotMul& r) {
-    uint32_t a, b, c, d;
-    mulwide(x, r.r6, a, b);
-    mulwide(x, r.r11, c, d);
-    return (a ^ b ^ c) ^ d ^ rotr32(x, 25);
-}
-__device__ __forceinline__ uint32_t bsig0_w(uint32_t x, const RotMul& r) {
-    uint32_t a, b, c, d;
-    mulwide(x, r.r2, a, b);
-    mulwide(x, r.r13, c, d);
-    return (a ^ b ^ c) ^ d ^ rotr32(x, 22);
-}
-
-template <int WIDE>
-__device__ __forceinline__ void sha256_compress_wide(Sha256State& s, uint32_t (&w)[16], const uint32_t one, const RotMul& rm) {
-    uint32_t a = s.h[0], b = s.h[1], c = s.h[2], d = s.h[3], e = s.h[4], f = s.h[5], g = s.h[6], h = s.h[7];
-#define CTMR_WROUND(a, b, c, d, e, f, g, h, k, w)                                          \
-    do {                                                                                   \
-        uint32_t t1_ = (h) + (w) + (k);                                                    \
-        t1_ = fadd(fadd((WIDE >= 2 ? bsig1_w((e), rm) : bsig1(e)), t1_, one), ch((e), (f), (g)), one); \
-        uint32_t t2_ = fadd((WIDE >= 3 ? bsig0_w((a), rm) : bsig0(a)), maj((a), (b), (c)), one);       \
-        (d) = fadd((d), t1_, one);                                                         \
-        (h) = fadd(t1_, t2_, one);                                                         \
-    } while (0)
-#pragma unroll 1
-    for (int it = 0; it < 4; ++it) {
-        if (it != 0) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-                w[j] = fadd(fadd(fadd(ssig1_w(w[(j - 2) & 15], rm), w[j], one), w[(j - 7) & 15], one), ssig0_w(w[(j - 15) & 15], rm), one);
-        }
-        const uint32_t* kp = kSha256K + 16 * it;
-#pragma unroll
-        for (int j = 0; j < 16; j += 8) {
-            CTMR_WROUND(a, b, c, d, e, f, g, h, kp[j + 0], w[j + 0]);
-            CTMR_WROUND(h, a, b, c, d, e, f, g, kp[j + 1], w[j + 1]);
-            CTMR_WROUND(g, h, a, b, c, d, e, f, kp[j + 2], w[j + 2]);
-            CTMR_WROUND(f, g, h, a, b, c, d, e, kp[j + 3], w[j + 3]);
-            CTMR_WROUND(e, f, g, h, a, b, c, d, kp[j + 4], w[j + 4]);
-            CTMR_WROUND(d, e, f, g, h, a, b, c, kp[j + 5], w[j + 5]);
-            CTMR_WROUND(c, d, e, f, g, h, a, b, kp[j + 6], w[j + 6]);
-            CTMR_WROUND(b, c, d, e, f, g, h, a, kp[j + 7], w[j + 7]);
-        }
-    }
-#undef CTMR_WROUND
-    s.h[0] += a; s.h[1] += b; s.h[2] += c; s.h[3] += d; s.h[4] += e; s.h[5] += f; s.h[6] += g; s.h[7] += h;
-}
-
 // Padding for the trailing blocks of a message of `len` bytes.  `q` is the byte position of word
 // w inside the message; data bytes at positions >= len are garbage and get masked here.
 __device__ __forceinline__ uint32_t sha256_pad_word(uint32_t w, uint32_t q, uint32_t len) {

@@ -338,22 +338,10 @@ int group_round(ctmr_group* g, RawChunk* ch, int parity, ctmr_ctx** failed) {
         if (rc) return rc;
         if (cnt) {
             ch[r].dout.keys = c->keys_scratch;
-            MapParams p;
-            fill_map_params(c, &ch[r].db, &ch[r].dout, p, 3, c->slot_scratch, parity);
-            if (c->bucket_by_length && cnt > 64 && p.sha256) {
-                if (cnt > c->order_cap) {
-                    CU(c, cudaStreamSynchronize(s));
-                    cudaFree(c->order_scratch);
-                    c->order_scratch = nullptr;
-                    c->order_cap = 0;
-                    CU(c, cudaMalloc(&c->order_scratch, cnt * sizeof(uint32_t)));
-                    c->order_cap = cnt;
-                }
-                if (!c->len_hist) CU(c, cudaMalloc(&c->len_hist, 256 * sizeof(unsigned int)));
-                CU(c, launch_len_order(ch[r].db.offsets, ch[r].db.lens, cnt, ch[r].db.blob_bytes, c->len_hist, c->order_scratch, c->sm_count, s));
-                p.order = c->order_scratch;
-            }
-            CU(c, launch_map(p, c->sm_count, s));
+            rc = ensure_order(c, cnt);
+            if (rc) return rc;
+            rc = map_slice(c, &ch[r].db, &ch[r].dout, c->slot_scratch, parity, c->order_scratch, c->len_hist, s);
+            if (rc) return rc;
         }
         rc = round_publish(c, parity, s);
         if (rc) return rc;
@@ -370,11 +358,8 @@ int group_round(ctmr_group* g, RawChunk* ch, int parity, ctmr_ctx** failed) {
             if (q != r) CU(c, cudaStreamWaitEvent(s, g->m[q]->ev_g[0], 0));
         rc = round_owner_insert(c, parity, maxr, s);
         if (rc) return rc;
-        if (cnt) CU(c, launch_resolve(c->st, c->keys_scratch, cnt, c->slot_scratch, c->pair_scratch, ch[r].dout.was_unknown, s));
-        rc = round_owner_resolve(c, parity, maxr, s);
-        if (rc) return rc;
-        if (cnt) CU(c, launch_resolve_pairs(c->st, c->keys_scratch, cnt, c->pair_scratch, ch[r].dout.was_unknown, ch[r].dout.first_issuer_hour, s));
-        rc = round_owner_pairs(c, parity, maxr, s);
+        rc = round_resolve(c, parity, maxr, c->keys_scratch, cnt, c->slot_scratch, c->pair_scratch, ch[r].dout.was_unknown,
+                           ch[r].dout.first_issuer_hour, s);
         if (rc) return rc;
         CU(c, cudaEventRecord(c->ev_g[1], s));
     }

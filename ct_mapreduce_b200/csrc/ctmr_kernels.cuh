@@ -135,12 +135,10 @@ struct MapParams {
     const uint32_t* issuer_idx;
     const uint32_t* issuer_map;
     uint32_t issuer_map_len;
-    uint32_t debug_skip_walk;  // profiling aid (CTMR_DEBUG_SKIP_WALK=1): time K_map without the DER walker; results invalid
     uint64_t first_index;
     int64_t now_sec;
     uint32_t now_frac_nonzero;
     uint32_t one;  // always 1: a multiplier ptxas cannot fold (see fadd in ctmr_device.cuh)
-    uint32_t rot_mul[12];  // 2^(32-n) multipliers of the IMAD.WIDE rotations (RotMul in ctmr_device.cuh)
     uint8_t* status;
     uint8_t* sha256;
     int64_t* exp_hour;
@@ -152,7 +150,6 @@ struct MapParams {
     uint32_t* crldp_off;
     uint32_t* crldp_len;
     unsigned long long* status_counts;
-    unsigned long long* work_counter;  // [1] scratch of the dynamically scheduled map kernel
     const uint32_t* order;             // [n] length-bucketed processing order (NULL = entry order)
     // fused K_insert (slot_of != NULL): keys this rank owns go straight into its table (slot -> slot_of), keys owned
     // elsewhere are appended to the owner's inbox (slot_of = 0xFFFFFFFF)
@@ -161,14 +158,10 @@ struct MapParams {
     uint64_t table_mask;
     int* error_flag;
     uint32_t* slot_of;
-    uint32_t light_prefetch;  // map_light_kernel: low 4 bits = leading 128-byte lines to prefetch per record, bit 4 = also the tail
-    uint32_t pad_lp;
     FilterCfg filter;
 };
 
 cudaError_t launch_map(const MapParams& p, int sm_count, cudaStream_t s);
-cudaError_t launch_map_v1(const MapParams& p, int sm_count, cudaStream_t s);  // ctmr_map_alt.cu
-cudaError_t launch_map_v3(const MapParams& p, int sm_count, cudaStream_t s);  // ctmr_map_alt.cu
 cudaError_t launch_sha_ceiling(uint32_t iters, int rolled, int ctas_per_sm, int sm_count, uint32_t* sink, cudaStream_t s);
 cudaError_t launch_len_order(const uint64_t* offsets, const uint32_t* lens, uint64_t n, uint64_t blob_bytes, unsigned int* hist256, uint32_t* order,
                              int sm_count, cudaStream_t s);

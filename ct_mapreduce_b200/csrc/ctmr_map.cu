@@ -1,6 +1,6 @@
 // ctmr_map.cu -- the map half of the CT-entry hot path: hand-written sm_90a kernels.
 //
-// K_map        (map_stream_kernel<8,128,0,1>) lane-per-certificate map: DER walk + certIsFilteredOut + SHA-256(leaf DER).
+// K_map        (map_stream_kernel) lane-per-certificate map: DER walk + certIsFilteredOut + SHA-256(leaf DER).
 //              Each lane streams ITS certificate through a private double-buffered shared-memory window filled by
 //              asynchronous 16-byte global->shared copies (cp.async.cg -> SASS LDGSTS, per-thread commit / wait groups: no
 //              barrier is shared between lanes), so certificate bytes never occupy registers while the INT pipe runs the
@@ -8,7 +8,7 @@
 //              outputs, key record, and the key's route -- fused find-or-insert into this GPU's table when it owns the set,
 //              else an append to the owner GPU's inbox over NVLink (route_append).
 //              (cmd/ct-fetch/ct-fetch.go:44-70,198-213, storage/types.go:171-178,339-346; fingerprint =
-//              crypto/sha256.Sum256(cert.Raw).)  The TMA bulk-copy loader (LOADER = 1) is an experiment, see DESIGN.md.
+//              crypto/sha256.Sum256(cert.Raw).)
 // K_map_light  (map_light_kernel) the same outputs without the fingerprint: thread per certificate, loads through L1.
 // length bucketing (len_hist / len_scan / len_scatter): processing order with equally long records per warp.
 // sha_ceiling_kernel: the register-only SHA-256 microbenchmark the roofline is quoted against.
@@ -51,6 +51,8 @@ __device__ __forceinline__ void route_append(const RouteOut& r, bool remote, uin
 // through L1 (the full 256 KB is available as cache), 32 resident warps per SM to hide the pointer
 // chase.  The streaming kernel, which must stage every byte, is slower on this path.
 // ------------------------------------------------------------------------------------------------
+constexpr uint32_t kLightPrefetchLines = 2;  // leading 128-byte lines of a record prefetched to L2
+
 // 6 resident CTAs per SM (40 registers, a few bytes of spills) ran faster than 4 CTAs (56 registers) when measured before the
 // port; 8 CTAs (32 registers) spill too much
 __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant__ MapParams p) {
@@ -62,18 +64,14 @@ __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant
         const bool bad_span = end < off || end > p.blob_bytes || end - off > 0x7fffffffull;
         const uint32_t L = bad_span ? 0u : (uint32_t)(end - off);
         const uint8_t* d = p.blob + off;
-        if (p.light_prefetch && L) {
-            // The walk is a pointer chase (latency bound, not bandwidth bound): start the lines it is
-            // going to need -- header, serial, names, validity at the front; signatureAlgorithm + signature header at the
-            // back -- before the first dependent load, so that they arrive in parallel
+        if (L) {
+            // The walk is a pointer chase (latency bound, not bandwidth bound): start the lines it is going to need
+            // first -- header, serial, names, validity -- before the first dependent load, so that they arrive in
+            // parallel.  Two lines measured best before the port; a prefetch of the tail (signature header) did not pay.
             const uint8_t* base = reinterpret_cast<const uint8_t*>(reinterpret_cast<uint64_t>(d) & ~127ull);
             const uint32_t lines = (uint32_t)((d - base) + L + 127u) >> 7;
-            const uint32_t nl = min(p.light_prefetch & 15u, lines);
+            const uint32_t nl = min(kLightPrefetchLines, lines);
             for (uint32_t i = 0; i < nl; ++i) asm volatile("prefetch.global.L2 [%0];" ::"l"(base + 128u * i));
-            if ((p.light_prefetch & 16u) && L > 320u) {
-                const uint8_t* tail = reinterpret_cast<const uint8_t*>(reinterpret_cast<uint64_t>(d + L - 288u) & ~127ull);
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(tail));
-            }
         }
         ParsedCert pc;
         uint32_t issuer = CTMR_ISSUER_NONE;
@@ -171,30 +169,17 @@ __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant
 // K_map v2: single-pass streaming map.  The DER walker (ctmr_stream.cuh) and the SHA-256 loop both
 // eat from the same per-lane shared-memory window; global memory is touched once per byte, by
 // asynchronous copies only.  Chunks overlap by kOverlap bytes so that a TLV header (and the small
-// values the walker captures) never straddles a refill.
-//   LOADER 0: per-lane cp.async 16-byte copies (LDGSTS) + commit/wait groups -- no barrier at all
-//   LOADER 1: per-lane TMA bulk copy (UBLKCP) + per-warp mbarrier pair
+// values the walker captures) never straddles a refill.  Staging: per-lane cp.async 16-byte copies
+// (LDGSTS) + commit/wait groups -- no barrier at all.
 // ------------------------------------------------------------------------------------------------
-template <int WARPS, int CHUNK, int LOADER, int ROLLED>
-__global__ void __launch_bounds__(WARPS * 32) map_stream_kernel(const __grid_constant__ MapParams p) {
-    using Cfg = StreamCfg<WARPS, CHUNK, LOADER>;
+__global__ void __launch_bounds__(StreamCfg::kWarps * 32) map_stream_kernel(const __grid_constant__ MapParams p) {
+    using Cfg = StreamCfg;
+    constexpr int WARPS = Cfg::kWarps, CHUNK = Cfg::kChunk;
     constexpr uint32_t OV = Cfg::kOverlap;
     extern __shared__ __align__(128) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t* my_slots = smem + (size_t)warp * Cfg::kWarpBytes + (size_t)lane * Cfg::kSlot;  // stage s at + s*32*kSlot
     const uint32_t slot0 = smem_u32(my_slots), slot1 = slot0 + 32 * Cfg::kSlot;
-    uint32_t bar0 = 0, bar1 = 0, parity = 0;
-    if (LOADER == 1) {
-        uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)WARPS * Cfg::kWarpBytes + 16) + warp * 2;
-        bar0 = smem_u32(&bars[0]);
-        bar1 = smem_u32(&bars[1]);
-        if (lane == 0) {
-            mbar_init(bar0, 32);
-            mbar_init(bar1, 32);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        __syncthreads();
-    }
 
     const uint64_t ngroups = (p.n + 31) >> 5;
     const bool want_sha = p.sha256 != nullptr;
@@ -239,19 +224,9 @@ __global__ void __launch_bounds__(WARPS * 32) map_stream_kernel(const __grid_con
                     src = src_base + (size_t)c * CHUNK - OV;
                 }
             }
-            if (LOADER == 1) {
-                const uint32_t bar = (c & 1u) ? bar1 : bar0;
-                if (bytes) {
-                    mbar_arrive_expect_tx(bar, bytes);
-                    bulk_g2s(dst, src, bytes, bar);
-                } else {
-                    mbar_arrive(bar);
-                }
-            } else {
 #pragma unroll 1
-                for (uint32_t j = 0; j < bytes; j += 16u) cp_async16(dst + j, src + j);
-                cp_async_commit();
-            }
+            for (uint32_t j = 0; j < bytes; j += 16u) cp_async16(dst + j, src + j);
+            cp_async_commit();
         };
         issue(0);
         issue(1);
@@ -264,20 +239,14 @@ __global__ void __launch_bounds__(WARPS * 32) map_stream_kernel(const __grid_con
         st.init();
         const uint32_t sel = 0x0123u + 0x1111u * (m & 3u);
         const uint32_t one = p.one;
-        const RotMul rm = *reinterpret_cast<const RotMul*>(p.rot_mul);
 
         for (uint32_t c = 0; c < iters; ++c) {
             const uint32_t s = c & 1u;
-            if (LOADER == 1) {
-                mbar_wait(s ? bar1 : bar0, (parity >> s) & 1u);
-                parity ^= 1u << s;
-            } else {
-                cp_async_wait<1>();  // everything but the newest group (chunk c+1) has landed
-            }
+            cp_async_wait<1>();  // everything but the newest group (chunk c+1) has landed
             if (c < nch) {
                 const uint8_t* slot = my_slots + (size_t)s * 32 * Cfg::kSlot;
                 // ---- map: resume the TLV walk over the newly staged bytes
-                if (act && w.st < W_DONE && !p.debug_skip_walk) {
+                if (act && w.st < W_DONE) {
                     const uint32_t avail = min((c + 1u) * CHUNK, L);
                     const SmemWindow rd{(s ? slot1 : slot0) + m + OV - c * CHUNK};
                     walk_advance(w, rd, far, bad_span ? 0u : avail, L, p.filter, key_words);
@@ -301,15 +270,13 @@ __global__ void __launch_bounds__(WARPS * 32) map_stream_kernel(const __grid_con
                             wd[15] = L << 3;
                         }
                     }
-                    if (ROLLED >= 2) sha256_compress_wide<ROLLED - 1>(st, wd, one, rm);
-                    else if (ROLLED == 1) sha256_compress_rolled(st, wd, one);
-                    else sha256_compress(st, wd, one);
+                    sha256_compress_rolled(st, wd, one);
                 }
             }
             if (c + 2u < iters) issue(c + 2u);
-            else if (LOADER != 1) cp_async_commit();  // keep "newest group = the one after chunk c+1" true at the tail
+            else cp_async_commit();  // keep "newest group = the one after chunk c+1" true at the tail
         }
-        if (LOADER != 1) cp_async_wait<0>();
+        cp_async_wait<0>();
 
         // ---- certIsFilteredOut + Store preconditions, in the reference's order
         if (act) {
@@ -390,25 +357,6 @@ __global__ void __launch_bounds__(WARPS * 32) map_stream_kernel(const __grid_con
             }
         }
     }
-}
-
-template <int WARPS, int CHUNK, int LOADER, int ROLLED = 0>
-static cudaError_t launch_stream_t(const MapParams& p, int sm_count, int ctas_per_sm, cudaStream_t s) {
-    using Cfg = StreamCfg<WARPS, CHUNK, LOADER>;
-    auto kern = map_stream_kernel<WARPS, CHUNK, LOADER, ROLLED>;
-    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem);
-    if (err != cudaSuccess) return err;
-    const uint64_t ngroups = (p.n + 31) / 32;
-    uint64_t ctas = (uint64_t)sm_count * ctas_per_sm;
-    // The grid is persistent and fills every SM, so a kernel launched on another stream while K_map runs (the
-    // NCCL key exchange of the previous sub-batch at N>1) finds no free shared memory / registers until K_map
-    // ends.  Leaving a few CTA slots empty gives such kernels somewhere to run.
-    static const int reserve = env_int("CTMR_MAP_RESERVE_CTAS", 0);
-    if (reserve > 0 && (uint64_t)reserve < ctas) ctas -= (uint64_t)reserve;
-    const uint64_t need = (ngroups + WARPS - 1) / WARPS;
-    if (need < ctas) ctas = need ? need : 1;
-    kern<<<(unsigned)ctas, WARPS * 32, Cfg::kSmem, s>>>(p);
-    return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -529,51 +477,22 @@ cudaError_t launch_sha_ceiling(uint32_t iters, int rolled, int ctas_per_sm, int 
     return cudaGetLastError();
 }
 
-// Shape of the persistent grid = the best measured before the port (DESIGN.md §3, K_map).  A build with
-// CTMR_EXPERIMENTS=1 adds the environment overrides used for the A/B runs (tools/ab_*.sh).
 cudaError_t launch_map(const MapParams& p, int sm_count, cudaStream_t s) {
     if (p.n == 0) return cudaSuccess;
-    static const int light = env_int("CTMR_MAP_LIGHT", 1);
-    if (p.sha256 == nullptr && light) {  // no fingerprint requested: nothing to stream
+    if (p.sha256 == nullptr) {  // no fingerprint requested: nothing to stream
         map_light_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, s>>>(p);
         return cudaGetLastError();
     }
-#ifdef CTMR_EXPERIMENTS  // tuning + measured-and-rejected variants (DESIGN.md): not in the product build
-    static const int variant = env_int("CTMR_MAP_VARIANT", 2);   // 1: v1 (global-memory walk), 2: streaming walk
-    static const int loader = env_int("CTMR_MAP_LOADER", 0);     // 0: cp.async (LDGSTS), 1: TMA bulk copy
-    static const int warps = env_int("CTMR_MAP_WARPS", 8);
-    static const int chunk = env_int("CTMR_MAP_CHUNK", 128);
-    static const int cps = env_int("CTMR_MAP_CTAS_PER_SM", 0);
-    static const int rolled = env_int("CTMR_MAP_ROLLED", 1);
-    if (variant != 2 && p.lens) return cudaErrorNotSupported;  // only the streaming kernel takes explicit lengths
-    if (variant == 1) return launch_map_v1(p, sm_count, s);
-    if (variant == 3) return launch_map_v3(p, sm_count, s);
-    if (loader == 1) {  // TMA bulk-copy loader, like for like with the shipped kernel: 8 warps, 128-byte chunks, rolled SHA-256
-        if (chunk == 128 && warps == 8) return launch_stream_t<8, 128, 1, 1>(p, sm_count, cps ? cps : 2, s);
-        if (chunk == 128) return launch_stream_t<4, 128, 1, 1>(p, sm_count, cps ? cps : 4, s);
-        return launch_stream_t<4, 256, 1, 1>(p, sm_count, cps ? cps : 2, s);
-    }
-    if (rolled >= 2 && chunk == 128) {
-        if (rolled == 2) return launch_stream_t<8, 128, 0, 2>(p, sm_count, cps ? cps : 2, s);
-        if (rolled == 3) return launch_stream_t<8, 128, 0, 3>(p, sm_count, cps ? cps : 2, s);
-        if (rolled == 4) return launch_stream_t<8, 128, 0, 4>(p, sm_count, cps ? cps : 2, s);
-    }
-    if (rolled && chunk == 64) return launch_stream_t<8, 64, 0, 1>(p, sm_count, cps ? cps : 3, s);
-    if (rolled && chunk == 128 && warps == 6) return launch_stream_t<6, 128, 0, 1>(p, sm_count, cps ? cps : 3, s);
-    if (rolled && chunk == 256) {
-        if (warps == 4) return launch_stream_t<4, 256, 0, 1>(p, sm_count, cps ? cps : 2, s);
-        return launch_stream_t<8, 256, 0, 1>(p, sm_count, cps ? cps : 1, s);
-    }
-    if (!rolled) {
-        if (chunk == 128) return warps == 8 ? launch_stream_t<8, 128, 0>(p, sm_count, cps ? cps : 2, s)
-                                            : launch_stream_t<4, 128, 0>(p, sm_count, cps ? cps : 4, s);
-        return warps == 8 ? launch_stream_t<8, 256, 0>(p, sm_count, cps ? cps : 1, s) : launch_stream_t<4, 256, 0>(p, sm_count, cps ? cps : 2, s);
-    }
-    return launch_stream_t<8, 128, 0, 1>(p, sm_count, cps ? cps : 2, s);
-#else
-    // the shipped shape: 8 warps x 32 lanes, 128-byte chunks, cp.async staging, rolled SHA-256, 2 CTAs per SM
-    return launch_stream_t<8, 128, 0, 1>(p, sm_count, 2, s);
-#endif
+    using Cfg = StreamCfg;
+    cudaError_t err = cudaFuncSetAttribute(map_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem);
+    if (err != cudaSuccess) return err;
+    // persistent grid: kCtasPerSm CTAs on every SM, fewer when the batch has fewer warp groups
+    const uint64_t ngroups = (p.n + 31) / 32;
+    uint64_t ctas = (uint64_t)sm_count * Cfg::kCtasPerSm;
+    const uint64_t need = (ngroups + Cfg::kWarps - 1) / Cfg::kWarps;
+    if (need < ctas) ctas = need ? need : 1;
+    map_stream_kernel<<<(unsigned)ctas, Cfg::kWarps * 32, Cfg::kSmem, s>>>(p);
+    return cudaGetLastError();
 }
 
 }  // namespace ctmr

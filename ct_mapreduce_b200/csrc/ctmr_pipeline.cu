@@ -188,7 +188,6 @@ int agree_rounds(ctmr_ctx* c, uint64_t mine, uint64_t* agreed) {
 int issue_map(ctmr_ctx* c, Stage& s, int sidx, const BatchArgs& a, const Slice& sl, const uint32_t* map_dev, bool want_meta) {
     CU(c, cudaSetDevice(c->device));
     const uint64_t cnt = sl.hi - sl.lo;
-    const bool fused = c->fuse_insert || c->px.world > 1;  // a group always fuses: the routing is K_map's epilogue
     int rc = round_begin(c, sidx, s.stream);  // exchange parity = stage
     if (rc) return rc;
     if (cnt) {
@@ -220,15 +219,8 @@ int issue_map(ctmr_ctx* c, Stage& s, int sidx, const BatchArgs& a, const Slice& 
             dout.crldp_off = s.spans + 2 * E;
             dout.crldp_len = s.spans + 3 * E;
         }
-        MapParams p;
-        fill_map_params(c, &db, &dout, p, sidx, fused ? s.slot_of : nullptr, sidx);
-        if (c->bucket_by_length && cnt > 64 && p.sha256) {
-            CU(c, launch_len_order(s.offsets, nullptr, cnt, db.blob_bytes, s.len_hist, s.order, c->sm_count, s.stream));
-            p.order = s.order;
-        }
-        CU(c, launch_map(p, c->sm_count, s.stream));
-        // inserts commute (atomic max on ~index); only RESOLVE must see every earlier entry inserted
-        if (!fused) CU(c, launch_insert(c->st, s.keys, cnt, s.slot_of, s.stream));
+        rc = map_slice(c, &db, &dout, s.slot_of, sidx, s.order, s.len_hist, s.stream);
+        if (rc) return rc;
     }
     rc = round_publish(c, sidx, s.stream);  // how many records this rank left in each owner's inbox
     if (rc) return rc;
@@ -242,12 +234,7 @@ int issue_owner_insert(ctmr_ctx* c, Stage& s, int sidx) {
 }
 
 int issue_resolve(ctmr_ctx* c, Stage& s, int sidx, const Slice& sl) {
-    const uint64_t cnt = sl.hi - sl.lo;
-    if (cnt) CU(c, launch_resolve(c->st, s.keys, cnt, s.slot_of, s.pair_slot, s.was_unknown, s.stream));
-    int rc = round_owner_resolve(c, sidx, c->stage_entries, s.stream);
-    if (rc) return rc;
-    if (cnt) CU(c, launch_resolve_pairs(c->st, s.keys, cnt, s.pair_slot, s.was_unknown, s.first, s.stream));
-    rc = round_owner_pairs(c, sidx, c->stage_entries, s.stream);
+    int rc = round_resolve(c, sidx, c->stage_entries, s.keys, sl.hi - sl.lo, s.slot_of, s.pair_slot, s.was_unknown, s.first, s.stream);
     if (rc) return rc;
     CU(c, cudaEventRecord(s.reduced, s.stream));
     return CTMR_OK;

@@ -250,7 +250,7 @@ int ctmr_reduce_device(ctmr_ctx* ctx, const ctmr_key* keys, uint64_t m, uint8_t*
 int ctmr_process_device(ctmr_ctx* ctx, const ctmr_dev_batch* batch, const ctmr_dev_out* out, void* stream);
 
 /* CUDA-event timings of the last ctmr_process_device call, valid once its stream has been synchronised:
- * map_ms = summed duration of the K_map stage (measured on the stream it ran on), total_ms = whole call */
+ * map_ms = span of the K_map launches (first start to last end), total_ms = whole call */
 int ctmr_profile_last(ctmr_ctx* ctx, float* map_ms, float* total_ms);
 
 /* copy the per-issuer histogram (uint64 [n_slots], dense index order) and the status counters

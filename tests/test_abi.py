@@ -73,16 +73,33 @@ def _sass_of(kernel_substr):
 
 
 def test_shipped_hot_kernel_is_what_design_md_says():
-    """The product build carries sm_90a SASS only, the hot kernel it ships (and only that instantiation of the streaming
-    map) stages certificates with asynchronous global->shared copies and keeps SHA-256's additions off the ALU pipe;
-    the measured-and-rejected variants (TMA bulk loader, v1, dynamic scheduling) are NOT linked in."""
+    """The library carries sm_90a SASS only, its one streaming map kernel stages certificates with asynchronous
+    global->shared copies and keeps SHA-256's additions off the ALU pipe; the measured-and-rejected variants (TMA bulk
+    loader, v1, dynamic scheduling, see DESIGN.md) are not in it."""
     blocks = _sass_of("map_stream_kernel")
-    assert len(blocks) == 1, [b.split("\n", 1)[0] for b in blocks]   # one shipped instantiation: <8,128,0,1>
+    assert len(blocks) == 1, [b.split("\n", 1)[0] for b in blocks]   # one streaming map kernel
     hot = blocks[0]
     assert "LDGSTS" in hot            # per-lane cp.async staging
-    assert "UBLKCP" not in hot        # the TMA bulk loader is an experiment (CTMR_EXPERIMENTS=1), see DESIGN.md
+    assert "UBLKCP" not in hot        # no TMA bulk loader, see DESIGN.md
     assert hot.count("SHF.") > 150 and hot.count("IMAD") > 100   # rotations on ALU, additions on the FMA pipe
     assert not _sass_of("map_kernel_v1") and not _sass_of("map_dyn_kernel")
+
+
+def test_library_reads_no_tuning_switches():
+    """What the library computes, and how fast, does not hang on environment variables: the only ones it reads are the
+    rounds of the collective call (documented in include/ctmr.h), the peer barrier's timeout and the front end's text
+    capacity (which the tests shrink)."""
+    kept = {"CTMR_PEER_ROUNDS", "CTMR_PEER_TIMEOUT_MS", "CTMR_FE_TEXT_CAP"}
+    csrc = os.path.join(ROOT, "ct_mapreduce_b200", "csrc")
+    read = {}
+    for f in sorted(os.listdir(csrc)):
+        txt = open(os.path.join(csrc, f), errors="ignore").read()
+        for name in re.findall(r'\b(?:getenv|env_int)\(\s*"([^"]*)"', txt):
+            read.setdefault(name, []).append(f)
+        # a name that is not a literal could hide a switch from this test: only env_int's own body passes one on
+        assert re.findall(r'\bgetenv\(\s*(?!")([^)]*)\)', txt) in ([], ["name"]), f
+    assert "CTMR_PEER_ROUNDS" in read
+    assert set(read) <= kept, {k: v for k, v in read.items() if k not in kept}
 
 
 def test_table_atomics_are_local_and_only_string_identities_cross_gpus():

@@ -1,5 +1,5 @@
-// ctmr_api.cu -- the C ABI of include/ctmr.h: context, issuer registry, host-buffer batch
-// pipeline (H2D / kernels / D2H overlapped over three streams) and the device-resident entry points.
+// ctmr_api.cu -- the C ABI of include/ctmr.h: context, issuer registry, the steps of a round of the key exchange and
+// run_round, which sequences them for every caller, and the device-resident entry points.
 // There is deliberately no CPU implementation of the path in this file or anywhere in the library:
 // without a CUDA device ctmr_create fails.
 #include "ctmr_ctx.cuh"
@@ -140,6 +140,10 @@ static void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev
     }
 }
 
+// K_map over one slice on stream s.  fused_slot_of != NULL: the keys go straight into the table (this rank's) or to
+// their owners' inboxes of exchange `parity`, slot -> fused_slot_of.  The fingerprint path of more than 64 entries first
+// orders the slice by length into order[0..n), with len_hist (256 counters) as scratch: rounds that may run concurrently
+// pass separate histograms.
 int map_slice(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, uint32_t* fused_slot_of, int parity, uint32_t* order,
               unsigned int* len_hist, cudaStream_t s) {
     MapParams p;
@@ -228,16 +232,20 @@ int alloc_exchange(ctmr_ctx* c, uint32_t world) {
     return CTMR_OK;
 }
 
+// The steps of one round of the exchange on stream s (no-ops on a single GPU); run_round sequences them.
+// before K_map: the cursors of this parity to 0
 int round_begin(ctmr_ctx* c, int parity, cudaStream_t s) {
     if (c->px.world <= 1) return CTMR_OK;
     CU(c, cudaMemsetAsync(c->cursors + (size_t)parity * kMaxWorld, 0, kMaxWorld * sizeof(unsigned long long), s));
     return CTMR_OK;
 }
+// after K_map: the region sizes to the owners
 int round_publish(ctmr_ctx* c, int parity, cudaStream_t s) {
     if (c->px.world <= 1) return CTMR_OK;
     CU(c, launch_publish_counts(c->px, (uint32_t)parity, c->cursors + (size_t)parity * kMaxWorld, s));
     return CTMR_OK;
 }
+// owner: the inbox records into the table, then their was_unknown, counts and pair slots, then their first_issuer_hour
 int round_owner_insert(ctmr_ctx* c, int parity, uint64_t maxr, cudaStream_t s) {
     if (c->px.world <= 1) return CTMR_OK;
     CU(c, launch_inbox_insert(c->st, c->px, (uint32_t)parity, maxr, c->in_slot, s));
@@ -253,12 +261,15 @@ int round_owner_pairs(ctmr_ctx* c, int parity, uint64_t maxr, cudaStream_t s) {
     CU(c, launch_inbox_pairs(c->st, c->px, (uint32_t)parity, maxr, c->in_pair, s));
     return CTMR_OK;
 }
+// the bits of the entries routed away, from their owners
 int round_pull(ctmr_ctx* c, int parity, uint64_t maxr, uint8_t* was_unknown, uint8_t* first, cudaStream_t s) {
     if (c->px.world <= 1) return CTMR_OK;
     CU(c, launch_pull_bits(c->px, (uint32_t)parity, c->cursors + (size_t)parity * kMaxWorld,
                            c->rev + (uint64_t)parity * c->px.world * c->px.X, maxr, was_unknown, first, s));
     return CTMR_OK;
 }
+// the owner passes of a round after every insert of it (own keys and inbox records) has landed, in the order
+// lowest-index-wins needs: K_resolve, inbox resolve, K_pairs, inbox pairs
 int round_resolve(ctmr_ctx* c, int parity, uint64_t maxr, const ctmr_key* keys, uint64_t cnt, const uint32_t* slot_of,
                   uint32_t* pair_slot, uint8_t* was_unknown, uint8_t* first, cudaStream_t s) {
     CU(c, launch_resolve(c->st, keys, cnt, slot_of, pair_slot, was_unknown, s));
@@ -266,6 +277,94 @@ int round_resolve(ctmr_ctx* c, int parity, uint64_t maxr, const ctmr_key* keys, 
     if (rc) return rc;
     CU(c, launch_resolve_pairs(c->st, keys, cnt, pair_slot, was_unknown, first, s));
     return round_owner_pairs(c, parity, maxr, s);
+}
+
+// A sync: member r's reduce stream waits for event `ev` of every other member, then meets the other processes at
+// `channel` (peer_barrier does nothing unless the ctx is in PEER_IPC mode).
+static int sync_members(const RoundMember* m, uint32_t W, uint32_t r, cudaEvent_t RoundMember::*ev, uint32_t channel) {
+    ctmr_ctx* c = m[r].c;
+    for (uint32_t q = 0; q < W; ++q)
+        if (q != r) CU(c, cudaStreamWaitEvent(m[r].reduce_stream, m[q].*ev, 0));
+    return peer_barrier(c, channel, m[r].reduce_stream);
+}
+
+// One round of the key exchange, the one sequence the host pipeline, the group front end and ctmr_process_device share:
+//
+//     map + route: round_begin, K_map (a key of a set this GPU owns goes straight into its table, any other key is
+//                  appended as a 64-byte record to the OWNER's inbox over NVLink), round_publish
+//     -- sync 1: every member's appends of this round have landed --
+//     owner passes: inbox insert; K_resolve and K_pairs over the own entries AND the inbox records (round_resolve)
+//     -- sync 2: every owner's bits of this round are ready --
+//     pull of the bits of the entries routed away [-> string identities: insert, sync 3, read-back]
+//
+// sync = CUDA events between the members one process drives, a barrier kernel on flags in peer memory between
+// processes.  Sync 1, and the chain (or one reduce stream) that orders the owner passes of consecutive rounds, give the
+// invariant lowest-index-wins needs: when an entry is resolved, every entry with a lower global index has been inserted.
+int run_round(const RoundMember* m, uint32_t W, int parity, uint64_t max_per_region, bool want_meta, ctmr_ctx** failed) {
+    // The host issues phase p for every member before phase p + 1 for any member: cudaStreamWaitEvent on an event that
+    // has not been recorded yet returns at once and waits for nothing.
+    auto each = [&](auto phase) -> int {
+        for (uint32_t r = 0; r < W; ++r) {
+            *failed = m[r].c;
+            CU(m[r].c, cudaSetDevice(m[r].c->device));
+            const int rc = phase(m[r], r);
+            if (rc) return rc;
+        }
+        return CTMR_OK;
+    };
+    int rc = each([&](const RoundMember& x, uint32_t) -> int {  // map + route: own keys into the own table, the others to their owners
+        ctmr_ctx* c = x.c;
+        if (x.map_start) CU(c, cudaEventRecord(x.map_start, x.map_stream));
+        int rc = round_begin(c, parity, x.map_stream);
+        if (rc == CTMR_OK && x.db.n) rc = map_slice(c, &x.db, &x.dout, x.slot_of, parity, x.order, x.len_hist, x.map_stream);
+        if (rc) return rc;
+        if (x.map_end) CU(c, cudaEventRecord(x.map_end, x.map_stream));
+        rc = round_publish(c, parity, x.map_stream);
+        if (rc) return rc;
+        CU(c, cudaEventRecord(x.mapped, x.map_stream));
+        return CTMR_OK;
+    });
+    if (rc) return rc;
+    rc = each([&](const RoundMember& x, uint32_t r) -> int {  // sync 1: every member's appends have landed; the owner passes
+        ctmr_ctx* c = x.c;
+        const cudaStream_t s = x.reduce_stream;
+        if (x.map_stream != s) CU(c, cudaStreamWaitEvent(s, x.mapped, 0));
+        int rc = sync_members(m, W, r, &RoundMember::mapped, x.ch_map);
+        if (rc == CTMR_OK) rc = round_owner_insert(c, parity, max_per_region, s);
+        if (rc) return rc;
+        if (x.prev_reduced) CU(c, cudaStreamWaitEvent(s, x.prev_reduced, 0));
+        rc = round_resolve(c, parity, max_per_region, x.dout.keys, x.db.n, x.slot_of, x.pair_slot, x.dout.was_unknown,
+                           x.dout.first_issuer_hour, s);
+        if (rc) return rc;
+        if (x.reduced) CU(c, cudaEventRecord(x.reduced, s));
+        return CTMR_OK;
+    });
+    if (rc) return rc;
+    rc = each([&](const RoundMember& x, uint32_t r) -> int {  // sync 2: every owner has the bits ready; pull, string identities' insert
+        ctmr_ctx* c = x.c;
+        const cudaStream_t s = x.reduce_stream;
+        int rc = sync_members(m, W, r, &RoundMember::reduced, x.ch_resolve);
+        if (rc == CTMR_OK) rc = round_pull(c, parity, max_per_region, x.dout.was_unknown, x.dout.first_issuer_hour, s);
+        if (rc || !want_meta) return rc;
+        if (x.prev_meta_done) CU(c, cudaStreamWaitEvent(s, x.prev_meta_done, 0));
+        const ctmr_dev_out& o = x.dout;
+        if (x.db.n)  // needs this member's was_unknown bits, i.e. the pull
+            CU(c, launch_meta_insert(c->st, x.db.blob, x.db.offsets, o.keys, x.db.n, o.was_unknown, o.issuer_name_off, o.issuer_name_len,
+                                     o.crldp_off, o.crldp_len, x.meta_slots, s));
+        if (x.meta_done) CU(c, cudaEventRecord(x.meta_done, s));
+        return CTMR_OK;
+    });
+    if (rc == CTMR_OK && want_meta)
+        rc = each([&](const RoundMember& x, uint32_t r) -> int {  // sync 3: every member's string identities are in; read-back
+            ctmr_ctx* c = x.c;
+            int rc = sync_members(m, W, r, &RoundMember::meta_done, x.ch_meta);
+            if (rc == CTMR_OK && x.db.n)
+                CU(c, launch_meta_resolve(c->st, x.dout.keys, x.db.n, x.meta_slots, x.dout.first_issuer_dn, x.dout.first_crldp,
+                                          x.reduce_stream));
+            return rc;
+        });
+    if (rc == CTMR_OK) *failed = nullptr;
+    return rc;
 }
 
 // Rounds of E entries with a SHORT last round (a quarter of E): what a call exposes at its end is the reduce chain of its
@@ -296,6 +395,19 @@ int reduce_on(ctmr_ctx* c, const ctmr_key* keys, uint64_t m, uint32_t* slot_of, 
     return CTMR_OK;
 }
 
+// the outputs of entries [lo, ..): every array of o offset by lo entries
+ctmr_dev_out dev_out_at(const ctmr_dev_out& o, uint64_t lo) {
+    auto at = [lo](auto* p, uint64_t per = 1) { return p ? p + lo * per : p; };
+    ctmr_dev_out w;
+    w.status = at(o.status); w.sha256 = at(o.sha256, 32); w.exp_hour = at(o.exp_hour);
+    w.serial_off = at(o.serial_off); w.serial_len = at(o.serial_len); w.keys = at(o.keys);
+    w.was_unknown = at(o.was_unknown); w.first_issuer_hour = at(o.first_issuer_hour);
+    w.issuer_name_off = at(o.issuer_name_off); w.issuer_name_len = at(o.issuer_name_len);
+    w.crldp_off = at(o.crldp_off); w.crldp_len = at(o.crldp_len);
+    w.first_issuer_dn = at(o.first_issuer_dn); w.first_crldp = at(o.first_crldp);
+    return w;
+}
+
 
 // ------------------------------------------------------------------------------------------------ front end plumbing
 void fe_destroy(ctmr_ctx* c) {
@@ -319,6 +431,8 @@ void fe_destroy(ctmr_ctx* c) {
     if (f->ev0) cudaEventDestroy(f->ev0);
     if (f->ev1) cudaEventDestroy(f->ev1);
     if (f->ev2) cudaEventDestroy(f->ev2);
+    for (cudaEvent_t e : {f->mapped, f->reduced, f->meta_done})
+        if (e) cudaEventDestroy(e);
     delete f;
     c->fe = nullptr;
 }
@@ -451,7 +565,10 @@ int ensure_frontend(ctmr_ctx* c) {
     if (cudaMemsetAsync(f->slots_dev, 0, (f->slot_mask + 1) * sizeof(IssuerCertSlot), c->stream) != cudaSuccess ||
         cudaStreamSynchronize(c->stream) != cudaSuccess ||
         cudaEventCreate(&f->ev0) != cudaSuccess ||
-        cudaEventCreate(&f->ev1) != cudaSuccess || cudaEventCreate(&f->ev2) != cudaSuccess) {
+        cudaEventCreate(&f->ev1) != cudaSuccess || cudaEventCreate(&f->ev2) != cudaSuccess ||
+        cudaEventCreateWithFlags(&f->mapped, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&f->reduced, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&f->meta_done, cudaEventDisableTiming) != cudaSuccess) {
         fail(c, CTMR_E_CUDA, "front end: initialisation failed");
         return bail(CTMR_E_CUDA);
     }
@@ -578,8 +695,6 @@ void ctmr_destroy(ctmr_ctx* c) {
     }
     cudaFree(c->xchg); cudaFree(c->cursors); cudaFree(c->rev); cudaFree(c->in_slot); cudaFree(c->in_pair);
     for (cudaEvent_t e : c->ev_pulled)
-        if (e) cudaEventDestroy(e);
-    for (cudaEvent_t e : c->ev_g)
         if (e) cudaEventDestroy(e);
     cudaFree(c->shared); cudaFree(c->small_dev);
     cudaFree(c->issuer_map_dev); cudaFree(c->keys_scratch); cudaFree(c->slot_scratch); cudaFree(c->pair_scratch);
@@ -829,72 +944,48 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     const bool coll = c->peer_mode == PEER_IPC && world > 1;
     if (c->peer_mode == PEER_GROUP && world > 1)
         return fail(c, CTMR_E_INVALID, "members of an in-process group are driven through ctmr_group_process_batch");
+    if (want_meta && world > 1) return fail(c, CTMR_E_INVALID, "first_issuer_dn / first_crldp of a group come from the host-buffer call");
     const int nsub = coll ? (int)peer_rounds() : (b->n >= (1u << 21) ? 8 : (b->n >= (1u << 18) ? 2 : 1));
     const uint64_t per_round = device_round_entries(b->n, (uint32_t)nsub);
     if (coll && per_round > c->px.X)
         return fail(c, CTMR_E_BATCH_TOO_LARGE, "entries per round exceed the key-exchange regions: raise config.max_round_entries to ceil(n / ctmr_peer_rounds())");
-    ctmr_key* keys = o->keys ? o->keys : c->keys_scratch;
-    uint8_t* wu = o->was_unknown ? o->was_unknown : c->bits_scratch;
-    uint8_t* fi = o->first_issuer_hour ? o->first_issuer_hour : c->bits_scratch + b->n;
+    ctmr_dev_out all = *o;  // the outputs the rounds write, scratch where the caller asks for none
+    if (!all.keys) all.keys = c->keys_scratch;
+    if (!all.was_unknown) all.was_unknown = c->bits_scratch;
+    if (!all.first_issuer_hour) all.first_issuer_hour = c->bits_scratch + b->n;
     CU(c, cudaEventRecord(c->ev_fork, user));
     CU(c, cudaStreamWaitEvent(c->stream_a, c->ev_fork, 0));
     CU(c, cudaStreamWaitEvent(c->stream_a2, c->ev_fork, 0));
     CU(c, cudaStreamWaitEvent(c->stream_b, c->ev_fork, 0));
     for (int k = 0; k < nsub; ++k) {
-        uint64_t lo, hi;
-        lo = std::min<uint64_t>(b->n, per_round * k);
-        hi = std::min<uint64_t>(b->n, per_round * (k + 1));
-        const uint64_t cnt = hi - lo;
-        ctmr_dev_batch sb = *b;
-        sb.offsets = b->offsets + lo;
-        sb.lens = b->lens ? b->lens + lo : nullptr;
-        sb.n = cnt;
-        sb.issuer_idx = b->issuer_idx ? b->issuer_idx + lo : nullptr;
-        sb.first_index = coll ? b->first_index + ((uint64_t)k * world + rank) * per_round : b->first_index + lo;
-        ctmr_dev_out so{};
-        so.status = o->status ? o->status + lo : nullptr;
-        so.sha256 = o->sha256 ? o->sha256 + lo * 32 : nullptr;
-        so.exp_hour = o->exp_hour ? o->exp_hour + lo : nullptr;
-        so.serial_off = o->serial_off ? o->serial_off + lo : nullptr;
-        so.serial_len = o->serial_len ? o->serial_len + lo : nullptr;
-        so.keys = keys + lo;
-        so.issuer_name_off = o->issuer_name_off ? o->issuer_name_off + lo : nullptr;
-        so.issuer_name_len = o->issuer_name_len ? o->issuer_name_len + lo : nullptr;
-        so.crldp_off = o->crldp_off ? o->crldp_off + lo : nullptr;
-        so.crldp_len = o->crldp_len ? o->crldp_len + lo : nullptr;
-        const int parity = k % (int)kParities;
+        const uint64_t lo = std::min<uint64_t>(b->n, per_round * k), hi = std::min<uint64_t>(b->n, per_round * (k + 1));
+        RoundMember x;
+        x.c = c;
+        x.db = *b;
+        x.db.offsets = b->offsets + lo;
+        x.db.lens = b->lens ? b->lens + lo : nullptr;
+        x.db.n = hi - lo;
+        x.db.issuer_idx = b->issuer_idx ? b->issuer_idx + lo : nullptr;
+        x.db.first_index = coll ? b->first_index + ((uint64_t)k * world + rank) * per_round : b->first_index + lo;
+        x.dout = dev_out_at(all, lo);
+        x.slot_of = c->slot_scratch + lo; x.pair_slot = c->pair_scratch + lo; x.order = c->order_scratch + lo;
+        x.len_hist = c->len_hist_sub[k];
+        x.meta_slots = c->meta_scratch + 2 * lo;
         // consecutive K_map launches on alternating streams: the next launch's CTAs fill the SMs the previous one's
         // draining tail leaves idle (a persistent grid ends with its slowest warps)
-        cudaStream_t sa = (k & 1) ? c->stream_a2 : c->stream_a;
-        if (world > 1 && k >= (int)kParities) CU(c, cudaStreamWaitEvent(sa, c->ev_pulled[parity], 0));  // the parity's regions are free again
-        CU(c, cudaEventRecord(c->ev_map0[k], sa));
-        rc = round_begin(c, parity, sa);
+        x.map_stream = (k & 1) ? c->stream_a2 : c->stream_a;
+        x.reduce_stream = c->stream_b;
+        x.mapped = c->ev_tok[k];  // K_map + the published sizes; one reduce stream orders the rounds, so no chain
+        x.map_start = c->ev_map0[k];
+        x.map_end = c->ev_map1[k];  // before the publish: map_ms times K_map alone
+        x.ch_map = CH_DEV_MAP;
+        x.ch_resolve = x.ch_meta = CH_DEV_RESOLVE;  // sync 3 meets no barrier: a collective call has no string identities
+        const int parity = k % (int)kParities;
+        if (world > 1 && k >= (int)kParities) CU(c, cudaStreamWaitEvent(x.map_stream, c->ev_pulled[parity], 0));  // the parity's regions are free again
+        ctmr_ctx* failed = nullptr;
+        rc = run_round(&x, 1, parity, per_round, want_meta, &failed);
         if (rc) return rc;
-        rc = map_slice(c, &sb, &so, c->slot_scratch + lo, parity, c->order_scratch + lo, c->len_hist_sub[k], sa);
-        if (rc) return rc;
-        CU(c, cudaEventRecord(c->ev_map1[k], sa));
-        rc = round_publish(c, parity, sa);  // region sizes to the owners (outside K_map's timed bracket)
-        if (rc) return rc;
-        CU(c, cudaEventRecord(c->ev_tok[k], sa));   // ordering token: K_map + the published sizes
-        CU(c, cudaStreamWaitEvent(c->stream_b, c->ev_tok[k], 0));
-        cudaStream_t sbm = c->stream_b;
-        rc = peer_barrier(c, CH_DEV_MAP, sbm);  // every rank's appends of rounds <= k have landed in the owners' inboxes
-        if (rc) return rc;
-        rc = round_owner_insert(c, parity, per_round, sbm);
-        if (rc) return rc;
-        rc = round_resolve(c, parity, per_round, keys + lo, cnt, c->slot_scratch + lo, c->pair_scratch + lo, wu + lo, fi + lo, sbm);
-        if (rc) return rc;
-        rc = peer_barrier(c, CH_DEV_RESOLVE, sbm);  // every owner has the result bits of this round's records ready
-        if (rc) return rc;
-        rc = round_pull(c, parity, per_round, wu + lo, fi + lo, sbm);
-        if (rc) return rc;
-        if (world > 1) CU(c, cudaEventRecord(c->ev_pulled[parity], sbm));
-        if (want_meta) {
-            if (world > 1) return fail(c, CTMR_E_INVALID, "first_issuer_dn / first_crldp of a group come from the host-buffer call");
-            CU(c, launch_meta(c->st, sb.blob, sb.offsets, keys + lo, cnt, wu + lo, so.issuer_name_off, so.issuer_name_len, so.crldp_off,
-                              so.crldp_len, c->meta_scratch + 2 * lo, o->first_issuer_dn ? o->first_issuer_dn + lo : nullptr,
-                              o->first_crldp ? o->first_crldp + lo : nullptr, sbm));
-        }
+        if (world > 1) CU(c, cudaEventRecord(c->ev_pulled[parity], c->stream_b));
         CU(c, cudaEventRecord(c->ev_red1[k], c->stream_b));
     }
     c->last_sub = nsub;

@@ -1,6 +1,8 @@
 // ctmr_ctx.cuh -- internal: the context behind the opaque ctmr_ctx of include/ctmr.h, shared by the translation
-// units that implement the C ABI (ctmr_api.cu: lifecycle, issuers, device entry points, read side, front end;
-// ctmr_pipeline.cu: the host-buffer batch pipeline on one GPU, on a group of GPUs, and across processes).
+// units that implement the C ABI (ctmr_api.cu: lifecycle, issuers, the steps of a round and run_round, which sequences
+// one round of the key exchange for all three callers, device entry points, read side, front end plumbing;
+// ctmr_pipeline.cu: the host-buffer batch pipeline on one GPU, on a group of GPUs, and across processes, and the copy of
+// a round's outputs to the host; ctmr_frontend_api.cu: the wire-format front end on one GPU and on a group).
 #pragma once
 #include <algorithm>
 #include <array>
@@ -107,6 +109,7 @@ struct FrontEnd {
     uint32_t unknown_cap = 0;
     unsigned int* unknown_count = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
+    cudaEvent_t mapped = nullptr, reduced = nullptr, meta_done = nullptr;  // round events of ctmr_group_process_raw
     float fe_ms = 0.f, path_ms = 0.f;
     uint64_t launches = 0;
     PemStage pem;
@@ -166,7 +169,6 @@ struct ctmr_ctx {
     unsigned long long* cursors = nullptr;  // [kParities][kMaxWorld] records appended per owner (local)
     uint32_t* rev = nullptr;                // [kParities][world][X] inbox position -> entry
     uint32_t *in_slot = nullptr, *in_pair = nullptr;  // [kParities][world][X] owner-side scratch of the inbox records
-    cudaEvent_t ev_g[3] = {};               // ctmr_group_process_raw: mapped / reduced / string identities inserted
     cudaEvent_t ev_pulled[kParities] = {};  // ctmr_process_device: round k's bits pulled (its exchange parity may be reused)
     unsigned long long epoch[kPeerChannels] = {};
     struct ctmr_group* group = nullptr;    // set when the ctx is a member of an in-process group
@@ -218,28 +220,37 @@ int fail(ctmr_ctx* ctx, int code, const std::string& msg);
     } while (0)
 
 uint64_t pow2_at_least(uint64_t v);
-// K_map over one slice on stream s.  fused_slot_of != NULL: the keys go straight into the table (this rank's) or to
-// their owners' inboxes of exchange `parity`, slot -> fused_slot_of.  The fingerprint path of more than 64 entries first
-// orders the slice by length into order[0..n), with len_hist (256 counters) as scratch: rounds that may run concurrently
-// pass separate histograms.
-int map_slice(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, uint32_t* fused_slot_of, int parity, uint32_t* order,
-              unsigned int* len_hist, cudaStream_t s);
 int ensure_order(ctmr_ctx* c, uint64_t n);   // c->order_scratch holds >= n entries, c->len_hist exists
 // key exchange: allocation for a group of `world` ranks, views of every rank's area
 size_t exchange_bytes(uint32_t world, uint64_t X);
 int alloc_exchange(ctmr_ctx* c, uint32_t world);
 void attach_exchange(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
-// one round of the exchange on stream s (no-ops on a single GPU)
-int round_begin(ctmr_ctx* c, int parity, cudaStream_t s);                       // before K_map: cursors of this parity to 0
-int round_publish(ctmr_ctx* c, int parity, cudaStream_t s);                     // after K_map: region sizes to the owners
-int round_owner_insert(ctmr_ctx* c, int parity, uint64_t max_per_region, cudaStream_t s);   // owner: inbox records into the table
-int round_owner_resolve(ctmr_ctx* c, int parity, uint64_t max_per_region, cudaStream_t s);  // ... their was_unknown, counts, pair slots
-int round_owner_pairs(ctmr_ctx* c, int parity, uint64_t max_per_region, cudaStream_t s);    // ... their first_issuer_hour
-int round_pull(ctmr_ctx* c, int parity, uint64_t max_per_region, uint8_t* was_unknown, uint8_t* first, cudaStream_t s);
-// the owner passes of a round after every insert of it (own keys and inbox records) has landed, in the order
-// lowest-index-wins needs: K_resolve, inbox resolve, K_pairs, inbox pairs
-int round_resolve(ctmr_ctx* c, int parity, uint64_t max_per_region, const ctmr_key* keys, uint64_t cnt, const uint32_t* slot_of,
-                  uint32_t* pair_slot, uint8_t* was_unknown, uint8_t* first, cudaStream_t s);
+
+// One member's part of a round of the key exchange: the GPU (ctx), its slice and where the slice's results and scratch
+// live (all device memory, [db.n] each unless noted), its streams, events and barrier channels.
+struct RoundMember {
+    ctmr_ctx* c = nullptr;
+    ctmr_dev_batch db{};  // db.n == 0: an empty slice, which still takes part in every sync
+    ctmr_dev_out dout{};  // keys, was_unknown and first_issuer_hour are required; spans and first_* when string identities are wanted
+    uint32_t *slot_of = nullptr, *pair_slot = nullptr;
+    uint32_t* order = nullptr;           // K_map's length order, with len_hist (256 counters) as scratch
+    unsigned int* len_hist = nullptr;
+    uint32_t* meta_slots = nullptr;      // [2 * db.n]
+    cudaStream_t map_stream = nullptr;   // round_begin, K_map, round_publish
+    cudaStream_t reduce_stream = nullptr;  // everything after sync 1; may be map_stream
+    // this round's events; reduced and meta_done may be null where nothing waits for them (one member, no chain)
+    cudaEvent_t mapped = nullptr, reduced = nullptr, meta_done = nullptr;
+    cudaEvent_t prev_reduced = nullptr, prev_meta_done = nullptr;  // optional: the previous round's, to chain on
+    cudaEvent_t map_start = nullptr, map_end = nullptr;            // optional: timing events around K_map
+    uint32_t ch_map = 0, ch_resolve = 0, ch_meta = 0;              // peer_barrier channels of sync 1, 2 and 3
+};
+// Issues one round for the W members this process drives: map + route, sync 1, owner passes, sync 2, pull, and with
+// want_meta the string identities (insert, sync 3, read-back).  `parity` selects the exchange regions and
+// max_per_region bounds one member's slice.  On error *failed names the member that failed.
+int run_round(const RoundMember* m, uint32_t W, int parity, uint64_t max_per_region, bool want_meta, ctmr_ctx** failed);
+// D2H of entries [0, cnt) of device outputs to entries [lo, lo + cnt) of the caller's outputs: every per-entry array of
+// ctmr_out that both sides have, on stream s
+int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* out, uint64_t lo, cudaStream_t s);
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise

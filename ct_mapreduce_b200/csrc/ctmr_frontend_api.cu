@@ -8,8 +8,9 @@
 //   front    fe_decode / fe_frame / fe_tbs / fe_issuer: the decoded leaves stay in the arena, the chunk becomes a
 //            device-resident batch (ctmr_dev_batch with explicit lengths);
 //   path     K_map ... K_pairs over that batch in place -- ctmr_process_device on one GPU; on a group one ROUND of the key
-//            exchange (ctmr_pipeline.cu's scheme with device-resident slices): every member maps its chunk, hands
-//            foreign keys to their owners over NVLink, the owners reduce, the bits are pulled back;
+//            exchange (run_round, ctmr_api.cu, with each member's chunk as its slice and its stream for everything):
+//            every member maps its chunk, hands foreign keys to their owners over NVLink, the owners reduce, the bits
+//            are pulled back;
 //   back     x509 leaf failures, PEM of the new certificates, outputs to the host.
 // On a group a round takes one chunk per member, cut from ONE contiguous window of the batch, so that entry i keeps
 // global index next_index + i and the result equals the single-GPU / sequential run on the same pages.
@@ -204,7 +205,6 @@ int fe_back(ctmr_ctx* c, const ctmr_raw_out* out, RawChunk& ch, uint64_t* pem_ba
     CU(c, cudaSetDevice(c->device));
     const uint64_t cnt = ch.hi - ch.lo, lo = ch.lo, E = f->cap_entries;
     const ctmr_out* po = &out->path;
-    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
     const bool want_pem = po->pem != nullptr;
     if (!cnt) {
         CU(c, cudaStreamSynchronize(s));
@@ -219,23 +219,10 @@ int fe_back(ctmr_ctx* c, const ctmr_raw_out* out, RawChunk& ch, uint64_t* pem_ba
         rc = pem_chunk(c, f->pem, f->decoded, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, lo, pem_base, s);
         if (rc) return rc;
     }
+    const int rc = copy_out(c, ch.dout, cnt, po, lo, s);
+    if (rc) return rc;
 #define FE_D2H(dst, src, bytes) \
     if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * ((bytes) / cnt), (src), (bytes), cudaMemcpyDeviceToHost, s))
-    FE_D2H(po->status, f->status, cnt);
-    FE_D2H(po->sha256, f->sha, cnt * 32);
-    FE_D2H(po->exp_hour, f->exp_hour, cnt * 8);
-    FE_D2H(po->serial_off, f->serial_off, cnt * 4);
-    FE_D2H(po->serial_len, f->serial_len, cnt * 4);
-    FE_D2H(po->was_unknown, f->was_unknown, cnt);
-    FE_D2H(po->first_issuer_hour, f->first, cnt);
-    if (want_meta) {
-        FE_D2H(po->issuer_name_off, ch.dout.issuer_name_off, cnt * 4);
-        FE_D2H(po->issuer_name_len, ch.dout.issuer_name_len, cnt * 4);
-        FE_D2H(po->crldp_off, ch.dout.crldp_off, cnt * 4);
-        FE_D2H(po->crldp_len, ch.dout.crldp_len, cnt * 4);
-        FE_D2H(po->first_issuer_dn, ch.dout.first_issuer_dn, cnt);
-        FE_D2H(po->first_crldp, ch.dout.first_crldp, cnt);
-    }
     FE_D2H(out->entry_status, f->entry_status, cnt);
     FE_D2H(out->entry_type, f->entry_type, cnt);
     FE_D2H(out->timestamp_ms, f->timestamp, cnt * 8);
@@ -318,82 +305,26 @@ void for_each_member(uint32_t W, std::vector<int>& rcs, F fn) {
     for (uint32_t r = started; r < W; ++r) rcs[r] = fn(r);
 }
 
-// One round of the path over the members' device-resident chunks: map + route, [events], owner passes, [events], pull,
-// [string identities: insert, events, read-back].  Each member works on its own stream; rounds are serialised by the
-// callers' fe_back, which is also what orders the rounds for lowest-index-wins.
-int group_round(ctmr_group* g, RawChunk* ch, int parity, ctmr_ctx** failed) {
-    const uint32_t W = (uint32_t)g->m.size();
-    int rc;
-    for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = g->m[r];
-        *failed = c;
-        CU(c, cudaSetDevice(c->device));
-        cudaStream_t s = c->stream;
-        const uint64_t cnt = ch[r].hi - ch[r].lo;
-        rc = ensure_scratch(c, std::max<uint64_t>(cnt, 1));
-        if (rc) return rc;
-        for (cudaEvent_t& e : c->ev_g)
-            if (!e) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        rc = round_begin(c, parity, s);
-        if (rc) return rc;
-        if (cnt) {
-            ch[r].dout.keys = c->keys_scratch;
-            rc = ensure_order(c, cnt);
-            if (rc) return rc;
-            rc = map_slice(c, &ch[r].db, &ch[r].dout, c->slot_scratch, parity, c->order_scratch, c->len_hist, s);
-            if (rc) return rc;
-        }
-        rc = round_publish(c, parity, s);
-        if (rc) return rc;
-        CU(c, cudaEventRecord(c->ev_g[0], s));
-    }
-    const uint64_t maxr = g->m[0]->fe->cap_entries;
-    for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = g->m[r];
-        *failed = c;
-        CU(c, cudaSetDevice(c->device));
-        cudaStream_t s = c->stream;
-        const uint64_t cnt = ch[r].hi - ch[r].lo;
-        for (uint32_t q = 0; q < W; ++q)
-            if (q != r) CU(c, cudaStreamWaitEvent(s, g->m[q]->ev_g[0], 0));
-        rc = round_owner_insert(c, parity, maxr, s);
-        if (rc) return rc;
-        rc = round_resolve(c, parity, maxr, c->keys_scratch, cnt, c->slot_scratch, c->pair_scratch, ch[r].dout.was_unknown,
-                           ch[r].dout.first_issuer_hour, s);
-        if (rc) return rc;
-        CU(c, cudaEventRecord(c->ev_g[1], s));
-    }
-    bool any_meta = false;
-    for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = g->m[r];
-        *failed = c;
-        CU(c, cudaSetDevice(c->device));
-        cudaStream_t s = c->stream;
-        const uint64_t cnt = ch[r].hi - ch[r].lo;
-        for (uint32_t q = 0; q < W; ++q)
-            if (q != r) CU(c, cudaStreamWaitEvent(s, g->m[q]->ev_g[1], 0));
-        rc = round_pull(c, parity, maxr, ch[r].dout.was_unknown, ch[r].dout.first_issuer_hour, s);
-        if (rc) return rc;
-        const bool want_meta = ch[r].dout.first_issuer_dn || ch[r].dout.first_crldp;
-        any_meta |= want_meta;
-        if (want_meta && cnt)
-            CU(c, launch_meta_insert(c->st, ch[r].db.blob, ch[r].db.offsets, c->keys_scratch, cnt, ch[r].dout.was_unknown, ch[r].dout.issuer_name_off,
-                                     ch[r].dout.issuer_name_len, ch[r].dout.crldp_off, ch[r].dout.crldp_len, c->meta_scratch, s));
-        CU(c, cudaEventRecord(c->ev_g[2], s));
-    }
-    if (any_meta)
-        for (uint32_t r = 0; r < W; ++r) {
-            ctmr_ctx* c = g->m[r];
-            *failed = c;
-            CU(c, cudaSetDevice(c->device));
-            cudaStream_t s = c->stream;
-            const uint64_t cnt = ch[r].hi - ch[r].lo;
-            for (uint32_t q = 0; q < W; ++q)
-                if (q != r) CU(c, cudaStreamWaitEvent(s, g->m[q]->ev_g[2], 0));
-            if (cnt)
-                CU(c, launch_meta_resolve(c->st, c->keys_scratch, cnt, c->meta_scratch, ch[r].dout.first_issuer_dn, ch[r].dout.first_crldp, s));
-        }
-    *failed = nullptr;
+// A member's device-resident chunk as its part of round `parity` (run_round).  Everything runs on the member's stream,
+// so there is no chain: fe_back waits for each round before the next is issued.
+int fe_member(ctmr_ctx* c, const RawChunk& ch, int parity, RoundMember& x) {
+    CU(c, cudaSetDevice(c->device));
+    int rc = ensure_scratch(c, std::max<uint64_t>(ch.db.n, 1));
+    if (rc == CTMR_OK) rc = ensure_order(c, ch.db.n);
+    if (rc) return rc;
+    x = RoundMember{};
+    x.c = c;
+    x.db = ch.db;
+    x.dout = ch.dout;
+    x.dout.keys = c->keys_scratch;
+    x.slot_of = c->slot_scratch; x.pair_slot = c->pair_scratch; x.order = c->order_scratch; x.len_hist = c->len_hist;
+    x.meta_slots = c->meta_scratch;
+    x.map_stream = x.reduce_stream = c->stream;
+    x.mapped = c->fe->mapped; x.reduced = c->fe->reduced; x.meta_done = c->fe->meta_done;
+    // the members of an in-process group meet through their events; peer_barrier does nothing for them
+    x.ch_map = CH_STAGE_MAP + parity;
+    x.ch_resolve = CH_STAGE_RESOLVE + parity;
+    x.ch_meta = CH_STAGE_META + parity;
     return CTMR_OK;
 }
 
@@ -448,6 +379,8 @@ int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out,
         c->fe->fe_ms = c->fe->path_ms = 0.f;
         c->fe->launches = 0;
     }
+    const ctmr_out* po = &out->path;
+    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
     uint64_t pem_base = 0, pos = 0;
     std::vector<RawChunk> cur, nxt;
     rc = plan_round(g, b, 0, 0, cur, failed);
@@ -468,7 +401,14 @@ int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out,
                 *failed = g->m[r];
                 return rcs[r];
             }
-        rc = group_round(g, cur.data(), k % (int)kParities, failed);
+        const int parity = k % (int)kParities;
+        RoundMember rm[kMaxWorld];
+        for (uint32_t r = 0; r < W; ++r) {
+            *failed = g->m[r];
+            rc = fe_member(g->m[r], cur[r], parity, rm[r]);
+            if (rc) return rc;
+        }
+        rc = run_round(rm, W, parity, c0->fe->cap_entries, want_meta, failed);
         if (rc) return rc;
         if (out->path.pem) {
             for (uint32_t r = 0; r < W; ++r) {  // in entry order: the PEM texts are appended in that order

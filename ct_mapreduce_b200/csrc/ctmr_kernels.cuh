@@ -181,13 +181,9 @@ cudaError_t launch_inbox_pairs(const DeviceState& st, const PeerExchange& px, ui
 cudaError_t launch_publish_counts(const PeerExchange& px, uint32_t parity, const unsigned long long* cursor, cudaStream_t s);
 cudaError_t launch_pull_bits(const PeerExchange& px, uint32_t parity, const unsigned long long* cursor, const uint32_t* rev,
                              uint64_t max_per_region, uint8_t* was_unknown, uint8_t* first_issuer_hour, cudaStream_t s);
-cudaError_t launch_meta(const DeviceState& st, const uint8_t* blob, const uint64_t* offsets, const ctmr_key* keys, uint64_t m,
-                        const uint8_t* was_unknown, const uint32_t* name_off, const uint32_t* name_len, const uint32_t* crl_off,
-                        const uint32_t* crl_len, uint32_t* meta_slots /* [2*m] scratch */, uint8_t* first_dn, uint8_t* first_crl,
-                        cudaStream_t s);
 cudaError_t launch_meta_insert(const DeviceState& st, const uint8_t* blob, const uint64_t* offsets, const ctmr_key* keys, uint64_t m,
                                const uint8_t* was_unknown, const uint32_t* name_off, const uint32_t* name_len, const uint32_t* crl_off,
-                               const uint32_t* crl_len, uint32_t* meta_slots, cudaStream_t s);
+                               const uint32_t* crl_len, uint32_t* meta_slots /* [2*m] scratch */, cudaStream_t s);
 cudaError_t launch_meta_resolve(const DeviceState& st, const ctmr_key* keys, uint64_t m, const uint32_t* meta_slots, uint8_t* first_dn,
                                 uint8_t* first_crl, cudaStream_t s);
 cudaError_t launch_evict_pairs(const DeviceState& st, int64_t now_sec, int sm_count, cudaStream_t s);

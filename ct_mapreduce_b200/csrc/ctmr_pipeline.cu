@@ -5,20 +5,12 @@
 // most `stage_entries` entries and runs, on the stream of the round's stage (three stages rotate, so H2D, kernels
 // and D2H of consecutive rounds overlap):
 //
-//     H2D slice -> K_map (DER walk + filter + SHA-256 + key routing: a key of a set this GPU owns goes straight into
-//                  its table, any other key is appended as a 64-byte record to the OWNER's inbox over NVLink)
-//     -- sync 1: every member's appends of this round have landed --
-//     owner passes: insert of the inbox records; K_resolve (was_unknown = "mine is the lowest index of the slot",
-//                  per-issuer counts, (issuer, hour) first-seen + cardinality) and K_pairs (first_issuer_hour) over
-//                  the own entries AND the inbox records, whose bits go to the owner's outbox
-//     -- sync 2: every owner's bits of this round are ready --
-//     pull of the bits of the entries routed away (contiguous peer reads) [-> string identities: insert, sync 3,
-//                  read-back] -> D2H of the requested outputs [-> PEM]
+//     H2D slice -> one round of the key exchange (run_round, ctmr_api.cu: K_map with key routing, sync 1, owner
+//                  passes, sync 2, pull [, string identities]) -> D2H of the requested outputs [-> PEM]
 //
-// sync = nothing on one GPU; CUDA events recorded on every member's stream and waited for by every member's stream
-// in a one-process group; a barrier kernel spinning on flags in peer memory between processes.  Rounds are ordered
-// by a per-member chain (resolve of round k waits for resolve of round k-1), which with sync 1 gives the invariant
-// the lowest-index-wins rule needs: when an entry is resolved, every entry with a lower global index has been inserted.
+// The stage index is the round's exchange parity and picks its barrier channels.  Rounds are ordered by a per-member
+// chain (the owner passes of round k wait for those of round k-1), which with sync 1 gives the invariant the
+// lowest-index-wins rule needs: when an entry is resolved, every entry with a lower global index has been inserted.
 #include <sched.h>
 
 #include <fstream>
@@ -118,6 +110,26 @@ int pem_chunk(ctmr_ctx* c, PemStage& ps, const uint8_t* blob, const uint64_t* of
     return CTMR_OK;
 }
 
+int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* out, uint64_t lo, cudaStream_t s) {
+#define D2H(field, per) \
+    if (out->field && d.field) CU(c, cudaMemcpyAsync(out->field + lo * (per), d.field, cnt * (per) * sizeof *d.field, cudaMemcpyDeviceToHost, s))
+    D2H(status, 1);
+    D2H(sha256, 32);
+    D2H(exp_hour, 1);
+    D2H(serial_off, 1);
+    D2H(serial_len, 1);
+    D2H(was_unknown, 1);
+    D2H(first_issuer_hour, 1);
+    D2H(issuer_name_off, 1);
+    D2H(issuer_name_len, 1);
+    D2H(crldp_off, 1);
+    D2H(crldp_len, 1);
+    D2H(first_issuer_dn, 1);
+    D2H(first_crldp, 1);
+#undef D2H
+    return CTMR_OK;
+}
+
 }  // namespace ctmr_host
 
 namespace {
@@ -185,17 +197,21 @@ int agree_rounds(ctmr_ctx* c, uint64_t mine, uint64_t* agreed) {
     return CTMR_OK;
 }
 
-int issue_map(ctmr_ctx* c, Stage& s, int sidx, const BatchArgs& a, const Slice& sl, const uint32_t* map_dev, bool want_meta) {
+// Upload of one member's slice to stage `sidx`, and the slice's description for run_round.  chain: the round follows
+// another, whose owner passes (and string identities) this round's must follow.
+int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Slice& sl, const uint32_t* map_dev, bool want_meta,
+                RoundMember& x) {
+    Stage& s = c->stages[sidx];
+    const uint64_t cnt = sl.hi - sl.lo, E = c->stage_entries;
     CU(c, cudaSetDevice(c->device));
-    const uint64_t cnt = sl.hi - sl.lo;
-    int rc = round_begin(c, sidx, s.stream);  // exchange parity = stage
-    if (rc) return rc;
+    x = RoundMember{};
+    x.c = c;
     if (cnt) {
         const uint64_t bytes = a.offsets[sl.hi] - a.offsets[sl.lo];
         if (bytes) CU(c, cudaMemcpyAsync(s.blob, a.blob + a.offsets[sl.lo], bytes, cudaMemcpyHostToDevice, s.stream));
         CU(c, cudaMemcpyAsync(s.offsets, a.offsets + sl.lo, (cnt + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s.stream));
         if (a.issuer_idx) CU(c, cudaMemcpyAsync(s.issuer_idx, a.issuer_idx + sl.lo, cnt * sizeof(uint32_t), cudaMemcpyHostToDevice, s.stream));
-        ctmr_dev_batch db{};
+        ctmr_dev_batch& db = x.db;
         db.blob = s.blob - a.offsets[sl.lo];  // offsets stay absolute
         db.blob_bytes = a.offsets[sl.hi];
         db.offsets = s.offsets;
@@ -205,83 +221,57 @@ int issue_map(ctmr_ctx* c, Stage& s, int sidx, const BatchArgs& a, const Slice& 
         db.issuer_map_len = a.n_issuers;
         db.first_index = sl.first_index;
         db.now_unix_ns = a.now_unix_ns;
-        ctmr_dev_out dout{};
-        dout.status = s.status;
-        dout.sha256 = a.out->sha256 ? s.sha : nullptr;
-        dout.exp_hour = s.exp_hour;
-        dout.serial_off = s.serial_off;
-        dout.serial_len = s.serial_len;
-        dout.keys = s.keys;
-        const uint64_t E = c->stage_entries;
-        if (want_meta) {
-            dout.issuer_name_off = s.spans;
-            dout.issuer_name_len = s.spans + E;
-            dout.crldp_off = s.spans + 2 * E;
-            dout.crldp_len = s.spans + 3 * E;
-        }
-        rc = map_slice(c, &db, &dout, s.slot_of, sidx, s.order, s.len_hist, s.stream);
-        if (rc) return rc;
     }
-    rc = round_publish(c, sidx, s.stream);  // how many records this rank left in each owner's inbox
-    if (rc) return rc;
-    CU(c, cudaEventRecord(s.mapped, s.stream));
-    return CTMR_OK;
-}
-
-// the owner's work of a round: the records other ranks left in its inbox and its own entries' keys
-int issue_owner_insert(ctmr_ctx* c, Stage& s, int sidx) {
-    return round_owner_insert(c, sidx, c->stage_entries, s.stream);
-}
-
-int issue_resolve(ctmr_ctx* c, Stage& s, int sidx, const Slice& sl) {
-    int rc = round_resolve(c, sidx, c->stage_entries, s.keys, sl.hi - sl.lo, s.slot_of, s.pair_slot, s.was_unknown, s.first, s.stream);
-    if (rc) return rc;
-    CU(c, cudaEventRecord(s.reduced, s.stream));
-    return CTMR_OK;
-}
-
-// string identities of the new certificates: insert (needs this rank's was_unknown bits, i.e. the pull), then -- after
-// every rank's inserts -- the read-back
-int issue_meta_insert(ctmr_ctx* c, Stage& s, const BatchArgs& a, const Slice& sl) {
-    const uint64_t cnt = sl.hi - sl.lo, E = c->stage_entries;
-    if (cnt)
-        CU(c, launch_meta_insert(c->st, s.blob - a.offsets[sl.lo], s.offsets, s.keys, cnt, s.was_unknown, s.spans, s.spans + E,
-                                 s.spans + 2 * E, s.spans + 3 * E, s.meta_slots, s.stream));
-    CU(c, cudaEventRecord(s.meta_done, s.stream));
-    return CTMR_OK;
-}
-
-int issue_finish(ctmr_ctx* c, Stage& s, const BatchArgs& a, const Slice& sl, bool want_meta, bool want_pem, uint64_t* pem_base) {
-    const uint64_t cnt = sl.hi - sl.lo, lo = sl.lo, E = c->stage_entries;
-    const ctmr_out* out = a.out;
-    if (!cnt) return CTMR_OK;
+    ctmr_dev_out& dout = x.dout;
+    dout.status = s.status;
+    dout.sha256 = a.out->sha256 ? s.sha : nullptr;
+    dout.exp_hour = s.exp_hour;
+    dout.serial_off = s.serial_off;
+    dout.serial_len = s.serial_len;
+    dout.was_unknown = s.was_unknown;
+    dout.first_issuer_hour = s.first;
+    dout.keys = s.keys;
     if (want_meta) {
-        CU(c, launch_meta_resolve(c->st, s.keys, cnt, s.meta_slots, s.first_meta, s.first_meta + E, s.stream));
-        if (out->issuer_name_off) CU(c, cudaMemcpyAsync(out->issuer_name_off + lo, s.spans, cnt * 4, cudaMemcpyDeviceToHost, s.stream));
-        if (out->issuer_name_len) CU(c, cudaMemcpyAsync(out->issuer_name_len + lo, s.spans + E, cnt * 4, cudaMemcpyDeviceToHost, s.stream));
-        if (out->crldp_off) CU(c, cudaMemcpyAsync(out->crldp_off + lo, s.spans + 2 * E, cnt * 4, cudaMemcpyDeviceToHost, s.stream));
-        if (out->crldp_len) CU(c, cudaMemcpyAsync(out->crldp_len + lo, s.spans + 3 * E, cnt * 4, cudaMemcpyDeviceToHost, s.stream));
-        if (out->first_issuer_dn) CU(c, cudaMemcpyAsync(out->first_issuer_dn + lo, s.first_meta, cnt, cudaMemcpyDeviceToHost, s.stream));
-        if (out->first_crldp) CU(c, cudaMemcpyAsync(out->first_crldp + lo, s.first_meta + E, cnt, cudaMemcpyDeviceToHost, s.stream));
+        dout.issuer_name_off = s.spans;
+        dout.issuer_name_len = s.spans + E;
+        dout.crldp_off = s.spans + 2 * E;
+        dout.crldp_len = s.spans + 3 * E;
+        dout.first_issuer_dn = s.first_meta;
+        dout.first_crldp = s.first_meta + E;
     }
-    if (out->status) CU(c, cudaMemcpyAsync(out->status + lo, s.status, cnt, cudaMemcpyDeviceToHost, s.stream));
-    if (out->sha256) CU(c, cudaMemcpyAsync(out->sha256 + lo * 32, s.sha, cnt * 32, cudaMemcpyDeviceToHost, s.stream));
-    if (out->exp_hour) CU(c, cudaMemcpyAsync(out->exp_hour + lo, s.exp_hour, cnt * sizeof(int64_t), cudaMemcpyDeviceToHost, s.stream));
-    if (out->serial_off) CU(c, cudaMemcpyAsync(out->serial_off + lo, s.serial_off, cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-    if (out->serial_len) CU(c, cudaMemcpyAsync(out->serial_len + lo, s.serial_len, cnt * sizeof(uint32_t), cudaMemcpyDeviceToHost, s.stream));
-    if (out->was_unknown) CU(c, cudaMemcpyAsync(out->was_unknown + lo, s.was_unknown, cnt, cudaMemcpyDeviceToHost, s.stream));
-    if (out->first_issuer_hour) CU(c, cudaMemcpyAsync(out->first_issuer_hour + lo, s.first, cnt, cudaMemcpyDeviceToHost, s.stream));
-    if (want_pem) {  // StoreCertificatePEM's argument for this slice's new certificates (the host waits for this slice here)
-        int rc = pem_ensure(c, s.pem, c->stage_entries, c->stage_bytes);
-        if (rc) return rc;
-        rc = pem_chunk(c, s.pem, s.blob - a.offsets[lo], s.offsets, nullptr, s.was_unknown, cnt, out, lo, pem_base, s.stream);
-        if (rc) return rc;
+    x.slot_of = s.slot_of; x.pair_slot = s.pair_slot; x.order = s.order; x.len_hist = s.len_hist; x.meta_slots = s.meta_slots;
+    x.map_stream = x.reduce_stream = s.stream;
+    x.mapped = s.mapped; x.reduced = s.reduced; x.meta_done = s.meta_done;
+    if (chain) {
+        const Stage& prev = c->stages[(sidx + kStages - 1) % kStages];
+        x.prev_reduced = prev.reduced;
+        x.prev_meta_done = prev.meta_done;
     }
+    x.ch_map = CH_STAGE_MAP + sidx;
+    x.ch_resolve = CH_STAGE_RESOLVE + sidx;
+    x.ch_meta = CH_STAGE_META + sidx;
     return CTMR_OK;
+}
+
+// the requested outputs of one member's slice in stage `sidx` to the caller's buffers [, PEM]
+int stage_out(const RoundMember& x, int sidx, const BatchArgs& a, const Slice& sl, bool want_pem, uint64_t* pem_base) {
+    ctmr_ctx* c = x.c;
+    Stage& s = c->stages[sidx];
+    const uint64_t cnt = sl.hi - sl.lo;
+    if (!cnt) return CTMR_OK;
+    CU(c, cudaSetDevice(c->device));
+    int rc = copy_out(c, x.dout, cnt, a.out, sl.lo, s.stream);
+    if (rc || !want_pem) return rc;
+    // StoreCertificatePEM's argument for this slice's new certificates (the host waits for this slice here)
+    rc = pem_ensure(c, s.pem, c->stage_entries, c->stage_bytes);
+    if (rc) return rc;
+    return pem_chunk(c, s.pem, x.db.blob, x.db.offsets, nullptr, x.dout.was_unknown, cnt, a.out, sl.lo, pem_base, s.stream);
 }
 
 // The pipeline.  m[0..W) = the member GPUs this process drives (W == 1: a plain ctx, or one rank of a multi-process
 // group).  `plan` rows beyond a rank's own rounds are empty slices (multi-process: every rank runs the agreed number).
+// Each round: every member's upload on its stage's stream, run_round (exchange parity and barrier channels = stage,
+// chained to the previous stage), then the outputs in member order, so that PEM texts are appended in entry order.
 int run_rounds(ctmr_ctx** m, uint32_t W, const BatchArgs& a, const std::vector<std::vector<Slice>>& plan,
                const std::vector<const uint32_t*>& map_dev, ctmr_ctx** failed) {
     const ctmr_out* out = a.out;
@@ -297,48 +287,13 @@ int run_rounds(ctmr_ctx** m, uint32_t W, const BatchArgs& a, const std::vector<s
             return rc;              \
         }                           \
     } while (0)
+    RoundMember rm[kMaxWorld];
     for (size_t k = 0; k < plan.size(); ++k) {
         const int sidx = (int)(k % kStages);
-        for (uint32_t r = 0; r < W; ++r)  // ---- upload + map + insert at the owners
-            RR(r, issue_map(m[r], m[r]->stages[sidx], sidx, a, plan[k][r], map_dev[r], want_meta));
-        for (uint32_t r = 0; r < W; ++r) {  // ---- sync 1 (every member's appends have landed), then the owners' passes
-            ctmr_ctx* c = m[r];
-            Stage& s = c->stages[sidx];
-            *failed = c;
-            CU(c, cudaSetDevice(c->device));
-            for (uint32_t q = 0; q < W; ++q)
-                if (q != r) CU(c, cudaStreamWaitEvent(s.stream, m[q]->stages[sidx].mapped, 0));
-            RR(r, peer_barrier(c, CH_STAGE_MAP + sidx, s.stream));
-            RR(r, issue_owner_insert(c, s, sidx));
-            if (k > 0) CU(c, cudaStreamWaitEvent(s.stream, c->stages[(k - 1) % kStages].reduced, 0));  // the chain of rounds
-            RR(r, issue_resolve(c, s, sidx, plan[k][r]));
-        }
-        for (uint32_t r = 0; r < W; ++r) {  // ---- sync 2 (the owners have the bits ready), pull, [string identities]
-            ctmr_ctx* c = m[r];
-            Stage& s = c->stages[sidx];
-            *failed = c;
-            CU(c, cudaSetDevice(c->device));
-            for (uint32_t q = 0; q < W; ++q)
-                if (q != r) CU(c, cudaStreamWaitEvent(s.stream, m[q]->stages[sidx].reduced, 0));
-            RR(r, peer_barrier(c, CH_STAGE_RESOLVE + sidx, s.stream));
-            RR(r, round_pull(c, sidx, c->stage_entries, s.was_unknown, s.first, s.stream));
-            if (want_meta) {
-                if (k > 0) CU(c, cudaStreamWaitEvent(s.stream, c->stages[(k - 1) % kStages].meta_done, 0));  // their own chain of rounds
-                RR(r, issue_meta_insert(c, s, a, plan[k][r]));
-            }
-        }
-        for (uint32_t r = 0; r < W; ++r) {  // ---- [sync 3: every member's string identities are in], outputs
-            ctmr_ctx* c = m[r];
-            Stage& s = c->stages[sidx];
-            *failed = c;
-            CU(c, cudaSetDevice(c->device));
-            if (want_meta) {
-                for (uint32_t q = 0; q < W; ++q)
-                    if (q != r) CU(c, cudaStreamWaitEvent(s.stream, m[q]->stages[sidx].meta_done, 0));
-                RR(r, peer_barrier(c, CH_STAGE_META + sidx, s.stream));
-            }
-            RR(r, issue_finish(c, s, a, plan[k][r], want_meta, want_pem, &pem_base));
-        }
+        for (uint32_t r = 0; r < W; ++r) RR(r, stage_slice(m[r], sidx, k > 0, a, plan[k][r], map_dev[r], want_meta, rm[r]));
+        rc = run_round(rm, W, sidx, m[0]->stage_entries, want_meta, failed);
+        if (rc) return rc;
+        for (uint32_t r = 0; r < W; ++r) RR(r, stage_out(rm[r], sidx, a, plan[k][r], want_pem, &pem_base));
     }
 #undef RR
     for (uint32_t r = 0; r < W; ++r) {

@@ -257,14 +257,7 @@ __global__ void __launch_bounds__(256) meta_resolve_kernel(DeviceState st, const
 
 static inline unsigned blocks_for(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
-cudaError_t launch_meta(const DeviceState& st, const uint8_t* blob, const uint64_t* offsets, const ctmr_key* keys, uint64_t m,
-                        const uint8_t* was_unknown, const uint32_t* name_off, const uint32_t* name_len, const uint32_t* crl_off,
-                        const uint32_t* crl_len, uint32_t* meta_slots, uint8_t* first_dn, uint8_t* first_crl, cudaStream_t s) {
-    if (!m) return cudaSuccess;
-    cudaError_t e = launch_meta_insert(st, blob, offsets, keys, m, was_unknown, name_off, name_len, crl_off, crl_len, meta_slots, s);
-    return e != cudaSuccess ? e : launch_meta_resolve(st, keys, m, meta_slots, first_dn, first_crl, s);
-}
-// the two halves separately: in a group a barrier separates every rank's inserts from the read-back
+// string identities in two halves: in a group a sync separates every rank's inserts from the read-back
 cudaError_t launch_meta_insert(const DeviceState& st, const uint8_t* blob, const uint64_t* offsets, const ctmr_key* keys, uint64_t m,
                                const uint8_t* was_unknown, const uint32_t* name_off, const uint32_t* name_len, const uint32_t* crl_off,
                                const uint32_t* crl_len, uint32_t* meta_slots, cudaStream_t s) {

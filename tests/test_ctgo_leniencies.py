@@ -15,36 +15,24 @@ the wild; the synthetic corpus and the reference's three fixtures contain none.
 import numpy as np
 import pytest
 
+import der_build as D
 from conftest import NOW_NS, pack
+from der_build import tlv
 
 ST_OK, ST_PARSE_ERR, ST_FILTER_CA, ST_FILTER_EXPIRED, ST_FILTER_CN = 0, 1, 2, 3, 4
 
 
-def tlv(tag, body):
-    n = len(body)
-    if n < 128:
-        return bytes([tag, n]) + body
-    if n < 256:
-        return bytes([tag, 0x81, n]) + body
-    return bytes([tag, 0x82, n >> 8, n & 0xFF]) + body
-
-
-ALG = bytes.fromhex("300d06092a864886f70d01010b0500")
-RSA_ALG = bytes.fromhex("300d06092a864886f70d0101010500")
-GOOD_KEY = tlv(0x30, tlv(0x02, b"\x00\xc1" + b"\x11" * 15) + tlv(0x02, b"\x01\x00\x01"))
+ALG = D.SHA256_RSA
+RSA_ALG = D.RSA_ENC
+GOOD_KEY = D.RSA_KEY_BITS[1:]
 
 
 def name(cn_tag=0x0C, cn=b"ca"):
-    return tlv(0x30, tlv(0x31, tlv(0x30, bytes.fromhex("0603550403") + tlv(cn_tag, cn))))
+    return [[D.cn(cn, cn_tag)]]
 
 
 def cert(issuer=None, serial=b"\x01", key=GOOD_KEY, extensions=None):
-    issuer = issuer if issuer is not None else name()
-    spki = tlv(0x30, RSA_ALG + tlv(0x03, b"\x00" + key))
-    ext = tlv(0xA3, tlv(0x30, b"".join(extensions))) if extensions else b""
-    tbs = tlv(0x30, bytes.fromhex("a003020102") + tlv(0x02, serial) + ALG + issuer +
-              tlv(0x30, tlv(0x17, b"900101000000Z") + tlv(0x17, b"300615123045Z")) + name() + spki + ext)
-    return tlv(0x30, tbs + ALG + tlv(0x03, b"\x00" + b"\x5a" * 16))
+    return D.cert(issuer=issuer, serial=serial, subject=name(), spki_bits=b"\x00" + key, extensions=extensions).der
 
 
 def extension(oid_hex, value, critical=False):

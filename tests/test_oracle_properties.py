@@ -11,6 +11,7 @@ import hashlib
 import numpy as np
 from hypothesis import given, settings, strategies as st
 
+import der_build as D
 from conftest import pack
 
 
@@ -39,18 +40,7 @@ def test_exp_hour_and_ids_match_datetime(ora, sec):
 
 def _cert_with_times(nb: bytes, na: bytes, nb_tag=0x17, na_tag=0x17, serial: bytes = b"\x01") -> bytes:
     """A minimal certificate skeleton (no extensions) with the given validity encodings and serial content octets."""
-    def tlv(tag, body):
-        n = len(body)
-        if n < 128:
-            return bytes([tag, n]) + body
-        if n < 256:
-            return bytes([tag, 0x81, n]) + body
-        return bytes([tag, 0x82, n >> 8, n & 0xFF]) + body
-    name = tlv(0x30, tlv(0x31, tlv(0x30, bytes.fromhex("0603550403") + tlv(0x0C, b"ca"))))
-    alg = bytes.fromhex("300d06092a864886f70d01010b0500")
-    spki = tlv(0x30, bytes.fromhex("300d06092a864886f70d0101010500") + tlv(0x03, b"\x00" + tlv(0x30, tlv(0x02, b"\x00\xc1" + b"\x11" * 15) + tlv(0x02, b"\x01\x00\x01"))))
-    tbs = tlv(0x30, bytes.fromhex("a003020102") + tlv(0x02, serial) + alg + name + tlv(0x30, tlv(nb_tag, nb) + tlv(na_tag, na)) + name + spki)
-    return tlv(0x30, tbs + alg + tlv(0x03, b"\x00" + b"\x5a" * 16))
+    return D.cert(serial=serial, subject=[[D.cn(b"ca")]], not_before=D.tlv(nb_tag, nb), not_after=D.tlv(na_tag, na)).der
 
 
 def _fmt_utc(t: datetime.datetime) -> bytes:

@@ -854,11 +854,11 @@ int ctmr_register_issuers(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offs
                 return fail(c, CTMR_E_TOO_MANY_ISSUERS, "more distinct issuers than config.max_issuers");
             }
             if (ok[i]) c->issuer_by_digest.emplace(std::string(reinterpret_cast<const char*>(dig.data() + 32 * i), 32), idx[i]);
-            c->issuer_by_der.emplace(ders[fresh[i]], idx[i]);
-            if (c->fe) {
+            if (c->fe) {  // first the mirror: a DER it has no room for must not count as registered (a retry fails the same way)
                 int rc2 = fe_add_issuer(c, ders[fresh[i]], idx[i]);
                 if (rc2) return rc2;
             }
+            c->issuer_by_der.emplace(ders[fresh[i]], idx[i]);
         }
         for (uint32_t k = 0; k < n; ++k)
             if (dense_out[k] == CTMR_ISSUER_NONE) dense_out[k] = c->issuer_by_der[ders[k]];

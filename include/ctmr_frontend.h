@@ -79,7 +79,13 @@ typedef struct ctmr_raw_out {
 } ctmr_raw_out;
 
 /* Decode + frame + identify issuers + map + reduce.  Synchronous.  Entries take the global indices
- * following those of earlier ctmr_process_batch / ctmr_process_raw calls on this ctx. */
+ * following those of earlier ctmr_process_batch / ctmr_process_raw calls on this ctx.
+ *
+ * Chain[0] is identified on the GPU through a per-ctx mirror keyed by the certificate's bytes: it holds
+ * 2 x config.max_issuers distinct Chain[0] DERs.  Every distinct DER takes a slot, also a reissue of a
+ * known key and a DER that does not parse (which resolves to CTMR_ISSUER_BAD), so the mirror can fill
+ * before the issuer registry does.  A batch that meets one DER more fails with CTMR_E_TOO_MANY_ISSUERS;
+ * the DERs already held keep resolving in later calls. */
 int ctmr_process_raw(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_out* out);
 
 /* The same on every GPU of a group (ctmr_group_create, ctmr.h): each round takes one chunk per GPU out of ONE contiguous

@@ -32,7 +32,10 @@ EXPORTS = [
     "ctmr_process_device", "ctmr_read_histogram_device",
     "ctmr_check_device", "ctmr_reset_device", "ctmr_profile_last", "ctmr_preload_known", "ctmr_snapshot_size",
     "ctmr_snapshot_save", "ctmr_snapshot_load", "ctmr_evict_expired", "ctmr_sha256_ceiling_device", "ctmr_synth_offsets_device", "ctmr_synth_write_device", "ctmr_synth_truth_device", "ctmr_synth_issuers_host", "ctmr_synth_raw_pages_host",
+    "ctmr_synth_tiles_host",
     "ctmr_process_raw", "ctmr_group_process_raw", "ctmr_frontend_profile_last",  # include/ctmr_frontend.h
+    "ctmr_process_tiles", "ctmr_group_process_tiles", "ctmr_register_chain_certs", "ctmr_group_register_chain_certs",
+    "ctmr_tiles_profile_last",
     # several GPUs: one process (group) / one process per GPU (peer)
     "ctmr_group_create", "ctmr_group_destroy", "ctmr_group_last_error", "ctmr_group_size", "ctmr_group_member",
     "ctmr_group_process_batch", "ctmr_group_issuer_counts", "ctmr_group_set_cardinality", "ctmr_group_status_counters",
@@ -48,6 +51,9 @@ PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment overrid
 def peer_rounds() -> int:
     return int(load().ctmr_peer_rounds())
 E_PAIR_TABLE_FULL, E_META_TABLE_FULL, E_PEER_TIMEOUT, E_PEER = -8, -9, -10, -11
+E_UNKNOWN_ISSUER = -12
+# per-entry outcome of the front end (include/ctmr_frontend.h CTMR_FE_*)
+FE_OK, FE_BAD_BASE64, FE_BAD_LEAF, FE_UNKNOWN_TYPE, FE_BAD_EXTRA, FE_BAD_CERT, FE_BAD_TILE, FE_BAD_INDEX = range(8)
 
 
 class Config(C.Structure):
@@ -91,6 +97,20 @@ class RawOut(C.Structure):
     """ctmr_raw_out (include/ctmr_frontend.h)."""
     _fields_ = [("path", Out)] + [(n, C.c_void_p) for n in
                                   ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_src", "leaf_off", "leaf_len")]
+
+
+class TileBatch(C.Structure):
+    """ctmr_tile_batch (include/ctmr_frontend.h)."""
+    _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_uint64), ("tile_off", C.c_void_p), ("tile_len", C.c_void_p),
+                ("tile_index", C.c_void_p), ("tile_width", C.c_void_p), ("n_tiles", C.c_uint64), ("now_unix_ns", C.c_int64)]
+
+
+class TileOut(C.Structure):
+    """ctmr_tile_out (include/ctmr_frontend.h)."""
+    _fields_ = [("path", Out)] + [(n, C.c_void_p) for n in
+                                  ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_index", "leaf_off", "leaf_len",
+                                   "leaf_hash", "tile_status", "missing_fp")] + \
+               [("missing_cap", C.c_uint32), ("tiles_done", C.c_uint64), ("n_missing", C.c_uint32)]
 
 
 class SynthCfg(C.Structure):
@@ -168,6 +188,13 @@ def load():
     L.ctmr_process_raw.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut)]
     L.ctmr_group_process_raw.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut)]
     L.ctmr_frontend_profile_last.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(u64)]
+    L.ctmr_process_tiles.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut)]
+    L.ctmr_group_process_tiles.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut)]
+    L.ctmr_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
+    L.ctmr_tiles_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
+    L.ctmr_group_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
+    L.ctmr_synth_tiles_host.argtypes = [C.POINTER(SynthCfg), u64, u64, vp, vp, u64, vp, vp]
+    L.ctmr_synth_tiles_host.restype = u64
     L.ctmr_group_create.argtypes = [C.POINTER(Config), vp, u32, C.POINTER(vp)]
     L.ctmr_group_destroy.argtypes = [vp]
     L.ctmr_group_destroy.restype = None

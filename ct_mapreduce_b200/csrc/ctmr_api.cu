@@ -428,6 +428,7 @@ void fe_destroy(ctmr_ctx* c) {
     cudaFree(f->serial_len); cudaFree(f->spans); cudaFree(f->slots_dev); cudaFree(f->arena); cudaFree(f->pending);
     cudaFree(f->unknown_list); cudaFree(f->unknown_count);
     pem_free(f->pem);
+    tiles_free(f);
     if (f->ev0) cudaEventDestroy(f->ev0);
     if (f->ev1) cudaEventDestroy(f->ev1);
     if (f->ev2) cudaEventDestroy(f->ev2);
@@ -494,7 +495,7 @@ int fe_clear_issuers(ctmr_ctx* c) {
     f->arena_used = 0;
     CU(c, cudaMemsetAsync(f->slots_dev, 0, (f->slot_mask + 1) * sizeof(IssuerCertSlot), c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    return CTMR_OK;
+    return tiles_clear_fingerprints(c);  // the tiles' fingerprint table follows the mirror
 }
 
 int ensure_frontend(ctmr_ctx* c) {
@@ -1361,7 +1362,7 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
 }
 
 int ctmr_frontend_profile_last(ctmr_ctx* c, float* frontend_ms, float* path_ms, uint64_t* frontend_launches) {
-    if (!c || !c->fe) return fail(c, CTMR_E_INVALID, "no ctmr_process_raw call to report");
+    if (!c || !c->fe) return fail(c, CTMR_E_INVALID, "no ctmr_process_raw / ctmr_process_tiles call to report");
     if (frontend_ms) *frontend_ms = c->fe->fe_ms;
     if (path_ms) *path_ms = c->fe->path_ms;
     if (frontend_launches) *frontend_launches = c->fe->launches;

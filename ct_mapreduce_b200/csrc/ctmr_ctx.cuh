@@ -79,6 +79,24 @@ struct FeStage {
     std::vector<uint8_t> pack;  // host staging of the slow path (strings scattered over more than one chunk of text)
 };
 
+// static-ct-api tiles (ctmr_process_tiles): per-chunk buffers beyond the front end's, and the fingerprint table.
+// Allocated on the first tile call or chain-certificate registration.
+struct TileState {
+    TileDesc *tiles[2] = {}, *h_tiles[2] = {};  // per upload stage: the chunk's tiles, device and pinned host
+    uint8_t* tile_bad = nullptr;
+    uint64_t *entry_off = nullptr, *leaf_index = nullptr, *leaf_data_off = nullptr;
+    uint32_t *entry_tile = nullptr, *te_len = nullptr;
+    unsigned int* first_stop = nullptr;
+    uint8_t* leaf_hash = nullptr;
+    cudaEvent_t ev_split0 = nullptr, ev_split1 = nullptr;  // around tile_split: the serial walk is timed on its own
+    float split_ms = 0.f;
+    // fingerprint -> dense issuer index: device table, host copy, host memo keyed by the 32 bytes
+    FpSlot* fp_dev = nullptr;
+    std::vector<FpSlot> fp_host;
+    uint64_t fp_mask = 0, fp_used = 0;
+    std::unordered_map<std::string, uint32_t> fp_memo;
+};
+
 // CT wire-format front end (include/ctmr_frontend.h): device buffers of one chunk + the device mirror of
 // the issuer registry keyed by certificate bytes
 struct FrontEnd {
@@ -113,6 +131,7 @@ struct FrontEnd {
     float fe_ms = 0.f, path_ms = 0.f;
     uint64_t launches = 0;
     PemStage pem;
+    TileState* tl = nullptr;   // tiles_ensure
 };
 
 }  // namespace ctmr_host
@@ -266,6 +285,9 @@ int snap_shard_save(ctmr_ctx* c, uint8_t* p);
 int snap_shard_load(ctmr_ctx* c, const uint8_t* p);
 int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n);
 int frontend_ensure(ctmr_ctx* c);   // allocates the front end's buffers on first use (ctmr_api.cu)
+int tiles_ensure(ctmr_ctx* c);      // ... and the tile buffers + fingerprint table (ctmr_frontend_api.cu), after frontend_ensure
+void tiles_free(FrontEnd* f);
+int tiles_clear_fingerprints(ctmr_ctx* c);
 int ensure_scratch(ctmr_ctx* c, uint64_t n);
 uint64_t device_round_entries(uint64_t n, uint32_t rounds);   // E of a ctmr_process_device call cut into `rounds` rounds
 uint32_t peer_rounds();   // rounds of the collective ctmr_process_device (CTMR_PEER_ROUNDS, env override for experiments)

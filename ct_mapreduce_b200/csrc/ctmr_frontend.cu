@@ -328,6 +328,11 @@ cudaError_t launch_fe_decode(const FeParams& p, void* scan_temp, size_t scan_tem
 cudaError_t launch_fe_frame(const FeParams& p, cudaStream_t s) {
     if (p.n == 0) return cudaSuccess;
     fe_frame_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, s>>>(p);
+    return launch_fe_tbs(p, s);
+}
+
+cudaError_t launch_fe_tbs(const FeParams& p, cudaStream_t s) {
+    if (p.n == 0) return cudaSuccess;
     fe_tbs_kernel<<<(unsigned)((p.n + 127) / 128), 128, 0, s>>>(p);
     return cudaGetLastError();
 }

@@ -1,6 +1,7 @@
 // ctmr_frontend_api.cu -- the entry points of include/ctmr_frontend.h: get-entries strings -> base64 decode -> TLS framing ->
 // Chain[0] identification -> the path (SURVEY.md §8(f)-2), on one GPU (ctmr_process_raw) and on a group of GPUs driven by
-// one process (ctmr_group_process_raw).
+// one process (ctmr_group_process_raw); static-ct-api data tiles -> split -> framing -> Chain[0] by fingerprint -> the path
+// (ctmr_process_tiles, ctmr_group_process_tiles, ctmr_register_chain_certs).
 //
 // A call is cut into CHUNKS (entry and character budgets of the front end's buffers).  Per chunk:
 //   upload   the chunk's characters and string spans, on a copy stream, into one of two upload stages -- chunk k+1's
@@ -97,15 +98,37 @@ int fe_upload(ctmr_ctx* c, const ctmr_raw_batch* b, RawChunk& ch) {
     return CTMR_OK;
 }
 
+// where the path writes a chunk's results: the front end's per-chunk buffers (sha256 and string identities when asked for)
+ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
+    const uint64_t E = f->cap_entries;
+    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
+    ctmr_dev_out dout{};
+    dout.status = f->status;
+    dout.sha256 = po->sha256 ? f->sha : nullptr;
+    dout.exp_hour = f->exp_hour;
+    dout.serial_off = f->serial_off;
+    dout.serial_len = f->serial_len;
+    dout.was_unknown = f->was_unknown;
+    dout.first_issuer_hour = f->first;
+    if (want_meta) {
+        dout.issuer_name_off = f->spans;
+        dout.issuer_name_len = f->spans + E;
+        dout.crldp_off = f->spans + 2 * E;
+        dout.crldp_len = f->spans + 3 * E;
+        dout.first_issuer_dn = f->first_meta;
+        dout.first_crldp = f->first_meta + E;
+    }
+    return dout;
+}
+
 // decode + frame + Chain[0] -> dense index of an uploaded chunk; leaves ch.db / ch.dout describing the device-resident batch
 int fe_front(ctmr_ctx* c, const ctmr_raw_batch* b, const ctmr_raw_out* out, RawChunk& ch, uint64_t first_index) {
     FrontEnd* f = c->fe;
     cudaStream_t s = c->stream;
     CU(c, cudaSetDevice(c->device));
     FeStage& st = f->stage[ch.stage];
-    const uint64_t cnt = ch.hi - ch.lo, E = f->cap_entries;
+    const uint64_t cnt = ch.hi - ch.lo;
     const ctmr_out* po = &out->path;
-    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
     CU(c, cudaStreamWaitEvent(s, st.uploaded, 0));
     FeParams& p = ch.p;
     p = FeParams{};
@@ -179,22 +202,7 @@ int fe_front(ctmr_ctx* c, const ctmr_raw_batch* b, const ctmr_raw_out* out, RawC
     db.issuer_idx = f->issuer_idx;
     db.first_index = first_index;
     db.now_unix_ns = b->now_unix_ns;
-    ctmr_dev_out& dout = ch.dout;
-    dout.status = f->status;
-    dout.sha256 = po->sha256 ? f->sha : nullptr;
-    dout.exp_hour = f->exp_hour;
-    dout.serial_off = f->serial_off;
-    dout.serial_len = f->serial_len;
-    dout.was_unknown = f->was_unknown;
-    dout.first_issuer_hour = f->first;
-    if (want_meta) {
-        dout.issuer_name_off = f->spans;
-        dout.issuer_name_len = f->spans + E;
-        dout.crldp_off = f->spans + 2 * E;
-        dout.crldp_len = f->spans + 3 * E;
-        dout.first_issuer_dn = f->first_meta;
-        dout.first_crldp = f->first_meta + E;
-    }
+    ch.dout = chunk_path_out(f, po);
     return CTMR_OK;
 }
 
@@ -306,16 +314,16 @@ void for_each_member(uint32_t W, std::vector<int>& rcs, F fn) {
 }
 
 // A member's device-resident chunk as its part of round `parity` (run_round).  Everything runs on the member's stream,
-// so there is no chain: fe_back waits for each round before the next is issued.
-int fe_member(ctmr_ctx* c, const RawChunk& ch, int parity, RoundMember& x) {
+// so there is no chain: the back half waits for each round before the next is issued.
+int fe_member(ctmr_ctx* c, const ctmr_dev_batch& db, const ctmr_dev_out& dout, int parity, RoundMember& x) {
     CU(c, cudaSetDevice(c->device));
-    int rc = ensure_scratch(c, std::max<uint64_t>(ch.db.n, 1));
-    if (rc == CTMR_OK) rc = ensure_order(c, ch.db.n);
+    int rc = ensure_scratch(c, std::max<uint64_t>(db.n, 1));
+    if (rc == CTMR_OK) rc = ensure_order(c, db.n);
     if (rc) return rc;
     x = RoundMember{};
     x.c = c;
-    x.db = ch.db;
-    x.dout = ch.dout;
+    x.db = db;
+    x.dout = dout;
     x.dout.keys = c->keys_scratch;
     x.slot_of = c->slot_scratch; x.pair_slot = c->pair_scratch; x.order = c->order_scratch; x.len_hist = c->len_hist;
     x.meta_slots = c->meta_scratch;
@@ -328,18 +336,22 @@ int fe_member(ctmr_ctx* c, const RawChunk& ch, int parity, RoundMember& x) {
     return CTMR_OK;
 }
 
-// cut the next round out of the batch: one chunk per member from ONE contiguous window starting at `pos`
-int plan_round(ctmr_group* g, const ctmr_raw_batch* b, uint64_t pos, int stage, std::vector<RawChunk>& ch, ctmr_ctx** failed) {
+// Cut the next round out of a batch of `total` units (entries, or tiles) starting at `pos`: one chunk per member from ONE
+// contiguous window, q units each, q halved until every member's chunk fits (fit(c, lo, want, &hi) says how far a
+// chunk starting at lo gets), then each chunk's upload is issued (upload(c, chunk)).
+template <class Chunk, class Fit, class Upload>
+int plan_round(ctmr_group* g, uint64_t total, uint64_t q_max, uint64_t pos, int stage, std::vector<Chunk>& ch, ctmr_ctx** failed,
+               const char* too_large, Fit fit, Upload upload) {
     const uint32_t W = (uint32_t)g->m.size();
     ctmr_ctx* c0 = g->m[0];
     *failed = c0;
-    uint64_t q = std::min<uint64_t>(c0->fe->cap_entries, (b->n - pos + W - 1) / W);
+    uint64_t q = std::max<uint64_t>(1, std::min<uint64_t>(q_max, (total - pos + W - 1) / W));
     for (;;) {
         bool fits = true;
         for (uint32_t r = 0; r < W && fits; ++r) {
-            const uint64_t lo = std::min(b->n, pos + r * q), want = std::min(b->n, pos + (r + 1) * q);
+            const uint64_t lo = std::min(total, pos + r * q), want = std::min(total, pos + (r + 1) * q);
             uint64_t hi = 0;
-            int rc = fe_fit(g->m[r], b, lo, want - lo, &hi);
+            int rc = fit(g->m[r], lo, want - lo, &hi);
             if (rc) {
                 *failed = g->m[r];
                 return rc;
@@ -347,20 +359,27 @@ int plan_round(ctmr_group* g, const ctmr_raw_batch* b, uint64_t pos, int stage, 
             fits = hi == want;
         }
         if (fits) break;
-        if (q == 1) return fail(c0, CTMR_E_BATCH_TOO_LARGE, "a single entry exceeds the front end's character budget");
+        if (q == 1) return fail(c0, CTMR_E_BATCH_TOO_LARGE, too_large);
         q = (q + 1) / 2;
     }
-    ch.assign(W, RawChunk{});
+    ch.assign(W, Chunk{});
     for (uint32_t r = 0; r < W; ++r) {
-        ch[r].lo = std::min(b->n, pos + r * q);
-        ch[r].hi = std::min(b->n, pos + (r + 1) * q);
+        ch[r].lo = std::min(total, pos + r * q);
+        ch[r].hi = std::min(total, pos + (r + 1) * q);
         ch[r].stage = stage;
         *failed = g->m[r];
-        int rc = fe_upload(g->m[r], b, ch[r]);
+        int rc = upload(g->m[r], ch[r]);
         if (rc) return rc;
     }
     *failed = nullptr;
     return CTMR_OK;
+}
+
+int plan_raw_round(ctmr_group* g, const ctmr_raw_batch* b, uint64_t pos, int stage, std::vector<RawChunk>& ch, ctmr_ctx** failed) {
+    return plan_round(
+        g, b->n, g->m[0]->fe->cap_entries, pos, stage, ch, failed, "a single entry exceeds the front end's character budget",
+        [b](ctmr_ctx* c, uint64_t lo, uint64_t want, uint64_t* hi) { return fe_fit(c, b, lo, want, hi); },
+        [b](ctmr_ctx* c, RawChunk& x) { return fe_upload(c, b, x); });
 }
 
 int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_ctx** failed) {
@@ -383,12 +402,12 @@ int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out,
     const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
     uint64_t pem_base = 0, pos = 0;
     std::vector<RawChunk> cur, nxt;
-    rc = plan_round(g, b, 0, 0, cur, failed);
+    rc = plan_raw_round(g, b, 0, 0, cur, failed);
     if (rc) return rc;
     for (int k = 0;; ++k) {
         const uint64_t end = cur[W - 1].hi;
         if (end < b->n) {  // the next round's uploads overlap this round's kernels and host round trips
-            rc = plan_round(g, b, end, (k + 1) & 1, nxt, failed);
+            rc = plan_raw_round(g, b, end, (k + 1) & 1, nxt, failed);
             if (rc) return rc;
         }
         // The front halves wait on the host (issuer identification round trips, the arena size): one thread per member, so
@@ -405,7 +424,7 @@ int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out,
         RoundMember rm[kMaxWorld];
         for (uint32_t r = 0; r < W; ++r) {
             *failed = g->m[r];
-            rc = fe_member(g->m[r], cur[r], parity, rm[r]);
+            rc = fe_member(g->m[r], cur[r].db, cur[r].dout, parity, rm[r]);
             if (rc) return rc;
         }
         rc = run_round(rm, W, parity, c0->fe->cap_entries, want_meta, failed);
@@ -436,6 +455,461 @@ int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out,
         if (rc) return rc;
     }
     *failed = nullptr;
+    return CTMR_OK;
+}
+
+// ================================================================================================================
+// static-ct-api data tiles (ctmr_process_tiles).  The same chunk / upload / front / path / back structure as above, with
+// chunks cut on tile boundaries.  The uploaded tile bytes ARE the path's input: K_map reads the leaves where the upload
+// put them, so the stage stays busy until the chunk's back half has run.
+// ================================================================================================================
+struct TileChunk {
+    uint64_t lo = 0, hi = 0;      // tiles of the caller's batch
+    uint64_t e0 = 0, e1 = 0;      // their entries
+    uint64_t bytes = 0;           // tile bytes uploaded
+    int stage = 0;
+    TileParams p{};
+    ctmr_dev_batch db{};
+    ctmr_dev_out dout{};
+    bool stopped = false;         // holds the first tile with an unknown Chain[0] fingerprint; [lo, hi) cut before it
+    std::vector<std::array<uint8_t, 32>> missing;  // that tile's unknown fingerprints, sorted
+};
+
+// entries before each tile: ent[t] = sum of widths of tiles [0, t); validates widths and spans
+int tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, std::vector<uint64_t>& ent) {
+    if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (b->n_tiles && (!b->data || !b->tile_off || !b->tile_len || !b->tile_index || !b->tile_width))
+        return fail(c, CTMR_E_INVALID, "null batch buffers");
+    if ((out->path.pem != nullptr) != (out->path.pem_off != nullptr)) return fail(c, CTMR_E_INVALID, "pem and pem_off go together");
+    if (out->missing_cap && !out->missing_fp) return fail(c, CTMR_E_INVALID, "missing_cap without missing_fp");
+    ent.assign(b->n_tiles + 1, 0);
+    for (uint64_t t = 0; t < b->n_tiles; ++t) {
+        if (b->tile_width[t] < 1 || b->tile_width[t] > 256) return fail(c, CTMR_E_INVALID, "tile width outside 1..256");
+        if (b->tile_off[t] > b->data_bytes || b->tile_len[t] > b->data_bytes - b->tile_off[t])
+            return fail(c, CTMR_E_INVALID, "tile outside the data buffer");
+        ent[t + 1] = ent[t] + b->tile_width[t];
+    }
+    return CTMR_OK;
+}
+
+// How many tiles starting at `lo` fit one chunk (at most max_tiles): the entry budget and half the byte budget
+int tile_fit(ctmr_ctx* c, const ctmr_tile_batch* b, const std::vector<uint64_t>& ent, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) {
+    FrontEnd* f = c->fe;
+    uint64_t hi = lo, bytes = 0;
+    while (hi < b->n_tiles && hi - lo < max_tiles && ent[hi + 1] - ent[lo] <= f->cap_entries && bytes + b->tile_len[hi] <= f->cap_text / 2) {
+        bytes += b->tile_len[hi];
+        ++hi;
+    }
+    *hi_out = hi;
+    return CTMR_OK;
+}
+
+// tiles [lo, hi) into upload stage ch.stage, asynchronously on the copy stream
+int tile_upload(ctmr_ctx* c, const ctmr_tile_batch* b, const std::vector<uint64_t>& ent, TileChunk& ch) {
+    FrontEnd* f = c->fe;
+    TileState* tl = f->tl;
+    FeStage& st = f->stage[ch.stage];
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaStreamWaitEvent(f->copy_stream, st.consumed, 0));  // the chunk that last used this stage is done with it
+    ch.e0 = ent[ch.lo];
+    ch.e1 = ent[ch.hi];
+    const uint64_t cnt = ch.hi - ch.lo;
+    TileDesc* h = tl->h_tiles[ch.stage];
+    uint64_t bytes = 0, min_off = ~0ull, max_end = 0;
+    for (uint64_t t = ch.lo; t < ch.hi; ++t) {
+        bytes += b->tile_len[t];
+        min_off = std::min(min_off, b->tile_off[t]);
+        max_end = std::max(max_end, b->tile_off[t] + b->tile_len[t]);
+    }
+    const bool one_copy = cnt && max_end - min_off <= f->cap_text;  // tiles back to back in the caller's buffer
+    uint64_t w = 0;
+    if (!one_copy) st.pack.resize(bytes);
+    for (uint64_t i = 0; i < cnt; ++i) {
+        const uint64_t t = ch.lo + i;
+        TileDesc& d = h[i];
+        d.data_off = b->tile_off[t];
+        d.index = b->tile_index[t];
+        d.len = b->tile_len[t];
+        d.first = (uint32_t)(ent[t] - ch.e0);
+        d.width = b->tile_width[t];
+        d.pad = 0;
+        if (one_copy) {
+            d.staged_off = b->tile_off[t] - min_off;
+        } else {
+            d.staged_off = w;
+            std::memcpy(st.pack.data() + w, b->data + b->tile_off[t], d.len);
+            w += d.len;
+        }
+    }
+    ch.bytes = one_copy ? max_end - min_off : w;
+    if (ch.bytes)
+        CU(c, cudaMemcpyAsync(st.text + 16, one_copy ? b->data + min_off : st.pack.data(), ch.bytes, cudaMemcpyHostToDevice, f->copy_stream));
+    if (cnt) CU(c, cudaMemcpyAsync(tl->tiles[ch.stage], h, cnt * sizeof(TileDesc), cudaMemcpyHostToDevice, f->copy_stream));
+    CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
+    return CTMR_OK;
+}
+
+// split + frame + fingerprint -> dense index of an uploaded chunk.  A chunk holding a tile with an unknown Chain[0]
+// fingerprint is cut before that tile (ch.stopped, ch.missing).  Leaves ch.db / ch.dout describing the device-resident batch.
+int tile_front(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, TileChunk& ch) {
+    FrontEnd* f = c->fe;
+    TileState* tl = f->tl;
+    cudaStream_t s = c->stream;
+    CU(c, cudaSetDevice(c->device));
+    FeStage& st = f->stage[ch.stage];
+    CU(c, cudaStreamWaitEvent(s, st.uploaded, 0));
+    TileParams& p = ch.p;
+    p = TileParams{};
+    p.data = st.text + 16;
+    p.tiles = tl->tiles[ch.stage];
+    p.n_tiles = (uint32_t)(ch.hi - ch.lo);
+    p.n = ch.e1 - ch.e0;
+    p.tile_bad = tl->tile_bad; p.entry_off = tl->entry_off; p.entry_tile = tl->entry_tile; p.te_len = tl->te_len;
+    p.leaf_index = tl->leaf_index; p.leaf_data_off = tl->leaf_data_off; p.first_stop = tl->first_stop; p.leaf_hash = tl->leaf_hash;
+    FeParams& q = p.fe;
+    q.n = p.n;
+    q.decoded = st.text + 16;
+    q.entry_status = f->entry_status; q.entry_type = f->entry_type; q.timestamp = f->timestamp; q.leaf_len_out = f->leaf_len_out;
+    q.leaf_abs = f->leaf_abs; q.chain_abs = f->chain_abs; q.chain_len = f->chain_len; q.tbs_abs = f->tbs_abs; q.tbs_len = f->tbs_len;
+    q.issuer_idx = f->issuer_idx;
+    ch.db = ctmr_dev_batch{};
+    ch.dout = ctmr_dev_out{};
+    ch.stopped = false;
+    ch.missing.clear();
+    CU(c, cudaEventRecord(f->ev0, s));
+    if (p.n) {
+        unsigned int stop = ~0u;
+        CU(c, cudaMemsetAsync(tl->first_stop, 0xFF, 4, s));
+        CU(c, cudaEventRecord(tl->ev_split0, s));
+        CU(c, launch_tile_split(p, s));
+        CU(c, cudaEventRecord(tl->ev_split1, s));
+        CU(c, launch_tile_frame(p, s));
+        CU(c, launch_tile_issuer(p, FpTable{tl->fp_dev, tl->fp_mask}, s));
+        f->launches += 4;  // split, frame, tbs, issuer
+        if (out->leaf_hash) {
+            CU(c, launch_tile_leaf_hash(p, s));
+            ++f->launches;
+        }
+        CU(c, cudaMemcpyAsync(&stop, tl->first_stop, 4, cudaMemcpyDeviceToHost, s));
+        CU(c, cudaStreamSynchronize(s));
+        float split = 0.f;
+        CU(c, cudaEventElapsedTime(&split, tl->ev_split0, tl->ev_split1));
+        tl->split_ms += split;
+        if (stop != ~0u) {  // nothing is resolved on a guess: tiles from `stop` on wait for the host to register their issuers
+            const TileDesc& td = tl->h_tiles[ch.stage][stop];
+            std::vector<uint32_t> idx(td.width);
+            std::vector<uint64_t> at(td.width);
+            CU(c, cudaMemcpyAsync(idx.data(), f->issuer_idx + td.first, td.width * 4ull, cudaMemcpyDeviceToHost, s));
+            CU(c, cudaMemcpyAsync(at.data(), f->chain_abs + td.first, td.width * 8ull, cudaMemcpyDeviceToHost, s));
+            CU(c, cudaStreamSynchronize(s));
+            for (uint32_t j = 0; j < td.width; ++j) {
+                if (idx[j] != CTMR_ISSUER_UNRESOLVED) continue;
+                std::array<uint8_t, 32> fp;
+                std::memcpy(fp.data(), b->data + td.data_off + (at[j] - td.staged_off), 32);  // the host's own copy of the tile
+                ch.missing.push_back(fp);
+            }
+            std::sort(ch.missing.begin(), ch.missing.end());
+            ch.missing.erase(std::unique(ch.missing.begin(), ch.missing.end()), ch.missing.end());
+            ch.stopped = true;
+            ch.hi = ch.lo + stop;
+            ch.e1 = ch.e0 + td.first;
+            p.n_tiles = stop;
+            p.n = q.n = td.first;
+        }
+    }
+    CU(c, cudaEventRecord(f->ev1, s));
+    ctmr_dev_batch& db = ch.db;
+    db.blob = p.data;
+    db.blob_bytes = ch.bytes;
+    db.offsets = f->leaf_abs;
+    db.lens = f->leaf_len_out;
+    db.n = p.n;
+    db.issuer_idx = f->issuer_idx;
+    db.now_unix_ns = b->now_unix_ns;
+    ch.dout = chunk_path_out(f, &out->path);
+    return CTMR_OK;
+}
+
+// after the path: x509 leaf failures, PEM, outputs to the host; waits for the chunk and releases its stage
+int tile_back(ctmr_ctx* c, const ctmr_tile_out* out, TileChunk& ch, uint64_t* pem_base) {
+    FrontEnd* f = c->fe;
+    TileState* tl = f->tl;
+    cudaStream_t s = c->stream;
+    CU(c, cudaSetDevice(c->device));
+    FeStage& st = f->stage[ch.stage];
+    const uint64_t cnt = ch.e1 - ch.e0, lo = ch.e0, nt = ch.hi - ch.lo;
+    const ctmr_out* po = &out->path;
+    if (cnt) {
+        CU(c, launch_fe_finish(ch.p.fe, f->status, s));
+        ++f->launches;
+    }
+    CU(c, cudaEventRecord(f->ev2, s));
+    if (cnt && po->pem) {
+        int rc = pem_ensure(c, f->pem, f->cap_entries, f->cap_decoded);
+        if (rc) return rc;
+        rc = pem_chunk(c, f->pem, ch.p.data, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, lo, pem_base, s);
+        if (rc) return rc;
+    }
+    CU(c, cudaEventRecord(st.consumed, s));  // the leaves in the stage have been read for the last time
+    std::vector<uint8_t> bad(nt);
+    if (cnt) {
+        const int rc = copy_out(c, ch.dout, cnt, po, lo, s);
+        if (rc) return rc;
+#define TL_D2H(dst, src, per) \
+    if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * (per), (src), cnt * (per), cudaMemcpyDeviceToHost, s))
+        TL_D2H(out->entry_status, f->entry_status, 1);
+        TL_D2H(out->entry_type, f->entry_type, 1);
+        TL_D2H(out->timestamp_ms, f->timestamp, 8);
+        TL_D2H(out->issuer, f->issuer_idx, 4);
+        TL_D2H(out->leaf_index, tl->leaf_index, 8);
+        TL_D2H(out->leaf_off, tl->leaf_data_off, 8);
+        TL_D2H(out->leaf_len, f->leaf_len_out, 4);
+        TL_D2H(out->leaf_hash, tl->leaf_hash, 32);
+#undef TL_D2H
+        if (out->tile_status) CU(c, cudaMemcpyAsync(bad.data(), tl->tile_bad, nt, cudaMemcpyDeviceToHost, s));
+    }
+    CU(c, cudaStreamSynchronize(s));
+    if (out->tile_status)
+        for (uint64_t i = 0; i < nt; ++i) out->tile_status[ch.lo + i] = bad[i] ? CTMR_FE_BAD_TILE : CTMR_FE_OK;
+    float a = 0.f, d = 0.f;
+    CU(c, cudaEventElapsedTime(&a, f->ev0, f->ev1));
+    CU(c, cudaEventElapsedTime(&d, f->ev1, f->ev2));
+    f->fe_ms += a;
+    f->path_ms += d;
+    return CTMR_OK;
+}
+
+// the stop: tiles_done, the unknown fingerprints, and the call's result code
+int tile_stop(ctmr_ctx* c, ctmr_tile_out* out, const TileChunk& ch) {
+    out->tiles_done = ch.hi;
+    out->n_missing = (uint32_t)std::min<size_t>(ch.missing.size(), out->missing_cap);
+    for (uint32_t i = 0; i < out->n_missing; ++i) std::memcpy(out->missing_fp + 32ull * i, ch.missing[i].data(), 32);
+    return fail(c, CTMR_E_UNKNOWN_ISSUER, "tile " + std::to_string(ch.hi) + " names a Chain[0] fingerprint that is not registered "
+                                          "(ctmr_register_chain_certs, then call again from tiles_done)");
+}
+
+int tiles_prepare(ctmr_ctx* c) {
+    CU(c, cudaSetDevice(c->device));
+    int rc = frontend_ensure(c);
+    if (rc == CTMR_OK) rc = tiles_ensure(c);
+    if (rc) return rc;
+    c->fe->fe_ms = c->fe->path_ms = c->fe->tl->split_ms = 0.f;
+    c->fe->launches = 0;
+    return CTMR_OK;
+}
+
+// *done_entries: entries that took their indices (all of them unless the call stops or fails)
+int process_tiles_single(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries) {
+    std::vector<uint64_t> ent;
+    int rc = tile_args(c, b, out, ent);
+    if (rc) return rc;
+    const uint64_t n = ent[b->n_tiles];
+    *done_entries = n;
+    out->tiles_done = 0;
+    out->n_missing = 0;
+    if (b->n_tiles == 0) return CTMR_OK;
+    rc = tiles_prepare(c);
+    if (rc) return rc;
+    uint64_t pem_base = 0;
+    TileChunk ch[2];
+    const char* too_large = "a single tile exceeds the front end's staging budget";
+    rc = tile_fit(c, b, ent, 0, ~0ull, &ch[0].hi);
+    if (rc) return rc;
+    if (ch[0].hi == 0) return fail(c, CTMR_E_BATCH_TOO_LARGE, too_large);
+    rc = tile_upload(c, b, ent, ch[0]);
+    if (rc) return rc;
+    for (int k = 0;; ++k) {
+        TileChunk& cur = ch[k & 1];
+        if (cur.hi < b->n_tiles) {  // next chunk's upload overlaps this chunk's kernels
+            TileChunk& nx = ch[(k + 1) & 1];
+            nx = TileChunk{};
+            nx.lo = cur.hi;
+            nx.stage = (k + 1) & 1;
+            rc = tile_fit(c, b, ent, nx.lo, ~0ull, &nx.hi);
+            if (rc) return rc;
+            if (nx.hi == nx.lo) return fail(c, CTMR_E_BATCH_TOO_LARGE, too_large);
+            rc = tile_upload(c, b, ent, nx);
+            if (rc) return rc;
+        }
+        rc = tile_front(c, b, out, cur);
+        if (rc) return rc;
+        cur.db.first_index = c->next_index + cur.e0;
+        if (cur.db.n) {
+            rc = ctmr_process_device(c, &cur.db, &cur.dout, c->stream);
+            if (rc) return rc;
+        }
+        rc = tile_back(c, out, cur, &pem_base);
+        if (rc) return rc;
+        out->tiles_done = cur.hi;
+        if (cur.stopped) {
+            *done_entries = cur.e1;
+            if (out->path.pem) out->path.pem_off[cur.e1] = pem_base;
+            rc = ctmr_check_device(c, nullptr);  // a table that filled up during the completed tiles is this call's error
+            return rc ? rc : tile_stop(c, out, cur);
+        }
+        if (cur.hi >= b->n_tiles) break;
+    }
+    if (out->path.pem) out->path.pem_off[n] = pem_base;
+    return ctmr_check_device(c, nullptr);
+}
+
+int process_tiles_group(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries, ctmr_ctx** failed) {
+    const uint32_t W = (uint32_t)g->m.size();
+    ctmr_ctx* c0 = g->m[0];
+    *failed = c0;
+    std::vector<uint64_t> ent;
+    int rc = tile_args(c0, b, out, ent);
+    if (rc) return rc;
+    const uint64_t n = ent[b->n_tiles];
+    *done_entries = n;
+    out->tiles_done = 0;
+    out->n_missing = 0;
+    if (b->n_tiles == 0) return CTMR_OK;
+    for (uint32_t r = 0; r < W; ++r) {
+        *failed = g->m[r];
+        rc = tiles_prepare(g->m[r]);
+        if (rc) return rc;
+    }
+    auto plan = [&](uint64_t pos, int stage, std::vector<TileChunk>& ch) {
+        return plan_round(
+            g, b->n_tiles, ~0ull, pos, stage, ch, failed, "a single tile exceeds the front end's staging budget",
+            [&](ctmr_ctx* c, uint64_t lo, uint64_t want, uint64_t* hi) { return tile_fit(c, b, ent, lo, want, hi); },
+            [&](ctmr_ctx* c, TileChunk& x) { return tile_upload(c, b, ent, x); });
+    };
+    const ctmr_out* po = &out->path;
+    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
+    uint64_t pem_base = 0;
+    std::vector<TileChunk> cur, nxt;
+    rc = plan(0, 0, cur);
+    if (rc) return rc;
+    for (int k = 0;; ++k) {
+        const uint64_t end = cur[W - 1].hi;
+        if (end < b->n_tiles) {  // the next round's uploads overlap this round's kernels
+            rc = plan(end, (k + 1) & 1, nxt);
+            if (rc) return rc;
+        }
+        std::vector<int> rcs;
+        for_each_member(W, rcs, [&](uint32_t r) { return tile_front(g->m[r], b, out, cur[r]); });
+        for (uint32_t r = 0; r < W; ++r)
+            if (rcs[r]) {
+                *failed = g->m[r];
+                return rcs[r];
+            }
+        // a stop in member r: the later members' chunks run empty (their entries must not touch the tables)
+        uint32_t stop = W;
+        for (uint32_t r = 0; r < W && stop == W; ++r)
+            if (cur[r].stopped) stop = r;
+        for (uint32_t r = stop + 1; r < W; ++r) {
+            TileChunk& x = cur[r];
+            x.hi = x.lo;
+            x.e1 = x.e0;
+            x.p.n_tiles = 0;
+            x.p.n = x.p.fe.n = x.db.n = 0;
+        }
+        const int parity = k % (int)kParities;
+        RoundMember rm[kMaxWorld];
+        for (uint32_t r = 0; r < W; ++r) {
+            *failed = g->m[r];
+            cur[r].db.first_index = g->next_index + cur[r].e0;
+            rc = fe_member(g->m[r], cur[r].db, cur[r].dout, parity, rm[r]);
+            if (rc) return rc;
+        }
+        rc = run_round(rm, W, parity, c0->fe->cap_entries, want_meta, failed);
+        if (rc) return rc;
+        for (uint32_t r = 0; r < W; ++r) {  // in entry order: PEM texts are appended in that order
+            *failed = g->m[r];
+            rc = tile_back(g->m[r], out, cur[r], &pem_base);
+            if (rc) return rc;
+        }
+        if (stop < W) {
+            *done_entries = cur[stop].e1;
+            if (out->path.pem) out->path.pem_off[cur[stop].e1] = pem_base;
+            for (uint32_t r = 0; r < W; ++r) {  // a table that filled up during the completed tiles is this call's error
+                *failed = g->m[r];
+                rc = ctmr_check_device(g->m[r], nullptr);
+                if (rc) return rc;
+            }
+            *failed = g->m[stop];
+            return tile_stop(g->m[stop], out, cur[stop]);
+        }
+        out->tiles_done = end;
+        if (end >= b->n_tiles) break;
+        cur.swap(nxt);
+    }
+    if (out->path.pem) out->path.pem_off[n] = pem_base;
+    for (uint32_t r = 0; r < W; ++r) {
+        *failed = g->m[r];
+        rc = ctmr_check_device(g->m[r], nullptr);
+        if (rc) return rc;
+    }
+    *failed = nullptr;
+    return CTMR_OK;
+}
+
+// Fingerprints of chain certificates on the GPU, then: a fingerprint table slot for each new one (capacity first, so a
+// certificate the table cannot take is never registered), the registry (ctmr_register_issuers), the slots written.
+int register_chain_certs(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint32_t* dense_out, uint8_t* fp_out) {
+    if (n && (!blob || !offsets || !dense_out)) return fail(c, CTMR_E_INVALID, "bad argument");
+    CU(c, cudaSetDevice(c->device));
+    int rc = frontend_ensure(c);
+    if (rc == CTMR_OK) rc = tiles_ensure(c);
+    if (rc || n == 0) return rc;
+    TileState* tl = c->fe->tl;
+    for (uint32_t k = 0; k < n; ++k)
+        if (offsets[k + 1] < offsets[k]) return fail(c, CTMR_E_INVALID, "chain certificate offsets not monotonic");
+    const uint64_t base = offsets[0], bytes = offsets[n] - base;
+    std::vector<uint64_t> rel(n + 1);
+    for (uint32_t k = 0; k <= n; ++k) rel[k] = offsets[k] - base;
+    std::vector<uint8_t> fps(32ull * n);
+    uint8_t *d_blob = nullptr, *d_fp = nullptr;
+    uint64_t* d_off = nullptr;
+    auto release = [&]() { cudaFree(d_blob); cudaFree(d_off); cudaFree(d_fp); };
+    cudaError_t e = cudaMalloc(&d_blob, bytes + 64);
+    if (e == cudaSuccess) e = cudaMalloc(&d_off, (n + 1) * 8ull);
+    if (e == cudaSuccess) e = cudaMalloc(&d_fp, 32ull * n);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blob, blob + base, bytes, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, rel.data(), (n + 1) * 8ull, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = launch_fingerprints(d_blob, d_off, n, d_fp, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(fps.data(), d_fp, 32ull * n, cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    release();
+    if (e != cudaSuccess) return fail(c, CTMR_E_CUDA, std::string("chain certificate fingerprints: ") + cudaGetErrorString(e));
+    if (fp_out) std::memcpy(fp_out, fps.data(), fps.size());
+    std::vector<uint32_t> fresh;  // first position of each fingerprint the table does not hold yet
+    std::unordered_map<std::string, uint32_t> seen;
+    for (uint32_t k = 0; k < n; ++k) {
+        std::string key(reinterpret_cast<const char*>(fps.data() + 32ull * k), 32);
+        if (!tl->fp_memo.count(key) && seen.emplace(key, k).second) fresh.push_back(k);
+    }
+    if (fresh.empty()) {
+        for (uint32_t k = 0; k < n; ++k) dense_out[k] = tl->fp_memo[std::string(reinterpret_cast<const char*>(fps.data() + 32ull * k), 32)];
+        return CTMR_OK;
+    }
+    if (tl->fp_used + fresh.size() > 2ull * c->st.max_issuers)
+        return fail(c, CTMR_E_TOO_MANY_ISSUERS, "more chain certificate fingerprints than the table holds (raise config.max_issuers)");
+    std::vector<uint8_t> packed;
+    std::vector<uint64_t> poff(1, 0);
+    for (uint32_t k : fresh) {
+        packed.insert(packed.end(), blob + offsets[k], blob + offsets[k + 1]);
+        poff.push_back(packed.size());
+    }
+    std::vector<uint32_t> dense(fresh.size());
+    rc = ctmr_register_issuers(c, packed.data(), poff.data(), (uint32_t)fresh.size(), dense.data());
+    if (rc) return rc;
+    for (size_t i = 0; i < fresh.size(); ++i) {
+        FpSlot sl{};
+        std::memcpy(sl.w, fps.data() + 32ull * fresh[i], 32);
+        sl.idx = dense[i];
+        sl.used = 1;
+        uint64_t slot = ((((uint64_t)sl.w[1]) << 32) | sl.w[0]) & tl->fp_mask;
+        while (tl->fp_host[slot].used) slot = (slot + 1) & tl->fp_mask;
+        tl->fp_host[slot] = sl;
+        ++tl->fp_used;
+        tl->fp_memo.emplace(std::string(reinterpret_cast<const char*>(sl.w), 32), sl.idx);
+        CU(c, cudaMemcpyAsync(tl->fp_dev + slot, &tl->fp_host[slot], sizeof sl, cudaMemcpyHostToDevice, c->stream));
+    }
+    CU(c, cudaStreamSynchronize(c->stream));
+    for (uint32_t k = 0; k < n; ++k) dense_out[k] = tl->fp_memo[std::string(reinterpret_cast<const char*>(fps.data() + 32ull * k), 32)];
     return CTMR_OK;
 }
 
@@ -483,4 +957,123 @@ int ctmr_group_process_raw(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out*
     return rc;
 }
 
+int ctmr_process_tiles(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_tiles");
+    uint64_t done = 0;
+    const int rc = process_tiles_single(c, b, out, &done);
+    c->next_index += done;  // after a stop only the completed tiles' entries; after a failure all of them
+    if (rc != CTMR_OK) drain_frontend(c);
+    return rc;
+}
+
+int ctmr_group_process_tiles(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    ctmr_ctx* failed = nullptr;
+    uint64_t done = 0;
+    int rc;
+    if (g->m.size() == 1) {  // a group of one is a plain ctx
+        ctmr_ctx* c = g->m[0];
+        c->next_index = g->next_index;
+        rc = process_tiles_single(c, b, out, &done);
+        failed = c;
+    } else {
+        rc = process_tiles_group(g, b, out, &done, &failed);
+    }
+    g->next_index += done;
+    if (rc != CTMR_OK) {
+        for (ctmr_ctx* c : g->m) drain_frontend(c);
+        if (failed) g->err = failed->err;
+    }
+    return rc;
+}
+
+int ctmr_tiles_profile_last(ctmr_ctx* c, float* split_ms) {
+    if (!c || !c->fe || !c->fe->tl) return fail(c, CTMR_E_INVALID, "no ctmr_process_tiles call to report");
+    if (split_ms) *split_ms = c->fe->tl->split_ms;
+    return CTMR_OK;
+}
+
+int ctmr_register_chain_certs(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint32_t* dense_out, uint8_t* fp_out) {
+    if (!c) return CTMR_E_INVALID;
+    return register_chain_certs(c, blob, offsets, n, dense_out, fp_out);
+}
+
+int ctmr_group_register_chain_certs(ctmr_group* g, const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint32_t* dense_out,
+                                    uint8_t* fp_out) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    for (ctmr_ctx* c : g->m) {  // every member's table, from the one registry: the same dense indices everywhere
+        const int rc = register_chain_certs(c, blob, offsets, n, dense_out, fp_out);
+        if (rc) {
+            g->err = c->err;
+            return rc;
+        }
+    }
+    return CTMR_OK;
+}
+
 }  // extern "C"
+
+namespace ctmr_host {
+
+int tiles_ensure(ctmr_ctx* c) {
+    FrontEnd* f = c->fe;
+    if (f->tl) return CTMR_OK;
+    TileState* tl = new (std::nothrow) TileState();
+    if (!tl) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    f->tl = tl;
+    const uint64_t E = f->cap_entries;
+    tl->fp_mask = pow2_at_least(4ull * c->st.max_issuers) - 1;
+    tl->fp_host.assign(tl->fp_mask + 1, FpSlot{});
+    cudaError_t e = cudaSuccess;
+    for (int k = 0; k < 2 && e == cudaSuccess; ++k) {
+        e = cudaMalloc(&tl->tiles[k], E * sizeof(TileDesc));
+        if (e == cudaSuccess) e = cudaMallocHost(&tl->h_tiles[k], E * sizeof(TileDesc));
+    }
+    if (e == cudaSuccess) e = cudaMalloc(&tl->tile_bad, E);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->entry_off, E * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->leaf_index, E * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->leaf_data_off, E * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->entry_tile, E * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->te_len, E * 4);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->first_stop, 16);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->leaf_hash, E * 32);
+    if (e == cudaSuccess) e = cudaMalloc(&tl->fp_dev, (tl->fp_mask + 1) * sizeof(FpSlot));
+    if (e == cudaSuccess) e = cudaEventCreate(&tl->ev_split0);
+    if (e == cudaSuccess) e = cudaEventCreate(&tl->ev_split1);
+    if (e == cudaSuccess) e = cudaMemsetAsync(tl->fp_dev, 0, (tl->fp_mask + 1) * sizeof(FpSlot), c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        tiles_free(f);
+        return fail(c, e == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA, std::string("tiles: ") + cudaGetErrorString(e));
+    }
+    return CTMR_OK;
+}
+
+void tiles_free(FrontEnd* f) {
+    TileState* tl = f->tl;
+    if (!tl) return;
+    for (int k = 0; k < 2; ++k) {
+        cudaFree(tl->tiles[k]);
+        cudaFreeHost(tl->h_tiles[k]);
+    }
+    cudaFree(tl->tile_bad); cudaFree(tl->entry_off); cudaFree(tl->leaf_index); cudaFree(tl->leaf_data_off);
+    cudaFree(tl->entry_tile); cudaFree(tl->te_len); cudaFree(tl->first_stop); cudaFree(tl->leaf_hash); cudaFree(tl->fp_dev);
+    if (tl->ev_split0) cudaEventDestroy(tl->ev_split0);
+    if (tl->ev_split1) cudaEventDestroy(tl->ev_split1);
+    delete tl;
+    f->tl = nullptr;
+}
+
+int tiles_clear_fingerprints(ctmr_ctx* c) {
+    TileState* tl = c->fe ? c->fe->tl : nullptr;
+    if (!tl) return CTMR_OK;
+    std::fill(tl->fp_host.begin(), tl->fp_host.end(), FpSlot{});
+    tl->fp_used = 0;
+    tl->fp_memo.clear();
+    CU(c, cudaMemsetAsync(tl->fp_dev, 0, (tl->fp_mask + 1) * sizeof(FpSlot), c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return CTMR_OK;
+}
+
+}  // namespace ctmr_host

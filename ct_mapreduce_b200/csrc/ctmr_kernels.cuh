@@ -273,6 +273,55 @@ cudaError_t launch_fe_decode(const FeParams& p, void* scan_temp, size_t scan_tem
 cudaError_t launch_fe_frame(const FeParams& p, cudaStream_t s);
 cudaError_t launch_fe_issuer(const FeParams& p, const IssuerCertTable& tab, uint64_t* pending, uint64_t pending_mask,
                              uint32_t* unknown_list, uint32_t unknown_cap, unsigned int* unknown_count, int sm_count, cudaStream_t s);
+cudaError_t launch_fe_tbs(const FeParams& p, cudaStream_t s);
 cudaError_t launch_fe_finish(const FeParams& p, const uint8_t* status, cudaStream_t s);
+
+// ---- static-ct-api data tiles (ctmr_tiles.cu, ctmr_process_tiles) ------------------------------------------------
+// one tile of a chunk as uploaded: where it sits in the staging buffer and in the caller's data
+struct TileDesc {
+    uint64_t staged_off;  // in TileParams.data
+    uint64_t data_off;    // in ctmr_tile_batch.data
+    uint64_t index;       // N of tile/data/<N>
+    uint32_t len;
+    uint32_t first;       // chunk-local index of the tile's first entry
+    uint32_t width;
+    uint32_t pad;
+};
+static_assert(sizeof(TileDesc) == 40, "TileDesc layout");
+
+// fingerprint -> dense issuer index (ctmr_register_chain_certs): open addressing on the fingerprint's first 8 bytes
+struct FpSlot {
+    uint32_t w[8];  // SHA-256 fingerprint, bytes in order
+    uint32_t idx;   // dense issuer index or CTMR_ISSUER_BAD
+    uint32_t used;
+    uint64_t pad;
+};
+static_assert(sizeof(FpSlot) == 48, "FpSlot layout");
+struct FpTable {
+    const FpSlot* slots;
+    uint64_t mask;
+};
+
+struct TileParams {
+    const uint8_t* data;       // staged tile bytes (16 bytes of slack before, 64 after)
+    const TileDesc* tiles;     // [n_tiles]
+    uint32_t n_tiles;
+    uint64_t n;                // entries = sum of widths
+    uint8_t* tile_bad;         // [n_tiles]
+    uint64_t* entry_off;       // [n] TileLeaf start in data
+    uint32_t* entry_tile;      // [n] chunk-local tile
+    uint32_t* te_len;          // [n] bytes of the TimestampedEntry
+    uint64_t* leaf_index;      // [n]
+    uint64_t* leaf_data_off;   // [n] the path's certificate, offset in the caller's data
+    unsigned int* first_stop;  // [1] lowest chunk-local tile holding an unknown Chain[0] fingerprint
+    uint8_t* leaf_hash;        // [n][32]
+    FeParams fe;               // per-entry outputs shared with the get-entries front end; fe.decoded = data
+};
+
+cudaError_t launch_tile_split(const TileParams& p, cudaStream_t s);
+cudaError_t launch_tile_frame(const TileParams& p, cudaStream_t s);
+cudaError_t launch_tile_issuer(const TileParams& p, const FpTable& tab, cudaStream_t s);
+cudaError_t launch_tile_leaf_hash(const TileParams& p, cudaStream_t s);
+cudaError_t launch_fingerprints(const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint8_t* fps, cudaStream_t s);
 
 }  // namespace ctmr

@@ -1,4 +1,5 @@
-// ctmr_synth_pages.cu -- HOST-side synthesis of RFC 6962 get-entries response bodies around the synthetic corpus
+// ctmr_synth_pages.cu -- HOST-side synthesis of RFC 6962 get-entries response bodies and of static-ct-api data tiles around
+// the synthetic corpus
 // (bench / test tooling for the CT wire-format front end; nothing here runs on the GPU or inside a timed region).
 // Byte-identical to tools/bench_frontend.py's Python construction (tests/test_frontend_oracle.py checks that), but
 // threaded and ~100x faster, so that a benchmark does not spend its GPU-box minutes building input.
@@ -94,36 +95,74 @@ struct Issuers {
     std::vector<std::array<uint8_t, 32>> key_hash;
 };
 
-// leaf_input / extra_data of synthetic entry i (the construction of tools/bench_frontend.py: every third entry a
-// precert_entry, chains of one or two certificates, timestamps 1 690 000 000 000 + i)
-void make_entry(const ctmr_synth_cfg* cfg, const Issuers& iss, uint64_t i, std::vector<uint8_t>& leaf, std::vector<uint8_t>& li,
-                std::vector<uint8_t>& ed) {
+// Synthetic entry i, the part both formats share (the construction of tools/bench_frontend.py: every third entry a
+// precert_entry, chains of one or two certificates, timestamps 1 690 000 000 000 + i): the leaf certificate, and the
+// TimestampedEntry up to its CtExtensions (timestamp, entry_type, ASN.1Cert or PreCert) in `te`.
+struct SynthEntry {
+    uint32_t chain[2];  // issuers of Chain[0] and Chain[1]
+    int n_chain;
+    bool precert;
+};
+
+SynthEntry synth_entry(const ctmr_synth_cfg* cfg, const Issuers& iss, uint64_t i, std::vector<uint8_t>& leaf, std::vector<uint8_t>& te) {
     ctmr_synth_plan pl;
     ctmr_synth_plan_make(cfg, i, &pl);
     leaf.resize(ctmr_synth_cert_len(cfg, i));
     ctmr_synth_cert_write(cfg, &pl, leaf.data());
-    const uint32_t k = pl.issuer, k2 = (k + 1) % cfg->n_issuers;
-    const int n_chain = 1 + (int)(i % 2);
-    std::vector<uint8_t> chain;
-    put_opaque24(chain, iss.der[k].data(), iss.der[k].size());
-    if (n_chain == 2) put_opaque24(chain, iss.der[k2].data(), iss.der[k2].size());
-    li.clear();
-    ed.clear();
-    li.push_back(0); li.push_back(0);  // v1, timestamped_entry
+    SynthEntry e{{pl.issuer, (pl.issuer + 1) % cfg->n_issuers}, 1 + (int)(i % 2), i % 3 == 0};
+    te.clear();
     const uint64_t ts = 1690000000000ull + i;
-    for (int b = 7; b >= 0; --b) li.push_back((uint8_t)(ts >> (8 * b)));
-    if (i % 3 == 0) {  // precert_entry: issuer_key_hash, TBSCertificate; extra_data = pre_certificate + chain
-        li.push_back(0); li.push_back(1);
-        li.insert(li.end(), iss.key_hash[k].begin(), iss.key_hash[k].end());
+    for (int b = 7; b >= 0; --b) te.push_back((uint8_t)(ts >> (8 * b)));
+    te.push_back(0); te.push_back(e.precert ? 1 : 0);
+    if (e.precert) {  // PreCert: issuer_key_hash, TBSCertificate
+        te.insert(te.end(), iss.key_hash[e.chain[0]].begin(), iss.key_hash[e.chain[0]].end());
         const uint8_t* tbs = leaf.data() + der_hdr(leaf.data());
-        put_opaque24(li, tbs, der_hdr(tbs) + der_len(tbs));
-        put_opaque24(ed, leaf.data(), leaf.size());
+        put_opaque24(te, tbs, der_hdr(tbs) + der_len(tbs));
     } else {
-        li.push_back(0); li.push_back(0);
-        put_opaque24(li, leaf.data(), leaf.size());
+        put_opaque24(te, leaf.data(), leaf.size());
     }
+    return e;
+}
+
+// leaf_input / extra_data of synthetic entry i as a get-entries entry: no CtExtensions, the chain as DERs
+void make_entry(const ctmr_synth_cfg* cfg, const Issuers& iss, uint64_t i, std::vector<uint8_t>& leaf, std::vector<uint8_t>& li,
+                std::vector<uint8_t>& ed) {
+    std::vector<uint8_t> te;
+    const SynthEntry e = synth_entry(cfg, iss, i, leaf, te);
+    std::vector<uint8_t> chain;
+    for (int m = 0; m < e.n_chain; ++m) put_opaque24(chain, iss.der[e.chain[m]].data(), iss.der[e.chain[m]].size());
+    li.assign({0, 0});  // v1, timestamped_entry
+    li.insert(li.end(), te.begin(), te.end());
     li.push_back(0); li.push_back(0);  // no CtExtensions
+    ed.clear();
+    if (e.precert) put_opaque24(ed, leaf.data(), leaf.size());  // PrecertChainEntry.pre_certificate
     put_opaque24(ed, chain.data(), chain.size());
+}
+
+// TileLeaf of synthetic entry i (static-ct-api data tiles): the same TimestampedEntry with a leaf_index extension, the
+// pre_certificate of a precert entry, and the chain as fingerprints
+void make_tile_leaf(const ctmr_synth_cfg* cfg, const Issuers& iss, const uint8_t* fps, uint64_t i, std::vector<uint8_t>& leaf,
+                    std::vector<uint8_t>& out) {
+    const SynthEntry e = synth_entry(cfg, iss, i, leaf, out);
+    const uint8_t ext[10] = {0, 8, 0, 0, 5, (uint8_t)(i >> 32), (uint8_t)(i >> 24), (uint8_t)(i >> 16), (uint8_t)(i >> 8), (uint8_t)i};
+    out.insert(out.end(), ext, ext + 10);  // CtExtensions: one leaf_index extension
+    if (e.precert) put_opaque24(out, leaf.data(), leaf.size());
+    out.push_back(0); out.push_back((uint8_t)(32 * e.n_chain));
+    for (int m = 0; m < e.n_chain; ++m) out.insert(out.end(), fps + 32ull * e.chain[m], fps + 32ull * e.chain[m] + 32);
+}
+
+Issuers make_issuers(const ctmr_synth_cfg* cfg) {
+    Issuers iss;
+    iss.der.resize(cfg->n_issuers);
+    iss.key_hash.resize(cfg->n_issuers);
+    for (uint32_t k = 0; k < cfg->n_issuers; ++k) {
+        ctmr_synth_issuer_plan ip;
+        ctmr_synth_issuer_plan_make(cfg, k, &ip);
+        iss.der[k].resize(ip.total);
+        ctmr_synth_issuer_write(cfg, &ip, iss.der[k].data());
+        Sha256::digest(iss.der[k].data(), iss.der[k].size(), iss.key_hash[k].data());
+    }
+    return iss;
 }
 
 }  // namespace
@@ -135,16 +174,7 @@ extern "C" {
 uint64_t ctmr_synth_raw_pages_host(const struct ctmr_synth_cfg* cfg, uint64_t first, uint64_t n, uint32_t page, uint8_t* text, uint64_t cap,
                                    uint64_t* leaf_off, uint32_t* leaf_len, uint64_t* extra_off, uint32_t* extra_len) {
     if (!cfg || page == 0) return 0;
-    Issuers iss;
-    iss.der.resize(cfg->n_issuers);
-    iss.key_hash.resize(cfg->n_issuers);
-    for (uint32_t k = 0; k < cfg->n_issuers; ++k) {
-        ctmr_synth_issuer_plan ip;
-        ctmr_synth_issuer_plan_make(cfg, k, &ip);
-        iss.der[k].resize(ip.total);
-        ctmr_synth_issuer_write(cfg, &ip, iss.der[k].data());
-        Sha256::digest(iss.der[k].data(), iss.der[k].size(), iss.key_hash[k].data());
-    }
+    const Issuers iss = make_issuers(cfg);
     static const char kOpen[] = "{\"entries\":[", kLeaf[] = "{\"leaf_input\":\"", kExtra[] = "\",\"extra_data\":\"", kEnd[] = "\"}", kClose[] = "]}";
     const uint64_t n_pages = (n + page - 1) / page;
     // pass 1 (threaded): per-page sizes; pass 2: write at the prefix offsets
@@ -188,6 +218,46 @@ uint64_t ctmr_synth_raw_pages_host(const struct ctmr_synth_cfg* cfg, uint64_t fi
             if (j + 1 < hi) *o++ = ',';
         }
         lit(kClose, sizeof kClose - 1);
+    });
+    return total;
+}
+
+/* static-ct-api data tiles first_tile .. first_tile + n_tiles - 1 of the same entries, back to back (ctmr.h) */
+uint64_t ctmr_synth_tiles_host(const struct ctmr_synth_cfg* cfg, uint64_t first_tile, uint64_t n_tiles, const uint8_t* issuer_fps,
+                               uint8_t* data, uint64_t cap, uint64_t* tile_off, uint32_t* tile_len) {
+    if (!cfg || !issuer_fps || n_tiles == 0) return 0;
+    const Issuers iss = make_issuers(cfg);
+    const unsigned T = std::max(1u, std::min(std::thread::hardware_concurrency(), 64u));
+    std::vector<uint64_t> off(n_tiles + 1, 0);
+    auto for_tiles = [&](auto&& fn) {
+        std::vector<std::thread> th;
+        for (unsigned t = 0; t < T; ++t)
+            th.emplace_back([&, t] {
+                std::vector<uint8_t> leaf, tl;
+                for (uint64_t x = t; x < n_tiles; x += T) fn(x, leaf, tl);
+            });
+        for (auto& x : th) x.join();
+    };
+    for_tiles([&](uint64_t x, std::vector<uint8_t>& leaf, std::vector<uint8_t>& tl) {
+        uint64_t bytes = 0;
+        for (uint64_t j = 0; j < 256; ++j) {
+            make_tile_leaf(cfg, iss, issuer_fps, 256 * (first_tile + x) + j, leaf, tl);
+            bytes += tl.size();
+        }
+        off[x + 1] = bytes;
+    });
+    for (uint64_t x = 0; x < n_tiles; ++x) off[x + 1] += off[x];
+    const uint64_t total = off[n_tiles];
+    if (!data || cap < total) return total;
+    for_tiles([&](uint64_t x, std::vector<uint8_t>& leaf, std::vector<uint8_t>& tl) {
+        uint8_t* o = data + off[x];
+        for (uint64_t j = 0; j < 256; ++j) {
+            make_tile_leaf(cfg, iss, issuer_fps, 256 * (first_tile + x) + j, leaf, tl);
+            std::memcpy(o, tl.data(), tl.size());
+            o += tl.size();
+        }
+        if (tile_off) tile_off[x] = off[x];
+        if (tile_len) tile_len[x] = (uint32_t)(off[x + 1] - off[x]);
     });
     return total;
 }

@@ -16,6 +16,7 @@ All arithmetic happens in the CUDA kernels; nothing here parses, hashes or de-du
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
 from dataclasses import dataclass
 
 import numpy as np
@@ -62,6 +63,12 @@ class KnownCertificatesView:
         return out.value
 
 
+def _pack(ders):
+    offsets = np.zeros(len(ders) + 1, np.uint64)
+    offsets[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
+    return np.frombuffer(b"".join(ders) or b"\0", np.uint8).copy(), offsets
+
+
 def _attach_pem(o: "capi.Out", res: BatchResult, n: int, der_bytes: int):
     """Room for the PEM of every certificate of the batch (the worst case: all new)."""
     res.pem = np.zeros(der_bytes // 3 * 4 + der_bytes // 48 + 64 * n + 256, np.uint8)
@@ -87,6 +94,20 @@ class RawBatchResult:
         self.leaf_src = np.zeros(n, np.uint8)
         self.leaf_off = np.zeros(n, np.uint32)
         self.leaf_len = np.zeros(n, np.uint32)
+
+
+class TileBatchResult(RawBatchResult):
+    """Outputs of ctmr_process_tiles (ctmr_tile_out)."""
+
+    def __init__(self, n: int, n_tiles: int, want_sha: bool = True, want_meta: bool = False, want_leaf_hash: bool = False):
+        super().__init__(n, want_sha, want_meta)
+        del self.leaf_src
+        self.leaf_off = np.zeros(n, np.uint64)
+        self.leaf_index = np.zeros(n, np.uint64)
+        self.leaf_hash = np.zeros((n, 32), np.uint8) if want_leaf_hash else None
+        self.tile_status = np.zeros(n_tiles, np.uint8)
+        self.tiles_done = 0
+        self.missing = []   # fingerprints (bytes) of the unregistered Chain[0] certificates of tile `tiles_done`
 
 
 class GpuCertDatabase:
@@ -233,6 +254,93 @@ class GpuCertDatabase:
 
     def _process_raw_fn(self):
         return self._lib.ctmr_process_raw
+
+    # ------------------------------------------------------------------ static-ct-api data tiles (include/ctmr_frontend.h)
+    def register_chain_certs(self, blob, offsets):
+        """Chain certificates -> (dense issuer indices, SHA-256 fingerprints [n][32]); the fingerprints become known to
+        store_tiles."""
+        blob = np.ascontiguousarray(blob, np.uint8)
+        offsets = np.ascontiguousarray(offsets, np.uint64)
+        n = offsets.size - 1
+        dense = np.zeros(max(n, 1), np.uint32)
+        fps = np.zeros((max(n, 1), 32), np.uint8)
+        self._check(self._register_chain_fn()(self._h, capi.ptr(blob) if blob.size else None, capi.ptr(offsets), n, capi.ptr(dense),
+                                              capi.ptr(fps)))
+        return dense[:n], fps[:n]
+
+    def _register_chain_fn(self):
+        return self._lib.ctmr_register_chain_certs
+
+    def _process_tiles_fn(self):
+        return self._lib.ctmr_process_tiles
+
+    def store_tiles(self, data, tile_off, tile_len, tile_index, tile_width, now_unix_ns: int, want_sha: bool = True,
+                    want_meta: bool = False, want_pem: bool = False, want_leaf_hash: bool = False, missing_cap: int = 256,
+                    fetch=None) -> "TileBatchResult":
+        """static-ct-api data tiles through ctmr_process_tiles.  Without `fetch`, a tile naming an unregistered Chain[0]
+        stops the call: the result has tiles_done < n_tiles and the missing fingerprints.  With fetch(fingerprints) ->
+        DERs, those certificates are registered and the call resumes from there until every tile is done."""
+        data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
+        tile_off, tile_index = np.ascontiguousarray(tile_off, np.uint64), np.ascontiguousarray(tile_index, np.uint64)
+        tile_len, tile_width = np.ascontiguousarray(tile_len, np.uint32), np.ascontiguousarray(tile_width, np.uint16)
+        nt = tile_off.size
+        ent = np.zeros(nt + 1, np.int64)
+        ent[1:] = np.cumsum(tile_width.astype(np.int64))
+        n = int(ent[-1])
+        r = TileBatchResult(n, nt, want_sha, want_meta, want_leaf_hash)
+        p = r.path
+        if want_pem:
+            _attach_pem(capi.Out(), p, n, int(tile_len.astype(np.int64).sum()))
+        miss = np.zeros((max(missing_cap, 1), 32), np.uint8)
+        t0, pem_base = 0, 0
+        while True:
+            e0 = int(ent[t0])
+
+            def at(a, per=1):
+                return None if a is None else capi.ptr(a) + e0 * per * a.itemsize
+
+            o = capi.TileOut()
+            o.path = capi.Out(at(p.status), at(p.sha256, 32) if want_sha else None, at(p.exp_hour), at(p.serial_off),
+                              at(p.serial_len), at(p.was_unknown), at(p.first_issuer_hour),
+                              *([at(p.issuer_name_off), at(p.issuer_name_len), at(p.crldp_off), at(p.crldp_len),
+                                 at(p.first_issuer_dn), at(p.first_crldp)] if want_meta else [None] * 6))
+            if want_pem:
+                o.path.pem, o.path.pem_cap, o.path.pem_off = capi.ptr(p.pem) + pem_base, p.pem.size - pem_base, at(p.pem_off)
+            for name in ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_index", "leaf_off", "leaf_len"):
+                setattr(o, name, at(getattr(r, name)))
+            o.leaf_hash = at(r.leaf_hash, 32)
+            o.tile_status = capi.ptr(r.tile_status) + t0
+            o.missing_fp, o.missing_cap = capi.ptr(miss), missing_cap
+            b = capi.TileBatch(capi.ptr(data), data.size, capi.ptr(tile_off) + 8 * t0, capi.ptr(tile_len) + 4 * t0,
+                               capi.ptr(tile_index) + 8 * t0, capi.ptr(tile_width) + 2 * t0, nt - t0, now_unix_ns)
+            rc = self._process_tiles_fn()(self._h, C.byref(b), C.byref(o))
+            done = int(o.tiles_done)
+            if want_pem:
+                e1 = int(ent[t0 + done])
+                p.pem_off[e0:e1 + 1] += pem_base
+                pem_base = int(p.pem_off[e1])
+            t0 += done
+            r.tiles_done = t0
+            r.missing = [miss[k].tobytes() for k in range(o.n_missing)] if rc == capi.E_UNKNOWN_ISSUER else []
+            if rc != capi.E_UNKNOWN_ISSUER:
+                self._check(rc)
+                return r
+            if fetch is None:
+                return r
+            ders = [bytes(d) for d in fetch(r.missing)]
+            # a log that serves the wrong bytes at issuer/<hex> would otherwise stop at this tile for ever
+            got = [hashlib.sha256(d).digest() for d in ders]
+            if set(got) != set(r.missing):
+                raise CtmrError(capi.E_UNKNOWN_ISSUER, "fetch returned certificates whose SHA-256 does not match the missing "
+                                "fingerprints of tile %d" % t0)
+            self.register_chain_certs(*_pack(ders))
+
+
+    def tiles_profile_last(self) -> float:
+        """Milliseconds of tile_split (the serial per-tile walk) in the last store_tiles call, part of frontend_ms."""
+        a = C.c_float(0)
+        self._check(self._lib.ctmr_tiles_profile_last(self._h, C.byref(a)))
+        return a.value
 
     def frontend_profile_last(self):
         """(frontend_ms, path_ms, frontend_launches) of the last store_raw_entries call (CUDA events inside the library)."""
@@ -387,6 +495,12 @@ class GpuCertGroup(GpuCertDatabase):
     def _process_raw_fn(self):
         return self._lib.ctmr_group_process_raw
 
+    def _process_tiles_fn(self):
+        return self._lib.ctmr_group_process_tiles
+
+    def _register_chain_fn(self):
+        return self._lib.ctmr_group_register_chain_certs
+
     def register_issuers(self, issuer_blob, issuer_offsets):
         return self.members[0].register_issuers(issuer_blob, issuer_offsets)   # the registry is the group's
 
@@ -456,7 +570,7 @@ class GpuCertGroup(GpuCertDatabase):
     # the device-resident / per-ctx entry points of the base class do not take a group handle
     map_device = reduce_device = process_device = read_histogram_device = profile_last = sha256_ceiling = _single_ctx_only
     reset_device = check_device = peer_export = peer_attach = peer_barrier_device = _single_ctx_only
-    peer_allreduce_histogram_device = frontend_profile_last = _single_ctx_only
+    peer_allreduce_histogram_device = frontend_profile_last = tiles_profile_last = _single_ctx_only
 
 
 # ---------------------------------------------------------------------- synthetic corpus (bench/test tooling)

@@ -91,3 +91,93 @@ def get_entries_body(entries) -> bytes:
     """A get-entries response body for (leaf_input bytes, extra_data bytes) pairs."""
     parts = [b'{"leaf_input":"' + base64.b64encode(li) + b'","extra_data":"' + base64.b64encode(ed) + b'"}' for li, ed in entries]
     return b'{"entries":[' + b",".join(parts) + b"]}"
+
+
+# ---- static-ct-api data tiles (C2SP static-ct-api; include/ctmr_frontend.h) ---------------------------------------
+# TileLeaf := TimestampedEntry [ASN.1Cert pre_certificate] Fingerprint certificate_chain<0..2^16-1>.  A tile is up to 256
+# TileLeafs back to back; the GPU splits them (ctmr_process_tiles).  These helpers build tiles and restate one as the
+# get-entries entries it stands for.
+
+def leaf_index_extension(index: int) -> bytes:
+    """The leaf_index CT extension: extension_type 0, 5 bytes of uint40."""
+    return b"\x00" + struct.pack(">H", 5) + int(index).to_bytes(5, "big")
+
+
+def tile_leaf_x509(timestamp_ms: int, cert_der: bytes, chain_fps, extensions: bytes) -> bytes:
+    """TileLeaf of an x509_entry; `extensions` is the CtExtensions body (e.g. leaf_index_extension(i))."""
+    fps = b"".join(chain_fps)
+    return merkle_tree_leaf_x509(timestamp_ms, cert_der, extensions)[2:] + struct.pack(">H", len(fps)) + fps
+
+
+def tile_leaf_precert(timestamp_ms: int, issuer_key_hash: bytes, tbs_der: bytes, pre_certificate: bytes, chain_fps,
+                      extensions: bytes) -> bytes:
+    """TileLeaf of a precert_entry: PreCert in the TimestampedEntry, then the pre_certificate, then the fingerprints."""
+    fps = b"".join(chain_fps)
+    return (merkle_tree_leaf_precert(timestamp_ms, issuer_key_hash, tbs_der, extensions)[2:] + _opaque24(pre_certificate) +
+            struct.pack(">H", len(fps)) + fps)
+
+
+def data_tile(leaves) -> bytes:
+    """tile/data/<N>: the TileLeafs concatenated, no separators or padding."""
+    return b"".join(leaves)
+
+
+def split_tile(tile: bytes, width: int):
+    """The `width` TileLeafs of a tile as (timestamped_entry, entry_type, pre_certificate or None, [fingerprints]);
+    None when the tile does not split into exactly `width` well-framed TileLeafs."""
+    out, q, L = [], 0, len(tile)
+
+    def take(n):
+        nonlocal q
+        if q + n > L:
+            raise ValueError
+        q += n
+        return tile[q - n:q]
+    try:
+        for _ in range(width):
+            start = q
+            take(8)
+            etype = struct.unpack(">H", take(2))[0]
+            if etype not in (0, 1):
+                return None
+            if etype == 1:
+                take(32)
+            n = int.from_bytes(take(3), "big")
+            if n == 0:
+                return None
+            take(n)
+            take(struct.unpack(">H", take(2))[0])
+            te = tile[start:q]
+            pre = None
+            if etype == 1:
+                n = int.from_bytes(take(3), "big")
+                if n == 0:
+                    return None
+                pre = take(n)
+            n = struct.unpack(">H", take(2))[0]
+            if n % 32:
+                return None
+            fps = take(n)
+            out.append((te, etype, pre, [fps[k:k + 32] for k in range(0, n, 32)]))
+    except ValueError:
+        return None
+    return out if q == L else None
+
+
+def tile_to_get_entries(tile: bytes, certs_by_fp, width: int = 256):
+    """The get-entries entries (leaf_input, extra_data) a tile stands for: leaf_input = 00 00 || TimestampedEntry,
+    extra_data = CertificateChain / PrecertChainEntry of the DERs behind the fingerprints (certs_by_fp[fp])."""
+    leaves = split_tile(tile, width)
+    if leaves is None:
+        raise ValueError("tile does not split into %d TileLeafs" % width)
+    out = []
+    for te, etype, pre, fps in leaves:
+        chain = [certs_by_fp[fp] for fp in fps]
+        out.append((b"\x00\x00" + te, precert_chain_entry(pre, chain) if etype == 1 else certificate_chain(chain)))
+    return out
+
+
+def leaf_hash(timestamped_entry: bytes) -> bytes:
+    """RFC 6962 §2.1 leaf hash of a MerkleTreeLeaf{v1, timestamped_entry}: what the level-0 hash tile holds."""
+    import hashlib
+    return hashlib.sha256(b"\x00\x00\x00" + timestamped_entry).digest()

@@ -54,7 +54,8 @@ enum {
     CTMR_E_PAIR_TABLE_FULL = -8,  /* (issuer, expDate) table exhausted: raise config.pair_capacity_log2 */
     CTMR_E_META_TABLE_FULL = -9,  /* IssuerMetadata string-identity table exhausted: raise config.meta_capacity_log2 */
     CTMR_E_PEER_TIMEOUT = -10,    /* a rank of the group did not reach a barrier (a peer failed or the calls diverged) */
-    CTMR_E_PEER = -11             /* peer access / CUDA IPC between the GPUs of a group is not available */
+    CTMR_E_PEER = -11,            /* peer access / CUDA IPC between the GPUs of a group is not available */
+    CTMR_E_UNKNOWN_ISSUER = -12   /* ctmr_process_tiles: a Chain[0] fingerprint is not registered (ctmr_frontend.h) */
 };
 
 /* ---- per-entry status -------------------------------------------------------------------- */
@@ -355,6 +356,13 @@ uint64_t ctmr_synth_issuers_host(const struct ctmr_synth_cfg* cfg, uint64_t* off
  * text != NULL and cap suffices. */
 uint64_t ctmr_synth_raw_pages_host(const struct ctmr_synth_cfg* cfg, uint64_t first, uint64_t n, uint32_t page, uint8_t* text,
                                    uint64_t cap, uint64_t* leaf_off, uint32_t* leaf_len, uint64_t* extra_off, uint32_t* extra_len);
+
+/* host-side: static-ct-api data tiles first_tile .. first_tile + n_tiles - 1 (256 entries each) of the same entries as
+ * ctmr_synth_raw_pages_host (entry i = 256 * N + j of tile N), for input to ctmr_process_tiles (ctmr_frontend.h).
+ * issuer_fps ([cfg->n_issuers][32]) are the fingerprints of the synthetic issuers, passed in by the caller.  Returns the
+ * bytes needed; writes the tiles back to back and their spans when data != NULL and cap suffices. */
+uint64_t ctmr_synth_tiles_host(const struct ctmr_synth_cfg* cfg, uint64_t first_tile, uint64_t n_tiles, const uint8_t* issuer_fps,
+                               uint8_t* data, uint64_t cap, uint64_t* tile_off, uint32_t* tile_len);
 
 #ifdef __cplusplus
 }

@@ -39,8 +39,12 @@ enum {
     CTMR_FE_BAD_LEAF = 2,     /* leaf_input is not a v1 timestamped MerkleTreeLeaf, or has trailing data */
     CTMR_FE_UNKNOWN_TYPE = 3, /* entry_type is neither x509_entry(0) nor precert_entry(1) */
     CTMR_FE_BAD_EXTRA = 4,    /* extra_data is not the chain structure its entry type requires */
-    CTMR_FE_BAD_CERT = 5      /* x509: the leaf certificate, precert: the TBSCertificate of the leaf, has a fatal
+    CTMR_FE_BAD_CERT = 5,     /* x509: the leaf certificate, precert: the TBSCertificate of the leaf, has a fatal
                                  parse error ("failed to parse (pre)certificate in MerkleTreeLeaf") */
+    CTMR_FE_BAD_TILE = 6,     /* static-ct-api data tile that does not split into exactly `width` well-framed TileLeafs
+                                 (ctmr_process_tiles): every entry of the tile gets it */
+    CTMR_FE_BAD_INDEX = 7     /* TileLeaf whose leaf_index extension is missing, repeated, not 5 bytes long or not
+                                 256 * N + j (ctmr_process_tiles) */
 };
 
 #define CTMR_ENTRY_X509 0u
@@ -94,9 +98,88 @@ int ctmr_process_raw(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_out* o
  * the outputs equal those of ctmr_process_raw on one GPU for the same pages. */
 int ctmr_group_process_raw(ctmr_group* g, const ctmr_raw_batch* batch, ctmr_raw_out* out);
 
-/* CUDA-event timings of the last ctmr_process_raw call: front-end kernels (decode, framing, issuer
- * identification) and the map/reduce that followed, summed over its chunks, in milliseconds */
+/* CUDA-event timings of the last front-end call (raw or tiles): front-end kernels (decode, framing, issuer
+ * identification; for tiles the split, framing, fingerprint look-up and leaf hashes) and the map/reduce that
+ * followed, summed over its chunks, in milliseconds */
 int ctmr_frontend_profile_last(ctmr_ctx* ctx, float* frontend_ms, float* path_ms, uint64_t* frontend_launches);
+
+/* ---- static-ct-api data tiles (C2SP static-ct-api) --------------------------------------------------------------
+ * A data tile holds up to 256 TileLeafs back to back, no separators (big-endian, TLS vectors, RFC 5246 §4):
+ *   TileLeaf := TimestampedEntry (RFC 6962 §3.4)
+ *               [ ASN.1Cert pre_certificate ]                  opaque<1..2^24-1>, precert_entry only
+ *               Fingerprint certificate_chain<0..2^16-1>       byte length a multiple of 32
+ * A Fingerprint is SHA-256 of a chain certificate's DER (the log serves the DER at issuer/<hex>).  The
+ * TimestampedEntry's CtExtensions must carry exactly one leaf_index extension (type 0, 5 bytes, uint40) equal to
+ * 256 * N + j for entry j of tile N.  An entry is processed as the get-entries entry with
+ * leaf_input = 00 00 || TimestampedEntry and the chain DERs behind the fingerprints; Chain[0] is the certificate
+ * behind the first fingerprint. */
+
+/* n_tiles tiles; HOST buffers.  Tile t is data[tile_off[t] .. tile_off[t] + tile_len[t]) with tile_width[t] entries
+ * (1..256: 256 for a full tile, W for a partial tile .p/W), and is tile number tile_index[t] of its log.  Tiles need not
+ * be consecutive and may come from several logs.  The entries of the batch are the tiles' entries in tile order. */
+typedef struct ctmr_tile_batch {
+    const uint8_t* data;
+    uint64_t data_bytes;
+    const uint64_t* tile_off;    /* [n_tiles] */
+    const uint32_t* tile_len;    /* [n_tiles] */
+    const uint64_t* tile_index;  /* [n_tiles] N of tile/data/<N> */
+    const uint16_t* tile_width;  /* [n_tiles] */
+    uint64_t n_tiles;
+    int64_t now_unix_ns;
+} ctmr_tile_batch;
+
+/* Caller-allocated outputs; per-entry arrays [n = sum of widths], any pointer may be NULL.  Only entries and tiles
+ * before tiles_done are written. */
+typedef struct ctmr_tile_out {
+    ctmr_out path;            /* as ctmr_raw_out.path; pem_off has n + 1 entries */
+    uint8_t* entry_status;    /* CTMR_FE_* (OK, BAD_CERT, BAD_TILE, BAD_INDEX) */
+    uint8_t* entry_type;      /* CTMR_ENTRY_*; CTMR_ENTRY_OTHER for entries of a bad tile */
+    uint64_t* timestamp_ms;
+    uint32_t* issuer;         /* dense index of Chain[0], CTMR_ISSUER_NONE, CTMR_ISSUER_BAD */
+    uint64_t* leaf_index;     /* the leaf_index extension's value (0 when absent or malformed) */
+    uint64_t* leaf_off;       /* absolute offset in batch.data of the certificate the path processed (x509: the leaf,
+                                 precert: pre_certificate), so the host can cut its DER; 0 with leaf_len 0 when dropped */
+    uint32_t* leaf_len;
+    uint8_t* leaf_hash;       /* [n][32] RFC 6962 §2.1 leaf hash SHA-256(00 || 00 00 || TimestampedEntry); zero for
+                                 entries of a bad tile */
+    uint8_t* tile_status;     /* [n_tiles] CTMR_FE_OK or CTMR_FE_BAD_TILE */
+    uint8_t* missing_fp;      /* [missing_cap][32] */
+    uint32_t missing_cap;
+    uint64_t tiles_done;      /* written: tiles completed (n_tiles unless the call returned CTMR_E_UNKNOWN_ISSUER) */
+    uint32_t n_missing;       /* written: fingerprints listed in missing_fp */
+} ctmr_tile_out;
+
+/* Split + frame + fingerprint -> dense index + map + reduce.  Synchronous.  Entries take the global indices following
+ * those of earlier ctmr_process_batch / ctmr_process_raw / ctmr_process_tiles calls on this ctx.
+ *
+ * Chain[0] is looked up by fingerprint in a per-ctx table filled by ctmr_register_chain_certs; nothing is resolved on a
+ * guess.  When tile k is the first tile holding a Chain[0] fingerprint the table does not know, tiles [0, k) are
+ * completed with full outputs and indices, tiles_done = k, the distinct unknown fingerprints of tile k (sorted, at most
+ * missing_cap) go to missing_fp, and the call returns CTMR_E_UNKNOWN_ISSUER; no entry of tile k or later touches the
+ * tables or takes an index.  Register those certificates and call again with tiles [k, n_tiles): the combined result
+ * equals one call made with every certificate registered beforehand.  A width outside 1..256 or a tile outside data is
+ * CTMR_E_INVALID before any work; a tile larger than the front end's staging budget is CTMR_E_BATCH_TOO_LARGE. */
+int ctmr_process_tiles(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_tile_out* out);
+
+/* The same on a group: each round takes one chunk of whole tiles per GPU out of ONE contiguous window of the batch and
+ * runs as one round of the group's key exchange, so the outputs equal those of ctmr_process_tiles on one GPU. */
+int ctmr_group_process_tiles(ctmr_group* g, const ctmr_tile_batch* batch, ctmr_tile_out* out);
+
+/* CUDA-event time of tile_split (the serial per-tile walk) in the last ctmr_process_tiles call on this ctx, summed over
+ * its chunks, in milliseconds: a part of the frontend_ms that ctmr_frontend_profile_last reports */
+int ctmr_tiles_profile_last(ctmr_ctx* ctx, float* split_ms);
+
+/* Chain certificates blob[offsets[k] .. offsets[k+1]) for k < n: SHA-256 fingerprint computed on the GPU, the certificate
+ * registered as with ctmr_register_issuers (dense index, or CTMR_ISSUER_BAD when it does not parse), and
+ * fingerprint -> dense index recorded in the ctx's fingerprint table.  The table holds 2 x config.max_issuers
+ * fingerprints (CTMR_E_TOO_MANY_ISSUERS beyond that; a certificate that fails that way is not registered).  Like the
+ * Chain[0] mirror it is cleared by ctmr_snapshot_load and is not part of a snapshot: register the certificates again
+ * after a restore (they get the same dense indices).  fp_out ([n][32]) may be NULL. */
+int ctmr_register_chain_certs(ctmr_ctx* ctx, const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint32_t* dense_out,
+                              uint8_t* fp_out);
+/* The same for every member of a group, from the group's one issuer registry. */
+int ctmr_group_register_chain_certs(ctmr_group* g, const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint32_t* dense_out,
+                                    uint8_t* fp_out);
 
 #ifdef __cplusplus
 }

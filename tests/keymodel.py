@@ -5,6 +5,8 @@ Mirrors, and must change with:
   ctmr_common.cuh   key_hash (the slot hash), known_insert (home slot (h >> 7) & mask, linear probing, tag (h & ~3) | 2)
   ctmr_device.cuh   mix64
   ctmr_kernels.cuh  KnownSlot {inv_first, tag, body[12]} (64 bytes), PairSlot {key, inv_first, count, pad} (32 bytes)
+  ctmr_reduce.cu    pair_insert (home slot mix64(key) & mask, linear probing, inv_first = ~lowest new index of the
+                    (issuer, hour)), evict_pairs_kernel (an expired set's count is 0 again, its first-seen index stays)
   ctmr_map.cu       the key body: (u32)(i32)exp_hour, dense issuer, then {serial_len, serial[39]} packed little-endian
   ctmr_api.cu       SnapHeader (8-byte magic + six u64) followed by the table, then the pair table
 """
@@ -70,10 +72,13 @@ def key_hash_np(bodies: np.ndarray) -> np.ndarray:
 
 
 class KeyModel:
-    """What the table must hold: key body -> lowest global entry index, from the oracle's per-entry outputs."""
+    """What the table must hold: key body -> lowest global entry index, from the oracle's per-entry outputs; and per
+    (hour, issuer) the lowest index of a NEW certificate, which eviction does not forget (the reference's
+    seenExpDateBefore memo is process memory, not Redis)."""
 
     def __init__(self):
         self.first: dict = {}
+        self.pair_first: dict = {}
         self.next_index = 0
 
     def add(self, blob, offsets, r_ora, dense_issuer, first_index=None):
@@ -88,6 +93,9 @@ class KeyModel:
             a = int(offsets[i]) + int(r_ora.serial_off[i])
             k = key_body(int(r_ora.exp_hour[i]), int(dense_issuer[i]), bytes(blob[a:a + sl]))
             gi = base + int(i)
+            if k not in self.first:  # a new certificate: entries come in index order
+                pk = (k[0], k[1])
+                self.pair_first[pk] = min(self.pair_first.get(pk, gi), gi)
             if gi < self.first.get(k, 1 << 64):
                 self.first[k] = gi
         self.next_index = max(self.next_index, base + n)
@@ -139,10 +147,23 @@ def check_table(snap: np.ndarray, model: KeyModel, used: int | None = None):
         assert used == len(seen)
     want = model.pair_counts()
     got = {}
-    for p in pairs[pairs["key"] != 0]:
+    pmask = pairs.size - 1
+    pkeys = pairs["key"]
+    for pos in np.nonzero(pkeys != 0)[0]:
+        p = pairs[pos]
         k = int(p["key"]) - 1
-        got[(k & 0xFFFFFFFF, k >> 32)] = int(p["count"])
+        hk = (k & 0xFFFFFFFF, k >> 32)
+        assert hk not in got, ("pair stored twice", hk)
+        got[hk] = int(p["count"])
+        assert hk in model.pair_first, ("pair slot of a set no new certificate opened", pos, hk)
+        assert (~int(p["inv_first"])) & M64 == model.pair_first[hk], ("pair first index", pos, hk)
+        home = int(mix64(int(p["key"])) & pmask)
+        s = home
+        while s != pos:  # no hole between the pair's home slot and its slot
+            assert pkeys[s] != 0, ("hole in the pair probe chain", home, s, pos)
+            s = (s + 1) & pmask
     for k, v in got.items():
         assert v == want.get(k, 0), ("pair count", k, v, want.get(k, 0))
     assert set(want) <= set(got)
+    assert set(got) == set(model.pair_first), "pair slots missing"
     return len(seen)

@@ -109,22 +109,54 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// Shape of the streaming map (K_map): the best measured before the port (DESIGN.md §3, K_map).
+// Shape of the streaming map (K_map, DESIGN.md §3).  Each lane stages its record in a private ring of kRing bytes
+// (two chunks) plus a 16-byte mirror of the ring's first granule, so that the hash's 17-word reads never wrap.
 struct StreamCfg {
     static constexpr int kWarps = 8;       // warps per CTA, one certificate per lane
     static constexpr int kChunk = 128;     // record bytes staged per lane and step
-    static constexpr int kCtasPerSm = 2;   // resident CTAs per SM of the persistent grid
-    static constexpr int kOverlap = 48;  // >= kWalkNeed, multiple of 16
-    // Lane slots are kSlot bytes apart and every lane reads the same word of its own slot, so the stride
+    static constexpr int kCtasPerSm = 3;   // resident CTAs per SM of the persistent grid (24 warps)
+    static constexpr int kRing = 2 * kChunk;
+    // Lane rings are kLaneBytes apart and every lane reads the same word of its own ring, so the stride
     // decides the bank pattern: 16-byte granules (cp.async) allow at best 8 distinct bank groups; an odd
-    // number of granules per slot reaches that (4-way worst case), an even one collapses to 2 groups (16-way).
-    static constexpr int kSlotRaw = kOverlap + kChunk + 16;
-    static constexpr int kSlot = kSlotRaw + (((kSlotRaw / 16) % 2 == 0) ? 16 : 0);
-    static constexpr int kWarpBytes = 2 * 32 * kSlot;
+    // number of granules per lane reaches that (4-way worst case), an even one collapses to 2 groups (16-way).
+    static constexpr int kLaneBytes = kRing + 16;
+    static constexpr int kWarpBytes = 32 * kLaneBytes;
     static constexpr int kBlocksPerChunk = kChunk / 64;
-    // +16: the walker's word-wise header read may touch the word after the last staged byte
-    static constexpr size_t kSmem = (size_t)kWarps * kWarpBytes + 16;
+    static constexpr int kGranulesPerChunk = kChunk / 16;
+    static constexpr size_t kSmem = (size_t)kWarps * kWarpBytes;
 };
+static_assert((StreamCfg::kLaneBytes / 16) % 2 == 1, "odd number of 16-byte granules per lane");
+static_assert(StreamCfg::kCtasPerSm * (StreamCfg::kSmem + 1024) <= 228 * 1024, "kCtasPerSm CTAs fit one SM's shared memory");
+
+// K_map's copy schedule.  Source granule y is the 16 bytes at 16*y from the record's 16-byte aligned base, i.e. record
+// bytes [16y - m, 16y + 16 - m) for a record m bytes past that base; it lives at ring offset 16*y mod kRing.  Chunk k
+// (record bytes [k*kChunk, (k+1)*kChunk)) spans source granules [8k, 8k + 8], the ninth only when m != 0.  When
+// m != 0 and k > 0 chunk k-1 has already brought granule 8k, so every chunk but the first copies at most 8 granules.
+// `yend` is one past the record's last source granule.  [y0, ymid) and [ymid, y1) are the two parts of the copy
+// (ring_step says why there are two); neither crosses the ring's end.
+struct RingCopy {
+    uint32_t y0, ymid, y1;
+};
+__host__ __device__ __forceinline__ RingCopy ring_chunk_copy(uint32_t k, uint32_t m, uint32_t yend) {
+    constexpr uint32_t G = StreamCfg::kGranulesPerChunk;
+    const uint32_t lo = G * k + (k != 0u && m != 0u ? 1u : 0u), next = G * (k + 1u);
+    const uint32_t y1 = yend < next + (m != 0u ? 1u : 0u) ? yend : next + (m != 0u ? 1u : 0u);
+    const uint32_t ymid = y1 < next ? y1 : next;
+    return RingCopy{lo < ymid ? lo : ymid, ymid, y1};
+}
+
+// One step of K_map's loop, entered when chunk c has landed (chunk c-1 is still in the other half of the ring): walk
+// chunk c (the walker may look back up to kWalkNeed bytes into chunk c-1), copy chunk c+1 into chunk c-1's half, hash
+// chunk c.  The copy overlaps the hash.  Its ninth granule (m != 0) lies kRing bytes past chunk c's first granule and
+// shares that granule's ring slot, which the hash is still reading: that one granule is copied after the hash.
+template <class Walk, class Copy, class Hash>
+__host__ __device__ __forceinline__ void ring_step(uint32_t c, uint32_t m, uint32_t yend, Walk&& walk, Copy&& copy, Hash&& hash) {
+    walk();
+    const RingCopy r = ring_chunk_copy(c + 1u, m, yend);
+    copy(r.y0, r.ymid);
+    hash();
+    copy(r.ymid, r.y1);
+}
 
 struct GlobalBytes {
     const uint8_t* d;

@@ -1,10 +1,10 @@
 // ctmr_map.cu -- the map half of the CT-entry hot path: hand-written sm_90a kernels.
 //
 // K_map        (map_stream_kernel) lane-per-certificate map: DER walk + certIsFilteredOut + SHA-256(leaf DER).
-//              Each lane streams ITS certificate through a private double-buffered shared-memory window filled by
+//              Each lane streams ITS certificate through a private two-chunk shared-memory ring filled by
 //              asynchronous 16-byte global->shared copies (cp.async.cg -> SASS LDGSTS, per-thread commit / wait groups: no
 //              barrier is shared between lanes), so certificate bytes never occupy registers while the INT pipe runs the
-//              64-round compression; the resumable walker (ctmr_stream.cuh) eats from the same window.  Epilogue: filter,
+//              64-round compression; the resumable walker (ctmr_stream.cuh) eats from the same ring.  Epilogue: filter,
 //              outputs, key record, and the key's route -- fused find-or-insert into this GPU's table when it owns the set,
 //              else an append to the owner GPU's inbox over NVLink (route_append).
 //              (cmd/ct-fetch/ct-fetch.go:44-70,198-213, storage/types.go:171-178,339-346; fingerprint =
@@ -167,19 +167,19 @@ __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant
 
 // ------------------------------------------------------------------------------------------------
 // K_map v2: single-pass streaming map.  The DER walker (ctmr_stream.cuh) and the SHA-256 loop both
-// eat from the same per-lane shared-memory window; global memory is touched once per byte, by
-// asynchronous copies only.  Chunks overlap by kOverlap bytes so that a TLV header (and the small
-// values the walker captures) never straddles a refill.  Staging: per-lane cp.async 16-byte copies
-// (LDGSTS) + commit/wait groups -- no barrier at all.
+// eat from the same per-lane shared-memory ring of two chunks; global memory is touched once per
+// byte, by asynchronous copies only, and every byte is copied once (ring_step in ctmr_common.cuh:
+// the next chunk is copied after the walk, so the walker can still look back into the previous one).
+// Staging: per-lane cp.async 16-byte copies (LDGSTS) + commit/wait groups -- no barrier at all.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(StreamCfg::kWarps * 32) map_stream_kernel(const __grid_constant__ MapParams p) {
+__global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm) map_stream_kernel(const __grid_constant__ MapParams p) {
     using Cfg = StreamCfg;
     constexpr int WARPS = Cfg::kWarps, CHUNK = Cfg::kChunk;
-    constexpr uint32_t OV = Cfg::kOverlap;
+    static_assert(Cfg::kRing == (int)kRingBytes && CHUNK >= (int)kWalkNeed + 16, "ring geometry");
     extern __shared__ __align__(128) uint8_t smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint8_t* my_slots = smem + (size_t)warp * Cfg::kWarpBytes + (size_t)lane * Cfg::kSlot;  // stage s at + s*32*kSlot
-    const uint32_t slot0 = smem_u32(my_slots), slot1 = slot0 + 32 * Cfg::kSlot;
+    const uint8_t* my_ring = smem + (size_t)warp * Cfg::kWarpBytes + (size_t)lane * Cfg::kLaneBytes;
+    const uint32_t ring = smem_u32(my_ring);
 
     const uint64_t ngroups = (p.n + 31) >> 5;
     const bool want_sha = p.sha256 != nullptr;
@@ -205,31 +205,23 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32) map_stream_kernel(cons
         uint32_t nch = (nb + Cfg::kBlocksPerChunk - 1) / Cfg::kBlocksPerChunk;
         nch = nch > ndata ? nch : ndata;                    // without SHA the walker alone drives the stream
         if (act && nch == 0u) nch = 1u;                     // empty record: one step so that the walker reports the error
-        uint32_t iters = warp_max_u32(nch);
-        iters = iters < 2u ? 2u : iters;
+        const uint32_t iters = warp_max_u32(nch);
+        const uint32_t yend = L ? (m + L + 15u) >> 4 : 0u;  // source granules holding record bytes
 
-        // chunk c stages record bytes [c*CHUNK - OV, c*CHUNK + CHUNK) (chunk 0: [0, CHUNK)); byte x sits
-        // at slot offset m + OV + x - c*CHUNK in every chunk
-        auto issue = [&](uint32_t c) {
-            const uint32_t slot = (c & 1u) ? slot1 : slot0;
-            uint32_t bytes = 0, dst = slot;
-            const uint8_t* src = src_base;
-            if (c < ndata) {
-                const uint32_t db = min((uint32_t)CHUNK, L - c * CHUNK);
-                if (c == 0u) {
-                    bytes = (m + db + 15u) & ~15u;
-                    dst = slot + OV;
-                } else {
-                    bytes = (m + OV + db + 15u) & ~15u;
-                    src = src_base + (size_t)c * CHUNK - OV;
-                }
-            }
+        // source granules [y0, y1) to their ring slots (the range never crosses the ring's end); the ring's
+        // first granule also goes to the mirror behind the ring
+        auto copy = [&](uint32_t y0, uint32_t y1) {
+            const uint8_t* src = src_base + 16u * y0;
+            const uint32_t dst = ring + ((16u * y0) & (Cfg::kRing - 1u));
+            if (y0 < y1 && dst == ring) cp_async16(ring + Cfg::kRing, src);
 #pragma unroll 1
-            for (uint32_t j = 0; j < bytes; j += 16u) cp_async16(dst + j, src + j);
-            cp_async_commit();
+            for (uint32_t j = 0; j < 16u * (y1 - y0); j += 16u) cp_async16(dst + j, src + j);
         };
-        issue(0);
-        issue(1);
+        {
+            const RingCopy r0 = ring_chunk_copy(0u, m, yend);
+            copy(r0.y0, r0.y1);
+            cp_async_commit();
+        }
 
         Walker w;
         w.init();
@@ -241,42 +233,43 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32) map_stream_kernel(cons
         const uint32_t one = p.one;
 
         for (uint32_t c = 0; c < iters; ++c) {
-            const uint32_t s = c & 1u;
-            cp_async_wait<1>();  // everything but the newest group (chunk c+1) has landed
+            cp_async_wait<0>();  // chunk c has landed
             if (c < nch) {
-                const uint8_t* slot = my_slots + (size_t)s * 32 * Cfg::kSlot;
                 // ---- map: resume the TLV walk over the newly staged bytes
-                if (act && w.st < W_DONE) {
-                    const uint32_t avail = min((c + 1u) * CHUNK, L);
-                    const SmemWindow rd{(s ? slot1 : slot0) + m + OV - c * CHUNK};
-                    walk_advance(w, rd, far, bad_span ? 0u : avail, L, p.filter, key_words);
-                }
-                // ---- fingerprint: the chunk's 64-byte blocks
-#pragma unroll 1
-                for (uint32_t bb = 0; bb < (uint32_t)Cfg::kBlocksPerChunk; ++bb) {
-                    const uint32_t b = c * Cfg::kBlocksPerChunk + bb;
-                    if (b >= nb) break;
-                    const uint32_t* sw = reinterpret_cast<const uint32_t*>(slot) + ((m + OV + 64u * bb) >> 2);
-                    uint32_t x[17], wd[16];
-#pragma unroll
-                    for (int i = 0; i < 17; ++i) x[i] = sw[i];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) wd[i] = __byte_perm(x[i], x[i + 1], sel);
-                    if (b >= nfull) {
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) wd[i] = sha256_pad_word(wd[i], b * 64u + 4u * i, L);
-                        if (b == nb - 1u) {
-                            wd[14] = L >> 29;
-                            wd[15] = L << 3;
-                        }
+                auto walk = [&] {
+                    if (act && w.st < W_DONE) {
+                        const uint32_t avail = min((c + 1u) * CHUNK, L);
+                        walk_advance(w, SmemWindow{ring, m}, far, bad_span ? 0u : avail, L, p.filter, key_words);
                     }
-                    sha256_compress_rolled(st, wd, one);
-                }
+                };
+                // ---- fingerprint: the chunk's 64-byte blocks, whose words start at ring offset (c*CHUNK + m) mod kRing
+                auto hash = [&] {
+#pragma unroll 1
+                    for (uint32_t bb = 0; bb < (uint32_t)Cfg::kBlocksPerChunk; ++bb) {
+                        const uint32_t b = c * Cfg::kBlocksPerChunk + bb;
+                        if (b >= nb) break;
+                        const uint32_t* sw = reinterpret_cast<const uint32_t*>(my_ring) + (((c & 1u) * CHUNK + m + 64u * bb) >> 2);
+                        uint32_t x[17], wd[16];
+#pragma unroll
+                        for (int i = 0; i < 17; ++i) x[i] = sw[i];
+#pragma unroll
+                        for (int i = 0; i < 16; ++i) wd[i] = __byte_perm(x[i], x[i + 1], sel);
+                        if (b >= nfull) {
+#pragma unroll
+                            for (int i = 0; i < 16; ++i) wd[i] = sha256_pad_word(wd[i], b * 64u + 4u * i, L);
+                            if (b == nb - 1u) {
+                                wd[14] = L >> 29;
+                                wd[15] = L << 3;
+                            }
+                        }
+                        sha256_compress_rolled(st, wd, one);
+                    }
+                };
+                ring_step(c, m, yend, walk, copy, hash);
+                cp_async_commit();
             }
-            if (c + 2u < iters) issue(c + 2u);
-            else cp_async_commit();  // keep "newest group = the one after chunk c+1" true at the tail
         }
-        cp_async_wait<0>();
+        cp_async_wait<0>();  // nothing is in flight when the ring takes the warp's next records
 
         // ---- certIsFilteredOut + Store preconditions, in the reference's order
         if (act) {
@@ -485,6 +478,9 @@ cudaError_t launch_map(const MapParams& p, int sm_count, cudaStream_t s) {
     }
     using Cfg = StreamCfg;
     cudaError_t err = cudaFuncSetAttribute(map_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem);
+    if (err != cudaSuccess) return err;
+    // kCtasPerSm rings need the largest shared-memory carve-out
+    err = cudaFuncSetAttribute(map_stream_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
     if (err != cudaSuccess) return err;
     // persistent grid: kCtasPerSm CTAs on every SM, fewer when the batch has fewer warp groups
     const uint64_t ngroups = (p.n + 31) / 32;

@@ -61,14 +61,17 @@ struct Walker {
 
 constexpr uint32_t kWalkNeed = 48;  // most bytes any single state reads from `pos` (W_SERIAL: 6 + 39)
 
-// Byte x of the record, read from the lane's shared-memory window.  `base` is the 32-bit
-// shared-space address that record offset 0 maps to (it may lie below the slot: only staged
-// offsets are ever dereferenced).
+// Byte x of the record, read from the lane's shared-memory ring: record offset x sits at ring offset (x + m) mod
+// kRingBytes, where `ring` is the ring's 32-bit shared-space address and m the record's misalignment.  A read never
+// leaves the ring; only staged offsets are ever used.
+constexpr uint32_t kRingBytes = 256;  // StreamCfg::kRing
+
 struct SmemWindow {
-    uint32_t base;
+    uint32_t ring, m;
+    __device__ __forceinline__ uint32_t at(uint32_t x) const { return ring + ((x + m) & (kRingBytes - 1u)); }
     __device__ __forceinline__ uint32_t operator()(uint32_t x) const {
         uint32_t v;
-        asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(base + x));
+        asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(at(x)));
         return v;
     }
 };
@@ -80,11 +83,12 @@ static __device__ __noinline__ uint64_t w_hdr_packed(SmemWindow rd, uint32_t pos
     constexpr uint64_t kFail = ~0ull;
     if (pos + 2u > lim) return kFail;
     // the four bytes at `pos` in one go: two aligned 32-bit shared loads + a funnel shift
-    // (tag | len0 << 8 | len1 << 16 | len2 << 24); the window has slack past the staged bytes
-    const uint32_t a = rd.base + pos, wa = a & ~3u;
+    // (tag | len0 << 8 | len1 << 16 | len2 << 24); each word's ring offset is masked on its own, so the
+    // second one wraps to the ring's start where the first one ends at the ring's end
+    const uint32_t a = pos + rd.m;
     uint32_t lo, hi;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(lo) : "r"(wa));
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(hi) : "r"(wa + 4u));
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(lo) : "r"(rd.ring + (a & (kRingBytes - 4u))));
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(hi) : "r"(rd.ring + ((a + 4u) & (kRingBytes - 4u))));
     const uint32_t v = __funnelshift_r(lo, hi, (a & 3u) * 8u);
     const uint32_t tag = v & 0xffu, l = (v >> 8) & 0xffu;
     if ((tag & 0x1fu) == 0x1fu) return kFail;

@@ -35,7 +35,7 @@ EXPORTS = [
     "ctmr_synth_tiles_host",
     "ctmr_process_raw", "ctmr_group_process_raw", "ctmr_frontend_profile_last",  # include/ctmr_frontend.h
     "ctmr_process_tiles", "ctmr_group_process_tiles", "ctmr_register_chain_certs", "ctmr_group_register_chain_certs",
-    "ctmr_tiles_profile_last",
+    "ctmr_tiles_profile_last", "ctmr_process_raw_tree", "ctmr_process_tiles_tree",
     # several GPUs: one process (group) / one process per GPU (peer)
     "ctmr_group_create", "ctmr_group_destroy", "ctmr_group_last_error", "ctmr_group_size", "ctmr_group_member",
     "ctmr_group_process_batch", "ctmr_group_issuer_counts", "ctmr_group_set_cardinality", "ctmr_group_status_counters",
@@ -111,6 +111,11 @@ class TileOut(C.Structure):
                                   ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_index", "leaf_off", "leaf_len",
                                    "leaf_hash", "tile_status", "missing_fp")] + \
                [("missing_cap", C.c_uint32), ("tiles_done", C.c_uint64), ("n_missing", C.c_uint32)]
+
+
+class Tree(C.Structure):
+    """ctmr_tree (include/ctmr_frontend.h): the Merkle tree of one log as its right edge."""
+    _fields_ = [("size", C.c_uint64), ("edge", (C.c_uint8 * 32) * 64), ("root", C.c_uint8 * 32)]
 
 
 class SynthCfg(C.Structure):
@@ -192,6 +197,8 @@ def load():
     L.ctmr_group_process_tiles.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut)]
     L.ctmr_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_tiles_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
+    L.ctmr_process_raw_tree.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), C.POINTER(Tree)]
+    L.ctmr_process_tiles_tree.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), C.POINTER(Tree)]
     L.ctmr_group_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_synth_tiles_host.argtypes = [C.POINTER(SynthCfg), u64, u64, vp, vp, u64, vp, vp]
     L.ctmr_synth_tiles_host.restype = u64

@@ -429,6 +429,7 @@ void fe_destroy(ctmr_ctx* c) {
     cudaFree(f->unknown_list); cudaFree(f->unknown_count);
     pem_free(f->pem);
     tiles_free(f);
+    tree_free(f);
     if (f->ev0) cudaEventDestroy(f->ev0);
     if (f->ev1) cudaEventDestroy(f->ev1);
     if (f->ev2) cudaEventDestroy(f->ev2);

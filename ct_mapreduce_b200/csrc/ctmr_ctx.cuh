@@ -97,6 +97,17 @@ struct TileState {
     std::unordered_map<std::string, uint32_t> fp_memo;
 };
 
+// the log's Merkle tree (ctmr_process_raw_tree / ctmr_process_tiles_tree): the call's tree on the device and the scratch
+// of the fold.  Allocated on the first tree call.
+struct TreeState {
+    TreeDev* dev = nullptr;       // the tree for the whole call: uploaded at its start, read back at its end
+    TreeDev* host = nullptr;      // pinned staging of those two copies
+    uint8_t* leaf = nullptr;      // [cap_entries][32] get-entries leaf hashes of a chunk
+    uint8_t* lvl[2] = {};         // [cap_entries / 2 + 2][32] each: ping-pong level buffers
+    uint64_t base = 0;            // log position of the call's first entry
+    bool active = false;          // a tree call is running: the chunks fold their leaves
+};
+
 // CT wire-format front end (include/ctmr_frontend.h): device buffers of one chunk + the device mirror of
 // the issuer registry keyed by certificate bytes
 struct FrontEnd {
@@ -132,6 +143,7 @@ struct FrontEnd {
     uint64_t launches = 0;
     PemStage pem;
     TileState* tl = nullptr;   // tiles_ensure
+    TreeState* tree = nullptr; // tree_ensure
 };
 
 }  // namespace ctmr_host
@@ -288,6 +300,7 @@ int frontend_ensure(ctmr_ctx* c);   // allocates the front end's buffers on firs
 int tiles_ensure(ctmr_ctx* c);      // ... and the tile buffers + fingerprint table (ctmr_frontend_api.cu), after frontend_ensure
 void tiles_free(FrontEnd* f);
 int tiles_clear_fingerprints(ctmr_ctx* c);
+void tree_free(FrontEnd* f);        // the Merkle tree's state (ctmr_frontend_api.cu)
 int ensure_scratch(ctmr_ctx* c, uint64_t n);
 uint64_t device_round_entries(uint64_t n, uint32_t rounds);   // E of a ctmr_process_device call cut into `rounds` rounds
 uint32_t peer_rounds();   // rounds of the collective ctmr_process_device (CTMR_PEER_ROUNDS, env override for experiments)

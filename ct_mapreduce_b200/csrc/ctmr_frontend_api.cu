@@ -121,6 +121,60 @@ ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
     return dout;
 }
 
+// ---- the log's Merkle tree (ctmr_process_raw_tree, ctmr_process_tiles_tree) ----------------------------------------------
+int tree_ensure(ctmr_ctx* c) {
+    FrontEnd* f = c->fe;
+    if (f->tree) return CTMR_OK;
+    TreeState* tr = new (std::nothrow) TreeState();
+    if (!tr) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    f->tree = tr;
+    const uint64_t E = f->cap_entries;
+    cudaError_t e = cudaMalloc(&tr->dev, sizeof(TreeDev));
+    if (e == cudaSuccess) e = cudaMallocHost(&tr->host, sizeof(TreeDev));
+    if (e == cudaSuccess) e = cudaMalloc(&tr->leaf, E * 32);
+    for (int k = 0; k < 2 && e == cudaSuccess; ++k) e = cudaMalloc(&tr->lvl[k], (E / 2 + 2) * 32);
+    if (e != cudaSuccess) {
+        tree_free(f);
+        return fail(c, e == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA, std::string("tree: ") + cudaGetErrorString(e));
+    }
+    return CTMR_OK;
+}
+
+// the caller's tree to the device for the whole call; the call's entries start at log position `base`
+int tree_begin(ctmr_ctx* c, const ctmr_tree* tree, uint64_t base) {
+    int rc = tree_ensure(c);
+    if (rc) return rc;
+    TreeState* tr = c->fe->tree;
+    std::memcpy(&tr->host->t, tree, sizeof(ctmr_tree));
+    tr->host->missing = ~0ull;
+    CU(c, cudaMemcpyAsync(tr->dev, tr->host, sizeof(TreeDev), cudaMemcpyHostToDevice, c->stream));
+    tr->base = base;
+    tr->active = true;
+    return CTMR_OK;
+}
+
+// folds entries [0, cnt) of a chunk, log positions first_pos.., into the tree (see FoldChunk)
+int tree_fold(ctmr_ctx* c, const uint8_t* leaves, const uint8_t* flags, uint32_t stride, uint32_t match, uint64_t first_pos, uint64_t cnt) {
+    TreeState* tr = c->fe->tree;
+    const FoldChunk fc{tr->dev, leaves, flags, stride, match, first_pos, cnt};
+    uint32_t launches = 0;
+    CU(c, launch_tree_fold(fc, tr->lvl, c->stream, &launches));
+    c->fe->launches += launches;
+    return CTMR_OK;
+}
+
+// the root, and the tree back to the caller
+int tree_end(ctmr_ctx* c, ctmr_tree* tree) {
+    TreeState* tr = c->fe->tree;
+    CU(c, launch_tree_root(tr->dev, c->stream));
+    CU(c, cudaMemcpyAsync(tr->host, tr->dev, sizeof(TreeDev), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    std::memcpy(tree, &tr->host->t, sizeof(ctmr_tree));
+    return CTMR_OK;
+}
+
+bool tree_active(const FrontEnd* f) { return f->tree && f->tree->active; }
+
 // decode + frame + Chain[0] -> dense index of an uploaded chunk; leaves ch.db / ch.dout describing the device-resident batch
 int fe_front(ctmr_ctx* c, const ctmr_raw_batch* b, const ctmr_raw_out* out, RawChunk& ch, uint64_t first_index) {
     FrontEnd* f = c->fe;
@@ -184,6 +238,12 @@ int fe_front(ctmr_ctx* c, const ctmr_raw_batch* b, const ctmr_raw_out* out, RawC
             int rc = ctmr_register_issuers(c, blob.data(), offs.data(), n_unknown, dense.data());
             if (rc) return rc;
             if (f->slots_used == before) return fail(c, CTMR_E_CUDA, "front end: unresolved Chain[0] is already registered");
+        }
+        if (tree_active(f)) {  // the leaves of this chunk into the tree, while the arena still holds them
+            CU(c, launch_raw_leaf_hash(p, f->tree->leaf, s));
+            ++f->launches;
+            const int rc = tree_fold(c, f->tree->leaf, f->str_bad, 2, 1, f->tree->base + ch.lo, cnt);
+            if (rc) return rc;
         }
     } else {
         CU(c, cudaEventRecord(st.consumed, s));
@@ -256,16 +316,23 @@ int check_args(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out) {
     return CTMR_OK;
 }
 
-int process_raw_single(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out) {
+// tree: fold the entries into it too (ctmr_process_raw_tree), written back only when the call succeeds
+int process_raw_single(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree = nullptr) {
     int rc = check_args(c, b, out);
     if (rc) return rc;
-    if (b->n == 0) return CTMR_OK;
+    if (tree && b->n > ~0ull - tree->size) return fail(c, CTMR_E_INVALID, "tree size + entries wraps around 2^64");
+    if (b->n == 0 && !tree) return CTMR_OK;
     CU(c, cudaSetDevice(c->device));
     rc = frontend_ensure(c);
     if (rc) return rc;
     FrontEnd* f = c->fe;
     f->fe_ms = f->path_ms = 0.f;
     f->launches = 0;
+    if (tree) {
+        rc = tree_begin(c, tree, tree->size);
+        if (rc) return rc;
+        if (b->n == 0) return tree_end(c, tree);
+    }
     uint64_t pem_base = 0;
     RawChunk ch[2];
     rc = fe_fit(c, b, 0, ~0ull, &ch[0].hi);
@@ -295,7 +362,8 @@ int process_raw_single(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out) 
         if (cur.hi >= b->n) break;
     }
     if (out->path.pem) out->path.pem_off[b->n] = pem_base;
-    return ctmr_check_device(c, nullptr);
+    rc = ctmr_check_device(c, nullptr);
+    return rc || !tree ? rc : tree_end(c, tree);
 }
 
 // fn(r) for every member, on one thread each (the halves of a chunk wait on the host: issuer round trips, D2H); sequential if
@@ -586,7 +654,7 @@ int tile_front(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, 
         CU(c, launch_tile_frame(p, s));
         CU(c, launch_tile_issuer(p, FpTable{tl->fp_dev, tl->fp_mask}, s));
         f->launches += 4;  // split, frame, tbs, issuer
-        if (out->leaf_hash) {
+        if (out->leaf_hash || tree_active(f)) {
             CU(c, launch_tile_leaf_hash(p, s));
             ++f->launches;
         }
@@ -615,6 +683,10 @@ int tile_front(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, 
             ch.e1 = ch.e0 + td.first;
             p.n_tiles = stop;
             p.n = q.n = td.first;
+        }
+        if (p.n && tree_active(f)) {  // the completed tiles' leaves into the tree; a bad tile has none
+            const int rc = tree_fold(c, tl->leaf_hash, f->entry_status, 1, CTMR_FE_BAD_TILE, f->tree->base + ch.e0, p.n);
+            if (rc) return rc;
         }
     }
     CU(c, cudaEventRecord(f->ev1, s));
@@ -698,18 +770,42 @@ int tiles_prepare(ctmr_ctx* c) {
     return CTMR_OK;
 }
 
-// *done_entries: entries that took their indices (all of them unless the call stops or fails)
-int process_tiles_single(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries) {
+// ctmr_process_tiles_tree's rules for the tiles of one log, checked before any work like tile_args
+int tree_tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tree* tree, uint64_t n) {
+    if (b->n_tiles == 0) return CTMR_OK;
+    if (b->tile_index[0] > (~0ull - n) >> 8) return fail(c, CTMR_E_INVALID, "tree: the batch's last leaf index does not fit 64 bits");
+    for (uint64_t t = 0; t + 1 < b->n_tiles; ++t) {
+        if (b->tile_index[t + 1] != b->tile_index[t] + 1) return fail(c, CTMR_E_INVALID, "tree: tiles are not consecutive");
+        if (b->tile_width[t] != 256) return fail(c, CTMR_E_INVALID, "tree: a partial tile that is not the last");
+    }
+    const uint64_t first = 256 * b->tile_index[0];
+    if (tree->size < first || tree->size > first + b->tile_width[0])
+        return fail(c, CTMR_E_INVALID, "tree: size is not inside the batch's first tile");
+    return CTMR_OK;
+}
+
+// *done_entries: entries that took their indices (all of them unless the call stops or fails).  tree: fold the entries
+// into it too (ctmr_process_tiles_tree), written back when the call succeeds or stops at an unknown Chain[0].
+int process_tiles_single(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries, ctmr_tree* tree = nullptr) {
     std::vector<uint64_t> ent;
     int rc = tile_args(c, b, out, ent);
     if (rc) return rc;
     const uint64_t n = ent[b->n_tiles];
+    if (tree) {
+        rc = tree_tile_args(c, b, tree, n);
+        if (rc) return rc;
+    }
     *done_entries = n;
     out->tiles_done = 0;
     out->n_missing = 0;
-    if (b->n_tiles == 0) return CTMR_OK;
+    if (b->n_tiles == 0 && !tree) return CTMR_OK;
     rc = tiles_prepare(c);
     if (rc) return rc;
+    if (tree) {
+        rc = tree_begin(c, tree, b->n_tiles ? 256 * b->tile_index[0] : 0);
+        if (rc) return rc;
+        if (b->n_tiles == 0) return tree_end(c, tree);
+    }
     uint64_t pem_base = 0;
     TileChunk ch[2];
     const char* too_large = "a single tile exceeds the front end's staging budget";
@@ -745,12 +841,14 @@ int process_tiles_single(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* o
             *done_entries = cur.e1;
             if (out->path.pem) out->path.pem_off[cur.e1] = pem_base;
             rc = ctmr_check_device(c, nullptr);  // a table that filled up during the completed tiles is this call's error
+            if (rc == CTMR_OK && tree) rc = tree_end(c, tree);  // the completed tiles are in the tree: resume from there
             return rc ? rc : tile_stop(c, out, cur);
         }
         if (cur.hi >= b->n_tiles) break;
     }
     if (out->path.pem) out->path.pem_off[n] = pem_base;
-    return ctmr_check_device(c, nullptr);
+    rc = ctmr_check_device(c, nullptr);
+    return rc || !tree ? rc : tree_end(c, tree);
 }
 
 int process_tiles_group(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries, ctmr_ctx** failed) {
@@ -988,6 +1086,29 @@ int ctmr_group_process_tiles(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_
     return rc;
 }
 
+int ctmr_process_raw_tree(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
+    const int rc = process_raw_single(c, b, out, tree);
+    if (c->fe && c->fe->tree) c->fe->tree->active = false;
+    if (b) c->next_index += b->n;  // as ctmr_process_raw
+    if (rc != CTMR_OK) drain_frontend(c);
+    return rc;
+}
+
+int ctmr_process_tiles_tree(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, ctmr_tree* tree) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
+    uint64_t done = 0;
+    const int rc = process_tiles_single(c, b, out, &done, tree);
+    if (c->fe && c->fe->tree) c->fe->tree->active = false;
+    c->next_index += done;  // as ctmr_process_tiles
+    if (rc != CTMR_OK) drain_frontend(c);
+    return rc;
+}
+
 int ctmr_tiles_profile_last(ctmr_ctx* c, float* split_ms) {
     if (!c || !c->fe || !c->fe->tl) return fail(c, CTMR_E_INVALID, "no ctmr_process_tiles call to report");
     if (split_ms) *split_ms = c->fe->tl->split_ms;
@@ -1063,6 +1184,14 @@ void tiles_free(FrontEnd* f) {
     if (tl->ev_split1) cudaEventDestroy(tl->ev_split1);
     delete tl;
     f->tl = nullptr;
+}
+
+void tree_free(FrontEnd* f) {
+    TreeState* tr = f->tree;
+    if (!tr) return;
+    cudaFree(tr->dev); cudaFreeHost(tr->host); cudaFree(tr->leaf); cudaFree(tr->lvl[0]); cudaFree(tr->lvl[1]);
+    delete tr;
+    f->tree = nullptr;
 }
 
 int tiles_clear_fingerprints(ctmr_ctx* c) {

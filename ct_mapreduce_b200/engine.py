@@ -63,6 +63,28 @@ class KnownCertificatesView:
         return out.value
 
 
+@dataclass
+class LogTree:
+    """The RFC 6962 Merkle tree over the first `size` entries of one log, held as its right edge (ctmr_tree): edge[k] is
+    the root of a complete subtree of 2^k leaves for every bit k set in size.  Pass it as tree= to store_raw_entries /
+    store_tiles; the result's .tree is the tree after the batch, and .root is what the log's signed tree head of that
+    size must carry."""
+    size: int = 0
+    edge: np.ndarray | None = None   # [64][32] uint8
+    root: bytes = b""
+
+    def to_c(self) -> "capi.Tree":
+        t = capi.Tree()
+        t.size = int(self.size)
+        if self.edge is not None:
+            C.memmove(t.edge, np.ascontiguousarray(self.edge, np.uint8).tobytes(), 64 * 32)
+        return t
+
+    @classmethod
+    def from_c(cls, t: "capi.Tree") -> "LogTree":
+        return cls(int(t.size), np.frombuffer(bytes(t.edge), np.uint8).reshape(64, 32).copy(), bytes(t.root))
+
+
 def _pack(ders):
     offsets = np.zeros(len(ders) + 1, np.uint64)
     offsets[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
@@ -94,6 +116,7 @@ class RawBatchResult:
         self.leaf_src = np.zeros(n, np.uint8)
         self.leaf_off = np.zeros(n, np.uint32)
         self.leaf_len = np.zeros(n, np.uint32)
+        self.tree = None    # LogTree after the batch, when the call was given one
 
 
 class TileBatchResult(RawBatchResult):
@@ -229,9 +252,10 @@ class GpuCertDatabase:
 
     # ------------------------------------------------------------------ CT wire-format front end (include/ctmr_frontend.h)
     def store_raw_entries(self, text, leaf_off, leaf_len, extra_off, extra_len, now_unix_ns: int, want_sha: bool = True,
-                          want_meta: bool = False, want_pem: bool = False) -> "RawBatchResult":
+                          want_meta: bool = False, want_pem: bool = False, tree: LogTree | None = None) -> "RawBatchResult":
         """get-entries strings (base64 leaf_input / extra_data, spans into `text`) through ctmr_process_raw:
-        what GetRawEntries' JSON decode, ct.LogEntryFromLeaf (ct-fetch.go:424,452) and insertCTWorker + Store do."""
+        what GetRawEntries' JSON decode, ct.LogEntryFromLeaf (ct-fetch.go:424,452) and insertCTWorker + Store do.
+        With tree= (the log's entries before these), ctmr_process_raw_tree also folds the entries into it: r.tree."""
         text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else np.ascontiguousarray(text, np.uint8)
         leaf_off, extra_off = np.ascontiguousarray(leaf_off, np.uint64), np.ascontiguousarray(extra_off, np.uint64)
         leaf_len, extra_len = np.ascontiguousarray(leaf_len, np.uint32), np.ascontiguousarray(extra_len, np.uint32)
@@ -249,7 +273,12 @@ class GpuCertDatabase:
             _attach_pem(o.path, p, n, (int(leaf_len.sum()) + int(extra_len.sum())) // 4 * 3)
         b = capi.RawBatch(capi.ptr(text), text.size, capi.ptr(leaf_off), capi.ptr(leaf_len), capi.ptr(extra_off), capi.ptr(extra_len),
                           n, now_unix_ns)
-        self._check(self._process_raw_fn()(self._h, C.byref(b), C.byref(o)))
+        if tree is None:
+            self._check(self._process_raw_fn()(self._h, C.byref(b), C.byref(o)))
+            return r
+        ct = tree.to_c()
+        self._check(self._lib.ctmr_process_raw_tree(self._h, C.byref(b), C.byref(o), C.byref(ct)))
+        r.tree = LogTree.from_c(ct)
         return r
 
     def _process_raw_fn(self):
@@ -276,10 +305,12 @@ class GpuCertDatabase:
 
     def store_tiles(self, data, tile_off, tile_len, tile_index, tile_width, now_unix_ns: int, want_sha: bool = True,
                     want_meta: bool = False, want_pem: bool = False, want_leaf_hash: bool = False, missing_cap: int = 256,
-                    fetch=None) -> "TileBatchResult":
+                    fetch=None, tree: LogTree | None = None) -> "TileBatchResult":
         """static-ct-api data tiles through ctmr_process_tiles.  Without `fetch`, a tile naming an unregistered Chain[0]
         stops the call: the result has tiles_done < n_tiles and the missing fingerprints.  With fetch(fingerprints) ->
-        DERs, those certificates are registered and the call resumes from there until every tile is done."""
+        DERs, those certificates are registered and the call resumes from there until every tile is done.  With tree= (the
+        log's entries before these; consecutive tiles of that log), ctmr_process_tiles_tree also folds the entries into
+        it and every resumed call carries it on: r.tree."""
         data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
         tile_off, tile_index = np.ascontiguousarray(tile_off, np.uint64), np.ascontiguousarray(tile_index, np.uint64)
         tile_len, tile_width = np.ascontiguousarray(tile_len, np.uint32), np.ascontiguousarray(tile_width, np.uint16)
@@ -292,6 +323,7 @@ class GpuCertDatabase:
         if want_pem:
             _attach_pem(capi.Out(), p, n, int(tile_len.astype(np.int64).sum()))
         miss = np.zeros((max(missing_cap, 1), 32), np.uint8)
+        ct = tree.to_c() if tree is not None else None
         t0, pem_base = 0, 0
         while True:
             e0 = int(ent[t0])
@@ -313,7 +345,14 @@ class GpuCertDatabase:
             o.missing_fp, o.missing_cap = capi.ptr(miss), missing_cap
             b = capi.TileBatch(capi.ptr(data), data.size, capi.ptr(tile_off) + 8 * t0, capi.ptr(tile_len) + 4 * t0,
                                capi.ptr(tile_index) + 8 * t0, capi.ptr(tile_width) + 2 * t0, nt - t0, now_unix_ns)
-            rc = self._process_tiles_fn()(self._h, C.byref(b), C.byref(o))
+            if ct is not None and t0 > 0 and ct.size < 256 * int(tile_index[t0]):
+                ct = None  # a bad tile among the completed tiles stopped the fold: r.tree is final, the rest runs plain
+            if ct is None:
+                rc = self._process_tiles_fn()(self._h, C.byref(b), C.byref(o))
+            else:  # written back on success and at the stop: the resumed call continues this tree
+                rc = self._lib.ctmr_process_tiles_tree(self._h, C.byref(b), C.byref(o), C.byref(ct))
+                if rc in (0, capi.E_UNKNOWN_ISSUER):
+                    r.tree = LogTree.from_c(ct)
             done = int(o.tiles_done)
             if want_pem:
                 e1 = int(ent[t0 + done])
@@ -497,6 +536,16 @@ class GpuCertGroup(GpuCertDatabase):
 
     def _process_tiles_fn(self):
         return self._lib.ctmr_group_process_tiles
+
+    def store_raw_entries(self, *a, tree=None, **k):
+        if tree is not None:  # members hold disjoint slices: the fold would have to be ordered across GPUs
+            raise CtmrError(capi.E_INVALID, "tree= takes one ctx: a group has no tree form")
+        return super().store_raw_entries(*a, **k)
+
+    def store_tiles(self, *a, tree=None, **k):
+        if tree is not None:
+            raise CtmrError(capi.E_INVALID, "tree= takes one ctx: a group has no tree form")
+        return super().store_tiles(*a, **k)
 
     def _register_chain_fn(self):
         return self._lib.ctmr_group_register_chain_certs

@@ -128,9 +128,22 @@ func (r *RawResult) Free() {
 // ProcessRaw = GetRawEntries' base64 decode + ct.LogEntryFromLeaf + insertCTWorker + Store decisions for
 // every entry of the accumulated pages, in page order, on one GPU or on every GPU of the group.
 func (d *DB) ProcessRaw(p *RawPages, nowUnixNs int64, r *RawResult) error {
+	return d.processRaw(p, nowUnixNs, r, nil)
+}
+
+// processRaw also folds the entries into tree when it is not nil (ProcessRawTree, tree.go).
+func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree) error {
 	n := len(p.LeafOff)
-	if n == 0 {
+	if tree != nil && d.g != nil {
+		return fmt.Errorf("ProcessRawTree: a group has no tree form; use one DB per GPU")
+	}
+	if n == 0 && tree == nil {
 		return nil
+	}
+	if n == 0 { // the root of the tree as it stands
+		b := (*C.ctmr_raw_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_raw_batch{}))))
+		defer C.free(unsafe.Pointer(b))
+		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
 	}
 	b := (*C.ctmr_raw_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_raw_batch{}))))
 	defer C.free(unsafe.Pointer(b))
@@ -152,6 +165,9 @@ func (d *DB) ProcessRaw(p *RawPages, nowUnixNs int64, r *RawResult) error {
 	b.now_unix_ns = C.int64_t(nowUnixNs)
 	if d.g != nil { // several GPUs: one chunk per GPU per round, the same outputs in entry order
 		return d.err(C.ctmr_group_process_raw(d.g, b, r.raw), "ctmr_group_process_raw")
+	}
+	if tree != nil {
+		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
 	}
 	return d.err(C.ctmr_process_raw(d.h, b, r.raw), "ctmr_process_raw")
 }

@@ -119,7 +119,21 @@ func (d *DB) RegisterChainCerts(ders [][]byte) ([]uint32, error) {
 // registered before the call resumes from that tile.  The result equals one call made with every certificate
 // registered beforehand: every per-entry output of a resumed call, PEM included, lands at the entries it belongs to.
 func (d *DB) ProcessTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error)) error {
+	return d.processTiles(t, nowUnixNs, r, fetch, nil)
+}
+
+// processTiles also folds the entries into tree when it is not nil (ProcessTilesTree, tree.go): the library writes the
+// tree back at every stop, so each resumed call carries it on from the tiles completed so far.
+func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree) error {
+	if tree != nil && d.g != nil {
+		return fmt.Errorf("ProcessTilesTree: a group has no tree form; use one DB per GPU")
+	}
 	if len(t.Off) == 0 {
+		if tree != nil { // the root of the tree as it stands
+			b := (*C.ctmr_tile_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_batch{}))))
+			defer C.free(unsafe.Pointer(b))
+			return d.err(C.ctmr_process_tiles_tree(d.h, b, r.out, tree.c()), "ctmr_process_tiles_tree")
+		}
 		return nil
 	}
 	var pin runtime.Pinner
@@ -142,9 +156,13 @@ func (d *DB) ProcessTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 		b.n_tiles, b.now_unix_ns = C.uint64_t(len(t.Off)-t0), C.int64_t(nowUnixNs)
 		*o = *r.out
 		shiftTileOut(o, e0, t0, pemBase) // a resumed call writes from entry e0, tile t0 and PEM byte pemBase on
+		// a bad tile among the tiles completed before a stop ended the fold: the tree is final, the rest runs plain
+		fold := tree != nil && (t0 == 0 || tree.Size >= 256*t.Index[t0])
 		var rc C.int
 		if d.g != nil {
 			rc = C.ctmr_group_process_tiles(d.g, b, o)
+		} else if fold {
+			rc = C.ctmr_process_tiles_tree(d.h, b, o, tree.c())
 		} else {
 			rc = C.ctmr_process_tiles(d.h, b, o)
 		}

@@ -1,0 +1,43 @@
+// cgo binding of the Merkle tree forms of include/ctmr_frontend.h: the entries a run ingests, folded into the log's
+// RFC 6962 Merkle tree on the GPU, so that the run can be checked against the log's signed tree head.
+//
+// NOT COMPILED IN THIS REPOSITORY'S CI: the build image has no Go toolchain.  See INTEGRATION.md §2b and §2c.
+package ctmr
+
+/*
+#include "ctmr_frontend.h"
+*/
+import "C"
+
+import "unsafe"
+
+// Tree mirrors ctmr_tree: the Merkle tree over the first Size entries of one log, held as its right edge.  It holds no
+// pointers, so it is passed to the library straight from Go memory.  Keep it next to LogState: a restarted run resumes
+// the tree from it.
+type Tree struct {
+	Size uint64
+	Edge [64][32]byte // for every bit k set in Size, the root of the complete subtree of 2^k leaves ending below Size
+	Root [32]byte     // MTH of the first Size entries after the call; compare with SHA256RootHash / the checkpoint
+}
+
+// the layouts agree, or this does not compile
+var _ [unsafe.Sizeof(C.ctmr_tree{}) - unsafe.Sizeof(Tree{})]struct{}
+var _ [unsafe.Sizeof(Tree{}) - unsafe.Sizeof(C.ctmr_tree{})]struct{}
+
+func (t *Tree) c() *C.ctmr_tree { return (*C.ctmr_tree)(unsafe.Pointer(t)) }
+
+// ProcessRawTree is ProcessRaw, and the pages' entries folded into tree as the log's entries tree.Size, tree.Size+1, ....
+// An entry whose leaf_input is not base64 has no leaf: the fold stops before it and tree.Size says where.  On an error
+// tree is unchanged.  One GPU only: a group returns an error.
+func (d *DB) ProcessRawTree(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree) error {
+	return d.processRaw(p, nowUnixNs, r, tree)
+}
+
+// ProcessTilesTree is ProcessTiles, and the tiles' entries folded into tree.  The tiles must be consecutive tiles of one
+// log, full but for the last, with tree.Size inside the first: its leaves below tree.Size are skipped.  A bad tile stops
+// the fold at its first leaf, and the rest of the batch is still processed.  The fetch/register/resume loop carries the
+// tree from call to call; once a bad tile has stopped the fold, it resumes with ProcessTiles' plain call and the tree
+// stays as it is.  Tree and outputs equal those of one call with every certificate registered first.  One GPU only.
+func (d *DB) ProcessTilesTree(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree) error {
+	return d.processTiles(t, nowUnixNs, r, fetch, tree)
+}

@@ -99,7 +99,8 @@ int ctmr_process_raw(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_out* o
 int ctmr_group_process_raw(ctmr_group* g, const ctmr_raw_batch* batch, ctmr_raw_out* out);
 
 /* CUDA-event timings of the last front-end call (raw or tiles): front-end kernels (decode, framing, issuer
- * identification; for tiles the split, framing, fingerprint look-up and leaf hashes) and the map/reduce that
+ * identification; for tiles the split, framing, fingerprint look-up and leaf hashes; for the tree forms also the leaf
+ * hashes and the Merkle fold) and the map/reduce that
  * followed, summed over its chunks, in milliseconds */
 int ctmr_frontend_profile_last(ctmr_ctx* ctx, float* frontend_ms, float* path_ms, uint64_t* frontend_launches);
 
@@ -180,6 +181,44 @@ int ctmr_register_chain_certs(ctmr_ctx* ctx, const uint8_t* blob, const uint64_t
 /* The same for every member of a group, from the group's one issuer registry. */
 int ctmr_group_register_chain_certs(ctmr_group* g, const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint32_t* dense_out,
                                     uint8_t* fp_out);
+
+/* ---- the log's Merkle tree (RFC 6962 §2.1) -----------------------------------------------------------------------------
+ * A log signs only the root hash of its tree head (get-sth SHA256RootHash, a static-ct-api checkpoint's root hash): the
+ * entries a client ingested are the log's entries when the Merkle tree over them has that root.  These calls fold every
+ * entry of a batch into the tree on the GPU, next to the rest of the front end's work.
+ *
+ * The Merkle tree over the leaves [0, size) of ONE log, held as its right edge (compact range).  The struct holds no
+ * pointers, so a Go caller may pass it from Go memory.  The root is r = edge[lowest set bit of size], then for each
+ * higher set bit k in ascending order r = SHA-256(0x01 || edge[k] || r). */
+typedef struct ctmr_tree {
+    uint64_t size;          /* in/out: leaves folded in so far */
+    uint8_t  edge[64][32];  /* in/out: for every bit k set in size, the MTH of the 2^k leaves
+                               [(size >> (k+1)) << (k+1), that + 2^k); rows of clear bits are ignored on input, zero on output */
+    uint8_t  root[32];      /* out: MTH(D[0:size]) after the call; SHA-256("") for size 0 */
+} ctmr_tree;
+
+/* ctmr_process_raw, and the batch's entries folded into *tree as leaves tree->size, tree->size + 1, ... of the log.  Every
+ * output, the return code and the indices are those of ctmr_process_raw.  The leaf hash is SHA-256(0x00 || decoded
+ * leaf_input); it needs no parse, so BAD_LEAF, UNKNOWN_TYPE, BAD_EXTRA and BAD_CERT entries fold too.  Only an entry whose
+ * leaf_input is not base64 has no leaf: the fold stops before it and tree->size says where.  tree->size + n must not wrap
+ * around 2^64 (CTMR_E_INVALID).  On an error *tree is left as it was passed in.  As with ctmr_process_raw, the batch's n
+ * global indices are taken after any failure, this one included, so that a retry does not reuse them. */
+int ctmr_process_raw_tree(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_out* out, ctmr_tree* tree);
+
+/* ctmr_process_tiles, and the batch's entries folded into *tree.  Before any work, with no index taken and *tree untouched
+ * (CTMR_E_INVALID otherwise): the tiles are consecutive (tile_index[t+1] == tile_index[t] + 1), every tile but the last is
+ * full (width 256), 256 * tile_index[0] <= tree->size <= 256 * tile_index[0] + tile_width[0], and the last leaf index fits
+ * 64 bits.  Leaves of the first tile below tree->size are already in the tree and are skipped.  A bad tile
+ * (CTMR_FE_BAD_TILE) stops the fold at its first leaf not yet in the tree; the rest of the batch is processed as usual.
+ * On the stop at an unknown Chain[0] (CTMR_E_UNKNOWN_ISSUER) *tree is written and holds the completed tiles.  Resume
+ * from tiles_done in one of two ways:
+ *   - tree->size >= 256 * tile_index[tiles_done]: no bad tile stopped the fold.  Call ctmr_process_tiles_tree again
+ *     with the same tree;
+ *   - tree->size is below that: a bad tile among the completed tiles stopped the fold, and the tree is final for this
+ *     batch.  Call ctmr_process_tiles for the rest; a tree call would fail the size rule above.
+ * Either way the tree and every output equal those of one call made with every certificate registered first.  On any
+ * other error *tree is left as it was passed in. */
+int ctmr_process_tiles_tree(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_tile_out* out, ctmr_tree* tree);
 
 #ifdef __cplusplus
 }

@@ -491,7 +491,8 @@ int ctmr_group_issuer_counts(ctmr_group* g, uint8_t* digests, uint64_t* counts, 
             take = k;
             if (counts) std::copy(part.begin(), part.begin() + k, counts);
         } else if (counts) {
-            // unsigned wrap-around on purpose: TTL eviction subtracts at the owner what the home rank added
+            // every shard counts the keys of the sets it owns (the owner resolves its own entries and its inbox records,
+            // receives the preloads and evicts its sets), so each part is exact and the sum is the group's count
             for (size_t i = 0; i < std::min(k, take); ++i) counts[i] += part[i];
         }
     }

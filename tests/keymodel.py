@@ -120,9 +120,10 @@ def decode_snapshot(snap: np.ndarray):
     return table, pairs
 
 
-def check_table(snap: np.ndarray, model: KeyModel, used: int | None = None):
-    """Every ready slot against the model; returns the number of slots checked."""
-    table, pairs = decode_snapshot(snap)
+def check_table(snap, model: KeyModel, used: int | None = None, owner=None):
+    """Every ready slot against the model; returns the number of slots checked.  `snap` is a ctx snapshot or one shard's
+    decoded (table, pairs); owner = (key_owner, world, rank): every key and pair must be one the shard owns."""
+    table, pairs = snap if isinstance(snap, tuple) else decode_snapshot(snap)
     mask = table.size - 1
     tags = table["tag"]
     ready = (tags & np.uint64(3)) == np.uint64(2)
@@ -133,6 +134,8 @@ def check_table(snap: np.ndarray, model: KeyModel, used: int | None = None):
         body = tuple(int(x) for x in table["body"][pos])
         h = key_hash(body)
         assert int(tags[pos]) == ready_tag(h), ("tag is not the restated hash", pos)
+        if owner is not None:
+            assert owner[0](body[0], body[1], owner[1]) == owner[2], ("key stored outside its owner's shard", pos, body[:2])
         assert body in model.first, ("slot holds a key no entry produced", pos, body)
         assert body not in seen, ("key stored twice", body)
         seen.add(body)
@@ -154,6 +157,8 @@ def check_table(snap: np.ndarray, model: KeyModel, used: int | None = None):
         k = int(p["key"]) - 1
         hk = (k & 0xFFFFFFFF, k >> 32)
         assert hk not in got, ("pair stored twice", hk)
+        if owner is not None:
+            assert owner[0](hk[0], hk[1], owner[1]) == owner[2], ("pair stored outside its owner's shard", pos, hk)
         got[hk] = int(p["count"])
         assert hk in model.pair_first, ("pair slot of a set no new certificate opened", pos, hk)
         assert (~int(p["inv_first"])) & M64 == model.pair_first[hk], ("pair first index", pos, hk)

@@ -138,7 +138,7 @@ struct FrontEnd {
     uint32_t unknown_cap = 0;
     unsigned int* unknown_count = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
-    cudaEvent_t mapped = nullptr, reduced = nullptr, meta_done = nullptr;  // round events of ctmr_group_process_raw
+    cudaEvent_t mapped = nullptr, reduced = nullptr, meta_done = nullptr;  // round events of the group front end (fe_member)
     float fe_ms = 0.f, path_ms = 0.f;
     uint64_t launches = 0;
     PemStage pem;
@@ -282,6 +282,7 @@ int run_round(const RoundMember* m, uint32_t W, int parity, uint64_t max_per_reg
 // D2H of entries [0, cnt) of device outputs to entries [lo, lo + cnt) of the caller's outputs: every per-entry array of
 // ctmr_out that both sides have, on stream s
 int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* out, uint64_t lo, cudaStream_t s);
+int group_fail(ctmr_group* g, ctmr_ctx* c, int rc);   // c's error becomes g's last error (when both are given); returns rc
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise

@@ -1,107 +1,63 @@
-// ctmr_frontend_api.cu -- the entry points of include/ctmr_frontend.h: get-entries strings -> base64 decode -> TLS framing ->
-// Chain[0] identification -> the path (SURVEY.md §8(f)-2), on one GPU (ctmr_process_raw) and on a group of GPUs driven by
-// one process (ctmr_group_process_raw); static-ct-api data tiles -> split -> framing -> Chain[0] by fingerprint -> the path
-// (ctmr_process_tiles, ctmr_group_process_tiles, ctmr_register_chain_certs).
+// ctmr_frontend_api.cu -- the entry points of include/ctmr_frontend.h (SURVEY.md §8(f)-2): get-entries strings -> base64
+// decode -> TLS framing -> Chain[0] identification -> the path (ctmr_process_raw); static-ct-api data tiles -> split ->
+// framing -> Chain[0] by fingerprint -> the path (ctmr_process_tiles, ctmr_register_chain_certs).  Each runs on one GPU, on
+// a group of GPUs driven by one process (ctmr_group_*), and on one GPU with the log's Merkle tree folded in
+// (ctmr_process_*_tree).
 //
-// A call is cut into CHUNKS (entry and character budgets of the front end's buffers).  Per chunk:
-//   upload   the chunk's characters and string spans, on a copy stream, into one of two upload stages -- chunk k+1's
-//            upload overlaps chunk k's kernels and the host round trips of its issuer identification;
-//   front    fe_decode / fe_frame / fe_tbs / fe_issuer: the decoded leaves stay in the arena, the chunk becomes a
-//            device-resident batch (ctmr_dev_batch with explicit lengths);
-//   path     K_map ... K_pairs over that batch in place -- ctmr_process_device on one GPU; on a group one ROUND of the key
+// One driver serves them all (process_members, over the members of the call: one ctx, or the members of a group).  A call
+// is cut into ROUNDS of one CHUNK per member (entry and character budgets of the front end's buffers).  Per round:
+//   upload   each chunk's characters and string spans (pages) or tile bytes (tiles), on a copy stream, into one of two
+//            upload stages -- round k+1's uploads overlap round k's kernels and the host round trips of its issuer
+//            identification;
+//   front    pages: fe_decode / fe_frame / fe_tbs / fe_issuer, the decoded leaves stay in the arena; tiles: tile_split /
+//            tile_frame / fe_tbs / tile_issuer, the leaves stay in the stage.  The chunk becomes a device-resident batch
+//            (ctmr_dev_batch with explicit lengths);
+//   path     K_map ... K_pairs over that batch in place -- ctmr_process_device on one GPU; on a group one round of the key
 //            exchange (run_round, ctmr_api.cu, with each member's chunk as its slice and its stream for everything):
 //            every member maps its chunk, hands foreign keys to their owners over NVLink, the owners reduce, the bits
 //            are pulled back;
 //   back     x509 leaf failures, PEM of the new certificates, outputs to the host.
-// On a group a round takes one chunk per member, cut from ONE contiguous window of the batch, so that entry i keeps
-// global index next_index + i and the result equals the single-GPU / sequential run on the same pages.
+// On one GPU a chunk is as large as the budgets allow.  On a group a round takes one chunk per member, cut from ONE
+// contiguous window of the batch, so that entry i keeps global index next_index + i and the result equals the
+// single-GPU run on the same input.  The two formats (Pages, Tiles) supply only what differs between them.
 #include <thread>
 
 #include "ctmr_ctx.cuh"
 
 namespace {
 
-struct RawChunk {
-    uint64_t lo = 0, hi = 0;      // entries of the caller's batch
-    uint64_t text_bytes = 0;      // characters uploaded for it
+// One member's chunk of a round: units [lo, hi) of the caller's batch (entries of pages, or tiles) and their entries
+// [e0, e1) (the same range for pages), from its upload to its back half.
+struct Chunk {
+    uint64_t lo = 0, hi = 0;
+    uint64_t e0 = 0, e1 = 0;
+    uint64_t bytes = 0;           // uploaded: the characters of pages, the tile bytes of tiles
     int stage = 0;                // upload stage it sits in
-    FeParams p{};
+    TileParams p{};               // the front end's kernel parameters; pages use p.fe only
     ctmr_dev_batch db{};
     ctmr_dev_out dout{};
+    bool stopped = false;         // tiles: holds the first tile with an unknown Chain[0] fingerprint; [lo, hi) cut before it
+    std::vector<std::array<uint8_t, 32>> missing;  // that tile's unknown fingerprints, sorted
+
+    // keeps the first `units` units, which hold `entries` entries
+    void cut(uint64_t units, uint64_t entries) {
+        hi = lo + units;
+        e1 = e0 + entries;
+        p.n_tiles = (uint32_t)units;
+        p.n = p.fe.n = db.n = entries;
+    }
 };
 
-// How many entries starting at `lo` fit one chunk (at most max_entries): entry budget and half the character budget
-// (the other half belongs to the stage being uploaded next).  Also validates the spans.
-int fe_fit(ctmr_ctx* c, const ctmr_raw_batch* b, uint64_t lo, uint64_t max_entries, uint64_t* hi_out) {
-    FrontEnd* f = c->fe;
-    uint64_t hi = lo, chars = 0;
-    while (hi < b->n && hi - lo < max_entries && hi - lo < f->cap_entries) {
-        const uint64_t l1 = b->leaf_input_off[hi] + b->leaf_input_len[hi], x1 = b->extra_data_off[hi] + b->extra_data_len[hi];
-        if (l1 > b->text_bytes || x1 > b->text_bytes) return fail(c, CTMR_E_INVALID, "string span outside the text buffer");
-        const uint64_t add = (uint64_t)b->leaf_input_len[hi] + b->extra_data_len[hi];
-        if (chars + add > f->cap_text / 2) break;
-        chars += add;
-        ++hi;
-    }
-    *hi_out = hi;
-    return CTMR_OK;
-}
+bool want_meta(const ctmr_out* o) { return o->first_issuer_dn || o->first_crldp || o->issuer_name_off || o->crldp_off; }
 
-// Characters and spans of entries [lo, hi) into upload stage `which`, asynchronously on the copy stream.
-int fe_upload(ctmr_ctx* c, const ctmr_raw_batch* b, RawChunk& ch) {
-    FrontEnd* f = c->fe;
-    FeStage& st = f->stage[ch.stage];
-    const uint64_t lo = ch.lo, cnt = ch.hi - ch.lo;
-    CU(c, cudaSetDevice(c->device));
-    CU(c, cudaStreamWaitEvent(f->copy_stream, st.consumed, 0));  // the decode that last read this stage has run
-    if (!cnt) {
-        ch.text_bytes = 0;
-        CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
-        return CTMR_OK;
-    }
-    uint64_t chars = 0, min_off = ~0ull, max_end = 0;
-    for (uint64_t i = lo; i < ch.hi; ++i) {
-        const uint64_t l0 = b->leaf_input_off[i], l1 = l0 + b->leaf_input_len[i];
-        const uint64_t x0 = b->extra_data_off[i], x1 = x0 + b->extra_data_len[i];
-        chars += (uint64_t)b->leaf_input_len[i] + b->extra_data_len[i];
-        min_off = std::min(min_off, std::min(l0, x0));
-        max_end = std::max(max_end, std::max(l1, x1));
-    }
-    std::memcpy(st.h_leaf_len, b->leaf_input_len + lo, cnt * 4);
-    std::memcpy(st.h_extra_len, b->extra_data_len + lo, cnt * 4);
-    if (max_end - min_off <= f->cap_text) {  // strings in place inside the response bodies: one copy
-        ch.text_bytes = max_end - min_off;
-        for (uint64_t i = 0; i < cnt; ++i) {
-            st.h_leaf_off[i] = b->leaf_input_off[lo + i] - min_off;
-            st.h_extra_off[i] = b->extra_data_off[lo + i] - min_off;
-        }
-        CU(c, cudaMemcpyAsync(st.text + 16, b->text + min_off, ch.text_bytes, cudaMemcpyHostToDevice, f->copy_stream));
-    } else {  // scattered: pack on the host first
-        st.pack.resize(chars);
-        uint64_t w = 0;
-        for (uint64_t i = 0; i < cnt; ++i) {
-            st.h_leaf_off[i] = w;
-            std::memcpy(st.pack.data() + w, b->text + b->leaf_input_off[lo + i], b->leaf_input_len[lo + i]);
-            w += b->leaf_input_len[lo + i];
-            st.h_extra_off[i] = w;
-            std::memcpy(st.pack.data() + w, b->text + b->extra_data_off[lo + i], b->extra_data_len[lo + i]);
-            w += b->extra_data_len[lo + i];
-        }
-        ch.text_bytes = w;
-        CU(c, cudaMemcpyAsync(st.text + 16, st.pack.data(), ch.text_bytes, cudaMemcpyHostToDevice, f->copy_stream));
-    }
-    CU(c, cudaMemcpyAsync(st.leaf_off, st.h_leaf_off, cnt * 8, cudaMemcpyHostToDevice, f->copy_stream));
-    CU(c, cudaMemcpyAsync(st.extra_off, st.h_extra_off, cnt * 8, cudaMemcpyHostToDevice, f->copy_stream));
-    CU(c, cudaMemcpyAsync(st.leaf_len, st.h_leaf_len, cnt * 4, cudaMemcpyHostToDevice, f->copy_stream));
-    CU(c, cudaMemcpyAsync(st.extra_len, st.h_extra_len, cnt * 4, cudaMemcpyHostToDevice, f->copy_stream));
-    CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
+int check_pem(ctmr_ctx* c, const ctmr_out* o) {
+    if ((o->pem != nullptr) != (o->pem_off != nullptr)) return fail(c, CTMR_E_INVALID, "pem and pem_off go together");
     return CTMR_OK;
 }
 
 // where the path writes a chunk's results: the front end's per-chunk buffers (sha256 and string identities when asked for)
 ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
     const uint64_t E = f->cap_entries;
-    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
     ctmr_dev_out dout{};
     dout.status = f->status;
     dout.sha256 = po->sha256 ? f->sha : nullptr;
@@ -110,7 +66,7 @@ ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
     dout.serial_len = f->serial_len;
     dout.was_unknown = f->was_unknown;
     dout.first_issuer_hour = f->first;
-    if (want_meta) {
+    if (want_meta(po)) {
         dout.issuer_name_off = f->spans;
         dout.issuer_name_len = f->spans + E;
         dout.crldp_off = f->spans + 2 * E;
@@ -120,6 +76,20 @@ ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
     }
     return dout;
 }
+
+// the front end's buffers on a member, and its counters of this call
+int fe_prepare(ctmr_ctx* c) {
+    CU(c, cudaSetDevice(c->device));
+    const int rc = frontend_ensure(c);
+    if (rc) return rc;
+    c->fe->fe_ms = c->fe->path_ms = 0.f;
+    c->fe->launches = 0;
+    return CTMR_OK;
+}
+
+// D2H of a chunk's device rows [0, cnt) of `per` bytes each to rows [lo, lo + cnt) of the caller's `dst`, if it asked for them
+#define CHUNK_D2H(dst, src, per) \
+    if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * (per), (src), cnt * (per), cudaMemcpyDeviceToHost, s))
 
 // ---- the log's Merkle tree (ctmr_process_raw_tree, ctmr_process_tiles_tree) ----------------------------------------------
 int tree_ensure(ctmr_ctx* c) {
@@ -175,19 +145,123 @@ int tree_end(ctmr_ctx* c, ctmr_tree* tree) {
 
 bool tree_active(const FrontEnd* f) { return f->tree && f->tree->active; }
 
+// ================================================================================================================
+// get-entries pages: the units of a chunk are entries.  The stage is free again once the chunk is decoded.
+// ================================================================================================================
+struct Pages {
+    static constexpr const char* kTooLarge = "a single entry exceeds the front end's character budget";
+    static constexpr bool kStageHoldsLeaves = false;
+    const ctmr_raw_batch* b;
+    ctmr_raw_out* out;
+    uint64_t done;  // entries that take their indices: all n whenever there is a batch, also when the call fails
+
+    Pages(const ctmr_raw_batch* b_, ctmr_raw_out* out_) : b(b_), out(out_), done(b_ ? b_->n : 0) {}
+    int check(ctmr_ctx* c, const ctmr_tree* tree) const;
+    uint64_t units() const { return b->n; }
+    uint64_t q_max(const ctmr_ctx* c) const { return c->fe->cap_entries; }
+    uint64_t tree_base(const ctmr_tree* tree) const { return tree->size; }
+    int prepare(ctmr_ctx* c) const { return fe_prepare(c); }
+    int fit(ctmr_ctx* c, uint64_t lo, uint64_t max_entries, uint64_t* hi_out) const;
+    int upload(ctmr_ctx* c, Chunk& ch) const;
+    int front(ctmr_ctx* c, Chunk& ch) const;
+    int copy_back(ctmr_ctx* c, const Chunk& ch) const;
+    void completed(uint64_t) const {}
+    int stop(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }  // a page chunk never stops
+};
+
+// tree: ctmr_process_raw_tree's rule as well
+int Pages::check(ctmr_ctx* c, const ctmr_tree* tree) const {
+    if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (b->n && (!b->text || !b->leaf_input_off || !b->leaf_input_len || !b->extra_data_off || !b->extra_data_len))
+        return fail(c, CTMR_E_INVALID, "null batch buffers");
+    const int rc = check_pem(c, &out->path);
+    if (rc) return rc;
+    if (tree && b->n > ~0ull - tree->size) return fail(c, CTMR_E_INVALID, "tree size + entries wraps around 2^64");
+    return CTMR_OK;
+}
+
+// How many entries starting at `lo` fit one chunk (at most max_entries): entry budget and half the character budget
+// (the other half belongs to the stage being uploaded next).  Also validates the spans.
+int Pages::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_entries, uint64_t* hi_out) const {
+    FrontEnd* f = c->fe;
+    uint64_t hi = lo, chars = 0;
+    while (hi < b->n && hi - lo < max_entries && hi - lo < f->cap_entries) {
+        const uint64_t l1 = b->leaf_input_off[hi] + b->leaf_input_len[hi], x1 = b->extra_data_off[hi] + b->extra_data_len[hi];
+        if (l1 > b->text_bytes || x1 > b->text_bytes) return fail(c, CTMR_E_INVALID, "string span outside the text buffer");
+        const uint64_t add = (uint64_t)b->leaf_input_len[hi] + b->extra_data_len[hi];
+        if (chars + add > f->cap_text / 2) break;
+        chars += add;
+        ++hi;
+    }
+    *hi_out = hi;
+    return CTMR_OK;
+}
+
+// Characters and spans of entries [lo, hi) into upload stage ch.stage, asynchronously on the copy stream.
+int Pages::upload(ctmr_ctx* c, Chunk& ch) const {
+    FrontEnd* f = c->fe;
+    FeStage& st = f->stage[ch.stage];
+    const uint64_t lo = ch.lo, cnt = ch.hi - ch.lo;
+    ch.e0 = ch.lo;
+    ch.e1 = ch.hi;
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaStreamWaitEvent(f->copy_stream, st.consumed, 0));  // the decode that last read this stage has run
+    if (!cnt) {
+        ch.bytes = 0;
+        CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
+        return CTMR_OK;
+    }
+    uint64_t chars = 0, min_off = ~0ull, max_end = 0;
+    for (uint64_t i = lo; i < ch.hi; ++i) {
+        const uint64_t l0 = b->leaf_input_off[i], l1 = l0 + b->leaf_input_len[i];
+        const uint64_t x0 = b->extra_data_off[i], x1 = x0 + b->extra_data_len[i];
+        chars += (uint64_t)b->leaf_input_len[i] + b->extra_data_len[i];
+        min_off = std::min(min_off, std::min(l0, x0));
+        max_end = std::max(max_end, std::max(l1, x1));
+    }
+    std::memcpy(st.h_leaf_len, b->leaf_input_len + lo, cnt * 4);
+    std::memcpy(st.h_extra_len, b->extra_data_len + lo, cnt * 4);
+    if (max_end - min_off <= f->cap_text) {  // strings in place inside the response bodies: one copy
+        ch.bytes = max_end - min_off;
+        for (uint64_t i = 0; i < cnt; ++i) {
+            st.h_leaf_off[i] = b->leaf_input_off[lo + i] - min_off;
+            st.h_extra_off[i] = b->extra_data_off[lo + i] - min_off;
+        }
+        CU(c, cudaMemcpyAsync(st.text + 16, b->text + min_off, ch.bytes, cudaMemcpyHostToDevice, f->copy_stream));
+    } else {  // scattered: pack on the host first
+        st.pack.resize(chars);
+        uint64_t w = 0;
+        for (uint64_t i = 0; i < cnt; ++i) {
+            st.h_leaf_off[i] = w;
+            std::memcpy(st.pack.data() + w, b->text + b->leaf_input_off[lo + i], b->leaf_input_len[lo + i]);
+            w += b->leaf_input_len[lo + i];
+            st.h_extra_off[i] = w;
+            std::memcpy(st.pack.data() + w, b->text + b->extra_data_off[lo + i], b->extra_data_len[lo + i]);
+            w += b->extra_data_len[lo + i];
+        }
+        ch.bytes = w;
+        CU(c, cudaMemcpyAsync(st.text + 16, st.pack.data(), ch.bytes, cudaMemcpyHostToDevice, f->copy_stream));
+    }
+    CU(c, cudaMemcpyAsync(st.leaf_off, st.h_leaf_off, cnt * 8, cudaMemcpyHostToDevice, f->copy_stream));
+    CU(c, cudaMemcpyAsync(st.extra_off, st.h_extra_off, cnt * 8, cudaMemcpyHostToDevice, f->copy_stream));
+    CU(c, cudaMemcpyAsync(st.leaf_len, st.h_leaf_len, cnt * 4, cudaMemcpyHostToDevice, f->copy_stream));
+    CU(c, cudaMemcpyAsync(st.extra_len, st.h_extra_len, cnt * 4, cudaMemcpyHostToDevice, f->copy_stream));
+    CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
+    return CTMR_OK;
+}
+
 // decode + frame + Chain[0] -> dense index of an uploaded chunk; leaves ch.db / ch.dout describing the device-resident batch
-int fe_front(ctmr_ctx* c, const ctmr_raw_batch* b, const ctmr_raw_out* out, RawChunk& ch, uint64_t first_index) {
+int Pages::front(ctmr_ctx* c, Chunk& ch) const {
     FrontEnd* f = c->fe;
     cudaStream_t s = c->stream;
     CU(c, cudaSetDevice(c->device));
     FeStage& st = f->stage[ch.stage];
     const uint64_t cnt = ch.hi - ch.lo;
-    const ctmr_out* po = &out->path;
     CU(c, cudaStreamWaitEvent(s, st.uploaded, 0));
-    FeParams& p = ch.p;
+    FeParams& p = ch.p.fe;
     p = FeParams{};
     p.text = st.text + 16;
-    p.text_bytes = ch.text_bytes;
+    p.text_bytes = ch.bytes;
     p.leaf_off = st.leaf_off; p.leaf_len = st.leaf_len; p.extra_off = st.extra_off; p.extra_len = st.extra_len;
     p.n = cnt;
     p.pad_size = f->pad_size; p.dec_off = f->dec_off; p.dec_len = f->dec_len; p.str_bad = f->str_bad; p.decoded = f->decoded;
@@ -260,295 +334,76 @@ int fe_front(ctmr_ctx* c, const ctmr_raw_batch* b, const ctmr_raw_out* out, RawC
     db.lens = f->leaf_len_out;
     db.n = cnt;
     db.issuer_idx = f->issuer_idx;
-    db.first_index = first_index;
     db.now_unix_ns = b->now_unix_ns;
-    ch.dout = chunk_path_out(f, po);
+    ch.dout = chunk_path_out(f, &out->path);
     return CTMR_OK;
 }
 
-// after the path: x509 leaf failures, PEM, outputs to the host; waits for the chunk
-int fe_back(ctmr_ctx* c, const ctmr_raw_out* out, RawChunk& ch, uint64_t* pem_base) {
+// the front end's own outputs of a chunk, after the path's; waits for the chunk
+int Pages::copy_back(ctmr_ctx* c, const Chunk& ch) const {
     FrontEnd* f = c->fe;
     cudaStream_t s = c->stream;
-    CU(c, cudaSetDevice(c->device));
-    const uint64_t cnt = ch.hi - ch.lo, lo = ch.lo, E = f->cap_entries;
-    const ctmr_out* po = &out->path;
-    const bool want_pem = po->pem != nullptr;
-    if (!cnt) {
-        CU(c, cudaStreamSynchronize(s));
-        return CTMR_OK;
+    const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0;
+    if (cnt) {
+        CHUNK_D2H(out->entry_status, f->entry_status, 1);
+        CHUNK_D2H(out->entry_type, f->entry_type, 1);
+        CHUNK_D2H(out->timestamp_ms, f->timestamp, 8);
+        CHUNK_D2H(out->issuer, f->issuer_idx, 4);
+        CHUNK_D2H(out->leaf_src, f->leaf_src, 1);
+        CHUNK_D2H(out->leaf_off, f->leaf_rel, 4);
+        CHUNK_D2H(out->leaf_len, f->leaf_len_out, 4);
     }
-    CU(c, launch_fe_finish(ch.p, f->status, s));
-    ++f->launches;
-    CU(c, cudaEventRecord(f->ev2, s));
-    if (want_pem) {  // the decoded DER exists only on the device: its PEM is how new certificates reach the host
-        int rc = pem_ensure(c, f->pem, E, f->cap_decoded);
-        if (rc) return rc;
-        rc = pem_chunk(c, f->pem, f->decoded, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, lo, pem_base, s);
-        if (rc) return rc;
-    }
-    const int rc = copy_out(c, ch.dout, cnt, po, lo, s);
-    if (rc) return rc;
-#define FE_D2H(dst, src, bytes) \
-    if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * ((bytes) / cnt), (src), (bytes), cudaMemcpyDeviceToHost, s))
-    FE_D2H(out->entry_status, f->entry_status, cnt);
-    FE_D2H(out->entry_type, f->entry_type, cnt);
-    FE_D2H(out->timestamp_ms, f->timestamp, cnt * 8);
-    FE_D2H(out->issuer, f->issuer_idx, cnt * 4);
-    FE_D2H(out->leaf_src, f->leaf_src, cnt);
-    FE_D2H(out->leaf_off, f->leaf_rel, cnt * 4);
-    FE_D2H(out->leaf_len, f->leaf_len_out, cnt * 4);
-#undef FE_D2H
     CU(c, cudaStreamSynchronize(s));
-    float a = 0.f, d = 0.f;
-    CU(c, cudaEventElapsedTime(&a, f->ev0, f->ev1));
-    CU(c, cudaEventElapsedTime(&d, f->ev1, f->ev2));
-    f->fe_ms += a;
-    f->path_ms += d;
-    return CTMR_OK;
-}
-
-int check_args(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out) {
-    if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
-    if (b->n && (!b->text || !b->leaf_input_off || !b->leaf_input_len || !b->extra_data_off || !b->extra_data_len))
-        return fail(c, CTMR_E_INVALID, "null batch buffers");
-    if ((out->path.pem != nullptr) != (out->path.pem_off != nullptr)) return fail(c, CTMR_E_INVALID, "pem and pem_off go together");
-    return CTMR_OK;
-}
-
-// tree: fold the entries into it too (ctmr_process_raw_tree), written back only when the call succeeds
-int process_raw_single(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree = nullptr) {
-    int rc = check_args(c, b, out);
-    if (rc) return rc;
-    if (tree && b->n > ~0ull - tree->size) return fail(c, CTMR_E_INVALID, "tree size + entries wraps around 2^64");
-    if (b->n == 0 && !tree) return CTMR_OK;
-    CU(c, cudaSetDevice(c->device));
-    rc = frontend_ensure(c);
-    if (rc) return rc;
-    FrontEnd* f = c->fe;
-    f->fe_ms = f->path_ms = 0.f;
-    f->launches = 0;
-    if (tree) {
-        rc = tree_begin(c, tree, tree->size);
-        if (rc) return rc;
-        if (b->n == 0) return tree_end(c, tree);
-    }
-    uint64_t pem_base = 0;
-    RawChunk ch[2];
-    rc = fe_fit(c, b, 0, ~0ull, &ch[0].hi);
-    if (rc) return rc;
-    if (ch[0].hi == 0) return fail(c, CTMR_E_BATCH_TOO_LARGE, "a single entry exceeds the front end's character budget");
-    rc = fe_upload(c, b, ch[0]);
-    if (rc) return rc;
-    for (int k = 0;; ++k) {
-        RawChunk& cur = ch[k & 1];
-        if (cur.hi < b->n) {  // next chunk's upload overlaps this chunk's kernels
-            RawChunk& nx = ch[(k + 1) & 1];
-            nx = RawChunk{};
-            nx.lo = cur.hi;
-            nx.stage = (k + 1) & 1;
-            rc = fe_fit(c, b, nx.lo, ~0ull, &nx.hi);
-            if (rc) return rc;
-            if (nx.hi == nx.lo) return fail(c, CTMR_E_BATCH_TOO_LARGE, "a single entry exceeds the front end's character budget");
-            rc = fe_upload(c, b, nx);
-            if (rc) return rc;
-        }
-        rc = fe_front(c, b, out, cur, c->next_index + cur.lo);
-        if (rc) return rc;
-        rc = ctmr_process_device(c, &cur.db, &cur.dout, c->stream);
-        if (rc) return rc;
-        rc = fe_back(c, out, cur, &pem_base);
-        if (rc) return rc;
-        if (cur.hi >= b->n) break;
-    }
-    if (out->path.pem) out->path.pem_off[b->n] = pem_base;
-    rc = ctmr_check_device(c, nullptr);
-    return rc || !tree ? rc : tree_end(c, tree);
-}
-
-// fn(r) for every member, on one thread each (the halves of a chunk wait on the host: issuer round trips, D2H); sequential if
-// threads cannot be had.  No exception leaves this function (C ABI).
-template <class F>
-void for_each_member(uint32_t W, std::vector<int>& rcs, F fn) {
-    rcs.assign(W, CTMR_OK);
-    std::vector<std::thread> th;
-    uint32_t started = 0;
-    try {
-        for (; started < W; ++started) th.emplace_back([&rcs, &fn, r = started] { rcs[r] = fn(r); });
-    } catch (...) {
-    }
-    for (std::thread& t : th) t.join();
-    for (uint32_t r = started; r < W; ++r) rcs[r] = fn(r);
-}
-
-// A member's device-resident chunk as its part of round `parity` (run_round).  Everything runs on the member's stream,
-// so there is no chain: the back half waits for each round before the next is issued.
-int fe_member(ctmr_ctx* c, const ctmr_dev_batch& db, const ctmr_dev_out& dout, int parity, RoundMember& x) {
-    CU(c, cudaSetDevice(c->device));
-    int rc = ensure_scratch(c, std::max<uint64_t>(db.n, 1));
-    if (rc == CTMR_OK) rc = ensure_order(c, db.n);
-    if (rc) return rc;
-    x = RoundMember{};
-    x.c = c;
-    x.db = db;
-    x.dout = dout;
-    x.dout.keys = c->keys_scratch;
-    x.slot_of = c->slot_scratch; x.pair_slot = c->pair_scratch; x.order = c->order_scratch; x.len_hist = c->len_hist;
-    x.meta_slots = c->meta_scratch;
-    x.map_stream = x.reduce_stream = c->stream;
-    x.mapped = c->fe->mapped; x.reduced = c->fe->reduced; x.meta_done = c->fe->meta_done;
-    // the members of an in-process group meet through their events; peer_barrier does nothing for them
-    x.ch_map = CH_STAGE_MAP + parity;
-    x.ch_resolve = CH_STAGE_RESOLVE + parity;
-    x.ch_meta = CH_STAGE_META + parity;
-    return CTMR_OK;
-}
-
-// Cut the next round out of a batch of `total` units (entries, or tiles) starting at `pos`: one chunk per member from ONE
-// contiguous window, q units each, q halved until every member's chunk fits (fit(c, lo, want, &hi) says how far a
-// chunk starting at lo gets), then each chunk's upload is issued (upload(c, chunk)).
-template <class Chunk, class Fit, class Upload>
-int plan_round(ctmr_group* g, uint64_t total, uint64_t q_max, uint64_t pos, int stage, std::vector<Chunk>& ch, ctmr_ctx** failed,
-               const char* too_large, Fit fit, Upload upload) {
-    const uint32_t W = (uint32_t)g->m.size();
-    ctmr_ctx* c0 = g->m[0];
-    *failed = c0;
-    uint64_t q = std::max<uint64_t>(1, std::min<uint64_t>(q_max, (total - pos + W - 1) / W));
-    for (;;) {
-        bool fits = true;
-        for (uint32_t r = 0; r < W && fits; ++r) {
-            const uint64_t lo = std::min(total, pos + r * q), want = std::min(total, pos + (r + 1) * q);
-            uint64_t hi = 0;
-            int rc = fit(g->m[r], lo, want - lo, &hi);
-            if (rc) {
-                *failed = g->m[r];
-                return rc;
-            }
-            fits = hi == want;
-        }
-        if (fits) break;
-        if (q == 1) return fail(c0, CTMR_E_BATCH_TOO_LARGE, too_large);
-        q = (q + 1) / 2;
-    }
-    ch.assign(W, Chunk{});
-    for (uint32_t r = 0; r < W; ++r) {
-        ch[r].lo = std::min(total, pos + r * q);
-        ch[r].hi = std::min(total, pos + (r + 1) * q);
-        ch[r].stage = stage;
-        *failed = g->m[r];
-        int rc = upload(g->m[r], ch[r]);
-        if (rc) return rc;
-    }
-    *failed = nullptr;
-    return CTMR_OK;
-}
-
-int plan_raw_round(ctmr_group* g, const ctmr_raw_batch* b, uint64_t pos, int stage, std::vector<RawChunk>& ch, ctmr_ctx** failed) {
-    return plan_round(
-        g, b->n, g->m[0]->fe->cap_entries, pos, stage, ch, failed, "a single entry exceeds the front end's character budget",
-        [b](ctmr_ctx* c, uint64_t lo, uint64_t want, uint64_t* hi) { return fe_fit(c, b, lo, want, hi); },
-        [b](ctmr_ctx* c, RawChunk& x) { return fe_upload(c, b, x); });
-}
-
-int process_raw_group(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_ctx** failed) {
-    const uint32_t W = (uint32_t)g->m.size();
-    ctmr_ctx* c0 = g->m[0];
-    *failed = c0;
-    int rc = check_args(c0, b, out);
-    if (rc) return rc;
-    if (b->n == 0) return CTMR_OK;
-    for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = g->m[r];
-        *failed = c;
-        CU(c, cudaSetDevice(c->device));
-        rc = frontend_ensure(c);
-        if (rc) return rc;
-        c->fe->fe_ms = c->fe->path_ms = 0.f;
-        c->fe->launches = 0;
-    }
-    const ctmr_out* po = &out->path;
-    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
-    uint64_t pem_base = 0, pos = 0;
-    std::vector<RawChunk> cur, nxt;
-    rc = plan_raw_round(g, b, 0, 0, cur, failed);
-    if (rc) return rc;
-    for (int k = 0;; ++k) {
-        const uint64_t end = cur[W - 1].hi;
-        if (end < b->n) {  // the next round's uploads overlap this round's kernels and host round trips
-            rc = plan_raw_round(g, b, end, (k + 1) & 1, nxt, failed);
-            if (rc) return rc;
-        }
-        // The front halves wait on the host (issuer identification round trips, the arena size): one thread per member, so
-        // that the members' waits overlap instead of adding up.  Each thread touches its own ctx only; the issuer registry
-        // they all resolve against is device memory reached with atomics.
-        std::vector<int> rcs;
-        for_each_member(W, rcs, [&](uint32_t r) { return fe_front(g->m[r], b, out, cur[r], g->next_index + cur[r].lo); });
-        for (uint32_t r = 0; r < W; ++r)
-            if (rcs[r]) {
-                *failed = g->m[r];
-                return rcs[r];
-            }
-        const int parity = k % (int)kParities;
-        RoundMember rm[kMaxWorld];
-        for (uint32_t r = 0; r < W; ++r) {
-            *failed = g->m[r];
-            rc = fe_member(g->m[r], cur[r].db, cur[r].dout, parity, rm[r]);
-            if (rc) return rc;
-        }
-        rc = run_round(rm, W, parity, c0->fe->cap_entries, want_meta, failed);
-        if (rc) return rc;
-        if (out->path.pem) {
-            for (uint32_t r = 0; r < W; ++r) {  // in entry order: the PEM texts are appended in that order
-                *failed = g->m[r];
-                rc = fe_back(g->m[r], out, cur[r], &pem_base);
-                if (rc) return rc;
-            }
-        } else {  // disjoint output ranges: the members' copies and waits overlap as well
-            for_each_member(W, rcs, [&](uint32_t r) { return fe_back(g->m[r], out, cur[r], &pem_base); });
-            for (uint32_t r = 0; r < W; ++r)
-                if (rcs[r]) {
-                    *failed = g->m[r];
-                    return rcs[r];
-                }
-        }
-        pos = end;
-        if (end >= b->n) break;
-        cur.swap(nxt);
-    }
-    (void)pos;
-    if (out->path.pem) out->path.pem_off[b->n] = pem_base;
-    for (uint32_t r = 0; r < W; ++r) {
-        *failed = g->m[r];
-        rc = ctmr_check_device(g->m[r], nullptr);
-        if (rc) return rc;
-    }
-    *failed = nullptr;
     return CTMR_OK;
 }
 
 // ================================================================================================================
-// static-ct-api data tiles (ctmr_process_tiles).  The same chunk / upload / front / path / back structure as above, with
-// chunks cut on tile boundaries.  The uploaded tile bytes ARE the path's input: K_map reads the leaves where the upload
-// put them, so the stage stays busy until the chunk's back half has run.
+// static-ct-api data tiles: the units of a chunk are tiles.  The uploaded tile bytes ARE the path's input: K_map reads
+// the leaves where the upload put them, so the stage stays busy until the chunk's PEM has been encoded.
 // ================================================================================================================
-struct TileChunk {
-    uint64_t lo = 0, hi = 0;      // tiles of the caller's batch
-    uint64_t e0 = 0, e1 = 0;      // their entries
-    uint64_t bytes = 0;           // tile bytes uploaded
-    int stage = 0;
-    TileParams p{};
-    ctmr_dev_batch db{};
-    ctmr_dev_out dout{};
-    bool stopped = false;         // holds the first tile with an unknown Chain[0] fingerprint; [lo, hi) cut before it
-    std::vector<std::array<uint8_t, 32>> missing;  // that tile's unknown fingerprints, sorted
+struct Tiles {
+    static constexpr const char* kTooLarge = "a single tile exceeds the front end's staging budget";
+    static constexpr bool kStageHoldsLeaves = true;
+    const ctmr_tile_batch* b;
+    ctmr_tile_out* out;
+    uint64_t done = 0;         // entries that take their indices: none when the arguments fail, those before a stop, else all
+    std::vector<uint64_t> ent;  // entries before each tile: ent[t] = sum of widths of tiles [0, t)
+
+    Tiles(const ctmr_tile_batch* b_, ctmr_tile_out* out_) : b(b_), out(out_) {}
+    int check(ctmr_ctx* c, const ctmr_tree* tree);
+    uint64_t units() const { return b->n_tiles; }
+    uint64_t q_max(const ctmr_ctx*) const { return ~0ull; }  // fit keeps a chunk inside the entry budget
+    uint64_t tree_base(const ctmr_tree*) const { return b->n_tiles ? 256 * b->tile_index[0] : 0; }
+    int prepare(ctmr_ctx* c) const;
+    int fit(ctmr_ctx* c, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) const;
+    int upload(ctmr_ctx* c, Chunk& ch) const;
+    int front(ctmr_ctx* c, Chunk& ch) const;
+    int copy_back(ctmr_ctx* c, const Chunk& ch) const;
+    void completed(uint64_t tiles) const { out->tiles_done = tiles; }
+    int stop(ctmr_ctx* c, const Chunk& ch) const;
 };
 
-// entries before each tile: ent[t] = sum of widths of tiles [0, t); validates widths and spans
-int tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, std::vector<uint64_t>& ent) {
+// ctmr_process_tiles_tree's rules for the tiles of one log, checked before any work like the widths and spans
+int tree_tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tree* tree, uint64_t n) {
+    if (b->n_tiles == 0) return CTMR_OK;
+    if (b->tile_index[0] > (~0ull - n) >> 8) return fail(c, CTMR_E_INVALID, "tree: the batch's last leaf index does not fit 64 bits");
+    for (uint64_t t = 0; t + 1 < b->n_tiles; ++t) {
+        if (b->tile_index[t + 1] != b->tile_index[t] + 1) return fail(c, CTMR_E_INVALID, "tree: tiles are not consecutive");
+        if (b->tile_width[t] != 256) return fail(c, CTMR_E_INVALID, "tree: a partial tile that is not the last");
+    }
+    const uint64_t first = 256 * b->tile_index[0];
+    if (tree->size < first || tree->size > first + b->tile_width[0])
+        return fail(c, CTMR_E_INVALID, "tree: size is not inside the batch's first tile");
+    return CTMR_OK;
+}
+
+// validates widths and spans (and with a tree its rules), fills ent
+int Tiles::check(ctmr_ctx* c, const ctmr_tree* tree) {
     if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n_tiles && (!b->data || !b->tile_off || !b->tile_len || !b->tile_index || !b->tile_width))
         return fail(c, CTMR_E_INVALID, "null batch buffers");
-    if ((out->path.pem != nullptr) != (out->path.pem_off != nullptr)) return fail(c, CTMR_E_INVALID, "pem and pem_off go together");
+    int rc = check_pem(c, &out->path);
+    if (rc) return rc;
     if (out->missing_cap && !out->missing_fp) return fail(c, CTMR_E_INVALID, "missing_cap without missing_fp");
     ent.assign(b->n_tiles + 1, 0);
     for (uint64_t t = 0; t < b->n_tiles; ++t) {
@@ -557,11 +412,26 @@ int tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, s
             return fail(c, CTMR_E_INVALID, "tile outside the data buffer");
         ent[t + 1] = ent[t] + b->tile_width[t];
     }
+    if (tree) {
+        rc = tree_tile_args(c, b, tree, ent[b->n_tiles]);
+        if (rc) return rc;
+    }
+    done = ent[b->n_tiles];
+    out->tiles_done = 0;
+    out->n_missing = 0;
+    return CTMR_OK;
+}
+
+int Tiles::prepare(ctmr_ctx* c) const {
+    int rc = fe_prepare(c);
+    if (rc == CTMR_OK) rc = tiles_ensure(c);
+    if (rc) return rc;
+    c->fe->tl->split_ms = 0.f;
     return CTMR_OK;
 }
 
 // How many tiles starting at `lo` fit one chunk (at most max_tiles): the entry budget and half the byte budget
-int tile_fit(ctmr_ctx* c, const ctmr_tile_batch* b, const std::vector<uint64_t>& ent, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) {
+int Tiles::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) const {
     FrontEnd* f = c->fe;
     uint64_t hi = lo, bytes = 0;
     while (hi < b->n_tiles && hi - lo < max_tiles && ent[hi + 1] - ent[lo] <= f->cap_entries && bytes + b->tile_len[hi] <= f->cap_text / 2) {
@@ -573,7 +443,7 @@ int tile_fit(ctmr_ctx* c, const ctmr_tile_batch* b, const std::vector<uint64_t>&
 }
 
 // tiles [lo, hi) into upload stage ch.stage, asynchronously on the copy stream
-int tile_upload(ctmr_ctx* c, const ctmr_tile_batch* b, const std::vector<uint64_t>& ent, TileChunk& ch) {
+int Tiles::upload(ctmr_ctx* c, Chunk& ch) const {
     FrontEnd* f = c->fe;
     TileState* tl = f->tl;
     FeStage& st = f->stage[ch.stage];
@@ -619,7 +489,7 @@ int tile_upload(ctmr_ctx* c, const ctmr_tile_batch* b, const std::vector<uint64_
 
 // split + frame + fingerprint -> dense index of an uploaded chunk.  A chunk holding a tile with an unknown Chain[0]
 // fingerprint is cut before that tile (ch.stopped, ch.missing).  Leaves ch.db / ch.dout describing the device-resident batch.
-int tile_front(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, TileChunk& ch) {
+int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
     FrontEnd* f = c->fe;
     TileState* tl = f->tl;
     cudaStream_t s = c->stream;
@@ -679,10 +549,7 @@ int tile_front(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, 
             std::sort(ch.missing.begin(), ch.missing.end());
             ch.missing.erase(std::unique(ch.missing.begin(), ch.missing.end()), ch.missing.end());
             ch.stopped = true;
-            ch.hi = ch.lo + stop;
-            ch.e1 = ch.e0 + td.first;
-            p.n_tiles = stop;
-            p.n = q.n = td.first;
+            ch.cut(stop, td.first);
         }
         if (p.n && tree_active(f)) {  // the completed tiles' leaves into the tree; a bad tile has none
             const int rc = tree_fold(c, tl->leaf_hash, f->entry_status, 1, CTMR_FE_BAD_TILE, f->tree->base + ch.e0, p.n);
@@ -702,47 +569,180 @@ int tile_front(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tile_out* out, 
     return CTMR_OK;
 }
 
-// after the path: x509 leaf failures, PEM, outputs to the host; waits for the chunk and releases its stage
-int tile_back(ctmr_ctx* c, const ctmr_tile_out* out, TileChunk& ch, uint64_t* pem_base) {
+// the front end's own outputs of a chunk, after the path's; waits for the chunk
+int Tiles::copy_back(ctmr_ctx* c, const Chunk& ch) const {
     FrontEnd* f = c->fe;
     TileState* tl = f->tl;
     cudaStream_t s = c->stream;
-    CU(c, cudaSetDevice(c->device));
-    FeStage& st = f->stage[ch.stage];
-    const uint64_t cnt = ch.e1 - ch.e0, lo = ch.e0, nt = ch.hi - ch.lo;
-    const ctmr_out* po = &out->path;
-    if (cnt) {
-        CU(c, launch_fe_finish(ch.p.fe, f->status, s));
-        ++f->launches;
-    }
-    CU(c, cudaEventRecord(f->ev2, s));
-    if (cnt && po->pem) {
-        int rc = pem_ensure(c, f->pem, f->cap_entries, f->cap_decoded);
-        if (rc) return rc;
-        rc = pem_chunk(c, f->pem, ch.p.data, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, lo, pem_base, s);
-        if (rc) return rc;
-    }
-    CU(c, cudaEventRecord(st.consumed, s));  // the leaves in the stage have been read for the last time
+    const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0, nt = ch.hi - ch.lo;
     std::vector<uint8_t> bad(nt);
     if (cnt) {
-        const int rc = copy_out(c, ch.dout, cnt, po, lo, s);
-        if (rc) return rc;
-#define TL_D2H(dst, src, per) \
-    if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * (per), (src), cnt * (per), cudaMemcpyDeviceToHost, s))
-        TL_D2H(out->entry_status, f->entry_status, 1);
-        TL_D2H(out->entry_type, f->entry_type, 1);
-        TL_D2H(out->timestamp_ms, f->timestamp, 8);
-        TL_D2H(out->issuer, f->issuer_idx, 4);
-        TL_D2H(out->leaf_index, tl->leaf_index, 8);
-        TL_D2H(out->leaf_off, tl->leaf_data_off, 8);
-        TL_D2H(out->leaf_len, f->leaf_len_out, 4);
-        TL_D2H(out->leaf_hash, tl->leaf_hash, 32);
-#undef TL_D2H
+        CHUNK_D2H(out->entry_status, f->entry_status, 1);
+        CHUNK_D2H(out->entry_type, f->entry_type, 1);
+        CHUNK_D2H(out->timestamp_ms, f->timestamp, 8);
+        CHUNK_D2H(out->issuer, f->issuer_idx, 4);
+        CHUNK_D2H(out->leaf_index, tl->leaf_index, 8);
+        CHUNK_D2H(out->leaf_off, tl->leaf_data_off, 8);
+        CHUNK_D2H(out->leaf_len, f->leaf_len_out, 4);
+        CHUNK_D2H(out->leaf_hash, tl->leaf_hash, 32);
         if (out->tile_status) CU(c, cudaMemcpyAsync(bad.data(), tl->tile_bad, nt, cudaMemcpyDeviceToHost, s));
     }
     CU(c, cudaStreamSynchronize(s));
     if (out->tile_status)
         for (uint64_t i = 0; i < nt; ++i) out->tile_status[ch.lo + i] = bad[i] ? CTMR_FE_BAD_TILE : CTMR_FE_OK;
+    return CTMR_OK;
+}
+
+// the stop: the unknown fingerprints, and the call's result code
+int Tiles::stop(ctmr_ctx* c, const Chunk& ch) const {
+    out->n_missing = (uint32_t)std::min<size_t>(ch.missing.size(), out->missing_cap);
+    for (uint32_t i = 0; i < out->n_missing; ++i) std::memcpy(out->missing_fp + 32ull * i, ch.missing[i].data(), 32);
+    return fail(c, CTMR_E_UNKNOWN_ISSUER, "tile " + std::to_string(ch.hi) + " names a Chain[0] fingerprint that is not registered "
+                                          "(ctmr_register_chain_certs, then call again from tiles_done)");
+}
+
+#undef CHUNK_D2H
+
+// ================================================================================================================
+// the driver
+// ================================================================================================================
+
+// fn(r) for every member: in member order, or with `threads` on one thread each (the halves of a chunk wait on the host:
+// issuer round trips, D2H), in order if threads cannot be had.  Returns the error of the first member in member order
+// that failed, and names it in *failed.  No exception leaves this function (C ABI).
+template <class F>
+int for_each_member(ctmr_ctx** m, uint32_t W, bool threads, ctmr_ctx** failed, F fn) {
+    std::vector<int> rcs(W, CTMR_OK);
+    std::vector<std::thread> th;
+    uint32_t started = 0;
+    if (threads) {
+        try {
+            for (; started < W; ++started) th.emplace_back([&rcs, &fn, r = started] { rcs[r] = fn(r); });
+        } catch (...) {
+        }
+        for (std::thread& t : th) t.join();
+    }
+    for (uint32_t r = started; r < W; ++r)
+        if ((rcs[r] = fn(r)) != CTMR_OK) break;
+    for (uint32_t r = 0; r < W; ++r)
+        if (rcs[r]) {
+            *failed = m[r];
+            return rcs[r];
+        }
+    return CTMR_OK;
+}
+
+// Cuts the round that starts at unit `pos` and issues its uploads into stage `stage`.  One member takes the greedy chunk
+// fit returns.  A group takes one chunk per member from ONE contiguous window, q units each, q halved until every
+// member's chunk fits.
+template <class Format>
+int plan_round(ctmr_ctx** m, uint32_t W, const Format& fm, uint64_t pos, int stage, std::vector<Chunk>& ch, ctmr_ctx** failed) {
+    const uint64_t total = fm.units();
+    *failed = m[0];
+    uint64_t q = 0;
+    if (W == 1) {
+        uint64_t hi = 0;
+        const int rc = fm.fit(m[0], pos, ~0ull, &hi);
+        if (rc) return rc;
+        if (hi == pos) return fail(m[0], CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
+        q = hi - pos;
+    } else {
+        q = std::max<uint64_t>(1, std::min<uint64_t>(fm.q_max(m[0]), (total - pos + W - 1) / W));
+        for (;;) {
+            bool fits = true;
+            for (uint32_t r = 0; r < W && fits; ++r) {
+                const uint64_t lo = std::min(total, pos + r * q), want = std::min(total, pos + (r + 1) * q);
+                uint64_t hi = 0;
+                const int rc = fm.fit(m[r], lo, want - lo, &hi);
+                if (rc) {
+                    *failed = m[r];
+                    return rc;
+                }
+                fits = hi == want;
+            }
+            if (fits) break;
+            if (q == 1) return fail(m[0], CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
+            q = (q + 1) / 2;
+        }
+    }
+    ch.assign(W, Chunk{});
+    for (uint32_t r = 0; r < W; ++r) {
+        ch[r].lo = std::min(total, pos + r * q);
+        ch[r].hi = std::min(total, pos + (r + 1) * q);
+        ch[r].stage = stage;
+        *failed = m[r];
+        const int rc = fm.upload(m[r], ch[r]);
+        if (rc) return rc;
+    }
+    return CTMR_OK;
+}
+
+// A member's device-resident chunk as its part of round `parity` (run_round).  Everything runs on the member's stream,
+// so there is no chain: the back half waits for each round before the next is issued.
+int fe_member(ctmr_ctx* c, const ctmr_dev_batch& db, const ctmr_dev_out& dout, int parity, RoundMember& x) {
+    CU(c, cudaSetDevice(c->device));
+    int rc = ensure_scratch(c, std::max<uint64_t>(db.n, 1));
+    if (rc == CTMR_OK) rc = ensure_order(c, db.n);
+    if (rc) return rc;
+    x = RoundMember{};
+    x.c = c;
+    x.db = db;
+    x.dout = dout;
+    x.dout.keys = c->keys_scratch;
+    x.slot_of = c->slot_scratch; x.pair_slot = c->pair_scratch; x.order = c->order_scratch; x.len_hist = c->len_hist;
+    x.meta_slots = c->meta_scratch;
+    x.map_stream = x.reduce_stream = c->stream;
+    x.mapped = c->fe->mapped; x.reduced = c->fe->reduced; x.meta_done = c->fe->meta_done;
+    // the members of an in-process group meet through their events; peer_barrier does nothing for them
+    x.ch_map = CH_STAGE_MAP + parity;
+    x.ch_resolve = CH_STAGE_RESOLVE + parity;
+    x.ch_meta = CH_STAGE_META + parity;
+    return CTMR_OK;
+}
+
+// The path over round k's chunks.  One member: ctmr_process_device on the ctx's stream, which overlaps the map and the
+// reduce of a large chunk.  A group: one round of the key exchange, each member's chunk as its slice.
+int run_path(ctmr_ctx** m, uint32_t W, int k, Chunk* cur, bool meta, ctmr_ctx** failed) {
+    if (W == 1) {
+        *failed = m[0];
+        return cur[0].db.n ? ctmr_process_device(m[0], &cur[0].db, &cur[0].dout, m[0]->stream) : CTMR_OK;
+    }
+    const int parity = k % (int)kParities;
+    RoundMember rm[kMaxWorld];
+    for (uint32_t r = 0; r < W; ++r) {
+        *failed = m[r];
+        const int rc = fe_member(m[r], cur[r].db, cur[r].dout, parity, rm[r]);
+        if (rc) return rc;
+    }
+    return run_round(rm, W, parity, m[0]->fe->cap_entries, meta, failed);
+}
+
+// after the path: x509 leaf failures, PEM, outputs to the host; waits for the chunk
+template <class Format>
+int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
+    FrontEnd* f = c->fe;
+    cudaStream_t s = c->stream;
+    CU(c, cudaSetDevice(c->device));
+    const uint64_t cnt = ch.e1 - ch.e0;
+    const ctmr_out* po = &fm.out->path;
+    if (cnt) {
+        CU(c, launch_fe_finish(ch.p.fe, f->status, s));
+        ++f->launches;
+    }
+    CU(c, cudaEventRecord(f->ev2, s));
+    if (cnt && po->pem) {  // the new certificates' PEM, encoded from the DER in HBM
+        int rc = pem_ensure(c, f->pem, f->cap_entries, f->cap_decoded);
+        if (rc) return rc;
+        rc = pem_chunk(c, f->pem, ch.p.fe.decoded, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, ch.e0, pem_base, s);
+        if (rc) return rc;
+    }
+    if (Format::kStageHoldsLeaves) CU(c, cudaEventRecord(f->stage[ch.stage].consumed, s));  // the leaves' last read is done
+    if (cnt) {
+        const int rc = copy_out(c, ch.dout, cnt, po, ch.e0, s);
+        if (rc) return rc;
+    }
+    const int rc = fm.copy_back(c, ch);
+    if (rc) return rc;
     float a = 0.f, d = 0.f;
     CU(c, cudaEventElapsedTime(&a, f->ev0, f->ev1));
     CU(c, cudaEventElapsedTime(&d, f->ev1, f->ev2));
@@ -751,197 +751,102 @@ int tile_back(ctmr_ctx* c, const ctmr_tile_out* out, TileChunk& ch, uint64_t* pe
     return CTMR_OK;
 }
 
-// the stop: tiles_done, the unknown fingerprints, and the call's result code
-int tile_stop(ctmr_ctx* c, ctmr_tile_out* out, const TileChunk& ch) {
-    out->tiles_done = ch.hi;
-    out->n_missing = (uint32_t)std::min<size_t>(ch.missing.size(), out->missing_cap);
-    for (uint32_t i = 0; i < out->n_missing; ++i) std::memcpy(out->missing_fp + 32ull * i, ch.missing[i].data(), 32);
-    return fail(c, CTMR_E_UNKNOWN_ISSUER, "tile " + std::to_string(ch.hi) + " names a Chain[0] fingerprint that is not registered "
-                                          "(ctmr_register_chain_certs, then call again from tiles_done)");
-}
-
-int tiles_prepare(ctmr_ctx* c) {
-    CU(c, cudaSetDevice(c->device));
-    int rc = frontend_ensure(c);
-    if (rc == CTMR_OK) rc = tiles_ensure(c);
+// One front-end call on the members m[0..W): one ctx (W == 1), or the members of a group.  The batch's entries take the
+// global indices from *next_index on; tree (one member only): fold the entries into it too, written back when the call
+// succeeds or stops.  A stop (tiles) ends the call after the round that meets it.  On error *failed names the member
+// that failed.
+template <class Format>
+int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, ctmr_tree* tree, ctmr_ctx** failed) {
+    *failed = m[0];
+    int rc = fm.check(m[0], tree);
     if (rc) return rc;
-    c->fe->fe_ms = c->fe->path_ms = c->fe->tl->split_ms = 0.f;
-    c->fe->launches = 0;
-    return CTMR_OK;
-}
-
-// ctmr_process_tiles_tree's rules for the tiles of one log, checked before any work like tile_args
-int tree_tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tree* tree, uint64_t n) {
-    if (b->n_tiles == 0) return CTMR_OK;
-    if (b->tile_index[0] > (~0ull - n) >> 8) return fail(c, CTMR_E_INVALID, "tree: the batch's last leaf index does not fit 64 bits");
-    for (uint64_t t = 0; t + 1 < b->n_tiles; ++t) {
-        if (b->tile_index[t + 1] != b->tile_index[t] + 1) return fail(c, CTMR_E_INVALID, "tree: tiles are not consecutive");
-        if (b->tile_width[t] != 256) return fail(c, CTMR_E_INVALID, "tree: a partial tile that is not the last");
-    }
-    const uint64_t first = 256 * b->tile_index[0];
-    if (tree->size < first || tree->size > first + b->tile_width[0])
-        return fail(c, CTMR_E_INVALID, "tree: size is not inside the batch's first tile");
-    return CTMR_OK;
-}
-
-// *done_entries: entries that took their indices (all of them unless the call stops or fails).  tree: fold the entries
-// into it too (ctmr_process_tiles_tree), written back when the call succeeds or stops at an unknown Chain[0].
-int process_tiles_single(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries, ctmr_tree* tree = nullptr) {
-    std::vector<uint64_t> ent;
-    int rc = tile_args(c, b, out, ent);
-    if (rc) return rc;
-    const uint64_t n = ent[b->n_tiles];
-    if (tree) {
-        rc = tree_tile_args(c, b, tree, n);
-        if (rc) return rc;
-    }
-    *done_entries = n;
-    out->tiles_done = 0;
-    out->n_missing = 0;
-    if (b->n_tiles == 0 && !tree) return CTMR_OK;
-    rc = tiles_prepare(c);
-    if (rc) return rc;
-    if (tree) {
-        rc = tree_begin(c, tree, b->n_tiles ? 256 * b->tile_index[0] : 0);
-        if (rc) return rc;
-        if (b->n_tiles == 0) return tree_end(c, tree);
-    }
-    uint64_t pem_base = 0;
-    TileChunk ch[2];
-    const char* too_large = "a single tile exceeds the front end's staging budget";
-    rc = tile_fit(c, b, ent, 0, ~0ull, &ch[0].hi);
-    if (rc) return rc;
-    if (ch[0].hi == 0) return fail(c, CTMR_E_BATCH_TOO_LARGE, too_large);
-    rc = tile_upload(c, b, ent, ch[0]);
-    if (rc) return rc;
-    for (int k = 0;; ++k) {
-        TileChunk& cur = ch[k & 1];
-        if (cur.hi < b->n_tiles) {  // next chunk's upload overlaps this chunk's kernels
-            TileChunk& nx = ch[(k + 1) & 1];
-            nx = TileChunk{};
-            nx.lo = cur.hi;
-            nx.stage = (k + 1) & 1;
-            rc = tile_fit(c, b, ent, nx.lo, ~0ull, &nx.hi);
-            if (rc) return rc;
-            if (nx.hi == nx.lo) return fail(c, CTMR_E_BATCH_TOO_LARGE, too_large);
-            rc = tile_upload(c, b, ent, nx);
-            if (rc) return rc;
-        }
-        rc = tile_front(c, b, out, cur);
-        if (rc) return rc;
-        cur.db.first_index = c->next_index + cur.e0;
-        if (cur.db.n) {
-            rc = ctmr_process_device(c, &cur.db, &cur.dout, c->stream);
-            if (rc) return rc;
-        }
-        rc = tile_back(c, out, cur, &pem_base);
-        if (rc) return rc;
-        out->tiles_done = cur.hi;
-        if (cur.stopped) {
-            *done_entries = cur.e1;
-            if (out->path.pem) out->path.pem_off[cur.e1] = pem_base;
-            rc = ctmr_check_device(c, nullptr);  // a table that filled up during the completed tiles is this call's error
-            if (rc == CTMR_OK && tree) rc = tree_end(c, tree);  // the completed tiles are in the tree: resume from there
-            return rc ? rc : tile_stop(c, out, cur);
-        }
-        if (cur.hi >= b->n_tiles) break;
-    }
-    if (out->path.pem) out->path.pem_off[n] = pem_base;
-    rc = ctmr_check_device(c, nullptr);
-    return rc || !tree ? rc : tree_end(c, tree);
-}
-
-int process_tiles_group(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out, uint64_t* done_entries, ctmr_ctx** failed) {
-    const uint32_t W = (uint32_t)g->m.size();
-    ctmr_ctx* c0 = g->m[0];
-    *failed = c0;
-    std::vector<uint64_t> ent;
-    int rc = tile_args(c0, b, out, ent);
-    if (rc) return rc;
-    const uint64_t n = ent[b->n_tiles];
-    *done_entries = n;
-    out->tiles_done = 0;
-    out->n_missing = 0;
-    if (b->n_tiles == 0) return CTMR_OK;
+    const uint64_t total = fm.units();
+    if (total == 0 && !tree) return CTMR_OK;
     for (uint32_t r = 0; r < W; ++r) {
-        *failed = g->m[r];
-        rc = tiles_prepare(g->m[r]);
+        *failed = m[r];
+        rc = fm.prepare(m[r]);
         if (rc) return rc;
     }
-    auto plan = [&](uint64_t pos, int stage, std::vector<TileChunk>& ch) {
-        return plan_round(
-            g, b->n_tiles, ~0ull, pos, stage, ch, failed, "a single tile exceeds the front end's staging budget",
-            [&](ctmr_ctx* c, uint64_t lo, uint64_t want, uint64_t* hi) { return tile_fit(c, b, ent, lo, want, hi); },
-            [&](ctmr_ctx* c, TileChunk& x) { return tile_upload(c, b, ent, x); });
-    };
-    const ctmr_out* po = &out->path;
-    const bool want_meta = po->first_issuer_dn || po->first_crldp || po->issuer_name_off || po->crldp_off;
+    *failed = m[0];
+    if (tree) {
+        rc = tree_begin(m[0], tree, fm.tree_base(tree));
+        if (rc) return rc;
+        if (total == 0) return tree_end(m[0], tree);
+    }
+    const ctmr_out* po = &fm.out->path;
     uint64_t pem_base = 0;
-    std::vector<TileChunk> cur, nxt;
-    rc = plan(0, 0, cur);
+    std::vector<Chunk> ch[2];  // round k's chunks in ch[k & 1], uploaded into stage k & 1
+    rc = plan_round(m, W, fm, 0, 0, ch[0], failed);
     if (rc) return rc;
+    Chunk* cur = nullptr;
+    uint32_t stop = W;  // the member whose chunk holds the stop
     for (int k = 0;; ++k) {
+        cur = ch[k & 1].data();
         const uint64_t end = cur[W - 1].hi;
-        if (end < b->n_tiles) {  // the next round's uploads overlap this round's kernels
-            rc = plan(end, (k + 1) & 1, nxt);
+        if (end < total) {  // the next round's uploads overlap this round's kernels and host round trips
+            rc = plan_round(m, W, fm, end, (k + 1) & 1, ch[(k + 1) & 1], failed);
             if (rc) return rc;
         }
-        std::vector<int> rcs;
-        for_each_member(W, rcs, [&](uint32_t r) { return tile_front(g->m[r], b, out, cur[r]); });
-        for (uint32_t r = 0; r < W; ++r)
-            if (rcs[r]) {
-                *failed = g->m[r];
-                return rcs[r];
-            }
-        // a stop in member r: the later members' chunks run empty (their entries must not touch the tables)
-        uint32_t stop = W;
-        for (uint32_t r = 0; r < W && stop == W; ++r)
-            if (cur[r].stopped) stop = r;
-        for (uint32_t r = stop + 1; r < W; ++r) {
-            TileChunk& x = cur[r];
-            x.hi = x.lo;
-            x.e1 = x.e0;
-            x.p.n_tiles = 0;
-            x.p.n = x.p.fe.n = x.db.n = 0;
-        }
-        const int parity = k % (int)kParities;
-        RoundMember rm[kMaxWorld];
+        // The front halves wait on the host (issuer identification round trips, the arena size): one thread per member,
+        // so that the members' waits overlap instead of adding up.  Each thread touches its own ctx only; the issuer
+        // registry they all resolve against is device memory reached with atomics.
+        rc = for_each_member(m, W, W > 1, failed, [&](uint32_t r) { return fm.front(m[r], cur[r]); });
+        if (rc) return rc;
         for (uint32_t r = 0; r < W; ++r) {
-            *failed = g->m[r];
-            cur[r].db.first_index = g->next_index + cur[r].e0;
-            rc = fe_member(g->m[r], cur[r].db, cur[r].dout, parity, rm[r]);
-            if (rc) return rc;
+            if (stop < W) cur[r].cut(0, 0);  // after a stop in an earlier member: its entries must not touch the tables
+            else if (cur[r].stopped) stop = r;
+            cur[r].db.first_index = *next_index + cur[r].e0;
         }
-        rc = run_round(rm, W, parity, c0->fe->cap_entries, want_meta, failed);
+        rc = run_path(m, W, k, cur, want_meta(po), failed);
         if (rc) return rc;
-        for (uint32_t r = 0; r < W; ++r) {  // in entry order: PEM texts are appended in that order
-            *failed = g->m[r];
-            rc = tile_back(g->m[r], out, cur[r], &pem_base);
-            if (rc) return rc;
-        }
-        if (stop < W) {
-            *done_entries = cur[stop].e1;
-            if (out->path.pem) out->path.pem_off[cur[stop].e1] = pem_base;
-            for (uint32_t r = 0; r < W; ++r) {  // a table that filled up during the completed tiles is this call's error
-                *failed = g->m[r];
-                rc = ctmr_check_device(g->m[r], nullptr);
-                if (rc) return rc;
-            }
-            *failed = g->m[stop];
-            return tile_stop(g->m[stop], out, cur[stop]);
-        }
-        out->tiles_done = end;
-        if (end >= b->n_tiles) break;
-        cur.swap(nxt);
+        // in entry order when there is PEM (the texts are appended in that order); otherwise each member writes its own
+        // ranges of the outputs, and on a group the members' copies and waits overlap
+        rc = for_each_member(m, W, W > 1 && !po->pem, failed, [&](uint32_t r) { return back(m[r], fm, cur[r], &pem_base); });
+        if (rc) return rc;
+        fm.completed(stop < W ? cur[stop].hi : end);
+        if (stop < W || end >= total) break;
     }
-    if (out->path.pem) out->path.pem_off[n] = pem_base;
+    if (stop < W) fm.done = cur[stop].e1;
+    if (po->pem) po->pem_off[fm.done] = pem_base;
+    for (uint32_t r = 0; r < W; ++r) {  // a table that filled up during the completed chunks is this call's error
+        *failed = m[r];
+        rc = ctmr_check_device(m[r], nullptr);
+        if (rc) return rc;
+    }
+    *failed = m[0];
+    if (tree) {  // at a stop the completed tiles are in the tree: the resumed call continues from there
+        rc = tree_end(m[0], tree);
+        if (rc) return rc;
+    }
+    if (stop == W) return CTMR_OK;
+    *failed = m[stop];
+    return fm.stop(m[stop], cur[stop]);
+}
+
+// an upload of the NEXT chunk may still be reading the caller's text and an output copy may still be writing the caller's
+// arrays: neither may outlive a failed call
+void drain_frontend(ctmr_ctx* c) {
+    if (!c || !c->fe) return;
+    const std::string keep = c->err;
+    cudaSetDevice(c->device);
+    cudaStreamSynchronize(c->fe->copy_stream);
+    cudaStreamSynchronize(c->stream);
+    c->err = keep;
+}
+
+// Every front-end entry point: the call on members m[0..W), then, also after a failure, the entries that took their
+// indices are used up (a retry must not reuse them: its entries then read as known), the tree is the caller's again,
+// and a failure drains every member and becomes the last error of the group g (if any).
+template <class Format>
+int front_end_call(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format fm, ctmr_tree* tree, ctmr_group* g) {
+    ctmr_ctx* failed = nullptr;
+    const int rc = process_members(m, W, next_index, fm, tree, &failed);
+    *next_index += fm.done;
     for (uint32_t r = 0; r < W; ++r) {
-        *failed = g->m[r];
-        rc = ctmr_check_device(g->m[r], nullptr);
-        if (rc) return rc;
+        if (m[r]->fe && m[r]->fe->tree) m[r]->fe->tree->active = false;
+        if (rc != CTMR_OK) drain_frontend(m[r]);
     }
-    *failed = nullptr;
-    return CTMR_OK;
+    return rc != CTMR_OK ? group_fail(g, failed, rc) : rc;
 }
 
 // Fingerprints of chain certificates on the GPU, then: a fingerprint table slot for each new one (capacity first, so a
@@ -1011,17 +916,6 @@ int register_chain_certs(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offse
     return CTMR_OK;
 }
 
-// an upload of the NEXT chunk may still be reading the caller's text and an output copy may still be writing the caller's
-// arrays: neither may outlive a failed call
-void drain_frontend(ctmr_ctx* c) {
-    if (!c || !c->fe) return;
-    const std::string keep = c->err;
-    cudaSetDevice(c->device);
-    cudaStreamSynchronize(c->fe->copy_stream);
-    cudaStreamSynchronize(c->stream);
-    c->err = keep;
-}
-
 }  // namespace
 
 extern "C" {
@@ -1029,84 +923,37 @@ extern "C" {
 int ctmr_process_raw(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_raw");
-    const int rc = process_raw_single(c, b, out);
-    if (b) c->next_index += b->n;  // also after a failure: a retry must not reuse the indices
-    if (rc != CTMR_OK) drain_frontend(c);
-    return rc;
+    return front_end_call(&c, 1, &c->next_index, Pages(b, out), nullptr, nullptr);
 }
 
 int ctmr_group_process_raw(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out) {
     if (!g || g->m.empty()) return CTMR_E_INVALID;
-    ctmr_ctx* failed = nullptr;
-    int rc;
-    if (g->m.size() == 1) {  // a group of one is a plain ctx
-        ctmr_ctx* c = g->m[0];
-        c->next_index = g->next_index;
-        rc = process_raw_single(c, b, out);
-        failed = c;
-    } else {
-        rc = process_raw_group(g, b, out, &failed);
-    }
-    if (b) g->next_index += b->n;  // also after a failure: a retry must not reuse the indices (its entries then read as known)
-    if (rc != CTMR_OK) {
-        for (ctmr_ctx* c : g->m) drain_frontend(c);
-        if (failed) g->err = failed->err;
-    }
-    return rc;
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Pages(b, out), nullptr, g);
 }
 
 int ctmr_process_tiles(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_tiles");
-    uint64_t done = 0;
-    const int rc = process_tiles_single(c, b, out, &done);
-    c->next_index += done;  // after a stop only the completed tiles' entries; after a failure all of them
-    if (rc != CTMR_OK) drain_frontend(c);
-    return rc;
+    return front_end_call(&c, 1, &c->next_index, Tiles(b, out), nullptr, nullptr);
 }
 
 int ctmr_group_process_tiles(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out) {
     if (!g || g->m.empty()) return CTMR_E_INVALID;
-    ctmr_ctx* failed = nullptr;
-    uint64_t done = 0;
-    int rc;
-    if (g->m.size() == 1) {  // a group of one is a plain ctx
-        ctmr_ctx* c = g->m[0];
-        c->next_index = g->next_index;
-        rc = process_tiles_single(c, b, out, &done);
-        failed = c;
-    } else {
-        rc = process_tiles_group(g, b, out, &done, &failed);
-    }
-    g->next_index += done;
-    if (rc != CTMR_OK) {
-        for (ctmr_ctx* c : g->m) drain_frontend(c);
-        if (failed) g->err = failed->err;
-    }
-    return rc;
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Tiles(b, out), nullptr, g);
 }
 
 int ctmr_process_raw_tree(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree) {
     if (!c) return CTMR_E_INVALID;
     if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
-    const int rc = process_raw_single(c, b, out, tree);
-    if (c->fe && c->fe->tree) c->fe->tree->active = false;
-    if (b) c->next_index += b->n;  // as ctmr_process_raw
-    if (rc != CTMR_OK) drain_frontend(c);
-    return rc;
+    return front_end_call(&c, 1, &c->next_index, Pages(b, out), tree, nullptr);
 }
 
 int ctmr_process_tiles_tree(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, ctmr_tree* tree) {
     if (!c) return CTMR_E_INVALID;
     if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
-    uint64_t done = 0;
-    const int rc = process_tiles_single(c, b, out, &done, tree);
-    if (c->fe && c->fe->tree) c->fe->tree->active = false;
-    c->next_index += done;  // as ctmr_process_tiles
-    if (rc != CTMR_OK) drain_frontend(c);
-    return rc;
+    return front_end_call(&c, 1, &c->next_index, Tiles(b, out), tree, nullptr);
 }
 
 int ctmr_tiles_profile_last(ctmr_ctx* c, float* split_ms) {

@@ -130,6 +130,11 @@ int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* o
     return CTMR_OK;
 }
 
+int group_fail(ctmr_group* g, ctmr_ctx* c, int rc) {
+    if (g && c) g->err = c->err;
+    return rc;
+}
+
 }  // namespace ctmr_host
 
 namespace {
@@ -148,11 +153,6 @@ struct Slice {
     uint64_t lo = 0, hi = 0;      // entries of the caller's batch
     uint64_t first_index = 0;     // global index of entry lo
 };
-
-int group_fail(ctmr_group* g, ctmr_ctx* c, int rc) {
-    if (g && c) g->err = c->err;
-    return rc;
-}
 
 // rounds x members.  Every slice respects the entry budget and the byte budget of a stage.
 int plan_rounds(ctmr_ctx* c0, uint32_t W, const BatchArgs& a, std::vector<std::vector<Slice>>& plan) {

@@ -343,7 +343,7 @@ def test_issuer_id_at_sha256_block_boundaries(eng, ora):
 # ------------------------------------------------------------------------------------------------ 6. Chain[0] collisions
 
 def chunks_of(ll, xl, cap_entries, cap_text):
-    """fe_fit (ctmr_frontend_api.cu): entries per chunk under the entry budget and half the character budget."""
+    """Pages::fit (ctmr_frontend_api.cu): entries per chunk under the entry budget and half the character budget."""
     out, lo = [], 0
     while lo < ll.size:
         hi, chars = lo, 0

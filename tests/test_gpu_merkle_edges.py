@@ -257,7 +257,7 @@ def test_pages_two_without_a_leaf_the_lowest_wins(eng, pair):
 # ---------------------------------------------------------------------------------------------------------- 3. chunks
 def chunk_launches(first_pos, n, m, chars=None, cap_text=None):
     """the launches a tree call adds to the plain call: per chunk, raw_leaf_hash and the fold.  A chunk takes at most m
-    entries and, when chars (leaf_input + extra_data characters per entry) are given, half of cap_text (fe_fit)."""
+    entries and, when chars (leaf_input + extra_data characters per entry) are given, half of cap_text (Pages::fit)."""
     out, j = 0, 0
     while j < n:
         c, used = 0, 0
@@ -456,7 +456,7 @@ def test_tiles_bad_partial_last_tile(eng, tp, want_leaf_hash):
 
 
 def tile_chunks(tl, cap_text, cap_entries=1 << 18):
-    """tile_fit: the first tile of every chunk"""
+    """Tiles::fit: the first tile of every chunk"""
     starts, lo = [], 0
     while lo < len(tl.tiles):
         starts.append(lo)

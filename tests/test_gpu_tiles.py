@@ -381,7 +381,7 @@ def test_mixing_entry_points_and_restore(eng, ora):
         del r1
 
 
-def _group_case(eng, ora, devices):
+def _group_case(eng, ora, devices, want_pem=True):
     cp = Corpus(ora, [256] * 9 + [50], seed=47)
     with eng.GpuCertDatabase(log_expired_entries=True, table_capacity=1 << 16) as db:
         cp.register(db)
@@ -391,10 +391,10 @@ def _group_case(eng, ora, devices):
         # first only some issuers: the stop lands inside a member's window and the resume completes it
         some = cp.certs[: len(cp.certs) // 2]
         cp.register(g, some)
-        got = g.store_tiles(*cp.args(), NOW_NS, want_pem=True, want_leaf_hash=True,
+        got = g.store_tiles(*cp.args(), NOW_NS, want_pem=want_pem, want_leaf_hash=True,
                             fetch=lambda fps: [cp.by_fp[f] for f in fps])
         assert got.tiles_done == 10
-        for f in PATH_FIELDS + ("sha256", "pem", "pem_off"):
+        for f in PATH_FIELDS + ("sha256",) + (("pem", "pem_off") if want_pem else ()):
             assert np.array_equal(getattr(got.path, f), getattr(want.path, f)), f
         for f in ("entry_status", "leaf_hash", "leaf_off", "tile_status"):
             assert np.array_equal(getattr(got, f), getattr(want, f)), f
@@ -403,6 +403,74 @@ def _group_case(eng, ora, devices):
 
 def test_group_of_three_shards_on_one_gpu(eng, ora):
     _group_case(eng, ora, [0, 0, 0])
+
+
+def test_group_of_three_shards_without_pem(eng, ora):
+    """without PEM the members' back halves run on one thread each"""
+    _group_case(eng, ora, [0, 0, 0], want_pem=False)
+
+
+def _one_ctx_and_group_of_one(eng, calls):
+    """calls(db) -> results, on one ctx and on GpuCertGroup([0]); returns both, each with the known-certificate table"""
+    out = []
+    for make in (eng.GpuCertDatabase, lambda **kw: eng.GpuCertGroup([0], **kw)):
+        with make(log_expired_entries=True, table_capacity=1 << 16) as db:
+            out.append((calls(db), ready_slots(getattr(db, "members", [db])[0])))
+    return out
+
+
+def _same_calls(a, b, fields):
+    for k, (x, y) in enumerate(zip(a, b)):
+        for f in PATH_FIELDS + ("sha256", "pem", "pem_off"):
+            assert np.array_equal(getattr(x.path, f), getattr(y.path, f)), (k, f)
+        for f in fields:
+            assert np.array_equal(getattr(x, f), getattr(y, f)), (k, f)
+
+
+def test_group_of_one_pages(eng, ora):
+    """A group of one runs get-entries pages as one ctx does.  Two calls, the second holding new pages and then the
+    first call's again: every output and the table slot by slot (lowest entry index included) are one ctx's, and the
+    second call finds the first call's certificates known."""
+    from ct_mapreduce_b200 import frontend as fe
+    cp = Corpus(ora, [256] * 6, seed=61)
+    ents = [fe.tile_to_get_entries(b"".join(t), cp.by_fp) for t in cp.tile_leaves]
+    bodies = [fe.get_entries_body(sum(ents[:3], [])), fe.get_entries_body(sum(ents[3:] + ents[:3], []))]
+
+    def calls(db):
+        rs = [db.store_raw_entries(body, *fe.find_entry_spans(body), NOW_NS, want_pem=True) for body in bodies]
+        assert rs[0].path.was_unknown.any() and not rs[1].path.was_unknown[768:].any()
+        for r in rs:  # dense indices follow the order in which the GPU meets new issuers: their digests are compared
+            r.issuer = [db.issuer_digest(int(i)) if i < 0xFFFFFFFE else int(i) for i in r.issuer]
+        return rs
+    (one, one_slots), (grp, grp_slots) = _one_ctx_and_group_of_one(eng, calls)
+    _same_calls(one, grp, ("entry_status", "entry_type", "timestamp_ms", "leaf_src", "leaf_off", "leaf_len"))
+    assert [r.issuer for r in one] == [r.issuer for r in grp]
+    assert one_slots == grp_slots
+
+
+def test_group_of_one_tiles_stop_and_resume(eng, ora):
+    """A group of one runs tiles as one ctx does.  A call that stops at an unregistered Chain[0], the call that resumes
+    from tiles_done after the registration, and the first call's tiles again: every output and the table slot by slot
+    are one ctx's, and the later calls find the first call's certificates known."""
+    cp = Corpus(ora, [256] * 8 + [31], seed=19)
+    r_all = to.tiles_process(ora, ora.DB(b"", True), *cp.args(), cp.by_fp, NOW_NS)
+    first = [cp.by_fp[f] for f in {r_all.chain0_fp[i] for i in range(768)} - {None}]
+
+    def calls(db):
+        cp.register(db, first)
+        r1 = db.store_tiles(*cp.args(), NOW_NS, want_pem=True, want_leaf_hash=True)
+        k = r1.tiles_done
+        assert 3 <= k < 9 and r1.missing
+        cp.register(db)
+        r2 = db.store_tiles(*cp.args(slice(k, None)), NOW_NS, want_pem=True, want_leaf_hash=True)
+        r3 = db.store_tiles(*cp.args(slice(0, k)), NOW_NS, want_pem=True, want_leaf_hash=True)
+        assert r2.tiles_done == 9 - k and r3.tiles_done == k and not r3.path.was_unknown.any()
+        return r1, r2, r3
+    (one, one_slots), (grp, grp_slots) = _one_ctx_and_group_of_one(eng, calls)
+    assert [r.missing for r in one] == [r.missing for r in grp]
+    _same_calls(one, grp, ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_index", "leaf_off", "leaf_len",
+                           "leaf_hash", "tile_status"))
+    assert one_slots == grp_slots
 
 
 def test_group_all_gpus(eng, ora):

@@ -24,8 +24,7 @@ uint64_t pow2_at_least(uint64_t v) {
 
 namespace {
 
-void fe_destroy(ctmr_ctx* c);
-int fe_add_issuer(ctmr_ctx* c, const std::string& der, uint32_t idx);
+int fe_add_issuer(ctmr_ctx* c, FrontEnd* f, const std::string& der, uint32_t idx);
 int fe_clear_issuers(ctmr_ctx* c);
 
 // strings.Split(*ctconfig.IssuerCNFilter, ",") -- no trimming (ct-fetch.go:58)
@@ -77,15 +76,14 @@ namespace ctmr_host {
 int ensure_scratch(ctmr_ctx* c, uint64_t n) {
     if (n <= c->scratch_cap) return CTMR_OK;
     CU(c, cudaDeviceSynchronize());
-    cudaFree(c->keys_scratch); cudaFree(c->slot_scratch); cudaFree(c->pair_scratch); cudaFree(c->bits_scratch);
-    cudaFree(c->meta_scratch);
-    c->keys_scratch = nullptr; c->slot_scratch = c->pair_scratch = nullptr; c->bits_scratch = nullptr; c->meta_scratch = nullptr;
-    c->scratch_cap = 0;
-    CU(c, cudaMalloc(&c->keys_scratch, n * sizeof(ctmr_key)));
-    CU(c, cudaMalloc(&c->slot_scratch, n * sizeof(uint32_t)));
-    CU(c, cudaMalloc(&c->pair_scratch, n * sizeof(uint32_t)));
-    CU(c, cudaMalloc(&c->bits_scratch, 2 * n));
-    CU(c, cudaMalloc(&c->meta_scratch, 2 * n * sizeof(uint32_t)));
+    c->scratch_cap = 0;  // the old buffers go first, so that peak memory is the new set
+    c->keys_scratch.reset(); c->slot_scratch.reset(); c->pair_scratch.reset(); c->bits_scratch.reset(); c->meta_scratch.reset();
+    DevBuf<ctmr_key> keys;
+    DevBuf<uint32_t> slot, pair, meta;
+    DevBuf<uint8_t> bits;
+    CU(c, alloc(keys, n)); CU(c, alloc(slot, n)); CU(c, alloc(pair, n)); CU(c, alloc(bits, 2 * n)); CU(c, alloc(meta, 2 * n));
+    c->keys_scratch = std::move(keys); c->slot_scratch = std::move(slot); c->pair_scratch = std::move(pair);
+    c->bits_scratch = std::move(bits); c->meta_scratch = std::move(meta);
     c->scratch_cap = n;
     return CTMR_OK;
 }
@@ -159,13 +157,38 @@ int map_slice(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, uint3
 int ensure_order(ctmr_ctx* c, uint64_t n) {
     if (n > c->order_cap) {
         CU(c, cudaDeviceSynchronize());  // the old buffer may still be in use
-        cudaFree(c->order_scratch);
-        c->order_scratch = nullptr;
         c->order_cap = 0;
-        CU(c, cudaMalloc(&c->order_scratch, n * sizeof(uint32_t)));
+        CU(c, alloc(c->order_scratch, n));
         c->order_cap = n;
     }
-    if (!c->len_hist) CU(c, cudaMalloc(&c->len_hist, 256 * sizeof(unsigned int)));
+    if (!c->len_hist) CU(c, alloc(c->len_hist, 256));
+    return CTMR_OK;
+}
+
+// what ctmr_process_device needs for a batch of n entries: scratch, the length order, its streams, events and histograms
+int ensure_device_path(ctmr_ctx* c, uint64_t n) {
+    int rc = ensure_scratch(c, n);
+    if (rc) return rc;
+    rc = ensure_order(c, n);
+    if (rc || c->dp) return rc;
+    std::unique_ptr<DevicePipeline> dp(new (std::nothrow) DevicePipeline());
+    if (!dp) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    CU(c, create(dp->stream_a));
+    CU(c, create(dp->stream_a2));
+    CU(c, create(dp->ev_join_a2));
+    CU(c, create(dp->stream_b));
+    CU(c, create(dp->ev_fork));
+    CU(c, create(dp->ev_join_a));
+    CU(c, create(dp->ev_join_b));
+    for (int k = 0; k < kMaxRounds; ++k) {
+        CU(c, create(dp->ev_map0[k], cudaEventDefault));
+        CU(c, create(dp->ev_map1[k], cudaEventDefault));
+        CU(c, create(dp->ev_red1[k], cudaEventDefault));
+        CU(c, create(dp->ev_tok[k]));
+        CU(c, alloc(dp->len_hist[k], 256));
+    }
+    for (Event& e : dp->ev_pulled) CU(c, create(e));
+    c->dp = std::move(dp);
     return CTMR_OK;
 }
 
@@ -218,17 +241,20 @@ void attach_exchange(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_
 
 int alloc_exchange(ctmr_ctx* c, uint32_t world) {
     if (c->xchg || world <= 1) return CTMR_OK;
-    c->X = c->cfg_round_entries ? c->cfg_round_entries : c->stage_entries;
-    if (c->X < c->stage_entries) c->X = c->stage_entries;  // the host pipeline maps stage_entries per round
-    const size_t per = (size_t)kParities * world * c->X;
-    CU(c, cudaMalloc(&c->xchg, exchange_bytes(world, c->X)));
-    CU(c, cudaMemsetAsync(c->xchg, 0, 4096, c->stream));
-    CU(c, cudaMalloc(&c->cursors, (size_t)kParities * kMaxWorld * sizeof(unsigned long long)));
+    const uint64_t X = std::max(c->cfg_round_entries ? c->cfg_round_entries : c->stage_entries,
+                                c->stage_entries);  // the host pipeline maps stage_entries per round
+    const size_t per = (size_t)kParities * world * X;
+    DevBuf<uint8_t> xchg;  // set last: a ctx with c->xchg has all of the exchange
+    CU(c, alloc(xchg, exchange_bytes(world, X)));
+    CU(c, cudaMemsetAsync(xchg, 0, 4096, c->stream));
+    CU(c, alloc(c->cursors, (size_t)kParities * kMaxWorld));
     CU(c, cudaMemsetAsync(c->cursors, 0, (size_t)kParities * kMaxWorld * sizeof(unsigned long long), c->stream));
-    CU(c, cudaMalloc(&c->rev, per * sizeof(uint32_t)));
-    CU(c, cudaMalloc(&c->in_slot, per * sizeof(uint32_t)));
-    CU(c, cudaMalloc(&c->in_pair, per * sizeof(uint32_t)));
+    CU(c, alloc(c->rev, per));
+    CU(c, alloc(c->in_slot, per));
+    CU(c, alloc(c->in_pair, per));
     CU(c, cudaStreamSynchronize(c->stream));
+    c->X = X;
+    c->xchg = std::move(xchg);
     return CTMR_OK;
 }
 
@@ -410,35 +436,6 @@ ctmr_dev_out dev_out_at(const ctmr_dev_out& o, uint64_t lo) {
 
 
 // ------------------------------------------------------------------------------------------------ front end plumbing
-void fe_destroy(ctmr_ctx* c) {
-    FrontEnd* f = c->fe;
-    if (!f) return;
-    for (FeStage& st : f->stage) {
-        cudaFree(st.text); cudaFree(st.leaf_off); cudaFree(st.extra_off); cudaFree(st.leaf_len); cudaFree(st.extra_len);
-        cudaFreeHost(st.h_leaf_off); cudaFreeHost(st.h_extra_off); cudaFreeHost(st.h_leaf_len); cudaFreeHost(st.h_extra_len);
-        if (st.uploaded) cudaEventDestroy(st.uploaded);
-        if (st.consumed) cudaEventDestroy(st.consumed);
-    }
-    if (f->copy_stream) cudaStreamDestroy(f->copy_stream);
-    cudaFree(f->pad_size); cudaFree(f->dec_off); cudaFree(f->dec_len); cudaFree(f->str_bad); cudaFree(f->decoded);
-    cudaFree(f->scan_temp); cudaFree(f->entry_status); cudaFree(f->entry_type); cudaFree(f->leaf_src); cudaFree(f->timestamp);
-    cudaFree(f->leaf_abs); cudaFree(f->chain_abs); cudaFree(f->tbs_abs); cudaFree(f->leaf_rel); cudaFree(f->leaf_len_out);
-    cudaFree(f->chain_len); cudaFree(f->tbs_len); cudaFree(f->issuer_idx); cudaFree(f->status); cudaFree(f->sha);
-    cudaFree(f->was_unknown); cudaFree(f->first); cudaFree(f->first_meta); cudaFree(f->exp_hour); cudaFree(f->serial_off);
-    cudaFree(f->serial_len); cudaFree(f->spans); cudaFree(f->slots_dev); cudaFree(f->arena); cudaFree(f->pending);
-    cudaFree(f->unknown_list); cudaFree(f->unknown_count);
-    pem_free(f->pem);
-    tiles_free(f);
-    tree_free(f);
-    if (f->ev0) cudaEventDestroy(f->ev0);
-    if (f->ev1) cudaEventDestroy(f->ev1);
-    if (f->ev2) cudaEventDestroy(f->ev2);
-    for (cudaEvent_t e : {f->mapped, f->reduced, f->meta_done})
-        if (e) cudaEventDestroy(e);
-    delete f;
-    c->fe = nullptr;
-}
-
 uint64_t host_issuer_cert_hash(const std::string& der) {
     const uint32_t len = (uint32_t)der.size();
     uint64_t acc = 0;
@@ -451,9 +448,8 @@ uint64_t host_issuer_cert_hash(const std::string& der) {
     return issuer_cert_finish(acc, len);
 }
 
-// one more certificate in the device mirror: bytes into the arena, slot into the probe table
-int fe_add_issuer(ctmr_ctx* c, const std::string& der, uint32_t idx) {
-    FrontEnd* f = c->fe;
+// one more certificate in f, c's front end (installed or being built): bytes into the arena, slot into the probe table
+int fe_add_issuer(ctmr_ctx* c, FrontEnd* f, const std::string& der, uint32_t idx) {
     if (der.empty()) return CTMR_OK;  // the framing never yields an empty Chain[0]
     if (2 * (f->slots_used + 1) > f->slot_mask + 1)
         return fail(c, CTMR_E_TOO_MANY_ISSUERS, "more distinct Chain[0] certificates than the front end's table holds (raise config.max_issuers)");
@@ -461,13 +457,12 @@ int fe_add_issuer(ctmr_ctx* c, const std::string& der, uint32_t idx) {
     if (f->arena_used + padded > f->arena_cap) {
         uint64_t cap = f->arena_cap ? f->arena_cap * 2 : (64ull << 20);
         while (f->arena_used + padded > cap) cap *= 2;
-        uint8_t* bigger = nullptr;
+        DevBuf<uint8_t> bigger;
         CU(c, cudaDeviceSynchronize());
-        CU(c, cudaMalloc(&bigger, cap));
+        CU(c, alloc(bigger, cap));
         if (f->arena_used) CU(c, cudaMemcpyAsync(bigger, f->arena, f->arena_used, cudaMemcpyDeviceToDevice, c->stream));
         CU(c, cudaStreamSynchronize(c->stream));
-        cudaFree(f->arena);
-        f->arena = bigger;
+        f->arena = std::move(bigger);
         f->arena_cap = cap;
     }
     std::string buf = der;
@@ -489,7 +484,7 @@ int fe_add_issuer(ctmr_ctx* c, const std::string& der, uint32_t idx) {
 }
 
 int fe_clear_issuers(ctmr_ctx* c) {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     CU(c, cudaDeviceSynchronize());
     std::fill(f->slots_host.begin(), f->slots_host.end(), IssuerCertSlot{});
     f->slots_used = 0;
@@ -501,9 +496,8 @@ int fe_clear_issuers(ctmr_ctx* c) {
 
 int ensure_frontend(ctmr_ctx* c) {
     if (c->fe) return CTMR_OK;
-    FrontEnd* f = new (std::nothrow) FrontEnd();
+    std::unique_ptr<FrontEnd> f(new (std::nothrow) FrontEnd());
     if (!f) return fail(c, CTMR_E_NOMEM, "host allocation failed");
-    c->fe = f;
     const uint64_t E = c->stage_entries;
     uint64_t T = E * 6144ull < (64ull << 20) ? (64ull << 20) : E * 6144ull;  // leaf_input + extra_data characters per chunk
     if (const char* ev = getenv("CTMR_FE_TEXT_CAP")) {  // tests shrink it to reach the multi-chunk and packing paths
@@ -513,71 +507,45 @@ int ensure_frontend(ctmr_ctx* c) {
     f->cap_entries = E;
     f->cap_text = T;
     f->cap_decoded = T / 4 * 3 + 32 * E + 256;
-    auto bail = [&](int code) {
-        fe_destroy(c);
-        return code;
-    };
-#define FEM(ptr, bytes)                                                                    \
-    do {                                                                                   \
-        cudaError_t e_ = cudaMalloc(&(ptr), (bytes));                                      \
-        if (e_ != cudaSuccess) {                                                           \
-            fail(c, e_ == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA,           \
-                 std::string("front end: cudaMalloc: ") + cudaGetErrorString(e_));         \
-            return bail(e_ == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA);      \
-        }                                                                                  \
-    } while (0)
     for (FeStage& st : f->stage) {
-        FEM(st.text, 16 + T + 64);
-        FEM(st.leaf_off, E * 8); FEM(st.extra_off, E * 8); FEM(st.leaf_len, E * 4); FEM(st.extra_len, E * 4);
-        if (cudaMallocHost(&st.h_leaf_off, E * 8) != cudaSuccess || cudaMallocHost(&st.h_extra_off, E * 8) != cudaSuccess ||
-            cudaMallocHost(&st.h_leaf_len, E * 4) != cudaSuccess || cudaMallocHost(&st.h_extra_len, E * 4) != cudaSuccess ||
-            cudaEventCreateWithFlags(&st.uploaded, cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&st.consumed, cudaEventDisableTiming) != cudaSuccess ||
-            cudaMemsetAsync(st.text, 0, 16 + T + 64, c->stream) != cudaSuccess) {
-            fail(c, CTMR_E_NOMEM, "front end: staging allocation failed");
-            return bail(CTMR_E_NOMEM);
-        }
+        CU(c, alloc(st.text, 16 + T + 64));
+        CU(c, alloc(st.leaf_off, E)); CU(c, alloc(st.extra_off, E)); CU(c, alloc(st.leaf_len, E)); CU(c, alloc(st.extra_len, E));
+        CU(c, alloc(st.h_leaf_off, E)); CU(c, alloc(st.h_extra_off, E)); CU(c, alloc(st.h_leaf_len, E)); CU(c, alloc(st.h_extra_len, E));
+        CU(c, create(st.uploaded));
+        CU(c, create(st.consumed));
+        CU(c, cudaMemsetAsync(st.text, 0, 16 + T + 64, c->stream));
     }
-    if (cudaStreamCreateWithFlags(&f->copy_stream, cudaStreamNonBlocking) != cudaSuccess) {
-        fail(c, CTMR_E_CUDA, "front end: stream creation failed");
-        return bail(CTMR_E_CUDA);
-    }
-    FEM(f->pad_size, (2 * E + 1) * 8); FEM(f->dec_off, (2 * E + 1) * 8); FEM(f->dec_len, 2 * E * 4); FEM(f->str_bad, 2 * E);
-    FEM(f->decoded, f->cap_decoded);
-    if (cudaMemsetAsync(f->decoded, 0, f->cap_decoded, c->stream) != cudaSuccess) {  // the 16-byte padding between decoded strings is read (never consumed) by K_map's staging
-        fail(c, CTMR_E_CUDA, "front end: arena initialisation failed");
-        return bail(CTMR_E_CUDA);
-    }
+    CU(c, create(f->copy_stream));
+    CU(c, alloc(f->pad_size, 2 * E + 1)); CU(c, alloc(f->dec_off, 2 * E + 1)); CU(c, alloc(f->dec_len, 2 * E)); CU(c, alloc(f->str_bad, 2 * E));
+    CU(c, alloc(f->decoded, f->cap_decoded));
+    // the 16-byte padding between decoded strings is read (never consumed) by K_map's staging
+    CU(c, cudaMemsetAsync(f->decoded, 0, f->cap_decoded, c->stream));
     f->scan_temp_bytes = fe_scan_temp_bytes(2 * E + 1);
-    FEM(f->scan_temp, f->scan_temp_bytes ? f->scan_temp_bytes : 16);
-    FEM(f->entry_status, E); FEM(f->entry_type, E); FEM(f->leaf_src, E); FEM(f->timestamp, E * 8);
-    FEM(f->leaf_abs, E * 8); FEM(f->chain_abs, E * 8); FEM(f->tbs_abs, E * 8);
-    FEM(f->leaf_rel, E * 4); FEM(f->leaf_len_out, E * 4); FEM(f->chain_len, E * 4); FEM(f->tbs_len, E * 4); FEM(f->issuer_idx, E * 4);
-    FEM(f->status, E); FEM(f->sha, E * 32); FEM(f->was_unknown, E); FEM(f->first, E); FEM(f->first_meta, 2 * E);
-    FEM(f->exp_hour, E * 8); FEM(f->serial_off, E * 4); FEM(f->serial_len, E * 4); FEM(f->spans, 4 * E * 4);
+    CU(c, alloc(f->scan_temp, f->scan_temp_bytes ? f->scan_temp_bytes : 16));
+    CU(c, alloc(f->entry_status, E)); CU(c, alloc(f->entry_type, E)); CU(c, alloc(f->leaf_src, E)); CU(c, alloc(f->timestamp, E));
+    CU(c, alloc(f->leaf_abs, E)); CU(c, alloc(f->chain_abs, E)); CU(c, alloc(f->tbs_abs, E));
+    CU(c, alloc(f->leaf_rel, E)); CU(c, alloc(f->leaf_len_out, E)); CU(c, alloc(f->chain_len, E)); CU(c, alloc(f->tbs_len, E));
+    CU(c, alloc(f->issuer_idx, E));
+    CU(c, alloc(f->status, E)); CU(c, alloc(f->sha, E * 32)); CU(c, alloc(f->was_unknown, E)); CU(c, alloc(f->first, E));
+    CU(c, alloc(f->first_meta, 2 * E));
+    CU(c, alloc(f->exp_hour, E)); CU(c, alloc(f->serial_off, E)); CU(c, alloc(f->serial_len, E)); CU(c, alloc(f->spans, 4 * E));
     f->slot_mask = pow2_at_least(4ull * c->st.max_issuers) - 1;
-    FEM(f->slots_dev, (f->slot_mask + 1) * sizeof(IssuerCertSlot));
+    CU(c, alloc(f->slots_dev, f->slot_mask + 1));
     f->slots_host.assign(f->slot_mask + 1, IssuerCertSlot{});
     f->pending_mask = (1ull << 16) - 1;
-    FEM(f->pending, (f->pending_mask + 1) * 8);
+    CU(c, alloc(f->pending, f->pending_mask + 1));
     f->unknown_cap = 1u << 14;
-    FEM(f->unknown_list, f->unknown_cap * 4);
-    FEM(f->unknown_count, 16);
-#undef FEM
-    if (cudaMemsetAsync(f->slots_dev, 0, (f->slot_mask + 1) * sizeof(IssuerCertSlot), c->stream) != cudaSuccess ||
-        cudaStreamSynchronize(c->stream) != cudaSuccess ||
-        cudaEventCreate(&f->ev0) != cudaSuccess ||
-        cudaEventCreate(&f->ev1) != cudaSuccess || cudaEventCreate(&f->ev2) != cudaSuccess ||
-        cudaEventCreateWithFlags(&f->mapped, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&f->reduced, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&f->meta_done, cudaEventDisableTiming) != cudaSuccess) {
-        fail(c, CTMR_E_CUDA, "front end: initialisation failed");
-        return bail(CTMR_E_CUDA);
-    }
+    CU(c, alloc(f->unknown_list, f->unknown_cap));
+    CU(c, alloc(f->unknown_count, 4));
+    CU(c, cudaMemsetAsync(f->slots_dev, 0, (f->slot_mask + 1) * sizeof(IssuerCertSlot), c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    CU(c, create(f->ev0, cudaEventDefault)); CU(c, create(f->ev1, cudaEventDefault)); CU(c, create(f->ev2, cudaEventDefault));
+    CU(c, create(f->mapped)); CU(c, create(f->reduced)); CU(c, create(f->meta_done));
     for (const auto& kv : c->issuer_by_der) {  // certificates registered before the front end existed
-        int rc = fe_add_issuer(c, kv.first, kv.second);
+        int rc = fe_add_issuer(c, f.get(), kv.first, kv.second);
         if (rc) return rc;
     }
+    c->fe = std::move(f);
     return CTMR_OK;
 }
 
@@ -611,68 +579,43 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
         (void)cudaGetLastError();
         return fail(nullptr, CTMR_E_NO_DEVICE, "no usable CUDA device (libctmr has no CPU fallback)");
     }
-    ctmr_ctx* c = new (std::nothrow) ctmr_ctx();
+    std::unique_ptr<ctmr_ctx> c(new (std::nothrow) ctmr_ctx());  // failures below report through ctmr_last_error(NULL)
     if (!c) return fail(nullptr, CTMR_E_NOMEM, "host allocation failed");
-    auto bail = [&](int code) {
-        g_create_error = c->err;
-        ctmr_destroy(c);
-        return code;
-    };
     c->device = cfg->device;
     c->flags = cfg->flags;
-    if (build_filter(cfg, c->filter)) {
-        c->err = "issuerCNFilter too long (max 446 bytes, 32 prefixes)";
-        return bail(CTMR_E_INVALID);
-    }
-#define CUC(call)                                                              \
-    do {                                                                       \
-        cudaError_t e_ = (call);                                               \
-        if (e_ != cudaSuccess) {                                               \
-            c->err = std::string(#call) + ": " + cudaGetErrorString(e_);       \
-            return bail(e_ == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA); \
-        }                                                                      \
-    } while (0)
-    CUC(cudaSetDevice(c->device));
+    if (build_filter(cfg, c->filter)) return fail(nullptr, CTMR_E_INVALID, "issuerCNFilter too long (max 446 bytes, 32 prefixes)");
+    CU(nullptr, cudaSetDevice(c->device));
     cudaDeviceProp prop;
-    CUC(cudaGetDeviceProperties(&prop, c->device));
-    if (prop.major != 9 || prop.minor != 0) {
-        c->err = "libctmr is built for sm_90a (H100) only";
-        return bail(CTMR_E_NO_DEVICE);
-    }
+    CU(nullptr, cudaGetDeviceProperties(&prop, c->device));
+    if (prop.major != 9 || prop.minor != 0) return fail(nullptr, CTMR_E_NO_DEVICE, "libctmr is built for sm_90a (H100) only");
     c->sm_count = prop.multiProcessorCount;
-    CUC(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+    CU(nullptr, create(c->stream));
     const uint64_t cap = pow2_at_least(cfg->table_capacity ? cfg->table_capacity : (1ull << 20));
-    if (cap > (1ull << 32) - 16) {
-        c->err = "table_capacity above 2^32 slots";
-        return bail(CTMR_E_INVALID);
-    }
+    if (cap > (1ull << 32) - 16) return fail(nullptr, CTMR_E_INVALID, "table_capacity above 2^32 slots");
     c->st.table_mask = cap - 1;
     const uint32_t plog = cfg->pair_capacity_log2 ? cfg->pair_capacity_log2 : 24;
     const uint32_t mlog = cfg->meta_capacity_log2 ? cfg->meta_capacity_log2 : 20;
-    if (plog > 32 || mlog > 26) {
-        c->err = "pair_capacity_log2 above 32 or meta_capacity_log2 above 26";
-        return bail(CTMR_E_INVALID);
-    }
+    if (plog > 32 || mlog > 26) return fail(nullptr, CTMR_E_INVALID, "pair_capacity_log2 above 32 or meta_capacity_log2 above 26");
     c->st.pair_mask = (1ull << plog) - 1;
     c->st.meta_mask = (1ull << mlog) - 1;  // IssuerMetadata string identities: O(issuers x few)
     c->st.max_issuers = cfg->max_issuers ? cfg->max_issuers : 65536;
     // ONE allocation for everything another rank of a group may address (tables, histograms, barrier flags, issuer
     // registry): one CUDA IPC handle exports it; on a single GPU it is simply this ctx's state
     c->lay = make_layout(cap, c->st.pair_mask + 1, c->st.meta_mask + 1, c->st.max_issuers);
-    CUC(cudaMalloc(&c->shared, c->lay.total));
-    CUC(cudaMemsetAsync(c->shared, 0, c->lay.total, c->stream));
+    CU(nullptr, alloc(c->shared, c->lay.total));
+    CU(nullptr, cudaMemsetAsync(c->shared, 0, c->lay.total, c->stream));
     c->st.table = reinterpret_cast<KnownSlot*>(c->shared + c->lay.table);
     c->st.pairs = reinterpret_cast<PairSlot*>(c->shared + c->lay.pairs);
     c->st.meta = reinterpret_cast<MetaSlot*>(c->shared + c->lay.meta);
     c->st.issuer_counts = reinterpret_cast<unsigned long long*>(c->shared + c->lay.issuer_counts);
     c->st.status_counts = reinterpret_cast<unsigned long long*>(c->shared + c->lay.status_counts);
-    CUC(cudaMalloc(&c->small_dev, 128 * sizeof(unsigned long long)));
-    CUC(cudaMemsetAsync(c->small_dev, 0, 128 * sizeof(unsigned long long), c->stream));
-    c->st.slots_used = c->small_dev + 72;     // [1]
-    c->st.error_flag = reinterpret_cast<int*>(c->small_dev + 73);
+    CU(nullptr, alloc(c->small, 1));
+    CU(nullptr, cudaMemsetAsync(c->small, 0, sizeof(SmallDev), c->stream));
+    c->st.slots_used = &c->small->slots_used;
+    c->st.error_flag = &c->small->error_flag;
     {
         uint8_t* self[1] = {c->shared};
-        attach_views(c, self, 1, 0);  // a single GPU is a group of one
+        attach_views(c.get(), self, 1, 0);  // a single GPU is a group of one
     }
     c->stage_entries = cfg->max_batch_entries ? (cfg->max_batch_entries < kStageEntries ? cfg->max_batch_entries : kStageEntries)
                                               : kStageEntries;
@@ -680,9 +623,8 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
     c->stage_bytes = want_bytes < kStageBytes ? want_bytes : kStageBytes;
     c->cfg_round_entries = cfg->max_round_entries;
     c->px.world = 1;
-    CUC(cudaStreamSynchronize(c->stream));
-#undef CUC
-    *out = c;
+    CU(nullptr, cudaStreamSynchronize(c->stream));
+    *out = c.release();
     return CTMR_OK;
 }
 
@@ -690,33 +632,6 @@ void ctmr_destroy(ctmr_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
-    stages_destroy(c);
-    for (uint32_t r = 0; r < kMaxWorld; ++r) {
-        if (c->ipc_base[r]) cudaIpcCloseMemHandle(c->ipc_base[r]);
-        if (c->ipc_xchg[r]) cudaIpcCloseMemHandle(c->ipc_xchg[r]);
-    }
-    cudaFree(c->xchg); cudaFree(c->cursors); cudaFree(c->rev); cudaFree(c->in_slot); cudaFree(c->in_pair);
-    for (cudaEvent_t e : c->ev_pulled)
-        if (e) cudaEventDestroy(e);
-    cudaFree(c->shared); cudaFree(c->small_dev);
-    cudaFree(c->issuer_map_dev); cudaFree(c->keys_scratch); cudaFree(c->slot_scratch); cudaFree(c->pair_scratch);
-    cudaFree(c->bits_scratch); cudaFree(c->meta_scratch); cudaFree(c->order_scratch); cudaFree(c->len_hist);
-    for (int k = 0; k < kMaxRounds; ++k) {
-        cudaFree(c->len_hist_sub[k]);
-        if (c->ev_map0[k]) cudaEventDestroy(c->ev_map0[k]);
-        if (c->ev_map1[k]) cudaEventDestroy(c->ev_map1[k]);
-        if (c->ev_red1[k]) cudaEventDestroy(c->ev_red1[k]);
-        if (c->ev_tok[k]) cudaEventDestroy(c->ev_tok[k]);
-    }
-    if (c->ev_join_a2) cudaEventDestroy(c->ev_join_a2);
-    if (c->stream_a2) cudaStreamDestroy(c->stream_a2);
-    if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-    if (c->ev_join_a) cudaEventDestroy(c->ev_join_a);
-    if (c->ev_join_b) cudaEventDestroy(c->ev_join_b);
-    if (c->stream_a) cudaStreamDestroy(c->stream_a);
-    if (c->stream_b) cudaStreamDestroy(c->stream_b);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    fe_destroy(c);
     delete c;
 }
 
@@ -767,8 +682,8 @@ int lookup_digest(ctmr_ctx* c, const uint8_t digest[32], bool insert, uint32_t* 
         return CTMR_OK;
     }
     if (!insert) return CTMR_OK;
-    uint8_t* d_dig = reinterpret_cast<uint8_t*>(c->small_dev + 100);  // [4] words = 32 bytes
-    uint32_t* d_idx = reinterpret_cast<uint32_t*>(c->small_dev + 104);
+    uint8_t* d_dig = c->small->digest;
+    uint32_t* d_idx = &c->small->idx;
     uint32_t idx = CTMR_ISSUER_BAD;
     CU(c, cudaMemcpyAsync(d_dig, digest, 32, cudaMemcpyHostToDevice, c->stream));
     CU(c, launch_issuer_registry(c->reg, d_dig, nullptr, 1, d_idx, c->st.error_flag, c->stream));
@@ -786,10 +701,8 @@ int lookup_digest(ctmr_ctx* c, const uint8_t digest[32], bool insert, uint32_t* 
 
 int upload_issuer_map(ctmr_ctx* c, const uint32_t* dense, uint32_t n) {
     if (n > c->issuer_map_cap) {
-        cudaFree(c->issuer_map_dev);
-        c->issuer_map_dev = nullptr;
         c->issuer_map_cap = 0;
-        CU(c, cudaMalloc(&c->issuer_map_dev, (size_t)n * sizeof(uint32_t)));
+        CU(c, alloc(c->issuer_map_dev, n));
         c->issuer_map_cap = n;
     }
     CU(c, cudaMemcpyAsync(c->issuer_map_dev, dense, n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
@@ -830,15 +743,14 @@ int ctmr_register_issuers(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offs
             poff.push_back(packed.size());
         }
         const uint32_t nf = (uint32_t)fresh.size();
-        uint8_t *d_blob = nullptr, *d_dig = nullptr, *d_ok = nullptr;
-        uint64_t* d_off = nullptr;
-        uint32_t* d_idx = nullptr;
-        auto release = [&]() { cudaFree(d_blob); cudaFree(d_off); cudaFree(d_dig); cudaFree(d_ok); cudaFree(d_idx); };
-        CU(c, cudaMalloc(&d_blob, packed.size() + 64));
-        CU(c, cudaMalloc(&d_off, poff.size() * sizeof(uint64_t)));
-        CU(c, cudaMalloc(&d_dig, nf * 32));
-        CU(c, cudaMalloc(&d_ok, nf));
-        CU(c, cudaMalloc(&d_idx, nf * sizeof(uint32_t)));
+        DevBuf<uint8_t> d_blob, d_dig, d_ok;
+        DevBuf<uint64_t> d_off;
+        DevBuf<uint32_t> d_idx;
+        CU(c, alloc(d_blob, packed.size() + 64));
+        CU(c, alloc(d_off, poff.size()));
+        CU(c, alloc(d_dig, nf * 32));
+        CU(c, alloc(d_ok, nf));
+        CU(c, alloc(d_idx, nf));
         CU(c, cudaMemcpyAsync(d_blob, packed.data(), packed.size(), cudaMemcpyHostToDevice, c->stream));
         CU(c, cudaMemcpyAsync(d_off, poff.data(), poff.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
         CU(c, launch_issuer_prepare(d_blob, d_off, nf, d_dig, d_ok, c->stream));
@@ -849,7 +761,6 @@ int ctmr_register_issuers(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offs
         CU(c, cudaMemcpyAsync(ok.data(), d_ok, nf, cudaMemcpyDeviceToHost, c->stream));
         CU(c, cudaMemcpyAsync(idx.data(), d_idx, nf * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
         CU(c, cudaStreamSynchronize(c->stream));
-        release();
         for (uint32_t i = 0; i < nf; ++i) {
             if (ok[i] && idx[i] == CTMR_ISSUER_BAD) {
                 ctmr_check_device(c, nullptr);  // clears the flag
@@ -857,7 +768,7 @@ int ctmr_register_issuers(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offs
             }
             if (ok[i]) c->issuer_by_digest.emplace(std::string(reinterpret_cast<const char*>(dig.data() + 32 * i), 32), idx[i]);
             if (c->fe) {  // first the mirror: a DER it has no room for must not count as registered (a retry fails the same way)
-                int rc2 = fe_add_issuer(c, ders[fresh[i]], idx[i]);
+                int rc2 = fe_add_issuer(c, c->fe.get(), ders[fresh[i]], idx[i]);
                 if (rc2) return rc2;
             }
             c->issuer_by_der.emplace(ders[fresh[i]], idx[i]);
@@ -912,27 +823,9 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     if (!c || !b || !o) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n && (!b->blob || !b->offsets)) return fail(c, CTMR_E_INVALID, "null batch buffers");
     CU(c, cudaSetDevice(c->device));
-    int rc = ensure_scratch(c, b->n);
+    int rc = ensure_device_path(c, b->n);
     if (rc) return rc;
-    rc = ensure_order(c, b->n);
-    if (rc) return rc;
-    if (!c->stream_a) {
-        CU(c, cudaStreamCreateWithFlags(&c->stream_a, cudaStreamNonBlocking));
-        CU(c, cudaStreamCreateWithFlags(&c->stream_a2, cudaStreamNonBlocking));
-        CU(c, cudaEventCreateWithFlags(&c->ev_join_a2, cudaEventDisableTiming));
-        CU(c, cudaStreamCreateWithFlags(&c->stream_b, cudaStreamNonBlocking));
-        CU(c, cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming));
-        CU(c, cudaEventCreateWithFlags(&c->ev_join_a, cudaEventDisableTiming));
-        CU(c, cudaEventCreateWithFlags(&c->ev_join_b, cudaEventDisableTiming));
-        for (int k = 0; k < kMaxRounds; ++k) {
-            CU(c, cudaEventCreate(&c->ev_map0[k]));
-            CU(c, cudaEventCreate(&c->ev_map1[k]));
-            CU(c, cudaEventCreate(&c->ev_red1[k]));
-            CU(c, cudaEventCreateWithFlags(&c->ev_tok[k], cudaEventDisableTiming));
-            CU(c, cudaMalloc(&c->len_hist_sub[k], 256 * sizeof(unsigned int)));
-        }
-        for (cudaEvent_t& e : c->ev_pulled) CU(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    }
+    DevicePipeline& dp = *c->dp;
     const bool want_meta = o->first_issuer_dn || o->first_crldp;
     if (want_meta && !(o->issuer_name_off && o->issuer_name_len && o->crldp_off && o->crldp_len))
         return fail(c, CTMR_E_INVALID, "first_issuer_dn / first_crldp need the four span outputs as well");
@@ -955,10 +848,10 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     if (!all.keys) all.keys = c->keys_scratch;
     if (!all.was_unknown) all.was_unknown = c->bits_scratch;
     if (!all.first_issuer_hour) all.first_issuer_hour = c->bits_scratch + b->n;
-    CU(c, cudaEventRecord(c->ev_fork, user));
-    CU(c, cudaStreamWaitEvent(c->stream_a, c->ev_fork, 0));
-    CU(c, cudaStreamWaitEvent(c->stream_a2, c->ev_fork, 0));
-    CU(c, cudaStreamWaitEvent(c->stream_b, c->ev_fork, 0));
+    CU(c, cudaEventRecord(dp.ev_fork, user));
+    CU(c, cudaStreamWaitEvent(dp.stream_a, dp.ev_fork, 0));
+    CU(c, cudaStreamWaitEvent(dp.stream_a2, dp.ev_fork, 0));
+    CU(c, cudaStreamWaitEvent(dp.stream_b, dp.ev_fork, 0));
     for (int k = 0; k < nsub; ++k) {
         const uint64_t lo = std::min<uint64_t>(b->n, per_round * k), hi = std::min<uint64_t>(b->n, per_round * (k + 1));
         RoundMember x;
@@ -971,32 +864,32 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
         x.db.first_index = coll ? b->first_index + ((uint64_t)k * world + rank) * per_round : b->first_index + lo;
         x.dout = dev_out_at(all, lo);
         x.slot_of = c->slot_scratch + lo; x.pair_slot = c->pair_scratch + lo; x.order = c->order_scratch + lo;
-        x.len_hist = c->len_hist_sub[k];
+        x.len_hist = dp.len_hist[k];
         x.meta_slots = c->meta_scratch + 2 * lo;
         // consecutive K_map launches on alternating streams: the next launch's CTAs fill the SMs the previous one's
         // draining tail leaves idle (a persistent grid ends with its slowest warps)
-        x.map_stream = (k & 1) ? c->stream_a2 : c->stream_a;
-        x.reduce_stream = c->stream_b;
-        x.mapped = c->ev_tok[k];  // K_map + the published sizes; one reduce stream orders the rounds, so no chain
-        x.map_start = c->ev_map0[k];
-        x.map_end = c->ev_map1[k];  // before the publish: map_ms times K_map alone
+        x.map_stream = (k & 1) ? dp.stream_a2 : dp.stream_a;
+        x.reduce_stream = dp.stream_b;
+        x.mapped = dp.ev_tok[k];  // K_map + the published sizes; one reduce stream orders the rounds, so no chain
+        x.map_start = dp.ev_map0[k];
+        x.map_end = dp.ev_map1[k];  // before the publish: map_ms times K_map alone
         x.ch_map = CH_DEV_MAP;
         x.ch_resolve = x.ch_meta = CH_DEV_RESOLVE;  // sync 3 meets no barrier: a collective call has no string identities
         const int parity = k % (int)kParities;
-        if (world > 1 && k >= (int)kParities) CU(c, cudaStreamWaitEvent(x.map_stream, c->ev_pulled[parity], 0));  // the parity's regions are free again
+        if (world > 1 && k >= (int)kParities) CU(c, cudaStreamWaitEvent(x.map_stream, dp.ev_pulled[parity], 0));  // the parity's regions are free again
         ctmr_ctx* failed = nullptr;
         rc = run_round(&x, 1, parity, per_round, want_meta, &failed);
         if (rc) return rc;
-        if (world > 1) CU(c, cudaEventRecord(c->ev_pulled[parity], c->stream_b));
-        CU(c, cudaEventRecord(c->ev_red1[k], c->stream_b));
+        if (world > 1) CU(c, cudaEventRecord(dp.ev_pulled[parity], dp.stream_b));
+        CU(c, cudaEventRecord(dp.ev_red1[k], dp.stream_b));
     }
     c->last_sub = nsub;
-    CU(c, cudaEventRecord(c->ev_join_a2, c->stream_a2));
-    CU(c, cudaStreamWaitEvent(user, c->ev_join_a2, 0));
-    CU(c, cudaEventRecord(c->ev_join_a, c->stream_a));
-    CU(c, cudaEventRecord(c->ev_join_b, c->stream_b));
-    CU(c, cudaStreamWaitEvent(user, c->ev_join_a, 0));
-    CU(c, cudaStreamWaitEvent(user, c->ev_join_b, 0));
+    CU(c, cudaEventRecord(dp.ev_join_a2, dp.stream_a2));
+    CU(c, cudaStreamWaitEvent(user, dp.ev_join_a2, 0));
+    CU(c, cudaEventRecord(dp.ev_join_a, dp.stream_a));
+    CU(c, cudaEventRecord(dp.ev_join_b, dp.stream_b));
+    CU(c, cudaStreamWaitEvent(user, dp.ev_join_a, 0));
+    CU(c, cudaStreamWaitEvent(user, dp.ev_join_b, 0));
     return CTMR_OK;
 }
 
@@ -1013,10 +906,10 @@ int ctmr_profile_last(ctmr_ctx* c, float* map_ms, float* total_ms) {
     float m = 0.f, t = 0.f;
     for (int k = 0; k < c->last_sub; ++k) {
         float d = 0.f;
-        CU(c, cudaEventElapsedTime(&d, c->ev_map0[0], c->ev_map1[k]));
+        CU(c, cudaEventElapsedTime(&d, c->dp->ev_map0[0], c->dp->ev_map1[k]));
         m = d > m ? d : m;
     }
-    CU(c, cudaEventElapsedTime(&t, c->ev_map0[0], c->ev_red1[c->last_sub - 1]));
+    CU(c, cudaEventElapsedTime(&t, c->dp->ev_map0[0], c->dp->ev_red1[c->last_sub - 1]));
     if (map_ms) *map_ms = m;
     if (total_ms) *total_ms = t;
     return CTMR_OK;
@@ -1046,7 +939,7 @@ int ctmr_reset_device(ctmr_ctx* c, void* stream) {
     CU(c, cudaMemsetAsync(c->st.meta, 0, (c->st.meta_mask + 1) * sizeof(MetaSlot), s));
     CU(c, cudaMemsetAsync(c->st.issuer_counts, 0, c->st.max_issuers * sizeof(unsigned long long), s));
     CU(c, cudaMemsetAsync(c->st.status_counts, 0, CTMR_ST__COUNT * sizeof(unsigned long long), s));
-    CU(c, cudaMemsetAsync(c->small_dev + 64, 0, 16 * sizeof(unsigned long long), s));
+    CU(c, cudaMemsetAsync(&c->small->slots_used, 0, offsetof(SmallDev, cardinality), s));  // slots_used and the error flag
     return peer_barrier(c, CH_RESET_B, s);
 }
 
@@ -1169,21 +1062,24 @@ int snap_shard_load(ctmr_ctx* c, const uint8_t* p) {
 
 // the device registry (rank 0's region) again, digest i at index i: cleared, then filled by ONE launch of the
 // find-or-insert kernel, which takes a call's digests in order
-int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n) {
+int snap_registry_alloc(ctmr_ctx* c, uint64_t n, RegistryUpload& u) {
+    CU(c, cudaSetDevice(c->device));
+    if (n) {
+        CU(c, alloc(u.digests, n * 32));
+        CU(c, alloc(u.idx, n));
+    }
+    return CTMR_OK;
+}
+
+int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n, const RegistryUpload& u) {
     CU(c, cudaSetDevice(c->device));
     CU(c, cudaMemsetAsync(c->reg.slots, 0, (c->reg.mask + 1) * sizeof(IssuerRegSlot), c->stream));
     CU(c, cudaMemsetAsync(c->reg.by_index, 0, (size_t)c->reg.max_issuers * 32, c->stream));
     CU(c, cudaMemsetAsync(c->reg.counter, 0, sizeof(unsigned long long), c->stream));
     if (n) {
-        uint8_t* d_dig = nullptr;
-        uint32_t* d_idx = nullptr;
-        CU(c, cudaMalloc(&d_dig, n * 32));
-        CU(c, cudaMalloc(&d_idx, n * sizeof(uint32_t)));
-        CU(c, cudaMemcpyAsync(d_dig, digests, n * 32, cudaMemcpyHostToDevice, c->stream));
-        CU(c, launch_issuer_registry(c->reg, d_dig, nullptr, (uint32_t)n, d_idx, c->st.error_flag, c->stream));
+        CU(c, cudaMemcpyAsync(u.digests, digests, n * 32, cudaMemcpyHostToDevice, c->stream));
+        CU(c, launch_issuer_registry(c->reg, u.digests, nullptr, (uint32_t)n, u.idx, c->st.error_flag, c->stream));
         CU(c, cudaStreamSynchronize(c->stream));
-        cudaFree(d_dig);
-        cudaFree(d_idx);
     }
     int rc = refresh_digests(c);
     if (rc) return rc;
@@ -1245,10 +1141,13 @@ int ctmr_snapshot_load(ctmr_ctx* c, const uint8_t* buf, uint64_t bytes) {
         return fail(c, CTMR_E_INVALID, "snapshot was taken with different capacities (table / pairs / max_issuers)");
     if (bytes < sizeof h + snap_shard_bytes(c) + h.n_issuers * 32 || h.n_issuers > h.max_issuers) return fail(c, CTMR_E_INVALID, "truncated snapshot");
     if (c->st.peer.world > 1) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_snapshot_*");
-    int rc = snap_shard_load(c, buf + sizeof h);
+    RegistryUpload u;
+    int rc = snap_registry_alloc(c, h.n_issuers, u);
+    if (rc) return rc;
+    rc = snap_shard_load(c, buf + sizeof h);
     if (rc) return rc;
     c->next_index = h.next_index;
-    return snap_registry_restore(c, buf + sizeof h + snap_shard_bytes(c), h.n_issuers);
+    return snap_registry_restore(c, buf + sizeof h + snap_shard_bytes(c), h.n_issuers, u);
 }
 
 // ------------------------------------------------------------------------------------------------ tooling
@@ -1256,10 +1155,10 @@ int ctmr_sha256_ceiling_device(ctmr_ctx* c, uint32_t iters, uint32_t rolled, uin
                                uint64_t* blocks_out) {
     if (!c || !iters || !ctas_per_sm || ctas_per_sm > 8) return fail(c, CTMR_E_INVALID, "bad argument");
     CU(c, cudaSetDevice(c->device));
-    cudaEvent_t e0, e1;
-    CU(c, cudaEventCreate(&e0));
-    CU(c, cudaEventCreate(&e1));
-    uint32_t* sink = reinterpret_cast<uint32_t*>(c->small_dev + 90);
+    Event e0, e1;
+    CU(c, create(e0, cudaEventDefault));
+    CU(c, create(e1, cudaEventDefault));
+    uint32_t* sink = &c->small->sha_sink;
     CU(c, launch_sha_ceiling(iters / 8 + 1, (int)rolled, (int)ctas_per_sm, c->sm_count, sink, c->stream));  // warm-up
     CU(c, cudaEventRecord(e0, c->stream));
     CU(c, launch_sha_ceiling(iters, (int)rolled, (int)ctas_per_sm, c->sm_count, sink, c->stream));
@@ -1267,8 +1166,6 @@ int ctmr_sha256_ceiling_device(ctmr_ctx* c, uint32_t iters, uint32_t rolled, uin
     CU(c, cudaEventSynchronize(e1));
     float ms = 0.f;
     CU(c, cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
     if (ms_out) *ms_out = ms;
     if (blocks_out) *blocks_out = (uint64_t)c->sm_count * ctas_per_sm * 256ull * iters;
     return CTMR_OK;
@@ -1306,9 +1203,9 @@ int ctmr_set_cardinality(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32]
     if (rc) return rc;
     if (!found || exp_hour > INT32_MAX || exp_hour < INT32_MIN) return CTMR_OK;
     // one probe of the set's (issuer, hour) slot at its owner -- which may be another GPU of the group
-    CU(c, launch_cardinality(c->st, (int32_t)exp_hour, issuer, c->small_dev + 80, c->stream));
+    CU(c, launch_cardinality(c->st, (int32_t)exp_hour, issuer, &c->small->cardinality, c->stream));
     unsigned long long v = 0;
-    CU(c, cudaMemcpyAsync(&v, c->small_dev + 80, sizeof v, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpyAsync(&v, &c->small->cardinality, sizeof v, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     *out = v;
     return CTMR_OK;
@@ -1326,9 +1223,9 @@ int ctmr_table_stats(ctmr_ctx* c, uint64_t* used, uint64_t* capacity) {
     if (!c) return CTMR_E_INVALID;
     CU(c, cudaSetDevice(c->device));
     unsigned long long u = 0;
-    CU(c, cudaMemsetAsync(c->small_dev + 81, 0, sizeof(unsigned long long), c->stream));
-    CU(c, launch_table_count(c->st, c->small_dev + 81, c->sm_count, c->stream));
-    CU(c, cudaMemcpyAsync(&u, c->small_dev + 81, sizeof u, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemsetAsync(&c->small->table_count, 0, sizeof(unsigned long long), c->stream));
+    CU(c, launch_table_count(c->st, &c->small->table_count, c->sm_count, c->stream));
+    CU(c, cudaMemcpyAsync(&u, &c->small->table_count, sizeof u, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     if (used) *used = u;
     if (capacity) *capacity = c->st.table_mask + 1;
@@ -1342,23 +1239,30 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     CU(c, cudaSetDevice(c->device));
     CU(c, cudaDeviceSynchronize());
     unsigned long long counters[2] = {0, 0};
-    unsigned long long* dev = c->small_dev + 92;  // [92] live, [93] expired, [94] compaction cursor
+    unsigned long long* dev = c->small->evict;  // live, expired, compaction cursor
+    // the count pass takes the expired keys off the per-issuer counts: a copy puts them back if the call cannot go on
+    std::vector<unsigned long long> counts_before(c->st.max_issuers);
+    CU(c, cudaMemcpyAsync(counts_before.data(), c->st.issuer_counts, counts_before.size() * sizeof(unsigned long long),
+                          cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaMemsetAsync(dev, 0, 3 * sizeof(unsigned long long), c->stream));
     CU(c, launch_evict_count(c->st, now_unix_sec, dev, c->sm_count, c->stream));
     CU(c, cudaMemcpyAsync(counters, dev, sizeof counters, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     if (evicted_out) *evicted_out = counters[1];
     if (counters[1] == 0) return CTMR_OK;
-    CU(c, launch_evict_pairs(c->st, now_unix_sec, c->sm_count, c->stream));  // the expired sets' cardinalities are 0 again
     // open addressing with linear probing: taking slots out would cut probe chains, so the survivors are
     // compacted aside, the table is cleared and they are inserted again (first-seen indices preserved)
-    KnownSlot* keep = nullptr;
-    if (counters[0]) CU(c, cudaMalloc(&keep, counters[0] * sizeof(KnownSlot)));
+    DevBuf<KnownSlot> keep;
+    if (counters[0] && alloc(keep, counters[0]) != cudaSuccess) {
+        CU(c, cudaMemcpy(c->st.issuer_counts, counts_before.data(), counts_before.size() * sizeof(unsigned long long),
+                         cudaMemcpyHostToDevice));
+        return fail(c, CTMR_E_NOMEM, "ctmr_evict_expired: no device memory for the surviving keys");
+    }
+    CU(c, launch_evict_pairs(c->st, now_unix_sec, c->sm_count, c->stream));  // the expired sets' cardinalities are 0 again
     if (counters[0]) CU(c, launch_evict_compact(c->st, now_unix_sec, keep, dev + 2, c->sm_count, c->stream));
     CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), c->stream));
     CU(c, launch_evict_reinsert(c->st, keep, counters[0], c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    cudaFree(keep);
     return ctmr_check_device(c, nullptr);
 }
 

@@ -3,12 +3,18 @@
 // one round of the key exchange for all three callers, device entry points, read side, front end plumbing;
 // ctmr_pipeline.cu: the host-buffer batch pipeline on one GPU, on a group of GPUs, and across processes, and the copy of
 // a round's outputs to the host; ctmr_frontend_api.cu: the wire-format front end on one GPU and on a group).
+//
+// Ownership: the ctx owns everything it allocates, through the handles below and std::unique_ptr, so deleting the ctx
+// releases it all.  The parts built on first use (the pipeline stages, ctmr_process_device's streams and events, the
+// front end and its tile and tree state) are built into a local and moved into the ctx only when every allocation
+// succeeded: a failed call leaves the ctx as it was, and the next call tries again.
 #pragma once
 #include <algorithm>
 #include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -21,6 +27,78 @@
 using namespace ctmr;
 
 namespace ctmr_host {
+
+// A handle owns one CUDA resource and releases it in its destructor.  A handle is released only while its ctx's device
+// is current: every entry point sets that device first, and ctmr_destroy sets it before it deletes the ctx.
+template <class P, class Arg, cudaError_t (*Release)(Arg)>
+class Own {
+  public:
+    Own() = default;
+    explicit Own(P p) : p_(p) {}
+    Own(Own&& o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+    Own& operator=(Own&& o) noexcept {
+        if (this != &o) {
+            reset();
+            p_ = o.p_;
+            o.p_ = nullptr;
+        }
+        return *this;
+    }
+    ~Own() { reset(); }
+    void reset() {
+        if (p_) Release(p_);
+        p_ = nullptr;
+    }
+    P get() const { return p_; }
+    operator P() const { return p_; }
+    P operator->() const { return p_; }
+
+  private:
+    P p_ = nullptr;
+};
+
+template <class T> using DevBuf = Own<T*, void*, cudaFree>;
+template <class T> using HostBuf = Own<T*, void*, cudaFreeHost>;  // pinned
+using Stream = Own<cudaStream_t, cudaStream_t, cudaStreamDestroy>;
+using Event = Own<cudaEvent_t, cudaEvent_t, cudaEventDestroy>;
+using IpcMap = Own<uint8_t*, void*, cudaIpcCloseMemHandle>;
+
+// n elements; a buffer the handle held is released first
+template <class T> cudaError_t alloc(DevBuf<T>& b, size_t n) {
+    b.reset();
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, n * sizeof(T));
+    if (e == cudaSuccess) b = DevBuf<T>(static_cast<T*>(p));
+    return e;
+}
+template <class T> cudaError_t alloc(HostBuf<T>& b, size_t n) {
+    b.reset();
+    void* p = nullptr;
+    const cudaError_t e = cudaMallocHost(&p, n * sizeof(T));
+    if (e == cudaSuccess) b = HostBuf<T>(static_cast<T*>(p));
+    return e;
+}
+inline cudaError_t create(Stream& s) {
+    s.reset();
+    cudaStream_t h = nullptr;
+    const cudaError_t e = cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking);
+    if (e == cudaSuccess) s = Stream(h);
+    return e;
+}
+inline cudaError_t create(Event& ev, unsigned flags = cudaEventDisableTiming) {
+    ev.reset();
+    cudaEvent_t h = nullptr;
+    const cudaError_t e = cudaEventCreateWithFlags(&h, flags);
+    if (e == cudaSuccess) ev = Event(h);
+    return e;
+}
+inline cudaError_t open(IpcMap& m, cudaIpcMemHandle_t handle) {
+    m.reset();
+    void* p = nullptr;
+    const cudaError_t e = cudaIpcOpenMemHandle(&p, handle, cudaIpcMemLazyEnablePeerAccess);
+    if (e == cudaSuccess) m = IpcMap(static_cast<uint8_t*>(p));
+    return e;
+}
 
 constexpr int kStages = 3;                      // host-API pipeline depth
 constexpr int kMaxRounds = 16;                  // rounds of one ctmr_process_device call
@@ -37,61 +115,74 @@ inline int env_int(const char* name, int dflt) {
 // device side of the PEM output (ctmr_out.pem): one per host-pipeline stage and one for the front end
 struct PemStage {
     uint64_t cap_entries = 0, cap_bytes = 0;
-    uint64_t *sizes = nullptr, *off = nullptr;
-    uint8_t* text = nullptr;
-    void* scan_temp = nullptr;
+    DevBuf<uint64_t> sizes, off;
+    DevBuf<uint8_t> text;
+    DevBuf<uint8_t> scan_temp;
     size_t scan_temp_bytes = 0;
     std::vector<uint64_t> host_off;
 };
 
 struct Stage {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t mapped = nullptr;   // recorded after this stage's K_map (its inserts have reached the owners' tables)
-    cudaEvent_t reduced = nullptr;  // recorded after this stage's owner passes (resolve + pairs of own entries and inbox records)
-    cudaEvent_t meta_done = nullptr;  // recorded after this stage's string-identity insert
-    uint8_t* blob = nullptr;
-    uint64_t* offsets = nullptr;
-    uint32_t* issuer_idx = nullptr;
-    uint8_t* status = nullptr;
-    uint8_t* sha = nullptr;
-    int64_t* exp_hour = nullptr;
-    uint32_t* serial_off = nullptr;
-    uint32_t* serial_len = nullptr;
-    uint8_t* was_unknown = nullptr;
-    uint8_t* first = nullptr;
-    ctmr_key* keys = nullptr;
-    uint32_t* slot_of = nullptr;
-    uint32_t* pair_slot = nullptr;
-    uint32_t* order = nullptr;
-    unsigned int* len_hist = nullptr;
-    uint32_t* spans = nullptr;       // [4][E]: issuer name off/len, crldp off/len
-    uint32_t* meta_slots = nullptr;  // [2*E]
-    uint8_t* first_meta = nullptr;   // [2][E]: first_issuer_dn, first_crldp
-    PemStage pem;                    // allocated when a caller first asks for PEM output
+    Stream stream;
+    Event mapped;     // recorded after this stage's K_map (its inserts have reached the owners' tables)
+    Event reduced;    // recorded after this stage's owner passes (resolve + pairs of own entries and inbox records)
+    Event meta_done;  // recorded after this stage's string-identity insert
+    DevBuf<uint8_t> blob;
+    DevBuf<uint64_t> offsets;
+    DevBuf<uint32_t> issuer_idx;
+    DevBuf<uint8_t> status;
+    DevBuf<uint8_t> sha;
+    DevBuf<int64_t> exp_hour;
+    DevBuf<uint32_t> serial_off;
+    DevBuf<uint32_t> serial_len;
+    DevBuf<uint8_t> was_unknown;
+    DevBuf<uint8_t> first;
+    DevBuf<ctmr_key> keys;
+    DevBuf<uint32_t> slot_of;
+    DevBuf<uint32_t> pair_slot;
+    DevBuf<uint32_t> order;
+    DevBuf<unsigned int> len_hist;
+    DevBuf<uint32_t> spans;       // [4][E]: issuer name off/len, crldp off/len
+    DevBuf<uint32_t> meta_slots;  // [2*E]
+    DevBuf<uint8_t> first_meta;   // [2][E]: first_issuer_dn, first_crldp
+    PemStage pem;                 // allocated when a caller first asks for PEM output
+};
+
+// ctmr_process_device pipelines map (stream A) against reduce (stream B) over its rounds
+struct DevicePipeline {
+    Stream stream_a, stream_a2, stream_b;  // K_map alternates between a and a2
+    Event ev_fork, ev_join_a, ev_join_a2, ev_join_b;
+    Event ev_map0[kMaxRounds], ev_map1[kMaxRounds], ev_red1[kMaxRounds];  // timed: ctmr_profile_last
+    Event ev_tok[kMaxRounds];
+    DevBuf<unsigned int> len_hist[kMaxRounds];
+    Event ev_pulled[kParities];  // round k's bits pulled (its exchange parity may be reused)
 };
 
 // one upload stage of the front end: a chunk's characters and string spans, device side and pinned host staging
 struct FeStage {
-    uint8_t* text = nullptr;  // [16 + cap_text + 64]
-    uint64_t *leaf_off = nullptr, *extra_off = nullptr, *h_leaf_off = nullptr, *h_extra_off = nullptr;
-    uint32_t *leaf_len = nullptr, *extra_len = nullptr, *h_leaf_len = nullptr, *h_extra_len = nullptr;
-    cudaEvent_t uploaded = nullptr, consumed = nullptr;
+    DevBuf<uint8_t> text;  // [16 + cap_text + 64]
+    DevBuf<uint64_t> leaf_off, extra_off;
+    HostBuf<uint64_t> h_leaf_off, h_extra_off;
+    DevBuf<uint32_t> leaf_len, extra_len;
+    HostBuf<uint32_t> h_leaf_len, h_extra_len;
+    Event uploaded, consumed;
     std::vector<uint8_t> pack;  // host staging of the slow path (strings scattered over more than one chunk of text)
 };
 
 // static-ct-api tiles (ctmr_process_tiles): per-chunk buffers beyond the front end's, and the fingerprint table.
 // Allocated on the first tile call or chain-certificate registration.
 struct TileState {
-    TileDesc *tiles[2] = {}, *h_tiles[2] = {};  // per upload stage: the chunk's tiles, device and pinned host
-    uint8_t* tile_bad = nullptr;
-    uint64_t *entry_off = nullptr, *leaf_index = nullptr, *leaf_data_off = nullptr;
-    uint32_t *entry_tile = nullptr, *te_len = nullptr;
-    unsigned int* first_stop = nullptr;
-    uint8_t* leaf_hash = nullptr;
-    cudaEvent_t ev_split0 = nullptr, ev_split1 = nullptr;  // around tile_split: the serial walk is timed on its own
+    DevBuf<TileDesc> tiles[2];  // per upload stage: the chunk's tiles, device and pinned host
+    HostBuf<TileDesc> h_tiles[2];
+    DevBuf<uint8_t> tile_bad;
+    DevBuf<uint64_t> entry_off, leaf_index, leaf_data_off;
+    DevBuf<uint32_t> entry_tile, te_len;
+    DevBuf<unsigned int> first_stop;
+    DevBuf<uint8_t> leaf_hash;
+    Event ev_split0, ev_split1;  // around tile_split: the serial walk is timed on its own
     float split_ms = 0.f;
     // fingerprint -> dense issuer index: device table, host copy, host memo keyed by the 32 bytes
-    FpSlot* fp_dev = nullptr;
+    DevBuf<FpSlot> fp_dev;
     std::vector<FpSlot> fp_host;
     uint64_t fp_mask = 0, fp_used = 0;
     std::unordered_map<std::string, uint32_t> fp_memo;
@@ -100,10 +191,10 @@ struct TileState {
 // the log's Merkle tree (ctmr_process_raw_tree / ctmr_process_tiles_tree): the call's tree on the device and the scratch
 // of the fold.  Allocated on the first tree call.
 struct TreeState {
-    TreeDev* dev = nullptr;       // the tree for the whole call: uploaded at its start, read back at its end
-    TreeDev* host = nullptr;      // pinned staging of those two copies
-    uint8_t* leaf = nullptr;      // [cap_entries][32] get-entries leaf hashes of a chunk
-    uint8_t* lvl[2] = {};         // [cap_entries / 2 + 2][32] each: ping-pong level buffers
+    DevBuf<TreeDev> dev;          // the tree for the whole call: uploaded at its start, read back at its end
+    HostBuf<TreeDev> host;        // pinned staging of those two copies
+    DevBuf<uint8_t> leaf;         // [cap_entries][32] get-entries leaf hashes of a chunk
+    DevBuf<uint8_t> lvl[2];       // [cap_entries / 2 + 2][32] each: ping-pong level buffers
     uint64_t base = 0;            // log position of the call's first entry
     bool active = false;          // a tree call is running: the chunks fold their leaves
 };
@@ -113,37 +204,49 @@ struct TreeState {
 struct FrontEnd {
     uint64_t cap_entries = 0, cap_text = 0, cap_decoded = 0;
     FeStage stage[2];          // upload double buffer
-    cudaStream_t copy_stream = nullptr;
-    uint64_t *pad_size = nullptr, *dec_off = nullptr;
-    uint32_t* dec_len = nullptr;
-    uint8_t *str_bad = nullptr, *decoded = nullptr;
-    void* scan_temp = nullptr;
+    Stream copy_stream;
+    DevBuf<uint64_t> pad_size, dec_off;
+    DevBuf<uint32_t> dec_len;
+    DevBuf<uint8_t> str_bad, decoded;
+    DevBuf<uint8_t> scan_temp;
     size_t scan_temp_bytes = 0;
-    uint8_t *entry_status = nullptr, *entry_type = nullptr, *leaf_src = nullptr;
-    uint64_t *timestamp = nullptr, *leaf_abs = nullptr, *chain_abs = nullptr, *tbs_abs = nullptr;
-    uint32_t *leaf_rel = nullptr, *leaf_len_out = nullptr, *chain_len = nullptr, *tbs_len = nullptr, *issuer_idx = nullptr;
+    DevBuf<uint8_t> entry_status, entry_type, leaf_src;
+    DevBuf<uint64_t> timestamp, leaf_abs, chain_abs, tbs_abs;
+    DevBuf<uint32_t> leaf_rel, leaf_len_out, chain_len, tbs_len, issuer_idx;
     // outputs of the path for this chunk
-    uint8_t *status = nullptr, *sha = nullptr, *was_unknown = nullptr, *first = nullptr, *first_meta = nullptr;
-    int64_t* exp_hour = nullptr;
-    uint32_t *serial_off = nullptr, *serial_len = nullptr, *spans = nullptr;
+    DevBuf<uint8_t> status, sha, was_unknown, first, first_meta;
+    DevBuf<int64_t> exp_hour;
+    DevBuf<uint32_t> serial_off, serial_len, spans;
     // issuer certificates by bytes
-    IssuerCertSlot* slots_dev = nullptr;
+    DevBuf<IssuerCertSlot> slots_dev;
     std::vector<IssuerCertSlot> slots_host;
     uint64_t slot_mask = 0, slots_used = 0;
-    uint8_t* arena = nullptr;
+    DevBuf<uint8_t> arena;
     uint64_t arena_cap = 0, arena_used = 0;
-    uint64_t* pending = nullptr;
+    DevBuf<uint64_t> pending;
     uint64_t pending_mask = 0;
-    uint32_t* unknown_list = nullptr;
+    DevBuf<uint32_t> unknown_list;
     uint32_t unknown_cap = 0;
-    unsigned int* unknown_count = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
-    cudaEvent_t mapped = nullptr, reduced = nullptr, meta_done = nullptr;  // round events of the group front end (fe_member)
+    DevBuf<unsigned int> unknown_count;
+    Event ev0, ev1, ev2;
+    Event mapped, reduced, meta_done;  // round events of the group front end (fe_member)
     float fe_ms = 0.f, path_ms = 0.f;
     uint64_t launches = 0;
     PemStage pem;
-    TileState* tl = nullptr;   // tiles_ensure
-    TreeState* tree = nullptr; // tree_ensure
+    std::unique_ptr<TileState> tl;    // tiles_ensure
+    std::unique_ptr<TreeState> tree;  // tree_ensure
+};
+
+// the ctx's private device words (one allocation)
+struct SmallDev {
+    unsigned long long slots_used;   // DeviceState::slots_used points here (no kernel reads it)
+    int error_flag;                  // DeviceState::error_flag
+    unsigned long long cardinality;  // ctmr_set_cardinality's probe result
+    unsigned long long table_count;  // ctmr_table_stats' count
+    unsigned long long evict[3];     // ctmr_evict_expired: live, expired, compaction cursor
+    uint32_t sha_sink;               // ctmr_sha256_ceiling_device's sink
+    alignas(16) uint8_t digest[32];  // lookup_digest: one digest to register
+    uint32_t idx;                    //   and its index
 };
 
 }  // namespace ctmr_host
@@ -177,56 +280,50 @@ struct ctmr_ctx {
     int device = 0;
     int sm_count = 132;
     uint32_t flags = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     DeviceState st{};
     FilterCfg filter{};
     uint64_t next_index = 0;
     uint64_t stage_entries = 0, stage_bytes = 0;
-    bool stages_ready = false;
-    Stage stages[kStages];
+    std::unique_ptr<Stage[]> stages;  // [kStages], ensure_stages
     // shared region + the views of every rank's region (a single GPU is a group of one)
-    uint8_t* shared = nullptr;
+    DevBuf<uint8_t> shared;
     SharedLayout lay{};
     PeerFlags pf{};
     IssuerRegistry reg{};                  // lives in rank 0's region
     int peer_mode = PEER_NONE;
-    void* ipc_base[kMaxWorld] = {};        // mappings opened with cudaIpcOpenMemHandle (closed on destroy)
-    void* ipc_xchg[kMaxWorld] = {};
+    IpcMap ipc_base[kMaxWorld];            // the other ranks' regions, opened with cudaIpcOpenMemHandle
+    IpcMap ipc_xchg[kMaxWorld];
     // key exchange of a group: peer-visible area (inboxes, result bits, region sizes) + private bookkeeping
-    uint8_t* xchg = nullptr;
+    DevBuf<uint8_t> xchg;
     uint64_t X = 0, cfg_round_entries = 0;
     uint32_t exported_world = 0;            // ctmr_peer_export was called for a group of this size (the views follow at attach)
     PeerExchange px{};
-    unsigned long long* cursors = nullptr;  // [kParities][kMaxWorld] records appended per owner (local)
-    uint32_t* rev = nullptr;                // [kParities][world][X] inbox position -> entry
-    uint32_t *in_slot = nullptr, *in_pair = nullptr;  // [kParities][world][X] owner-side scratch of the inbox records
-    cudaEvent_t ev_pulled[kParities] = {};  // ctmr_process_device: round k's bits pulled (its exchange parity may be reused)
+    DevBuf<unsigned long long> cursors;     // [kParities][kMaxWorld] records appended per owner (local)
+    DevBuf<uint32_t> rev;                   // [kParities][world][X] inbox position -> entry
+    DevBuf<uint32_t> in_slot, in_pair;      // [kParities][world][X] owner-side scratch of the inbox records
     unsigned long long epoch[kPeerChannels] = {};
     struct ctmr_group* group = nullptr;    // set when the ctx is a member of an in-process group
     // issuer memo on the host (the registry itself is on the device): DER -> index, digest -> index, index -> digest
     std::unordered_map<std::string, uint32_t> issuer_by_der;
     std::unordered_map<std::string, uint32_t> issuer_by_digest;
     std::vector<std::array<uint8_t, 32>> digests;
-    uint32_t* issuer_map_dev = nullptr;
+    DevBuf<uint32_t> issuer_map_dev;
     uint32_t issuer_map_cap = 0;
     // scratch of the device-resident entry points
-    ctmr_key* keys_scratch = nullptr;
-    uint32_t* slot_scratch = nullptr;
-    uint32_t* pair_scratch = nullptr;
-    uint8_t* bits_scratch = nullptr;
-    uint32_t* meta_scratch = nullptr;  // [2*cap]
+    DevBuf<ctmr_key> keys_scratch;
+    DevBuf<uint32_t> slot_scratch;
+    DevBuf<uint32_t> pair_scratch;
+    DevBuf<uint8_t> bits_scratch;
+    DevBuf<uint32_t> meta_scratch;  // [2*cap]
     uint64_t scratch_cap = 0;
-    uint32_t* order_scratch = nullptr;  // length-bucketed order of the device entry points (ensure_order)
+    DevBuf<uint32_t> order_scratch;  // length-bucketed order of the device entry points (ensure_order)
     uint64_t order_cap = 0;
-    unsigned int* len_hist = nullptr;
-    // ctmr_process_device pipelines map (stream A) against reduce (stream B) over kSub sub-batches
-    cudaStream_t stream_a = nullptr, stream_a2 = nullptr, stream_b = nullptr;  // K_map alternates between a and a2
-    cudaEvent_t ev_fork = nullptr, ev_join_a = nullptr, ev_join_a2 = nullptr, ev_join_b = nullptr;
-    cudaEvent_t ev_map0[kMaxRounds] = {}, ev_map1[kMaxRounds] = {}, ev_red1[kMaxRounds] = {}, ev_tok[kMaxRounds] = {};
+    DevBuf<unsigned int> len_hist;
+    std::unique_ptr<DevicePipeline> dp;  // ctmr_process_device
     int last_sub = 0;
-    unsigned int* len_hist_sub[kMaxRounds] = {};
-    unsigned long long* small_dev = nullptr;  // [128] private counters / cursors / results (error flag at +73; words 84..87 unused)
-    FrontEnd* fe = nullptr;
+    DevBuf<SmallDev> small;
+    std::unique_ptr<FrontEnd> fe;
     std::string err;
 };
 
@@ -296,17 +393,20 @@ int ensure_stages(ctmr_ctx* c);
 uint64_t snap_shard_bytes(ctmr_ctx* c);
 int snap_shard_save(ctmr_ctx* c, uint8_t* p);
 int snap_shard_load(ctmr_ctx* c, const uint8_t* p);
-int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n);
+// a snapshot's issuer digests on their way into the registry: allocated before a load overwrites anything
+struct RegistryUpload {
+    DevBuf<uint8_t> digests;
+    DevBuf<uint32_t> idx;
+};
+int snap_registry_alloc(ctmr_ctx* c, uint64_t n, RegistryUpload& u);
+int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n, const RegistryUpload& u);
 int frontend_ensure(ctmr_ctx* c);   // allocates the front end's buffers on first use (ctmr_api.cu)
 int tiles_ensure(ctmr_ctx* c);      // ... and the tile buffers + fingerprint table (ctmr_frontend_api.cu), after frontend_ensure
-void tiles_free(FrontEnd* f);
 int tiles_clear_fingerprints(ctmr_ctx* c);
-void tree_free(FrontEnd* f);        // the Merkle tree's state (ctmr_frontend_api.cu)
 int ensure_scratch(ctmr_ctx* c, uint64_t n);
+int ensure_device_path(ctmr_ctx* c, uint64_t n);   // what ctmr_process_device needs for n entries
 uint64_t device_round_entries(uint64_t n, uint32_t rounds);   // E of a ctmr_process_device call cut into `rounds` rounds
 uint32_t peer_rounds();   // rounds of the collective ctmr_process_device (CTMR_PEER_ROUNDS, env override for experiments)
-void pem_free(PemStage& ps);
-void stages_destroy(ctmr_ctx* c);
 int pem_ensure(ctmr_ctx* c, PemStage& ps, uint64_t entries, uint64_t der_bytes);
 int pem_chunk(ctmr_ctx* c, PemStage& ps, const uint8_t* blob, const uint64_t* offsets, const uint32_t* lens, const uint8_t* select,
               uint64_t cnt, const ctmr_out* out, uint64_t first, uint64_t* base, cudaStream_t s);

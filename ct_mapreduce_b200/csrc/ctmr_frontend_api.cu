@@ -60,7 +60,7 @@ ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
     const uint64_t E = f->cap_entries;
     ctmr_dev_out dout{};
     dout.status = f->status;
-    dout.sha256 = po->sha256 ? f->sha : nullptr;
+    dout.sha256 = po->sha256 ? f->sha.get() : nullptr;
     dout.exp_hour = f->exp_hour;
     dout.serial_off = f->serial_off;
     dout.serial_len = f->serial_len;
@@ -93,20 +93,16 @@ int fe_prepare(ctmr_ctx* c) {
 
 // ---- the log's Merkle tree (ctmr_process_raw_tree, ctmr_process_tiles_tree) ----------------------------------------------
 int tree_ensure(ctmr_ctx* c) {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     if (f->tree) return CTMR_OK;
-    TreeState* tr = new (std::nothrow) TreeState();
+    std::unique_ptr<TreeState> tr(new (std::nothrow) TreeState());
     if (!tr) return fail(c, CTMR_E_NOMEM, "host allocation failed");
-    f->tree = tr;
     const uint64_t E = f->cap_entries;
-    cudaError_t e = cudaMalloc(&tr->dev, sizeof(TreeDev));
-    if (e == cudaSuccess) e = cudaMallocHost(&tr->host, sizeof(TreeDev));
-    if (e == cudaSuccess) e = cudaMalloc(&tr->leaf, E * 32);
-    for (int k = 0; k < 2 && e == cudaSuccess; ++k) e = cudaMalloc(&tr->lvl[k], (E / 2 + 2) * 32);
-    if (e != cudaSuccess) {
-        tree_free(f);
-        return fail(c, e == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA, std::string("tree: ") + cudaGetErrorString(e));
-    }
+    CU(c, alloc(tr->dev, 1));
+    CU(c, alloc(tr->host, 1));
+    CU(c, alloc(tr->leaf, E * 32));
+    for (DevBuf<uint8_t>& lvl : tr->lvl) CU(c, alloc(lvl, (E / 2 + 2) * 32));
+    f->tree = std::move(tr);
     return CTMR_OK;
 }
 
@@ -114,7 +110,7 @@ int tree_ensure(ctmr_ctx* c) {
 int tree_begin(ctmr_ctx* c, const ctmr_tree* tree, uint64_t base) {
     int rc = tree_ensure(c);
     if (rc) return rc;
-    TreeState* tr = c->fe->tree;
+    TreeState* tr = c->fe->tree.get();
     std::memcpy(&tr->host->t, tree, sizeof(ctmr_tree));
     tr->host->missing = ~0ull;
     CU(c, cudaMemcpyAsync(tr->dev, tr->host, sizeof(TreeDev), cudaMemcpyHostToDevice, c->stream));
@@ -125,17 +121,18 @@ int tree_begin(ctmr_ctx* c, const ctmr_tree* tree, uint64_t base) {
 
 // folds entries [0, cnt) of a chunk, log positions first_pos.., into the tree (see FoldChunk)
 int tree_fold(ctmr_ctx* c, const uint8_t* leaves, const uint8_t* flags, uint32_t stride, uint32_t match, uint64_t first_pos, uint64_t cnt) {
-    TreeState* tr = c->fe->tree;
+    TreeState* tr = c->fe->tree.get();
     const FoldChunk fc{tr->dev, leaves, flags, stride, match, first_pos, cnt};
+    uint8_t* const lvl[2] = {tr->lvl[0], tr->lvl[1]};
     uint32_t launches = 0;
-    CU(c, launch_tree_fold(fc, tr->lvl, c->stream, &launches));
+    CU(c, launch_tree_fold(fc, lvl, c->stream, &launches));
     c->fe->launches += launches;
     return CTMR_OK;
 }
 
 // the root, and the tree back to the caller
 int tree_end(ctmr_ctx* c, ctmr_tree* tree) {
-    TreeState* tr = c->fe->tree;
+    TreeState* tr = c->fe->tree.get();
     CU(c, launch_tree_root(tr->dev, c->stream));
     CU(c, cudaMemcpyAsync(tr->host, tr->dev, sizeof(TreeDev), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
@@ -153,7 +150,8 @@ struct Pages {
     static constexpr bool kStageHoldsLeaves = false;
     const ctmr_raw_batch* b;
     ctmr_raw_out* out;
-    uint64_t done;  // entries that take their indices: all n whenever there is a batch, also when the call fails
+    uint64_t done;  // entries that take their indices: all n whenever there is a batch, also when the call fails once a
+                    // chunk has reached the path
 
     Pages(const ctmr_raw_batch* b_, ctmr_raw_out* out_) : b(b_), out(out_), done(b_ ? b_->n : 0) {}
     int check(ctmr_ctx* c, const ctmr_tree* tree) const;
@@ -183,7 +181,7 @@ int Pages::check(ctmr_ctx* c, const ctmr_tree* tree) const {
 // How many entries starting at `lo` fit one chunk (at most max_entries): entry budget and half the character budget
 // (the other half belongs to the stage being uploaded next).  Also validates the spans.
 int Pages::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_entries, uint64_t* hi_out) const {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     uint64_t hi = lo, chars = 0;
     while (hi < b->n && hi - lo < max_entries && hi - lo < f->cap_entries) {
         const uint64_t l1 = b->leaf_input_off[hi] + b->leaf_input_len[hi], x1 = b->extra_data_off[hi] + b->extra_data_len[hi];
@@ -199,7 +197,7 @@ int Pages::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_entries, uint64_t* hi_out)
 
 // Characters and spans of entries [lo, hi) into upload stage ch.stage, asynchronously on the copy stream.
 int Pages::upload(ctmr_ctx* c, Chunk& ch) const {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     FeStage& st = f->stage[ch.stage];
     const uint64_t lo = ch.lo, cnt = ch.hi - ch.lo;
     ch.e0 = ch.lo;
@@ -252,7 +250,7 @@ int Pages::upload(ctmr_ctx* c, Chunk& ch) const {
 
 // decode + frame + Chain[0] -> dense index of an uploaded chunk; leaves ch.db / ch.dout describing the device-resident batch
 int Pages::front(ctmr_ctx* c, Chunk& ch) const {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     cudaStream_t s = c->stream;
     CU(c, cudaSetDevice(c->device));
     FeStage& st = f->stage[ch.stage];
@@ -341,7 +339,7 @@ int Pages::front(ctmr_ctx* c, Chunk& ch) const {
 
 // the front end's own outputs of a chunk, after the path's; waits for the chunk
 int Pages::copy_back(ctmr_ctx* c, const Chunk& ch) const {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     cudaStream_t s = c->stream;
     const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0;
     if (cnt) {
@@ -432,7 +430,7 @@ int Tiles::prepare(ctmr_ctx* c) const {
 
 // How many tiles starting at `lo` fit one chunk (at most max_tiles): the entry budget and half the byte budget
 int Tiles::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) const {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     uint64_t hi = lo, bytes = 0;
     while (hi < b->n_tiles && hi - lo < max_tiles && ent[hi + 1] - ent[lo] <= f->cap_entries && bytes + b->tile_len[hi] <= f->cap_text / 2) {
         bytes += b->tile_len[hi];
@@ -444,8 +442,8 @@ int Tiles::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) c
 
 // tiles [lo, hi) into upload stage ch.stage, asynchronously on the copy stream
 int Tiles::upload(ctmr_ctx* c, Chunk& ch) const {
-    FrontEnd* f = c->fe;
-    TileState* tl = f->tl;
+    FrontEnd* f = c->fe.get();
+    TileState* tl = f->tl.get();
     FeStage& st = f->stage[ch.stage];
     CU(c, cudaSetDevice(c->device));
     CU(c, cudaStreamWaitEvent(f->copy_stream, st.consumed, 0));  // the chunk that last used this stage is done with it
@@ -490,8 +488,8 @@ int Tiles::upload(ctmr_ctx* c, Chunk& ch) const {
 // split + frame + fingerprint -> dense index of an uploaded chunk.  A chunk holding a tile with an unknown Chain[0]
 // fingerprint is cut before that tile (ch.stopped, ch.missing).  Leaves ch.db / ch.dout describing the device-resident batch.
 int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
-    FrontEnd* f = c->fe;
-    TileState* tl = f->tl;
+    FrontEnd* f = c->fe.get();
+    TileState* tl = f->tl.get();
     cudaStream_t s = c->stream;
     CU(c, cudaSetDevice(c->device));
     FeStage& st = f->stage[ch.stage];
@@ -571,8 +569,8 @@ int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
 
 // the front end's own outputs of a chunk, after the path's; waits for the chunk
 int Tiles::copy_back(ctmr_ctx* c, const Chunk& ch) const {
-    FrontEnd* f = c->fe;
-    TileState* tl = f->tl;
+    FrontEnd* f = c->fe.get();
+    TileState* tl = f->tl.get();
     cudaStream_t s = c->stream;
     const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0, nt = ch.hi - ch.lo;
     std::vector<uint8_t> bad(nt);
@@ -720,7 +718,7 @@ int run_path(ctmr_ctx** m, uint32_t W, int k, Chunk* cur, bool meta, ctmr_ctx** 
 // after the path: x509 leaf failures, PEM, outputs to the host; waits for the chunk
 template <class Format>
 int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     cudaStream_t s = c->stream;
     CU(c, cudaSetDevice(c->device));
     const uint64_t cnt = ch.e1 - ch.e0;
@@ -731,9 +729,7 @@ int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
     }
     CU(c, cudaEventRecord(f->ev2, s));
     if (cnt && po->pem) {  // the new certificates' PEM, encoded from the DER in HBM
-        int rc = pem_ensure(c, f->pem, f->cap_entries, f->cap_decoded);
-        if (rc) return rc;
-        rc = pem_chunk(c, f->pem, ch.p.fe.decoded, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, ch.e0, pem_base, s);
+        const int rc = pem_chunk(c, f->pem, ch.p.fe.decoded, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, ch.e0, pem_base, s);
         if (rc) return rc;
     }
     if (Format::kStageHoldsLeaves) CU(c, cudaEventRecord(f->stage[ch.stage].consumed, s));  // the leaves' last read is done
@@ -760,11 +756,18 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
     *failed = m[0];
     int rc = fm.check(m[0], tree);
     if (rc) return rc;
+    // The entries take their indices once a chunk reaches the path; a call that fails before has changed no table.
+    const uint64_t takes = fm.done;
+    fm.done = 0;
     const uint64_t total = fm.units();
     if (total == 0 && !tree) return CTMR_OK;
+    const ctmr_out* po = &fm.out->path;
+    // everything the call builds on first use, before its first kernel
     for (uint32_t r = 0; r < W; ++r) {
         *failed = m[r];
         rc = fm.prepare(m[r]);
+        if (rc == CTMR_OK && po->pem) rc = pem_ensure(m[r], m[r]->fe->pem, m[r]->fe->cap_entries, m[r]->fe->cap_decoded);
+        if (rc == CTMR_OK && W == 1) rc = ensure_device_path(m[r], m[r]->fe->cap_entries);  // ctmr_process_device
         if (rc) return rc;
     }
     *failed = m[0];
@@ -773,7 +776,6 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
         if (rc) return rc;
         if (total == 0) return tree_end(m[0], tree);
     }
-    const ctmr_out* po = &fm.out->path;
     uint64_t pem_base = 0;
     std::vector<Chunk> ch[2];  // round k's chunks in ch[k & 1], uploaded into stage k & 1
     rc = plan_round(m, W, fm, 0, 0, ch[0], failed);
@@ -797,6 +799,7 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
             else if (cur[r].stopped) stop = r;
             cur[r].db.first_index = *next_index + cur[r].e0;
         }
+        fm.done = takes;
         rc = run_path(m, W, k, cur, want_meta(po), failed);
         if (rc) return rc;
         // in entry order when there is PEM (the texts are appended in that order); otherwise each member writes its own
@@ -857,26 +860,23 @@ int register_chain_certs(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offse
     int rc = frontend_ensure(c);
     if (rc == CTMR_OK) rc = tiles_ensure(c);
     if (rc || n == 0) return rc;
-    TileState* tl = c->fe->tl;
+    TileState* tl = c->fe->tl.get();
     for (uint32_t k = 0; k < n; ++k)
         if (offsets[k + 1] < offsets[k]) return fail(c, CTMR_E_INVALID, "chain certificate offsets not monotonic");
     const uint64_t base = offsets[0], bytes = offsets[n] - base;
     std::vector<uint64_t> rel(n + 1);
     for (uint32_t k = 0; k <= n; ++k) rel[k] = offsets[k] - base;
     std::vector<uint8_t> fps(32ull * n);
-    uint8_t *d_blob = nullptr, *d_fp = nullptr;
-    uint64_t* d_off = nullptr;
-    auto release = [&]() { cudaFree(d_blob); cudaFree(d_off); cudaFree(d_fp); };
-    cudaError_t e = cudaMalloc(&d_blob, bytes + 64);
-    if (e == cudaSuccess) e = cudaMalloc(&d_off, (n + 1) * 8ull);
-    if (e == cudaSuccess) e = cudaMalloc(&d_fp, 32ull * n);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blob, blob + base, bytes, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, rel.data(), (n + 1) * 8ull, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = launch_fingerprints(d_blob, d_off, n, d_fp, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(fps.data(), d_fp, 32ull * n, cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    release();
-    if (e != cudaSuccess) return fail(c, CTMR_E_CUDA, std::string("chain certificate fingerprints: ") + cudaGetErrorString(e));
+    DevBuf<uint8_t> d_blob, d_fp;
+    DevBuf<uint64_t> d_off;
+    CU(c, alloc(d_blob, bytes + 64));
+    CU(c, alloc(d_off, n + 1));
+    CU(c, alloc(d_fp, 32ull * n));
+    CU(c, cudaMemcpyAsync(d_blob, blob + base, bytes, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(d_off, rel.data(), (n + 1) * 8ull, cudaMemcpyHostToDevice, c->stream));
+    CU(c, launch_fingerprints(d_blob, d_off, n, d_fp, c->stream));
+    CU(c, cudaMemcpyAsync(fps.data(), d_fp, 32ull * n, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
     if (fp_out) std::memcpy(fp_out, fps.data(), fps.size());
     std::vector<uint32_t> fresh;  // first position of each fingerprint the table does not hold yet
     std::unordered_map<std::string, uint32_t> seen;
@@ -985,64 +985,36 @@ int ctmr_group_register_chain_certs(ctmr_group* g, const uint8_t* blob, const ui
 namespace ctmr_host {
 
 int tiles_ensure(ctmr_ctx* c) {
-    FrontEnd* f = c->fe;
+    FrontEnd* f = c->fe.get();
     if (f->tl) return CTMR_OK;
-    TileState* tl = new (std::nothrow) TileState();
+    std::unique_ptr<TileState> tl(new (std::nothrow) TileState());
     if (!tl) return fail(c, CTMR_E_NOMEM, "host allocation failed");
-    f->tl = tl;
     const uint64_t E = f->cap_entries;
     tl->fp_mask = pow2_at_least(4ull * c->st.max_issuers) - 1;
     tl->fp_host.assign(tl->fp_mask + 1, FpSlot{});
-    cudaError_t e = cudaSuccess;
-    for (int k = 0; k < 2 && e == cudaSuccess; ++k) {
-        e = cudaMalloc(&tl->tiles[k], E * sizeof(TileDesc));
-        if (e == cudaSuccess) e = cudaMallocHost(&tl->h_tiles[k], E * sizeof(TileDesc));
+    for (int k = 0; k < 2; ++k) {
+        CU(c, alloc(tl->tiles[k], E));
+        CU(c, alloc(tl->h_tiles[k], E));
     }
-    if (e == cudaSuccess) e = cudaMalloc(&tl->tile_bad, E);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->entry_off, E * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->leaf_index, E * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->leaf_data_off, E * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->entry_tile, E * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->te_len, E * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->first_stop, 16);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->leaf_hash, E * 32);
-    if (e == cudaSuccess) e = cudaMalloc(&tl->fp_dev, (tl->fp_mask + 1) * sizeof(FpSlot));
-    if (e == cudaSuccess) e = cudaEventCreate(&tl->ev_split0);
-    if (e == cudaSuccess) e = cudaEventCreate(&tl->ev_split1);
-    if (e == cudaSuccess) e = cudaMemsetAsync(tl->fp_dev, 0, (tl->fp_mask + 1) * sizeof(FpSlot), c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) {
-        tiles_free(f);
-        return fail(c, e == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA, std::string("tiles: ") + cudaGetErrorString(e));
-    }
+    CU(c, alloc(tl->tile_bad, E));
+    CU(c, alloc(tl->entry_off, E));
+    CU(c, alloc(tl->leaf_index, E));
+    CU(c, alloc(tl->leaf_data_off, E));
+    CU(c, alloc(tl->entry_tile, E));
+    CU(c, alloc(tl->te_len, E));
+    CU(c, alloc(tl->first_stop, 4));
+    CU(c, alloc(tl->leaf_hash, E * 32));
+    CU(c, alloc(tl->fp_dev, tl->fp_mask + 1));
+    CU(c, create(tl->ev_split0, cudaEventDefault));
+    CU(c, create(tl->ev_split1, cudaEventDefault));
+    CU(c, cudaMemsetAsync(tl->fp_dev, 0, (tl->fp_mask + 1) * sizeof(FpSlot), c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    f->tl = std::move(tl);
     return CTMR_OK;
 }
 
-void tiles_free(FrontEnd* f) {
-    TileState* tl = f->tl;
-    if (!tl) return;
-    for (int k = 0; k < 2; ++k) {
-        cudaFree(tl->tiles[k]);
-        cudaFreeHost(tl->h_tiles[k]);
-    }
-    cudaFree(tl->tile_bad); cudaFree(tl->entry_off); cudaFree(tl->leaf_index); cudaFree(tl->leaf_data_off);
-    cudaFree(tl->entry_tile); cudaFree(tl->te_len); cudaFree(tl->first_stop); cudaFree(tl->leaf_hash); cudaFree(tl->fp_dev);
-    if (tl->ev_split0) cudaEventDestroy(tl->ev_split0);
-    if (tl->ev_split1) cudaEventDestroy(tl->ev_split1);
-    delete tl;
-    f->tl = nullptr;
-}
-
-void tree_free(FrontEnd* f) {
-    TreeState* tr = f->tree;
-    if (!tr) return;
-    cudaFree(tr->dev); cudaFreeHost(tr->host); cudaFree(tr->leaf); cudaFree(tr->lvl[0]); cudaFree(tr->lvl[1]);
-    delete tr;
-    f->tree = nullptr;
-}
-
 int tiles_clear_fingerprints(ctmr_ctx* c) {
-    TileState* tl = c->fe ? c->fe->tl : nullptr;
+    TileState* tl = c->fe ? c->fe->tl.get() : nullptr;
     if (!tl) return CTMR_OK;
     std::fill(tl->fp_host.begin(), tl->fp_host.end(), FpSlot{});
     tl->fp_used = 0;

@@ -21,74 +21,57 @@ namespace ctmr_host {
 
 // ------------------------------------------------------------------------------------------------ stages
 int ensure_stages(ctmr_ctx* c) {
-    if (c->stages_ready) return CTMR_OK;
+    if (c->stages) return CTMR_OK;
+    std::unique_ptr<Stage[]> stages(new (std::nothrow) Stage[kStages]);
+    if (!stages) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    const uint64_t E = c->stage_entries;
     for (int k = 0; k < kStages; ++k) {
-        Stage& s = c->stages[k];
-        const uint64_t E = c->stage_entries;
-        CU(c, cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-        CU(c, cudaEventCreateWithFlags(&s.mapped, cudaEventDisableTiming));
-        CU(c, cudaEventCreateWithFlags(&s.reduced, cudaEventDisableTiming));
-        CU(c, cudaEventCreateWithFlags(&s.meta_done, cudaEventDisableTiming));
-        CU(c, cudaMalloc(&s.blob, c->stage_bytes + 64));
+        Stage& s = stages[k];
+        CU(c, create(s.stream));
+        CU(c, create(s.mapped));
+        CU(c, create(s.reduced));
+        CU(c, create(s.meta_done));
+        CU(c, alloc(s.blob, c->stage_bytes + 64));
         // K_map stages records in 16-byte pieces, so its last copy may read up to 15 bytes past the slice's data (inside
         // this allocation, never consumed): written once here so that those bytes are defined (compute-sanitizer initcheck)
         CU(c, cudaMemsetAsync(s.blob, 0, c->stage_bytes + 64, s.stream));
-        CU(c, cudaMalloc(&s.offsets, (E + 1) * sizeof(uint64_t)));
-        CU(c, cudaMalloc(&s.issuer_idx, E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.status, E));
-        CU(c, cudaMalloc(&s.sha, E * 32));
-        CU(c, cudaMalloc(&s.exp_hour, E * sizeof(int64_t)));
-        CU(c, cudaMalloc(&s.serial_off, E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.serial_len, E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.was_unknown, E));
-        CU(c, cudaMalloc(&s.first, E));
-        CU(c, cudaMalloc(&s.keys, E * sizeof(ctmr_key)));
-        CU(c, cudaMalloc(&s.slot_of, E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.pair_slot, E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.order, E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.len_hist, 256 * sizeof(unsigned int)));
-        CU(c, cudaMalloc(&s.spans, 4 * E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.meta_slots, 2 * E * sizeof(uint32_t)));
-        CU(c, cudaMalloc(&s.first_meta, 2 * E));
+        CU(c, alloc(s.offsets, E + 1));
+        CU(c, alloc(s.issuer_idx, E));
+        CU(c, alloc(s.status, E));
+        CU(c, alloc(s.sha, E * 32));
+        CU(c, alloc(s.exp_hour, E));
+        CU(c, alloc(s.serial_off, E));
+        CU(c, alloc(s.serial_len, E));
+        CU(c, alloc(s.was_unknown, E));
+        CU(c, alloc(s.first, E));
+        CU(c, alloc(s.keys, E));
+        CU(c, alloc(s.slot_of, E));
+        CU(c, alloc(s.pair_slot, E));
+        CU(c, alloc(s.order, E));
+        CU(c, alloc(s.len_hist, 256));
+        CU(c, alloc(s.spans, 4 * E));
+        CU(c, alloc(s.meta_slots, 2 * E));
+        CU(c, alloc(s.first_meta, 2 * E));
     }
-    c->stages_ready = true;
+    c->stages = std::move(stages);
     return CTMR_OK;
 }
 
-void stages_destroy(ctmr_ctx* c) {
-    for (Stage& s : c->stages) {
-        cudaFree(s.blob); cudaFree(s.offsets); cudaFree(s.issuer_idx); cudaFree(s.status); cudaFree(s.sha);
-        cudaFree(s.exp_hour); cudaFree(s.serial_off); cudaFree(s.serial_len); cudaFree(s.was_unknown); cudaFree(s.first);
-        cudaFree(s.keys); cudaFree(s.slot_of); cudaFree(s.pair_slot); cudaFree(s.order); cudaFree(s.len_hist); cudaFree(s.spans);
-        cudaFree(s.meta_slots); cudaFree(s.first_meta);
-        pem_free(s.pem);
-        if (s.mapped) cudaEventDestroy(s.mapped);
-        if (s.reduced) cudaEventDestroy(s.reduced);
-        if (s.meta_done) cudaEventDestroy(s.meta_done);
-        if (s.stream) cudaStreamDestroy(s.stream);
-        s = Stage{};
-    }
-    c->stages_ready = false;
-}
-
 // ------------------------------------------------------------------------------------------------ PEM output
-void pem_free(PemStage& ps) {
-    cudaFree(ps.sizes); cudaFree(ps.off); cudaFree(ps.text); cudaFree(ps.scan_temp);
-    ps = PemStage{};
-}
-
 int pem_ensure(ctmr_ctx* c, PemStage& ps, uint64_t entries, uint64_t der_bytes) {
     const uint64_t need_bytes = der_bytes / 3 * 4 + der_bytes / 48 + 64 * entries + 256;  // body + newlines + boundary lines
     if (ps.cap_entries >= entries && ps.cap_bytes >= need_bytes) return CTMR_OK;
     CU(c, cudaDeviceSynchronize());
-    pem_free(ps);
-    CU(c, cudaMalloc(&ps.sizes, (entries + 1) * 8));
-    CU(c, cudaMalloc(&ps.off, (entries + 1) * 8));
-    CU(c, cudaMalloc(&ps.text, need_bytes));
-    ps.scan_temp_bytes = pem_scan_temp_bytes(entries + 1);
-    CU(c, cudaMalloc(&ps.scan_temp, ps.scan_temp_bytes ? ps.scan_temp_bytes : 16));
-    ps.cap_entries = entries;
-    ps.cap_bytes = need_bytes;
+    ps = PemStage{};  // the old buffers go first, so that peak memory is the new set
+    PemStage grown;
+    CU(c, alloc(grown.sizes, entries + 1));
+    CU(c, alloc(grown.off, entries + 1));
+    CU(c, alloc(grown.text, need_bytes));
+    grown.scan_temp_bytes = pem_scan_temp_bytes(entries + 1);
+    CU(c, alloc(grown.scan_temp, grown.scan_temp_bytes ? grown.scan_temp_bytes : 16));
+    grown.cap_entries = entries;
+    grown.cap_bytes = need_bytes;
+    ps = std::move(grown);
     return CTMR_OK;
 }
 
@@ -216,7 +199,7 @@ int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Sli
         db.blob_bytes = a.offsets[sl.hi];
         db.offsets = s.offsets;
         db.n = cnt;
-        db.issuer_idx = a.issuer_idx ? s.issuer_idx : nullptr;
+        db.issuer_idx = a.issuer_idx ? s.issuer_idx.get() : nullptr;
         db.issuer_map = map_dev;
         db.issuer_map_len = a.n_issuers;
         db.first_index = sl.first_index;
@@ -224,7 +207,7 @@ int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Sli
     }
     ctmr_dev_out& dout = x.dout;
     dout.status = s.status;
-    dout.sha256 = a.out->sha256 ? s.sha : nullptr;
+    dout.sha256 = a.out->sha256 ? s.sha.get() : nullptr;
     dout.exp_hour = s.exp_hour;
     dout.serial_off = s.serial_off;
     dout.serial_len = s.serial_len;
@@ -263,8 +246,6 @@ int stage_out(const RoundMember& x, int sidx, const BatchArgs& a, const Slice& s
     int rc = copy_out(c, x.dout, cnt, a.out, sl.lo, s.stream);
     if (rc || !want_pem) return rc;
     // StoreCertificatePEM's argument for this slice's new certificates (the host waits for this slice here)
-    rc = pem_ensure(c, s.pem, c->stage_entries, c->stage_bytes);
-    if (rc) return rc;
     return pem_chunk(c, s.pem, x.db.blob, x.db.offsets, nullptr, x.dout.was_unknown, cnt, a.out, sl.lo, pem_base, s.stream);
 }
 
@@ -315,10 +296,10 @@ int run_rounds(ctmr_ctx** m, uint32_t W, const BatchArgs& a, const std::vector<s
 void drain(ctmr_ctx** m, uint32_t W) {
     for (uint32_t r = 0; r < W; ++r) {
         ctmr_ctx* c = m[r];
-        if (!c->stages_ready) continue;
+        if (!c->stages) continue;
         const std::string keep = c->err;
         cudaSetDevice(c->device);
-        for (Stage& s : c->stages) cudaStreamSynchronize(s.stream);
+        for (int k = 0; k < kStages; ++k) cudaStreamSynchronize(c->stages[k].stream);
         c->err = keep;
     }
 }
@@ -363,6 +344,17 @@ int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, const 
     std::vector<std::vector<Slice>> plan;
     rc = plan_rounds(c0, W, a, plan);
     if (rc) return rc;
+    if (out->pem) {  // the PEM staging of every stage a slice uses, before anything is inserted
+        for (size_t k = 0; k < plan.size(); ++k)
+            for (uint32_t r = 0; r < W; ++r) {
+                if (plan[k][r].hi == plan[k][r].lo) continue;
+                *failed = m[r];
+                CU(m[r], cudaSetDevice(m[r]->device));
+                rc = pem_ensure(m[r], m[r]->stages[k % kStages].pem, m[r]->stage_entries, m[r]->stage_bytes);
+                if (rc) return rc;
+            }
+        *failed = c0;
+    }
     uint64_t advance = n;
     if (ipc) {
         // collective call: the agreed number of rounds, each rank's round k at (k * world + rank) * E above the base
@@ -410,9 +402,10 @@ int ctmr_group_create(const ctmr_config* cfg, const int32_t* devices, uint32_t n
     *out = nullptr;
     ctmr_group* g = new (std::nothrow) ctmr_group();
     if (!g) return fail(nullptr, CTMR_E_NOMEM, "host allocation failed");
-    auto bail = [&](int code, const std::string& msg) {
+    auto bail = [&](int code, const std::string& msg) {  // msg may be a member's error: report before destroying
+        fail(nullptr, code, msg);
         ctmr_group_destroy(g);
-        return fail(nullptr, code, msg);
+        return code;
     };
     for (uint32_t r = 0; r < n_devices; ++r) {
         ctmr_config mc = *cfg;
@@ -619,13 +612,15 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes) 
         h.max_issuers != c0->st.max_issuers || h.n_issuers > h.max_issuers)
         return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "snapshot was taken by a group of another size or with other capacities"));
     if (bytes < sizeof h + h.members * h.shard_bytes + h.n_issuers * 32) return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "truncated snapshot"));
+    RegistryUpload u;
+    if (const int rc = snap_registry_alloc(c0, h.n_issuers, u)) return group_fail(g, c0, rc);
     const uint8_t* p = buf + sizeof h;
     for (ctmr_ctx* c : g->m) {
         const int rc = snap_shard_load(c, p);
         if (rc) return group_fail(g, c, rc);
         p += h.shard_bytes;
     }
-    const int rc = snap_registry_restore(c0, p, h.n_issuers);
+    const int rc = snap_registry_restore(c0, p, h.n_issuers, u);
     if (rc) return group_fail(g, c0, rc);
     g->next_index = h.next_index;
     return CTMR_OK;
@@ -691,12 +686,7 @@ int ctmr_peer_attach(ctmr_ctx* c, uint32_t rank, uint32_t world, const uint8_t* 
     if (world == 1) return CTMR_OK;
     if (!c->xchg || c->exported_world != world) return fail(c, CTMR_E_INVALID, "call ctmr_peer_export(ctx, world, ...) with this group size first");
     uint8_t *bases[kMaxWorld] = {}, *xb[kMaxWorld] = {};
-    auto close_all = [&]() {
-        for (uint32_t q = 0; q < kMaxWorld; ++q) {
-            if (c->ipc_base[q]) { cudaIpcCloseMemHandle(c->ipc_base[q]); c->ipc_base[q] = nullptr; }
-            if (c->ipc_xchg[q]) { cudaIpcCloseMemHandle(c->ipc_xchg[q]); c->ipc_xchg[q] = nullptr; }
-        }
-    };
+    IpcMap base_maps[kMaxWorld], xchg_maps[kMaxWorld];  // into the ctx once every rank's region is open
     for (uint32_t r = 0; r < world; ++r) {
         PeerHandle h;
         std::memcpy(&h, handles + (size_t)r * CTMR_PEER_HANDLE_BYTES, sizeof h);
@@ -709,21 +699,17 @@ int ctmr_peer_attach(ctmr_ctx* c, uint32_t rank, uint32_t world, const uint8_t* 
             xb[r] = c->xchg;
             continue;
         }
-        void *p = nullptr, *x = nullptr;
-        cudaError_t e = cudaIpcOpenMemHandle(&p, h.mem, cudaIpcMemLazyEnablePeerAccess);
-        if (e == cudaSuccess) {
-            c->ipc_base[r] = p;
-            e = cudaIpcOpenMemHandle(&x, h.xchg, cudaIpcMemLazyEnablePeerAccess);
-            if (e == cudaSuccess) c->ipc_xchg[r] = x;
-        }
+        cudaError_t e = open(base_maps[r], h.mem);
+        if (e == cudaSuccess) e = open(xchg_maps[r], h.xchg);
         if (e != cudaSuccess) {
             (void)cudaGetLastError();
-            close_all();
             return fail(c, CTMR_E_PEER, "cudaIpcOpenMemHandle(rank " + std::to_string(r) + "): " + cudaGetErrorString(e));
         }
-        bases[r] = static_cast<uint8_t*>(p);
-        xb[r] = static_cast<uint8_t*>(x);
+        bases[r] = base_maps[r];
+        xb[r] = xchg_maps[r];
     }
+    std::swap(c->ipc_base, base_maps);
+    std::swap(c->ipc_xchg, xchg_maps);
     attach_views(c, bases, world, rank);
     attach_exchange(c, xb, world, rank);
     c->peer_mode = PEER_IPC;

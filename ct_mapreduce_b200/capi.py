@@ -35,7 +35,8 @@ EXPORTS = [
     "ctmr_synth_tiles_host",
     "ctmr_process_raw", "ctmr_group_process_raw", "ctmr_frontend_profile_last",  # include/ctmr_frontend.h
     "ctmr_process_tiles", "ctmr_group_process_tiles", "ctmr_register_chain_certs", "ctmr_group_register_chain_certs",
-    "ctmr_tiles_profile_last", "ctmr_process_raw_tree", "ctmr_process_tiles_tree",
+    "ctmr_tiles_profile_last", "ctmr_process_raw_tree", "ctmr_process_tiles_tree", "ctmr_process_raw_trees",
+    "ctmr_process_tiles_trees",
     # several GPUs: one process (group) / one process per GPU (peer)
     "ctmr_group_create", "ctmr_group_destroy", "ctmr_group_last_error", "ctmr_group_size", "ctmr_group_member",
     "ctmr_group_process_batch", "ctmr_group_issuer_counts", "ctmr_group_set_cardinality", "ctmr_group_status_counters",
@@ -54,6 +55,8 @@ E_PAIR_TABLE_FULL, E_META_TABLE_FULL, E_PEER_TIMEOUT, E_PEER = -8, -9, -10, -11
 E_UNKNOWN_ISSUER = -12
 # per-entry outcome of the front end (include/ctmr_frontend.h CTMR_FE_*)
 FE_OK, FE_BAD_BASE64, FE_BAD_LEAF, FE_UNKNOWN_TYPE, FE_BAD_EXTRA, FE_BAD_CERT, FE_BAD_TILE, FE_BAD_INDEX = range(8)
+NO_TREE = 0xFFFFFFFF   # CTMR_NO_TREE: an entry or tile of ctmr_process_*_trees that folds into no tree
+MAX_TREES = 1024       # CTMR_MAX_TREES
 
 
 class Config(C.Structure):
@@ -199,6 +202,8 @@ def load():
     L.ctmr_tiles_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
     L.ctmr_process_raw_tree.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), C.POINTER(Tree)]
     L.ctmr_process_tiles_tree.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), C.POINTER(Tree)]
+    L.ctmr_process_raw_trees.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), vp, vp, u32]
+    L.ctmr_process_tiles_trees.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), vp, vp, u32]
     L.ctmr_group_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_synth_tiles_host.argtypes = [C.POINTER(SynthCfg), u64, u64, vp, vp, u64, vp, vp]
     L.ctmr_synth_tiles_host.restype = u64

@@ -188,15 +188,24 @@ struct TileState {
     std::unordered_map<std::string, uint32_t> fp_memo;
 };
 
-// the log's Merkle tree (ctmr_process_raw_tree / ctmr_process_tiles_tree): the call's tree on the device and the scratch
-// of the fold.  Allocated on the first tree call.
+// the logs' Merkle trees (ctmr_process_*_tree, ctmr_process_*_trees): the call's trees on the device and the scratch of
+// the fold.  Allocated on the first tree call, for cap_trees trees; a call with more trees builds it again, larger.
 struct TreeState {
-    DevBuf<TreeDev> dev;          // the tree for the whole call: uploaded at its start, read back at its end
-    HostBuf<TreeDev> host;        // pinned staging of those two copies
+    uint32_t cap_trees = 0;
+    DevBuf<TreeDev> dev;          // [cap_trees] the trees for the whole call: uploaded at its start, read back at its end
+    HostBuf<TreeDev> host;        // [cap_trees] pinned staging of those two copies
+    DevBuf<FoldTree> desc;        // [cap_trees] the trees of the chunk being folded
+    HostBuf<FoldTree> h_desc;
+    DevBuf<uint32_t> order[2];    // [cap_entries] per upload stage: the chunk's entries grouped by tree
+    HostBuf<uint32_t> h_order[2];
     DevBuf<uint8_t> leaf;         // [cap_entries][32] get-entries leaf hashes of a chunk
-    DevBuf<uint8_t> lvl[2];       // [cap_entries / 2 + 2][32] each: ping-pong level buffers
-    uint64_t base = 0;            // log position of the call's first entry
-    bool active = false;          // a tree call is running: the chunks fold their leaves
+    DevBuf<uint8_t> lvl[2];       // [cap_entries / 2 + 2 * cap_trees][32] each: ping-pong level buffers
+    // the call
+    uint32_t n_trees = 0;
+    const uint32_t* log = nullptr;  // the tree of each entry (pages) or tile (tiles); NULL: everything goes to tree 0
+    std::vector<uint64_t> next;     // [n_trees] log position of each tree's next entry to be uploaded
+    std::vector<uint32_t> count;    // [n_trees] scratch of the grouping
+    bool active = false;            // a tree call is running: the chunks fold their leaves
 };
 
 // CT wire-format front end (include/ctmr_frontend.h): device buffers of one chunk + the device mirror of

@@ -38,6 +38,11 @@ struct Chunk {
     ctmr_dev_out dout{};
     bool stopped = false;         // tiles: holds the first tile with an unknown Chain[0] fingerprint; [lo, hi) cut before it
     std::vector<std::array<uint8_t, 32>> missing;  // that tile's unknown fingerprints, sorted
+    // tree calls (tree_group): the trees of the chunk's entries, in tree order; whether their order was uploaded into the
+    // stage (it is not when it is the identity); how many entries it lists
+    std::vector<FoldTree> fold;
+    bool ordered = false;
+    uint64_t listed = 0;
 
     // keeps the first `units` units, which hold `entries` entries
     void cut(uint64_t units, uint64_t entries) {
@@ -91,56 +96,152 @@ int fe_prepare(ctmr_ctx* c) {
 #define CHUNK_D2H(dst, src, per) \
     if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * (per), (src), cnt * (per), cudaMemcpyDeviceToHost, s))
 
-// ---- the log's Merkle tree (ctmr_process_raw_tree, ctmr_process_tiles_tree) ----------------------------------------------
-int tree_ensure(ctmr_ctx* c) {
+// ---- the logs' Merkle trees (ctmr_process_*_tree, ctmr_process_*_trees) ------------------------------------------------
+// The trees of a tree call: the one-tree forms pass one tree and no log (every entry is the tree's); the routed forms
+// pass n trees and the tree of every entry (pages) or tile (tiles), CTMR_NO_TREE for none.
+struct TreeArgs {
+    ctmr_tree* trees = nullptr;
+    uint32_t n = 0;
+    const uint32_t* log = nullptr;
+    bool routed = false;
+};
+
+// the arguments of a routed call before the format's own rules: `units` entries or tiles, and their trees
+int tree_route_args(ctmr_ctx* c, const TreeArgs* t, uint64_t units) {
+    if (t->n > CTMR_MAX_TREES) return fail(c, CTMR_E_INVALID, "trees: more than CTMR_MAX_TREES trees");
+    if (t->n && !t->trees) return fail(c, CTMR_E_INVALID, "trees: null trees");
+    if (units && !t->log) return fail(c, CTMR_E_INVALID, "trees: null log ids");
+    for (uint64_t u = 0; u < units; ++u)
+        if (t->log[u] >= t->n && t->log[u] != CTMR_NO_TREE) return fail(c, CTMR_E_INVALID, "trees: a log id names no tree");
+    return CTMR_OK;
+}
+
+// the tree state for n trees, built whole (a smaller one is released first)
+int tree_ensure(ctmr_ctx* c, uint32_t n) {
     FrontEnd* f = c->fe.get();
-    if (f->tree) return CTMR_OK;
+    if (f->tree && f->tree->cap_trees >= n) return CTMR_OK;
+    f->tree.reset();
     std::unique_ptr<TreeState> tr(new (std::nothrow) TreeState());
     if (!tr) return fail(c, CTMR_E_NOMEM, "host allocation failed");
     const uint64_t E = f->cap_entries;
-    CU(c, alloc(tr->dev, 1));
-    CU(c, alloc(tr->host, 1));
+    const uint32_t cap = (uint32_t)pow2_at_least(std::max<uint32_t>(n, 1));
+    CU(c, alloc(tr->dev, cap));
+    CU(c, alloc(tr->host, cap));
+    CU(c, alloc(tr->desc, cap));
+    CU(c, alloc(tr->h_desc, cap));
+    for (int k = 0; k < 2; ++k) {
+        CU(c, alloc(tr->order[k], E));
+        CU(c, alloc(tr->h_order[k], E));
+    }
     CU(c, alloc(tr->leaf, E * 32));
-    for (DevBuf<uint8_t>& lvl : tr->lvl) CU(c, alloc(lvl, (E / 2 + 2) * 32));
+    for (DevBuf<uint8_t>& lvl : tr->lvl) CU(c, alloc(lvl, (E / 2 + 2ull * cap) * 32));
+    tr->cap_trees = cap;
     f->tree = std::move(tr);
     return CTMR_OK;
 }
 
-// the caller's tree to the device for the whole call; the call's entries start at log position `base`
-int tree_begin(ctmr_ctx* c, const ctmr_tree* tree, uint64_t base) {
-    int rc = tree_ensure(c);
+// the caller's trees to the device for the whole call; next[d]: log position of tree d's first entry in the call
+int tree_begin(ctmr_ctx* c, const TreeArgs* t, const std::vector<uint64_t>& next) {
+    int rc = tree_ensure(c, t->n);
     if (rc) return rc;
     TreeState* tr = c->fe->tree.get();
-    std::memcpy(&tr->host->t, tree, sizeof(ctmr_tree));
-    tr->host->missing = ~0ull;
-    CU(c, cudaMemcpyAsync(tr->dev, tr->host, sizeof(TreeDev), cudaMemcpyHostToDevice, c->stream));
-    tr->base = base;
+    for (uint32_t d = 0; d < t->n; ++d) {
+        std::memcpy(&tr->host[d].t, &t->trees[d], sizeof(ctmr_tree));
+        tr->host[d].missing = ~0ull;
+    }
+    CU(c, cudaMemcpyAsync(tr->dev, tr->host, t->n * sizeof(TreeDev), cudaMemcpyHostToDevice, c->stream));
+    tr->n_trees = t->n;
+    tr->log = t->log;
+    tr->next = next;
+    tr->count.assign(t->n, 0);
     tr->active = true;
     return CTMR_OK;
 }
 
-// folds entries [0, cnt) of a chunk, log positions first_pos.., into the tree (see FoldChunk)
-int tree_fold(ctmr_ctx* c, const uint8_t* leaves, const uint8_t* flags, uint32_t stride, uint32_t match, uint64_t first_pos, uint64_t cnt) {
+bool tree_active(const FrontEnd* f) { return f->tree && f->tree->active; }
+
+// Groups the entries of units [ch.lo, ch.hi) by tree (unit u holds width(u) entries) into ch.fold, each tree's entries
+// taking its next log positions, and uploads their order into the chunk's stage on the copy stream unless it is the
+// identity (one tree and no entry of none).
+template <class Width>
+int tree_group(ctmr_ctx* c, Chunk& ch, Width width) {
+    ch.fold.clear();
+    ch.ordered = false;
+    ch.listed = 0;
+    if (!tree_active(c->fe.get())) return CTMR_OK;
     TreeState* tr = c->fe->tree.get();
-    const FoldChunk fc{tr->dev, leaves, flags, stride, match, first_pos, cnt};
+    std::vector<uint32_t>& cnt = tr->count;
+    std::fill(cnt.begin(), cnt.end(), 0u);
+    uint64_t none = 0;
+    for (uint64_t u = ch.lo; u < ch.hi; ++u) {
+        const uint32_t l = tr->log ? tr->log[u] : 0;
+        if (l == CTMR_NO_TREE) none += width(u);
+        else cnt[l] += width(u);
+    }
+    uint32_t off = 0;
+    for (uint32_t d = 0; d < tr->n_trees; ++d) {
+        if (!cnt[d]) continue;
+        ch.fold.push_back(FoldTree{tr->next[d], d, off, cnt[d], 0});
+        tr->next[d] += cnt[d];
+        off += cnt[d];
+    }
+    ch.listed = off;
+    ch.ordered = none || ch.fold.size() > 1;
+    if (!ch.ordered || !off) return CTMR_OK;
+    for (const FoldTree& t : ch.fold) cnt[t.tree] = t.off;  // from here on: each tree's next slot in the order
+    uint32_t* h = tr->h_order[ch.stage];
+    uint32_t e = 0;
+    for (uint64_t u = ch.lo; u < ch.hi; ++u) {
+        const uint32_t l = tr->log ? tr->log[u] : 0, w = width(u);
+        if (l != CTMR_NO_TREE)
+            for (uint32_t k = 0; k < w; ++k) h[cnt[l]++] = e + k;
+        e += w;
+    }
+    CU(c, cudaMemcpyAsync(tr->order[ch.stage], h, off * 4ull, cudaMemcpyHostToDevice, c->fe->copy_stream));
+    return CTMR_OK;
+}
+
+// a chunk cut to units [ch.lo, ch.hi) (tiles, at a stop) folds only their entries: each tree keeps the head of its run
+template <class Width>
+void tree_cut(ctmr_ctx* c, Chunk& ch, Width width) {
+    if (ch.fold.empty()) return;
+    TreeState* tr = c->fe->tree.get();
+    std::vector<uint32_t>& cnt = tr->count;
+    std::fill(cnt.begin(), cnt.end(), 0u);
+    for (uint64_t u = ch.lo; u < ch.hi; ++u) {
+        const uint32_t l = tr->log ? tr->log[u] : 0;
+        if (l != CTMR_NO_TREE) cnt[l] += width(u);
+    }
+    std::vector<FoldTree> kept;
+    for (FoldTree t : ch.fold)
+        if ((t.cnt = cnt[t.tree]) != 0) kept.push_back(t);
+    ch.fold.swap(kept);
+}
+
+// folds a chunk's leaves into its trees (see FoldChunk)
+int tree_fold(ctmr_ctx* c, const Chunk& ch, const uint8_t* leaves, const uint8_t* flags, uint32_t stride, uint32_t match) {
+    if (ch.fold.empty()) return CTMR_OK;
+    TreeState* tr = c->fe->tree.get();
+    const uint32_t n = (uint32_t)ch.fold.size();
+    std::memcpy(tr->h_desc, ch.fold.data(), n * sizeof(FoldTree));
+    CU(c, cudaMemcpyAsync(tr->desc, tr->h_desc, n * sizeof(FoldTree), cudaMemcpyHostToDevice, c->stream));
+    const FoldChunk fc{tr->dev, tr->desc, n, stride, ch.ordered ? tr->order[ch.stage].get() : nullptr, ch.listed, leaves, flags, match};
     uint8_t* const lvl[2] = {tr->lvl[0], tr->lvl[1]};
     uint32_t launches = 0;
-    CU(c, launch_tree_fold(fc, lvl, c->stream, &launches));
+    CU(c, launch_tree_fold(fc, ch.fold.data(), lvl, c->stream, &launches));
     c->fe->launches += launches;
     return CTMR_OK;
 }
 
-// the root, and the tree back to the caller
-int tree_end(ctmr_ctx* c, ctmr_tree* tree) {
+// the roots, and the trees back to the caller
+int tree_end(ctmr_ctx* c, const TreeArgs* t) {
     TreeState* tr = c->fe->tree.get();
-    CU(c, launch_tree_root(tr->dev, c->stream));
-    CU(c, cudaMemcpyAsync(tr->host, tr->dev, sizeof(TreeDev), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, launch_tree_root(tr->dev, t->n, c->stream));
+    CU(c, cudaMemcpyAsync(tr->host, tr->dev, t->n * sizeof(TreeDev), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    std::memcpy(tree, &tr->host->t, sizeof(ctmr_tree));
+    for (uint32_t d = 0; d < t->n; ++d) std::memcpy(&t->trees[d], &tr->host[d].t, sizeof(ctmr_tree));
     return CTMR_OK;
 }
-
-bool tree_active(const FrontEnd* f) { return f->tree && f->tree->active; }
 
 // ================================================================================================================
 // get-entries pages: the units of a chunk are entries.  The stage is free again once the chunk is decoded.
@@ -153,11 +254,12 @@ struct Pages {
     uint64_t done;  // entries that take their indices: all n whenever there is a batch, also when the call fails once a
                     // chunk has reached the path
 
+    std::vector<uint64_t> tree_pos;  // tree calls: log position of each tree's first entry
+
     Pages(const ctmr_raw_batch* b_, ctmr_raw_out* out_) : b(b_), out(out_), done(b_ ? b_->n : 0) {}
-    int check(ctmr_ctx* c, const ctmr_tree* tree) const;
+    int check(ctmr_ctx* c, const TreeArgs* tree);
     uint64_t units() const { return b->n; }
     uint64_t q_max(const ctmr_ctx* c) const { return c->fe->cap_entries; }
-    uint64_t tree_base(const ctmr_tree* tree) const { return tree->size; }
     int prepare(ctmr_ctx* c) const { return fe_prepare(c); }
     int fit(ctmr_ctx* c, uint64_t lo, uint64_t max_entries, uint64_t* hi_out) const;
     int upload(ctmr_ctx* c, Chunk& ch) const;
@@ -167,14 +269,31 @@ struct Pages {
     int stop(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }  // a page chunk never stops
 };
 
-// tree: ctmr_process_raw_tree's rule as well
-int Pages::check(ctmr_ctx* c, const ctmr_tree* tree) const {
+// tree: ctmr_process_raw_tree's rule as well; a routed call's rules fail before any index is taken
+int Pages::check(ctmr_ctx* c, const TreeArgs* tree) {
     if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n && (!b->text || !b->leaf_input_off || !b->leaf_input_len || !b->extra_data_off || !b->extra_data_len))
         return fail(c, CTMR_E_INVALID, "null batch buffers");
-    const int rc = check_pem(c, &out->path);
+    int rc = check_pem(c, &out->path);
     if (rc) return rc;
-    if (tree && b->n > ~0ull - tree->size) return fail(c, CTMR_E_INVALID, "tree size + entries wraps around 2^64");
+    if (!tree) return CTMR_OK;
+    if (!tree->routed) {
+        if (b->n > ~0ull - tree->trees[0].size) return fail(c, CTMR_E_INVALID, "tree size + entries wraps around 2^64");
+        tree_pos.assign(1, tree->trees[0].size);
+        return CTMR_OK;
+    }
+    rc = tree_route_args(c, tree, b->n);
+    std::vector<uint64_t> cnt(tree->n, 0);
+    for (uint64_t i = 0; rc == CTMR_OK && i < b->n; ++i)
+        if (tree->log[i] != CTMR_NO_TREE) ++cnt[tree->log[i]];
+    for (uint32_t d = 0; rc == CTMR_OK && d < tree->n; ++d)
+        if (cnt[d] > ~0ull - tree->trees[d].size) rc = fail(c, CTMR_E_INVALID, "trees: a tree's size + its entries wraps around 2^64");
+    if (rc) {
+        done = 0;
+        return rc;
+    }
+    tree_pos.resize(tree->n);
+    for (uint32_t d = 0; d < tree->n; ++d) tree_pos[d] = tree->trees[d].size;
     return CTMR_OK;
 }
 
@@ -209,6 +328,8 @@ int Pages::upload(ctmr_ctx* c, Chunk& ch) const {
         CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
         return CTMR_OK;
     }
+    const int rc = tree_group(c, ch, [](uint64_t) { return 1u; });
+    if (rc) return rc;
     uint64_t chars = 0, min_off = ~0ull, max_end = 0;
     for (uint64_t i = lo; i < ch.hi; ++i) {
         const uint64_t l0 = b->leaf_input_off[i], l1 = l0 + b->leaf_input_len[i];
@@ -311,10 +432,10 @@ int Pages::front(ctmr_ctx* c, Chunk& ch) const {
             if (rc) return rc;
             if (f->slots_used == before) return fail(c, CTMR_E_CUDA, "front end: unresolved Chain[0] is already registered");
         }
-        if (tree_active(f)) {  // the leaves of this chunk into the tree, while the arena still holds them
+        if (!ch.fold.empty()) {  // the leaves of this chunk into its trees, while the arena still holds them
             CU(c, launch_raw_leaf_hash(p, f->tree->leaf, s));
             ++f->launches;
-            const int rc = tree_fold(c, f->tree->leaf, f->str_bad, 2, 1, f->tree->base + ch.lo, cnt);
+            const int rc = tree_fold(c, ch, f->tree->leaf, f->str_bad, 2, 1);
             if (rc) return rc;
         }
     } else {
@@ -366,12 +487,12 @@ struct Tiles {
     ctmr_tile_out* out;
     uint64_t done = 0;         // entries that take their indices: none when the arguments fail, those before a stop, else all
     std::vector<uint64_t> ent;  // entries before each tile: ent[t] = sum of widths of tiles [0, t)
+    std::vector<uint64_t> tree_pos;  // tree calls: log position of each tree's first entry (its first tile's)
 
     Tiles(const ctmr_tile_batch* b_, ctmr_tile_out* out_) : b(b_), out(out_) {}
-    int check(ctmr_ctx* c, const ctmr_tree* tree);
+    int check(ctmr_ctx* c, const TreeArgs* tree);
     uint64_t units() const { return b->n_tiles; }
     uint64_t q_max(const ctmr_ctx*) const { return ~0ull; }  // fit keeps a chunk inside the entry budget
-    uint64_t tree_base(const ctmr_tree*) const { return b->n_tiles ? 256 * b->tile_index[0] : 0; }
     int prepare(ctmr_ctx* c) const;
     int fit(ctmr_ctx* c, uint64_t lo, uint64_t max_tiles, uint64_t* hi_out) const;
     int upload(ctmr_ctx* c, Chunk& ch) const;
@@ -381,22 +502,33 @@ struct Tiles {
     int stop(ctmr_ctx* c, const Chunk& ch) const;
 };
 
-// ctmr_process_tiles_tree's rules for the tiles of one log, checked before any work like the widths and spans
-int tree_tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const ctmr_tree* tree, uint64_t n) {
-    if (b->n_tiles == 0) return CTMR_OK;
-    if (b->tile_index[0] > (~0ull - n) >> 8) return fail(c, CTMR_E_INVALID, "tree: the batch's last leaf index does not fit 64 bits");
-    for (uint64_t t = 0; t + 1 < b->n_tiles; ++t) {
-        if (b->tile_index[t + 1] != b->tile_index[t] + 1) return fail(c, CTMR_E_INVALID, "tree: tiles are not consecutive");
-        if (b->tile_width[t] != 256) return fail(c, CTMR_E_INVALID, "tree: a partial tile that is not the last");
+// ctmr_process_tiles_tree's rules for the tiles of one log (the batch's tiles of log `log`; every tile without a log),
+// checked before any work like the widths and spans.  *first_pos: the log position of its first tile.
+int tree_tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const uint32_t* tile_log, uint32_t log, const ctmr_tree* tree,
+                   uint64_t* first_pos) {
+    uint64_t first = ~0ull, prev = ~0ull, n = 0;
+    for (uint64_t t = 0; t < b->n_tiles; ++t) {
+        if (tile_log && tile_log[t] != log) continue;
+        if (prev != ~0ull) {
+            if (b->tile_index[t] != b->tile_index[prev] + 1) return fail(c, CTMR_E_INVALID, "tree: tiles are not consecutive");
+            if (b->tile_width[prev] != 256) return fail(c, CTMR_E_INVALID, "tree: a partial tile that is not the last");
+        } else {
+            first = t;
+        }
+        prev = t;
+        n += b->tile_width[t];
     }
-    const uint64_t first = 256 * b->tile_index[0];
-    if (tree->size < first || tree->size > first + b->tile_width[0])
+    *first_pos = 0;
+    if (first == ~0ull) return CTMR_OK;
+    if (b->tile_index[first] > (~0ull - n) >> 8) return fail(c, CTMR_E_INVALID, "tree: the batch's last leaf index does not fit 64 bits");
+    *first_pos = 256 * b->tile_index[first];
+    if (tree->size < *first_pos || tree->size > *first_pos + b->tile_width[first])
         return fail(c, CTMR_E_INVALID, "tree: size is not inside the batch's first tile");
     return CTMR_OK;
 }
 
 // validates widths and spans (and with a tree its rules), fills ent
-int Tiles::check(ctmr_ctx* c, const ctmr_tree* tree) {
+int Tiles::check(ctmr_ctx* c, const TreeArgs* tree) {
     if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n_tiles && (!b->data || !b->tile_off || !b->tile_len || !b->tile_index || !b->tile_width))
         return fail(c, CTMR_E_INVALID, "null batch buffers");
@@ -411,8 +543,16 @@ int Tiles::check(ctmr_ctx* c, const ctmr_tree* tree) {
         ent[t + 1] = ent[t] + b->tile_width[t];
     }
     if (tree) {
-        rc = tree_tile_args(c, b, tree, ent[b->n_tiles]);
-        if (rc) return rc;
+        const uint32_t* log = tree->routed ? tree->log : nullptr;
+        if (tree->routed) {
+            rc = tree_route_args(c, tree, b->n_tiles);
+            if (rc) return rc;
+        }
+        tree_pos.assign(tree->n, 0);
+        for (uint32_t d = 0; d < tree->n; ++d) {
+            rc = tree_tile_args(c, b, log, d, &tree->trees[d], &tree_pos[d]);
+            if (rc) return rc;
+        }
     }
     done = ent[b->n_tiles];
     out->tiles_done = 0;
@@ -481,6 +621,8 @@ int Tiles::upload(ctmr_ctx* c, Chunk& ch) const {
     if (ch.bytes)
         CU(c, cudaMemcpyAsync(st.text + 16, one_copy ? b->data + min_off : st.pack.data(), ch.bytes, cudaMemcpyHostToDevice, f->copy_stream));
     if (cnt) CU(c, cudaMemcpyAsync(tl->tiles[ch.stage], h, cnt * sizeof(TileDesc), cudaMemcpyHostToDevice, f->copy_stream));
+    const int rc = tree_group(c, ch, [this](uint64_t t) { return (uint32_t)b->tile_width[t]; });
+    if (rc) return rc;
     CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
     return CTMR_OK;
 }
@@ -522,7 +664,7 @@ int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
         CU(c, launch_tile_frame(p, s));
         CU(c, launch_tile_issuer(p, FpTable{tl->fp_dev, tl->fp_mask}, s));
         f->launches += 4;  // split, frame, tbs, issuer
-        if (out->leaf_hash || tree_active(f)) {
+        if (out->leaf_hash || !ch.fold.empty()) {
             CU(c, launch_tile_leaf_hash(p, s));
             ++f->launches;
         }
@@ -548,9 +690,10 @@ int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
             ch.missing.erase(std::unique(ch.missing.begin(), ch.missing.end()), ch.missing.end());
             ch.stopped = true;
             ch.cut(stop, td.first);
+            tree_cut(c, ch, [this](uint64_t t) { return (uint32_t)b->tile_width[t]; });
         }
-        if (p.n && tree_active(f)) {  // the completed tiles' leaves into the tree; a bad tile has none
-            const int rc = tree_fold(c, tl->leaf_hash, f->entry_status, 1, CTMR_FE_BAD_TILE, f->tree->base + ch.e0, p.n);
+        {  // the completed tiles' leaves into their trees; a bad tile has none
+            const int rc = tree_fold(c, ch, tl->leaf_hash, f->entry_status, 1, CTMR_FE_BAD_TILE);
             if (rc) return rc;
         }
     }
@@ -748,18 +891,19 @@ int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
 }
 
 // One front-end call on the members m[0..W): one ctx (W == 1), or the members of a group.  The batch's entries take the
-// global indices from *next_index on; tree (one member only): fold the entries into it too, written back when the call
-// succeeds or stops.  A stop (tiles) ends the call after the round that meets it.  On error *failed names the member
+// global indices from *next_index on; tree (one member only): fold the entries into the trees too, written back when the
+// call succeeds or stops.  A stop (tiles) ends the call after the round that meets it.  On error *failed names the member
 // that failed.
 template <class Format>
-int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, ctmr_tree* tree, ctmr_ctx** failed) {
+int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, const TreeArgs* targs, ctmr_ctx** failed) {
     *failed = m[0];
-    int rc = fm.check(m[0], tree);
+    int rc = fm.check(m[0], targs);
     if (rc) return rc;
     // The entries take their indices once a chunk reaches the path; a call that fails before has changed no table.
     const uint64_t takes = fm.done;
     fm.done = 0;
     const uint64_t total = fm.units();
+    const TreeArgs* tree = targs && targs->n ? targs : nullptr;  // a routed call of no tree folds nothing
     if (total == 0 && !tree) return CTMR_OK;
     const ctmr_out* po = &fm.out->path;
     // everything the call builds on first use, before its first kernel
@@ -772,7 +916,7 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
     }
     *failed = m[0];
     if (tree) {
-        rc = tree_begin(m[0], tree, fm.tree_base(tree));
+        rc = tree_begin(m[0], tree, fm.tree_pos);
         if (rc) return rc;
         if (total == 0) return tree_end(m[0], tree);
     }
@@ -841,12 +985,15 @@ void drain_frontend(ctmr_ctx* c) {
 // indices are used up (a retry must not reuse them: its entries then read as known), the tree is the caller's again,
 // and a failure drains every member and becomes the last error of the group g (if any).
 template <class Format>
-int front_end_call(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format fm, ctmr_tree* tree, ctmr_group* g) {
+int front_end_call(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format fm, const TreeArgs* tree, ctmr_group* g) {
     ctmr_ctx* failed = nullptr;
     const int rc = process_members(m, W, next_index, fm, tree, &failed);
     *next_index += fm.done;
     for (uint32_t r = 0; r < W; ++r) {
-        if (m[r]->fe && m[r]->fe->tree) m[r]->fe->tree->active = false;
+        if (m[r]->fe && m[r]->fe->tree) {
+            m[r]->fe->tree->active = false;
+            m[r]->fe->tree->log = nullptr;
+        }
         if (rc != CTMR_OK) drain_frontend(m[r]);
     }
     return rc != CTMR_OK ? group_fail(g, failed, rc) : rc;
@@ -946,14 +1093,32 @@ int ctmr_process_raw_tree(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* ou
     if (!c) return CTMR_E_INVALID;
     if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
-    return front_end_call(&c, 1, &c->next_index, Pages(b, out), tree, nullptr);
+    const TreeArgs t{tree, 1, nullptr, false};
+    return front_end_call(&c, 1, &c->next_index, Pages(b, out), &t, nullptr);
 }
 
 int ctmr_process_tiles_tree(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, ctmr_tree* tree) {
     if (!c) return CTMR_E_INVALID;
     if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
-    return front_end_call(&c, 1, &c->next_index, Tiles(b, out), tree, nullptr);
+    const TreeArgs t{tree, 1, nullptr, false};
+    return front_end_call(&c, 1, &c->next_index, Tiles(b, out), &t, nullptr);
+}
+
+int ctmr_process_raw_trees(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, const uint32_t* entry_log, ctmr_tree* trees,
+                           uint32_t n_trees) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    const TreeArgs t{trees, n_trees, entry_log, true};
+    return front_end_call(&c, 1, &c->next_index, Pages(b, out), &t, nullptr);
+}
+
+int ctmr_process_tiles_trees(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, const uint32_t* tile_log, ctmr_tree* trees,
+                             uint32_t n_trees) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    const TreeArgs t{trees, n_trees, tile_log, true};
+    return front_end_call(&c, 1, &c->next_index, Tiles(b, out), &t, nullptr);
 }
 
 int ctmr_tiles_profile_last(ctmr_ctx* c, float* split_ms) {

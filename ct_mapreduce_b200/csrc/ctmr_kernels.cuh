@@ -324,33 +324,48 @@ cudaError_t launch_tile_issuer(const TileParams& p, const FpTable& tab, cudaStre
 cudaError_t launch_tile_leaf_hash(const TileParams& p, cudaStream_t s);
 cudaError_t launch_fingerprints(const uint8_t* blob, const uint64_t* offsets, uint32_t n, uint8_t* fps, cudaStream_t s);
 
-// ---- the log's Merkle tree (ctmr_merkle.cu, ctmr_process_raw_tree / ctmr_process_tiles_tree) ---------------------------
-// The tree of one call lives on the device: the caller's ctmr_tree, plus the lowest log position of a leaf that is missing
-// in the chunk being folded (~0 when none).
+// ---- the logs' Merkle trees (ctmr_merkle.cu, ctmr_process_*_tree / ctmr_process_*_trees) -------------------------------
+// The trees of one call live on the device: each caller's ctmr_tree, plus the lowest log position of a leaf that is
+// missing in the chunk being folded (~0 when none).
 struct TreeDev {
     ctmr_tree t;
     unsigned long long missing;
 };
 
-// One chunk's leaves: leaf hash rows [cnt][32], row j = log position first_pos + j.  Entry j has no leaf when
-// flags[j * stride] == match.  The fold takes [t.size, end), where end is the first missing leaf at or above t.size, or
-// first_pos + cnt; nothing when t.size < first_pos (an earlier chunk stopped).
+// One tree's part of a chunk: its entries are order[off .. off + cnt) (chunk entries, in log order), entry order[off + j]
+// is log position first_pos + j.  The fold takes [t.size, end), where end is the first missing leaf at or above t.size,
+// or first_pos + cnt; nothing when t.size < first_pos (an earlier chunk stopped this tree).
+struct FoldTree {
+    uint64_t first_pos;
+    uint32_t tree;  // index into FoldChunk::trees
+    uint32_t off;
+    uint32_t cnt;   // > 0
+    uint32_t pad;
+};
+static_assert(sizeof(FoldTree) == 24, "FoldTree layout");
+
+// One chunk's leaves: leaf hash rows [chunk entries][32].  Entry e has no leaf when flags[e * stride] == match.  The
+// chunk folds into n_desc trees; desc is ordered by off, and order (NULL: the identity) lists the chunk's entries grouped
+// by tree, `total` of them (entries of no tree are left out).
 struct FoldChunk {
-    TreeDev* tree;
+    TreeDev* trees;
+    const FoldTree* desc;
+    uint32_t n_desc;
+    uint32_t stride;
+    const uint32_t* order;
+    uint64_t total;
     const uint8_t* leaves;
     const uint8_t* flags;
-    uint32_t stride;
     uint32_t match;
-    uint64_t first_pos;
-    uint64_t cnt;
 };
 
 // get-entries leaves: SHA-256(0x00 || decoded leaf_input) of p.n entries -> rows[n][32]; rows of bad leaf_inputs are not written
 cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t s);
-// folds a chunk into the tree: one launch for the missing leaf, one per level of the chunk's range (level buffers
-// lvl[2], each [cnt / 2 + 2][32]), one to commit the new size.  Returns the number of launches in *launches.
-cudaError_t launch_tree_fold(const FoldChunk& f, uint8_t* const lvl[2], cudaStream_t s, uint32_t* launches);
-// the root from the edge, rows of clear bits zeroed
-cudaError_t launch_tree_root(TreeDev* tree, cudaStream_t s);
+// Folds a chunk into its trees: one launch for the missing leaves, one per level of the widest tree range, for all trees
+// (level buffers lvl[2], each [total / 2 + 2 * n_desc][32]), one to commit the new sizes.  hdesc is the host copy of
+// f.desc (the level loop's bounds).  Returns the number of launches in *launches.
+cudaError_t launch_tree_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t* const lvl[2], cudaStream_t s, uint32_t* launches);
+// the roots of trees[0, n) from their edges, rows of clear bits zeroed
+cudaError_t launch_tree_root(TreeDev* trees, uint32_t n, cudaStream_t s);
 
 }  // namespace ctmr

@@ -1,20 +1,25 @@
-// ctmr_merkle.cu -- the log's Merkle tree (RFC 6962 §2.1) over the entries of ctmr_process_raw_tree /
-// ctmr_process_tiles_tree (include/ctmr_frontend.h).
+// ctmr_merkle.cu -- the logs' Merkle trees (RFC 6962 §2.1) over the entries of ctmr_process_raw_tree /
+// ctmr_process_tiles_tree (one tree) and ctmr_process_raw_trees / ctmr_process_tiles_trees (one tree per log of the
+// batch) (include/ctmr_frontend.h).  The one-tree calls are the case of one tree whose order is the identity.
 //
 //   K_raw_leaf_hash   thread per entry    SHA-256(0x00 || decoded leaf_input), read from the decoded arena
 //   (tile_leaf_hash)                      tiles: the leaf hashes of ctmr_tiles.cu, unchanged
-//   K_tree_missing    thread per entry    lowest log position of the chunk without a leaf (bad base64, bad tile)
-//   K_tree_level      thread per parent   one level of the chunk's range: parents of the pairs inside it, the left edge
+//   K_tree_missing    thread per entry    per tree, lowest log position of the chunk without a leaf (bad base64, bad tile)
+//   K_tree_level      thread per parent   one level of every tree's range: parents of the pairs inside it, the left edge
 //                                         node as the first left child, the last node as the new edge node
-//   K_tree_commit     one thread          the tree's new size
-//   K_tree_root       one thread          the root from the edge
+//   K_tree_commit     thread per tree     the tree's new size
+//   K_tree_root       thread per tree     the root from the edge
 //
-// The tree is held as its right edge (ctmr_tree): for every bit k of size, the root of the complete subtree of 2^k leaves
+// A tree is held as its right edge (ctmr_tree): for every bit k of size, the root of the complete subtree of 2^k leaves
 // ending at the highest multiple of 2^(k+1) at or below size.  Folding leaves [a, b) in: at level l the chunk covers node
 // positions [a_l, b_l) = [a >> l, b >> l); pairs (2p, 2p+1) inside it make the parents [a_l >> 1, b_l >> 1); an odd a_l
 // takes edge[l] as the left child of the first parent; an odd b_l leaves node b_l - 1 as the new edge[l].  Once the range
 // is empty the higher rows keep what they hold.  A chunk of n leaves costs about n node hashes of two compressions each
-// and one launch per level.
+// and one launch per level of its widest tree range.  The host lists a chunk's entries grouped by tree (FoldChunk.order),
+// so each tree reads its leaves as one run in log order; the threads of a level launch are split between the trees by
+// level_base.
+#include <algorithm>
+
 #include "ctmr_common.cuh"
 
 namespace ctmr {
@@ -92,51 +97,104 @@ __global__ void __launch_bounds__(128) raw_leaf_hash_kernel(FeParams p, uint8_t*
     store_row(rows + 32 * e, h);
 }
 
-// where this chunk's fold ends: see FoldChunk
-__device__ __forceinline__ uint64_t fold_end(const FoldChunk& f) {
-    const uint64_t size = f.tree->t.size, lim = f.first_pos + f.cnt, miss = f.tree->missing;
-    if (size < f.first_pos) return size;
+__host__ __device__ __forceinline__ uint64_t shr64(uint64_t x, uint32_t s) { return s >= 64u ? 0ull : x >> s; }
+
+// where a tree's fold of this chunk ends: see FoldTree
+__device__ __forceinline__ uint64_t fold_end(const TreeDev* tree, const FoldTree& d) {
+    const uint64_t size = tree->t.size, lim = d.first_pos + d.cnt, miss = tree->missing;
+    if (size < d.first_pos) return size;
     return miss < lim ? (miss > size ? miss : size) : lim;
 }
 
-__global__ void __launch_bounds__(256) tree_missing_kernel(FoldChunk f) {
-    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= f.cnt || f.flags[j * f.stride] != f.match) return;
-    const uint64_t pos = f.first_pos + j;
-    if (pos >= f.tree->t.size) atomicMin(&f.tree->missing, (unsigned long long)pos);
+// Tree d's first thread of a level-l launch, and its first row in that launch's level buffer.  Tree d has at most
+// (cnt >> (l + 1)) + 2 parents at level l, and consecutive trees' bases differ by at least that much, so the trees'
+// ranges of threads and rows never overlap; the last ends below (total >> (l + 1)) + 2 * n_desc.
+__device__ __forceinline__ uint64_t level_base(const FoldTree& d, uint32_t i, uint32_t level) {
+    return shr64(d.off, level + 1) + 2ull * i;
 }
 
-// src holds the level's nodes from position `base` on (level 0: the chunk's leaf rows from first_pos, higher levels: the
-// previous launch's parents from a_l); dst gets the parents from a_l >> 1 on.  Only thread 0 touches edge[level]: it
-// reads the old row for the first parent before it writes the new one.
+// the last tree i with key(i) <= k; f.n_desc when there is none (binary search: key is non-decreasing in i)
+template <class Key>
+__device__ __forceinline__ uint32_t find_tree(const FoldChunk& f, uint64_t k, Key key) {
+    if (key(0) > k) return f.n_desc;
+    uint32_t lo = 0, hi = f.n_desc;
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (key(mid) <= k) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// the leaf row of tree d's entry j (the chunk's entries in log order through f.order)
+__device__ __forceinline__ const uint8_t* leaf_row(const FoldChunk& f, const FoldTree& d, uint64_t j) {
+    const uint64_t at = d.off + j;
+    return f.leaves + 32 * (f.order ? (uint64_t)f.order[at] : at);
+}
+
+// one thread per listed entry: the lowest position of each tree without a leaf
+__global__ void __launch_bounds__(256) tree_missing_kernel(FoldChunk f) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= f.total) return;
+    const uint32_t i = find_tree(f, g, [&](uint32_t x) { return (uint64_t)f.desc[x].off; });
+    if (i == f.n_desc) return;
+    const FoldTree d = f.desc[i];
+    if (g >= (uint64_t)d.off + d.cnt) return;  // entries a tiles chunk cut off after its stop
+    const uint64_t e = f.order ? (uint64_t)f.order[g] : g;
+    if (f.flags[e * f.stride] != f.match) return;
+    TreeDev* tree = f.trees + d.tree;
+    const uint64_t pos = d.first_pos + (g - d.off);
+    if (pos >= tree->t.size) atomicMin(&tree->missing, (unsigned long long)pos);
+}
+
+// One level of every tree of the chunk.  Per tree: src holds the level's nodes from position `base` on (level 0: the
+// tree's leaf rows from first_pos, through the order; higher levels: the previous launch's parents from a_l, at the tree's
+// rows of that launch); dst gets the parents from a_l >> 1 on, at the tree's rows of this launch.  Only the tree's first
+// thread touches its edge[level]: it reads the old row for the first parent before it writes the new one.
 __global__ void __launch_bounds__(128) tree_level_kernel(FoldChunk f, uint32_t level, const uint8_t* __restrict__ src,
                                                         uint8_t* __restrict__ dst) {
     const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t a = f.tree->t.size >> level, b = fold_end(f) >> level;
+    const uint32_t i = find_tree(f, k, [&](uint32_t x) { return level_base(f.desc[x], x, level); });
+    if (i == f.n_desc) return;
+    const FoldTree d = f.desc[i];
+    TreeDev* tree = f.trees + d.tree;
+    const uint64_t a = tree->t.size >> level, b = fold_end(tree, d) >> level;
     if (a == b) return;
-    const uint64_t base = level == 0 ? f.first_pos : a, pa = a >> 1, pb = b >> 1, p = pa + k;
-    uint8_t* edge = f.tree->t.edge[level];
+    const uint64_t k0 = level_base(d, i, level), pa = a >> 1, pb = b >> 1, p = pa + (k - k0);
+    const uint64_t in = level == 0 ? 0 : level_base(d, i, level - 1);
+    auto row = [&](uint64_t pos) {  // node `pos` of this level
+        return level == 0 ? leaf_row(f, d, pos - d.first_pos) : src + 32 * (in + pos - a);
+    };
+    uint8_t* edge = tree->t.edge[level];
     if (p < pb) {
         uint32_t l[8], r[8], h[8];
-        load_row(2 * p < a ? edge : src + 32 * (2 * p - base), l);
-        load_row(src + 32 * (2 * p + 1 - base), r);
+        load_row(2 * p < a ? edge : row(2 * p), l);
+        load_row(row(2 * p + 1), r);
         node_hash(l, r, h);
-        store_row(dst + 32 * (p - pa), h);
+        store_row(dst + 32 * (k0 + p - pa), h);
     }
-    if (k == 0 && (b & 1)) {
+    if (k == k0 && (b & 1)) {
         uint32_t h[8];
-        load_row(src + 32 * (b - 1 - base), h);
+        load_row(row(b - 1), h);
         store_row(edge, h);
     }
 }
 
+// one thread per tree of the chunk
 __global__ void tree_commit_kernel(FoldChunk f) {
-    f.tree->t.size = fold_end(f);
-    f.tree->missing = ~0ull;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= f.n_desc) return;
+    const FoldTree d = f.desc[i];
+    TreeDev* tree = f.trees + d.tree;
+    tree->t.size = fold_end(tree, d);
+    tree->missing = ~0ull;
 }
 
-__global__ void tree_root_kernel(TreeDev* tree) {
-    ctmr_tree& t = tree->t;
+// one thread per tree of the call
+__global__ void tree_root_kernel(TreeDev* trees, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ctmr_tree& t = trees[i].t;
     const uint64_t size = t.size;
     uint32_t r[8];
     if (size == 0) {  // SHA-256 of the empty string
@@ -163,8 +221,6 @@ __global__ void tree_root_kernel(TreeDev* tree) {
         if (!((size >> k) & 1ull)) memset(t.edge[k], 0, 32);
 }
 
-__host__ __forceinline__ uint64_t shr64(uint64_t x, uint32_t s) { return s >= 64u ? 0ull : x >> s; }
-
 }  // namespace
 
 cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t s) {
@@ -173,25 +229,31 @@ cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t 
     return cudaGetLastError();
 }
 
-cudaError_t launch_tree_fold(const FoldChunk& f, uint8_t* const lvl[2], cudaStream_t s, uint32_t* launches) {
+cudaError_t launch_tree_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t* const lvl[2], cudaStream_t s, uint32_t* launches) {
     *launches = 0;
-    if (f.cnt == 0) return cudaSuccess;
-    tree_missing_kernel<<<(unsigned)((f.cnt + 255) / 256), 256, 0, s>>>(f);
+    if (f.n_desc == 0) return cudaSuccess;
+    tree_missing_kernel<<<(unsigned)((f.total + 255) / 256), 256, 0, s>>>(f);
     ++*launches;
-    // Levels where the chunk's own range [first_pos, first_pos + cnt) is empty are empty for the part that folds too
-    const uint64_t lo = f.first_pos, hi = f.first_pos + f.cnt;
-    for (uint32_t l = 0; l < 64u && shr64(lo, l) != shr64(hi, l); ++l) {
-        const uint64_t parents = shr64(hi, l + 1) - shr64(lo, l + 1) + 1;
-        tree_level_kernel<<<(unsigned)((parents + 127) / 128), 128, 0, s>>>(f, l, l == 0 ? f.leaves : lvl[(l - 1) & 1], lvl[l & 1]);
+    // Levels where a tree's own range [first_pos, first_pos + cnt) is empty are empty for the part that folds too: the
+    // chunk takes as many level launches as its widest range has levels
+    uint32_t levels = 0;
+    for (uint32_t i = 0; i < f.n_desc; ++i) {
+        const uint64_t x = hdesc[i].first_pos ^ (hdesc[i].first_pos + hdesc[i].cnt);
+        levels = std::max(levels, x ? 64u - (uint32_t)__builtin_clzll(x) : 0u);
+    }
+    for (uint32_t l = 0; l < levels; ++l) {
+        const uint64_t threads = shr64(f.total, l + 1) + 2ull * f.n_desc;
+        tree_level_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(f, l, l == 0 ? f.leaves : lvl[(l - 1) & 1], lvl[l & 1]);
         ++*launches;
     }
-    tree_commit_kernel<<<1, 1, 0, s>>>(f);
+    tree_commit_kernel<<<(f.n_desc + 127) / 128, 128, 0, s>>>(f);
     ++*launches;
     return cudaGetLastError();
 }
 
-cudaError_t launch_tree_root(TreeDev* tree, cudaStream_t s) {
-    tree_root_kernel<<<1, 1, 0, s>>>(tree);
+cudaError_t launch_tree_root(TreeDev* trees, uint32_t n, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    tree_root_kernel<<<(n + 127) / 128, 128, 0, s>>>(trees, n);
     return cudaGetLastError();
 }
 

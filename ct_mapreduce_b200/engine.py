@@ -85,6 +85,30 @@ class LogTree:
         return cls(int(t.size), np.frombuffer(bytes(t.edge), np.uint8).reshape(64, 32).copy(), bytes(t.root))
 
 
+def _trees_to_c(trees):
+    """[LogTree] -> a ctmr_tree array"""
+    arr = (capi.Tree * max(len(trees), 1))()
+    for d, t in enumerate(trees):
+        arr[d] = t.to_c()
+    return arr
+
+
+def _log_ids(log, n: int, what: str) -> np.ndarray:
+    log = np.ascontiguousarray(log, np.uint32)
+    if log.shape != (n,):
+        raise CtmrError(capi.E_INVALID, f"{what} must hold one log id per {'entry' if what == 'entry_log' else 'tile'}")
+    return log
+
+
+def _tree_args(tree, trees, log, name):
+    if tree is not None and trees is not None:
+        raise CtmrError(capi.E_INVALID, "pass tree= (one log) or trees= (one per log), not both")
+    if trees is None and log is not None:
+        raise CtmrError(capi.E_INVALID, f"{name} goes with trees=")
+    if trees is not None and log is None:
+        raise CtmrError(capi.E_INVALID, f"trees= needs {name}")
+
+
 def _pack(ders):
     offsets = np.zeros(len(ders) + 1, np.uint64)
     offsets[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
@@ -117,6 +141,7 @@ class RawBatchResult:
         self.leaf_off = np.zeros(n, np.uint32)
         self.leaf_len = np.zeros(n, np.uint32)
         self.tree = None    # LogTree after the batch, when the call was given one
+        self.trees = None   # [LogTree] after the batch, when the call was given trees= (one per log)
 
 
 class TileBatchResult(RawBatchResult):
@@ -252,10 +277,14 @@ class GpuCertDatabase:
 
     # ------------------------------------------------------------------ CT wire-format front end (include/ctmr_frontend.h)
     def store_raw_entries(self, text, leaf_off, leaf_len, extra_off, extra_len, now_unix_ns: int, want_sha: bool = True,
-                          want_meta: bool = False, want_pem: bool = False, tree: LogTree | None = None) -> "RawBatchResult":
+                          want_meta: bool = False, want_pem: bool = False, tree: LogTree | None = None, trees=None,
+                          entry_log=None) -> "RawBatchResult":
         """get-entries strings (base64 leaf_input / extra_data, spans into `text`) through ctmr_process_raw:
         what GetRawEntries' JSON decode, ct.LogEntryFromLeaf (ct-fetch.go:424,452) and insertCTWorker + Store do.
-        With tree= (the log's entries before these), ctmr_process_raw_tree also folds the entries into it: r.tree."""
+        With tree= (the log's entries before these), ctmr_process_raw_tree also folds the entries into it: r.tree.
+        With trees= (one LogTree per log) and entry_log= (the log of each entry, capi.NO_TREE for none),
+        ctmr_process_raw_trees folds each entry into its log's tree: r.trees."""
+        _tree_args(tree, trees, entry_log, "entry_log")
         text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else np.ascontiguousarray(text, np.uint8)
         leaf_off, extra_off = np.ascontiguousarray(leaf_off, np.uint64), np.ascontiguousarray(extra_off, np.uint64)
         leaf_len, extra_len = np.ascontiguousarray(leaf_len, np.uint32), np.ascontiguousarray(extra_len, np.uint32)
@@ -273,6 +302,13 @@ class GpuCertDatabase:
             _attach_pem(o.path, p, n, (int(leaf_len.sum()) + int(extra_len.sum())) // 4 * 3)
         b = capi.RawBatch(capi.ptr(text), text.size, capi.ptr(leaf_off), capi.ptr(leaf_len), capi.ptr(extra_off), capi.ptr(extra_len),
                           n, now_unix_ns)
+        if trees is not None:
+            log = _log_ids(entry_log, n, "entry_log")
+            arr = _trees_to_c(trees)
+            self._check(self._lib.ctmr_process_raw_trees(self._h, C.byref(b), C.byref(o), capi.ptr(log) if n else None,
+                                                         arr if trees else None, len(trees)))
+            r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
+            return r
         if tree is None:
             self._check(self._process_raw_fn()(self._h, C.byref(b), C.byref(o)))
             return r
@@ -305,12 +341,15 @@ class GpuCertDatabase:
 
     def store_tiles(self, data, tile_off, tile_len, tile_index, tile_width, now_unix_ns: int, want_sha: bool = True,
                     want_meta: bool = False, want_pem: bool = False, want_leaf_hash: bool = False, missing_cap: int = 256,
-                    fetch=None, tree: LogTree | None = None) -> "TileBatchResult":
+                    fetch=None, tree: LogTree | None = None, trees=None, tile_log=None) -> "TileBatchResult":
         """static-ct-api data tiles through ctmr_process_tiles.  Without `fetch`, a tile naming an unregistered Chain[0]
         stops the call: the result has tiles_done < n_tiles and the missing fingerprints.  With fetch(fingerprints) ->
         DERs, those certificates are registered and the call resumes from there until every tile is done.  With tree= (the
         log's entries before these; consecutive tiles of that log), ctmr_process_tiles_tree also folds the entries into
-        it and every resumed call carries it on: r.tree."""
+        it and every resumed call carries it on: r.tree.  With trees= (one LogTree per log) and tile_log= (the log of each
+        tile, capi.NO_TREE for none), ctmr_process_tiles_trees folds each tile into its log's tree: r.trees; a resumed
+        call carries the trees on, and passes as NO_TREE the rest of a log whose fold a bad tile stopped."""
+        _tree_args(tree, trees, tile_log, "tile_log")
         data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
         tile_off, tile_index = np.ascontiguousarray(tile_off, np.uint64), np.ascontiguousarray(tile_index, np.uint64)
         tile_len, tile_width = np.ascontiguousarray(tile_len, np.uint32), np.ascontiguousarray(tile_width, np.uint16)
@@ -324,6 +363,9 @@ class GpuCertDatabase:
             _attach_pem(capi.Out(), p, n, int(tile_len.astype(np.int64).sum()))
         miss = np.zeros((max(missing_cap, 1), 32), np.uint8)
         ct = tree.to_c() if tree is not None else None
+        if trees is not None:
+            tlog = _log_ids(tile_log, nt, "tile_log").copy()
+            arr = _trees_to_c(trees)
         t0, pem_base = 0, 0
         while True:
             e0 = int(ent[t0])
@@ -347,7 +389,17 @@ class GpuCertDatabase:
                                capi.ptr(tile_index) + 8 * t0, capi.ptr(tile_width) + 2 * t0, nt - t0, now_unix_ns)
             if ct is not None and t0 > 0 and ct.size < 256 * int(tile_index[t0]):
                 ct = None  # a bad tile among the completed tiles stopped the fold: r.tree is final, the rest runs plain
-            if ct is None:
+            if trees is not None:
+                if t0 > 0:  # a log whose tree stopped below its first tile of the rest: a bad tile stopped its fold
+                    for d in range(len(trees)):
+                        rest = np.flatnonzero(tlog[t0:] == d)
+                        if rest.size and arr[d].size < 256 * int(tile_index[t0 + rest[0]]):
+                            tlog[t0 + rest] = capi.NO_TREE
+                rc = self._lib.ctmr_process_tiles_trees(self._h, C.byref(b), C.byref(o), capi.ptr(tlog) + 4 * t0 if nt else None,
+                                                        arr if trees else None, len(trees))
+                if rc in (0, capi.E_UNKNOWN_ISSUER):
+                    r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
+            elif ct is None:
                 rc = self._process_tiles_fn()(self._h, C.byref(b), C.byref(o))
             else:  # written back on success and at the stop: the resumed call continues this tree
                 rc = self._lib.ctmr_process_tiles_tree(self._h, C.byref(b), C.byref(o), C.byref(ct))
@@ -537,14 +589,14 @@ class GpuCertGroup(GpuCertDatabase):
     def _process_tiles_fn(self):
         return self._lib.ctmr_group_process_tiles
 
-    def store_raw_entries(self, *a, tree=None, **k):
-        if tree is not None:  # members hold disjoint slices: the fold would have to be ordered across GPUs
-            raise CtmrError(capi.E_INVALID, "tree= takes one ctx: a group has no tree form")
+    def store_raw_entries(self, *a, tree=None, trees=None, **k):
+        if tree is not None or trees is not None:  # members hold disjoint slices: the fold would have to be ordered across GPUs
+            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: a group has no tree form")
         return super().store_raw_entries(*a, **k)
 
-    def store_tiles(self, *a, tree=None, **k):
-        if tree is not None:
-            raise CtmrError(capi.E_INVALID, "tree= takes one ctx: a group has no tree form")
+    def store_tiles(self, *a, tree=None, trees=None, **k):
+        if tree is not None or trees is not None:
+            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: a group has no tree form")
         return super().store_tiles(*a, **k)
 
     def _register_chain_fn(self):

@@ -41,6 +41,7 @@ type RawPages struct {
 	LeafLen   []uint32
 	ExtraOff  []uint64
 	ExtraLen  []uint32
+	Log       []uint32 // the log of each entry, for ProcessRawTrees (tree.go); NoTree for entries of Append
 }
 
 var (
@@ -49,8 +50,14 @@ var (
 )
 
 // Append copies one response body into the pinned text and records its string spans.  A body whose
-// strings carry JSON escapes (no CT log emits any) must be unescaped by the caller first.
+// strings carry JSON escapes (no CT log emits any) must be unescaped by the caller first.  Its entries belong to no
+// tree (AppendLog).
 func (p *RawPages) Append(body []byte) error {
+	return p.AppendLog(body, NoTree)
+}
+
+// AppendLog is Append for a body of log `log`: ProcessRawTrees folds its entries into trees[log].
+func (p *RawPages) AppendLog(body []byte, log uint32) error {
 	if p.Used+uint64(len(body)) > p.Cap {
 		return fmt.Errorf("raw page buffer full")
 	}
@@ -80,6 +87,9 @@ func (p *RawPages) Append(body []byte) error {
 	}
 	if len(p.LeafOff) != len(p.ExtraOff) {
 		return fmt.Errorf("get-entries body with %d leaf_input and %d extra_data strings", len(p.LeafOff), len(p.ExtraOff))
+	}
+	for len(p.Log) < len(p.LeafOff) {
+		p.Log = append(p.Log, log)
 	}
 	p.Used += uint64(len(body))
 	return nil
@@ -128,25 +138,27 @@ func (r *RawResult) Free() {
 // ProcessRaw = GetRawEntries' base64 decode + ct.LogEntryFromLeaf + insertCTWorker + Store decisions for
 // every entry of the accumulated pages, in page order, on one GPU or on every GPU of the group.
 func (d *DB) ProcessRaw(p *RawPages, nowUnixNs int64, r *RawResult) error {
-	return d.processRaw(p, nowUnixNs, r, nil)
+	return d.processRaw(p, nowUnixNs, r, nil, nil, false)
 }
 
-// processRaw also folds the entries into tree when it is not nil (ProcessRawTree, tree.go).
-func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree) error {
+// processRaw also folds the entries into tree when it is not nil (ProcessRawTree, tree.go), or, when routed, each entry
+// into trees[p.Log[i]] (ProcessRawTrees).
+func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree, trees []Tree, routed bool) error {
 	n := len(p.LeafOff)
-	if tree != nil && d.g != nil {
-		return fmt.Errorf("ProcessRawTree: a group has no tree form; use one DB per GPU")
+	if (tree != nil || routed) && d.g != nil {
+		return fmt.Errorf("ProcessRawTree(s): a group has no tree form; use one DB per GPU")
 	}
-	if n == 0 && tree == nil {
+	if n == 0 && tree == nil && !routed {
 		return nil
-	}
-	if n == 0 { // the root of the tree as it stands
-		b := (*C.ctmr_raw_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_raw_batch{}))))
-		defer C.free(unsafe.Pointer(b))
-		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
 	}
 	b := (*C.ctmr_raw_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_raw_batch{}))))
 	defer C.free(unsafe.Pointer(b))
+	if n == 0 { // the roots of the trees as they stand
+		if routed {
+			return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, nil, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")
+		}
+		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
+	}
 	// the span arrays are flat Go slices; the struct that points at them is C memory, and the pointers are only
 	// stored for the duration of the call -> pin them (Go 1.21 runtime.Pinner) so that the store is legal
 	var pin runtime.Pinner
@@ -165,6 +177,13 @@ func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree) 
 	b.now_unix_ns = C.int64_t(nowUnixNs)
 	if d.g != nil { // several GPUs: one chunk per GPU per round, the same outputs in entry order
 		return d.err(C.ctmr_group_process_raw(d.g, b, r.raw), "ctmr_group_process_raw")
+	}
+	if routed {
+		if len(p.Log) != n {
+			return fmt.Errorf("ProcessRawTrees: %d log ids for %d entries", len(p.Log), n)
+		}
+		log := (*C.uint32_t)(unsafe.Pointer(&p.Log[0])) // pointer-free Go memory, passed for the call only
+		return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, log, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")
 	}
 	if tree != nil {
 		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")

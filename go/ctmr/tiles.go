@@ -31,9 +31,15 @@ type Tiles struct {
 	Len       []uint32
 	Index     []uint64 // N of tile/data/<N>
 	Width     []uint16 // 256, or W of a partial tile .p/<W>
+	Log       []uint32 // the log of each tile, for ProcessTilesTrees (tree.go); NoTree for tiles of Append
 }
 
 func (t *Tiles) Append(body []byte, index uint64, width uint16) error {
+	return t.AppendLog(body, index, width, NoTree)
+}
+
+// AppendLog is Append for a tile of log `log`: ProcessTilesTrees folds its entries into trees[log].
+func (t *Tiles) AppendLog(body []byte, index uint64, width uint16, log uint32) error {
 	if t.Used+uint64(len(body)) > t.Cap {
 		return fmt.Errorf("tile buffer full")
 	}
@@ -42,6 +48,7 @@ func (t *Tiles) Append(body []byte, index uint64, width uint16) error {
 	t.Len = append(t.Len, uint32(len(body)))
 	t.Index = append(t.Index, index)
 	t.Width = append(t.Width, width)
+	t.Log = append(t.Log, log)
 	t.Used += uint64(len(body))
 	return nil
 }
@@ -119,22 +126,34 @@ func (d *DB) RegisterChainCerts(ders [][]byte) ([]uint32, error) {
 // registered before the call resumes from that tile.  The result equals one call made with every certificate
 // registered beforehand: every per-entry output of a resumed call, PEM included, lands at the entries it belongs to.
 func (d *DB) ProcessTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error)) error {
-	return d.processTiles(t, nowUnixNs, r, fetch, nil)
+	return d.processTiles(t, nowUnixNs, r, fetch, nil, nil, false)
 }
 
-// processTiles also folds the entries into tree when it is not nil (ProcessTilesTree, tree.go): the library writes the
-// tree back at every stop, so each resumed call carries it on from the tiles completed so far.
-func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree) error {
-	if tree != nil && d.g != nil {
-		return fmt.Errorf("ProcessTilesTree: a group has no tree form; use one DB per GPU")
+// processTiles also folds the entries into tree when it is not nil (ProcessTilesTree, tree.go), or, when routed, each
+// tile into trees[t.Log[k]] (ProcessTilesTrees): the library writes the trees back at every stop, so each resumed call
+// carries them on from the tiles completed so far.
+func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree,
+	trees []Tree, routed bool) error {
+	if (tree != nil || routed) && d.g != nil {
+		return fmt.Errorf("ProcessTilesTree(s): a group has no tree form; use one DB per GPU")
+	}
+	if routed && len(t.Log) != len(t.Off) {
+		return fmt.Errorf("ProcessTilesTrees: %d log ids for %d tiles", len(t.Log), len(t.Off))
 	}
 	if len(t.Off) == 0 {
-		if tree != nil { // the root of the tree as it stands
+		if tree != nil || routed { // the roots of the trees as they stand
 			b := (*C.ctmr_tile_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_batch{}))))
 			defer C.free(unsafe.Pointer(b))
+			if routed {
+				return d.err(C.ctmr_process_tiles_trees(d.h, b, r.out, nil, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_tiles_trees")
+			}
 			return d.err(C.ctmr_process_tiles_tree(d.h, b, r.out, tree.c()), "ctmr_process_tiles_tree")
 		}
 		return nil
+	}
+	var log []uint32 // routed: the tiles' logs, the rest of a log whose fold a bad tile stopped turned to NoTree
+	if routed {
+		log = append([]uint32(nil), t.Log...)
 	}
 	var pin runtime.Pinner
 	defer pin.Unpin()
@@ -158,9 +177,24 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 		shiftTileOut(o, e0, t0, pemBase) // a resumed call writes from entry e0, tile t0 and PEM byte pemBase on
 		// a bad tile among the tiles completed before a stop ended the fold: the tree is final, the rest runs plain
 		fold := tree != nil && (t0 == 0 || tree.Size >= 256*t.Index[t0])
+		if routed && t0 > 0 { // a log whose tree stopped below its first remaining tile: a bad tile ended its fold
+			stopped := map[uint32]bool{}
+			for k := t0; k < len(log); k++ {
+				if l := log[k]; l != NoTree {
+					if _, seen := stopped[l]; !seen {
+						stopped[l] = int(l) < len(trees) && trees[l].Size < 256*t.Index[k]
+					}
+					if stopped[l] {
+						log[k] = NoTree
+					}
+				}
+			}
+		}
 		var rc C.int
 		if d.g != nil {
 			rc = C.ctmr_group_process_tiles(d.g, b, o)
+		} else if routed {
+			rc = C.ctmr_process_tiles_trees(d.h, b, o, (*C.uint32_t)(unsafe.Pointer(&log[t0])), treesC(trees), C.uint32_t(len(trees)))
 		} else if fold {
 			rc = C.ctmr_process_tiles_tree(d.h, b, o, tree.c())
 		} else {

@@ -26,11 +26,34 @@ var _ [unsafe.Sizeof(Tree{}) - unsafe.Sizeof(C.ctmr_tree{})]struct{}
 
 func (t *Tree) c() *C.ctmr_tree { return (*C.ctmr_tree)(unsafe.Pointer(t)) }
 
+// NoTree mirrors CTMR_NO_TREE: an entry or tile that folds into no tree.  MaxTrees mirrors CTMR_MAX_TREES.
+const (
+	NoTree   = uint32(C.CTMR_NO_TREE)
+	MaxTrees = int(C.CTMR_MAX_TREES)
+)
+
+// treesC passes a []Tree to the library straight from Go memory: Tree holds no pointers.
+func treesC(trees []Tree) *C.ctmr_tree {
+	if len(trees) == 0 {
+		return nil
+	}
+	return trees[0].c()
+}
+
 // ProcessRawTree is ProcessRaw, and the pages' entries folded into tree as the log's entries tree.Size, tree.Size+1, ....
 // An entry whose leaf_input is not base64 has no leaf: the fold stops before it and tree.Size says where.  On an error
 // tree is unchanged.  One GPU only: a group returns an error.
 func (d *DB) ProcessRawTree(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree) error {
-	return d.processRaw(p, nowUnixNs, r, tree)
+	return d.processRaw(p, nowUnixNs, r, tree, nil, false)
+}
+
+// ProcessRawTrees is ProcessRaw, and every entry folded into the tree of its log: the entries of a body added with
+// AppendLog(body, log) are the next leaves of trees[log]; those added with Append fold nowhere.  This is the one flush
+// of a batcher that drains the pages of every log it syncs into one RawPages: each log keeps the one-tree rules on its
+// own entries, and a bad base64 leaf_input stops only its own log's tree.  Every tree gets its root written, also a tree
+// with no entry in the batch.  On an error every tree is unchanged.  One GPU only.
+func (d *DB) ProcessRawTrees(p *RawPages, nowUnixNs int64, r *RawResult, trees []Tree) error {
+	return d.processRaw(p, nowUnixNs, r, nil, trees, true)
 }
 
 // ProcessTilesTree is ProcessTiles, and the tiles' entries folded into tree.  The tiles must be consecutive tiles of one
@@ -39,5 +62,14 @@ func (d *DB) ProcessRawTree(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tr
 // tree from call to call; once a bad tile has stopped the fold, it resumes with ProcessTiles' plain call and the tree
 // stays as it is.  Tree and outputs equal those of one call with every certificate registered first.  One GPU only.
 func (d *DB) ProcessTilesTree(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree) error {
-	return d.processTiles(t, nowUnixNs, r, fetch, tree)
+	return d.processTiles(t, nowUnixNs, r, fetch, tree, nil, false)
+}
+
+// ProcessTilesTrees is ProcessTiles, and every tile folded into the tree of its log: a tile added with
+// AppendLog(body, index, width, log) is the next tile of trees[log]; one added with Append folds nowhere.  Each log's
+// tiles keep ProcessTilesTree's rules in batch order, interleaved with the other logs' in any way.  The resume loop
+// carries the trees; a log whose tree a bad tile stopped (its size is below its first remaining tile) goes on as
+// NoTree.  Trees and outputs equal those of one call with every certificate registered first.  One GPU only.
+func (d *DB) ProcessTilesTrees(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), trees []Tree) error {
+	return d.processTiles(t, nowUnixNs, r, fetch, nil, trees, true)
 }

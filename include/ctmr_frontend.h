@@ -220,6 +220,37 @@ int ctmr_process_raw_tree(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_o
  * other error *tree is left as it was passed in. */
 int ctmr_process_tiles_tree(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_tile_out* out, ctmr_tree* tree);
 
+/* ---- the Merkle trees of several logs in one call ---------------------------------------------------------------------
+ * A client that syncs many logs at once drains the entries of all of them into one batch.  These calls fold each entry
+ * into the tree of its own log; everything else -- outputs, return codes, global indices, PEM, the tiles' stop and
+ * resume -- is exactly that of ctmr_process_raw / ctmr_process_tiles.
+ *
+ * Routing: entry i (pages), or every entry of tile t (tiles), is the next leaf of trees[entry_log[i]] (trees[tile_log[t]]);
+ * CTMR_NO_TREE folds it into no tree.  The entries of one log appear in the batch in log order; they may be interleaved
+ * with other logs' in any way (page by page, entry by entry, tile by tile).  Each tree keeps the rules of the one-tree
+ * call on its own entries: the leaf hash is SHA-256(0x00 || decoded leaf_input), only bad base64 has no leaf and stops
+ * that tree's fold (no other tree's), and size + (entries of that log) must not wrap around 2^64 (pages); the log's tiles
+ * in batch order are consecutive, all full but its last, the tree's size lies inside its first tile (leaves below it are
+ * skipped), its last leaf index fits 64 bits, and a bad tile stops only its own log's fold (tiles).
+ *
+ * Before any work, with no index taken and no tree touched, CTMR_E_INVALID for: trees NULL with n_trees > 0, entry_log /
+ * tile_log NULL with entries / tiles in the batch, n_trees > CTMR_MAX_TREES, a log id >= n_trees that is not
+ * CTMR_NO_TREE, or a broken per-log rule.  Every tree passed in gets its root written, also a tree of no entry in the
+ * batch; rows of clear bits come back zero.  On CTMR_E_UNKNOWN_ISSUER (tiles) every tree is written back holding the
+ * completed tiles; on any other error every tree is left as passed in.  A member of a group is refused. */
+#define CTMR_NO_TREE 0xFFFFFFFFu
+#define CTMR_MAX_TREES 1024u   /* well above the number of logs any CT log list names */
+
+int ctmr_process_raw_trees(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_out* out,
+                           const uint32_t* entry_log /* [n] */, ctmr_tree* trees, uint32_t n_trees);
+
+/* Resume after CTMR_E_UNKNOWN_ISSUER from tiles_done: a log whose written-back tree->size is below 256 * tile_index of its
+ * first tile in the rest of the batch was stopped by a bad tile, and its tree is final for this batch: pass that log's
+ * remaining tiles as CTMR_NO_TREE.  Every other log resumes with its tree.  The trees and every output then equal those
+ * of one call made with every certificate registered first. */
+int ctmr_process_tiles_trees(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_tile_out* out,
+                             const uint32_t* tile_log /* [n_tiles] */, ctmr_tree* trees, uint32_t n_trees);
+
 #ifdef __cplusplus
 }
 #endif

@@ -43,7 +43,8 @@ EXPORTS = [
     "ctmr_group_table_stats", "ctmr_group_preload_known", "ctmr_group_evict_expired", "ctmr_group_reset",
     "ctmr_group_snapshot_size", "ctmr_group_snapshot_save", "ctmr_group_snapshot_load",
     "ctmr_peer_export", "ctmr_peer_attach", "ctmr_peer_barrier_device", "ctmr_peer_allreduce_histogram_device",
-    "ctmr_bind_host_to_device", "ctmr_peer_rounds", "ctmr_peer_round_entries",
+    "ctmr_bind_host_to_device", "ctmr_peer_rounds", "ctmr_peer_round_entries", "ctmr_peer_frontend_stopped",
+    "ctmr_next_index",
 ]
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -53,6 +54,7 @@ def peer_rounds() -> int:
     return int(load().ctmr_peer_rounds())
 E_PAIR_TABLE_FULL, E_META_TABLE_FULL, E_PEER_TIMEOUT, E_PEER = -8, -9, -10, -11
 E_UNKNOWN_ISSUER = -12
+E_PEER_FAILED = -13   # another rank's part of a collective call failed before any work
 # per-entry outcome of the front end (include/ctmr_frontend.h CTMR_FE_*)
 FE_OK, FE_BAD_BASE64, FE_BAD_LEAF, FE_UNKNOWN_TYPE, FE_BAD_EXTRA, FE_BAD_CERT, FE_BAD_TILE, FE_BAD_INDEX = range(8)
 NO_TREE = 0xFFFFFFFF   # CTMR_NO_TREE: an entry or tile of ctmr_process_*_trees that folds into no tree
@@ -235,6 +237,8 @@ def load():
     L.ctmr_peer_rounds.restype = u32
     L.ctmr_peer_round_entries.argtypes = [u64]
     L.ctmr_peer_round_entries.restype = u64
+    L.ctmr_peer_frontend_stopped.argtypes = [vp, C.POINTER(u32)]
+    L.ctmr_next_index.argtypes = [vp, C.POINTER(u64)]
     for name in EXPORTS:
         getattr(L, name)  # every symbol include/ctmr.h declares must resolve
     _lib = L

@@ -276,7 +276,11 @@ struct SharedLayout {
 
 enum PeerMode { PEER_NONE = 0, PEER_GROUP = 1 /* one process, ctmr_group */, PEER_IPC = 2 /* one process per GPU */ };
 
-// barrier channels (each is used from ONE stream per rank, so its epochs are stream ordered on every rank)
+// Barrier channels.  Every rank must pass a channel's epochs in the same order.  Inside one call each channel is used
+// from one stream per rank, so its epochs are stream ordered.  CH_STAGE_* serve two calls: the host pipeline's rounds
+// (on its stage streams) and the front end's collective rounds (on the ctx's stream).  Both calls are synchronous and
+// every rank makes the same sequence of collective calls, so no two calls' barriers on a channel are ever in flight
+// together.
 enum : uint32_t {
     CH_STAGE_MAP = 0,      // + stage index (3): after K_map of a host-pipeline round
     CH_STAGE_RESOLVE = 3,  // + stage index (3): after resolve of a host-pipeline round
@@ -333,6 +337,7 @@ struct ctmr_ctx {
     int last_sub = 0;
     DevBuf<SmallDev> small;
     std::unique_ptr<FrontEnd> fe;
+    uint32_t fe_peer_stopped = 0;  // ranks that stopped (tiles) in the last collective front-end call
     std::string err;
 };
 

@@ -1,8 +1,8 @@
 // ctmr_frontend_api.cu -- the entry points of include/ctmr_frontend.h (SURVEY.md §8(f)-2): get-entries strings -> base64
 // decode -> TLS framing -> Chain[0] identification -> the path (ctmr_process_raw); static-ct-api data tiles -> split ->
 // framing -> Chain[0] by fingerprint -> the path (ctmr_process_tiles, ctmr_register_chain_certs).  Each runs on one GPU, on
-// a group of GPUs driven by one process (ctmr_group_*), and on one GPU with the log's Merkle tree folded in
-// (ctmr_process_*_tree).
+// a group of GPUs driven by one process (ctmr_group_*), on one GPU with the log's Merkle tree folded in
+// (ctmr_process_*_tree), and as a collective call of one process per GPU (a ctx attached with ctmr_peer_attach).
 //
 // One driver serves them all (process_members, over the members of the call: one ctx, or the members of a group).  A call
 // is cut into ROUNDS of one CHUNK per member (entry and character budgets of the front end's buffers).  Per round:
@@ -60,8 +60,9 @@ int check_pem(ctmr_ctx* c, const ctmr_out* o) {
     return CTMR_OK;
 }
 
-// where the path writes a chunk's results: the front end's per-chunk buffers (sha256 and string identities when asked for)
-ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
+// where the path writes a chunk's results: the front end's per-chunk buffers (sha256 when asked for, string identities
+// when the call computes them)
+ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po, bool meta) {
     const uint64_t E = f->cap_entries;
     ctmr_dev_out dout{};
     dout.status = f->status;
@@ -71,7 +72,7 @@ ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po) {
     dout.serial_len = f->serial_len;
     dout.was_unknown = f->was_unknown;
     dout.first_issuer_hour = f->first;
-    if (want_meta(po)) {
+    if (meta) {
         dout.issuer_name_off = f->spans;
         dout.issuer_name_len = f->spans + E;
         dout.crldp_off = f->spans + 2 * E;
@@ -253,6 +254,7 @@ struct Pages {
     ctmr_raw_out* out;
     uint64_t done;  // entries that take their indices: all n whenever there is a batch, also when the call fails once a
                     // chunk has reached the path
+    bool meta = false;  // the call computes string identities (process_members)
 
     std::vector<uint64_t> tree_pos;  // tree calls: log position of each tree's first entry
 
@@ -271,7 +273,7 @@ struct Pages {
 
 // tree: ctmr_process_raw_tree's rule as well; a routed call's rules fail before any index is taken
 int Pages::check(ctmr_ctx* c, const TreeArgs* tree) {
-    if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (!b || !out || (tree && !tree->routed && !tree->trees)) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n && (!b->text || !b->leaf_input_off || !b->leaf_input_len || !b->extra_data_off || !b->extra_data_len))
         return fail(c, CTMR_E_INVALID, "null batch buffers");
     int rc = check_pem(c, &out->path);
@@ -454,7 +456,7 @@ int Pages::front(ctmr_ctx* c, Chunk& ch) const {
     db.n = cnt;
     db.issuer_idx = f->issuer_idx;
     db.now_unix_ns = b->now_unix_ns;
-    ch.dout = chunk_path_out(f, &out->path);
+    ch.dout = chunk_path_out(f, &out->path, meta);
     return CTMR_OK;
 }
 
@@ -486,6 +488,7 @@ struct Tiles {
     const ctmr_tile_batch* b;
     ctmr_tile_out* out;
     uint64_t done = 0;         // entries that take their indices: none when the arguments fail, those before a stop, else all
+    bool meta = false;         // the call computes string identities (process_members)
     std::vector<uint64_t> ent;  // entries before each tile: ent[t] = sum of widths of tiles [0, t)
     std::vector<uint64_t> tree_pos;  // tree calls: log position of each tree's first entry (its first tile's)
 
@@ -529,7 +532,7 @@ int tree_tile_args(ctmr_ctx* c, const ctmr_tile_batch* b, const uint32_t* tile_l
 
 // validates widths and spans (and with a tree its rules), fills ent
 int Tiles::check(ctmr_ctx* c, const TreeArgs* tree) {
-    if (!b || !out) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (!b || !out || (tree && !tree->routed && !tree->trees)) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n_tiles && (!b->data || !b->tile_off || !b->tile_len || !b->tile_index || !b->tile_width))
         return fail(c, CTMR_E_INVALID, "null batch buffers");
     int rc = check_pem(c, &out->path);
@@ -706,7 +709,7 @@ int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
     db.n = p.n;
     db.issuer_idx = f->issuer_idx;
     db.now_unix_ns = b->now_unix_ns;
-    ch.dout = chunk_path_out(f, &out->path);
+    ch.dout = chunk_path_out(f, &out->path, meta);
     return CTMR_OK;
 }
 
@@ -774,18 +777,20 @@ int for_each_member(ctmr_ctx** m, uint32_t W, bool threads, ctmr_ctx** failed, F
 }
 
 // Cuts the round that starts at unit `pos` and issues its uploads into stage `stage`.  One member takes the greedy chunk
-// fit returns.  A group takes one chunk per member from ONE contiguous window, q units each, q halved until every
-// member's chunk fits.
+// fit returns (an empty chunk at the end of the batch: a rank of a collective call runs its last rounds empty).  A group
+// takes one chunk per member from ONE contiguous window, q units each, q halved until every member's chunk fits.
 template <class Format>
 int plan_round(ctmr_ctx** m, uint32_t W, const Format& fm, uint64_t pos, int stage, std::vector<Chunk>& ch, ctmr_ctx** failed) {
     const uint64_t total = fm.units();
     *failed = m[0];
     uint64_t q = 0;
     if (W == 1) {
-        uint64_t hi = 0;
-        const int rc = fm.fit(m[0], pos, ~0ull, &hi);
-        if (rc) return rc;
-        if (hi == pos) return fail(m[0], CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
+        uint64_t hi = pos;
+        if (pos < total) {
+            const int rc = fm.fit(m[0], pos, ~0ull, &hi);
+            if (rc) return rc;
+            if (hi == pos) return fail(m[0], CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
+        }
         q = hi - pos;
     } else {
         q = std::max<uint64_t>(1, std::min<uint64_t>(fm.q_max(m[0]), (total - pos + W - 1) / W));
@@ -834,28 +839,103 @@ int fe_member(ctmr_ctx* c, const ctmr_dev_batch& db, const ctmr_dev_out& dout, i
     x.meta_slots = c->meta_scratch;
     x.map_stream = x.reduce_stream = c->stream;
     x.mapped = c->fe->mapped; x.reduced = c->fe->reduced; x.meta_done = c->fe->meta_done;
-    // the members of an in-process group meet through their events; peer_barrier does nothing for them
+    // The members of an in-process group meet through their events; peer_barrier does nothing for them.  The ranks of a
+    // collective call (one process per GPU) meet at these barriers, which the host pipeline's rounds use too: both
+    // calls are synchronous, so while a front-end call runs no stage stream of any rank has a barrier queued, and
+    // every rank passes each channel's epochs in the same order.
     x.ch_map = CH_STAGE_MAP + parity;
     x.ch_resolve = CH_STAGE_RESOLVE + parity;
     x.ch_meta = CH_STAGE_META + parity;
     return CTMR_OK;
 }
 
-// The path over round k's chunks.  One member: ctmr_process_device on the ctx's stream, which overlaps the map and the
-// reduce of a large chunk.  A group: one round of the key exchange, each member's chunk as its slice.
-int run_path(ctmr_ctx** m, uint32_t W, int k, Chunk* cur, bool meta, ctmr_ctx** failed) {
-    if (W == 1) {
+// ---- one process per GPU (ctmr_peer_*): every front-end call on an attached ctx is collective -------------------------
+// The ranks first agree, through the mailbox, on the number of rounds R, on whether the call computes string identities
+// and on whether every rank's checks passed.  Then every rank runs R rounds of the key exchange over its own chunks (an
+// empty chunk when it has none left, has stopped or has failed), and a last mailbox exchange tells every rank how many
+// ranks stopped at an unknown Chain[0] fingerprint: they resume with another collective call.
+bool peer_call(const ctmr_ctx* c) { return c->peer_mode == PEER_IPC && c->st.peer.world > 1; }
+
+// What the ranks of a collective call agreed on.
+struct PeerCall {
+    bool on = false;
+    uint64_t E = 0;       // entries per rank and round in the index rule: the largest chunk any rank may cut
+    uint64_t rounds = 0;  // R: the most chunks any rank has, at least 1
+    uint64_t span = 0;    // R * world * E: the indices the call takes once agreed
+};
+
+// The agreement word: the rank's chunk count, its E and whether it wants string identities, or that its checks failed.
+constexpr uint64_t kAgreeFailed = 1ull << 63, kAgreeMeta = 1ull << 62;
+constexpr int kAgreeEShift = 40;  // E <= kStageEntries < 2^22 in bits 40..61, the chunk count below 2^40
+static_assert(kStageEntries < (1ull << 22), "agreement word layout");
+
+// One word from every rank through the mailbox.  The second barrier keeps every rank from posting the next word
+// before each rank has read this one.  The row is valid only if no barrier timed out: the caller checks the device.
+int peer_exchange(ctmr_ctx* c, uint64_t mine, uint64_t* row) {
+    CU(c, launch_peer_post(c->pf, mine, c->stream));
+    int rc = peer_barrier(c, CH_MAILBOX, c->stream);
+    if (rc) return rc;
+    CU(c, cudaMemcpyAsync(row, c->pf.flags[c->pf.rank] + (size_t)kPeerChannels * kMaxWorld, kMaxWorld * sizeof(uint64_t),
+                          cudaMemcpyDeviceToHost, c->stream));
+    rc = peer_barrier(c, CH_MAILBOX, c->stream);
+    if (rc) return rc;
+    CU(c, cudaStreamSynchronize(c->stream));
+    return CTMR_OK;
+}
+
+// Posts this rank's part (`mine_rc`: the result of its checks) and reads every rank's.  Returns the rank's own error,
+// CTMR_E_PEER_FAILED when only another rank failed, or CTMR_OK with *pc filled in.
+int peer_agree(ctmr_ctx* c, int mine_rc, uint64_t chunks, uint64_t E, bool meta, PeerCall* pc, bool* meta_out) {
+    const std::string err = c->err;
+    uint64_t row[kMaxWorld] = {};
+    const uint64_t mine = mine_rc ? kAgreeFailed : chunks | E << kAgreeEShift | (meta ? kAgreeMeta : 0);
+    int rc = peer_exchange(c, mine, row);
+    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
+    if (rc) return rc;
+    if (mine_rc) {
+        c->err = err;
+        return mine_rc;
+    }
+    const uint32_t world = c->st.peer.world;
+    for (uint32_t r = 0; r < world; ++r) {
+        if (row[r] & kAgreeFailed) return fail(c, CTMR_E_PEER_FAILED, "rank " + std::to_string(r) + "'s part of this collective call failed before any work");
+        pc->rounds = std::max<uint64_t>(pc->rounds, row[r] & ((1ull << kAgreeEShift) - 1));
+        pc->E = std::max<uint64_t>(pc->E, (row[r] >> kAgreeEShift) & ((1ull << 22) - 1));
+        meta |= (row[r] & kAgreeMeta) != 0;
+    }
+    pc->rounds = std::max<uint64_t>(pc->rounds, 1);  // at least one round: its barriers fence the next call's post
+    pc->span = pc->rounds * world * pc->E;
+    *meta_out = meta;
+    return CTMR_OK;
+}
+
+// the chunks of the whole batch, cut by fit before the agreement exactly as the upload loop cuts them
+template <class Format>
+int count_chunks(ctmr_ctx* c, const Format& fm, uint64_t* chunks) {
+    for (uint64_t pos = 0, hi = 0; pos < fm.units(); pos = hi, ++*chunks) {
+        const int rc = fm.fit(c, pos, ~0ull, &hi);
+        if (rc) return rc;
+        if (hi == pos) return fail(c, CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
+    }
+    return CTMR_OK;
+}
+
+// The path over round k's chunks.  One ctx: ctmr_process_device on the ctx's stream, which overlaps the map and the
+// reduce of a large chunk.  A group, or a rank of a collective call: one round of the key exchange, each member's chunk
+// as its slice.
+int run_path(ctmr_ctx** m, uint32_t W, uint64_t k, Chunk* cur, bool meta, const PeerCall& pc, ctmr_ctx** failed) {
+    if (W == 1 && !pc.on) {
         *failed = m[0];
         return cur[0].db.n ? ctmr_process_device(m[0], &cur[0].db, &cur[0].dout, m[0]->stream) : CTMR_OK;
     }
-    const int parity = k % (int)kParities;
+    const int parity = (int)(k % kParities);
     RoundMember rm[kMaxWorld];
     for (uint32_t r = 0; r < W; ++r) {
         *failed = m[r];
         const int rc = fe_member(m[r], cur[r].db, cur[r].dout, parity, rm[r]);
         if (rc) return rc;
     }
-    return run_round(rm, W, parity, m[0]->fe->cap_entries, meta, failed);
+    return run_round(rm, W, parity, pc.on ? pc.E : m[0]->fe->cap_entries, meta, failed);
 }
 
 // after the path: x509 leaf failures, PEM, outputs to the host; waits for the chunk
@@ -890,84 +970,145 @@ int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
     return CTMR_OK;
 }
 
-// One front-end call on the members m[0..W): one ctx (W == 1), or the members of a group.  The batch's entries take the
-// global indices from *next_index on; tree (one member only): fold the entries into the trees too, written back when the
-// call succeeds or stops.  A stop (tiles) ends the call after the round that meets it.  On error *failed names the member
-// that failed.
+// One front-end call on the members m[0..W): one ctx (W == 1), or the members of a group; on a ctx attached to peers
+// (pc.on) this rank's part of a collective call.  The batch's entries take the global indices from *next_index on;
+// tree (one member only): fold the entries into the trees too, written back when the call succeeds or stops.  A stop
+// (tiles) ends the call after the round that meets it; on a collective call the rank runs its remaining rounds empty,
+// and so does a rank whose front or back half fails.  On error *failed names the member that failed.
 template <class Format>
-int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, const TreeArgs* targs, ctmr_ctx** failed) {
+int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, const TreeArgs* targs, PeerCall& pc,
+                    ctmr_ctx** failed) {
     *failed = m[0];
+    pc.on = W == 1 && peer_call(m[0]);
+    if (pc.on) m[0]->fe_peer_stopped = 0;
     int rc = fm.check(m[0], targs);
-    if (rc) return rc;
+    if (rc && !pc.on) return rc;
     // The entries take their indices once a chunk reaches the path; a call that fails before has changed no table.
     const uint64_t takes = fm.done;
     fm.done = 0;
-    const uint64_t total = fm.units();
+    const uint64_t total = rc ? 0 : fm.units();
     const TreeArgs* tree = targs && targs->n ? targs : nullptr;  // a routed call of no tree folds nothing
-    if (total == 0 && !tree) return CTMR_OK;
-    const ctmr_out* po = &fm.out->path;
-    // everything the call builds on first use, before its first kernel
-    for (uint32_t r = 0; r < W; ++r) {
-        *failed = m[r];
-        rc = fm.prepare(m[r]);
-        if (rc == CTMR_OK && po->pem) rc = pem_ensure(m[r], m[r]->fe->pem, m[r]->fe->cap_entries, m[r]->fe->cap_decoded);
-        if (rc == CTMR_OK && W == 1) rc = ensure_device_path(m[r], m[r]->fe->cap_entries);  // ctmr_process_device
+    if (total == 0 && !tree && !pc.on) return CTMR_OK;
+    const ctmr_out* po = rc ? nullptr : &fm.out->path;
+    // everything the call builds on first use, before its first kernel, and on a collective call its chunks
+    uint64_t chunks = 0;
+    const auto setup = [&]() -> int {
+        for (uint32_t r = 0; r < W; ++r) {
+            *failed = m[r];
+            int rc = fm.prepare(m[r]);
+            const uint64_t E = rc ? 0 : m[r]->fe->cap_entries;
+            if (rc == CTMR_OK && po->pem) rc = pem_ensure(m[r], m[r]->fe->pem, E, m[r]->fe->cap_decoded);
+            if (rc == CTMR_OK && pc.on) rc = ensure_scratch(m[r], E);  // the rounds' scratch (fe_member)
+            if (rc == CTMR_OK && pc.on) rc = ensure_order(m[r], E);
+            if (rc == CTMR_OK && W == 1 && !pc.on) rc = ensure_device_path(m[r], E);  // ctmr_process_device
+            if (rc) return rc;
+        }
+        *failed = m[0];
+        if (tree) {
+            const int rc = tree_begin(m[0], tree, fm.tree_pos);
+            if (rc) return rc;
+        }
+        return pc.on ? count_chunks(m[0], fm, &chunks) : CTMR_OK;
+    };
+    if (rc == CTMR_OK) rc = setup();
+    if (pc.on) {  // every check of every rank is done and no table has changed: the ranks go on together, or all return
+        bool meta = false;
+        // E <= the key-exchange region X: alloc_exchange sizes X to at least the stage size, the front end's entry budget
+        rc = peer_agree(m[0], rc, chunks, rc ? 0 : m[0]->fe->cap_entries, rc ? false : want_meta(po), &pc, &meta);
         if (rc) return rc;
-    }
-    *failed = m[0];
-    if (tree) {
-        rc = tree_begin(m[0], tree, fm.tree_pos);
+        fm.meta = meta;
+    } else {
         if (rc) return rc;
-        if (total == 0) return tree_end(m[0], tree);
+        fm.meta = want_meta(po);
+        if (tree && total == 0) return tree_end(m[0], tree);
     }
+    const uint64_t world = m[0]->st.peer.world, rank = m[0]->st.peer.rank;
     uint64_t pem_base = 0;
     std::vector<Chunk> ch[2];  // round k's chunks in ch[k & 1], uploaded into stage k & 1
     rc = plan_round(m, W, fm, 0, 0, ch[0], failed);
     if (rc) return rc;
     Chunk* cur = nullptr;
-    uint32_t stop = W;  // the member whose chunk holds the stop
-    for (int k = 0;; ++k) {
+    Chunk held;          // the chunk that holds the stop
+    uint32_t stop = W;   // the member whose chunk holds the stop
+    int local = CTMR_OK;  // a collective call: this rank's error after the agreement, returned at the end of the call
+    std::string local_err;
+    const auto fail_locally = [&](int code) {
+        local = code;
+        local_err = m[0]->err;
+    };
+    for (uint64_t k = 0;; ++k) {
         cur = ch[k & 1].data();
         const uint64_t end = cur[W - 1].hi;
-        if (end < total) {  // the next round's uploads overlap this round's kernels and host round trips
-            rc = plan_round(m, W, fm, end, (k + 1) & 1, ch[(k + 1) & 1], failed);
+        const bool idle = stop < W || local;  // a rank that stopped or failed runs its remaining rounds empty
+        const bool last = pc.on ? k + 1 >= pc.rounds : end >= total;
+        if (!last) {  // the next round's uploads overlap this round's kernels and host round trips
+            rc = plan_round(m, W, fm, idle ? total : end, (k + 1) & 1, ch[(k + 1) & 1], failed);
             if (rc) return rc;
         }
+        if (idle) cur[0].cut(0, 0);
         // The front halves wait on the host (issuer identification round trips, the arena size): one thread per member,
         // so that the members' waits overlap instead of adding up.  Each thread touches its own ctx only; the issuer
         // registry they all resolve against is device memory reached with atomics.
         rc = for_each_member(m, W, W > 1, failed, [&](uint32_t r) { return fm.front(m[r], cur[r]); });
-        if (rc) return rc;
+        const bool front_failed = rc != CTMR_OK;
+        if (front_failed) {
+            if (!pc.on) return rc;
+            fail_locally(rc);
+            cur[0].cut(0, 0);
+            cur[0].stopped = false;
+            cur[0].dout = chunk_path_out(m[0]->fe.get(), po, fm.meta);
+        }
         for (uint32_t r = 0; r < W; ++r) {
-            if (stop < W) cur[r].cut(0, 0);  // after a stop in an earlier member: its entries must not touch the tables
-            else if (cur[r].stopped) stop = r;
-            cur[r].db.first_index = *next_index + cur[r].e0;
+            if (stop < W) {
+                cur[r].cut(0, 0);  // after a stop in an earlier member: its entries must not touch the tables
+            } else if (cur[r].stopped) {
+                stop = r;
+                held = cur[r];
+            }
+            cur[r].db.first_index = *next_index + (pc.on ? (k * world + rank) * pc.E : cur[r].e0);
         }
         fm.done = takes;
-        rc = run_path(m, W, k, cur, want_meta(po), failed);
+        rc = run_path(m, W, k, cur, fm.meta, pc, failed);
         if (rc) return rc;
-        // in entry order when there is PEM (the texts are appended in that order); otherwise each member writes its own
-        // ranges of the outputs, and on a group the members' copies and waits overlap
-        rc = for_each_member(m, W, W > 1 && !po->pem, failed, [&](uint32_t r) { return back(m[r], fm, cur[r], &pem_base); });
-        if (rc) return rc;
-        fm.completed(stop < W ? cur[stop].hi : end);
-        if (stop < W || end >= total) break;
+        if (!front_failed) {
+            // in entry order when there is PEM (the texts are appended in that order); otherwise each member writes its
+            // own ranges of the outputs, and on a group the members' copies and waits overlap
+            rc = for_each_member(m, W, W > 1 && !po->pem, failed, [&](uint32_t r) { return back(m[r], fm, cur[r], &pem_base); });
+            if (rc && !pc.on) return rc;
+            if (rc) fail_locally(rc);
+            else if (!idle) fm.completed(stop < W ? held.hi : end);
+        }
+        if (last || (!pc.on && stop < W)) break;
     }
-    if (stop < W) fm.done = cur[stop].e1;
+    if (stop < W) fm.done = held.e1;
     if (po->pem) po->pem_off[fm.done] = pem_base;
-    for (uint32_t r = 0; r < W; ++r) {  // a table that filled up during the completed chunks is this call's error
+    for (uint32_t r = 0; r < W && !local; ++r) {  // a table that filled up during the completed chunks is this call's error
         *failed = m[r];
         rc = ctmr_check_device(m[r], nullptr);
-        if (rc) return rc;
+        if (rc && !pc.on) return rc;
+        if (rc) fail_locally(rc);
     }
     *failed = m[0];
-    if (tree) {  // at a stop the completed tiles are in the tree: the resumed call continues from there
+    if (tree && !local) {  // at a stop the completed tiles are in the tree: the resumed call continues from there
         rc = tree_end(m[0], tree);
+        if (rc && !pc.on) return rc;
+        if (rc) fail_locally(rc);
+    }
+    if (pc.on) {  // every rank learns how many ranks stopped: a resume loop calls again while any did
+        uint64_t row[kMaxWorld] = {};
+        rc = peer_exchange(m[0], stop < W ? 1 : 0, row);
         if (rc) return rc;
+        for (uint32_t r = 0; r < world; ++r) m[0]->fe_peer_stopped += row[r] != 0;
+        rc = ctmr_check_device(m[0], nullptr);  // a barrier that timed out; the count above is then unreliable
+        if (rc && !local) return rc;
+        if (local) {
+            m[0]->err = local_err;
+            return local;
+        }
     }
     if (stop == W) return CTMR_OK;
     *failed = m[stop];
-    return fm.stop(m[stop], cur[stop]);
+    return fm.stop(m[stop], held);
 }
 
 // an upload of the NEXT chunk may still be reading the caller's text and an output copy may still be writing the caller's
@@ -987,8 +1128,9 @@ void drain_frontend(ctmr_ctx* c) {
 template <class Format>
 int front_end_call(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format fm, const TreeArgs* tree, ctmr_group* g) {
     ctmr_ctx* failed = nullptr;
-    const int rc = process_members(m, W, next_index, fm, tree, &failed);
-    *next_index += fm.done;
+    PeerCall pc;  // a collective call takes pc.span indices once the ranks agreed, whatever happens after
+    const int rc = process_members(m, W, next_index, fm, tree, pc, &failed);
+    *next_index += pc.on ? pc.span : fm.done;
     for (uint32_t r = 0; r < W; ++r) {
         if (m[r]->fe && m[r]->fe->tree) {
             m[r]->fe->tree->active = false;
@@ -1069,7 +1211,7 @@ extern "C" {
 
 int ctmr_process_raw(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out) {
     if (!c) return CTMR_E_INVALID;
-    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_raw");
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_raw");
     return front_end_call(&c, 1, &c->next_index, Pages(b, out), nullptr, nullptr);
 }
 
@@ -1080,7 +1222,7 @@ int ctmr_group_process_raw(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out*
 
 int ctmr_process_tiles(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out) {
     if (!c) return CTMR_E_INVALID;
-    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_tiles");
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_tiles");
     return front_end_call(&c, 1, &c->next_index, Tiles(b, out), nullptr, nullptr);
 }
 
@@ -1091,16 +1233,14 @@ int ctmr_group_process_tiles(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_
 
 int ctmr_process_raw_tree(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree) {
     if (!c) return CTMR_E_INVALID;
-    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
-    if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     const TreeArgs t{tree, 1, nullptr, false};
     return front_end_call(&c, 1, &c->next_index, Pages(b, out), &t, nullptr);
 }
 
 int ctmr_process_tiles_tree(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, ctmr_tree* tree) {
     if (!c) return CTMR_E_INVALID;
-    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
-    if (!tree) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     const TreeArgs t{tree, 1, nullptr, false};
     return front_end_call(&c, 1, &c->next_index, Tiles(b, out), &t, nullptr);
 }
@@ -1108,7 +1248,7 @@ int ctmr_process_tiles_tree(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out
 int ctmr_process_raw_trees(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, const uint32_t* entry_log, ctmr_tree* trees,
                            uint32_t n_trees) {
     if (!c) return CTMR_E_INVALID;
-    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     const TreeArgs t{trees, n_trees, entry_log, true};
     return front_end_call(&c, 1, &c->next_index, Pages(b, out), &t, nullptr);
 }
@@ -1116,9 +1256,23 @@ int ctmr_process_raw_trees(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* o
 int ctmr_process_tiles_trees(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out, const uint32_t* tile_log, ctmr_tree* trees,
                              uint32_t n_trees) {
     if (!c) return CTMR_E_INVALID;
-    if (c->group || c->peer_mode != PEER_NONE) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     const TreeArgs t{trees, n_trees, tile_log, true};
     return front_end_call(&c, 1, &c->next_index, Tiles(b, out), &t, nullptr);
+}
+
+int ctmr_next_index(ctmr_ctx* c, uint64_t* next_index) {
+    if (!c) return CTMR_E_INVALID;
+    if (!next_index || c->group) return fail(c, CTMR_E_INVALID, "bad argument (a member of a group has no index of its own)");
+    *next_index = c->next_index;
+    return CTMR_OK;
+}
+
+int ctmr_peer_frontend_stopped(ctmr_ctx* c, uint32_t* ranks) {
+    if (!c) return CTMR_E_INVALID;
+    if (!ranks || !peer_call(c)) return fail(c, CTMR_E_INVALID, "not a ctx attached to peers (ctmr_peer_attach)");
+    *ranks = c->fe_peer_stopped;
+    return CTMR_OK;
 }
 
 int ctmr_tiles_profile_last(ctmr_ctx* c, float* split_ms) {

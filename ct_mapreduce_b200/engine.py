@@ -15,6 +15,7 @@ All arithmetic happens in the CUDA kernels; nothing here parses, hashes or de-du
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import hashlib
 from dataclasses import dataclass
@@ -161,6 +162,8 @@ class TileBatchResult(RawBatchResult):
 class GpuCertDatabase:
     """One ctmr_ctx = one GPU's share of the known-certificate state."""
 
+    _peers = False   # attached to peers in other processes (peer_attach): the front end is collective
+
     def __init__(self, device: int = 0, table_capacity: int = 1 << 22, issuer_cn_filter: bytes | str = b"",
                  log_expired_entries: bool = False, flags: int = 0, max_issuers: int = 0, max_batch_entries: int = 0,
                  max_batch_bytes: int = 0, pair_capacity_log2: int = 0, meta_capacity_log2: int = 0, max_round_entries: int = 0,
@@ -283,12 +286,16 @@ class GpuCertDatabase:
         what GetRawEntries' JSON decode, ct.LogEntryFromLeaf (ct-fetch.go:424,452) and insertCTWorker + Store do.
         With tree= (the log's entries before these), ctmr_process_raw_tree also folds the entries into it: r.tree.
         With trees= (one LogTree per log) and entry_log= (the log of each entry, capi.NO_TREE for none),
-        ctmr_process_raw_trees folds each entry into its log's tree: r.trees."""
-        _tree_args(tree, trees, entry_log, "entry_log")
-        text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else np.ascontiguousarray(text, np.uint8)
-        leaf_off, extra_off = np.ascontiguousarray(leaf_off, np.uint64), np.ascontiguousarray(extra_off, np.uint64)
-        leaf_len, extra_len = np.ascontiguousarray(leaf_len, np.uint32), np.ascontiguousarray(extra_len, np.uint32)
-        n = leaf_off.size
+        ctmr_process_raw_trees folds each entry into its log's tree: r.trees.
+        On a db attached to peers the call is collective; when another rank's tiles stopped (peer_frontend_stopped()),
+        every rank calls again until none is left, this one with an empty batch if it has nothing to add."""
+        with self._peer_refusal():
+            _tree_args(tree, trees, entry_log, "entry_log")
+            text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else np.ascontiguousarray(text, np.uint8)
+            leaf_off, extra_off = np.ascontiguousarray(leaf_off, np.uint64), np.ascontiguousarray(extra_off, np.uint64)
+            leaf_len, extra_len = np.ascontiguousarray(leaf_len, np.uint32), np.ascontiguousarray(extra_len, np.uint32)
+            n = leaf_off.size
+            log = _log_ids(entry_log, n, "entry_log") if trees is not None else None
         r = RawBatchResult(n, want_sha, want_meta)
         p = r.path
         o = capi.RawOut()
@@ -303,7 +310,6 @@ class GpuCertDatabase:
         b = capi.RawBatch(capi.ptr(text), text.size, capi.ptr(leaf_off), capi.ptr(leaf_len), capi.ptr(extra_off), capi.ptr(extra_len),
                           n, now_unix_ns)
         if trees is not None:
-            log = _log_ids(entry_log, n, "entry_log")
             arr = _trees_to_c(trees)
             self._check(self._lib.ctmr_process_raw_trees(self._h, C.byref(b), C.byref(o), capi.ptr(log) if n else None,
                                                          arr if trees else None, len(trees)))
@@ -348,12 +354,17 @@ class GpuCertDatabase:
         log's entries before these; consecutive tiles of that log), ctmr_process_tiles_tree also folds the entries into
         it and every resumed call carries it on: r.tree.  With trees= (one LogTree per log) and tile_log= (the log of each
         tile, capi.NO_TREE for none), ctmr_process_tiles_trees folds each tile into its log's tree: r.trees; a resumed
-        call carries the trees on, and passes as NO_TREE the rest of a log whose fold a bad tile stopped."""
-        _tree_args(tree, trees, tile_log, "tile_log")
-        data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
-        tile_off, tile_index = np.ascontiguousarray(tile_off, np.uint64), np.ascontiguousarray(tile_index, np.uint64)
-        tile_len, tile_width = np.ascontiguousarray(tile_len, np.uint32), np.ascontiguousarray(tile_width, np.uint16)
-        nt = tile_off.size
+        call carries the trees on, and passes as NO_TREE the rest of a log whose fold a bad tile stopped.
+        On a db attached to peers every call is collective: with fetch, this rank keeps calling while any rank stopped
+        (peer_frontend_stopped()), with an empty batch once its own tiles are done or its own call failed."""
+        with self._peer_refusal():
+            _tree_args(tree, trees, tile_log, "tile_log")
+            data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.ascontiguousarray(data, np.uint8)
+            tile_off, tile_index = np.ascontiguousarray(tile_off, np.uint64), np.ascontiguousarray(tile_index, np.uint64)
+            tile_len, tile_width = np.ascontiguousarray(tile_len, np.uint32), np.ascontiguousarray(tile_width, np.uint16)
+            nt = tile_off.size
+            if trees is not None:
+                tlog = _log_ids(tile_log, nt, "tile_log").copy()
         ent = np.zeros(nt + 1, np.int64)
         ent[1:] = np.cumsum(tile_width.astype(np.int64))
         n = int(ent[-1])
@@ -364,7 +375,6 @@ class GpuCertDatabase:
         miss = np.zeros((max(missing_cap, 1), 32), np.uint8)
         ct = tree.to_c() if tree is not None else None
         if trees is not None:
-            tlog = _log_ids(tile_log, nt, "tile_log").copy()
             arr = _trees_to_c(trees)
         t0, pem_base = 0, 0
         while True:
@@ -387,7 +397,7 @@ class GpuCertDatabase:
             o.missing_fp, o.missing_cap = capi.ptr(miss), missing_cap
             b = capi.TileBatch(capi.ptr(data), data.size, capi.ptr(tile_off) + 8 * t0, capi.ptr(tile_len) + 4 * t0,
                                capi.ptr(tile_index) + 8 * t0, capi.ptr(tile_width) + 2 * t0, nt - t0, now_unix_ns)
-            if ct is not None and t0 > 0 and ct.size < 256 * int(tile_index[t0]):
+            if ct is not None and 0 < t0 < nt and ct.size < 256 * int(tile_index[t0]):
                 ct = None  # a bad tile among the completed tiles stopped the fold: r.tree is final, the rest runs plain
             if trees is not None:
                 if t0 > 0:  # a log whose tree stopped below its first tile of the rest: a bad tile stopped its fold
@@ -414,17 +424,24 @@ class GpuCertDatabase:
             r.tiles_done = t0
             r.missing = [miss[k].tobytes() for k in range(o.n_missing)] if rc == capi.E_UNKNOWN_ISSUER else []
             if rc != capi.E_UNKNOWN_ISSUER:
+                if rc and fetch is not None:   # the others' resumed calls wait for this rank too
+                    err = CtmrError(rc, (self._lib.ctmr_last_error(self._h) or b"").decode())
+                    self._join_resumes()
+                    raise err
                 self._check(rc)
-                return r
+                if fetch is None or not self._peers or not self.peer_frontend_stopped():
+                    return r
+                continue   # another rank stopped: this rank joins its resumed call with what it has left (nothing)
             if fetch is None:
                 return r
-            ders = [bytes(d) for d in fetch(r.missing)]
-            # a log that serves the wrong bytes at issuer/<hex> would otherwise stop at this tile for ever
-            got = [hashlib.sha256(d).digest() for d in ders]
-            if set(got) != set(r.missing):
-                raise CtmrError(capi.E_UNKNOWN_ISSUER, "fetch returned certificates whose SHA-256 does not match the missing "
-                                "fingerprints of tile %d" % t0)
-            self.register_chain_certs(*_pack(ders))
+            with self._peer_refusal():   # a rank that gives up here still meets the others' resumed call
+                ders = [bytes(d) for d in fetch(r.missing)]
+                # a log that serves the wrong bytes at issuer/<hex> would otherwise stop at this tile for ever
+                got = [hashlib.sha256(d).digest() for d in ders]
+                if set(got) != set(r.missing):
+                    raise CtmrError(capi.E_UNKNOWN_ISSUER, "fetch returned certificates whose SHA-256 does not match the missing "
+                                    "fingerprints of tile %d" % t0)
+                self.register_chain_certs(*_pack(ders))
 
 
     def tiles_profile_last(self) -> float:
@@ -478,9 +495,42 @@ class GpuCertDatabase:
         return bytes(h)
 
     def peer_attach(self, rank: int, world: int, handles: list):
-        """handles[r] = rank r's peer_export().  Afterwards process_device / store_batch / reset_device are collective."""
+        """handles[r] = rank r's peer_export().  Afterwards process_device / store_batch / reset_device and the front end
+        (store_raw_entries, store_tiles, with or without trees) are collective."""
         buf = (C.c_uint8 * (capi.PEER_HANDLE_BYTES * world)).from_buffer_copy(b"".join(handles))
         self._check(self._lib.ctmr_peer_attach(self._h, rank, world, buf))
+        self._peers = world > 1
+
+    def peer_frontend_stopped(self) -> int:
+        """Ranks that stopped at an unknown Chain[0] fingerprint in the last collective store_raw_entries / store_tiles
+        call: a resume loop calls again on every rank while this is non-zero."""
+        n = C.c_uint32(0)
+        self._check(self._lib.ctmr_peer_frontend_stopped(self._h, C.byref(n)))
+        return n.value
+
+    def next_index(self) -> int:
+        """The global index the next host-buffer or front-end call on this ctx starts at (ctmr_next_index)."""
+        n = C.c_uint64(0)
+        self._check(self._lib.ctmr_next_index(self._h, C.byref(n)))
+        return n.value
+
+    @contextlib.contextmanager
+    def _peer_refusal(self):
+        """On a db attached to peers the front end is collective: a rank that gives up on a call before making it
+        (an argument its binding refuses, a failed fetch) still makes it with no batch, so that the other ranks return
+        CTMR_E_PEER_FAILED instead of waiting at a barrier."""
+        try:
+            yield
+        except Exception:
+            if self._peers:
+                self._lib.ctmr_process_raw(self._h, None, None)
+            raise
+
+    def _join_resumes(self):
+        """A rank whose own collective call failed joins, with an empty batch, the calls that resume other ranks' stops."""
+        while self._peers and self.peer_frontend_stopped():
+            if self._lib.ctmr_process_tiles(self._h, C.byref(capi.TileBatch()), C.byref(capi.TileOut())) != 0:
+                return
 
     def peer_barrier_device(self, stream=None):
         self._check(self._lib.ctmr_peer_barrier_device(self._h, stream))

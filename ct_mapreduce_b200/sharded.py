@@ -77,3 +77,34 @@ def host_batch_order(ns, stage_entries: int):
             lo, hi = min(n, k * stage_entries), min(n, (k + 1) * stage_entries)
             if hi > lo:
                 yield r, lo, hi
+
+
+def frontend_chunks(widths, entry_budget: int):
+    """The chunk sizes (in entries) one rank's front-end call cuts from its batch by the entry budget: units (entries of
+    pages, width 1 each; tiles, their widths) are taken greedily while the chunk stays within `entry_budget` entries.
+    (The character / byte budget of the staging buffers may cut earlier; callers keep batches well inside it.)"""
+    sizes, cur = [], 0
+    for w in widths:
+        w = int(w)
+        if cur and cur + w > entry_budget:
+            sizes.append(cur)
+            cur = 0
+        cur += w
+    if cur:
+        sizes.append(cur)
+    return sizes
+
+
+def frontend_indices(chunks, entry_budget: int, next_index: int = 0):
+    """The global index of every entry of a collective front-end call (ctmr_process_raw / ctmr_process_tiles and their
+    tree forms with peers attached): chunks[r] lists rank r's chunk sizes in entries (frontend_chunks).  Every rank runs
+    R = max(chunk counts) rounds, and entry j of rank r's chunk k takes next_index + (k * world + r) * E + j with E =
+    entry_budget.  Returns ([one uint64 array of indices per rank, in batch order], the call's span R * world * E)."""
+    import numpy as np
+    world = len(chunks)
+    rounds = max(1, max((len(c) for c in chunks), default=0))
+    out = []
+    for r, sizes in enumerate(chunks):
+        parts = [next_index + (k * world + r) * entry_budget + np.arange(s, dtype=np.uint64) for k, s in enumerate(sizes)]
+        out.append(np.concatenate(parts).astype(np.uint64) if parts else np.zeros(0, np.uint64))
+    return out, rounds * world * entry_budget

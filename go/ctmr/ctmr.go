@@ -58,8 +58,9 @@ type Config struct {
 // DB is one ctx (one GPU) or one group (several GPUs of the box behind one handle): the fan-out is
 // inside the library, invisible here (SURVEY.md §8(b)).
 type DB struct {
-	h *C.ctmr_ctx
-	g *C.ctmr_group
+	h    *C.ctmr_ctx
+	g    *C.ctmr_group
+	peer bool // attached to the DBs of other processes (PeerAttach): the batch calls and the front end are collective
 }
 
 func New(c Config) (*DB, error) {
@@ -100,6 +101,78 @@ func New(c Config) (*DB, error) {
 		return nil, fmt.Errorf("ctmr_group_create: %d: %s", int(rc), C.GoString(C.ctmr_group_last_error(nil)))
 	}
 	return db, nil
+}
+
+// PeerExport is the first step of one process per GPU (ctmr_peer_export): every process opens a DB on its own GPU with
+// the same Config and exports a handle for a group of `world` processes.  Carry the handles to every process by any
+// transport (they are plain bytes), then call PeerAttach everywhere.
+func (d *DB) PeerExport(world int) ([]byte, error) {
+	if d.g != nil {
+		return nil, fmt.Errorf("PeerExport: a group DB drives its GPUs itself; open one DB per GPU")
+	}
+	h := make([]byte, C.CTMR_PEER_HANDLE_BYTES)
+	rc := C.ctmr_peer_export(d.h, C.uint32_t(world), (*C.uint8_t)(unsafe.Pointer(&h[0])))
+	return h, d.err(rc, "ctmr_peer_export")
+}
+
+// PeerAttach attaches this DB as rank `rank` to the handles of all `world` processes (handles[r] = rank r's PeerExport).
+// From then on ProcessBatch, ProcessRaw, ProcessTiles and their tree forms are collective: every process makes the same
+// sequence of calls, each with its own batch (an empty one when it has nothing to add).
+func (d *DB) PeerAttach(rank, world int, handles [][]byte) error {
+	if len(handles) != world {
+		return fmt.Errorf("PeerAttach: %d handles for %d ranks", len(handles), world)
+	}
+	all := make([]byte, 0, world*int(C.CTMR_PEER_HANDLE_BYTES))
+	for _, h := range handles {
+		if len(h) != int(C.CTMR_PEER_HANDLE_BYTES) {
+			return fmt.Errorf("PeerAttach: a handle of %d bytes", len(h))
+		}
+		all = append(all, h...)
+	}
+	if err := d.err(C.ctmr_peer_attach(d.h, C.uint32_t(rank), C.uint32_t(world), (*C.uint8_t)(unsafe.Pointer(&all[0]))), "ctmr_peer_attach"); err != nil {
+		return err
+	}
+	d.peer = world > 1
+	return nil
+}
+
+// peerStopped: ranks that stopped at an unknown chain certificate in the last collective front-end call of a peer DB
+// (0 for other DBs)
+func (d *DB) peerStopped() (uint32, error) {
+	if !d.peer {
+		return 0, nil
+	}
+	var n C.uint32_t
+	err := d.err(C.ctmr_peer_frontend_stopped(d.h, &n), "ctmr_peer_frontend_stopped")
+	return uint32(n), err
+}
+
+// peerRefuse: a peer DB that gives up on a front-end call before making it still makes it, with no batch, so that the
+// other ranks return CTMR_E_PEER_FAILED instead of waiting at a barrier.  It returns err.
+func (d *DB) peerRefuse(err error) error {
+	if d.peer {
+		C.ctmr_process_raw(d.h, nil, nil)
+	}
+	return err
+}
+
+// peerJoinResumes: a peer DB whose own call failed joins, with an empty batch, the calls that resume other ranks'
+// stops, then returns err.
+func (d *DB) peerJoinResumes(err error) error {
+	for d.peer {
+		if n, e := d.peerStopped(); e != nil || n == 0 {
+			break
+		}
+		b := (*C.ctmr_tile_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_batch{}))))
+		o := (*C.ctmr_tile_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_out{}))))
+		rc := C.ctmr_process_tiles(d.h, b, o)
+		C.free(unsafe.Pointer(b))
+		C.free(unsafe.Pointer(o))
+		if rc != 0 {
+			break
+		}
+	}
+	return err
 }
 
 func (d *DB) Close() {

@@ -148,14 +148,17 @@ func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree, 
 	if (tree != nil || routed) && d.g != nil {
 		return fmt.Errorf("ProcessRawTree(s): a group has no tree form; use one DB per GPU")
 	}
-	if n == 0 && tree == nil && !routed {
+	if n == 0 && tree == nil && !routed && !d.peer {
 		return nil
 	}
 	b := (*C.ctmr_raw_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_raw_batch{}))))
 	defer C.free(unsafe.Pointer(b))
-	if n == 0 { // the roots of the trees as they stand
+	if n == 0 { // the roots of the trees as they stand; a peer DB's empty part of a collective call
 		if routed {
 			return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, nil, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")
+		}
+		if tree == nil {
+			return d.err(C.ctmr_process_raw(d.h, b, r.raw), "ctmr_process_raw")
 		}
 		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
 	}
@@ -180,7 +183,7 @@ func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree, 
 	}
 	if routed {
 		if len(p.Log) != n {
-			return fmt.Errorf("ProcessRawTrees: %d log ids for %d entries", len(p.Log), n)
+			return d.peerRefuse(fmt.Errorf("ProcessRawTrees: %d log ids for %d entries", len(p.Log), n))
 		}
 		log := (*C.uint32_t)(unsafe.Pointer(&p.Log[0])) // pointer-free Go memory, passed for the call only
 		return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, log, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")

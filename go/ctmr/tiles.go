@@ -138,9 +138,9 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 		return fmt.Errorf("ProcessTilesTree(s): a group has no tree form; use one DB per GPU")
 	}
 	if routed && len(t.Log) != len(t.Off) {
-		return fmt.Errorf("ProcessTilesTrees: %d log ids for %d tiles", len(t.Log), len(t.Off))
+		return d.peerRefuse(fmt.Errorf("ProcessTilesTrees: %d log ids for %d tiles", len(t.Log), len(t.Off)))
 	}
-	if len(t.Off) == 0 {
+	if len(t.Off) == 0 && !d.peer {
 		if tree != nil || routed { // the roots of the trees as they stand
 			b := (*C.ctmr_tile_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_batch{}))))
 			defer C.free(unsafe.Pointer(b))
@@ -157,26 +157,32 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 	}
 	var pin runtime.Pinner
 	defer pin.Unpin()
-	pin.Pin(&t.Off[0])
-	pin.Pin(&t.Len[0])
-	pin.Pin(&t.Index[0])
-	pin.Pin(&t.Width[0])
+	if len(t.Off) > 0 {
+		pin.Pin(&t.Off[0])
+		pin.Pin(&t.Len[0])
+		pin.Pin(&t.Index[0])
+		pin.Pin(&t.Width[0])
+	}
 	b := (*C.ctmr_tile_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_batch{}))))
 	defer C.free(unsafe.Pointer(b))
 	o := (*C.ctmr_tile_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_out{}))))
 	defer C.free(unsafe.Pointer(o))
 	pemBase := uint64(0)
-	for t0, e0 := 0, 0; t0 < len(t.Off); {
+	// A peer DB keeps calling while any rank of the collective call stopped: with nothing left, its part is empty.
+	for t0, e0 := 0, 0; t0 < len(t.Off) || d.peer; {
 		b.data, b.data_bytes = (*C.uint8_t)(t.Data), C.uint64_t(t.Used)
-		b.tile_off = (*C.uint64_t)(unsafe.Pointer(&t.Off[t0]))
-		b.tile_len = (*C.uint32_t)(unsafe.Pointer(&t.Len[t0]))
-		b.tile_index = (*C.uint64_t)(unsafe.Pointer(&t.Index[t0]))
-		b.tile_width = (*C.uint16_t)(unsafe.Pointer(&t.Width[t0]))
+		b.tile_off, b.tile_len, b.tile_index, b.tile_width = nil, nil, nil, nil
+		if t0 < len(t.Off) {
+			b.tile_off = (*C.uint64_t)(unsafe.Pointer(&t.Off[t0]))
+			b.tile_len = (*C.uint32_t)(unsafe.Pointer(&t.Len[t0]))
+			b.tile_index = (*C.uint64_t)(unsafe.Pointer(&t.Index[t0]))
+			b.tile_width = (*C.uint16_t)(unsafe.Pointer(&t.Width[t0]))
+		}
 		b.n_tiles, b.now_unix_ns = C.uint64_t(len(t.Off)-t0), C.int64_t(nowUnixNs)
 		*o = *r.out
 		shiftTileOut(o, e0, t0, pemBase) // a resumed call writes from entry e0, tile t0 and PEM byte pemBase on
 		// a bad tile among the tiles completed before a stop ended the fold: the tree is final, the rest runs plain
-		fold := tree != nil && (t0 == 0 || tree.Size >= 256*t.Index[t0])
+		fold := tree != nil && (t0 == 0 || t0 == len(t.Off) || tree.Size >= 256*t.Index[t0])
 		if routed && t0 > 0 { // a log whose tree stopped below its first remaining tile: a bad tile ended its fold
 			stopped := map[uint32]bool{}
 			for k := t0; k < len(log); k++ {
@@ -194,7 +200,11 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 		if d.g != nil {
 			rc = C.ctmr_group_process_tiles(d.g, b, o)
 		} else if routed {
-			rc = C.ctmr_process_tiles_trees(d.h, b, o, (*C.uint32_t)(unsafe.Pointer(&log[t0])), treesC(trees), C.uint32_t(len(trees)))
+			var lp *C.uint32_t
+			if t0 < len(log) {
+				lp = (*C.uint32_t)(unsafe.Pointer(&log[t0]))
+			}
+			rc = C.ctmr_process_tiles_trees(d.h, b, o, lp, treesC(trees), C.uint32_t(len(trees)))
 		} else if fold {
 			rc = C.ctmr_process_tiles_tree(d.h, b, o, tree.c())
 		} else {
@@ -213,7 +223,17 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 		}
 		t0, e0 = t0+done, e1
 		if rc != C.CTMR_E_UNKNOWN_ISSUER {
-			return d.err(rc, "ctmr_process_tiles")
+			if err := d.err(rc, "ctmr_process_tiles"); err != nil {
+				if fetch != nil { // the others' resumed calls wait for this rank too
+					return d.peerJoinResumes(err)
+				}
+				return err
+			}
+			// a peer DB whose part is done: another rank stopped, so it joins that rank's resumed call
+			if stopped, err := d.peerStopped(); err != nil || stopped == 0 || fetch == nil {
+				return err
+			}
+			continue
 		}
 		if fetch == nil {
 			return fmt.Errorf("ctmr_process_tiles: tile %d names an unregistered chain certificate", t0)
@@ -225,16 +245,16 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 			copy(fp[:], missing[32*k:])
 			der, err := fetch(fp)
 			if err != nil {
-				return err
+				return d.peerRefuse(err) // a peer DB that gives up still meets the others' resumed call
 			}
 			// a log serving the wrong bytes at issuer/<hex> would otherwise stop the loop at this tile for ever
 			if sha256.Sum256(der) != fp {
-				return fmt.Errorf("ctmr_process_tiles: the certificate fetched for fingerprint %x has another SHA-256", fp)
+				return d.peerRefuse(fmt.Errorf("ctmr_process_tiles: the certificate fetched for fingerprint %x has another SHA-256", fp))
 			}
 			ders = append(ders, der)
 		}
 		if _, err := d.RegisterChainCerts(ders); err != nil {
-			return err
+			return d.peerRefuse(err)
 		}
 	}
 	return nil

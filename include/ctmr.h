@@ -55,7 +55,8 @@ enum {
     CTMR_E_META_TABLE_FULL = -9,  /* IssuerMetadata string-identity table exhausted: raise config.meta_capacity_log2 */
     CTMR_E_PEER_TIMEOUT = -10,    /* a rank of the group did not reach a barrier (a peer failed or the calls diverged) */
     CTMR_E_PEER = -11,            /* peer access / CUDA IPC between the GPUs of a group is not available */
-    CTMR_E_UNKNOWN_ISSUER = -12   /* ctmr_process_tiles: a Chain[0] fingerprint is not registered (ctmr_frontend.h) */
+    CTMR_E_UNKNOWN_ISSUER = -12,  /* ctmr_process_tiles: a Chain[0] fingerprint is not registered (ctmr_frontend.h) */
+    CTMR_E_PEER_FAILED = -13      /* another rank's part of this collective call failed before any work (ctmr_frontend.h) */
 };
 
 /* ---- per-entry status -------------------------------------------------------------------- */
@@ -299,8 +300,10 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the
  * launcher offers (torch.distributed all_gather in this repository) and attaches them.  From then on
- * ctmr_process_device, ctmr_process_batch, ctmr_reset_device and ctmr_peer_* are COLLECTIVE: every rank must make
- * the same sequence of calls.  Inside them the ranks meet at barriers kept in peer memory (no host round trip, no
+ * ctmr_process_device, ctmr_process_batch, ctmr_reset_device, ctmr_peer_* and the six front-end calls of
+ * ctmr_frontend.h (ctmr_process_raw, ctmr_process_tiles and their _tree / _trees forms; their contract is stated
+ * there) are COLLECTIVE: every rank must make the same sequence of calls; any front-end call matches any other.
+ * Inside them the ranks meet at barriers kept in peer memory (no host round trip, no
  * NCCL on the data path); the global index of entry j of rank r's round k is first_index + (k * world + r) * E + j,
  * i.e. the result equals the sequential run over the rounds in rank order.  E = entries per rank and round: the host
  * pipeline's stage size for ctmr_process_batch; for ctmr_process_device (every rank passes the same n, R =
@@ -309,6 +312,11 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
 /* allocates this rank's key-exchange area for a group of `world` ranks and exports it together with the tables */
 int ctmr_peer_export(ctmr_ctx* ctx, uint32_t world, uint8_t handle_out[CTMR_PEER_HANDLE_BYTES]);
 int ctmr_peer_attach(ctmr_ctx* ctx, uint32_t rank, uint32_t world, const uint8_t* handles /* [world][CTMR_PEER_HANDLE_BYTES] */);
+/* *next_index = the global index the next ctmr_process_batch or front-end call on this ctx starts at: what the earlier
+ * calls used up, on a ctx of a multi-process group by the collective rules.  A ctmr_process_device call whose entries
+ * must follow them passes first_index >= this.  CTMR_E_INVALID for a member of an in-process group (the group holds the
+ * index). */
+int ctmr_next_index(ctmr_ctx* ctx, uint64_t* next_index);
 /* barrier over the group on `stream` (device side; returns immediately) */
 int ctmr_peer_barrier_device(ctmr_ctx* ctx, void* stream);
 /* all-reduce(sum) of [per-issuer unique counts || status counters] over peer memory, bracketed by barriers: the

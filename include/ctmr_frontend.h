@@ -251,6 +251,58 @@ int ctmr_process_raw_trees(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_
 int ctmr_process_tiles_trees(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_tile_out* out,
                              const uint32_t* tile_log /* [n_tiles] */, ctmr_tree* trees, uint32_t n_trees);
 
+/* ---- one process per GPU: the front end as a collective call ------------------------------------------------------------
+ * On a ctx attached to peers (ctmr_peer_attach, ctmr.h, world > 1) ctmr_process_raw, ctmr_process_tiles,
+ * ctmr_process_raw_tree, ctmr_process_tiles_tree, ctmr_process_raw_trees and ctmr_process_tiles_trees are COLLECTIVE.
+ * Each rank passes its own batch, and each front-end call on one rank must meet a front-end call on every other rank.
+ * The entry points may differ between the ranks of one call (pages on one rank, tiles with trees on another): their
+ * collective steps are the same.  A front-end call met by ctmr_process_batch, ctmr_process_device or any other
+ * collective call on another rank is undefined, as is any other mismatch of the collective sequence.
+ *
+ * Agreement.  Each rank checks its arguments (the rules of its entry point, trees included), builds what the call
+ * needs and cuts its whole batch into chunks exactly as on one GPU, E entries at most per chunk, before any upload:
+ * bad spans, widths or tree rules are CTMR_E_INVALID and an entry or tile beyond the staging budget is
+ * CTMR_E_BATCH_TOO_LARGE at this point.  E is the front end's entry budget (config.max_batch_entries), which the
+ * key-exchange regions always hold; when ranks were created with different budgets the largest is used in the index
+ * rule.  The ranks then exchange, through peer memory, their chunk counts, whether they want the string identities
+ * (first_issuer_dn / first_crldp) and whether their checks failed.  If any rank's checks failed, every rank returns
+ * before any index is taken or any table or tree changes: that rank with its own error, the others with
+ * CTMR_E_PEER_FAILED.  So an argument mistake that the library sees on one rank -- a NULL batch, output or tree
+ * included -- never leaves the others waiting at a barrier.  A rank that skips the call, for instance because its own
+ * code refused the arguments before calling, does: such a rank still makes the call (a NULL batch will do), so that
+ * the others return CTMR_E_PEER_FAILED.
+ *
+ * Rounds and indices.  Otherwise every rank runs R = the largest chunk count (at least 1) rounds of the key exchange;
+ * a rank that has run out of chunks runs its remaining rounds empty.  Entry j of rank r's chunk in round k takes the
+ * global index next_index + (k * world + r) * E + j, the rule of the collective ctmr_process_batch, so the result
+ * equals the sequential run over the rounds, inside a round the ranks in order.  Every rank advances its next index by
+ * R * world * E once the agreement has succeeded, whatever happens after, and by nothing when it failed
+ * (ctmr_next_index reads it, e.g. to place a later ctmr_process_device call's first_index).  When any rank
+ * wants the string identities every rank computes them (its entries then count for the first-seen rules) and
+ * returns them where its caller asked.
+ *
+ * Stops and failures after the agreement.  A tiles stop at an unknown Chain[0] fingerprint ends the rank's part at the
+ * stop tile, as on one GPU (tiles_done, missing_fp, CTMR_E_UNKNOWN_ISSUER); the rank runs its remaining rounds empty.
+ * A front or back half that fails with a library error does the same and returns that error at the end of the call:
+ * CTMR_E_TOO_MANY_ISSUERS (the issuer registry or the Chain[0] mirror is full), CTMR_E_BATCH_TOO_LARGE (pem_cap too
+ * small), and a table that filled up (CTMR_E_TABLE_FULL, CTMR_E_PAIR_TABLE_FULL, CTMR_E_META_TABLE_FULL).  A CUDA error
+ * (CTMR_E_CUDA, CTMR_E_NOMEM of a device allocation) that leaves the GPU unable to run the remaining barriers ends the
+ * rank's part at once, and the other ranks wait until CTMR_E_PEER_TIMEOUT, as in every collective call.
+ *
+ * Resume.  The call ends with one more exchange, so that every rank knows how many ranks stopped at an unknown
+ * fingerprint: ctmr_peer_frontend_stopped.  A resume loop keeps calling on every rank while it is non-zero; a rank with
+ * nothing left passes an empty batch.  A rank whose own call failed is not counted (it has nothing to resume), but
+ * while the count is non-zero the others call again, so it joins those calls with an empty batch before it gives up.
+ *
+ * Trees.  Each rank folds its own batch's entries into its own caller-held trees, with the one-GPU rules: log order is
+ * batch order on that rank, and global indices do not enter the tree.  Members of an in-process group (ctmr_group_*)
+ * keep refusing the tree forms. */
+
+/* *ranks = the ranks that stopped at an unknown Chain[0] fingerprint (CTMR_E_UNKNOWN_ISSUER) in the last collective
+ * front-end call on this ctx; 0 after a call that failed before any work.  CTMR_E_INVALID on a ctx not attached to
+ * peers. */
+int ctmr_peer_frontend_stopped(ctmr_ctx* ctx, uint32_t* ranks);
+
 #ifdef __cplusplus
 }
 #endif

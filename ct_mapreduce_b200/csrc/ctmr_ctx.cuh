@@ -189,7 +189,9 @@ struct TileState {
 };
 
 // the logs' Merkle trees (ctmr_process_*_tree, ctmr_process_*_trees): the call's trees on the device and the scratch of
-// the fold.  Allocated on the first tree call, for cap_trees trees; a call with more trees builds it again, larger.
+// the fold.  Allocated on the first tree call, for cap_trees trees; a call with more trees builds it again, larger.  On
+// a group (ctmr_group_process_*_tree(s)) member 0 holds the trees; every other member folds its chunks into ranges, and
+// member 0 receives and merges them.
 struct TreeState {
     uint32_t cap_trees = 0;
     DevBuf<TreeDev> dev;          // [cap_trees] the trees for the whole call: uploaded at its start, read back at its end
@@ -200,12 +202,22 @@ struct TreeState {
     HostBuf<uint32_t> h_order[2];
     DevBuf<uint8_t> leaf;         // [cap_entries][32] get-entries leaf hashes of a chunk
     DevBuf<uint8_t> lvl[2];       // [cap_entries / 2 + 2 * cap_trees][32] each: ping-pong level buffers
+    // a group's members 1..: per upload stage, the ranges of that stage's chunk, and the range fold's missing-leaf words
+    DevBuf<TreeRange> range[2];             // [cap_trees] each
+    DevBuf<unsigned long long> range_miss;  // [cap_trees]
+    // a group's member 0: the other members' ranges of a round, and events around the merge (timed)
+    DevBuf<TreeRange> recv;                 // [recv_members][cap_trees]
+    uint32_t recv_members = 0;
+    Event merge0, merge1;
     // the call
     uint32_t n_trees = 0;
     const uint32_t* log = nullptr;  // the tree of each entry (pages) or tile (tiles); NULL: everything goes to tree 0
     std::vector<uint64_t> next;     // [n_trees] log position of each tree's next entry to be uploaded
+    std::vector<uint64_t> start;    // [n_trees] each tree's size at the start of the call
     std::vector<uint32_t> count;    // [n_trees] scratch of the grouping
     bool active = false;            // a tree call is running: the chunks fold their leaves
+    bool ranges = false;            // this ctx folds its chunks into ranges (a group's member 1..)
+    bool merge_timed = false;       // merge0 / merge1 hold a merge whose time is not in fe_ms yet
 };
 
 // CT wire-format front end (include/ctmr_frontend.h): device buffers of one chunk + the device mirror of

@@ -117,10 +117,11 @@ int tree_route_args(ctmr_ctx* c, const TreeArgs* t, uint64_t units) {
     return CTMR_OK;
 }
 
-// the tree state for n trees, built whole (a smaller one is released first)
-int tree_ensure(ctmr_ctx* c, uint32_t n) {
+// the tree state for n trees, built whole (a smaller one is released first); `ranges`: with the range buffers of a
+// group's member 1..; `recv_members`: with member 0's room for that many members' ranges
+int tree_ensure(ctmr_ctx* c, uint32_t n, bool ranges, uint32_t recv_members) {
     FrontEnd* f = c->fe.get();
-    if (f->tree && f->tree->cap_trees >= n) return CTMR_OK;
+    if (f->tree && f->tree->cap_trees >= n && (!ranges || f->tree->range_miss) && f->tree->recv_members >= recv_members) return CTMR_OK;
     f->tree.reset();
     std::unique_ptr<TreeState> tr(new (std::nothrow) TreeState());
     if (!tr) return fail(c, CTMR_E_NOMEM, "host allocation failed");
@@ -136,19 +137,32 @@ int tree_ensure(ctmr_ctx* c, uint32_t n) {
     }
     CU(c, alloc(tr->leaf, E * 32));
     for (DevBuf<uint8_t>& lvl : tr->lvl) CU(c, alloc(lvl, (E / 2 + 2ull * cap) * 32));
+    if (ranges) {
+        for (DevBuf<TreeRange>& r : tr->range) CU(c, alloc(r, cap));
+        CU(c, alloc(tr->range_miss, cap));
+    }
+    if (recv_members) {
+        CU(c, alloc(tr->recv, (uint64_t)recv_members * cap));
+        CU(c, create(tr->merge0, cudaEventDefault));
+        CU(c, create(tr->merge1, cudaEventDefault));
+    }
+    tr->recv_members = recv_members;
     tr->cap_trees = cap;
     f->tree = std::move(tr);
     return CTMR_OK;
 }
 
-// the caller's trees to the device for the whole call; next[d]: log position of tree d's first entry in the call
-int tree_begin(ctmr_ctx* c, const TreeArgs* t, const std::vector<uint64_t>& next) {
-    int rc = tree_ensure(c, t->n);
+// The caller's trees to the device of member 0 (c) for the whole call, with room for the ranges of `others` more
+// members; next[d]: log position of tree d's first entry in the call
+int tree_begin(ctmr_ctx* c, const TreeArgs* t, const std::vector<uint64_t>& next, uint32_t others) {
+    int rc = tree_ensure(c, t->n, false, others);
     if (rc) return rc;
     TreeState* tr = c->fe->tree.get();
+    tr->start.resize(t->n);
     for (uint32_t d = 0; d < t->n; ++d) {
         std::memcpy(&tr->host[d].t, &t->trees[d], sizeof(ctmr_tree));
         tr->host[d].missing = ~0ull;
+        tr->start[d] = t->trees[d].size;
     }
     CU(c, cudaMemcpyAsync(tr->dev, tr->host, t->n * sizeof(TreeDev), cudaMemcpyHostToDevice, c->stream));
     tr->n_trees = t->n;
@@ -156,44 +170,56 @@ int tree_begin(ctmr_ctx* c, const TreeArgs* t, const std::vector<uint64_t>& next
     tr->next = next;
     tr->count.assign(t->n, 0);
     tr->active = true;
+    tr->ranges = false;
+    tr->merge_timed = false;
     return CTMR_OK;
 }
 
-bool tree_active(const FrontEnd* f) { return f->tree && f->tree->active; }
+// a group's member 1.. (c) of a call of n trees: range buffers, and the missing-leaf words at ~0
+int tree_begin_ranges(ctmr_ctx* c, uint32_t n) {
+    int rc = tree_ensure(c, n, true, 0);
+    if (rc) return rc;
+    TreeState* tr = c->fe->tree.get();
+    CU(c, cudaMemsetAsync(tr->range_miss, 0xFF, tr->cap_trees * sizeof(unsigned long long), c->stream));
+    tr->ranges = true;
+    return CTMR_OK;
+}
 
 // Groups the entries of units [ch.lo, ch.hi) by tree (unit u holds width(u) entries) into ch.fold, each tree's entries
-// taking its next log positions, and uploads their order into the chunk's stage on the copy stream unless it is the
-// identity (one tree and no entry of none).
+// taking its next log positions from the call's tree state `home` (member 0's: every member's upload reads and advances
+// it, in member order), and uploads their order into the stage of c's chunk on the copy stream unless it is the identity
+// (one tree and no entry of none).
 template <class Width>
-int tree_group(ctmr_ctx* c, Chunk& ch, Width width) {
+int tree_group(ctmr_ctx* c, TreeState* home, Chunk& ch, Width width) {
     ch.fold.clear();
     ch.ordered = false;
     ch.listed = 0;
-    if (!tree_active(c->fe.get())) return CTMR_OK;
-    TreeState* tr = c->fe->tree.get();
-    std::vector<uint32_t>& cnt = tr->count;
+    if (!home || !home->active) return CTMR_OK;
+    std::vector<uint32_t>& cnt = home->count;
     std::fill(cnt.begin(), cnt.end(), 0u);
     uint64_t none = 0;
     for (uint64_t u = ch.lo; u < ch.hi; ++u) {
-        const uint32_t l = tr->log ? tr->log[u] : 0;
+        const uint32_t l = home->log ? home->log[u] : 0;
         if (l == CTMR_NO_TREE) none += width(u);
         else cnt[l] += width(u);
     }
     uint32_t off = 0;
-    for (uint32_t d = 0; d < tr->n_trees; ++d) {
+    for (uint32_t d = 0; d < home->n_trees; ++d) {
         if (!cnt[d]) continue;
-        ch.fold.push_back(FoldTree{tr->next[d], d, off, cnt[d], 0});
-        tr->next[d] += cnt[d];
+        const uint64_t first = home->next[d], skip = home->start[d] > first ? home->start[d] - first : 0;  // <= 256
+        ch.fold.push_back(FoldTree{first, d, off, cnt[d], (uint32_t)skip});
+        home->next[d] += cnt[d];
         off += cnt[d];
     }
     ch.listed = off;
     ch.ordered = none || ch.fold.size() > 1;
     if (!ch.ordered || !off) return CTMR_OK;
     for (const FoldTree& t : ch.fold) cnt[t.tree] = t.off;  // from here on: each tree's next slot in the order
+    TreeState* tr = c->fe->tree.get();
     uint32_t* h = tr->h_order[ch.stage];
     uint32_t e = 0;
     for (uint64_t u = ch.lo; u < ch.hi; ++u) {
-        const uint32_t l = tr->log ? tr->log[u] : 0, w = width(u);
+        const uint32_t l = home->log ? home->log[u] : 0, w = width(u);
         if (l != CTMR_NO_TREE)
             for (uint32_t k = 0; k < w; ++k) h[cnt[l]++] = e + k;
         e += w;
@@ -202,15 +228,14 @@ int tree_group(ctmr_ctx* c, Chunk& ch, Width width) {
     return CTMR_OK;
 }
 
-// a chunk cut to units [ch.lo, ch.hi) (tiles, at a stop) folds only their entries: each tree keeps the head of its run
+// a chunk cut to units [ch.lo, ch.hi) (tiles, at a stop) folds only their entries: each tree keeps the head of its run.
+// The members' front halves run on threads of their own, so the counts are not home->count.
 template <class Width>
-void tree_cut(ctmr_ctx* c, Chunk& ch, Width width) {
+void tree_cut(const TreeState* home, Chunk& ch, Width width) {
     if (ch.fold.empty()) return;
-    TreeState* tr = c->fe->tree.get();
-    std::vector<uint32_t>& cnt = tr->count;
-    std::fill(cnt.begin(), cnt.end(), 0u);
+    std::vector<uint32_t> cnt(home->n_trees, 0u);
     for (uint64_t u = ch.lo; u < ch.hi; ++u) {
-        const uint32_t l = tr->log ? tr->log[u] : 0;
+        const uint32_t l = home->log ? home->log[u] : 0;
         if (l != CTMR_NO_TREE) cnt[l] += width(u);
     }
     std::vector<FoldTree> kept;
@@ -219,18 +244,60 @@ void tree_cut(ctmr_ctx* c, Chunk& ch, Width width) {
     ch.fold.swap(kept);
 }
 
-// folds a chunk's leaves into its trees (see FoldChunk)
+// folds a chunk's leaves into its trees (see FoldChunk), or on a group's member 1.. into its ranges of the chunk's stage
 int tree_fold(ctmr_ctx* c, const Chunk& ch, const uint8_t* leaves, const uint8_t* flags, uint32_t stride, uint32_t match) {
     if (ch.fold.empty()) return CTMR_OK;
     TreeState* tr = c->fe->tree.get();
     const uint32_t n = (uint32_t)ch.fold.size();
     std::memcpy(tr->h_desc, ch.fold.data(), n * sizeof(FoldTree));
     CU(c, cudaMemcpyAsync(tr->desc, tr->h_desc, n * sizeof(FoldTree), cudaMemcpyHostToDevice, c->stream));
-    const FoldChunk fc{tr->dev, tr->desc, n, stride, ch.ordered ? tr->order[ch.stage].get() : nullptr, ch.listed, leaves, flags, match};
+    const FoldChunk fc{tr->ranges ? nullptr : tr->dev.get(), tr->desc, n, stride, ch.ordered ? tr->order[ch.stage].get() : nullptr,
+                       ch.listed, leaves, flags, match};
     uint8_t* const lvl[2] = {tr->lvl[0], tr->lvl[1]};
     uint32_t launches = 0;
-    CU(c, launch_tree_fold(fc, ch.fold.data(), lvl, c->stream, &launches));
+    if (tr->ranges) CU(c, launch_range_fold(fc, ch.fold.data(), lvl, tr->range[ch.stage], tr->range_miss, c->stream, &launches));
+    else CU(c, launch_tree_fold(fc, ch.fold.data(), lvl, c->stream, &launches));
     c->fe->launches += launches;
+    return CTMR_OK;
+}
+
+// the last merge's time into member 0's fe_ms, once member 0's stream has passed it
+int tree_merge_time(ctmr_ctx* c) {
+    TreeState* tr = c->fe->tree.get();
+    if (!tr->merge_timed) return CTMR_OK;
+    float ms = 0.f;
+    CU(c, cudaEventElapsedTime(&ms, tr->merge0, tr->merge1));
+    c->fe->fe_ms += ms;
+    tr->merge_timed = false;
+    return CTMR_OK;
+}
+
+// A group's round: the ranges of members 1..upto-1 (members after a stop are left out) appended to the trees on member
+// 0, on its stream, in one launch.  Issued after the round's back halves, so before member 0's next front half, which
+// folds the next entries of each tree.  Each copy reads the member's ranges of this round's stage.  The member's range
+// fold of the next round writes the other stage's, and the one after that is issued only once the next round's back
+// half on member 0 has synchronized member 0's stream, which is past this copy.
+int tree_merge(ctmr_ctx** m, uint32_t upto, const Chunk* cur, ctmr_ctx** failed) {
+    ctmr_ctx* h = m[0];
+    *failed = h;
+    TreeState* tr = h->fe->tree.get();
+    if (upto < 2 || tr->n_trees == 0) return CTMR_OK;
+    CU(h, cudaSetDevice(h->device));
+    int rc = tree_merge_time(h);  // the previous round's: member 0's stream was synchronized since
+    if (rc) return rc;
+    RangeSet set{tr->recv, tr->cap_trees, upto - 1, {}};
+    for (uint32_t r = 1; r < upto; ++r) CU(h, cudaStreamWaitEvent(h->stream, m[r]->fe->ev1, 0));  // after the range fold
+    CU(h, cudaEventRecord(tr->merge0, h->stream));
+    for (uint32_t r = 1; r < upto; ++r) {
+        const uint32_t n = set.n[r - 1] = (uint32_t)cur[r].fold.size();
+        if (n)
+            CU(h, cudaMemcpyPeerAsync(tr->recv + (uint64_t)(r - 1) * tr->cap_trees, h->device, m[r]->fe->tree->range[cur[r].stage],
+                                      m[r]->device, n * sizeof(TreeRange), h->stream));
+    }
+    CU(h, launch_tree_merge(tr->dev, tr->n_trees, set, h->stream));
+    CU(h, cudaEventRecord(tr->merge1, h->stream));
+    ++h->fe->launches;
+    tr->merge_timed = true;
     return CTMR_OK;
 }
 
@@ -240,6 +307,8 @@ int tree_end(ctmr_ctx* c, const TreeArgs* t) {
     CU(c, launch_tree_root(tr->dev, t->n, c->stream));
     CU(c, cudaMemcpyAsync(tr->host, tr->dev, t->n * sizeof(TreeDev), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
+    const int rc = tree_merge_time(c);
+    if (rc) return rc;
     for (uint32_t d = 0; d < t->n; ++d) std::memcpy(&t->trees[d], &tr->host[d].t, sizeof(ctmr_tree));
     return CTMR_OK;
 }
@@ -257,6 +326,7 @@ struct Pages {
     bool meta = false;  // the call computes string identities (process_members)
 
     std::vector<uint64_t> tree_pos;  // tree calls: log position of each tree's first entry
+    TreeState* tree_state = nullptr;  // tree calls: the call's tree state, member 0's (process_members)
 
     Pages(const ctmr_raw_batch* b_, ctmr_raw_out* out_) : b(b_), out(out_), done(b_ ? b_->n : 0) {}
     int check(ctmr_ctx* c, const TreeArgs* tree);
@@ -330,7 +400,7 @@ int Pages::upload(ctmr_ctx* c, Chunk& ch) const {
         CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
         return CTMR_OK;
     }
-    const int rc = tree_group(c, ch, [](uint64_t) { return 1u; });
+    const int rc = tree_group(c, tree_state, ch, [](uint64_t) { return 1u; });
     if (rc) return rc;
     uint64_t chars = 0, min_off = ~0ull, max_end = 0;
     for (uint64_t i = lo; i < ch.hi; ++i) {
@@ -491,6 +561,7 @@ struct Tiles {
     bool meta = false;         // the call computes string identities (process_members)
     std::vector<uint64_t> ent;  // entries before each tile: ent[t] = sum of widths of tiles [0, t)
     std::vector<uint64_t> tree_pos;  // tree calls: log position of each tree's first entry (its first tile's)
+    TreeState* tree_state = nullptr;  // tree calls: the call's tree state, member 0's (process_members)
 
     Tiles(const ctmr_tile_batch* b_, ctmr_tile_out* out_) : b(b_), out(out_) {}
     int check(ctmr_ctx* c, const TreeArgs* tree);
@@ -624,7 +695,7 @@ int Tiles::upload(ctmr_ctx* c, Chunk& ch) const {
     if (ch.bytes)
         CU(c, cudaMemcpyAsync(st.text + 16, one_copy ? b->data + min_off : st.pack.data(), ch.bytes, cudaMemcpyHostToDevice, f->copy_stream));
     if (cnt) CU(c, cudaMemcpyAsync(tl->tiles[ch.stage], h, cnt * sizeof(TileDesc), cudaMemcpyHostToDevice, f->copy_stream));
-    const int rc = tree_group(c, ch, [this](uint64_t t) { return (uint32_t)b->tile_width[t]; });
+    const int rc = tree_group(c, tree_state, ch, [this](uint64_t t) { return (uint32_t)b->tile_width[t]; });
     if (rc) return rc;
     CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
     return CTMR_OK;
@@ -693,7 +764,7 @@ int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
             ch.missing.erase(std::unique(ch.missing.begin(), ch.missing.end()), ch.missing.end());
             ch.stopped = true;
             ch.cut(stop, td.first);
-            tree_cut(c, ch, [this](uint64_t t) { return (uint32_t)b->tile_width[t]; });
+            tree_cut(tree_state, ch, [this](uint64_t t) { return (uint32_t)b->tile_width[t]; });
         }
         {  // the completed tiles' leaves into their trees; a bad tile has none
             const int rc = tree_fold(c, ch, tl->leaf_hash, f->entry_status, 1, CTMR_FE_BAD_TILE);
@@ -972,7 +1043,9 @@ int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
 
 // One front-end call on the members m[0..W): one ctx (W == 1), or the members of a group; on a ctx attached to peers
 // (pc.on) this rank's part of a collective call.  The batch's entries take the global indices from *next_index on;
-// tree (one member only): fold the entries into the trees too, written back when the call succeeds or stops.  A stop
+// tree: fold the entries into the trees too, written back when the call succeeds or stops (on a group member 0 holds
+// the trees and folds its chunks into them; the others fold theirs into ranges, merged into the trees after each
+// round's back halves, tree_merge).  A stop
 // (tiles) ends the call after the round that meets it; on a collective call the rank runs its remaining rounds empty,
 // and so does a rank whose front or back half fails.  On error *failed names the member that failed.
 template <class Format>
@@ -1001,12 +1074,14 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
             if (rc == CTMR_OK && pc.on) rc = ensure_scratch(m[r], E);  // the rounds' scratch (fe_member)
             if (rc == CTMR_OK && pc.on) rc = ensure_order(m[r], E);
             if (rc == CTMR_OK && W == 1 && !pc.on) rc = ensure_device_path(m[r], E);  // ctmr_process_device
+            if (rc == CTMR_OK && tree && r > 0) rc = tree_begin_ranges(m[r], tree->n);
             if (rc) return rc;
         }
         *failed = m[0];
         if (tree) {
-            const int rc = tree_begin(m[0], tree, fm.tree_pos);
+            const int rc = tree_begin(m[0], tree, fm.tree_pos, W - 1);
             if (rc) return rc;
+            fm.tree_state = m[0]->fe->tree.get();
         }
         return pc.on ? count_chunks(m[0], fm, &chunks) : CTMR_OK;
     };
@@ -1077,6 +1152,10 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
             if (rc && !pc.on) return rc;
             if (rc) fail_locally(rc);
             else if (!idle) fm.completed(stop < W ? held.hi : end);
+        }
+        if (tree && W > 1) {  // the other members' ranges into the trees, up to the member that stopped
+            rc = tree_merge(m, stop < W ? stop + 1 : W, cur, failed);
+            if (rc) return rc;
         }
         if (last || (!pc.on && stop < W)) break;
     }
@@ -1259,6 +1338,32 @@ int ctmr_process_tiles_trees(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_ou
     if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
     const TreeArgs t{trees, n_trees, tile_log, true};
     return front_end_call(&c, 1, &c->next_index, Tiles(b, out), &t, nullptr);
+}
+
+int ctmr_group_process_raw_tree(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const TreeArgs t{tree, 1, nullptr, false};
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Pages(b, out), &t, g);
+}
+
+int ctmr_group_process_tiles_tree(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out, ctmr_tree* tree) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const TreeArgs t{tree, 1, nullptr, false};
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Tiles(b, out), &t, g);
+}
+
+int ctmr_group_process_raw_trees(ctmr_group* g, const ctmr_raw_batch* b, ctmr_raw_out* out, const uint32_t* entry_log, ctmr_tree* trees,
+                                 uint32_t n_trees) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const TreeArgs t{trees, n_trees, entry_log, true};
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Pages(b, out), &t, g);
+}
+
+int ctmr_group_process_tiles_trees(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out, const uint32_t* tile_log,
+                                   ctmr_tree* trees, uint32_t n_trees) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const TreeArgs t{trees, n_trees, tile_log, true};
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Tiles(b, out), &t, g);
 }
 
 int ctmr_next_index(ctmr_ctx* c, uint64_t* next_index) {

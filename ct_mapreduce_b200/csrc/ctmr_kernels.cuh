@@ -340,7 +340,8 @@ struct FoldTree {
     uint32_t tree;  // index into FoldChunk::trees
     uint32_t off;
     uint32_t cnt;   // > 0
-    uint32_t pad;
+    uint32_t skip;  // leaves first_pos .. first_pos + skip - 1 were in the tree before the call (a first tile that holds
+                    // its size): the range fold starts after them; the fold into a tree reads t.size instead
 };
 static_assert(sizeof(FoldTree) == 24, "FoldTree layout");
 
@@ -367,5 +368,38 @@ cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t 
 cudaError_t launch_tree_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t* const lvl[2], cudaStream_t s, uint32_t* launches);
 // the roots of trees[0, n) from their edges, rows of clear bits zeroed
 cudaError_t launch_tree_root(TreeDev* trees, uint32_t n, cudaStream_t s);
+
+// ---- the trees of a group call (ctmr_group_process_*_tree(s)): members 1.. fold their chunk into ranges ---------------
+// One tree's part of a member's chunk as the canonical decomposition of its leaves [begin, end) into complete subtrees.
+// begin = first_pos + skip; end is first_pos + cnt, or the member's first leaf at or above begin that is missing.  At
+// level l the range covers nodes [A_l, B_l), A_l = ceil(begin / 2^l), B_l = end >> l; an odd A_l leaves node A_l as
+// left[l], an odd B_l leaves node B_l - 1 as right[l], and the pairs between make level l + 1.  Rows of other levels are
+// not written.  The home member (member 0, which holds the trees) appends the range when begin is the tree's size.
+struct TreeRange {
+    uint64_t begin, end;
+    uint32_t tree;  // index into the call's trees
+    uint32_t pad;
+    uint8_t left[64][32];
+    uint8_t right[64][32];
+};
+static_assert(sizeof(TreeRange) == 4120 && sizeof(TreeRange) % 8 == 0, "TreeRange layout: rows stay 8-byte aligned");
+
+// The ranges of members 1..members (of one round) on the home member: member r's n[r - 1] ranges, ordered by tree, at
+// recv + (r - 1) * stride.
+struct RangeSet {
+    const TreeRange* recv;
+    uint32_t stride;
+    uint32_t members;
+    uint32_t n[kMaxWorld];
+};
+
+// Folds a chunk into one range per tree, out[i] for f.desc[i] (f.trees is not read): the launches of launch_tree_fold
+// (missing leaves, one per level of the widest tree range, commit), with miss[cap] as the missing-leaf words.  miss
+// must hold ~0 before the first chunk; each commit leaves it so.
+cudaError_t launch_range_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t* const lvl[2], TreeRange* out, unsigned long long* miss,
+                              cudaStream_t s, uint32_t* launches);
+// One launch, one thread per tree of trees[0, n): appends the members' ranges of that tree in member order, each only
+// when its begin is the tree's size, so that a tree stopped earlier keeps its size.
+cudaError_t launch_tree_merge(TreeDev* trees, uint32_t n, const RangeSet& set, cudaStream_t s);
 
 }  // namespace ctmr

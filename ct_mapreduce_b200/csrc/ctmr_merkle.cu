@@ -9,6 +9,12 @@
 //                                         node as the first left child, the last node as the new edge node
 //   K_tree_commit     thread per tree     the tree's new size
 //   K_tree_root       thread per tree     the root from the edge
+// On a group (ctmr_group_process_*_tree(s)) member 0 holds the trees and folds its chunk as above; members 1.. fold theirs
+// into ranges (TreeRange), which member 0 appends in member order:
+//   K_range_missing   thread per entry    per range, lowest log position of the chunk without a leaf
+//   K_range_level     thread per parent   tree_level with the range's odd first node stored as left[l], not paired
+//   K_range_commit    thread per range    the range's bounds
+//   K_tree_merge      thread per tree     the members' ranges appended to the edge (member 0, after the peer copies)
 //
 // A tree is held as its right edge (ctmr_tree): for every bit k of size, the root of the complete subtree of 2^k leaves
 // ending at the highest multiple of 2^(k+1) at or below size.  Folding leaves [a, b) in: at level l the chunk covers node
@@ -132,18 +138,26 @@ __device__ __forceinline__ const uint8_t* leaf_row(const FoldChunk& f, const Fol
     return f.leaves + 32 * (f.order ? (uint64_t)f.order[at] : at);
 }
 
+// listed entry g: whether it has no leaf, and then its tree's index in the chunk and its log position
+__device__ __forceinline__ bool no_leaf(const FoldChunk& f, uint64_t g, uint32_t* i_out, uint64_t* pos) {
+    if (g >= f.total) return false;
+    const uint32_t i = find_tree(f, g, [&](uint32_t x) { return (uint64_t)f.desc[x].off; });
+    if (i == f.n_desc) return false;
+    const FoldTree d = f.desc[i];
+    if (g >= (uint64_t)d.off + d.cnt) return false;  // entries a tiles chunk cut off after its stop
+    const uint64_t e = f.order ? (uint64_t)f.order[g] : g;
+    if (f.flags[e * f.stride] != f.match) return false;
+    *i_out = i;
+    *pos = d.first_pos + (g - d.off);
+    return true;
+}
+
 // one thread per listed entry: the lowest position of each tree without a leaf
 __global__ void __launch_bounds__(256) tree_missing_kernel(FoldChunk f) {
-    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= f.total) return;
-    const uint32_t i = find_tree(f, g, [&](uint32_t x) { return (uint64_t)f.desc[x].off; });
-    if (i == f.n_desc) return;
-    const FoldTree d = f.desc[i];
-    if (g >= (uint64_t)d.off + d.cnt) return;  // entries a tiles chunk cut off after its stop
-    const uint64_t e = f.order ? (uint64_t)f.order[g] : g;
-    if (f.flags[e * f.stride] != f.match) return;
-    TreeDev* tree = f.trees + d.tree;
-    const uint64_t pos = d.first_pos + (g - d.off);
+    uint32_t i;
+    uint64_t pos;
+    if (!no_leaf(f, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, &i, &pos)) return;
+    TreeDev* tree = f.trees + f.desc[i].tree;
     if (pos >= tree->t.size) atomicMin(&tree->missing, (unsigned long long)pos);
 }
 
@@ -221,6 +235,132 @@ __global__ void tree_root_kernel(TreeDev* trees, uint32_t n) {
         if (!((size >> k) & 1ull)) memset(t.edge[k], 0, 32);
 }
 
+// ---- ranges (members 1.. of a group call) and their merge on the home member -------------------------------------------
+// ceil(x / 2^s)
+__device__ __forceinline__ uint64_t shr64_up(uint64_t x, uint32_t s) {
+    return s >= 64u ? (x != 0) : (x >> s) + ((x & ((1ull << s) - 1ull)) != 0);
+}
+__device__ __forceinline__ uint64_t range_begin(const FoldTree& d) { return d.first_pos + d.skip; }
+// where a tree's range of this chunk ends: its first missing leaf at or above range_begin (miss), or the run's end
+__device__ __forceinline__ uint64_t range_end(const FoldTree& d, unsigned long long miss) {
+    const uint64_t lim = d.first_pos + d.cnt;
+    return miss < lim ? miss : lim;
+}
+
+// one thread per listed entry: the lowest position of each range without a leaf
+__global__ void __launch_bounds__(256) range_missing_kernel(FoldChunk f, unsigned long long* __restrict__ miss) {
+    uint32_t i;
+    uint64_t pos;
+    if (!no_leaf(f, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, &i, &pos)) return;
+    if (pos >= range_begin(f.desc[i])) atomicMin(&miss[i], (unsigned long long)pos);
+}
+
+// tree_level_kernel for ranges: level l of range i covers nodes [a, b) = [ceil(begin / 2^l), end >> l); an odd a is
+// stored as left[l] instead of being paired with the edge, so the pairs start at a + 1; an odd b leaves node b - 1 as
+// right[l].  The parents [(a + 1) >> 1, b >> 1) go to the range's rows of this launch.
+__global__ void __launch_bounds__(128) range_level_kernel(FoldChunk f, uint32_t level, const uint8_t* __restrict__ src,
+                                                         uint8_t* __restrict__ dst, TreeRange* __restrict__ out,
+                                                         const unsigned long long* __restrict__ miss) {
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t i = find_tree(f, k, [&](uint32_t x) { return level_base(f.desc[x], x, level); });
+    if (i == f.n_desc) return;
+    const FoldTree d = f.desc[i];
+    const uint64_t a = shr64_up(range_begin(d), level), b = range_end(d, miss[i]) >> level;
+    if (a >= b) return;
+    const uint64_t k0 = level_base(d, i, level), pa = (a + 1) >> 1, pb = b >> 1, p = pa + (k - k0);
+    const uint64_t in = level == 0 ? 0 : level_base(d, i, level - 1);
+    auto row = [&](uint64_t pos) {  // node `pos` of this level
+        return level == 0 ? leaf_row(f, d, pos - d.first_pos) : src + 32 * (in + pos - a);
+    };
+    if (p < pb) {
+        uint32_t l[8], r[8], h[8];
+        load_row(row(2 * p), l);
+        load_row(row(2 * p + 1), r);
+        node_hash(l, r, h);
+        store_row(dst + 32 * (k0 + p - pa), h);
+    }
+    if (k == k0) {
+        uint32_t h[8];
+        if (a & 1) {
+            load_row(row(a), h);
+            store_row(out[i].left[level], h);
+        }
+        if (b & 1) {
+            load_row(row(b - 1), h);
+            store_row(out[i].right[level], h);
+        }
+    }
+}
+
+// one thread per range of the chunk: its bounds and tree, and the missing-leaf word back to ~0
+__global__ void range_commit_kernel(FoldChunk f, TreeRange* __restrict__ out, unsigned long long* __restrict__ miss) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= f.n_desc) return;
+    const FoldTree d = f.desc[i];
+    out[i].begin = range_begin(d);
+    out[i].end = range_end(d, miss[i]);
+    out[i].tree = d.tree;
+    miss[i] = ~0ull;
+}
+
+// a complete subtree of 2^level leaves appended to the edge at position size (a multiple of 2^level): binary carry
+__device__ __forceinline__ void push_node(ctmr_tree& t, uint64_t& size, const uint8_t* row, uint32_t level) {
+    uint32_t h[8];
+    load_row(row, h);
+    uint32_t k = level;
+    for (; k < 64 && ((size >> k) & 1ull); ++k) {
+        uint32_t l[8], x[8];
+        load_row(t.edge[k], l);
+        node_hash(l, h, x);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) h[j] = x[j];
+    }
+    store_row(t.edge[k], h);
+    size += 1ull << level;
+}
+
+// one thread per tree of the call: each member's range of the tree, in member order, appended when it starts at the
+// tree's size -- left nodes by ascending level, then right nodes by descending level -- so that size ends at its end
+__global__ void tree_merge_kernel(TreeDev* trees, uint32_t n, RangeSet set) {
+    const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= n) return;
+    ctmr_tree& t = trees[d].t;
+    uint64_t size = t.size;
+    for (uint32_t r = 0; r < set.members; ++r) {
+        const TreeRange* g = set.recv + (uint64_t)r * set.stride;
+        uint32_t lo = 0, hi = set.n[r];
+        while (lo < hi) {  // the member's ranges are ordered by tree
+            const uint32_t mid = (lo + hi) >> 1;
+            if (g[mid].tree < d) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo == set.n[r] || g[lo].tree != d) continue;
+        const TreeRange& x = g[lo];
+        if (x.begin != size) continue;  // an earlier stop (or an earlier member's) ends the tree below this range
+        for (uint32_t l = 0; l < 64; ++l) {
+            const uint64_t a = shr64_up(x.begin, l), b = x.end >> l;
+            if (a >= b) break;
+            if (a & 1) push_node(t, size, x.left[l], l);
+        }
+        for (int l = 63; l >= 0; --l) {
+            const uint64_t a = shr64_up(x.begin, (uint32_t)l), b = x.end >> l;
+            if (a < b && (b & 1)) push_node(t, size, x.right[l], (uint32_t)l);
+        }
+    }
+    t.size = size;
+}
+
+// Levels where a tree's own range [first_pos, first_pos + cnt) is empty are empty for the part that folds too: the chunk
+// takes as many level launches as its widest range has levels
+uint32_t fold_levels(const FoldTree* hdesc, uint32_t n) {
+    uint32_t levels = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint64_t x = hdesc[i].first_pos ^ (hdesc[i].first_pos + hdesc[i].cnt);
+        levels = std::max(levels, x ? 64u - (uint32_t)__builtin_clzll(x) : 0u);
+    }
+    return levels;
+}
+
 }  // namespace
 
 cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t s) {
@@ -234,13 +374,7 @@ cudaError_t launch_tree_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t*
     if (f.n_desc == 0) return cudaSuccess;
     tree_missing_kernel<<<(unsigned)((f.total + 255) / 256), 256, 0, s>>>(f);
     ++*launches;
-    // Levels where a tree's own range [first_pos, first_pos + cnt) is empty are empty for the part that folds too: the
-    // chunk takes as many level launches as its widest range has levels
-    uint32_t levels = 0;
-    for (uint32_t i = 0; i < f.n_desc; ++i) {
-        const uint64_t x = hdesc[i].first_pos ^ (hdesc[i].first_pos + hdesc[i].cnt);
-        levels = std::max(levels, x ? 64u - (uint32_t)__builtin_clzll(x) : 0u);
-    }
+    const uint32_t levels = fold_levels(hdesc, f.n_desc);
     for (uint32_t l = 0; l < levels; ++l) {
         const uint64_t threads = shr64(f.total, l + 1) + 2ull * f.n_desc;
         tree_level_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(f, l, l == 0 ? f.leaves : lvl[(l - 1) & 1], lvl[l & 1]);
@@ -254,6 +388,29 @@ cudaError_t launch_tree_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t*
 cudaError_t launch_tree_root(TreeDev* trees, uint32_t n, cudaStream_t s) {
     if (n == 0) return cudaSuccess;
     tree_root_kernel<<<(n + 127) / 128, 128, 0, s>>>(trees, n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_range_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t* const lvl[2], TreeRange* out, unsigned long long* miss,
+                              cudaStream_t s, uint32_t* launches) {
+    *launches = 0;
+    if (f.n_desc == 0) return cudaSuccess;
+    range_missing_kernel<<<(unsigned)((f.total + 255) / 256), 256, 0, s>>>(f, miss);
+    ++*launches;
+    const uint32_t levels = fold_levels(hdesc, f.n_desc);
+    for (uint32_t l = 0; l < levels; ++l) {
+        const uint64_t threads = shr64(f.total, l + 1) + 2ull * f.n_desc;
+        range_level_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(f, l, l == 0 ? f.leaves : lvl[(l - 1) & 1], lvl[l & 1], out, miss);
+        ++*launches;
+    }
+    range_commit_kernel<<<(f.n_desc + 127) / 128, 128, 0, s>>>(f, out, miss);
+    ++*launches;
+    return cudaGetLastError();
+}
+
+cudaError_t launch_tree_merge(TreeDev* trees, uint32_t n, const RangeSet& set, cudaStream_t s) {
+    if (n == 0 || set.members == 0) return cudaSuccess;
+    tree_merge_kernel<<<(n + 127) / 128, 128, 0, s>>>(trees, n, set);
     return cudaGetLastError();
 }
 

@@ -311,20 +311,26 @@ class GpuCertDatabase:
                           n, now_unix_ns)
         if trees is not None:
             arr = _trees_to_c(trees)
-            self._check(self._lib.ctmr_process_raw_trees(self._h, C.byref(b), C.byref(o), capi.ptr(log) if n else None,
-                                                         arr if trees else None, len(trees)))
+            self._check(self._process_raw_trees_fn()(self._h, C.byref(b), C.byref(o), capi.ptr(log) if n else None,
+                                                     arr if trees else None, len(trees)))
             r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
             return r
         if tree is None:
             self._check(self._process_raw_fn()(self._h, C.byref(b), C.byref(o)))
             return r
         ct = tree.to_c()
-        self._check(self._lib.ctmr_process_raw_tree(self._h, C.byref(b), C.byref(o), C.byref(ct)))
+        self._check(self._process_raw_tree_fn()(self._h, C.byref(b), C.byref(o), C.byref(ct)))
         r.tree = LogTree.from_c(ct)
         return r
 
     def _process_raw_fn(self):
         return self._lib.ctmr_process_raw
+
+    def _process_raw_tree_fn(self):
+        return self._lib.ctmr_process_raw_tree
+
+    def _process_raw_trees_fn(self):
+        return self._lib.ctmr_process_raw_trees
 
     # ------------------------------------------------------------------ static-ct-api data tiles (include/ctmr_frontend.h)
     def register_chain_certs(self, blob, offsets):
@@ -344,6 +350,12 @@ class GpuCertDatabase:
 
     def _process_tiles_fn(self):
         return self._lib.ctmr_process_tiles
+
+    def _process_tiles_tree_fn(self):
+        return self._lib.ctmr_process_tiles_tree
+
+    def _process_tiles_trees_fn(self):
+        return self._lib.ctmr_process_tiles_trees
 
     def store_tiles(self, data, tile_off, tile_len, tile_index, tile_width, now_unix_ns: int, want_sha: bool = True,
                     want_meta: bool = False, want_pem: bool = False, want_leaf_hash: bool = False, missing_cap: int = 256,
@@ -405,14 +417,14 @@ class GpuCertDatabase:
                         rest = np.flatnonzero(tlog[t0:] == d)
                         if rest.size and arr[d].size < 256 * int(tile_index[t0 + rest[0]]):
                             tlog[t0 + rest] = capi.NO_TREE
-                rc = self._lib.ctmr_process_tiles_trees(self._h, C.byref(b), C.byref(o), capi.ptr(tlog) + 4 * t0 if nt else None,
-                                                        arr if trees else None, len(trees))
+                rc = self._process_tiles_trees_fn()(self._h, C.byref(b), C.byref(o), capi.ptr(tlog) + 4 * t0 if nt else None,
+                                                    arr if trees else None, len(trees))
                 if rc in (0, capi.E_UNKNOWN_ISSUER):
                     r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
             elif ct is None:
                 rc = self._process_tiles_fn()(self._h, C.byref(b), C.byref(o))
             else:  # written back on success and at the stop: the resumed call continues this tree
-                rc = self._lib.ctmr_process_tiles_tree(self._h, C.byref(b), C.byref(o), C.byref(ct))
+                rc = self._process_tiles_tree_fn()(self._h, C.byref(b), C.byref(o), C.byref(ct))
                 if rc in (0, capi.E_UNKNOWN_ISSUER):
                     r.tree = LogTree.from_c(ct)
             done = int(o.tiles_done)
@@ -639,15 +651,37 @@ class GpuCertGroup(GpuCertDatabase):
     def _process_tiles_fn(self):
         return self._lib.ctmr_group_process_tiles
 
+    def _process_raw_tree_fn(self):
+        return self._lib.ctmr_group_process_raw_tree
+
+    def _process_raw_trees_fn(self):
+        return self._lib.ctmr_group_process_raw_trees
+
+    def _process_tiles_tree_fn(self):
+        return self._lib.ctmr_group_process_tiles_tree
+
+    def _process_tiles_trees_fn(self):
+        return self._lib.ctmr_group_process_tiles_trees
+
     def store_raw_entries(self, *a, tree=None, trees=None, **k):
-        if tree is not None or trees is not None:  # members hold disjoint slices: the fold would have to be ordered across GPUs
-            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: a group has no tree form")
+        if tree is not None or trees is not None:
+            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: on a group use store_raw_entries_with_trees")
         return super().store_raw_entries(*a, **k)
 
     def store_tiles(self, *a, tree=None, trees=None, **k):
         if tree is not None or trees is not None:
-            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: a group has no tree form")
+            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: on a group use store_tiles_with_trees")
         return super().store_tiles(*a, **k)
+
+    def store_raw_entries_with_trees(self, *a, tree=None, trees=None, entry_log=None, **k):
+        """store_raw_entries with tree= or trees= / entry_log= on the group (ctmr_group_process_raw_tree(s)): the same
+        outputs as the plain group call, and r.tree / r.trees as the one-ctx call gives them"""
+        return GpuCertDatabase.store_raw_entries(self, *a, tree=tree, trees=trees, entry_log=entry_log, **k)
+
+    def store_tiles_with_trees(self, *a, fetch=None, tree=None, trees=None, tile_log=None, **k):
+        """store_tiles with tree= or trees= / tile_log= on the group (ctmr_group_process_tiles_tree(s)), with the same
+        fetch-and-resume loop and per-log resume rule as GpuCertDatabase.store_tiles"""
+        return GpuCertDatabase.store_tiles(self, *a, fetch=fetch, tree=tree, trees=trees, tile_log=tile_log, **k)
 
     def _register_chain_fn(self):
         return self._lib.ctmr_group_register_chain_certs

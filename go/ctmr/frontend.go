@@ -142,25 +142,16 @@ func (d *DB) ProcessRaw(p *RawPages, nowUnixNs int64, r *RawResult) error {
 }
 
 // processRaw also folds the entries into tree when it is not nil (ProcessRawTree, tree.go), or, when routed, each entry
-// into trees[p.Log[i]] (ProcessRawTrees).
+// into trees[p.Log[i]] (ProcessRawTrees), on one GPU or on every GPU of the group.
 func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree, trees []Tree, routed bool) error {
 	n := len(p.LeafOff)
-	if (tree != nil || routed) && d.g != nil {
-		return fmt.Errorf("ProcessRawTree(s): a group has no tree form; use one DB per GPU")
-	}
 	if n == 0 && tree == nil && !routed && !d.peer {
 		return nil
 	}
 	b := (*C.ctmr_raw_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_raw_batch{}))))
 	defer C.free(unsafe.Pointer(b))
 	if n == 0 { // the roots of the trees as they stand; a peer DB's empty part of a collective call
-		if routed {
-			return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, nil, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")
-		}
-		if tree == nil {
-			return d.err(C.ctmr_process_raw(d.h, b, r.raw), "ctmr_process_raw")
-		}
-		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
+		return d.rawCall(b, r, nil, tree, trees, routed)
 	}
 	// the span arrays are flat Go slices; the struct that points at them is C memory, and the pointers are only
 	// stored for the duration of the call -> pin them (Go 1.21 runtime.Pinner) so that the store is legal
@@ -178,18 +169,30 @@ func (d *DB) processRaw(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree, 
 	b.extra_data_len = (*C.uint32_t)(unsafe.Pointer(&p.ExtraLen[0]))
 	b.n = C.uint64_t(n)
 	b.now_unix_ns = C.int64_t(nowUnixNs)
-	if d.g != nil { // several GPUs: one chunk per GPU per round, the same outputs in entry order
-		return d.err(C.ctmr_group_process_raw(d.g, b, r.raw), "ctmr_group_process_raw")
-	}
+	var log *C.uint32_t
 	if routed {
 		if len(p.Log) != n {
 			return d.peerRefuse(fmt.Errorf("ProcessRawTrees: %d log ids for %d entries", len(p.Log), n))
 		}
-		log := (*C.uint32_t)(unsafe.Pointer(&p.Log[0])) // pointer-free Go memory, passed for the call only
-		return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, log, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")
+		log = (*C.uint32_t)(unsafe.Pointer(&p.Log[0])) // pointer-free Go memory, passed for the call only
 	}
-	if tree != nil {
+	return d.rawCall(b, r, log, tree, trees, routed)
+}
+
+// rawCall makes the plain, one-tree or routed call on the ctx, or on the group (several GPUs: one chunk per GPU per
+// round, the same outputs in entry order and the same trees).
+func (d *DB) rawCall(b *C.ctmr_raw_batch, r *RawResult, log *C.uint32_t, tree *Tree, trees []Tree, routed bool) error {
+	switch {
+	case routed && d.g != nil:
+		return d.err(C.ctmr_group_process_raw_trees(d.g, b, r.raw, log, treesC(trees), C.uint32_t(len(trees))), "ctmr_group_process_raw_trees")
+	case routed:
+		return d.err(C.ctmr_process_raw_trees(d.h, b, r.raw, log, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_raw_trees")
+	case tree != nil && d.g != nil:
+		return d.err(C.ctmr_group_process_raw_tree(d.g, b, r.raw, tree.c()), "ctmr_group_process_raw_tree")
+	case tree != nil:
 		return d.err(C.ctmr_process_raw_tree(d.h, b, r.raw, tree.c()), "ctmr_process_raw_tree")
+	case d.g != nil:
+		return d.err(C.ctmr_group_process_raw(d.g, b, r.raw), "ctmr_group_process_raw")
 	}
 	return d.err(C.ctmr_process_raw(d.h, b, r.raw), "ctmr_process_raw")
 }

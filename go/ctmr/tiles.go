@@ -130,13 +130,10 @@ func (d *DB) ProcessTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 }
 
 // processTiles also folds the entries into tree when it is not nil (ProcessTilesTree, tree.go), or, when routed, each
-// tile into trees[t.Log[k]] (ProcessTilesTrees): the library writes the trees back at every stop, so each resumed call
-// carries them on from the tiles completed so far.
+// tile into trees[t.Log[k]] (ProcessTilesTrees), on one GPU or on every GPU of the group: the library writes the trees
+// back at every stop, so each resumed call carries them on from the tiles completed so far.
 func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree,
 	trees []Tree, routed bool) error {
-	if (tree != nil || routed) && d.g != nil {
-		return fmt.Errorf("ProcessTilesTree(s): a group has no tree form; use one DB per GPU")
-	}
 	if routed && len(t.Log) != len(t.Off) {
 		return d.peerRefuse(fmt.Errorf("ProcessTilesTrees: %d log ids for %d tiles", len(t.Log), len(t.Off)))
 	}
@@ -144,10 +141,7 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 		if tree != nil || routed { // the roots of the trees as they stand
 			b := (*C.ctmr_tile_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_tile_batch{}))))
 			defer C.free(unsafe.Pointer(b))
-			if routed {
-				return d.err(C.ctmr_process_tiles_trees(d.h, b, r.out, nil, treesC(trees), C.uint32_t(len(trees))), "ctmr_process_tiles_trees")
-			}
-			return d.err(C.ctmr_process_tiles_tree(d.h, b, r.out, tree.c()), "ctmr_process_tiles_tree")
+			return d.err(d.tilesCall(b, r.out, nil, tree, trees, routed, true), "ctmr_process_tiles_tree(s)")
 		}
 		return nil
 	}
@@ -196,20 +190,11 @@ func (d *DB) processTiles(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(f
 				}
 			}
 		}
-		var rc C.int
-		if d.g != nil {
-			rc = C.ctmr_group_process_tiles(d.g, b, o)
-		} else if routed {
-			var lp *C.uint32_t
-			if t0 < len(log) {
-				lp = (*C.uint32_t)(unsafe.Pointer(&log[t0]))
-			}
-			rc = C.ctmr_process_tiles_trees(d.h, b, o, lp, treesC(trees), C.uint32_t(len(trees)))
-		} else if fold {
-			rc = C.ctmr_process_tiles_tree(d.h, b, o, tree.c())
-		} else {
-			rc = C.ctmr_process_tiles(d.h, b, o)
+		var lp *C.uint32_t
+		if routed && t0 < len(log) {
+			lp = (*C.uint32_t)(unsafe.Pointer(&log[t0]))
 		}
+		rc := d.tilesCall(b, o, lp, tree, trees, routed, fold)
 		done := int(o.tiles_done)
 		e1 := e0
 		for k := t0; k < t0+done; k++ {
@@ -298,4 +283,22 @@ func shiftTileOut(o *C.ctmr_tile_out, e0, t0 int, pemBase uint64) {
 	if o.tile_status != nil {
 		o.tile_status = (*C.uint8_t)(unsafe.Add(unsafe.Pointer(o.tile_status), t0))
 	}
+}
+
+// tilesCall makes the plain, one-tree (fold) or routed call on the ctx, or on the group (several GPUs: one chunk of
+// whole tiles per GPU per round, the same outputs, stop and trees).
+func (d *DB) tilesCall(b *C.ctmr_tile_batch, o *C.ctmr_tile_out, log *C.uint32_t, tree *Tree, trees []Tree, routed, fold bool) C.int {
+	switch {
+	case routed && d.g != nil:
+		return C.ctmr_group_process_tiles_trees(d.g, b, o, log, treesC(trees), C.uint32_t(len(trees)))
+	case routed:
+		return C.ctmr_process_tiles_trees(d.h, b, o, log, treesC(trees), C.uint32_t(len(trees)))
+	case fold && d.g != nil:
+		return C.ctmr_group_process_tiles_tree(d.g, b, o, tree.c())
+	case fold:
+		return C.ctmr_process_tiles_tree(d.h, b, o, tree.c())
+	case d.g != nil:
+		return C.ctmr_group_process_tiles(d.g, b, o)
+	}
+	return C.ctmr_process_tiles(d.h, b, o)
 }

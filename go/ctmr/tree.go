@@ -42,7 +42,7 @@ func treesC(trees []Tree) *C.ctmr_tree {
 
 // ProcessRawTree is ProcessRaw, and the pages' entries folded into tree as the log's entries tree.Size, tree.Size+1, ....
 // An entry whose leaf_input is not base64 has no leaf: the fold stops before it and tree.Size says where.  On an error
-// tree is unchanged.  One GPU only: a group returns an error.
+// tree is unchanged.  On a group the GPUs fold their chunks in log order and the tree is the one-GPU tree.
 func (d *DB) ProcessRawTree(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tree) error {
 	return d.processRaw(p, nowUnixNs, r, tree, nil, false)
 }
@@ -51,7 +51,7 @@ func (d *DB) ProcessRawTree(p *RawPages, nowUnixNs int64, r *RawResult, tree *Tr
 // AppendLog(body, log) are the next leaves of trees[log]; those added with Append fold nowhere.  This is the one flush
 // of a batcher that drains the pages of every log it syncs into one RawPages: each log keeps the one-tree rules on its
 // own entries, and a bad base64 leaf_input stops only its own log's tree.  Every tree gets its root written, also a tree
-// with no entry in the batch.  On an error every tree is unchanged.  One GPU only.
+// with no entry in the batch.  On an error every tree is unchanged.  On one GPU or a group.
 func (d *DB) ProcessRawTrees(p *RawPages, nowUnixNs int64, r *RawResult, trees []Tree) error {
 	return d.processRaw(p, nowUnixNs, r, nil, trees, true)
 }
@@ -60,7 +60,8 @@ func (d *DB) ProcessRawTrees(p *RawPages, nowUnixNs int64, r *RawResult, trees [
 // log, full but for the last, with tree.Size inside the first: its leaves below tree.Size are skipped.  A bad tile stops
 // the fold at its first leaf, and the rest of the batch is still processed.  The fetch/register/resume loop carries the
 // tree from call to call; once a bad tile has stopped the fold, it resumes with ProcessTiles' plain call and the tree
-// stays as it is.  Tree and outputs equal those of one call with every certificate registered first.  One GPU only.
+// stays as it is.  Tree and outputs equal those of one call with every certificate registered first.  On one GPU or a
+// group.
 func (d *DB) ProcessTilesTree(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), tree *Tree) error {
 	return d.processTiles(t, nowUnixNs, r, fetch, tree, nil, false)
 }
@@ -69,7 +70,7 @@ func (d *DB) ProcessTilesTree(t *Tiles, nowUnixNs int64, r *TileResult, fetch fu
 // AppendLog(body, index, width, log) is the next tile of trees[log]; one added with Append folds nowhere.  Each log's
 // tiles keep ProcessTilesTree's rules in batch order, interleaved with the other logs' in any way.  The resume loop
 // carries the trees; a log whose tree a bad tile stopped (its size is below its first remaining tile) goes on as
-// NoTree.  Trees and outputs equal those of one call with every certificate registered first.  One GPU only.
+// NoTree.  Trees and outputs equal those of one call with every certificate registered first.  On one GPU or a group.
 func (d *DB) ProcessTilesTrees(t *Tiles, nowUnixNs int64, r *TileResult, fetch func(fp [32]byte) ([]byte, error), trees []Tree) error {
 	return d.processTiles(t, nowUnixNs, r, fetch, nil, trees, true)
 }

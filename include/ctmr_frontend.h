@@ -251,6 +251,25 @@ int ctmr_process_raw_trees(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_
 int ctmr_process_tiles_trees(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_tile_out* out,
                              const uint32_t* tile_log /* [n_tiles] */, ctmr_tree* trees, uint32_t n_trees);
 
+/* ---- the trees on a group ----------------------------------------------------------------------------------------------
+ * The four tree calls on every GPU of a group (ctmr_group_create, ctmr.h).  Every output, return code, global index,
+ * PEM text, tiles_done, missing_fp and n_missing is that of ctmr_group_process_raw / ctmr_group_process_tiles on the
+ * same group, and every tree is that of the matching one-ctx call on the same batch, with all of its rules: the argument
+ * and per-log checks before any work (no index taken, no tree touched), the leaves that stop a fold, the leaves of a
+ * first tile below size, the trees written back at CTMR_E_UNKNOWN_ISSUER with the same resume rules, and every tree left
+ * as passed in on any other error.  A member ctx keeps refusing the one-ctx tree forms: a group's trees go through the
+ * group handle.
+ *
+ * In each round the first GPU of the group folds its chunk into the trees; every other GPU folds its chunk into a
+ * compact range per tree (at most 64 left and 64 right nodes), and the first GPU appends those ranges in member order
+ * after the round. */
+int ctmr_group_process_raw_tree(ctmr_group* g, const ctmr_raw_batch* batch, ctmr_raw_out* out, ctmr_tree* tree);
+int ctmr_group_process_tiles_tree(ctmr_group* g, const ctmr_tile_batch* batch, ctmr_tile_out* out, ctmr_tree* tree);
+int ctmr_group_process_raw_trees(ctmr_group* g, const ctmr_raw_batch* batch, ctmr_raw_out* out,
+                                 const uint32_t* entry_log /* [n] */, ctmr_tree* trees, uint32_t n_trees);
+int ctmr_group_process_tiles_trees(ctmr_group* g, const ctmr_tile_batch* batch, ctmr_tile_out* out,
+                                   const uint32_t* tile_log /* [n_tiles] */, ctmr_tree* trees, uint32_t n_trees);
+
 /* ---- one process per GPU: the front end as a collective call ------------------------------------------------------------
  * On a ctx attached to peers (ctmr_peer_attach, ctmr.h, world > 1) ctmr_process_raw, ctmr_process_tiles,
  * ctmr_process_raw_tree, ctmr_process_tiles_tree, ctmr_process_raw_trees and ctmr_process_tiles_trees are COLLECTIVE.
@@ -296,7 +315,7 @@ int ctmr_process_tiles_trees(ctmr_ctx* ctx, const ctmr_tile_batch* batch, ctmr_t
  *
  * Trees.  Each rank folds its own batch's entries into its own caller-held trees, with the one-GPU rules: log order is
  * batch order on that rank, and global indices do not enter the tree.  Members of an in-process group (ctmr_group_*)
- * keep refusing the tree forms. */
+ * keep refusing the one-ctx tree forms; the group's own tree calls are above. */
 
 /* *ranks = the ranks that stopped at an unknown Chain[0] fingerprint (CTMR_E_UNKNOWN_ISSUER) in the last collective
  * front-end call on this ctx; 0 after a call that failed before any work.  CTMR_E_INVALID on a ctx not attached to

@@ -37,7 +37,7 @@ EXPORTS = [
     "ctmr_process_tiles", "ctmr_group_process_tiles", "ctmr_register_chain_certs", "ctmr_group_register_chain_certs",
     "ctmr_tiles_profile_last", "ctmr_process_raw_tree", "ctmr_process_tiles_tree", "ctmr_process_raw_trees",
     "ctmr_process_tiles_trees", "ctmr_group_process_raw_tree", "ctmr_group_process_tiles_tree", "ctmr_group_process_raw_trees",
-    "ctmr_group_process_tiles_trees",
+    "ctmr_group_process_tiles_trees", "ctmr_process_raw_bodies", "ctmr_group_process_raw_bodies", "ctmr_bodies_profile_last",
     # several GPUs: one process (group) / one process per GPU (peer)
     "ctmr_group_create", "ctmr_group_destroy", "ctmr_group_last_error", "ctmr_group_size", "ctmr_group_member",
     "ctmr_group_process_batch", "ctmr_group_issuer_counts", "ctmr_group_set_cardinality", "ctmr_group_status_counters",
@@ -58,6 +58,8 @@ E_UNKNOWN_ISSUER = -12
 E_PEER_FAILED = -13   # another rank's part of a collective call failed before any work
 # per-entry outcome of the front end (include/ctmr_frontend.h CTMR_FE_*)
 FE_OK, FE_BAD_BASE64, FE_BAD_LEAF, FE_UNKNOWN_TYPE, FE_BAD_EXTRA, FE_BAD_CERT, FE_BAD_TILE, FE_BAD_INDEX = range(8)
+# body status of ctmr_process_raw_bodies (include/ctmr_frontend.h CTMR_BODY_*)
+BODY_OK, BODY_BAD_JSON, BODY_BAD_TYPE, BODY_TOO_MANY, BODY_REPEATED_ENTRIES = range(5)
 NO_TREE = 0xFFFFFFFF   # CTMR_NO_TREE: an entry or tile of ctmr_process_*_trees that folds into no tree
 MAX_TREES = 1024       # CTMR_MAX_TREES
 
@@ -103,6 +105,19 @@ class RawOut(C.Structure):
     """ctmr_raw_out (include/ctmr_frontend.h)."""
     _fields_ = [("path", Out)] + [(n, C.c_void_p) for n in
                                   ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_src", "leaf_off", "leaf_len")]
+
+
+class BodyBatch(C.Structure):
+    """ctmr_body_batch (include/ctmr_frontend.h)."""
+    _fields_ = [("text", C.c_void_p), ("text_bytes", C.c_uint64), ("body_off", C.c_void_p), ("body_len", C.c_void_p),
+                ("body_max", C.c_void_p), ("n_bodies", C.c_uint64), ("now_unix_ns", C.c_int64)]
+
+
+class BodyOut(C.Structure):
+    """ctmr_body_out (include/ctmr_frontend.h)."""
+    _fields_ = [("raw", RawOut)] + [(n, C.c_void_p) for n in
+                                    ("body_status", "body_first", "body_entries", "leaf_input_off", "leaf_input_len",
+                                     "extra_data_off", "extra_data_len", "escaped")] + [("n_entries", C.c_uint64)]
 
 
 class TileBatch(C.Structure):
@@ -211,6 +226,9 @@ def load():
     L.ctmr_group_process_tiles_tree.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), C.POINTER(Tree)]
     L.ctmr_group_process_raw_trees.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), vp, vp, u32]
     L.ctmr_group_process_tiles_trees.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), vp, vp, u32]
+    L.ctmr_process_raw_bodies.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut)]
+    L.ctmr_group_process_raw_bodies.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut)]
+    L.ctmr_bodies_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
     L.ctmr_group_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_synth_tiles_host.argtypes = [C.POINTER(SynthCfg), u64, u64, vp, vp, u64, vp, vp]
     L.ctmr_synth_tiles_host.restype = u64

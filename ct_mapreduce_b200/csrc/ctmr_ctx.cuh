@@ -188,6 +188,26 @@ struct TileState {
     std::unordered_map<std::string, uint32_t> fp_memo;
 };
 
+// whole get-entries bodies (ctmr_process_raw_bodies): the JSON kernels' buffers for a chunk of up to cap_text / 2 bytes
+// and cap_entries bodies and requested entries.  Allocated on the first bodies call.
+struct BodyState {
+    DevBuf<BodyDesc> desc[2];  // per upload stage: the chunk's bodies, device and pinned host
+    HostBuf<BodyDesc> h_desc[2];
+    DevBuf<unsigned long long> starts;
+    DevBuf<uint8_t> trans, carry;
+    DevBuf<BlockMasks> masks;
+    DevBuf<uint32_t> stack;
+    DevBuf<uint8_t> body_status;
+    DevBuf<uint32_t> body_count, body_base;
+    DevBuf<uint64_t> s_off[2], abs_off[2];
+    DevBuf<uint32_t> s_len[2], raw_len[2];
+    DevBuf<uint8_t> s_esc, esc;
+    DevBuf<uint8_t> temp;
+    size_t temp_bytes = 0;
+    Event ev_json0, ev_json1;  // around the JSON kernels: timed on their own
+    float json_ms = 0.f;
+};
+
 // the logs' Merkle trees (ctmr_process_*_tree, ctmr_process_*_trees): the call's trees on the device and the scratch of
 // the fold.  Allocated on the first tree call, for cap_trees trees; a call with more trees builds it again, larger.  On
 // a group (ctmr_group_process_*_tree(s)) member 0 holds the trees; every other member folds its chunks into ranges, and
@@ -256,6 +276,7 @@ struct FrontEnd {
     PemStage pem;
     std::unique_ptr<TileState> tl;    // tiles_ensure
     std::unique_ptr<TreeState> tree;  // tree_ensure
+    std::unique_ptr<BodyState> bd;    // bodies_ensure
 };
 
 // the ctx's private device words (one allocation)
@@ -429,6 +450,7 @@ int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n, const
 int frontend_ensure(ctmr_ctx* c);   // allocates the front end's buffers on first use (ctmr_api.cu)
 int tiles_ensure(ctmr_ctx* c);      // ... and the tile buffers + fingerprint table (ctmr_frontend_api.cu), after frontend_ensure
 int tiles_clear_fingerprints(ctmr_ctx* c);
+int bodies_ensure(ctmr_ctx* c);     // ... and the JSON buffers of ctmr_process_raw_bodies (ctmr_frontend_api.cu), after frontend_ensure
 int ensure_scratch(ctmr_ctx* c, uint64_t n);
 int ensure_device_path(ctmr_ctx* c, uint64_t n);   // what ctmr_process_device needs for n entries
 uint64_t device_round_entries(uint64_t n, uint32_t rounds);   // E of a ctmr_process_device call cut into `rounds` rounds

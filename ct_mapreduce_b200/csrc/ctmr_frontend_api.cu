@@ -339,6 +339,8 @@ struct Pages {
     int copy_back(ctmr_ctx* c, const Chunk& ch) const;
     void completed(uint64_t) const {}
     int stop(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }  // a page chunk never stops
+    void place(Chunk*, uint32_t) const {}  // entry positions are known at upload
+    uint64_t entries() const { return done; }
 };
 
 // tree: ctmr_process_raw_tree's rule as well; a routed call's rules fail before any index is taken
@@ -441,18 +443,16 @@ int Pages::upload(ctmr_ctx* c, Chunk& ch) const {
     return CTMR_OK;
 }
 
-// decode + frame + Chain[0] -> dense index of an uploaded chunk; leaves ch.db / ch.dout describing the device-resident batch
-int Pages::front(ctmr_ctx* c, Chunk& ch) const {
+// decode + frame + Chain[0] -> dense index of the cnt entries whose string spans are in stage ch.stage (text_bytes of
+// characters from the stage's text); leaves ch.db / ch.dout describing the device-resident batch.  Issued after f->ev0.
+int spans_front(ctmr_ctx* c, Chunk& ch, uint64_t text_bytes, uint64_t cnt, int64_t now_unix_ns, const ctmr_out* po, bool meta) {
     FrontEnd* f = c->fe.get();
     cudaStream_t s = c->stream;
-    CU(c, cudaSetDevice(c->device));
     FeStage& st = f->stage[ch.stage];
-    const uint64_t cnt = ch.hi - ch.lo;
-    CU(c, cudaStreamWaitEvent(s, st.uploaded, 0));
     FeParams& p = ch.p.fe;
     p = FeParams{};
     p.text = st.text + 16;
-    p.text_bytes = ch.bytes;
+    p.text_bytes = text_bytes;
     p.leaf_off = st.leaf_off; p.leaf_len = st.leaf_len; p.extra_off = st.extra_off; p.extra_len = st.extra_len;
     p.n = cnt;
     p.pad_size = f->pad_size; p.dec_off = f->dec_off; p.dec_len = f->dec_len; p.str_bad = f->str_bad; p.decoded = f->decoded;
@@ -461,7 +461,6 @@ int Pages::front(ctmr_ctx* c, Chunk& ch) const {
     p.chain_len = f->chain_len; p.tbs_abs = f->tbs_abs; p.tbs_len = f->tbs_len; p.issuer_idx = f->issuer_idx;
     ch.db = ctmr_dev_batch{};
     ch.dout = ctmr_dev_out{};
-    CU(c, cudaEventRecord(f->ev0, s));
     if (cnt) {
         CU(c, launch_fe_decode(p, f->scan_temp, f->scan_temp_bytes, c->sm_count, s));
         CU(c, cudaEventRecord(st.consumed, s));  // text and spans are dead once decoded: the stage may be refilled
@@ -525,13 +524,21 @@ int Pages::front(ctmr_ctx* c, Chunk& ch) const {
     db.lens = f->leaf_len_out;
     db.n = cnt;
     db.issuer_idx = f->issuer_idx;
-    db.now_unix_ns = b->now_unix_ns;
-    ch.dout = chunk_path_out(f, &out->path, meta);
+    db.now_unix_ns = now_unix_ns;
+    ch.dout = chunk_path_out(f, po, meta);
     return CTMR_OK;
 }
 
-// the front end's own outputs of a chunk, after the path's; waits for the chunk
-int Pages::copy_back(ctmr_ctx* c, const Chunk& ch) const {
+int Pages::front(ctmr_ctx* c, Chunk& ch) const {
+    FrontEnd* f = c->fe.get();
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaStreamWaitEvent(c->stream, f->stage[ch.stage].uploaded, 0));
+    CU(c, cudaEventRecord(f->ev0, c->stream));
+    return spans_front(c, ch, ch.bytes, ch.hi - ch.lo, b->now_unix_ns, &out->path, meta);
+}
+
+// the ctmr_raw_out outputs of a chunk's entries [e0, e1) after the path's, on c's stream (not waited for)
+int raw_copy_back(ctmr_ctx* c, const Chunk& ch, const ctmr_raw_out* out) {
     FrontEnd* f = c->fe.get();
     cudaStream_t s = c->stream;
     const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0;
@@ -544,7 +551,14 @@ int Pages::copy_back(ctmr_ctx* c, const Chunk& ch) const {
         CHUNK_D2H(out->leaf_off, f->leaf_rel, 4);
         CHUNK_D2H(out->leaf_len, f->leaf_len_out, 4);
     }
-    CU(c, cudaStreamSynchronize(s));
+    return CTMR_OK;
+}
+
+// the front end's own outputs of a chunk, after the path's; waits for the chunk
+int Pages::copy_back(ctmr_ctx* c, const Chunk& ch) const {
+    const int rc = raw_copy_back(c, ch, out);
+    if (rc) return rc;
+    CU(c, cudaStreamSynchronize(c->stream));
     return CTMR_OK;
 }
 
@@ -574,6 +588,8 @@ struct Tiles {
     int copy_back(ctmr_ctx* c, const Chunk& ch) const;
     void completed(uint64_t tiles) const { out->tiles_done = tiles; }
     int stop(ctmr_ctx* c, const Chunk& ch) const;
+    void place(Chunk*, uint32_t) const {}
+    uint64_t entries() const { return done; }
 };
 
 // ctmr_process_tiles_tree's rules for the tiles of one log (the batch's tiles of log `log`; every tile without a log),
@@ -814,6 +830,204 @@ int Tiles::stop(ctmr_ctx* c, const Chunk& ch) const {
     for (uint32_t i = 0; i < out->n_missing; ++i) std::memcpy(out->missing_fp + 32ull * i, ch.missing[i].data(), 32);
     return fail(c, CTMR_E_UNKNOWN_ISSUER, "tile " + std::to_string(ch.hi) + " names a Chain[0] fingerprint that is not registered "
                                           "(ctmr_register_chain_certs, then call again from tiles_done)");
+}
+
+// ================================================================================================================
+// whole get-entries bodies: the units of a chunk are bodies.  The JSON kernels (ctmr_json.cu) leave the entries' spans in
+// the stage as Pages::upload puts them, escaped strings unescaped into the stage's spare half, and the rest is Pages'.
+// A chunk's entries are counted on the device, so their positions are given out after the front halves (place).
+// ================================================================================================================
+struct Bodies {
+    static constexpr const char* kTooLarge = "a single body exceeds the front end's staging budget";
+    static constexpr bool kStageHoldsLeaves = false;
+    const ctmr_body_batch* b;
+    ctmr_body_out* bo;
+    ctmr_raw_out* out;  // &bo->raw
+    uint64_t done = 0;    // entries that take their indices after a failure: the sum of body_max
+    uint64_t placed = 0;  // entries found so far (positions given out)
+    bool meta = false;
+    std::vector<uint64_t> tree_pos;  // unused: bodies have no tree forms
+    TreeState* tree_state = nullptr;
+
+    Bodies(const ctmr_body_batch* b_, ctmr_body_out* bo_) : b(b_), bo(bo_), out(bo_ ? &bo_->raw : nullptr) {}
+    int check(ctmr_ctx* c, const TreeArgs* tree);
+    uint64_t units() const { return b->n_bodies; }
+    uint64_t q_max(const ctmr_ctx*) const { return ~0ull; }  // fit keeps a chunk inside the budgets
+    int prepare(ctmr_ctx* c) const;
+    int fit(ctmr_ctx* c, uint64_t lo, uint64_t max_bodies, uint64_t* hi_out) const;
+    int upload(ctmr_ctx* c, Chunk& ch) const;
+    int front(ctmr_ctx* c, Chunk& ch) const;
+    int copy_back(ctmr_ctx* c, const Chunk& ch) const;
+    void completed(uint64_t) const { bo->n_entries = placed; }
+    int stop(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }
+    void place(Chunk* cur, uint32_t W) {  // dense, in member order
+        for (uint32_t r = 0; r < W; ++r) {
+            cur[r].e0 = placed;
+            placed += cur[r].db.n;
+            cur[r].e1 = placed;
+        }
+    }
+    uint64_t entries() const { return placed; }
+};
+
+int Bodies::check(ctmr_ctx* c, const TreeArgs*) {
+    if (!b || !bo) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (b->n_bodies && (!b->text || !b->body_off || !b->body_len || !b->body_max)) return fail(c, CTMR_E_INVALID, "null batch buffers");
+    const int rc = check_pem(c, &out->path);
+    if (rc) return rc;
+    uint64_t requested = 0;
+    for (uint64_t i = 0; i < b->n_bodies; ++i) {
+        if (b->body_off[i] > b->text_bytes || b->body_len[i] > b->text_bytes - b->body_off[i])
+            return fail(c, CTMR_E_INVALID, "body outside the text buffer");
+        requested += b->body_max[i];
+    }
+    done = requested;  // only a batch that passed every check takes indices
+    bo->n_entries = 0;
+    return CTMR_OK;
+}
+
+// the budgets, before any work: a body must fit a chunk on its own
+int Bodies::prepare(ctmr_ctx* c) const {
+    int rc = fe_prepare(c);
+    if (rc == CTMR_OK) rc = bodies_ensure(c);
+    if (rc) return rc;
+    c->fe->bd->json_ms = 0.f;
+    for (uint64_t i = 0; i < b->n_bodies; ++i)
+        if (b->body_len[i] > c->fe->cap_text / 2 || b->body_max[i] > c->fe->cap_entries) return fail(c, CTMR_E_BATCH_TOO_LARGE, kTooLarge);
+    return CTMR_OK;
+}
+
+// How many bodies starting at `lo` fit one chunk (at most max_bodies): half the character budget (the other half takes
+// the unescaped strings), and at most cap_entries bodies and requested entries
+int Bodies::fit(ctmr_ctx* c, uint64_t lo, uint64_t max_bodies, uint64_t* hi_out) const {
+    FrontEnd* f = c->fe.get();
+    uint64_t hi = lo, bytes = 0, slots = 0;
+    while (hi < b->n_bodies && hi - lo < max_bodies && hi - lo < f->cap_entries && bytes + b->body_len[hi] <= f->cap_text / 2 &&
+           slots + b->body_max[hi] <= f->cap_entries) {
+        bytes += b->body_len[hi];
+        slots += b->body_max[hi];
+        ++hi;
+    }
+    *hi_out = hi;
+    return CTMR_OK;
+}
+
+// bodies [lo, hi) into upload stage ch.stage, asynchronously on the copy stream: one copy when they lie in order, apart
+// and close together in the caller's text, packed back to back otherwise
+int Bodies::upload(ctmr_ctx* c, Chunk& ch) const {
+    FrontEnd* f = c->fe.get();
+    BodyState* bd = f->bd.get();
+    FeStage& st = f->stage[ch.stage];
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaStreamWaitEvent(f->copy_stream, st.consumed, 0));
+    ch.e0 = ch.e1 = 0;
+    const uint64_t cnt = ch.hi - ch.lo;
+    bool in_order = true;
+    uint64_t bytes = 0, min_off = ~0ull, max_end = 0;
+    for (uint64_t i = ch.lo; i < ch.hi; ++i) {
+        if (i > ch.lo && b->body_off[i] < b->body_off[i - 1] + b->body_len[i - 1]) in_order = false;
+        bytes += b->body_len[i];
+        min_off = std::min(min_off, b->body_off[i]);
+        max_end = std::max(max_end, b->body_off[i] + b->body_len[i]);
+    }
+    const bool one_copy = cnt && in_order && max_end - min_off <= f->cap_text / 2;
+    BodyDesc* h = bd->h_desc[ch.stage];
+    uint64_t w = 0;
+    uint32_t slot = 0;
+    if (!one_copy) st.pack.resize(bytes);
+    for (uint64_t i = 0; i < cnt; ++i) {
+        const uint64_t k = ch.lo + i;
+        BodyDesc& d = h[i];
+        d.text_off = b->body_off[k];
+        d.len = b->body_len[k];
+        d.max = b->body_max[k];
+        d.slot0 = slot;
+        d.pad = 0;
+        slot += d.max;
+        if (one_copy) {
+            d.staged_off = b->body_off[k] - min_off;
+        } else {
+            d.staged_off = w;
+            std::memcpy(st.pack.data() + w, b->text + b->body_off[k], d.len);
+            w += d.len;
+        }
+    }
+    ch.bytes = one_copy ? max_end - min_off : w;
+    if (ch.bytes)
+        CU(c, cudaMemcpyAsync(st.text + 16, one_copy ? b->text + min_off : st.pack.data(), ch.bytes, cudaMemcpyHostToDevice, f->copy_stream));
+    if (cnt) CU(c, cudaMemcpyAsync(bd->desc[ch.stage], h, cnt * sizeof(BodyDesc), cudaMemcpyHostToDevice, f->copy_stream));
+    CU(c, cudaEventRecord(st.uploaded, f->copy_stream));
+    return CTMR_OK;
+}
+
+// JSON kernels, one read-back of the entry count (a sync of its own: fe_decode's grid depends on it), then what Pages
+// runs on its spans
+int Bodies::front(ctmr_ctx* c, Chunk& ch) const {
+    FrontEnd* f = c->fe.get();
+    BodyState* bd = f->bd.get();
+    cudaStream_t s = c->stream;
+    CU(c, cudaSetDevice(c->device));
+    FeStage& st = f->stage[ch.stage];
+    CU(c, cudaStreamWaitEvent(s, st.uploaded, 0));
+    CU(c, cudaEventRecord(f->ev0, s));
+    const uint64_t nb = ch.hi - ch.lo;
+    uint64_t sparse = 0;
+    for (uint64_t i = 0; i < nb; ++i) sparse += bd->h_desc[ch.stage][i].max;
+    BodyParams p{};
+    p.text = st.text + 16;
+    p.spare = f->cap_text / 2;
+    p.bodies = bd->desc[ch.stage];
+    p.n_bodies = (uint32_t)nb;
+    p.starts = bd->starts; p.trans = bd->trans; p.carry = bd->carry; p.masks = bd->masks; p.stack = bd->stack;
+    p.body_status = bd->body_status; p.body_count = bd->body_count; p.body_base = bd->body_base;
+    for (int k = 0; k < 2; ++k) {
+        p.s_off[k] = bd->s_off[k]; p.s_len[k] = bd->s_len[k]; p.abs_off[k] = bd->abs_off[k]; p.raw_len[k] = bd->raw_len[k];
+    }
+    p.off[0] = st.leaf_off; p.len[0] = st.leaf_len; p.off[1] = st.extra_off; p.len[1] = st.extra_len;
+    p.s_esc = bd->s_esc; p.esc = bd->esc;
+    uint32_t count = 0;
+    CU(c, cudaEventRecord(bd->ev_json0, s));
+    uint32_t launches = 0;
+    CU(c, launch_json_bodies(p, ch.bytes, sparse, bd->temp, bd->temp_bytes, s, &launches));
+    CU(c, cudaEventRecord(bd->ev_json1, s));
+    f->launches += launches;
+    if (nb) CU(c, cudaMemcpyAsync(&count, bd->body_base + nb, 4, cudaMemcpyDeviceToHost, s));
+    CU(c, cudaStreamSynchronize(s));
+    float ms = 0.f;
+    CU(c, cudaEventElapsedTime(&ms, bd->ev_json0, bd->ev_json1));
+    bd->json_ms += ms;
+    if (count > sparse) return fail(c, CTMR_E_CUDA, "bodies: more entries found than requested");
+    return spans_front(c, ch, f->cap_text, count, b->now_unix_ns, &out->path, meta);
+}
+
+int Bodies::copy_back(ctmr_ctx* c, const Chunk& ch) const {
+    FrontEnd* f = c->fe.get();
+    BodyState* bd = f->bd.get();
+    cudaStream_t s = c->stream;
+    int rc = raw_copy_back(c, ch, out);
+    if (rc) return rc;
+    const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0, nb = ch.hi - ch.lo;
+    if (cnt) {
+        CHUNK_D2H(bo->leaf_input_off, bd->abs_off[0], 8);
+        CHUNK_D2H(bo->leaf_input_len, bd->raw_len[0], 4);
+        CHUNK_D2H(bo->extra_data_off, bd->abs_off[1], 8);
+        CHUNK_D2H(bo->extra_data_len, bd->raw_len[1], 4);
+        CHUNK_D2H(bo->escaped, bd->esc, 1);
+    }
+    std::vector<uint8_t> status(nb);
+    std::vector<uint32_t> count(nb), base(nb);
+    if (nb) {
+        CU(c, cudaMemcpyAsync(status.data(), bd->body_status, nb, cudaMemcpyDeviceToHost, s));
+        CU(c, cudaMemcpyAsync(count.data(), bd->body_count, nb * 4, cudaMemcpyDeviceToHost, s));
+        CU(c, cudaMemcpyAsync(base.data(), bd->body_base, nb * 4, cudaMemcpyDeviceToHost, s));
+    }
+    CU(c, cudaStreamSynchronize(s));
+    for (uint64_t i = 0; i < nb; ++i) {
+        if (bo->body_status) bo->body_status[ch.lo + i] = status[i];
+        if (bo->body_entries) bo->body_entries[ch.lo + i] = count[i];
+        if (bo->body_first) bo->body_first[ch.lo + i] = ch.e0 + base[i];
+    }
+    return CTMR_OK;
 }
 
 #undef CHUNK_D2H
@@ -1133,6 +1347,7 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
             cur[0].stopped = false;
             cur[0].dout = chunk_path_out(m[0]->fe.get(), po, fm.meta);
         }
+        fm.place(cur, W);
         for (uint32_t r = 0; r < W; ++r) {
             if (stop < W) {
                 cur[r].cut(0, 0);  // after a stop in an earlier member: its entries must not touch the tables
@@ -1160,7 +1375,7 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
         if (last || (!pc.on && stop < W)) break;
     }
     if (stop < W) fm.done = held.e1;
-    if (po->pem) po->pem_off[fm.done] = pem_base;
+    if (po->pem) po->pem_off[fm.entries()] = pem_base;
     for (uint32_t r = 0; r < W && !local; ++r) {  // a table that filled up during the completed chunks is this call's error
         *failed = m[r];
         rc = ctmr_check_device(m[r], nullptr);
@@ -1209,7 +1424,7 @@ int front_end_call(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format fm, co
     ctmr_ctx* failed = nullptr;
     PeerCall pc;  // a collective call takes pc.span indices once the ranks agreed, whatever happens after
     const int rc = process_members(m, W, next_index, fm, tree, pc, &failed);
-    *next_index += pc.on ? pc.span : fm.done;
+    *next_index += pc.on ? pc.span : rc == CTMR_OK ? fm.entries() : fm.done;
     for (uint32_t r = 0; r < W; ++r) {
         if (m[r]->fe && m[r]->fe->tree) {
             m[r]->fe->tree->active = false;
@@ -1308,6 +1523,23 @@ int ctmr_process_tiles(ctmr_ctx* c, const ctmr_tile_batch* b, ctmr_tile_out* out
 int ctmr_group_process_tiles(ctmr_group* g, const ctmr_tile_batch* b, ctmr_tile_out* out) {
     if (!g || g->m.empty()) return CTMR_E_INVALID;
     return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Tiles(b, out), nullptr, g);
+}
+
+int ctmr_process_raw_bodies(ctmr_ctx* c, const ctmr_body_batch* b, ctmr_body_out* out) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_raw_bodies");
+    return front_end_call(&c, 1, &c->next_index, Bodies(b, out), nullptr, nullptr);
+}
+
+int ctmr_group_process_raw_bodies(ctmr_group* g, const ctmr_body_batch* b, ctmr_body_out* out) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Bodies(b, out), nullptr, g);
+}
+
+int ctmr_bodies_profile_last(ctmr_ctx* c, float* json_ms) {
+    if (!c || !c->fe || !c->fe->bd) return fail(c, CTMR_E_INVALID, "no ctmr_process_raw_bodies call to report");
+    if (json_ms) *json_ms = c->fe->bd->json_ms;
+    return CTMR_OK;
 }
 
 int ctmr_process_raw_tree(ctmr_ctx* c, const ctmr_raw_batch* b, ctmr_raw_out* out, ctmr_tree* tree) {
@@ -1434,6 +1666,38 @@ int tiles_ensure(ctmr_ctx* c) {
     CU(c, cudaMemsetAsync(tl->fp_dev, 0, (tl->fp_mask + 1) * sizeof(FpSlot), c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     f->tl = std::move(tl);
+    return CTMR_OK;
+}
+
+int bodies_ensure(ctmr_ctx* c) {
+    FrontEnd* f = c->fe.get();
+    if (f->bd) return CTMR_OK;
+    std::unique_ptr<BodyState> bd(new (std::nothrow) BodyState());
+    if (!bd) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    const uint64_t E = f->cap_entries, blocks = (f->cap_text / 2 + 63) / 64 + 1;
+    for (int k = 0; k < 2; ++k) {
+        CU(c, alloc(bd->desc[k], E));
+        CU(c, alloc(bd->h_desc[k], E));
+        CU(c, alloc(bd->s_off[k], E));
+        CU(c, alloc(bd->s_len[k], E));
+        CU(c, alloc(bd->abs_off[k], E));
+        CU(c, alloc(bd->raw_len[k], E));
+    }
+    CU(c, alloc(bd->starts, blocks + 1));
+    CU(c, alloc(bd->trans, blocks));
+    CU(c, alloc(bd->carry, blocks));
+    CU(c, alloc(bd->masks, blocks));
+    CU(c, alloc(bd->stack, blocks * 2 + 2));  // a bit per staged byte
+    CU(c, alloc(bd->body_status, E));
+    CU(c, alloc(bd->body_count, E + 1));
+    CU(c, alloc(bd->body_base, E + 1));
+    CU(c, alloc(bd->s_esc, E));
+    CU(c, alloc(bd->esc, E));
+    bd->temp_bytes = json_scan_temp_bytes(blocks, E);
+    CU(c, alloc(bd->temp, bd->temp_bytes ? bd->temp_bytes : 16));
+    CU(c, create(bd->ev_json0, cudaEventDefault));
+    CU(c, create(bd->ev_json1, cudaEventDefault));
+    f->bd = std::move(bd);
     return CTMR_OK;
 }
 

@@ -276,6 +276,53 @@ cudaError_t launch_fe_issuer(const FeParams& p, const IssuerCertTable& tab, uint
 cudaError_t launch_fe_tbs(const FeParams& p, cudaStream_t s);
 cudaError_t launch_fe_finish(const FeParams& p, const uint8_t* status, cudaStream_t s);
 
+// ---- whole get-entries response bodies (ctmr_json.cu, ctmr_process_raw_bodies) --------------------------------------
+// one body of a chunk as uploaded
+struct BodyDesc {
+    uint64_t staged_off;  // in BodyParams.text
+    uint64_t text_off;    // in ctmr_body_batch.text
+    uint32_t len;
+    uint32_t max;         // entries requested
+    uint32_t slot0;       // first of the body's `max` slots of the walk's spans (sum of max over earlier bodies)
+    uint32_t pad;
+};
+static_assert(sizeof(BodyDesc) == 32, "BodyDesc layout");
+
+// per 64-byte block of the staged text: tokens outside strings (structural characters, opening quotes, bytes of
+// scalars), unescaped quotes, backslashes, and characters that make a string invalid
+struct BlockMasks {
+    unsigned long long tok, quote, bs, bad;
+};
+
+struct BodyParams {
+    const uint8_t* text;       // staged bodies (16 bytes of slack before, 64 after the stage)
+    uint64_t spare;            // unescaped strings go to text + spare + their offset
+    const BodyDesc* bodies;    // [n_bodies]
+    uint32_t n_bodies;
+    unsigned long long* starts;  // [blocks + 1] body start bits
+    uint8_t* trans;            // [blocks] carry function of each block (4 x 2 bits)
+    uint8_t* carry;            // [blocks] composed functions of the blocks before
+    BlockMasks* masks;         // [blocks]
+    uint32_t* stack;           // container kinds deeper than 63 levels: bit staged_off + depth
+    uint8_t* body_status;      // [n_bodies] CTMR_BODY_*
+    uint32_t* body_count;      // [n_bodies + 1] entries of OK bodies (0 otherwise)
+    uint32_t* body_base;       // [n_bodies + 1] exclusive scan of body_count
+    uint64_t* s_off[2];        // [sum of max] the walk's spans by body slot, staged offsets (~0: absent or null)
+    uint32_t* s_len[2];
+    uint8_t* s_esc;
+    uint64_t* off[2];          // [entries] dense: where fe_decode reads each string (leaf_input, extra_data)
+    uint32_t* len[2];
+    uint64_t* abs_off[2];      // [entries] dense: the string's offset in the caller's text, its escaped length
+    uint32_t* raw_len[2];
+    uint8_t* esc;              // [entries] bit 0: leaf_input held a backslash, bit 1: extra_data did
+};
+
+size_t json_scan_temp_bytes(uint64_t blocks, uint64_t bodies);
+// classify, walk, compact and unescape the n_bodies bodies of `bytes` staged bytes with `sparse` = sum of max slots;
+// the entry count is left in body_base[n_bodies].  *launches: kernels issued.
+cudaError_t launch_json_bodies(const BodyParams& p, uint64_t bytes, uint64_t sparse, void* temp, size_t temp_bytes, cudaStream_t s,
+                               uint32_t* launches);
+
 // ---- static-ct-api data tiles (ctmr_tiles.cu, ctmr_process_tiles) ------------------------------------------------
 // one tile of a chunk as uploaded: where it sits in the staging buffer and in the caller's data
 struct TileDesc {

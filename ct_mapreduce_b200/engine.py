@@ -145,6 +145,34 @@ class RawBatchResult:
         self.trees = None   # [LogTree] after the batch, when the call was given trees= (one per log)
 
 
+class BodiesResult(RawBatchResult):
+    """Outputs of ctmr_process_raw_bodies (ctmr_body_out): per entry found, what ctmr_process_raw gives plus where its
+    strings lie in the text; per body, its status and its entries."""
+
+    def __init__(self, cap: int, n_bodies: int, want_sha: bool = True, want_meta: bool = False):
+        super().__init__(cap, want_sha, want_meta)
+        self.body_status = np.zeros(n_bodies, np.uint8)
+        self.body_first = np.zeros(n_bodies, np.uint64)
+        self.body_entries = np.zeros(n_bodies, np.uint32)
+        self.leaf_input_off = np.zeros(cap, np.uint64)
+        self.leaf_input_len = np.zeros(cap, np.uint32)
+        self.extra_data_off = np.zeros(cap, np.uint64)
+        self.extra_data_len = np.zeros(cap, np.uint32)
+        self.escaped = np.zeros(cap, np.uint8)
+        self.n_entries = 0
+
+    def trim(self, n: int):
+        """keeps the n entries the call wrote"""
+        self.n_entries = n
+        p, cap = self.path, self.leaf_input_off.shape[0]
+        for obj in (self, p):
+            for k, v in list(vars(obj).items()):
+                if isinstance(v, np.ndarray) and not k.startswith("body_") and k not in ("pem", "pem_off") and v.shape[:1] == (cap,):
+                    setattr(obj, k, v[:n])
+        if p.pem_off is not None:
+            p.pem_off = p.pem_off[:n + 1]
+
+
 class TileBatchResult(RawBatchResult):
     """Outputs of ctmr_process_tiles (ctmr_tile_out)."""
 
@@ -331,6 +359,46 @@ class GpuCertDatabase:
 
     def _process_raw_trees_fn(self):
         return self._lib.ctmr_process_raw_trees
+
+    def store_raw_bodies(self, text, body_off, body_len, body_max, now_unix_ns: int, want_sha: bool = True, want_meta: bool = False,
+                         want_pem: bool = False) -> "BodiesResult":
+        """Whole get-entries response bodies (body b is text[body_off[b]:body_off[b] + body_len[b]], body_max[b] the entries
+        requested) through ctmr_process_raw_bodies: the GPU finds the entries with encoding/json's rules, then does what
+        store_raw_entries does with them.  The per-entry arrays of the result hold the n_entries entries found, in (body,
+        position) order; r.body_status / r.body_first / r.body_entries say which are whose."""
+        with self._peer_refusal():
+            text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else np.ascontiguousarray(text, np.uint8)
+            body_off = np.ascontiguousarray(body_off, np.uint64)
+            body_len, body_max = np.ascontiguousarray(body_len, np.uint32), np.ascontiguousarray(body_max, np.uint32)
+            nb = body_off.size
+        cap = int(body_max.sum())
+        r = BodiesResult(cap, nb, want_sha, want_meta)
+        p = r.path
+        o = capi.BodyOut()
+        o.raw.path = capi.Out(capi.ptr(p.status), capi.ptr(p.sha256) if want_sha else None, capi.ptr(p.exp_hour), capi.ptr(p.serial_off),
+                              capi.ptr(p.serial_len), capi.ptr(p.was_unknown), capi.ptr(p.first_issuer_hour),
+                              *([capi.ptr(p.issuer_name_off), capi.ptr(p.issuer_name_len), capi.ptr(p.crldp_off), capi.ptr(p.crldp_len),
+                                 capi.ptr(p.first_issuer_dn), capi.ptr(p.first_crldp)] if want_meta else [None] * 6))
+        for name in ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_src", "leaf_off", "leaf_len"):
+            setattr(o.raw, name, capi.ptr(getattr(r, name)))
+        for name in ("body_status", "body_first", "body_entries", "leaf_input_off", "leaf_input_len", "extra_data_off",
+                     "extra_data_len", "escaped"):
+            setattr(o, name, capi.ptr(getattr(r, name)))
+        if want_pem:
+            _attach_pem(o.raw.path, p, cap, int(body_len.sum()) // 4 * 3)
+        b = capi.BodyBatch(capi.ptr(text), text.size, capi.ptr(body_off), capi.ptr(body_len), capi.ptr(body_max), nb, now_unix_ns)
+        self._check(self._process_raw_bodies_fn()(self._h, C.byref(b), C.byref(o)))
+        r.trim(int(o.n_entries))
+        return r
+
+    def _process_raw_bodies_fn(self):
+        return self._lib.ctmr_process_raw_bodies
+
+    def bodies_profile_last(self) -> float:
+        """Milliseconds of the JSON kernels in the last store_raw_bodies call, part of frontend_ms."""
+        a = C.c_float(0)
+        self._check(self._lib.ctmr_bodies_profile_last(self._h, C.byref(a)))
+        return a.value
 
     # ------------------------------------------------------------------ static-ct-api data tiles (include/ctmr_frontend.h)
     def register_chain_certs(self, blob, offsets):
@@ -647,6 +715,9 @@ class GpuCertGroup(GpuCertDatabase):
 
     def _process_raw_fn(self):
         return self._lib.ctmr_group_process_raw
+
+    def _process_raw_bodies_fn(self):
+        return self._lib.ctmr_group_process_raw_bodies
 
     def _process_tiles_fn(self):
         return self._lib.ctmr_group_process_tiles

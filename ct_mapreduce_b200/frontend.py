@@ -1,8 +1,9 @@
 """Host side of the CT wire-format front end (include/ctmr_frontend.h, SURVEY.md §8(f)-2).
 
-The GPU takes the base64 strings of RFC 6962 §4.6 get-entries responses as they came off the wire; the only
-thing left on the host is to say WHERE the strings are.  `find_entry_spans` does that for one response
-body: it stands in for the struct decode that ct-go's jsonclient performs into ct.GetEntriesResponse
+The GPU takes the base64 strings of RFC 6962 §4.6 get-entries responses as they came off the wire; with
+ctmr_process_raw the only thing left on the host is to say WHERE the strings are, and with ctmr_process_raw_bodies
+(GpuCertDatabase.store_raw_bodies) not even that: the GPU finds them in the whole bodies with encoding/json's rules.
+`find_entry_spans` does it on the host for one response body: it stands in for the struct decode that ct-go's jsonclient performs into ct.GetEntriesResponse
 (`{"entries":[{"leaf_input":"...","extra_data":"..."}, ...]}`) under LogClient.GetRawEntries
 (reference cmd/ct-fetch/ct-fetch.go:424) -- minus the base64 decode, which moved to the GPU.
 

@@ -98,6 +98,73 @@ int ctmr_process_raw(ctmr_ctx* ctx, const ctmr_raw_batch* batch, ctmr_raw_out* o
  * the outputs equal those of ctmr_process_raw on one GPU for the same pages. */
 int ctmr_group_process_raw(ctmr_group* g, const ctmr_raw_batch* batch, ctmr_raw_out* out);
 
+/* ---- whole get-entries response bodies ----------------------------------------------------------------------------
+ * The HTTP bodies as they came off the wire: the GPU validates each body as JSON and finds its entries with the rules
+ * of Go 1.13 encoding/json decoding it into ct-go's GetEntriesResponse (Unmarshal runs checkValid over the whole body
+ * first; reference cmd/ct-fetch/ct-fetch.go:424):
+ *   - validity (RFC 8259 as Go's scanner checks it): structure, the literals, number syntax, the escapes
+ *     \" \\ \/ \b \f \n \r \t \uXXXX, no raw byte below 0x20 inside a string, only space, tab, LF and CR as whitespace,
+ *     nothing but whitespace after the value.  An empty body or a UTF-8 BOM is invalid; invalid UTF-8 is not;
+ *   - types: the top level is an object or null (no entries); "entries" is an array or null; an element is an object or
+ *     null (an entry with both strings empty); "leaf_input" / "extra_data" are strings or null (empty).  Members of any
+ *     other name, at any depth and of any type, are skipped;
+ *   - keys are unescaped before they match: "leaf_input" and "extra_data" ASCII case-insensitively ('_' exactly),
+ *     "entries" as encoding/json's equalFoldRight does ('s' also matches U+017F).  Inside an element the last of a
+ *     repeated key wins and a missing key means empty;
+ *   - a string holding escapes is unescaped, and '\r' / '\n' are dropped as base64.StdEncoding skips them, before the
+ *     decode; a non-ASCII character makes the string CTMR_FE_BAD_BASE64.
+ * The entries of the OK bodies, in (body, position) order, then go through exactly what ctmr_process_raw does with
+ * their strings. */
+enum {
+    CTMR_BODY_OK = 0,
+    CTMR_BODY_BAD_JSON = 1,          /* checkValid fails */
+    CTMR_BODY_BAD_TYPE = 2,          /* valid JSON that does not fit GetEntriesResponse */
+    CTMR_BODY_TOO_MANY = 3,          /* more entries than body_max */
+    CTMR_BODY_REPEATED_ENTRIES = 4   /* a second top-level "entries" member: encoding/json decodes the later array into the
+                                        elements the earlier one filled; decode such a body on the host (ctmr_process_raw) */
+};
+
+/* n_bodies bodies; HOST buffers.  Body b is text[body_off[b] .. body_off[b] + body_len[b]); bodies may lie anywhere in
+ * text, also back to back. */
+typedef struct ctmr_body_batch {
+    const uint8_t* text;
+    uint64_t text_bytes;
+    const uint64_t* body_off;  /* [n_bodies] */
+    const uint32_t* body_len;  /* [n_bodies] */
+    const uint32_t* body_max;  /* [n_bodies] entries requested (end - start + 1 of the get-entries call) */
+    uint64_t n_bodies;
+    int64_t now_unix_ns;
+} ctmr_body_batch;
+
+/* Caller-allocated outputs; any pointer may be NULL.  Per-entry arrays hold sum of body_max entries, of which
+ * [0, n_entries) are written (raw.path.pem_off n_entries + 1). */
+typedef struct ctmr_body_out {
+    ctmr_raw_out raw;          /* as ctmr_process_raw writes them for the entries found */
+    uint8_t* body_status;      /* [n_bodies] CTMR_BODY_*; a body that is not OK contributes no entry */
+    uint64_t* body_first;      /* [n_bodies] position of the body's first entry in the per-entry arrays */
+    uint32_t* body_entries;    /* [n_bodies] */
+    uint64_t* leaf_input_off;  /* [entries] the string as found: offset in text (quotes excluded) and length, escapes */
+    uint32_t* leaf_input_len;  /*           included, so that the host can cut a new certificate out of its own text */
+    uint64_t* extra_data_off;  /*           (0 and 0 for a missing or null string) */
+    uint32_t* extra_data_len;
+    uint8_t* escaped;          /* [entries] bit 0: leaf_input held an escape, bit 1: extra_data did */
+    uint64_t n_entries;        /* written */
+} ctmr_body_out;
+
+/* Find the entries of every body, then decode + frame + identify issuers + map + reduce them as ctmr_process_raw does.
+ * Synchronous.  The entries take consecutive global indices in (body, position) order after those of earlier calls;
+ * a successful call advances the next index by n_entries.  After a failure once a chunk has reached the path, it
+ * advances by the sum of body_max, so that a retry never reuses an index.  A body longer than half the front end's
+ * character budget, or with more requested entries than its entry budget, is CTMR_E_BATCH_TOO_LARGE before any work.
+ * On a group member this call is refused; on a ctx attached to peers it is collective, with the rules of the front-end
+ * calls below (chunks of at most E entries requested). */
+int ctmr_process_raw_bodies(ctmr_ctx* ctx, const ctmr_body_batch* batch, ctmr_body_out* out);
+/* The same on every GPU of a group: the outputs equal those of ctmr_process_raw_bodies on one GPU. */
+int ctmr_group_process_raw_bodies(ctmr_group* g, const ctmr_body_batch* batch, ctmr_body_out* out);
+/* CUDA-event time of the JSON kernels (classify, walk, compaction, unescape) in the last bodies call on this ctx, summed
+ * over its chunks, in milliseconds: a part of the frontend_ms that ctmr_frontend_profile_last reports */
+int ctmr_bodies_profile_last(ctmr_ctx* ctx, float* json_ms);
+
 /* CUDA-event timings of the last front-end call (raw or tiles): front-end kernels (decode, framing, issuer
  * identification; for tiles the split, framing, fingerprint look-up and leaf hashes; for the tree forms also the leaf
  * hashes and the Merkle fold) and the map/reduce that
@@ -271,8 +338,9 @@ int ctmr_group_process_tiles_trees(ctmr_group* g, const ctmr_tile_batch* batch, 
                                    const uint32_t* tile_log /* [n_tiles] */, ctmr_tree* trees, uint32_t n_trees);
 
 /* ---- one process per GPU: the front end as a collective call ------------------------------------------------------------
- * On a ctx attached to peers (ctmr_peer_attach, ctmr.h, world > 1) ctmr_process_raw, ctmr_process_tiles,
- * ctmr_process_raw_tree, ctmr_process_tiles_tree, ctmr_process_raw_trees and ctmr_process_tiles_trees are COLLECTIVE.
+ * On a ctx attached to peers (ctmr_peer_attach, ctmr.h, world > 1) ctmr_process_raw, ctmr_process_raw_bodies,
+ * ctmr_process_tiles, ctmr_process_raw_tree, ctmr_process_tiles_tree, ctmr_process_raw_trees and ctmr_process_tiles_trees
+ * are COLLECTIVE.
  * Each rank passes its own batch, and each front-end call on one rank must meet a front-end call on every other rank.
  * The entry points may differ between the ranks of one call (pages on one rank, tiles with trees on another): their
  * collective steps are the same.  A front-end call met by ctmr_process_batch, ctmr_process_device or any other

@@ -38,6 +38,8 @@ EXPORTS = [
     "ctmr_tiles_profile_last", "ctmr_process_raw_tree", "ctmr_process_tiles_tree", "ctmr_process_raw_trees",
     "ctmr_process_tiles_trees", "ctmr_group_process_raw_tree", "ctmr_group_process_tiles_tree", "ctmr_group_process_raw_trees",
     "ctmr_group_process_tiles_trees", "ctmr_process_raw_bodies", "ctmr_group_process_raw_bodies", "ctmr_bodies_profile_last",
+    "ctmr_process_raw_bodies_tree", "ctmr_process_raw_bodies_trees", "ctmr_group_process_raw_bodies_tree",
+    "ctmr_group_process_raw_bodies_trees",
     # several GPUs: one process (group) / one process per GPU (peer)
     "ctmr_group_create", "ctmr_group_destroy", "ctmr_group_last_error", "ctmr_group_size", "ctmr_group_member",
     "ctmr_group_process_batch", "ctmr_group_issuer_counts", "ctmr_group_set_cardinality", "ctmr_group_status_counters",
@@ -229,6 +231,10 @@ def load():
     L.ctmr_process_raw_bodies.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut)]
     L.ctmr_group_process_raw_bodies.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut)]
     L.ctmr_bodies_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
+    L.ctmr_process_raw_bodies_tree.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, C.POINTER(Tree)]
+    L.ctmr_process_raw_bodies_trees.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, vp, vp, u32]
+    L.ctmr_group_process_raw_bodies_tree.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, C.POINTER(Tree)]
+    L.ctmr_group_process_raw_bodies_trees.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, vp, vp, u32]
     L.ctmr_group_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_synth_tiles_host.argtypes = [C.POINTER(SynthCfg), u64, u64, vp, vp, u64, vp, vp]
     L.ctmr_synth_tiles_host.restype = u64

@@ -188,9 +188,20 @@ struct TileState {
     std::unordered_map<std::string, uint32_t> fp_memo;
 };
 
+// the tree forms of the bodies call (ctmr_process_raw_bodies_tree(s)): each body's status and entry count, read back with
+// the chunk's entry count, and the fold windows of the chunk's bodies ([cap_entries] each).  Allocated on the first such
+// call.
+struct BodyFoldState {
+    HostBuf<uint8_t> h_status;
+    HostBuf<uint32_t> h_count;
+    HostBuf<BodyWindow> h_win;
+    DevBuf<BodyWindow> win;
+};
+
 // whole get-entries bodies (ctmr_process_raw_bodies): the JSON kernels' buffers for a chunk of up to cap_text / 2 bytes
 // and cap_entries bodies and requested entries.  Allocated on the first bodies call.
 struct BodyState {
+    std::unique_ptr<BodyFoldState> fold;  // bodies_fold_ensure
     DevBuf<BodyDesc> desc[2];  // per upload stage: the chunk's bodies, device and pinned host
     HostBuf<BodyDesc> h_desc[2];
     DevBuf<unsigned long long> starts;
@@ -451,6 +462,7 @@ int frontend_ensure(ctmr_ctx* c);   // allocates the front end's buffers on firs
 int tiles_ensure(ctmr_ctx* c);      // ... and the tile buffers + fingerprint table (ctmr_frontend_api.cu), after frontend_ensure
 int tiles_clear_fingerprints(ctmr_ctx* c);
 int bodies_ensure(ctmr_ctx* c);     // ... and the JSON buffers of ctmr_process_raw_bodies (ctmr_frontend_api.cu), after frontend_ensure
+int bodies_fold_ensure(ctmr_ctx* c);  // ... and the fold windows of its tree forms, after bodies_ensure
 int ensure_scratch(ctmr_ctx* c, uint64_t n);
 int ensure_device_path(ctmr_ctx* c, uint64_t n);   // what ctmr_process_device needs for n entries
 uint64_t device_round_entries(uint64_t n, uint32_t rounds);   // E of a ctmr_process_device call cut into `rounds` rounds

@@ -99,12 +99,14 @@ int fe_prepare(ctmr_ctx* c) {
 
 // ---- the logs' Merkle trees (ctmr_process_*_tree, ctmr_process_*_trees) ------------------------------------------------
 // The trees of a tree call: the one-tree forms pass one tree and no log (every entry is the tree's); the routed forms
-// pass n trees and the tree of every entry (pages) or tile (tiles), CTMR_NO_TREE for none.
+// pass n trees and the tree of every entry (pages), tile (tiles) or body (bodies), CTMR_NO_TREE for none.  Bodies also
+// pass the log position of every body's first entry (the start of its get-entries request).
 struct TreeArgs {
     ctmr_tree* trees = nullptr;
     uint32_t n = 0;
     const uint32_t* log = nullptr;
     bool routed = false;
+    const uint64_t* start = nullptr;
 };
 
 // the arguments of a routed call before the format's own rules: `units` entries or tiles, and their trees
@@ -339,7 +341,8 @@ struct Pages {
     int copy_back(ctmr_ctx* c, const Chunk& ch) const;
     void completed(uint64_t) const {}
     int stop(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }  // a page chunk never stops
-    void place(Chunk*, uint32_t) const {}  // entry positions are known at upload
+    void place(ctmr_ctx**, Chunk*, uint32_t) const {}  // entry positions are known at upload
+    int fold(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }  // folded in the front half
     uint64_t entries() const { return done; }
 };
 
@@ -588,7 +591,8 @@ struct Tiles {
     int copy_back(ctmr_ctx* c, const Chunk& ch) const;
     void completed(uint64_t tiles) const { out->tiles_done = tiles; }
     int stop(ctmr_ctx* c, const Chunk& ch) const;
-    void place(Chunk*, uint32_t) const {}
+    void place(ctmr_ctx**, Chunk*, uint32_t) const {}
+    int fold(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }  // folded in the front half
     uint64_t entries() const { return done; }
 };
 
@@ -836,6 +840,13 @@ int Tiles::stop(ctmr_ctx* c, const Chunk& ch) const {
 // whole get-entries bodies: the units of a chunk are bodies.  The JSON kernels (ctmr_json.cu) leave the entries' spans in
 // the stage as Pages::upload puts them, escaped strings unescaped into the stage's spare half, and the rest is Pages'.
 // A chunk's entries are counted on the device, so their positions are given out after the front halves (place).
+//
+// The tree forms (ctmr_process_raw_bodies_tree(s)): the entries of body b are log positions start[b], start[b] + 1, ...
+// of its log, known only once the front half has counted them, and a log may answer short, so that the bodies of a
+// pipelining client leave gaps or overlap.  The front half hashes the leaves and reads back each body's status and count
+// with the chunk's entry count; place walks the round's bodies in member order against each tree's end (the call's tree
+// state: member 0's `next`, and `stopped`) and leaves per body a window of the entries that fold; fold expands the
+// windows into the chunk's order on the device (body_fold_order) and folds, on each member's stream.
 // ================================================================================================================
 struct Bodies {
     static constexpr const char* kTooLarge = "a single body exceeds the front end's staging budget";
@@ -846,8 +857,11 @@ struct Bodies {
     uint64_t done = 0;    // entries that take their indices after a failure: the sum of body_max
     uint64_t placed = 0;  // entries found so far (positions given out)
     bool meta = false;
-    std::vector<uint64_t> tree_pos;  // unused: bodies have no tree forms
-    TreeState* tree_state = nullptr;
+    std::vector<uint64_t> tree_pos;  // tree calls: each tree's size at the start of the call, its first end
+    TreeState* tree_state = nullptr;  // tree calls: the call's tree state, member 0's (process_members)
+    const uint32_t* log = nullptr;    // tree calls: the log of each body (NULL: every body is tree 0's)
+    const uint64_t* start = nullptr;  // tree calls: the log position of each body's first entry
+    std::vector<uint8_t> stopped;     // tree calls: the trees whose fold has stopped for this call
 
     Bodies(const ctmr_body_batch* b_, ctmr_body_out* bo_) : b(b_), bo(bo_), out(bo_ ? &bo_->raw : nullptr) {}
     int check(ctmr_ctx* c, const TreeArgs* tree);
@@ -860,26 +874,55 @@ struct Bodies {
     int copy_back(ctmr_ctx* c, const Chunk& ch) const;
     void completed(uint64_t) const { bo->n_entries = placed; }
     int stop(ctmr_ctx*, const Chunk&) const { return CTMR_OK; }
-    void place(Chunk* cur, uint32_t W) {  // dense, in member order
-        for (uint32_t r = 0; r < W; ++r) {
-            cur[r].e0 = placed;
-            placed += cur[r].db.n;
-            cur[r].e1 = placed;
-        }
-    }
+    void place(ctmr_ctx** m, Chunk* cur, uint32_t W);
+    int fold(ctmr_ctx* c, const Chunk& ch) const;
     uint64_t entries() const { return placed; }
+    bool folds() const { return tree_state && tree_state->active; }
 };
 
-int Bodies::check(ctmr_ctx* c, const TreeArgs*) {
-    if (!b || !bo) return fail(c, CTMR_E_INVALID, "bad argument");
+// the tree rules of a tree call, per log in batch order: starts that never decrease, a first body that starts at or
+// below the tree's size, and starts whose requested entries do not wrap around 2^64
+int body_tree_args(ctmr_ctx* c, const ctmr_body_batch* b, const TreeArgs* tree) {
+    const uint64_t nb = b->n_bodies;
+    if (tree->routed) {
+        const int rc = tree_route_args(c, tree, nb);
+        if (rc) return rc;
+    }
+    if (nb && !tree->start) return fail(c, CTMR_E_INVALID, "trees: null body starts");
+    std::vector<uint64_t> prev(tree->n, 0);
+    std::vector<uint8_t> seen(tree->n, 0);
+    for (uint64_t i = 0; i < nb; ++i) {
+        const uint32_t l = tree->routed ? tree->log[i] : 0;
+        if (l == CTMR_NO_TREE) continue;
+        const uint64_t s = tree->start[i];
+        if (s > ~0ull - b->body_max[i]) return fail(c, CTMR_E_INVALID, "trees: a body's start + its requested entries wraps around 2^64");
+        if (!seen[l] && s > tree->trees[l].size) return fail(c, CTMR_E_INVALID, "trees: a log's first body starts after its tree's size");
+        if (seen[l] && s < prev[l]) return fail(c, CTMR_E_INVALID, "trees: a log's body starts decrease");
+        seen[l] = 1;
+        prev[l] = s;
+    }
+    return CTMR_OK;
+}
+
+int Bodies::check(ctmr_ctx* c, const TreeArgs* tree) {
+    if (!b || !bo || (tree && !tree->routed && !tree->trees)) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n_bodies && (!b->text || !b->body_off || !b->body_len || !b->body_max)) return fail(c, CTMR_E_INVALID, "null batch buffers");
-    const int rc = check_pem(c, &out->path);
+    int rc = check_pem(c, &out->path);
     if (rc) return rc;
     uint64_t requested = 0;
     for (uint64_t i = 0; i < b->n_bodies; ++i) {
         if (b->body_off[i] > b->text_bytes || b->body_len[i] > b->text_bytes - b->body_off[i])
             return fail(c, CTMR_E_INVALID, "body outside the text buffer");
         requested += b->body_max[i];
+    }
+    if (tree) {
+        rc = body_tree_args(c, b, tree);
+        if (rc) return rc;
+        log = tree->routed ? tree->log : nullptr;
+        start = tree->start;
+        tree_pos.resize(tree->n);
+        for (uint32_t d = 0; d < tree->n; ++d) tree_pos[d] = tree->trees[d].size;
+        stopped.assign(tree->n, 0);
     }
     done = requested;  // only a batch that passed every check takes indices
     bo->n_entries = 0;
@@ -890,6 +933,7 @@ int Bodies::check(ctmr_ctx* c, const TreeArgs*) {
 int Bodies::prepare(ctmr_ctx* c) const {
     int rc = fe_prepare(c);
     if (rc == CTMR_OK) rc = bodies_ensure(c);
+    if (rc == CTMR_OK && !tree_pos.empty()) rc = bodies_fold_ensure(c);
     if (rc) return rc;
     c->fe->bd->json_ms = 0.f;
     for (uint64_t i = 0; i < b->n_bodies; ++i)
@@ -960,8 +1004,9 @@ int Bodies::upload(ctmr_ctx* c, Chunk& ch) const {
     return CTMR_OK;
 }
 
-// JSON kernels, one read-back of the entry count (a sync of its own: fe_decode's grid depends on it), then what Pages
-// runs on its spans
+// JSON kernels, one read-back of the entry count (a sync of its own: fe_decode's grid depends on it; a tree call reads
+// each body's status and count with it), then what Pages runs on its spans; a tree call then hashes the leaves, which
+// fold once place has given out their positions
 int Bodies::front(ctmr_ctx* c, Chunk& ch) const {
     FrontEnd* f = c->fe.get();
     BodyState* bd = f->bd.get();
@@ -992,12 +1037,103 @@ int Bodies::front(ctmr_ctx* c, Chunk& ch) const {
     CU(c, cudaEventRecord(bd->ev_json1, s));
     f->launches += launches;
     if (nb) CU(c, cudaMemcpyAsync(&count, bd->body_base + nb, 4, cudaMemcpyDeviceToHost, s));
+    const bool tree = folds();
+    if (nb && tree) {
+        CU(c, cudaMemcpyAsync(bd->fold->h_status, bd->body_status, nb, cudaMemcpyDeviceToHost, s));
+        CU(c, cudaMemcpyAsync(bd->fold->h_count, bd->body_count, nb * 4, cudaMemcpyDeviceToHost, s));
+    }
     CU(c, cudaStreamSynchronize(s));
     float ms = 0.f;
     CU(c, cudaEventElapsedTime(&ms, bd->ev_json0, bd->ev_json1));
     bd->json_ms += ms;
     if (count > sparse) return fail(c, CTMR_E_CUDA, "bodies: more entries found than requested");
-    return spans_front(c, ch, f->cap_text, count, b->now_unix_ns, &out->path, meta);
+    const int rc = spans_front(c, ch, f->cap_text, count, b->now_unix_ns, &out->path, meta);
+    if (rc || !tree || !count) return rc;
+    CU(c, launch_raw_leaf_hash(ch.p.fe, f->tree->leaf, s));
+    ++f->launches;
+    CU(c, cudaEventRecord(f->ev1, s));
+    return CTMR_OK;
+}
+
+// A tree call's round, after its front halves: the bodies of members 0..W-1 in member order against each tree's end
+// (home->next) and stop.  Per body a window (BodyWindow) of the entries that fold; per member's chunk its trees
+// (ch.fold), and whether its order must be built (it is the identity when one tree takes every entry of the chunk).
+void Bodies::place(ctmr_ctx** m, Chunk* cur, uint32_t W) {  // positions: dense, in member order
+    for (uint32_t r = 0; r < W; ++r) {
+        cur[r].e0 = placed;
+        placed += cur[r].db.n;
+        cur[r].e1 = placed;
+    }
+    if (!folds()) return;
+    TreeState* home = tree_state;
+    std::vector<uint32_t>& cnt = home->count;
+    std::vector<uint64_t> first;
+    for (uint32_t r = 0; r < W; ++r) {
+        Chunk& ch = cur[r];
+        ch.fold.clear();
+        ch.ordered = false;
+        ch.listed = 0;
+        const uint64_t nb = ch.hi - ch.lo;
+        if (!nb) continue;
+        BodyFoldState* bf = m[r]->fe->bd->fold.get();
+        std::fill(cnt.begin(), cnt.end(), 0u);
+        first = home->next;
+        for (uint64_t i = 0; i < nb; ++i) {
+            const uint64_t u = ch.lo + i;
+            const uint32_t l = log ? log[u] : 0;
+            BodyWindow& w = bf->h_win[i];
+            w = BodyWindow{0, 0, 0};
+            if (l == CTMR_NO_TREE || stopped[l]) continue;
+            const uint64_t end = home->next[l];
+            if (bf->h_status[i] != CTMR_BODY_OK || start[u] > end) {  // positions unknown, or a gap: the fold stops at end
+                stopped[l] = 1;
+                continue;
+            }
+            const uint32_t n = bf->h_count[i];
+            const uint32_t skip = (uint32_t)std::min<uint64_t>(n, end - start[u]);  // already in the tree
+            w.first = skip;
+            w.cnt = n - skip;
+            cnt[l] += w.cnt;
+            home->next[l] = std::max(end, start[u] + n);
+        }
+        uint32_t off = 0;
+        for (uint32_t d = 0; d < home->n_trees; ++d) {
+            if (!cnt[d]) continue;
+            ch.fold.push_back(FoldTree{first[d], d, off, cnt[d], 0});
+            const uint32_t c_d = cnt[d];
+            cnt[d] = off;  // from here on: the tree's next slot in the order
+            off += c_d;
+        }
+        ch.listed = off;
+        ch.ordered = off && !(ch.fold.size() == 1 && off == ch.db.n);
+        if (!ch.ordered) continue;
+        for (uint64_t i = 0; i < nb; ++i) {
+            BodyWindow& w = bf->h_win[i];
+            if (!w.cnt) continue;
+            const uint32_t l = log ? log[ch.lo + i] : 0;
+            w.slot = cnt[l];
+            cnt[l] += w.cnt;
+        }
+    }
+}
+
+// a member's chunk into its trees (member 0) or ranges (members 1..), on its stream: the order from the windows unless
+// it is the identity, then the fold of the pages form
+int Bodies::fold(ctmr_ctx* c, const Chunk& ch) const {
+    if (ch.fold.empty()) return CTMR_OK;
+    FrontEnd* f = c->fe.get();
+    CU(c, cudaSetDevice(c->device));
+    if (ch.ordered) {
+        BodyFoldState* bf = f->bd->fold.get();
+        const uint64_t nb = ch.hi - ch.lo;
+        CU(c, cudaMemcpyAsync(bf->win, bf->h_win, nb * sizeof(BodyWindow), cudaMemcpyHostToDevice, c->stream));
+        CU(c, launch_body_fold_order(bf->win, (uint32_t)nb, f->bd->body_base, f->tree->order[ch.stage], c->stream));
+        ++f->launches;
+    }
+    const int rc = tree_fold(c, ch, f->tree->leaf, f->str_bad, 2, 1);
+    if (rc) return rc;
+    CU(c, cudaEventRecord(f->ev1, c->stream));  // the fold is front-end time, as in the pages form
+    return CTMR_OK;
 }
 
 int Bodies::copy_back(ctmr_ctx* c, const Chunk& ch) const {
@@ -1347,7 +1483,11 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
             cur[0].stopped = false;
             cur[0].dout = chunk_path_out(m[0]->fe.get(), po, fm.meta);
         }
-        fm.place(cur, W);
+        fm.place(m, cur, W);
+        if (tree) {  // bodies: the round's leaves into the trees, now that place has given out their log positions
+            rc = for_each_member(m, W, false, failed, [&](uint32_t r) { return fm.fold(m[r], cur[r]); });
+            if (rc) return rc;
+        }
         for (uint32_t r = 0; r < W; ++r) {
             if (stop < W) {
                 cur[r].cut(0, 0);  // after a stop in an earlier member: its entries must not touch the tables
@@ -1598,6 +1738,35 @@ int ctmr_group_process_tiles_trees(ctmr_group* g, const ctmr_tile_batch* b, ctmr
     return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Tiles(b, out), &t, g);
 }
 
+int ctmr_process_raw_bodies_tree(ctmr_ctx* c, const ctmr_body_batch* b, ctmr_body_out* out, const uint64_t* body_start, ctmr_tree* tree) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    const TreeArgs t{tree, 1, nullptr, false, body_start};
+    return front_end_call(&c, 1, &c->next_index, Bodies(b, out), &t, nullptr);
+}
+
+int ctmr_process_raw_bodies_trees(ctmr_ctx* c, const ctmr_body_batch* b, ctmr_body_out* out, const uint32_t* body_log,
+                                  const uint64_t* body_start, ctmr_tree* trees, uint32_t n_trees) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group || c->peer_mode == PEER_GROUP) return fail(c, CTMR_E_INVALID, "member of a group: the tree forms take one ctx");
+    const TreeArgs t{trees, n_trees, body_log, true, body_start};
+    return front_end_call(&c, 1, &c->next_index, Bodies(b, out), &t, nullptr);
+}
+
+int ctmr_group_process_raw_bodies_tree(ctmr_group* g, const ctmr_body_batch* b, ctmr_body_out* out, const uint64_t* body_start,
+                                       ctmr_tree* tree) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const TreeArgs t{tree, 1, nullptr, false, body_start};
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Bodies(b, out), &t, g);
+}
+
+int ctmr_group_process_raw_bodies_trees(ctmr_group* g, const ctmr_body_batch* b, ctmr_body_out* out, const uint32_t* body_log,
+                                        const uint64_t* body_start, ctmr_tree* trees, uint32_t n_trees) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const TreeArgs t{trees, n_trees, body_log, true, body_start};
+    return front_end_call(g->m.data(), (uint32_t)g->m.size(), &g->next_index, Bodies(b, out), &t, g);
+}
+
 int ctmr_next_index(ctmr_ctx* c, uint64_t* next_index) {
     if (!c) return CTMR_E_INVALID;
     if (!next_index || c->group) return fail(c, CTMR_E_INVALID, "bad argument (a member of a group has no index of its own)");
@@ -1698,6 +1867,20 @@ int bodies_ensure(ctmr_ctx* c) {
     CU(c, create(bd->ev_json0, cudaEventDefault));
     CU(c, create(bd->ev_json1, cudaEventDefault));
     f->bd = std::move(bd);
+    return CTMR_OK;
+}
+
+int bodies_fold_ensure(ctmr_ctx* c) {
+    BodyState* bd = c->fe->bd.get();
+    if (bd->fold) return CTMR_OK;
+    std::unique_ptr<BodyFoldState> bf(new (std::nothrow) BodyFoldState());
+    if (!bf) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    const uint64_t E = c->fe->cap_entries;
+    CU(c, alloc(bf->h_status, E));
+    CU(c, alloc(bf->h_count, E));
+    CU(c, alloc(bf->h_win, E));
+    CU(c, alloc(bf->win, E));
+    bd->fold = std::move(bf);
     return CTMR_OK;
 }
 

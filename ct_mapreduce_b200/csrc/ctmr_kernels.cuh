@@ -409,6 +409,18 @@ struct FoldChunk {
 
 // get-entries leaves: SHA-256(0x00 || decoded leaf_input) of p.n entries -> rows[n][32]; rows of bad leaf_inputs are not written
 cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t s);
+
+// The tree forms of the bodies call (ctmr_process_raw_bodies_tree(s)): what one body of a chunk folds.  Its entries
+// first .. first + cnt - 1 (body-local) take slots slot .. slot + cnt - 1 of the chunk's order; cnt == 0 folds none.
+struct BodyWindow {
+    uint32_t first;
+    uint32_t cnt;
+    uint32_t slot;
+};
+static_assert(sizeof(BodyWindow) == 12, "BodyWindow layout");
+// order[w.slot + k] = body_base[b] + w.first + k for every body b < n_bodies and k < w.cnt: the chunk's listed entries
+// grouped by tree, from the host's per-body windows and the JSON walk's per-body entry offsets
+cudaError_t launch_body_fold_order(const BodyWindow* win, uint32_t n_bodies, const uint32_t* body_base, uint32_t* order, cudaStream_t s);
 // Folds a chunk into its trees: one launch for the missing leaves, one per level of the widest tree range, for all trees
 // (level buffers lvl[2], each [total / 2 + 2 * n_desc][32]), one to commit the new sizes.  hdesc is the host copy of
 // f.desc (the level loop's bounds).  Returns the number of launches in *launches.

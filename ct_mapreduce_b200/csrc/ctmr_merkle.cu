@@ -4,6 +4,8 @@
 //
 //   K_raw_leaf_hash   thread per entry    SHA-256(0x00 || decoded leaf_input), read from the decoded arena
 //   (tile_leaf_hash)                      tiles: the leaf hashes of ctmr_tiles.cu, unchanged
+//   K_body_fold_order warp per body       bodies (ctmr_process_raw_bodies_tree(s)): the host's per-body windows and the JSON
+//                                         walk's body_base -> the chunk's order (entries skipped or after a stop unlisted)
 //   K_tree_missing    thread per entry    per tree, lowest log position of the chunk without a leaf (bad base64, bad tile)
 //   K_tree_level      thread per parent   one level of every tree's range: parents of the pairs inside it, the left edge
 //                                         node as the first left child, the last node as the new edge node
@@ -350,6 +352,16 @@ __global__ void tree_merge_kernel(TreeDev* trees, uint32_t n, RangeSet set) {
     t.size = size;
 }
 
+// one warp per body of the chunk: its window's entries into their slots of the order
+__global__ void __launch_bounds__(128) body_fold_order_kernel(const BodyWindow* __restrict__ win, uint32_t n_bodies,
+                                                             const uint32_t* __restrict__ body_base, uint32_t* __restrict__ order) {
+    const uint32_t b = blockIdx.x * 4u + (threadIdx.x >> 5);
+    if (b >= n_bodies) return;
+    const BodyWindow w = win[b];
+    const uint32_t e0 = body_base[b] + w.first;
+    for (uint32_t k = threadIdx.x & 31u; k < w.cnt; k += 32u) order[w.slot + k] = e0 + k;
+}
+
 // Levels where a tree's own range [first_pos, first_pos + cnt) is empty are empty for the part that folds too: the chunk
 // takes as many level launches as its widest range has levels
 uint32_t fold_levels(const FoldTree* hdesc, uint32_t n) {
@@ -366,6 +378,12 @@ uint32_t fold_levels(const FoldTree* hdesc, uint32_t n) {
 cudaError_t launch_raw_leaf_hash(const FeParams& p, uint8_t* rows, cudaStream_t s) {
     if (p.n == 0) return cudaSuccess;
     raw_leaf_hash_kernel<<<(unsigned)((p.n + 127) / 128), 128, 0, s>>>(p, rows);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_body_fold_order(const BodyWindow* win, uint32_t n_bodies, const uint32_t* body_base, uint32_t* order, cudaStream_t s) {
+    if (n_bodies == 0) return cudaSuccess;
+    body_fold_order_kernel<<<(n_bodies + 3u) / 4u, 128, 0, s>>>(win, n_bodies, body_base, order);
     return cudaGetLastError();
 }
 

@@ -361,16 +361,29 @@ class GpuCertDatabase:
         return self._lib.ctmr_process_raw_trees
 
     def store_raw_bodies(self, text, body_off, body_len, body_max, now_unix_ns: int, want_sha: bool = True, want_meta: bool = False,
-                         want_pem: bool = False) -> "BodiesResult":
+                         want_pem: bool = False, tree: LogTree | None = None, trees=None, body_log=None,
+                         body_start=None) -> "BodiesResult":
         """Whole get-entries response bodies (body b is text[body_off[b]:body_off[b] + body_len[b]], body_max[b] the entries
         requested) through ctmr_process_raw_bodies: the GPU finds the entries with encoding/json's rules, then does what
         store_raw_entries does with them.  The per-entry arrays of the result hold the n_entries entries found, in (body,
-        position) order; r.body_status / r.body_first / r.body_entries say which are whose."""
+        position) order; r.body_status / r.body_first / r.body_entries say which are whose.
+        With body_start= (the start of the get-entries request each body answers) and tree= (the log's entries before
+        these), ctmr_process_raw_bodies_tree also folds the entries into it: r.tree.  With trees= (one LogTree per log) and
+        body_log= (the log of each body, capi.NO_TREE for none), ctmr_process_raw_bodies_trees folds each body's entries
+        into its log's tree: r.trees.  A body that is not OK, or a gap between a log's bodies, stops that log's fold;
+        entries a body repeats below the tree's end are skipped."""
         with self._peer_refusal():
+            _tree_args(tree, trees, body_log, "body_log")
+            if body_start is not None and tree is None and trees is None:
+                raise CtmrError(capi.E_INVALID, "body_start goes with tree= or trees=")
             text = np.frombuffer(text, np.uint8) if isinstance(text, (bytes, bytearray, memoryview)) else np.ascontiguousarray(text, np.uint8)
             body_off = np.ascontiguousarray(body_off, np.uint64)
             body_len, body_max = np.ascontiguousarray(body_len, np.uint32), np.ascontiguousarray(body_max, np.uint32)
             nb = body_off.size
+            start = None if body_start is None else np.ascontiguousarray(body_start, np.uint64)
+            log = None if body_log is None else np.ascontiguousarray(body_log, np.uint32)
+            if (start is not None and start.shape != (nb,)) or (log is not None and log.shape != (nb,)):
+                raise CtmrError(capi.E_INVALID, "body_start and body_log hold one value per body")
         cap = int(body_max.sum())
         r = BodiesResult(cap, nb, want_sha, want_meta)
         p = r.path
@@ -387,12 +400,29 @@ class GpuCertDatabase:
         if want_pem:
             _attach_pem(o.raw.path, p, cap, int(body_len.sum()) // 4 * 3)
         b = capi.BodyBatch(capi.ptr(text), text.size, capi.ptr(body_off), capi.ptr(body_len), capi.ptr(body_max), nb, now_unix_ns)
-        self._check(self._process_raw_bodies_fn()(self._h, C.byref(b), C.byref(o)))
+        starts = capi.ptr(start) if start is not None and nb else None
+        if trees is not None:
+            arr = _trees_to_c(trees)
+            self._check(self._process_raw_bodies_trees_fn()(self._h, C.byref(b), C.byref(o), capi.ptr(log) if log is not None and nb else None,
+                                                            starts, arr if trees else None, len(trees)))
+            r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
+        elif tree is not None:
+            ct = tree.to_c()
+            self._check(self._process_raw_bodies_tree_fn()(self._h, C.byref(b), C.byref(o), starts, C.byref(ct)))
+            r.tree = LogTree.from_c(ct)
+        else:
+            self._check(self._process_raw_bodies_fn()(self._h, C.byref(b), C.byref(o)))
         r.trim(int(o.n_entries))
         return r
 
     def _process_raw_bodies_fn(self):
         return self._lib.ctmr_process_raw_bodies
+
+    def _process_raw_bodies_tree_fn(self):
+        return self._lib.ctmr_process_raw_bodies_tree
+
+    def _process_raw_bodies_trees_fn(self):
+        return self._lib.ctmr_process_raw_bodies_trees
 
     def bodies_profile_last(self) -> float:
         """Milliseconds of the JSON kernels in the last store_raw_bodies call, part of frontend_ms."""
@@ -719,6 +749,12 @@ class GpuCertGroup(GpuCertDatabase):
     def _process_raw_bodies_fn(self):
         return self._lib.ctmr_group_process_raw_bodies
 
+    def _process_raw_bodies_tree_fn(self):
+        return self._lib.ctmr_group_process_raw_bodies_tree
+
+    def _process_raw_bodies_trees_fn(self):
+        return self._lib.ctmr_group_process_raw_bodies_trees
+
     def _process_tiles_fn(self):
         return self._lib.ctmr_group_process_tiles
 
@@ -743,6 +779,17 @@ class GpuCertGroup(GpuCertDatabase):
         if tree is not None or trees is not None:
             raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: on a group use store_tiles_with_trees")
         return super().store_tiles(*a, **k)
+
+    def store_raw_bodies(self, *a, tree=None, trees=None, body_log=None, body_start=None, **k):
+        if tree is not None or trees is not None or body_log is not None or body_start is not None:
+            raise CtmrError(capi.E_INVALID, "tree= and trees= take one ctx: on a group use store_raw_bodies_with_trees")
+        return super().store_raw_bodies(*a, **k)
+
+    def store_raw_bodies_with_trees(self, *a, tree=None, trees=None, body_log=None, body_start=None, **k):
+        """store_raw_bodies with tree= or trees= / body_log=, and body_start=, on the group
+        (ctmr_group_process_raw_bodies_tree(s)): the same outputs as the plain group call, and r.tree / r.trees as the
+        one-ctx call gives them"""
+        return GpuCertDatabase.store_raw_bodies(self, *a, tree=tree, trees=trees, body_log=body_log, body_start=body_start, **k)
 
     def store_raw_entries_with_trees(self, *a, tree=None, trees=None, entry_log=None, **k):
         """store_raw_entries with tree= or trees= / entry_log= on the group (ctmr_group_process_raw_tree(s)): the same

@@ -221,6 +221,8 @@ type RawBodies struct {
 	BodyOff   []uint64
 	BodyLen   []uint32
 	BodyMax   []uint32
+	Start     []uint64 // the start of each body's get-entries request, for ProcessRawBodiesTree(s) (tree.go); 0 for Commit
+	Log       []uint32 // the log of each body, for ProcessRawBodiesTrees; NoTree for bodies of Commit / AppendBody
 }
 
 // Room is the pinned space left after the bodies recorded so far: a downloader may read the next body straight into
@@ -231,23 +233,38 @@ func (p *RawBodies) Room() []byte {
 
 // Commit records a body of n bytes read into Room(), for a get-entries request of maxEntries (end - start + 1).
 func (p *RawBodies) Commit(n int, maxEntries uint32) error {
+	return p.CommitLog(n, maxEntries, 0, NoTree)
+}
+
+// CommitLog is Commit for a body of log `log` that answers the get-entries request starting at log position `start`:
+// ProcessRawBodiesTree(s) folds its entries from there.  A log may answer short, so pass the request's start, not the
+// position where the previous answer ended.
+func (p *RawBodies) CommitLog(n int, maxEntries uint32, start uint64, log uint32) error {
 	if uint64(n) > p.Cap-p.Used || uint64(n) > 0xFFFFFFFF {
 		return fmt.Errorf("raw body buffer full")
 	}
 	p.BodyOff = append(p.BodyOff, p.Used)
 	p.BodyLen = append(p.BodyLen, uint32(n))
 	p.BodyMax = append(p.BodyMax, maxEntries)
+	p.Start = append(p.Start, start)
+	p.Log = append(p.Log, log)
 	p.Used += uint64(n)
 	return nil
 }
 
 // AppendBody copies one response body into the pinned text.
 func (p *RawBodies) AppendBody(body []byte, maxEntries uint32) error {
+	return p.AppendBodyLog(body, maxEntries, 0, NoTree)
+}
+
+// AppendBodyLog copies one response body of log `log`, the answer to the request starting at `start`, into the pinned
+// text (see CommitLog).
+func (p *RawBodies) AppendBodyLog(body []byte, maxEntries uint32, start uint64, log uint32) error {
 	if uint64(len(body)) > p.Cap-p.Used {
 		return fmt.Errorf("raw body buffer full")
 	}
 	copy(p.Room(), body)
-	return p.Commit(len(body), maxEntries)
+	return p.CommitLog(len(body), maxEntries, start, log)
 }
 
 // BodiesResult holds the outputs of ProcessRawBodies (ctmr_body_out): per entry found (sum of BodyMax rows, the first
@@ -335,6 +352,12 @@ type Repeated struct {
 // that page error too; r.BodyStatus says which bodies to fetch again.
 func (d *DB) ProcessRawBodies(p *RawBodies, nowUnixNs int64, r *BodiesResult, fallback *RawPages,
 	newResult func(n int) *RawResult) (*Repeated, error) {
+	return d.processRawBodies(p, nowUnixNs, r, fallback, newResult, nil, nil, false)
+}
+
+// processRawBodies: ProcessRawBodies and its tree forms (tree.go): one tree, or with `routed` one tree per log
+func (d *DB) processRawBodies(p *RawBodies, nowUnixNs int64, r *BodiesResult, fallback *RawPages,
+	newResult func(n int) *RawResult, tree *Tree, trees []Tree, routed bool) (*Repeated, error) {
 	b := (*C.ctmr_body_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_body_batch{}))))
 	defer C.free(unsafe.Pointer(b))
 	var pin runtime.Pinner
@@ -349,14 +372,33 @@ func (d *DB) ProcessRawBodies(p *RawBodies, nowUnixNs int64, r *BodiesResult, fa
 		b.body_len = (*C.uint32_t)(unsafe.Pointer(&p.BodyLen[0]))
 		b.body_max = (*C.uint32_t)(unsafe.Pointer(&p.BodyMax[0]))
 		b.n_bodies = C.uint64_t(n)
-	} else if !d.peer {
+	} else if !d.peer && tree == nil && !routed {  // a tree call still writes the roots
 		return nil, nil
 	}
 	b.now_unix_ns = C.int64_t(nowUnixNs)
+	var start *C.uint64_t
+	var log *C.uint32_t
+	if n := len(p.BodyOff); n > 0 && (tree != nil || routed) {
+		pin.Pin(&p.Start[0])
+		pin.Pin(&p.Log[0])
+		start = (*C.uint64_t)(unsafe.Pointer(&p.Start[0]))
+		log = (*C.uint32_t)(unsafe.Pointer(&p.Log[0]))
+	}
 	var err error
-	if d.g != nil {
+	switch {
+	case routed && d.g != nil:
+		err = d.err(C.ctmr_group_process_raw_bodies_trees(d.g, b, r.body, log, start, treesC(trees), C.uint32_t(len(trees))),
+			"ctmr_group_process_raw_bodies_trees")
+	case routed:
+		err = d.err(C.ctmr_process_raw_bodies_trees(d.h, b, r.body, log, start, treesC(trees), C.uint32_t(len(trees))),
+			"ctmr_process_raw_bodies_trees")
+	case tree != nil && d.g != nil:
+		err = d.err(C.ctmr_group_process_raw_bodies_tree(d.g, b, r.body, start, tree.c()), "ctmr_group_process_raw_bodies_tree")
+	case tree != nil:
+		err = d.err(C.ctmr_process_raw_bodies_tree(d.h, b, r.body, start, tree.c()), "ctmr_process_raw_bodies_tree")
+	case d.g != nil:
 		err = d.err(C.ctmr_group_process_raw_bodies(d.g, b, r.body), "ctmr_group_process_raw_bodies")
-	} else {
+	default:
 		err = d.err(C.ctmr_process_raw_bodies(d.h, b, r.body), "ctmr_process_raw_bodies")
 	}
 	if err != nil {

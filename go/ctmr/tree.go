@@ -56,6 +56,28 @@ func (d *DB) ProcessRawTrees(p *RawPages, nowUnixNs int64, r *RawResult, trees [
 	return d.processRaw(p, nowUnixNs, r, nil, trees, true)
 }
 
+// ProcessRawBodiesTree is ProcessRawBodies, and the bodies' entries folded into tree: entry j of a body recorded with
+// CommitLog / AppendBodyLog(..., start, log) is the log's entry start + j.  The bodies are walked in the order recorded
+// from tree.Size on: entries below it are already in the tree and are skipped, a body whose status is not BodyOK or that
+// starts above it (a short answer left a gap) stops the fold, and so does the first entry whose leaf_input is not
+// base64.  A stop is final for the call: fetch again from tree.Size.  A BodyRepeatedEntries body stops the fold too: its
+// entries still go through ProcessRaw, decoded on the host, but without a tree, so fetch that range again and fold it
+// with the next call.  The starts must not decrease and the first must not lie above tree.Size (CTMR_E_INVALID before
+// any work, tree unchanged).  Every output is that of ProcessRawBodies.  On one GPU or a group.
+func (d *DB) ProcessRawBodiesTree(p *RawBodies, nowUnixNs int64, r *BodiesResult, fallback *RawPages,
+	newResult func(n int) *RawResult, tree *Tree) (*Repeated, error) {
+	return d.processRawBodies(p, nowUnixNs, r, fallback, newResult, tree, nil, false)
+}
+
+// ProcessRawBodiesTrees is ProcessRawBodiesTree for the bodies of many logs in one batch: the entries of a body recorded
+// with CommitLog / AppendBodyLog(..., start, log) fold into trees[log], each log's bodies with the one-tree rules on their
+// own; bodies of Commit / AppendBody fold nowhere.  Every tree gets its root written.  On an error every tree is
+// unchanged.  On one GPU or a group.
+func (d *DB) ProcessRawBodiesTrees(p *RawBodies, nowUnixNs int64, r *BodiesResult, fallback *RawPages,
+	newResult func(n int) *RawResult, trees []Tree) (*Repeated, error) {
+	return d.processRawBodies(p, nowUnixNs, r, fallback, newResult, nil, trees, true)
+}
+
 // ProcessTilesTree is ProcessTiles, and the tiles' entries folded into tree.  The tiles must be consecutive tiles of one
 // log, full but for the last, with tree.Size inside the first: its leaves below tree.Size are skipped.  A bad tile stops
 // the fold at its first leaf, and the rest of the batch is still processed.  The fetch/register/resume loop carries the

@@ -300,9 +300,9 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the
  * launcher offers (torch.distributed all_gather in this repository) and attaches them.  From then on
- * ctmr_process_device, ctmr_process_batch, ctmr_reset_device, ctmr_peer_* and the six front-end calls of
- * ctmr_frontend.h (ctmr_process_raw, ctmr_process_tiles and their _tree / _trees forms; their contract is stated
- * there) are COLLECTIVE: every rank must make the same sequence of calls; any front-end call matches any other.
+ * ctmr_process_device, ctmr_process_batch, ctmr_reset_device, ctmr_peer_* and the nine front-end calls of
+ * ctmr_frontend.h (ctmr_process_raw, ctmr_process_tiles, ctmr_process_raw_bodies and their _tree / _trees forms; their
+ * contract is stated there) are COLLECTIVE: every rank must make the same sequence of calls; any front-end call matches any other.
  * Inside them the ranks meet at barriers kept in peer memory (no host round trip, no
  * NCCL on the data path); the global index of entry j of rank r's round k is first_index + (k * world + r) * E + j,
  * i.e. the result equals the sequential run over the rounds in rank order.  E = entries per rank and round: the host

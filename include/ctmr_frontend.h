@@ -337,10 +337,44 @@ int ctmr_group_process_raw_trees(ctmr_group* g, const ctmr_raw_batch* batch, ctm
 int ctmr_group_process_tiles_trees(ctmr_group* g, const ctmr_tile_batch* batch, ctmr_tile_out* out,
                                    const uint32_t* tile_log /* [n_tiles] */, ctmr_tree* trees, uint32_t n_trees);
 
+/* ---- the trees from whole get-entries bodies ---------------------------------------------------------------------------
+ * ctmr_process_raw_bodies / ctmr_group_process_raw_bodies, and each body's entries folded into its log's tree.  Every
+ * output, the return code, the global indices, body statuses, spans, PEM and string identities are those of the plain
+ * bodies call on the same batch.  body_start[b] is the start of the get-entries request that body b answers: entry j of
+ * the body is log position body_start[b] + j.  The one-tree forms fold every body into *tree; the routed forms fold body
+ * b into trees[body_log[b]], none for CTMR_NO_TREE.
+ *
+ * Before any work, with no index taken and no tree touched, CTMR_E_INVALID for: body_start NULL with bodies in the
+ * batch, body_log NULL in the routed forms, a log id >= n_trees that is not CTMR_NO_TREE, n_trees > CTMR_MAX_TREES, and
+ * per log in batch order: starts that decrease, a first body with start > tree.size, a start + body_max that wraps
+ * around 2^64.
+ *
+ * A log may answer a get-entries request with fewer entries than were asked for, so the bodies of a client that
+ * pipelines its requests may leave gaps or overlap.  Each tree walks its log's bodies in batch order with end = its size
+ * at the start of the call:
+ *   - a body that is not CTMR_BODY_OK stops the fold at end: its entries' positions are unknown;
+ *   - a body with start > end is a gap: the fold stops at end;
+ *   - otherwise its entries below end are already in the tree and are skipped unchecked, the rest are appended (the
+ *     first one whose leaf_input is not base64 stops the fold there), and end = max(end, start + entries).
+ * A stop is final for the call: tree->size says where to fetch again.  The leaf hash is that of the pages form
+ * (SHA-256(0x00 || decoded leaf_input)), so BAD_LEAF, BAD_EXTRA, UNKNOWN_TYPE and BAD_CERT entries fold.  Every tree
+ * passed in gets its root written; on any error every tree is left as passed in.  A member of a group is refused the
+ * one-ctx forms. */
+int ctmr_process_raw_bodies_tree(ctmr_ctx* ctx, const ctmr_body_batch* batch, ctmr_body_out* out,
+                                 const uint64_t* body_start /* [n_bodies] */, ctmr_tree* tree);
+int ctmr_process_raw_bodies_trees(ctmr_ctx* ctx, const ctmr_body_batch* batch, ctmr_body_out* out,
+                                  const uint32_t* body_log /* [n_bodies] */, const uint64_t* body_start /* [n_bodies] */,
+                                  ctmr_tree* trees, uint32_t n_trees);
+int ctmr_group_process_raw_bodies_tree(ctmr_group* g, const ctmr_body_batch* batch, ctmr_body_out* out,
+                                       const uint64_t* body_start /* [n_bodies] */, ctmr_tree* tree);
+int ctmr_group_process_raw_bodies_trees(ctmr_group* g, const ctmr_body_batch* batch, ctmr_body_out* out,
+                                        const uint32_t* body_log /* [n_bodies] */, const uint64_t* body_start /* [n_bodies] */,
+                                        ctmr_tree* trees, uint32_t n_trees);
+
 /* ---- one process per GPU: the front end as a collective call ------------------------------------------------------------
  * On a ctx attached to peers (ctmr_peer_attach, ctmr.h, world > 1) ctmr_process_raw, ctmr_process_raw_bodies,
- * ctmr_process_tiles, ctmr_process_raw_tree, ctmr_process_tiles_tree, ctmr_process_raw_trees and ctmr_process_tiles_trees
- * are COLLECTIVE.
+ * ctmr_process_tiles, ctmr_process_raw_tree, ctmr_process_tiles_tree, ctmr_process_raw_trees, ctmr_process_tiles_trees,
+ * ctmr_process_raw_bodies_tree and ctmr_process_raw_bodies_trees are COLLECTIVE.
  * Each rank passes its own batch, and each front-end call on one rank must meet a front-end call on every other rank.
  * The entry points may differ between the ranks of one call (pages on one rank, tiles with trees on another): their
  * collective steps are the same.  A front-end call met by ctmr_process_batch, ctmr_process_device or any other

@@ -1,18 +1,14 @@
 """Whole get-entries bodies on the GPU (ctmr_process_raw_bodies, include/ctmr_frontend.h) against a twin db fed by
 ctmr_process_raw with the spans tests/bodies_oracle.py finds (escaped strings replaced by their unescaped text): every
 per-entry output, the body statuses and counts, the string spans, the next index and the counters.  Marked gpu."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import bodies_oracle as bo
+from bodies_pair import PATH_FIELDS, RAW_FIELDS, next_idx, run_pair, synth_bodies  # noqa: F401 (re-exported)
 from conftest import NOW_NS
 
 pytestmark = pytest.mark.gpu
-
-RAW_FIELDS = ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_src", "leaf_off", "leaf_len")
-PATH_FIELDS = ("status", "sha256", "exp_hour", "serial_off", "serial_len", "was_unknown", "first_issuer_hour")
 
 
 @pytest.fixture(scope="module")
@@ -20,70 +16,6 @@ def eng():
     from ct_mapreduce_b200 import build, engine
     build.build()
     return engine
-
-
-def synth_bodies(n, page=1000, seed=20260922):
-    """n synthetic entries as back-to-back bodies of `page` entries (ctmr_synth_raw_pages_host)"""
-    from ct_mapreduce_b200 import capi
-    L = capi.load()
-    cfg = capi.synth_cfg(n, seed=seed, n_issuers=64)
-    need = L.ctmr_synth_raw_pages_host(C.byref(cfg), 0, n, page, None, 0, None, None, None, None)
-    text = np.zeros(need, np.uint8)
-    lo, ll, xo, xl = np.zeros(n, np.uint64), np.zeros(n, np.uint32), np.zeros(n, np.uint64), np.zeros(n, np.uint32)
-    assert L.ctmr_synth_raw_pages_host(C.byref(cfg), 0, n, page, capi.ptr(text), need, capi.ptr(lo), capi.ptr(ll), capi.ptr(xo),
-                                       capi.ptr(xl)) == need
-    starts = [int(lo[a]) - len(b'{"entries":[{"leaf_input":"') for a in range(0, n, page)] + [need]
-    return text.tobytes(), [text[starts[k]:starts[k + 1]].tobytes() for k in range(len(starts) - 1)]
-
-
-def next_idx(d):
-    from ct_mapreduce_b200 import engine
-    if isinstance(d, engine.GpuCertGroup):  # a group's next index is in its snapshot header
-        return int(np.frombuffer(d.snapshot()[48:56].tobytes(), np.uint64)[0])
-    return d.next_index()
-
-
-def run_pair(db, twin, bodies, maxes, text=None, offs=None, **kw):
-    """the bodies call on db and the twin's ctmr_process_raw call; compares everything"""
-    if text is None:
-        text = b"".join(bodies)
-        offs = np.cumsum([0] + [len(b) for b in bodies[:-1]]).astype(np.uint64)
-    lens = np.array([len(b) for b in bodies], np.uint32)
-    ttext, lo, ll, xo, xl, sts, cnts = bo.twin_batch(bodies, maxes)
-    n0 = next_idx(db)
-    t0 = twin.next_index()
-    r = db.store_raw_bodies(text, offs, lens, np.array(maxes, np.uint32), NOW_NS, **kw)
-    t = twin.store_raw_entries(ttext, np.array(lo, np.uint64), np.array(ll, np.uint32), np.array(xo, np.uint64), np.array(xl, np.uint32),
-                               NOW_NS, **kw)
-    assert r.body_status.tolist() == sts
-    assert r.body_entries.tolist() == cnts
-    assert r.body_first.tolist() == np.cumsum([0] + cnts[:-1]).tolist()
-    assert r.n_entries == sum(cnts) and next_idx(db) - n0 == sum(cnts) == twin.next_index() - t0
-    for f in RAW_FIELDS:
-        if f != "issuer":
-            assert np.array_equal(getattr(r, f), getattr(t, f)), f
-    # dense issuer indices are handed out in the order a parallel look-up meets new Chain[0]s: compare the issuers
-    dense = r.issuer < 0xFFFFFFFE
-    assert np.array_equal(dense, t.issuer < 0xFFFFFFFE) and np.array_equal(r.issuer[~dense], t.issuer[~dense])
-    assert [db.issuer_digest(int(i)) for i in r.issuer[dense]] == [twin.issuer_digest(int(i)) for i in t.issuer[dense]]
-    for f in PATH_FIELDS + (("issuer_name_off", "issuer_name_len", "crldp_off", "crldp_len", "first_issuer_dn", "first_crldp")
-                            if kw.get("want_meta") else ()):
-        assert np.array_equal(getattr(r.path, f), getattr(t.path, f)), f
-    if kw.get("want_pem"):
-        assert np.array_equal(r.path.pem_off, t.path.pem_off) and r.path.pem[:int(r.path.pem_off[-1])].tobytes() == \
-            t.path.pem[:int(t.path.pem_off[-1])].tobytes()
-    # the spans as found, in the caller's text
-    k = 0
-    for body, off, mx in zip(bodies, offs, maxes):
-        st, ents = bo.parse_body(body, mx)
-        for leaf, extra in ents:
-            for s, o_, l_, bit in ((leaf, r.leaf_input_off, r.leaf_input_len, 1), (extra, r.extra_data_off, r.extra_data_len, 2)):
-                assert (int(o_[k]), int(l_[k])) == ((0, 0) if s is None else (int(off) + s.off, s.len)), k
-                assert bool(r.escaped[k] & bit) == bool(s is not None and s.escaped), k
-            k += 1
-    assert {a: v for a, v in db.issuer_counts().items() if v} == {a: v for a, v in twin.issuer_counts().items() if v}
-    assert np.array_equal(db.status_counters(), twin.status_counters())
-    return r
 
 
 def corpus():

@@ -31,7 +31,8 @@ EXPORTS = [
     "ctmr_set_cardinality", "ctmr_status_counters", "ctmr_table_stats", "ctmr_map_device", "ctmr_reduce_device",
     "ctmr_process_device", "ctmr_read_histogram_device",
     "ctmr_check_device", "ctmr_reset_device", "ctmr_profile_last", "ctmr_preload_known", "ctmr_snapshot_size",
-    "ctmr_snapshot_save", "ctmr_snapshot_load", "ctmr_evict_expired", "ctmr_sha256_ceiling_device", "ctmr_synth_offsets_device", "ctmr_synth_write_device", "ctmr_synth_truth_device", "ctmr_synth_issuers_host", "ctmr_synth_raw_pages_host",
+    "ctmr_snapshot_save", "ctmr_snapshot_load", "ctmr_checkpoint_size", "ctmr_checkpoint_save", "ctmr_checkpoint_load",
+    "ctmr_evict_expired", "ctmr_sha256_ceiling_device", "ctmr_synth_offsets_device", "ctmr_synth_write_device", "ctmr_synth_truth_device", "ctmr_synth_issuers_host", "ctmr_synth_raw_pages_host",
     "ctmr_synth_tiles_host",
     "ctmr_process_raw", "ctmr_group_process_raw", "ctmr_frontend_profile_last",  # include/ctmr_frontend.h
     "ctmr_process_tiles", "ctmr_group_process_tiles", "ctmr_register_chain_certs", "ctmr_group_register_chain_certs",
@@ -45,6 +46,7 @@ EXPORTS = [
     "ctmr_group_process_batch", "ctmr_group_issuer_counts", "ctmr_group_set_cardinality", "ctmr_group_status_counters",
     "ctmr_group_table_stats", "ctmr_group_preload_known", "ctmr_group_evict_expired", "ctmr_group_reset",
     "ctmr_group_snapshot_size", "ctmr_group_snapshot_save", "ctmr_group_snapshot_load",
+    "ctmr_group_checkpoint_size", "ctmr_group_checkpoint_save", "ctmr_group_checkpoint_load",
     "ctmr_peer_export", "ctmr_peer_attach", "ctmr_peer_barrier_device", "ctmr_peer_allreduce_histogram_device",
     "ctmr_bind_host_to_device", "ctmr_peer_rounds", "ctmr_peer_round_entries", "ctmr_peer_frontend_stopped",
     "ctmr_next_index",
@@ -203,6 +205,9 @@ def load():
     L.ctmr_snapshot_size.argtypes = [vp, C.POINTER(u64)]
     L.ctmr_snapshot_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
     L.ctmr_snapshot_load.argtypes = [vp, vp, u64]
+    L.ctmr_checkpoint_size.argtypes = [vp, C.POINTER(u64)]
+    L.ctmr_checkpoint_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
+    L.ctmr_checkpoint_load.argtypes = [vp, vp, vp, u32]
     L.ctmr_evict_expired.argtypes = [vp, i64, C.POINTER(u64)]
     L.ctmr_sha256_ceiling_device.argtypes = [vp, u32, u32, u32, C.POINTER(C.c_float), C.POINTER(u64)]
     L.ctmr_profile_last.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]
@@ -258,6 +263,9 @@ def load():
     L.ctmr_group_snapshot_size.argtypes = [vp, C.POINTER(u64)]
     L.ctmr_group_snapshot_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
     L.ctmr_group_snapshot_load.argtypes = [vp, vp, u64]
+    L.ctmr_group_checkpoint_size.argtypes = [vp, C.POINTER(u64)]
+    L.ctmr_group_checkpoint_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
+    L.ctmr_group_checkpoint_load.argtypes = [vp, vp, vp, u32]
     L.ctmr_peer_export.argtypes = [vp, u32, vp]
     L.ctmr_peer_attach.argtypes = [vp, u32, u32, vp]
     L.ctmr_peer_barrier_device.argtypes = [vp, vp]

@@ -933,14 +933,8 @@ int ctmr_reset_device(ctmr_ctx* c, void* stream) {
     // multi-process group: collective.  Nobody may still be inserting into this shard when it is cleared, and nobody
     // may insert into it again before it has been cleared.
     int rc = peer_barrier(c, CH_RESET_A, s);
-    if (rc) return rc;
-    CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), s));
-    CU(c, cudaMemsetAsync(c->st.pairs, 0, (c->st.pair_mask + 1) * sizeof(PairSlot), s));
-    CU(c, cudaMemsetAsync(c->st.meta, 0, (c->st.meta_mask + 1) * sizeof(MetaSlot), s));
-    CU(c, cudaMemsetAsync(c->st.issuer_counts, 0, c->st.max_issuers * sizeof(unsigned long long), s));
-    CU(c, cudaMemsetAsync(c->st.status_counts, 0, CTMR_ST__COUNT * sizeof(unsigned long long), s));
-    CU(c, cudaMemsetAsync(&c->small->slots_used, 0, offsetof(SmallDev, cardinality), s));  // slots_used and the error flag
-    return peer_barrier(c, CH_RESET_B, s);
+    if (rc == CTMR_OK) rc = reset_tables(c, s);
+    return rc ? rc : peer_barrier(c, CH_RESET_B, s);
 }
 
 // Reads AND clears the sticky device-side failure flag: one failed batch does not poison the ctx.
@@ -960,6 +954,7 @@ int ctmr_check_device(ctmr_ctx* c, void* stream) {
     case CTMR_E_META_TABLE_FULL: return fail(c, flag, "IssuerMetadata string-identity table is full; raise config.meta_capacity_log2");
     case CTMR_E_TOO_MANY_ISSUERS: return fail(c, flag, "more distinct issuers than config.max_issuers");
     case CTMR_E_PEER_TIMEOUT: return fail(c, flag, "a rank of the group did not reach a barrier in time (peer failed, or the collective calls diverged; CTMR_PEER_TIMEOUT_MS)");
+    case CTMR_E_INVALID: return fail(c, flag, "a checkpoint record is out of range (issuer, serial length or slot tag)");
     default: return fail(c, CTMR_E_CUDA, "device-side failure flag set");
     }
 }
@@ -1052,11 +1047,25 @@ int snap_shard_load(ctmr_ctx* c, const uint8_t* p) {
     CU(c, cudaMemcpy(c->st.meta, p, m, cudaMemcpyHostToDevice)); p += m;
     CU(c, cudaMemcpy(c->st.issuer_counts, p, ic, cudaMemcpyHostToDevice)); p += ic;
     CU(c, cudaMemcpy(c->st.status_counts, p, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    return clear_issuer_memos(c);
+}
+
+int clear_issuer_memos(ctmr_ctx* c) {
     // host memos: the DER memo is rebuilt lazily, the digest memos come back from the device registry
     c->digests.clear();
     c->issuer_by_digest.clear();
     c->issuer_by_der.clear();
     if (c->fe) return fe_clear_issuers(c);
+    return CTMR_OK;
+}
+
+int reset_tables(ctmr_ctx* c, cudaStream_t s) {
+    CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), s));
+    CU(c, cudaMemsetAsync(c->st.pairs, 0, (c->st.pair_mask + 1) * sizeof(PairSlot), s));
+    CU(c, cudaMemsetAsync(c->st.meta, 0, (c->st.meta_mask + 1) * sizeof(MetaSlot), s));
+    CU(c, cudaMemsetAsync(c->st.issuer_counts, 0, c->st.max_issuers * sizeof(unsigned long long), s));
+    CU(c, cudaMemsetAsync(c->st.status_counts, 0, CTMR_ST__COUNT * sizeof(unsigned long long), s));
+    CU(c, cudaMemsetAsync(&c->small->slots_used, 0, offsetof(SmallDev, cardinality), s));  // slots_used and the error flag
     return CTMR_OK;
 }
 
@@ -1239,12 +1248,12 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     CU(c, cudaSetDevice(c->device));
     CU(c, cudaDeviceSynchronize());
     unsigned long long counters[2] = {0, 0};
-    unsigned long long* dev = c->small->evict;  // live, expired, compaction cursor
+    unsigned long long* dev = c->small->evict;  // live, expired
     // the count pass takes the expired keys off the per-issuer counts: a copy puts them back if the call cannot go on
     std::vector<unsigned long long> counts_before(c->st.max_issuers);
     CU(c, cudaMemcpyAsync(counts_before.data(), c->st.issuer_counts, counts_before.size() * sizeof(unsigned long long),
                           cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaMemsetAsync(dev, 0, 3 * sizeof(unsigned long long), c->stream));
+    CU(c, cudaMemsetAsync(dev, 0, 2 * sizeof(unsigned long long), c->stream));
     CU(c, launch_evict_count(c->st, now_unix_sec, dev, c->sm_count, c->stream));
     CU(c, cudaMemcpyAsync(counters, dev, sizeof counters, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
@@ -1252,16 +1261,23 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     if (counters[1] == 0) return CTMR_OK;
     // open addressing with linear probing: taking slots out would cut probe chains, so the survivors are
     // compacted aside, the table is cleared and they are inserted again (first-seen indices preserved)
+    const uint64_t slots = c->st.table_mask + 1;
     DevBuf<KnownSlot> keep;
-    if (counters[0] && alloc(keep, counters[0]) != cudaSuccess) {
+    CompactPlan plan;
+    int rc = CTMR_OK;
+    if (counters[0])
+        rc = alloc(keep, counters[0]) != cudaSuccess ? fail(c, CTMR_E_NOMEM, "ctmr_evict_expired: no device memory for the surviving keys")
+                                                     : compact_plan(c, c->st.table, slots, now_unix_sec, plan);
+    if (rc) {
         CU(c, cudaMemcpy(c->st.issuer_counts, counts_before.data(), counts_before.size() * sizeof(unsigned long long),
                          cudaMemcpyHostToDevice));
-        return fail(c, CTMR_E_NOMEM, "ctmr_evict_expired: no device memory for the surviving keys");
+        return rc;
     }
     CU(c, launch_evict_pairs(c->st, now_unix_sec, c->sm_count, c->stream));  // the expired sets' cardinalities are 0 again
-    if (counters[0]) CU(c, launch_evict_compact(c->st, now_unix_sec, keep, dev + 2, c->sm_count, c->stream));
-    CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), c->stream));
-    CU(c, launch_evict_reinsert(c->st, keep, counters[0], c->stream));
+    if (counters[0])
+        CU(c, launch_evict_compact(c->st.table, slots, now_unix_sec, 0, plan.tiles(), plan.dev.get(), keep.get(), (uint32_t*)nullptr, c->stream));
+    CU(c, cudaMemsetAsync(c->st.table, 0, slots * sizeof(KnownSlot), c->stream));
+    CU(c, launch_evict_reinsert(c->st, keep, counters[0], c->st.max_issuers, false, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     return ctmr_check_device(c, nullptr);
 }

@@ -296,7 +296,7 @@ struct SmallDev {
     int error_flag;                  // DeviceState::error_flag
     unsigned long long cardinality;  // ctmr_set_cardinality's probe result
     unsigned long long table_count;  // ctmr_table_stats' count
-    unsigned long long evict[3];     // ctmr_evict_expired: live, expired, compaction cursor
+    unsigned long long evict[2];     // ctmr_evict_expired: live, expired
     uint32_t sha_sink;               // ctmr_sha256_ceiling_device's sink
     alignas(16) uint8_t digest[32];  // lookup_digest: one digest to register
     uint32_t idx;                    //   and its index
@@ -330,6 +330,7 @@ enum : uint32_t {
     CH_STAGE_RESOLVE = 3,  // + stage index (3): after resolve of a host-pipeline round
     CH_DEV_MAP = 6, CH_DEV_RESOLVE = 7,  // ctmr_process_device
     CH_USER = 8, CH_HIST_A = 9, CH_HIST_B = 10, CH_RESET_A = 11, CH_RESET_B = 12, CH_MAILBOX = 13,
+    CH_CKPT = 14,                        // ctmr_checkpoint_*: every barrier and agreement of the collective size, save and load
     CH_STAGE_META = 16                   // + stage index (3): after the string-identity insert of a host-pipeline round
 };
 
@@ -441,6 +442,9 @@ int group_fail(ctmr_group* g, ctmr_ctx* c, int rc);   // c's error becomes g's l
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise
+// one word from every rank through the mailbox, row[r] = rank r's (ctmr_frontend_api.cu); the caller then checks the
+// device for a barrier that timed out
+int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row);
 int refresh_digests(ctmr_ctx* c);                                   // host memo <- device registry
 int lookup_digest(ctmr_ctx* c, const uint8_t digest[32], bool insert, uint32_t* idx_out, bool* found);
 int upload_issuer_map(ctmr_ctx* c, const uint32_t* dense, uint32_t n);
@@ -465,6 +469,36 @@ int bodies_ensure(ctmr_ctx* c);     // ... and the JSON buffers of ctmr_process_
 int bodies_fold_ensure(ctmr_ctx* c);  // ... and the fold windows of its tree forms, after bodies_ensure
 int ensure_scratch(ctmr_ctx* c, uint64_t n);
 int ensure_device_path(ctmr_ctx* c, uint64_t n);   // what ctmr_process_device needs for n entries
+// known-certificate table, pairs, string identities, per-issuer and status counters and the error flag to zero, on this
+// ctx alone (ctmr_reset_device brackets it with the group's barriers)
+int reset_tables(ctmr_ctx* c, cudaStream_t s);
+// after the registry was replaced: the host memos of it go, and so do the Chain[0] mirror and the tiles' fingerprints
+int clear_issuer_memos(ctmr_ctx* c);
+
+// Where a table's live slots go when they are compacted in slot order (launch_evict_compact): the exclusive prefix of the
+// live slots per tile of kCompactTile, on the host and on the device.  host[tiles()] = the live slots of the table.
+struct CompactPlan {
+    std::vector<unsigned long long> host;
+    DevBuf<unsigned long long> dev;
+    uint64_t tiles() const { return host.empty() ? 0 : host.size() - 1; }
+    uint64_t live() const { return host.empty() ? 0 : host.back(); }
+};
+template <class Slot>
+int compact_plan(ctmr_ctx* c, const Slot* table, uint64_t n_slots, int64_t now_sec, CompactPlan& p) {
+    const uint64_t tiles = (n_slots + kCompactTile - 1) / kCompactTile;
+    DevBuf<uint32_t> counts;
+    std::vector<uint32_t> h(tiles);
+    CU(c, alloc(counts, tiles));
+    CU(c, alloc(p.dev, tiles + 1));
+    CU(c, launch_evict_compact(table, n_slots, now_sec, 0, tiles, (const unsigned long long*)nullptr, (Slot*)nullptr, counts.get(), c->stream));
+    CU(c, cudaMemcpyAsync(h.data(), counts, tiles * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    p.host.assign(tiles + 1, 0);
+    for (uint64_t t = 0; t < tiles; ++t) p.host[t + 1] = p.host[t] + h[t];
+    CU(c, cudaMemcpyAsync(p.dev, p.host.data(), (tiles + 1) * sizeof(unsigned long long), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return CTMR_OK;
+}
 uint64_t device_round_entries(uint64_t n, uint32_t rounds);   // E of a ctmr_process_device call cut into `rounds` rounds
 uint32_t peer_rounds();   // rounds of the collective ctmr_process_device (CTMR_PEER_ROUNDS, env override for experiments)
 int pem_ensure(ctmr_ctx* c, PemStage& ps, uint64_t entries, uint64_t der_bytes);

@@ -1809,6 +1809,8 @@ int ctmr_group_register_chain_certs(ctmr_group* g, const uint8_t* blob, const ui
 
 namespace ctmr_host {
 
+int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row) { return peer_exchange(c, mine, row); }
+
 int tiles_ensure(ctmr_ctx* c) {
     FrontEnd* f = c->fe.get();
     if (f->tl) return CTMR_OK;

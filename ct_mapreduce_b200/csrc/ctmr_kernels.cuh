@@ -197,9 +197,20 @@ cudaError_t launch_issuer_prepare(const uint8_t* blob, const uint64_t* offsets, 
                                   uint8_t* ok, cudaStream_t s);
 cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, int sm_count, cudaStream_t s);
 cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters /* [2] */, int sm_count, cudaStream_t s);
-cudaError_t launch_evict_compact(const DeviceState& st, int64_t now_sec, KnownSlot* keep, unsigned long long* cursor, int sm_count,
-                                 cudaStream_t s);
-cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, cudaStream_t s);
+// Ordered compaction of a table's live slots (KnownSlot: ready and hour * 3600 > now_sec; PairSlot / MetaSlot: occupied),
+// over tiles [t0, t1) of kCompactTile slots.  counts != NULL: counts[b - t0] = live slots of tile b.  Otherwise tile b's live
+// slots go to keep[base[b] - base[t0] ...] in slot order (base = exclusive prefix of the counts over every tile).
+constexpr uint32_t kCompactTile = 4096;
+template <class Slot>
+cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, int64_t now_sec, uint64_t t0, uint64_t t1,
+                                 const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s);
+// Inserts n key records again (eviction's survivors, a checkpoint's keys): only those this rank owns under st.peer, each
+// checked first (issuer < n_issuers, serial length, ready tag; else the error flag is CTMR_E_INVALID); count: add each
+// inserted key to the per-issuer histogram.
+cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, uint32_t n_issuers, bool count, cudaStream_t s);
+// a checkpoint's pair records and string identities into this rank's tables (owner-filtered, checked the same way)
+cudaError_t launch_ckpt_pairs(const DeviceState& st, const PairSlot* rec, uint64_t n, uint32_t n_issuers, cudaStream_t s);
+cudaError_t launch_ckpt_meta(const DeviceState& st, const MetaSlot* rec, uint64_t n, cudaStream_t s);
 cudaError_t launch_cardinality(const DeviceState& st, int32_t exp_hour, uint32_t issuer, unsigned long long* out,
                                cudaStream_t s);
 

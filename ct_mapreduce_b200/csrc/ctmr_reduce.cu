@@ -400,39 +400,127 @@ __global__ void __launch_bounds__(256) evict_count_kernel(DeviceState st, int64_
     }
 }
 
-// pass 2: survivors, compacted (order irrelevant)
-__global__ void __launch_bounds__(256) evict_compact_kernel(DeviceState st, int64_t now_sec, KnownSlot* __restrict__ keep,
-                                                            unsigned long long* cursor) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= st.table_mask; i += (uint64_t)gridDim.x * blockDim.x) {
-        const KnownSlot sl = st.table[i];
-        if ((sl.tag & 3ull) != 2ull) continue;
-        if ((int64_t)(int32_t)sl.body[0] * 3600 <= now_sec) continue;
-        keep[atomicAdd(cursor, 1ull)] = sl;
+// pass 2: the live slots of a table, compacted in slot order (ctmr_evict_expired: the surviving keys; a checkpoint: the
+// ready keys, the pairs and the string identities).  Tile b (kCompactTile slots from t0 * kCompactTile on) is one CTA:
+// with counts set, counts[b] = its live slots; otherwise it writes them from keep[base[t0 + b] - base[t0]] on, in slot
+// order (a ballot per warp and a scan over the CTA's eight warps per row of 256 slots).  Two runs over the same state
+// write the same bytes.
+__device__ __forceinline__ bool slot_live(const KnownSlot& sl, int64_t now_sec) {
+    return (sl.tag & 3ull) == 2ull && (int64_t)(int32_t)sl.body[0] * 3600 > now_sec;
+}
+__device__ __forceinline__ bool slot_live(const PairSlot& sl, int64_t) { return sl.key != 0ull; }
+__device__ __forceinline__ bool slot_live(const MetaSlot& sl, int64_t) { return sl.h1 != 0ull; }
+
+template <class Slot>
+__global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restrict__ table, uint64_t n_slots, int64_t now_sec, uint64_t t0,
+                                                            const unsigned long long* __restrict__ base, Slot* __restrict__ keep,
+                                                            uint32_t* __restrict__ counts) {
+    __shared__ uint32_t warp_n[8];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const uint64_t tile = t0 + blockIdx.x;
+    uint64_t out = counts ? 0ull : base[tile] - base[t0];
+    uint32_t total = 0;
+    for (uint32_t row = 0; row < kCompactTile / 256u; ++row) {
+        const uint64_t i = tile * kCompactTile + row * 256u + threadIdx.x;
+        const bool live = i < n_slots && slot_live(table[i], now_sec);
+        const uint32_t ball = __ballot_sync(0xffffffffu, live);
+        if (lane == 0) warp_n[warp] = __popc(ball);
+        __syncthreads();
+        uint32_t before = 0, row_n = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < 8u; ++w) {
+            before += w < warp ? warp_n[w] : 0u;
+            row_n += warp_n[w];
+        }
+        if (live && !counts) keep[out + before + __popc(ball & ((1u << lane) - 1u))] = table[i];
+        out += row_n;
+        total += row_n;
+        __syncthreads();  // warp_n is rewritten by the next row
     }
+    if (counts && threadIdx.x == 0) counts[blockIdx.x] = total;
 }
 
-// pass 3 (after the table has been cleared): linear probing leaves no holes only if every survivor is re-inserted
-__global__ void __launch_bounds__(256) evict_reinsert_kernel(DeviceState st, const KnownSlot* __restrict__ keep, uint64_t n) {
+// pass 3 (after the table has been cleared), and a checkpoint's records on their way in: linear probing leaves no holes
+// only if every record is inserted again.  A record whose owner under this rank's world is another rank is skipped
+// (eviction: a rank only ever holds keys it owns).  Every index a record carries is checked before it is used: an
+// issuer >= n_issuers, a serial longer than CTMR_MAX_SERIAL or a slot that is not ready raises CTMR_E_INVALID.  count:
+// the inserted keys go into the per-issuer histogram (a checkpoint carries no histogram).
+__global__ void __launch_bounds__(256) evict_reinsert_kernel(DeviceState st, const KnownSlot* __restrict__ keep, uint64_t n,
+                                                             uint32_t n_issuers, bool count) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    const KnownSlot sl = keep[i];
+    if ((sl.tag & 3ull) != 2ull || sl.body[1] >= n_issuers || (sl.body[2] & 0xFFu) > CTMR_MAX_SERIAL) {
+        atomicExch(st.error_flag, CTMR_E_INVALID);
+        return;
+    }
+    if (st.peer.world > 1u && key_owner((int32_t)sl.body[0], sl.body[1], st.peer.world) != st.peer.rank) return;
     uint32_t body[12];
 #pragma unroll
-    for (int k = 0; k < 12; ++k) body[k] = keep[i].body[k];
-    known_insert<false>(st.table, st.table_mask, st.error_flag, body, keep[i].inv_first);  // a rank only ever holds keys it owns
+    for (int k = 0; k < 12; ++k) body[k] = sl.body[k];
+    if (known_insert<false>(st.table, st.table_mask, st.error_flag, body, sl.inv_first) != 0xFFFFFFFFu && count)
+        atomicAdd(st.issuer_counts + sl.body[1], 1ull);
+}
+
+// a checkpoint's (issuer, hour) records: the owner's pair slot again, with its first-seen index and its cardinality
+__global__ void __launch_bounds__(256) ckpt_pairs_kernel(DeviceState st, const PairSlot* __restrict__ rec, uint64_t n, uint32_t n_issuers) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const PairSlot p = rec[i];
+    if (p.key == 0ull || ((p.key - 1ull) >> 32) >= n_issuers) {
+        atomicExch(st.error_flag, CTMR_E_INVALID);
+        return;
+    }
+    const uint32_t issuer = (uint32_t)((p.key - 1ull) >> 32);
+    const int32_t hour = (int32_t)(uint32_t)(p.key - 1ull);
+    if (st.peer.world > 1u && key_owner(hour, issuer, st.peer.world) != st.peer.rank) return;
+    const uint32_t ps = pair_insert<false>(st.pairs, st.pair_mask, st.error_flag, p.key, p.inv_first);
+    if (ps != 0xFFFFFFFFu && p.count) tab_add<false>(&st.pairs[ps].count, p.count);
+}
+
+// a checkpoint's string identities: the owner's slot again, with its first-seen index
+__global__ void __launch_bounds__(256) ckpt_meta_kernel(DeviceState st, const MetaSlot* __restrict__ rec, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const MetaSlot m = rec[i];
+    if (m.h1 == 0ull || m.h2 == 0ull) {
+        atomicExch(st.error_flag, CTMR_E_INVALID);
+        return;
+    }
+    if (meta_owner(m.h1, st.peer.world) != (st.peer.world > 1u ? st.peer.rank : 0u)) return;
+    meta_insert_at<false>(st.meta, st.meta_mask, st.error_flag, m.h1, m.h2, m.inv_first);
 }
 
 cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters, int sm_count, cudaStream_t s) {
     evict_count_kernel<<<sm_count * 8, 256, 0, s>>>(st, now_sec, counters);
     return cudaGetLastError();
 }
-cudaError_t launch_evict_compact(const DeviceState& st, int64_t now_sec, KnownSlot* keep, unsigned long long* cursor, int sm_count,
-                                 cudaStream_t s) {
-    evict_compact_kernel<<<sm_count * 8, 256, 0, s>>>(st, now_sec, keep, cursor);
+template <class Slot>
+cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, int64_t now_sec, uint64_t t0, uint64_t t1,
+                                 const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s) {
+    if (t1 <= t0) return cudaSuccess;
+    evict_compact_kernel<Slot><<<(unsigned)(t1 - t0), 256, 0, s>>>(table, n_slots, now_sec, t0, base, keep, counts);
     return cudaGetLastError();
 }
-cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, cudaStream_t s) {
+template cudaError_t launch_evict_compact<KnownSlot>(const KnownSlot*, uint64_t, int64_t, uint64_t, uint64_t, const unsigned long long*,
+                                                     KnownSlot*, uint32_t*, cudaStream_t);
+template cudaError_t launch_evict_compact<PairSlot>(const PairSlot*, uint64_t, int64_t, uint64_t, uint64_t, const unsigned long long*,
+                                                    PairSlot*, uint32_t*, cudaStream_t);
+template cudaError_t launch_evict_compact<MetaSlot>(const MetaSlot*, uint64_t, int64_t, uint64_t, uint64_t, const unsigned long long*,
+                                                    MetaSlot*, uint32_t*, cudaStream_t);
+cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, uint32_t n_issuers, bool count, cudaStream_t s) {
     if (n == 0) return cudaSuccess;
-    evict_reinsert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st, keep, n);
+    evict_reinsert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st, keep, n, n_issuers, count);
+    return cudaGetLastError();
+}
+cudaError_t launch_ckpt_pairs(const DeviceState& st, const PairSlot* rec, uint64_t n, uint32_t n_issuers, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    ckpt_pairs_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st, rec, n, n_issuers);
+    return cudaGetLastError();
+}
+cudaError_t launch_ckpt_meta(const DeviceState& st, const MetaSlot* rec, uint64_t n, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    ckpt_meta_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st, rec, n);
     return cudaGetLastError();
 }
 

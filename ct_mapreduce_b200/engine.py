@@ -670,6 +670,30 @@ class GpuCertDatabase:
         snap = np.ascontiguousarray(snap, np.uint8)
         self._check(self._lib.ctmr_snapshot_load(self._h, capi.ptr(snap), snap.size))
 
+    def _checkpoint_fns(self):
+        return self._lib.ctmr_checkpoint_size, self._lib.ctmr_checkpoint_save, self._lib.ctmr_checkpoint_load
+
+    def checkpoint(self) -> np.ndarray:
+        """This db's part of a portable checkpoint (ctmr_checkpoint_save): loads into any table size, group size or number
+        of ranks.  On a db attached to peers it is collective, and every rank returns its own part."""
+        size, save, _ = self._checkpoint_fns()
+        need = C.c_uint64(0)
+        self._check(size(self._h, C.byref(need)))
+        buf = np.empty(max(need.value, 1), np.uint8)
+        wrote = C.c_uint64(0)
+        self._check(save(self._h, capi.ptr(buf), buf.size, C.byref(wrote)))
+        return buf[:wrote.value]
+
+    def load_checkpoint(self, parts):
+        """Replace the state with a checkpoint: `parts` = every part of it (a list of arrays, any order) or its one part.
+        Collective on a db attached to peers."""
+        if isinstance(parts, np.ndarray):
+            parts = [parts]
+        parts = [np.ascontiguousarray(p, np.uint8) for p in parts]
+        ptrs = (C.c_void_p * max(len(parts), 1))(*[p.ctypes.data for p in parts])
+        sizes = (C.c_uint64 * max(len(parts), 1))(*[p.size for p in parts])
+        self._check(self._checkpoint_fns()[2](self._h, ptrs, sizes, len(parts)))
+
     def evict_expired(self, now_unix_sec: int) -> int:
         """Apply the Redis TTLs (EXPIREAT(expDate) on every serials:: set, knowncertificates.go:98-104): sets with
         expDate <= now vanish.  Returns the number of serials dropped."""
@@ -837,6 +861,9 @@ class GpuCertGroup(GpuCertDatabase):
     def restore(self, snap: np.ndarray):
         snap = np.ascontiguousarray(snap, np.uint8)
         self._check(self._lib.ctmr_group_snapshot_load(self._h, capi.ptr(snap), snap.size))
+
+    def _checkpoint_fns(self):
+        return self._lib.ctmr_group_checkpoint_size, self._lib.ctmr_group_checkpoint_save, self._lib.ctmr_group_checkpoint_load
 
     def get_known_certificates(self, exp_hour: int, issuer_digest: bytes):
         grp = self

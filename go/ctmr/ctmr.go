@@ -25,6 +25,7 @@ import "C"
 
 import (
 	"fmt"
+	"runtime"
 	"unsafe"
 )
 
@@ -453,6 +454,56 @@ func (d *DB) Restore(snap []byte) error {
 		return d.err(C.ctmr_group_snapshot_load(d.g, (*C.uint8_t)(unsafe.Pointer(&snap[0])), C.uint64_t(len(snap))), "ctmr_group_snapshot_load")
 	}
 	return d.err(C.ctmr_snapshot_load(d.h, (*C.uint8_t)(unsafe.Pointer(&snap[0])), C.uint64_t(len(snap))), "ctmr_snapshot_load")
+}
+
+// Checkpoint returns this DB's part of a portable checkpoint (ctmr_checkpoint_save / ctmr_group_checkpoint_save): the
+// live records, not the slot layout, so it loads into any table size and any number of GPUs.  A DB attached to peers
+// (one process per GPU) saves its own part, collectively.
+func (d *DB) Checkpoint() ([]byte, error) {
+	var need, wrote C.uint64_t
+	var rc C.int
+	if d.g != nil {
+		rc = C.ctmr_group_checkpoint_size(d.g, &need)
+	} else {
+		rc = C.ctmr_checkpoint_size(d.h, &need)
+	}
+	if err := d.err(rc, "ctmr_checkpoint_size"); err != nil {
+		return nil, err
+	}
+	buf := make([]byte, int(need)+1) // never empty: &buf[0] is valid
+	if d.g != nil {
+		rc = C.ctmr_group_checkpoint_save(d.g, (*C.uint8_t)(unsafe.Pointer(&buf[0])), need, &wrote)
+	} else {
+		rc = C.ctmr_checkpoint_save(d.h, (*C.uint8_t)(unsafe.Pointer(&buf[0])), need, &wrote)
+	}
+	return buf[:int(wrote)], d.err(rc, "ctmr_checkpoint_save")
+}
+
+// LoadCheckpoint replaces the state with a checkpoint: every part of it, in any order.  The parts' addresses go to the
+// library in a C-allocated table, and the parts are pinned for the call (cgo's rule on Go pointers in C memory).
+func (d *DB) LoadCheckpoint(parts ...[]byte) error {
+	if len(parts) == 0 {
+		return fmt.Errorf("no checkpoint parts")
+	}
+	n := len(parts)
+	ptrs := (*[1 << 20]*C.uint8_t)(C.malloc(C.size_t(n) * C.size_t(unsafe.Sizeof(uintptr(0)))))[:n:n]
+	sizes := (*[1 << 20]C.uint64_t)(C.malloc(C.size_t(n) * 8))[:n:n]
+	defer C.free(unsafe.Pointer(&ptrs[0]))
+	defer C.free(unsafe.Pointer(&sizes[0]))
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for i, p := range parts {
+		if len(p) == 0 {
+			return fmt.Errorf("checkpoint part %d is empty", i)
+		}
+		pin.Pin(&p[0])
+		ptrs[i] = (*C.uint8_t)(unsafe.Pointer(&p[0]))
+		sizes[i] = C.uint64_t(len(p))
+	}
+	if d.g != nil {
+		return d.err(C.ctmr_group_checkpoint_load(d.g, &ptrs[0], &sizes[0], C.uint32_t(n)), "ctmr_group_checkpoint_load")
+	}
+	return d.err(C.ctmr_checkpoint_load(d.h, &ptrs[0], &sizes[0], C.uint32_t(n)), "ctmr_checkpoint_load")
 }
 
 func HostAlloc(n int) unsafe.Pointer { return C.ctmr_host_alloc(C.size_t(n)) }

@@ -187,10 +187,44 @@ int ctmr_evict_expired(ctmr_ctx* ctx, int64_t now_unix_sec, uint64_t* evicted_ou
 /* Snapshot of the derived device state (tables, histograms, issuer registry, next entry index) into a
  * caller buffer, and its restoration into a ctx created with the same capacities.  ctmr_snapshot_size
  * gives the bytes needed.  The reference's analogue is the state it keeps in Redis between runs
- * (storage/rediscache.go); its own resume logic is cmd/ct-fetch/ct-fetch.go:288-300. */
+ * (storage/rediscache.go); its own resume logic is cmd/ct-fetch/ct-fetch.go:288-300.
+ * To move the state into other capacities or another number of GPUs, use ctmr_checkpoint_* below. */
 int ctmr_snapshot_size(ctmr_ctx* ctx, uint64_t* bytes);
 int ctmr_snapshot_save(ctmr_ctx* ctx, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_snapshot_load(ctmr_ctx* ctx, const uint8_t* buf, uint64_t bytes);
+
+/* ---- portable checkpoint -------------------------------------------------------------------- */
+/* The live content of the state (not its slot layout), loadable into ANY shape: one ctx, a group of any size, or peer
+ * ranks of any world size, of any capacities that hold the content.  A checkpoint is one or more PARTS: a ctx or a group
+ * saves one part; a ctx attached to peers saves its own, so a world-rank deployment saves `world` parts.  A load takes
+ * every part of one checkpoint, in any order.  HOST buffers.
+ *
+ * Part layout (little-endian): a 128-byte header -- magic "CTMRCKP1", u32 part index, u32 part count, u64 n_issuers,
+ * u64 next_index, u64 status counters [CTMR_ST__COUNT] of this part, u64 keys, pairs, string identities, u64 0 -- then
+ * the registry digests [n_issuers][32] in dense-index order (every part carries the same list), the ready key slots
+ * (64 B each, as they lie in the table: inv_first keeps the first-seen index), the (issuer, hour) slots (32 B: key,
+ * inv_first, count) and the string identities (32 B).  Bytes = 128 + 32 n_issuers + 64 keys + 32 (pairs + strings).
+ * Two saves of one state are byte-equal.
+ *
+ * Save compacts the tables through a bounded staging buffer (no second table-sized allocation).  Load replaces the
+ * target's state: its tables are cleared, the registry rebuilt (digest i gets index i again), every member / rank
+ * inserts the records it owns under the TARGET's world (per-issuer counts are rebuilt from the keys), member 0 / rank 0
+ * holds the status counters (the sum over the parts), and the next index is the checkpoint's.  Like
+ * ctmr_snapshot_load, the Chain[0] mirror and the tiles' fingerprints are cleared: chain certificates are registered
+ * again and get the same dense indices.  Failures:
+ *   CTMR_E_INVALID          bad magic, truncation, parts that disagree (count, index given twice or missing,
+ *                           registry, next index), a NULL part: the target is untouched
+ *   CTMR_E_TOO_MANY_ISSUERS the registry exceeds the target's max_issuers: the target is untouched
+ *   CTMR_E_TABLE_FULL / CTMR_E_PAIR_TABLE_FULL / CTMR_E_META_TABLE_FULL (a target table too small), and
+ *   CTMR_E_INVALID for a record out of range (issuer >= n_issuers, serial longer than CTMR_MAX_SERIAL, a slot not
+ *   ready): the target is as after a reset with the checkpoint's registry, its next index unchanged
+ * On a ctx attached to peers the three calls are COLLECTIVE.  Save: a barrier, each rank writes its own part, a barrier.
+ * Load: the ranks agree on their checks before any change (a rank whose checks fail returns its error, the others
+ * CTMR_E_PEER_FAILED, nothing changes), and on the outcome of their inserts (a failure on one rank is every rank's).
+ * A member ctx of an in-process group is refused: use ctmr_group_checkpoint_*. */
+int ctmr_checkpoint_size(ctmr_ctx* ctx, uint64_t* bytes);
+int ctmr_checkpoint_save(ctmr_ctx* ctx, uint8_t* buf, uint64_t cap, uint64_t* written);
+int ctmr_checkpoint_load(ctmr_ctx* ctx, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
 
 /* ---- device-resident entry points ---------------------------------------------------------- */
 /* Same path with every buffer already in HBM on ctx's device (benchmarks, multi-GPU orchestration,
@@ -292,10 +326,14 @@ int ctmr_group_preload_known(ctmr_group* g, int64_t exp_hour, const uint8_t issu
 int ctmr_group_evict_expired(ctmr_group* g, int64_t now_unix_sec, uint64_t* evicted_out);
 int ctmr_group_reset(ctmr_group* g);
 /* snapshot of the whole group (every shard + the one issuer registry); restores into a group of the same size and
- * capacities (a set's owner depends on the group size) */
+ * capacities (a set's owner depends on the group size).  For another size or other capacities: ctmr_group_checkpoint_*. */
 int ctmr_group_snapshot_size(ctmr_group* g, uint64_t* bytes);
 int ctmr_group_snapshot_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
+/* portable checkpoint of the whole group: one part (every shard's records); loads any checkpoint (ctmr_checkpoint_*) */
+int ctmr_group_checkpoint_size(ctmr_group* g, uint64_t* bytes);
+int ctmr_group_checkpoint_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written);
+int ctmr_group_checkpoint_load(ctmr_group* g, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
 
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the

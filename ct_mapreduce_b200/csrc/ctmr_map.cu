@@ -172,6 +172,16 @@ __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant
 // the next chunk is copied after the walk, so the walker can still look back into the previous one).
 // Staging: per-lane cp.async 16-byte copies (LDGSTS) + commit/wait groups -- no barrier at all.
 // ------------------------------------------------------------------------------------------------
+// Timing experiments (tools/kmap_split.py compiles this file into libraries of its own with one or both set; libctmr.so
+// is built with neither): CTMR_KMAP_SKIP_WALK never calls the walker and stands a key made of the entry number in for
+// the serial, CTMR_KMAP_SKIP_HASH folds each block's 16 words into the state with XORs instead of compressing them.
+// Either makes the outputs wrong on purpose.
+#ifndef CTMR_KMAP_SKIP_WALK
+#define CTMR_KMAP_SKIP_WALK 0
+#endif
+#ifndef CTMR_KMAP_SKIP_HASH
+#define CTMR_KMAP_SKIP_HASH 0
+#endif
 __global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm) map_stream_kernel(const __grid_constant__ MapParams p) {
     using Cfg = StreamCfg;
     constexpr int WARPS = Cfg::kWarps, CHUNK = Cfg::kChunk;
@@ -237,7 +247,7 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm)
             if (c < nch) {
                 // ---- map: resume the TLV walk over the newly staged bytes
                 auto walk = [&] {
-                    if (act && w.st < W_DONE) {
+                    if (!CTMR_KMAP_SKIP_WALK && act && w.st < W_DONE) {
                         const uint32_t avail = min((c + 1u) * CHUNK, L);
                         walk_advance(w, SmemWindow{ring, m}, far, bad_span ? 0u : avail, L, p.filter, key_words);
                     }
@@ -262,7 +272,12 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm)
                                 wd[15] = L << 3;
                             }
                         }
+#if CTMR_KMAP_SKIP_HASH
+#pragma unroll
+                        for (int i = 0; i < 16; ++i) st.h[i & 7] ^= wd[i];
+#else
                         sha256_compress_rolled(st, wd, one);
+#endif
                     }
                 };
                 ring_step(c, m, yend, walk, copy, hash);
@@ -270,6 +285,16 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm)
             }
         }
         cp_async_wait<0>();  // nothing is in flight when the ring takes the warp's next records
+#if CTMR_KMAP_SKIP_WALK
+        if (act && !bad_span) {
+            w.st = W_DONE;
+            if (key_words) {
+                key_words[0] = 4u | ((uint32_t)e << 8);
+                key_words[1] = (uint32_t)e >> 24;
+                for (int i = 2; i < 10; ++i) key_words[i] = 0u;
+            }
+        }
+#endif
 
         // ---- certIsFilteredOut + Store preconditions, in the reference's order
         if (act) {
@@ -360,6 +385,10 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm)
 // histogram over 256 buckets, 256-entry scan, scatter.
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kLenBuckets = 256;
+// K_map's three resident CTAs hold 61,440 of an SM's 65,536 registers.  A 128-thread block of up to 32 registers fits
+// into the rest, a 256-thread block does not: it would wait until a K_map CTA of the round running on the other stream
+// retires, and K_map's next launch would wait behind it.
+constexpr uint32_t kLenThreads = 128;
 
 __device__ __forceinline__ uint32_t len_bucket(const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ lens, uint64_t e,
                                                uint64_t blob_bytes) {
@@ -370,15 +399,16 @@ __device__ __forceinline__ uint32_t len_bucket(const uint64_t* __restrict__ offs
     return (kLenBuckets - 1) - b;  // bucket 0 = longest
 }
 
-__global__ void __launch_bounds__(256) len_hist_kernel(const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ lens, uint64_t n, uint64_t blob_bytes,
+__global__ void __launch_bounds__(kLenThreads) len_hist_kernel(const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ lens, uint64_t n, uint64_t blob_bytes,
                                                        unsigned int* __restrict__ hist) {
     __shared__ unsigned int sh[kLenBuckets];
-    sh[threadIdx.x] = 0;
+    for (uint32_t b = threadIdx.x; b < kLenBuckets; b += blockDim.x) sh[b] = 0;
     __syncthreads();
     for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (uint64_t)gridDim.x * blockDim.x)
         atomicAdd(&sh[len_bucket(offsets, lens, e, blob_bytes)], 1u);
     __syncthreads();
-    if (sh[threadIdx.x]) atomicAdd(&hist[threadIdx.x], sh[threadIdx.x]);
+    for (uint32_t b = threadIdx.x; b < kLenBuckets; b += blockDim.x)
+        if (sh[b]) atomicAdd(&hist[b], sh[b]);
 }
 
 // exclusive scan of the 256 bucket counts by ONE WARP (8 buckets per lane + a shuffle scan): this tiny kernel sits on
@@ -405,7 +435,7 @@ __global__ void len_scan_kernel(unsigned int* hist_then_cursor) {
     }
 }
 
-__global__ void __launch_bounds__(256) len_scatter_kernel(const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ lens, uint64_t n, uint64_t blob_bytes,
+__global__ void __launch_bounds__(kLenThreads) len_scatter_kernel(const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ lens, uint64_t n, uint64_t blob_bytes,
                                                           unsigned int* __restrict__ cursor, uint32_t* __restrict__ order) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool in = e < n;
@@ -425,11 +455,11 @@ cudaError_t launch_len_order(const uint64_t* offsets, const uint32_t* lens, uint
     if (!n) return cudaSuccess;
     cudaError_t err = cudaMemsetAsync(hist256, 0, kLenBuckets * sizeof(unsigned int), s);
     if (err != cudaSuccess) return err;
-    const unsigned hb = (unsigned)((n + 256 * 8 - 1) / (256 * 8));
+    const unsigned hb = (unsigned)((n + kLenThreads * 8 - 1) / (kLenThreads * 8));
     const unsigned cap = (unsigned)sm_count * 8u;
-    len_hist_kernel<<<hb < cap ? (hb ? hb : 1u) : cap, 256, 0, s>>>(offsets, lens, n, blob_bytes, hist256);
+    len_hist_kernel<<<hb < cap ? (hb ? hb : 1u) : cap, kLenThreads, 0, s>>>(offsets, lens, n, blob_bytes, hist256);
     len_scan_kernel<<<1, 32, 0, s>>>(hist256);
-    len_scatter_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(offsets, lens, n, blob_bytes, hist256, order);
+    len_scatter_kernel<<<(unsigned)((n + kLenThreads - 1) / kLenThreads), kLenThreads, 0, s>>>(offsets, lens, n, blob_bytes, hist256, order);
     return cudaGetLastError();
 }
 

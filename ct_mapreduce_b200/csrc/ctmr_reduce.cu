@@ -281,7 +281,9 @@ cudaError_t launch_insert(const DeviceState& st, const ctmr_key* keys, uint64_t 
 cudaError_t launch_resolve(const DeviceState& st, const ctmr_key* keys, uint64_t m, const uint32_t* slot_of,
                            uint32_t* pair_slot, uint8_t* was_unknown, cudaStream_t s) {
     if (!m) return cudaSuccess;
-    resolve_kernel<<<blocks_for(m, 256), 256, 0, s>>>(st, keys, m, slot_of, pair_slot, was_unknown);
+    // 128 threads: the block fits beside K_map's three resident CTAs (ctmr_map.cu, kLenThreads), so the pass runs under
+    // the next round's K_map instead of waiting for its CTAs to retire
+    resolve_kernel<<<blocks_for(m, 128), 128, 0, s>>>(st, keys, m, slot_of, pair_slot, was_unknown);
     return cudaGetLastError();
 }
 cudaError_t launch_resolve_pairs(const DeviceState& st, const ctmr_key* keys, uint64_t m, const uint32_t* pair_slot,

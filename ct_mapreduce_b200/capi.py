@@ -50,6 +50,7 @@ EXPORTS = [
     "ctmr_peer_export", "ctmr_peer_attach", "ctmr_peer_barrier_device", "ctmr_peer_allreduce_histogram_device",
     "ctmr_bind_host_to_device", "ctmr_peer_rounds", "ctmr_peer_round_entries", "ctmr_peer_frontend_stopped",
     "ctmr_next_index",
+    "ctmr_revoked_known", "ctmr_group_revoked_known",   # CRLs joined with the known-certificate sets
 ]
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -60,6 +61,11 @@ def peer_rounds() -> int:
 E_PAIR_TABLE_FULL, E_META_TABLE_FULL, E_PEER_TIMEOUT, E_PEER = -8, -9, -10, -11
 E_UNKNOWN_ISSUER = -12
 E_PEER_FAILED = -13   # another rank's part of a collective call failed before any work
+# CRL and entry status of ctmr_revoked_known (include/ctmr.h CTMR_CRL_* / CTMR_RV_*)
+CRL_OK, CRL_BAD, CRL_BAD_ENTRIES, CRL_UNKNOWN_ISSUER = range(4)
+RV_OK, RV_INDIRECT, RV_SERIAL_TOO_LONG = range(3)
+CRL_F_DELTA, CRL_F_IDP = 1, 2
+CRL_MIN_ENTRY = 18     # bytes of the smallest revokedCertificates entry: entry_cap = total CRL bytes // 18 suffices
 # per-entry outcome of the front end (include/ctmr_frontend.h CTMR_FE_*)
 FE_OK, FE_BAD_BASE64, FE_BAD_LEAF, FE_UNKNOWN_TYPE, FE_BAD_EXTRA, FE_BAD_CERT, FE_BAD_TILE, FE_BAD_INDEX = range(8)
 # body status of ctmr_process_raw_bodies (include/ctmr_frontend.h CTMR_BODY_*)
@@ -141,6 +147,21 @@ class TileOut(C.Structure):
 class Tree(C.Structure):
     """ctmr_tree (include/ctmr_frontend.h): the Merkle tree of one log as its right edge."""
     _fields_ = [("size", C.c_uint64), ("edge", (C.c_uint8 * 32) * 64), ("root", C.c_uint8 * 32)]
+
+
+class CrlBatch(C.Structure):
+    """ctmr_crl_batch (include/ctmr.h)."""
+    _fields_ = [("data", C.c_void_p), ("data_bytes", C.c_uint64), ("crl_off", C.c_void_p), ("crl_len", C.c_void_p),
+                ("issuer_digest", C.c_void_p), ("n_crls", C.c_uint64)]
+
+
+class CrlOut(C.Structure):
+    """ctmr_crl_out (include/ctmr.h)."""
+    _fields_ = [(n, C.c_void_p) for n in
+                ("crl_status", "crl_flags", "this_update", "next_update", "tbs_off", "tbs_len", "issuer_name_off",
+                 "issuer_name_len", "crl_first", "crl_entries", "serial_off", "serial_len", "revoked_at", "reason",
+                 "entry_status", "known", "known_exp_hour", "known_sets")] + \
+               [("entry_cap", C.c_uint64), ("n_entries", C.c_uint64)]
 
 
 class SynthCfg(C.Structure):
@@ -276,6 +297,8 @@ def load():
     L.ctmr_peer_round_entries.restype = u64
     L.ctmr_peer_frontend_stopped.argtypes = [vp, C.POINTER(u32)]
     L.ctmr_next_index.argtypes = [vp, C.POINTER(u64)]
+    L.ctmr_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
+    L.ctmr_group_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
     for name in EXPORTS:
         getattr(L, name)  # every symbol include/ctmr.h declares must resolve
     _lib = L

@@ -290,6 +290,34 @@ struct FrontEnd {
     std::unique_ptr<BodyState> bd;    // bodies_ensure
 };
 
+// ctmr_revoked_known: the double-buffered staging of whole CRLs, the split's per-byte, per-candidate and per-entry
+// buffers (allocated on the first call, for chunks of `budget` bytes), and the join's set (grown to the largest chunk).
+// A group's members 1.. hold only the set arrays: a copy of member 0's set and their own answers.
+struct CrlState {
+    uint64_t budget = 0, cap_crls = 0, cap_cand = 0, cap_entries = 0;
+    Stream copy_stream;
+    DevBuf<uint8_t> stage[2];       // [budget + 64] each
+    DevBuf<CrlDesc> desc[2];        // [cap_crls] each
+    HostBuf<CrlDesc> h_desc[2];
+    Event uploaded[2], consumed[2];
+    DevBuf<CrlRes> res;             // [cap_crls]
+    DevBuf<uint32_t> cnt16, off16;  // [budget / 16 + 1]: candidates per 16 staged bytes and their exclusive scan
+    DevBuf<uint32_t> cpos, ccrl, link, jump[2];  // [cap_cand]
+    DevBuf<uint8_t> mark;           // [cap_cand]
+    DevBuf<uint8_t> temp;           // cub scans
+    size_t temp_bytes = 0;
+    // per entry [cap_entries]
+    DevBuf<uint32_t> epos, ecrl, eslot, esets;
+    DevBuf<uint64_t> eserial_off;
+    DevBuf<uint8_t> eserial_len, ereason, estatus, eknown;
+    DevBuf<int64_t> erevoked, ehour;
+    // the set of a chunk's (issuer, serial) pairs, and per pair the lowest hour and the number of sets holding it
+    uint64_t set_cap = 0;
+    DevBuf<CrlSetSlot> set;
+    DevBuf<int32_t> set_hour, recv_hour;   // recv_*: a group's member 0 receives the other members' answers there
+    DevBuf<uint32_t> set_count, recv_count;
+};
+
 // the ctx's private device words (one allocation)
 struct SmallDev {
     unsigned long long slots_used;   // DeviceState::slots_used points here (no kernel reads it)
@@ -383,6 +411,7 @@ struct ctmr_ctx {
     DevBuf<SmallDev> small;
     std::unique_ptr<FrontEnd> fe;
     uint32_t fe_peer_stopped = 0;  // ranks that stopped (tiles) in the last collective front-end call
+    std::unique_ptr<CrlState> crl;  // ctmr_revoked_known (ctmr_crl.cu)
     std::string err;
 };
 

@@ -472,4 +472,34 @@ cudaError_t launch_range_fold(const FoldChunk& f, const FoldTree* hdesc, uint8_t
 // when its begin is the tree's size, so that a tree stopped earlier keeps its size.
 cudaError_t launch_tree_merge(TreeDev* trees, uint32_t n, const RangeSet& set, cudaStream_t s);
 
+// ---- revoked known certificates (ctmr_crl.cu, ctmr_revoked_known) -----------------------------------------------------
+// one CRL of a chunk as uploaded
+struct CrlDesc {
+    uint64_t data_off;  // in ctmr_crl_batch.data
+    uint32_t staged;    // in the chunk's staging buffer
+    uint32_t len;
+    uint32_t issuer;    // dense issuer index, CTMR_ISSUER_NONE when the digest is not registered
+    uint32_t pad;
+};
+static_assert(sizeof(CrlDesc) == 24, "CrlDesc layout");
+
+// what crl_frame and the split leave per CRL of a chunk
+struct CrlRes {
+    int64_t this_update, next_update;
+    uint64_t tbs_off, name_off;  // absolute in ctmr_crl_batch.data
+    uint32_t tbs_len, name_len;
+    uint32_t cs, ce;             // revokedCertificates content span, staged positions (cs == ce: no entries)
+    uint32_t first, count;       // the CRL's entries in the chunk's entry arrays
+    uint32_t status, flags;      // CTMR_CRL_*, CTMR_CRL_F_*
+    uint32_t done, bad;          // the chain reached the content's end / an entry is malformed
+};
+static_assert(sizeof(CrlRes) == 72, "CrlRes layout");
+
+// one (issuer, serial) pair of the join: the key as words 1..11 of a KnownSlot body (issuer, {serial_len, serial[39]})
+struct CrlSetSlot {
+    uint32_t tag;  // 0 empty | (hash & ~3) | 1 pending | (hash & ~3) | 2 ready
+    uint32_t key[11];
+};
+static_assert(sizeof(CrlSetSlot) == 48, "CrlSetSlot layout");
+
 }  // namespace ctmr

@@ -10,6 +10,8 @@ points, and exposes the results under the reference's names:
                                        <- KnownCertificates.Count (storage/knowncertificates.go:57-63)
     GpuCertDatabase.issuer_counts      <- the per-issuer sum of cmd/storage-statistics/storage-statistics.go:44-53
     GpuCertDatabase.status_counters    <- metrics certIsFilteredOut.{CA,expired,cn-filtered}, insertCTWorker.Inserted
+    GpuCertDatabase.revoked_known      <- the join CRLite makes of an issuer's CRLs (crl::<issuer>) with its
+                                          serials::<expDate>::<issuer> sets (storage/knowncertificates.go:28-55)
 
 All arithmetic happens in the CUDA kernels; nothing here parses, hashes or de-duplicates.
 """
@@ -185,6 +187,50 @@ class TileBatchResult(RawBatchResult):
         self.tile_status = np.zeros(n_tiles, np.uint8)
         self.tiles_done = 0
         self.missing = []   # fingerprints (bytes) of the unregistered Chain[0] certificates of tile `tiles_done`
+
+
+class RevokedResult:
+    """Outputs of ctmr_revoked_known (include/ctmr.h ctmr_crl_out): per CRL, and per entry of the listed CRLs."""
+
+    _CRL = (("crl_status", np.uint8), ("crl_flags", np.uint8), ("this_update", np.int64), ("next_update", np.int64),
+            ("tbs_off", np.uint64), ("tbs_len", np.uint32), ("issuer_name_off", np.uint64), ("issuer_name_len", np.uint32),
+            ("crl_first", np.uint64), ("crl_entries", np.uint32))
+    _ENTRY = (("serial_off", np.uint64), ("serial_len", np.uint8), ("revoked_at", np.int64), ("reason", np.uint8),
+              ("entry_status", np.uint8), ("known", np.uint8), ("known_exp_hour", np.int64), ("known_sets", np.uint32))
+
+    def __init__(self, n_crls: int, entry_cap: int):
+        for name, dt in self._CRL:
+            setattr(self, name, np.zeros(n_crls, dt))
+        for name, dt in self._ENTRY:
+            setattr(self, name, np.zeros(max(entry_cap, 1), dt))
+        self.entry_cap = entry_cap
+        self.n_entries = 0
+
+    def to_c(self) -> "capi.CrlOut":
+        o = capi.CrlOut()
+        for name, _ in self._CRL + self._ENTRY:
+            setattr(o, name, getattr(self, name).ctypes.data)
+        o.entry_cap = self.entry_cap
+        return o
+
+    def trim(self, n: int):
+        for name, _ in self._ENTRY:
+            setattr(self, name, getattr(self, name)[:n])
+        self.n_entries = n
+
+    def serial(self, data: np.ndarray, e: int) -> bytes:
+        o = int(self.serial_off[e])
+        return bytes(data[o:o + int(self.serial_len[e])])
+
+
+def pack_crls(crls):
+    """(data, crl_off, crl_len) of a list of DER CRLs laid back to back."""
+    lens = np.array([len(c) for c in crls], np.uint64)
+    offs = np.zeros(len(crls), np.uint64)
+    if len(crls) > 1:
+        offs[1:] = np.cumsum(lens)[:-1]
+    data = np.frombuffer(b"".join(bytes(c) for c in crls), np.uint8) if crls else np.zeros(0, np.uint8)
+    return data, offs, lens
 
 
 class GpuCertDatabase:
@@ -673,6 +719,37 @@ class GpuCertDatabase:
     def _checkpoint_fns(self):
         return self._lib.ctmr_checkpoint_size, self._lib.ctmr_checkpoint_save, self._lib.ctmr_checkpoint_load
 
+    def _revoked_known_fn(self):
+        return self._lib.ctmr_revoked_known
+
+    def revoked_known(self, crls, issuer_digests, entry_cap: int | None = None) -> RevokedResult:
+        """Which revoked serials of these CRLs are known certificates (ctmr_revoked_known).  `crls`: a list of DER CRLs,
+        or (data, crl_off, crl_len); `issuer_digests`: per CRL the 32-byte Issuer.ID() digest whose crl:: set named it.
+        Read-only.  entry_cap defaults to the bound that always suffices (total bytes // 18)."""
+        if isinstance(crls, tuple):
+            data, offs, lens = (np.ascontiguousarray(a) for a in crls)
+            data, offs, lens = data.astype(np.uint8, copy=False), offs.astype(np.uint64), lens.astype(np.uint64)
+        else:
+            data, offs, lens = pack_crls(crls)
+        n = len(offs)
+        dig = np.frombuffer(b"".join(bytes(d) for d in issuer_digests), np.uint8) if n else np.zeros(32, np.uint8)
+        if dig.size != 32 * n:
+            raise ValueError("one 32-byte issuer digest per CRL")
+        cap = int(lens.sum()) // capi.CRL_MIN_ENTRY if entry_cap is None else int(entry_cap)
+        res = RevokedResult(n, cap)
+        b = capi.CrlBatch(capi.ptr(data) if data.size else None, data.size, capi.ptr(offs) if n else None,
+                          capi.ptr(lens) if n else None, capi.ptr(dig) if n else None, n)
+        o = res.to_c()
+        rc = self._revoked_known_fn()(self._h, C.byref(b), C.byref(o))
+        res.n_entries = int(o.n_entries)
+        try:
+            self._check(rc)
+        except CtmrError as e:
+            e.n_entries = res.n_entries  # CTMR_E_BATCH_TOO_LARGE: the entry_cap that suffices
+            raise
+        res.trim(int(o.n_entries))
+        return res
+
     def checkpoint(self) -> np.ndarray:
         """This db's part of a portable checkpoint (ctmr_checkpoint_save): loads into any table size, group size or number
         of ranks.  On a db attached to peers it is collective, and every rank returns its own part."""
@@ -864,6 +941,9 @@ class GpuCertGroup(GpuCertDatabase):
 
     def _checkpoint_fns(self):
         return self._lib.ctmr_group_checkpoint_size, self._lib.ctmr_group_checkpoint_save, self._lib.ctmr_group_checkpoint_load
+
+    def _revoked_known_fn(self):
+        return self._lib.ctmr_group_revoked_known
 
     def get_known_certificates(self, exp_hour: int, issuer_digest: bytes):
         grp = self

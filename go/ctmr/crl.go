@@ -1,0 +1,126 @@
+package ctmr
+
+/*
+#include <stdlib.h>
+#include "ctmr.h"
+*/
+import "C"
+
+import (
+	"unsafe"
+)
+
+// Revoked is one revokedCertificates entry of a CRL handed to RevokedKnown, with its join against the
+// "serials::<expDate>::<issuer>" sets the table holds.
+type Revoked struct {
+	Serial       []byte // INTEGER content octets (a view into the caller's CRL bytes)
+	RevokedAt    int64  // unix seconds
+	Reason       uint8  // reasonCode, 0xFF when absent
+	Status       uint8  // CTMR_RV_*
+	Known        bool   // some set serials::<h>::<issuer> holds the serial
+	KnownExpHour int64  // the lowest such h
+	KnownSets    uint32 // how many such h
+}
+
+// CRLResult is what RevokedKnown reports for one CRL.
+type CRLResult struct {
+	Status     uint8 // CTMR_CRL_*
+	Flags      uint8 // bit 0 deltaCRLIndicator, bit 1 issuingDistributionPoint
+	ThisUpdate int64
+	NextUpdate int64 // math.MinInt64 when absent
+	TBS        []byte // the signed bytes: verify the CRL's signature over them
+	Entries    []Revoked
+}
+
+// RevokedKnown parses DER CRLs on the GPU and answers, per entry, whether the serial is a known certificate of the
+// issuer whose crl:: set named the CRL (issuerIDs[i] is that Issuer.ID() digest, 32 bytes).  Read-only.  On a DB
+// attached to peers the library refuses the call.
+func (d *DB) RevokedKnown(crls [][]byte, issuerIDs [][32]byte) ([]CRLResult, error) {
+	n := len(crls)
+	if n == 0 {
+		return nil, nil
+	}
+	total := 0
+	for _, c := range crls {
+		total += len(c)
+	}
+	// flat C copies of the inputs: the batch struct itself holds pointers
+	data := C.malloc(C.size_t(total + 1))
+	defer C.free(data)
+	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8 * n)))[:n:n]
+	lens := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8 * n)))[:n:n]
+	dig := C.malloc(C.size_t(32 * n))
+	defer C.free(unsafe.Pointer(&offs[0]))
+	defer C.free(unsafe.Pointer(&lens[0]))
+	defer C.free(dig)
+	flat := unsafe.Slice((*byte)(data), total+1)
+	o := 0
+	for i, c := range crls {
+		copy(flat[o:], c)
+		offs[i], lens[i] = C.uint64_t(o), C.uint64_t(len(c))
+		copy(unsafe.Slice((*byte)(dig), 32*n)[32*i:], issuerIDs[i][:])
+		o += len(c)
+	}
+	capEntries := total/18 + 1
+	b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
+	defer C.free(unsafe.Pointer(b))
+	b.data, b.data_bytes = (*C.uint8_t)(data), C.uint64_t(total)
+	b.crl_off, b.crl_len = &offs[0], &lens[0]
+	b.issuer_digest, b.n_crls = (*C.uint8_t)(dig), C.uint64_t(n)
+	out := (*C.ctmr_crl_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_out{}))))
+	defer C.free(unsafe.Pointer(out))
+	alloc := func(per, count int) unsafe.Pointer {
+		p := C.calloc(C.size_t(count), C.size_t(per))
+		return p
+	}
+	ptrs := []unsafe.Pointer{
+		alloc(1, n), alloc(1, n), alloc(8, n), alloc(8, n), alloc(8, n), alloc(4, n), alloc(8, n), alloc(4, n),
+		alloc(8, capEntries), alloc(1, capEntries), alloc(8, capEntries), alloc(1, capEntries), alloc(1, capEntries),
+		alloc(1, capEntries), alloc(8, capEntries), alloc(4, capEntries),
+	}
+	for _, p := range ptrs {
+		defer C.free(p)
+	}
+	out.crl_status, out.crl_flags = (*C.uint8_t)(ptrs[0]), (*C.uint8_t)(ptrs[1])
+	out.this_update, out.next_update = (*C.int64_t)(ptrs[2]), (*C.int64_t)(ptrs[3])
+	out.tbs_off, out.tbs_len = (*C.uint64_t)(ptrs[4]), (*C.uint32_t)(ptrs[5])
+	out.crl_first, out.crl_entries = (*C.uint64_t)(ptrs[6]), (*C.uint32_t)(ptrs[7])
+	out.serial_off, out.serial_len = (*C.uint64_t)(ptrs[8]), (*C.uint8_t)(ptrs[9])
+	out.revoked_at, out.reason = (*C.int64_t)(ptrs[10]), (*C.uint8_t)(ptrs[11])
+	out.entry_status, out.known = (*C.uint8_t)(ptrs[12]), (*C.uint8_t)(ptrs[13])
+	out.known_exp_hour, out.known_sets = (*C.int64_t)(ptrs[14]), (*C.uint32_t)(ptrs[15])
+	out.entry_cap = C.uint64_t(capEntries)
+	var rc C.int
+	if d.g != nil {
+		rc = C.ctmr_group_revoked_known(d.g, b, out)
+	} else {
+		rc = C.ctmr_revoked_known(d.h, b, out)
+	}
+	if err := d.err(rc, "ctmr_revoked_known"); err != nil {
+		return nil, err
+	}
+	u8 := func(i, cnt int) []uint8 { return unsafe.Slice((*uint8)(ptrs[i]), cnt) }
+	i64 := func(i, cnt int) []int64 { return unsafe.Slice((*int64)(ptrs[i]), cnt) }
+	u64 := func(i, cnt int) []uint64 { return unsafe.Slice((*uint64)(ptrs[i]), cnt) }
+	u32 := func(i, cnt int) []uint32 { return unsafe.Slice((*uint32)(ptrs[i]), cnt) }
+	ne := int(out.n_entries)
+	res := make([]CRLResult, n)
+	for k := 0; k < n; k++ {
+		base := int(offs[k])
+		r := CRLResult{Status: u8(0, n)[k], Flags: u8(1, n)[k], ThisUpdate: i64(2, n)[k], NextUpdate: i64(3, n)[k]}
+		if r.Status == C.CTMR_CRL_OK || r.Status == C.CTMR_CRL_UNKNOWN_ISSUER {
+			to := int(u64(4, n)[k]) - base
+			r.TBS = crls[k][to : to+int(u32(5, n)[k])]
+		}
+		first, cnt := int(u64(6, n)[k]), int(u32(7, n)[k])
+		for e := first; e < first+cnt && e < ne; e++ {
+			so := int(u64(8, ne)[e]) - base
+			r.Entries = append(r.Entries, Revoked{
+				Serial: crls[k][so : so+int(u8(9, ne)[e])], RevokedAt: i64(10, ne)[e], Reason: u8(11, ne)[e],
+				Status: u8(12, ne)[e], Known: u8(13, ne)[e] != 0, KnownExpHour: i64(14, ne)[e], KnownSets: u32(15, ne)[e],
+			})
+		}
+		res[k] = r
+	}
+	return res, nil
+}

@@ -226,6 +226,70 @@ int ctmr_checkpoint_size(ctmr_ctx* ctx, uint64_t* bytes);
 int ctmr_checkpoint_save(ctmr_ctx* ctx, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_checkpoint_load(ctmr_ctx* ctx, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
 
+/* ---- revoked known certificates (CRLite's join of CRLs with the serials:: sets) ------------------- */
+/* Which revoked serials of an issuer's CRLs are known certificates, and in which "serials::<expDate>::<issuer>" set
+ * (storage/knowncertificates.go:28-55)?  A CRL entry carries no expiry, so the set cannot be named; the call parses the
+ * CRLs on the GPU (DESIGN.md "Revoked known certificates") and answers every entry from one pass over the table per chunk.
+ *
+ * Rules (RFC 5280 §5.1).  CertificateList ::= SEQUENCE { tbsCertList, AlgorithmIdentifier, BIT STRING } with nothing after
+ * the signatureValue and nothing after the outer SEQUENCE.  TBSCertList: version INTEGER OPTIONAL (absent = v1, else 1 =
+ * v2), signature AlgorithmIdentifier, issuer Name, thisUpdate Time, nextUpdate Time OPTIONAL, revokedCertificates SEQUENCE
+ * OF entry OPTIONAL (absent = no entries), [0] EXPLICIT crlExtensions OPTIONAL, nothing after.  An entry is SEQUENCE {
+ * userCertificate INTEGER (at least one octet), revocationDate Time, crlEntryExtensions Extensions OPTIONAL } with nothing
+ * after it; a reasonCode (2.5.29.21) must be an ENUMERATED of one octet.  TLV headers and Time follow the certificate
+ * walker (single-octet tags, minimal definite lengths; UTCTime pivots at 50, GeneralizedTime accepted).  Signatures are
+ * not verified: tbs_off / tbs_len give the host the signed bytes.  Parity with Go's x509.ParseDERCRL /
+ * ParseRevocationList is not pinned (as for ct-go in the front end): serials need not be minimal INTEGERs here.
+ *
+ * Match.  An entry is joined when its CRL is CTMR_CRL_OK and the entry is CTMR_RV_OK: its serial's raw content octets
+ * must equal a key's raw serial (NewSerial, storage/types.go:171-178) under the dense issuer of issuer_digest.  Minimal
+ * encodings of one integer are equal bytes; a non-minimal encoding on either side (00 01 against 01) does not match.
+ *
+ * Sizing.  The smallest entry is 18 bytes (SEQUENCE 2 + INTEGER 3 + a UTCTime without seconds 13), so entry_cap =
+ * (total CRL bytes) / 18 always suffices.  With a smaller entry_cap the call writes only n_entries (the count needed) and
+ * returns CTMR_E_BATCH_TOO_LARGE.  The CRLs are staged in chunks of whole CRLs of at most min(config.max_batch_bytes
+ * as the pipeline caps it, 256 MiB) bytes, each chunk one pass over the table; a CRL larger than a chunk is
+ * CTMR_E_BATCH_TOO_LARGE before any work.
+ *
+ * Read-only: no index is taken and no table, counter or registry changes, so the call may come between any other calls.
+ * A member ctx of a group (use ctmr_group_revoked_known) and a ctx attached to peers are refused with CTMR_E_INVALID.
+ * Out of scope: signature verification, fetching, and the semantics of delta and indirect CRLs beyond crl_flags and
+ * CTMR_RV_INDIRECT. */
+enum { CTMR_CRL_OK = 0, CTMR_CRL_BAD = 1,          /* CertificateList / TBSCertList framing or fields */
+       CTMR_CRL_BAD_ENTRIES = 2,                   /* revokedCertificates does not split into well-formed entries */
+       CTMR_CRL_UNKNOWN_ISSUER = 3 };              /* digest not in the registry: parsed, nothing joined */
+enum { CTMR_RV_OK = 0, CTMR_RV_INDIRECT = 1,       /* certificateIssuer entry extension (2.5.29.29): not joined */
+       CTMR_RV_SERIAL_TOO_LONG = 2 };              /* longer than CTMR_MAX_SERIAL: no key can hold it */
+#define CTMR_CRL_F_DELTA 1u                        /* crl_flags: deltaCRLIndicator (2.5.29.27) */
+#define CTMR_CRL_F_IDP 2u                          /* crl_flags: issuingDistributionPoint (2.5.29.28) */
+
+typedef struct ctmr_crl_batch {                    /* HOST buffers */
+    const uint8_t* data; uint64_t data_bytes;
+    const uint64_t* crl_off; const uint64_t* crl_len;   /* [n_crls] DER CertificateList */
+    const uint8_t* issuer_digest;                       /* [n_crls][32] Issuer.ID() digest whose crl:: set named the URL */
+    uint64_t n_crls;
+} ctmr_crl_batch;
+
+typedef struct ctmr_crl_out {                      /* caller-allocated, any pointer may be NULL */
+    uint8_t* crl_status; uint8_t* crl_flags;       /* [n_crls] bit 0 deltaCRLIndicator, bit 1 issuingDistributionPoint */
+    int64_t* this_update; int64_t* next_update;    /* unix seconds; next_update INT64_MIN when absent */
+    uint64_t* tbs_off; uint32_t* tbs_len;          /* tbsCertList span: the host verifies the signature without a parse */
+    uint64_t* issuer_name_off; uint32_t* issuer_name_len;
+    uint64_t* crl_first; uint32_t* crl_entries;    /* the CRL's entries in the per-entry arrays */
+    uint64_t* serial_off; uint8_t* serial_len;     /* [entry_cap] absolute in data: INTEGER content octets */
+    int64_t* revoked_at; uint8_t* reason;          /* reasonCode (2.5.29.21), 0xFF when absent */
+    uint8_t* entry_status;                         /* CTMR_RV_* */
+    uint8_t* known;                                /* 1 iff a set serials::<h>::<issuer> in the table holds the serial */
+    int64_t* known_exp_hour;                       /* the lowest such h (0 when not known) */
+    uint32_t* known_sets;                          /* how many such h (more than 1 = serial reuse) */
+    uint64_t entry_cap;
+    uint64_t n_entries;                            /* written; on CTMR_E_BATCH_TOO_LARGE the count needed */
+} ctmr_crl_out;
+/* Per CRL: CTMR_CRL_BAD and CTMR_CRL_BAD_ENTRIES CRLs have no entries (crl_entries 0) and only crl_status is meaningful;
+ * CTMR_CRL_OK and CTMR_CRL_UNKNOWN_ISSUER CRLs list every entry in order, entries of the CRLs back to back in CRL order.
+ * On a failed call (rc != 0) the outputs other than n_entries are undefined. */
+int ctmr_revoked_known(ctmr_ctx* ctx, const ctmr_crl_batch* batch, ctmr_crl_out* out);
+
 /* ---- device-resident entry points ---------------------------------------------------------- */
 /* Same path with every buffer already in HBM on ctx's device (benchmarks, multi-GPU orchestration,
  * hosts that receive entries by GPUDirect).  `stream` is a cudaStream_t passed as void*; NULL =
@@ -334,6 +398,9 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
 int ctmr_group_checkpoint_size(ctmr_group* g, uint64_t* bytes);
 int ctmr_group_checkpoint_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_group_checkpoint_load(ctmr_group* g, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
+/* ctmr_revoked_known over every shard: member 0 parses the CRLs and builds the set of (issuer, serial) pairs, each member
+ * scans its own table against a bulk copy of it, and member 0 merges the answers (lowest hour, sum of sets). */
+int ctmr_group_revoked_known(ctmr_group* g, const ctmr_crl_batch* batch, ctmr_crl_out* out);
 
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the

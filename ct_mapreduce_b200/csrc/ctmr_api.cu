@@ -410,6 +410,29 @@ int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s) {
     CU(c, launch_peer_barrier(c->pf, channel, ++c->epoch[channel], c->st.error_flag, s));
     return CTMR_OK;
 }
+
+// The second barrier keeps every rank from posting the next word before each rank has read this one.  The row is valid
+// only if no barrier timed out.
+int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row) {
+    CU(c, launch_peer_post(c->pf, mine, c->stream));
+    int rc = peer_barrier(c, CH_MAILBOX, c->stream);
+    if (rc) return rc;
+    CU(c, cudaMemcpyAsync(row, c->pf.flags[c->pf.rank] + (size_t)kPeerChannels * kMaxWorld, kMaxWorld * sizeof(uint64_t),
+                          cudaMemcpyDeviceToHost, c->stream));
+    rc = peer_barrier(c, CH_MAILBOX, c->stream);
+    if (rc) return rc;
+    CU(c, cudaStreamSynchronize(c->stream));
+    return CTMR_OK;
+}
+
+int PathOut::allocate(ctmr_ctx* c, uint64_t entries) {
+    cap = entries;
+    CU(c, alloc(status, entries)); CU(c, alloc(sha, entries * 32)); CU(c, alloc(was_unknown, entries)); CU(c, alloc(first, entries));
+    CU(c, alloc(exp_hour, entries)); CU(c, alloc(serial_off, entries)); CU(c, alloc(serial_len, entries));
+    CU(c, alloc(spans, 4 * entries)); CU(c, alloc(first_meta, 2 * entries));
+    CU(c, create(mapped)); CU(c, create(reduced)); CU(c, create(meta_done));
+    return CTMR_OK;
+}
 }  // namespace ctmr_host
 
 namespace {
@@ -526,9 +549,8 @@ int ensure_frontend(ctmr_ctx* c) {
     CU(c, alloc(f->leaf_abs, E)); CU(c, alloc(f->chain_abs, E)); CU(c, alloc(f->tbs_abs, E));
     CU(c, alloc(f->leaf_rel, E)); CU(c, alloc(f->leaf_len_out, E)); CU(c, alloc(f->chain_len, E)); CU(c, alloc(f->tbs_len, E));
     CU(c, alloc(f->issuer_idx, E));
-    CU(c, alloc(f->status, E)); CU(c, alloc(f->sha, E * 32)); CU(c, alloc(f->was_unknown, E)); CU(c, alloc(f->first, E));
-    CU(c, alloc(f->first_meta, 2 * E));
-    CU(c, alloc(f->exp_hour, E)); CU(c, alloc(f->serial_off, E)); CU(c, alloc(f->serial_len, E)); CU(c, alloc(f->spans, 4 * E));
+    int rc = f->out.allocate(c, E);
+    if (rc) return rc;
     f->slot_mask = pow2_at_least(4ull * c->st.max_issuers) - 1;
     CU(c, alloc(f->slots_dev, f->slot_mask + 1));
     f->slots_host.assign(f->slot_mask + 1, IssuerCertSlot{});
@@ -540,9 +562,8 @@ int ensure_frontend(ctmr_ctx* c) {
     CU(c, cudaMemsetAsync(f->slots_dev, 0, (f->slot_mask + 1) * sizeof(IssuerCertSlot), c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     CU(c, create(f->ev0, cudaEventDefault)); CU(c, create(f->ev1, cudaEventDefault)); CU(c, create(f->ev2, cudaEventDefault));
-    CU(c, create(f->mapped)); CU(c, create(f->reduced)); CU(c, create(f->meta_done));
     for (const auto& kv : c->issuer_by_der) {  // certificates registered before the front end existed
-        int rc = fe_add_issuer(c, f.get(), kv.first, kv.second);
+        rc = fe_add_issuer(c, f.get(), kv.first, kv.second);
         if (rc) return rc;
     }
     c->fe = std::move(f);

@@ -1,6 +1,7 @@
 // ctmr_ctx.cuh -- internal: the context behind the opaque ctmr_ctx of include/ctmr.h, shared by the translation
 // units that implement the C ABI (ctmr_api.cu: lifecycle, issuers, the steps of a round and run_round, which sequences
-// one round of the key exchange for all three callers, device entry points, read side, front end plumbing;
+// one round of the key exchange for all three callers, the ranks' barriers and mailbox, device entry points, read side,
+// front end plumbing;
 // ctmr_pipeline.cu: the host-buffer batch pipeline on one GPU, on a group of GPUs, and across processes, and the copy of
 // a round's outputs to the host; ctmr_frontend_api.cu: the wire-format front end on one GPU and on a group).
 //
@@ -122,29 +123,55 @@ struct PemStage {
     std::vector<uint64_t> host_off;
 };
 
+// where the path writes the results of one slice or chunk of up to cap entries, and the events of its round of the key
+// exchange: one per host-pipeline stage and one for the front end
+struct PathOut {
+    uint64_t cap = 0;
+    DevBuf<uint8_t> status, sha, was_unknown, first;
+    DevBuf<int64_t> exp_hour;
+    DevBuf<uint32_t> serial_off, serial_len;
+    DevBuf<uint32_t> spans;       // [4][cap]: issuer name off/len, crldp off/len
+    DevBuf<uint8_t> first_meta;   // [2][cap]: first_issuer_dn, first_crldp
+    Event mapped;     // recorded after the round's K_map (its inserts have reached the owners' tables)
+    Event reduced;    // recorded after the round's owner passes (resolve + pairs of own entries and inbox records)
+    Event meta_done;  // recorded after the round's string-identity insert
+
+    int allocate(ctmr_ctx* c, uint64_t entries);  // every buffer and event (ctmr_api.cu)
+    // the buffers as the path's outputs: sha256 when the caller asked for it, the spans and first_* when the call computes
+    // string identities; keys are the caller's to set
+    ctmr_dev_out dev_out(bool sha256, bool meta) const {
+        ctmr_dev_out d{};
+        d.status = status;
+        d.sha256 = sha256 ? sha.get() : nullptr;
+        d.exp_hour = exp_hour;
+        d.serial_off = serial_off;
+        d.serial_len = serial_len;
+        d.was_unknown = was_unknown;
+        d.first_issuer_hour = first;
+        if (meta) {
+            d.issuer_name_off = spans;
+            d.issuer_name_len = spans + cap;
+            d.crldp_off = spans + 2 * cap;
+            d.crldp_len = spans + 3 * cap;
+            d.first_issuer_dn = first_meta;
+            d.first_crldp = first_meta + cap;
+        }
+        return d;
+    }
+};
+
 struct Stage {
     Stream stream;
-    Event mapped;     // recorded after this stage's K_map (its inserts have reached the owners' tables)
-    Event reduced;    // recorded after this stage's owner passes (resolve + pairs of own entries and inbox records)
-    Event meta_done;  // recorded after this stage's string-identity insert
+    PathOut out;
     DevBuf<uint8_t> blob;
     DevBuf<uint64_t> offsets;
     DevBuf<uint32_t> issuer_idx;
-    DevBuf<uint8_t> status;
-    DevBuf<uint8_t> sha;
-    DevBuf<int64_t> exp_hour;
-    DevBuf<uint32_t> serial_off;
-    DevBuf<uint32_t> serial_len;
-    DevBuf<uint8_t> was_unknown;
-    DevBuf<uint8_t> first;
     DevBuf<ctmr_key> keys;
     DevBuf<uint32_t> slot_of;
     DevBuf<uint32_t> pair_slot;
     DevBuf<uint32_t> order;
     DevBuf<unsigned int> len_hist;
-    DevBuf<uint32_t> spans;       // [4][E]: issuer name off/len, crldp off/len
     DevBuf<uint32_t> meta_slots;  // [2*E]
-    DevBuf<uint8_t> first_meta;   // [2][E]: first_issuer_dn, first_crldp
     PemStage pem;                 // allocated when a caller first asks for PEM output
 };
 
@@ -265,10 +292,7 @@ struct FrontEnd {
     DevBuf<uint8_t> entry_status, entry_type, leaf_src;
     DevBuf<uint64_t> timestamp, leaf_abs, chain_abs, tbs_abs;
     DevBuf<uint32_t> leaf_rel, leaf_len_out, chain_len, tbs_len, issuer_idx;
-    // outputs of the path for this chunk
-    DevBuf<uint8_t> status, sha, was_unknown, first, first_meta;
-    DevBuf<int64_t> exp_hour;
-    DevBuf<uint32_t> serial_off, serial_len, spans;
+    PathOut out;  // the path's outputs for this chunk; its events serve the rounds of a group or collective call (fe_member)
     // issuer certificates by bytes
     DevBuf<IssuerCertSlot> slots_dev;
     std::vector<IssuerCertSlot> slots_host;
@@ -281,7 +305,6 @@ struct FrontEnd {
     uint32_t unknown_cap = 0;
     DevBuf<unsigned int> unknown_count;
     Event ev0, ev1, ev2;
-    Event mapped, reduced, meta_done;  // round events of the group front end (fe_member)
     float fe_ms = 0.f, path_ms = 0.f;
     uint64_t launches = 0;
     PemStage pem;
@@ -464,15 +487,58 @@ struct RoundMember {
 // want_meta the string identities (insert, sync 3, read-back).  `parity` selects the exchange regions and
 // max_per_region bounds one member's slice.  On error *failed names the member that failed.
 int run_round(const RoundMember* m, uint32_t W, int parity, uint64_t max_per_region, bool want_meta, ctmr_ctx** failed);
+
+// the call computes string identities: the caller asked for one of them
+inline bool want_meta(const ctmr_out* o) { return o->first_issuer_dn || o->first_crldp || o->issuer_name_off || o->crldp_off; }
+inline int check_pem(ctmr_ctx* c, const ctmr_out* o) {
+    if ((o->pem != nullptr) != (o->pem_off != nullptr)) return fail(c, CTMR_E_INVALID, "pem and pem_off go together");
+    return CTMR_OK;
+}
+
+// The window rule of a group round: the round cuts ONE contiguous window of units from `pos` on, q units per member
+// (member r's slice is [pos + r q, pos + (r + 1) q), clipped to `total`), so that every unit keeps its global index.
+// q starts at q0 and is halved, rounded up, until fits(r, lo, hi, &ok) leaves ok set for every member's slice.  *q = 0:
+// not even one unit per member fits.  An error of fits ends the search and is returned.
+template <class Fits>
+int split_window(uint64_t total, uint64_t pos, uint32_t W, uint64_t q0, Fits fits, uint64_t* q) {
+    for (*q = q0;; *q = (*q + 1) / 2) {
+        bool ok = true;
+        for (uint32_t r = 0; r < W && ok; ++r) {
+            const int rc = fits(r, std::min(total, pos + r * *q), std::min(total, pos + (r + 1) * *q), &ok);
+            if (rc) return rc;
+        }
+        if (ok) return CTMR_OK;
+        if (*q == 1) {
+            *q = 0;
+            return CTMR_OK;
+        }
+    }
+}
+
+// D2H of rows [0, cnt) of the device's `src` to rows [lo, lo + cnt) of the caller's `dst`, `per` elements of dst's type
+// a row, on s; nothing when the caller did not ask for the array (dst null) or the device has none (src null)
+template <class T>
+cudaError_t d2h_rows(T* dst, const void* src, uint64_t lo, uint64_t cnt, cudaStream_t s, uint64_t per = 1) {
+    if (!dst || !src) return cudaSuccess;
+    return cudaMemcpyAsync(dst + lo * per, src, cnt * per * sizeof(T), cudaMemcpyDeviceToHost, s);
+}
 // D2H of entries [0, cnt) of device outputs to entries [lo, lo + cnt) of the caller's outputs: every per-entry array of
 // ctmr_out that both sides have, on stream s
 int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* out, uint64_t lo, cudaStream_t s);
+// No copy into or out of the caller's buffers may outlive a failed call: waits for streams s[0..n) of c.  c's last
+// error stays the failure's.
+inline void drain_streams(ctmr_ctx* c, const cudaStream_t* s, int n) {
+    const std::string keep = c->err;
+    cudaSetDevice(c->device);
+    for (int k = 0; k < n; ++k) cudaStreamSynchronize(s[k]);
+    c->err = keep;
+}
 int group_fail(ctmr_group* g, ctmr_ctx* c, int rc);   // c's error becomes g's last error (when both are given); returns rc
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise
-// one word from every rank through the mailbox, row[r] = rank r's (ctmr_frontend_api.cu); the caller then checks the
-// device for a barrier that timed out
+// one word from every rank through the mailbox, row[r] = rank r's; the caller then checks the device for a barrier that
+// timed out
 int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row);
 int refresh_digests(ctmr_ctx* c);                                   // host memo <- device registry
 int lookup_digest(ctmr_ctx* c, const uint8_t digest[32], bool insert, uint32_t* idx_out, bool* found);

@@ -53,36 +53,6 @@ struct Chunk {
     }
 };
 
-bool want_meta(const ctmr_out* o) { return o->first_issuer_dn || o->first_crldp || o->issuer_name_off || o->crldp_off; }
-
-int check_pem(ctmr_ctx* c, const ctmr_out* o) {
-    if ((o->pem != nullptr) != (o->pem_off != nullptr)) return fail(c, CTMR_E_INVALID, "pem and pem_off go together");
-    return CTMR_OK;
-}
-
-// where the path writes a chunk's results: the front end's per-chunk buffers (sha256 when asked for, string identities
-// when the call computes them)
-ctmr_dev_out chunk_path_out(FrontEnd* f, const ctmr_out* po, bool meta) {
-    const uint64_t E = f->cap_entries;
-    ctmr_dev_out dout{};
-    dout.status = f->status;
-    dout.sha256 = po->sha256 ? f->sha.get() : nullptr;
-    dout.exp_hour = f->exp_hour;
-    dout.serial_off = f->serial_off;
-    dout.serial_len = f->serial_len;
-    dout.was_unknown = f->was_unknown;
-    dout.first_issuer_hour = f->first;
-    if (meta) {
-        dout.issuer_name_off = f->spans;
-        dout.issuer_name_len = f->spans + E;
-        dout.crldp_off = f->spans + 2 * E;
-        dout.crldp_len = f->spans + 3 * E;
-        dout.first_issuer_dn = f->first_meta;
-        dout.first_crldp = f->first_meta + E;
-    }
-    return dout;
-}
-
 // the front end's buffers on a member, and its counters of this call
 int fe_prepare(ctmr_ctx* c) {
     CU(c, cudaSetDevice(c->device));
@@ -92,10 +62,6 @@ int fe_prepare(ctmr_ctx* c) {
     c->fe->launches = 0;
     return CTMR_OK;
 }
-
-// D2H of a chunk's device rows [0, cnt) of `per` bytes each to rows [lo, lo + cnt) of the caller's `dst`, if it asked for them
-#define CHUNK_D2H(dst, src, per) \
-    if (dst) CU(c, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + lo * (per), (src), cnt * (per), cudaMemcpyDeviceToHost, s))
 
 // ---- the logs' Merkle trees (ctmr_process_*_tree, ctmr_process_*_trees) ------------------------------------------------
 // The trees of a tree call: the one-tree forms pass one tree and no log (every entry is the tree's); the routed forms
@@ -528,7 +494,7 @@ int spans_front(ctmr_ctx* c, Chunk& ch, uint64_t text_bytes, uint64_t cnt, int64
     db.n = cnt;
     db.issuer_idx = f->issuer_idx;
     db.now_unix_ns = now_unix_ns;
-    ch.dout = chunk_path_out(f, po, meta);
+    ch.dout = f->out.dev_out(po->sha256 != nullptr, meta);
     return CTMR_OK;
 }
 
@@ -546,13 +512,13 @@ int raw_copy_back(ctmr_ctx* c, const Chunk& ch, const ctmr_raw_out* out) {
     cudaStream_t s = c->stream;
     const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0;
     if (cnt) {
-        CHUNK_D2H(out->entry_status, f->entry_status, 1);
-        CHUNK_D2H(out->entry_type, f->entry_type, 1);
-        CHUNK_D2H(out->timestamp_ms, f->timestamp, 8);
-        CHUNK_D2H(out->issuer, f->issuer_idx, 4);
-        CHUNK_D2H(out->leaf_src, f->leaf_src, 1);
-        CHUNK_D2H(out->leaf_off, f->leaf_rel, 4);
-        CHUNK_D2H(out->leaf_len, f->leaf_len_out, 4);
+        CU(c, d2h_rows(out->entry_status, f->entry_status, lo, cnt, s));
+        CU(c, d2h_rows(out->entry_type, f->entry_type, lo, cnt, s));
+        CU(c, d2h_rows(out->timestamp_ms, f->timestamp, lo, cnt, s));
+        CU(c, d2h_rows(out->issuer, f->issuer_idx, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_src, f->leaf_src, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_off, f->leaf_rel, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_len, f->leaf_len_out, lo, cnt, s));
     }
     return CTMR_OK;
 }
@@ -800,7 +766,7 @@ int Tiles::front(ctmr_ctx* c, Chunk& ch) const {
     db.n = p.n;
     db.issuer_idx = f->issuer_idx;
     db.now_unix_ns = b->now_unix_ns;
-    ch.dout = chunk_path_out(f, &out->path, meta);
+    ch.dout = f->out.dev_out(out->path.sha256 != nullptr, meta);
     return CTMR_OK;
 }
 
@@ -812,14 +778,14 @@ int Tiles::copy_back(ctmr_ctx* c, const Chunk& ch) const {
     const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0, nt = ch.hi - ch.lo;
     std::vector<uint8_t> bad(nt);
     if (cnt) {
-        CHUNK_D2H(out->entry_status, f->entry_status, 1);
-        CHUNK_D2H(out->entry_type, f->entry_type, 1);
-        CHUNK_D2H(out->timestamp_ms, f->timestamp, 8);
-        CHUNK_D2H(out->issuer, f->issuer_idx, 4);
-        CHUNK_D2H(out->leaf_index, tl->leaf_index, 8);
-        CHUNK_D2H(out->leaf_off, tl->leaf_data_off, 8);
-        CHUNK_D2H(out->leaf_len, f->leaf_len_out, 4);
-        CHUNK_D2H(out->leaf_hash, tl->leaf_hash, 32);
+        CU(c, d2h_rows(out->entry_status, f->entry_status, lo, cnt, s));
+        CU(c, d2h_rows(out->entry_type, f->entry_type, lo, cnt, s));
+        CU(c, d2h_rows(out->timestamp_ms, f->timestamp, lo, cnt, s));
+        CU(c, d2h_rows(out->issuer, f->issuer_idx, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_index, tl->leaf_index, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_off, tl->leaf_data_off, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_len, f->leaf_len_out, lo, cnt, s));
+        CU(c, d2h_rows(out->leaf_hash, tl->leaf_hash, lo, cnt, s, 32));
         if (out->tile_status) CU(c, cudaMemcpyAsync(bad.data(), tl->tile_bad, nt, cudaMemcpyDeviceToHost, s));
     }
     CU(c, cudaStreamSynchronize(s));
@@ -1144,11 +1110,11 @@ int Bodies::copy_back(ctmr_ctx* c, const Chunk& ch) const {
     if (rc) return rc;
     const uint64_t lo = ch.e0, cnt = ch.e1 - ch.e0, nb = ch.hi - ch.lo;
     if (cnt) {
-        CHUNK_D2H(bo->leaf_input_off, bd->abs_off[0], 8);
-        CHUNK_D2H(bo->leaf_input_len, bd->raw_len[0], 4);
-        CHUNK_D2H(bo->extra_data_off, bd->abs_off[1], 8);
-        CHUNK_D2H(bo->extra_data_len, bd->raw_len[1], 4);
-        CHUNK_D2H(bo->escaped, bd->esc, 1);
+        CU(c, d2h_rows(bo->leaf_input_off, bd->abs_off[0], lo, cnt, s));
+        CU(c, d2h_rows(bo->leaf_input_len, bd->raw_len[0], lo, cnt, s));
+        CU(c, d2h_rows(bo->extra_data_off, bd->abs_off[1], lo, cnt, s));
+        CU(c, d2h_rows(bo->extra_data_len, bd->raw_len[1], lo, cnt, s));
+        CU(c, d2h_rows(bo->escaped, bd->esc, lo, cnt, s));
     }
     std::vector<uint8_t> status(nb);
     std::vector<uint32_t> count(nb), base(nb);
@@ -1165,8 +1131,6 @@ int Bodies::copy_back(ctmr_ctx* c, const Chunk& ch) const {
     }
     return CTMR_OK;
 }
-
-#undef CHUNK_D2H
 
 // ================================================================================================================
 // the driver
@@ -1199,7 +1163,7 @@ int for_each_member(ctmr_ctx** m, uint32_t W, bool threads, ctmr_ctx** failed, F
 
 // Cuts the round that starts at unit `pos` and issues its uploads into stage `stage`.  One member takes the greedy chunk
 // fit returns (an empty chunk at the end of the batch: a rank of a collective call runs its last rounds empty).  A group
-// takes one chunk per member from ONE contiguous window, q units each, q halved until every member's chunk fits.
+// takes one chunk per member from ONE contiguous window (split_window), a chunk fitting when fit keeps all of it.
 template <class Format>
 int plan_round(ctmr_ctx** m, uint32_t W, const Format& fm, uint64_t pos, int stage, std::vector<Chunk>& ch, ctmr_ctx** failed) {
     const uint64_t total = fm.units();
@@ -1214,23 +1178,17 @@ int plan_round(ctmr_ctx** m, uint32_t W, const Format& fm, uint64_t pos, int sta
         }
         q = hi - pos;
     } else {
-        q = std::max<uint64_t>(1, std::min<uint64_t>(fm.q_max(m[0]), (total - pos + W - 1) / W));
-        for (;;) {
-            bool fits = true;
-            for (uint32_t r = 0; r < W && fits; ++r) {
-                const uint64_t lo = std::min(total, pos + r * q), want = std::min(total, pos + (r + 1) * q);
-                uint64_t hi = 0;
-                const int rc = fm.fit(m[r], lo, want - lo, &hi);
-                if (rc) {
-                    *failed = m[r];
-                    return rc;
-                }
-                fits = hi == want;
-            }
-            if (fits) break;
-            if (q == 1) return fail(m[0], CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
-            q = (q + 1) / 2;
-        }
+        const auto fits = [&](uint32_t r, uint64_t lo, uint64_t want, bool* ok) {
+            uint64_t hi = 0;
+            const int rc = fm.fit(m[r], lo, want - lo, &hi);
+            if (rc) *failed = m[r];
+            *ok = hi == want;
+            return rc;
+        };
+        const uint64_t q0 = std::max<uint64_t>(1, std::min<uint64_t>(fm.q_max(m[0]), (total - pos + W - 1) / W));
+        const int rc = split_window(total, pos, W, q0, fits, &q);
+        if (rc) return rc;
+        if (q == 0) return fail(m[0], CTMR_E_BATCH_TOO_LARGE, Format::kTooLarge);
     }
     ch.assign(W, Chunk{});
     for (uint32_t r = 0; r < W; ++r) {
@@ -1259,7 +1217,7 @@ int fe_member(ctmr_ctx* c, const ctmr_dev_batch& db, const ctmr_dev_out& dout, i
     x.slot_of = c->slot_scratch; x.pair_slot = c->pair_scratch; x.order = c->order_scratch; x.len_hist = c->len_hist;
     x.meta_slots = c->meta_scratch;
     x.map_stream = x.reduce_stream = c->stream;
-    x.mapped = c->fe->mapped; x.reduced = c->fe->reduced; x.meta_done = c->fe->meta_done;
+    x.mapped = c->fe->out.mapped; x.reduced = c->fe->out.reduced; x.meta_done = c->fe->out.meta_done;
     // The members of an in-process group meet through their events; peer_barrier does nothing for them.  The ranks of a
     // collective call (one process per GPU) meet at these barriers, which the host pipeline's rounds use too: both
     // calls are synchronous, so while a front-end call runs no stage stream of any rank has a barrier queued, and
@@ -1290,27 +1248,13 @@ constexpr uint64_t kAgreeFailed = 1ull << 63, kAgreeMeta = 1ull << 62;
 constexpr int kAgreeEShift = 40;  // E <= kStageEntries < 2^22 in bits 40..61, the chunk count below 2^40
 static_assert(kStageEntries < (1ull << 22), "agreement word layout");
 
-// One word from every rank through the mailbox.  The second barrier keeps every rank from posting the next word
-// before each rank has read this one.  The row is valid only if no barrier timed out: the caller checks the device.
-int peer_exchange(ctmr_ctx* c, uint64_t mine, uint64_t* row) {
-    CU(c, launch_peer_post(c->pf, mine, c->stream));
-    int rc = peer_barrier(c, CH_MAILBOX, c->stream);
-    if (rc) return rc;
-    CU(c, cudaMemcpyAsync(row, c->pf.flags[c->pf.rank] + (size_t)kPeerChannels * kMaxWorld, kMaxWorld * sizeof(uint64_t),
-                          cudaMemcpyDeviceToHost, c->stream));
-    rc = peer_barrier(c, CH_MAILBOX, c->stream);
-    if (rc) return rc;
-    CU(c, cudaStreamSynchronize(c->stream));
-    return CTMR_OK;
-}
-
 // Posts this rank's part (`mine_rc`: the result of its checks) and reads every rank's.  Returns the rank's own error,
 // CTMR_E_PEER_FAILED when only another rank failed, or CTMR_OK with *pc filled in.
 int peer_agree(ctmr_ctx* c, int mine_rc, uint64_t chunks, uint64_t E, bool meta, PeerCall* pc, bool* meta_out) {
     const std::string err = c->err;
     uint64_t row[kMaxWorld] = {};
     const uint64_t mine = mine_rc ? kAgreeFailed : chunks | E << kAgreeEShift | (meta ? kAgreeMeta : 0);
-    int rc = peer_exchange(c, mine, row);
+    int rc = peer_mailbox(c, mine, row);
     if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
     if (rc) return rc;
     if (mine_rc) {
@@ -1368,12 +1312,12 @@ int back(ctmr_ctx* c, const Format& fm, const Chunk& ch, uint64_t* pem_base) {
     const uint64_t cnt = ch.e1 - ch.e0;
     const ctmr_out* po = &fm.out->path;
     if (cnt) {
-        CU(c, launch_fe_finish(ch.p.fe, f->status, s));
+        CU(c, launch_fe_finish(ch.p.fe, f->out.status, s));
         ++f->launches;
     }
     CU(c, cudaEventRecord(f->ev2, s));
     if (cnt && po->pem) {  // the new certificates' PEM, encoded from the DER in HBM
-        const int rc = pem_chunk(c, f->pem, ch.p.fe.decoded, f->leaf_abs, f->leaf_len_out, f->was_unknown, cnt, po, ch.e0, pem_base, s);
+        const int rc = pem_chunk(c, f->pem, ch.p.fe.decoded, f->leaf_abs, f->leaf_len_out, f->out.was_unknown, cnt, po, ch.e0, pem_base, s);
         if (rc) return rc;
     }
     if (Format::kStageHoldsLeaves) CU(c, cudaEventRecord(f->stage[ch.stage].consumed, s));  // the leaves' last read is done
@@ -1481,7 +1425,7 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
             fail_locally(rc);
             cur[0].cut(0, 0);
             cur[0].stopped = false;
-            cur[0].dout = chunk_path_out(m[0]->fe.get(), po, fm.meta);
+            cur[0].dout = m[0]->fe->out.dev_out(po->sha256 != nullptr, fm.meta);
         }
         fm.place(m, cur, W);
         if (tree) {  // bodies: the round's leaves into the trees, now that place has given out their log positions
@@ -1530,7 +1474,7 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
     }
     if (pc.on) {  // every rank learns how many ranks stopped: a resume loop calls again while any did
         uint64_t row[kMaxWorld] = {};
-        rc = peer_exchange(m[0], stop < W ? 1 : 0, row);
+        rc = peer_mailbox(m[0], stop < W ? 1 : 0, row);
         if (rc) return rc;
         for (uint32_t r = 0; r < world; ++r) m[0]->fe_peer_stopped += row[r] != 0;
         rc = ctmr_check_device(m[0], nullptr);  // a barrier that timed out; the count above is then unreliable
@@ -1549,11 +1493,8 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
 // arrays: neither may outlive a failed call
 void drain_frontend(ctmr_ctx* c) {
     if (!c || !c->fe) return;
-    const std::string keep = c->err;
-    cudaSetDevice(c->device);
-    cudaStreamSynchronize(c->fe->copy_stream);
-    cudaStreamSynchronize(c->stream);
-    c->err = keep;
+    const cudaStream_t s[] = {c->fe->copy_stream, c->stream};
+    drain_streams(c, s, 2);
 }
 
 // Every front-end entry point: the call on members m[0..W), then, also after a failure, the entries that took their
@@ -1808,8 +1749,6 @@ int ctmr_group_register_chain_certs(ctmr_group* g, const uint8_t* blob, const ui
 }  // extern "C"
 
 namespace ctmr_host {
-
-int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row) { return peer_exchange(c, mine, row); }
 
 int tiles_ensure(ctmr_ctx* c) {
     FrontEnd* f = c->fe.get();

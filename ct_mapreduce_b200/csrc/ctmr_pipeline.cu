@@ -28,30 +28,20 @@ int ensure_stages(ctmr_ctx* c) {
     for (int k = 0; k < kStages; ++k) {
         Stage& s = stages[k];
         CU(c, create(s.stream));
-        CU(c, create(s.mapped));
-        CU(c, create(s.reduced));
-        CU(c, create(s.meta_done));
+        const int rc = s.out.allocate(c, E);
+        if (rc) return rc;
         CU(c, alloc(s.blob, c->stage_bytes + 64));
         // K_map stages records in 16-byte pieces, so its last copy may read up to 15 bytes past the slice's data (inside
         // this allocation, never consumed): written once here so that those bytes are defined (compute-sanitizer initcheck)
         CU(c, cudaMemsetAsync(s.blob, 0, c->stage_bytes + 64, s.stream));
         CU(c, alloc(s.offsets, E + 1));
         CU(c, alloc(s.issuer_idx, E));
-        CU(c, alloc(s.status, E));
-        CU(c, alloc(s.sha, E * 32));
-        CU(c, alloc(s.exp_hour, E));
-        CU(c, alloc(s.serial_off, E));
-        CU(c, alloc(s.serial_len, E));
-        CU(c, alloc(s.was_unknown, E));
-        CU(c, alloc(s.first, E));
         CU(c, alloc(s.keys, E));
         CU(c, alloc(s.slot_of, E));
         CU(c, alloc(s.pair_slot, E));
         CU(c, alloc(s.order, E));
         CU(c, alloc(s.len_hist, 256));
-        CU(c, alloc(s.spans, 4 * E));
         CU(c, alloc(s.meta_slots, 2 * E));
-        CU(c, alloc(s.first_meta, 2 * E));
     }
     c->stages = std::move(stages);
     return CTMR_OK;
@@ -94,22 +84,19 @@ int pem_chunk(ctmr_ctx* c, PemStage& ps, const uint8_t* blob, const uint64_t* of
 }
 
 int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* out, uint64_t lo, cudaStream_t s) {
-#define D2H(field, per) \
-    if (out->field && d.field) CU(c, cudaMemcpyAsync(out->field + lo * (per), d.field, cnt * (per) * sizeof *d.field, cudaMemcpyDeviceToHost, s))
-    D2H(status, 1);
-    D2H(sha256, 32);
-    D2H(exp_hour, 1);
-    D2H(serial_off, 1);
-    D2H(serial_len, 1);
-    D2H(was_unknown, 1);
-    D2H(first_issuer_hour, 1);
-    D2H(issuer_name_off, 1);
-    D2H(issuer_name_len, 1);
-    D2H(crldp_off, 1);
-    D2H(crldp_len, 1);
-    D2H(first_issuer_dn, 1);
-    D2H(first_crldp, 1);
-#undef D2H
+    CU(c, d2h_rows(out->status, d.status, lo, cnt, s));
+    CU(c, d2h_rows(out->sha256, d.sha256, lo, cnt, s, 32));
+    CU(c, d2h_rows(out->exp_hour, d.exp_hour, lo, cnt, s));
+    CU(c, d2h_rows(out->serial_off, d.serial_off, lo, cnt, s));
+    CU(c, d2h_rows(out->serial_len, d.serial_len, lo, cnt, s));
+    CU(c, d2h_rows(out->was_unknown, d.was_unknown, lo, cnt, s));
+    CU(c, d2h_rows(out->first_issuer_hour, d.first_issuer_hour, lo, cnt, s));
+    CU(c, d2h_rows(out->issuer_name_off, d.issuer_name_off, lo, cnt, s));
+    CU(c, d2h_rows(out->issuer_name_len, d.issuer_name_len, lo, cnt, s));
+    CU(c, d2h_rows(out->crldp_off, d.crldp_off, lo, cnt, s));
+    CU(c, d2h_rows(out->crldp_len, d.crldp_len, lo, cnt, s));
+    CU(c, d2h_rows(out->first_issuer_dn, d.first_issuer_dn, lo, cnt, s));
+    CU(c, d2h_rows(out->first_crldp, d.first_crldp, lo, cnt, s));
     return CTMR_OK;
 }
 
@@ -137,42 +124,31 @@ struct Slice {
     uint64_t first_index = 0;     // global index of entry lo
 };
 
-// rounds x members.  Every slice respects the entry budget and the byte budget of a stage.
+// rounds x members.  Every slice respects the entry budget and the byte budget of a stage; W == 1 halves as well.
 int plan_rounds(ctmr_ctx* c0, uint32_t W, const BatchArgs& a, std::vector<std::vector<Slice>>& plan) {
     const uint64_t E = c0->stage_entries, B = c0->stage_bytes;
-    uint64_t pos = 0;
-    while (pos < a.n) {
-        uint64_t q = std::min<uint64_t>(E, (a.n - pos + W - 1) / W);
-        for (;;) {  // shrink until every member's slice fits the byte budget
-            bool fits = true;
-            for (uint32_t r = 0; r < W && fits; ++r) {
-                const uint64_t lo = std::min(a.n, pos + r * q), hi = std::min(a.n, pos + (r + 1) * q);
-                fits = a.offsets[hi] - a.offsets[lo] <= B;
-            }
-            if (fits) break;
-            if (q == 1) return fail(c0, CTMR_E_BATCH_TOO_LARGE, "a single entry exceeds the staging budget (config.max_batch_bytes)");
-            q = (q + 1) / 2;
-        }
+    const auto fits = [&](uint32_t, uint64_t lo, uint64_t hi, bool* ok) {
+        *ok = a.offsets[hi] - a.offsets[lo] <= B;
+        return CTMR_OK;
+    };
+    for (uint64_t pos = 0, q = 0; pos < a.n; pos = std::min(a.n, pos + W * q)) {
+        split_window(a.n, pos, W, std::min<uint64_t>(E, (a.n - pos + W - 1) / W), fits, &q);
+        if (q == 0) return fail(c0, CTMR_E_BATCH_TOO_LARGE, "a single entry exceeds the staging budget (config.max_batch_bytes)");
         std::vector<Slice> round(W);
         for (uint32_t r = 0; r < W; ++r) {
             round[r].lo = std::min(a.n, pos + r * q);
             round[r].hi = std::min(a.n, pos + (r + 1) * q);
         }
         plan.push_back(std::move(round));
-        pos = std::min(a.n, pos + W * q);
     }
     return CTMR_OK;
 }
 
 // multi-process group: the ranks agree on the number of rounds of this collective call (the largest any rank needs)
 int agree_rounds(ctmr_ctx* c, uint64_t mine, uint64_t* agreed) {
-    CU(c, launch_peer_post(c->pf, mine, c->stream));
-    int rc = peer_barrier(c, CH_MAILBOX, c->stream);
-    if (rc) return rc;
-    unsigned long long row[kMaxWorld] = {};
-    CU(c, cudaMemcpyAsync(row, c->pf.flags[c->pf.rank] + (size_t)kPeerChannels * kMaxWorld, sizeof row, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    rc = ctmr_check_device(c, nullptr);
+    uint64_t row[kMaxWorld] = {};
+    int rc = peer_mailbox(c, mine, row);
+    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
     if (rc) return rc;
     uint64_t mx = mine;
     for (uint32_t r = 0; r < c->pf.world; ++r) mx = std::max<uint64_t>(mx, row[r]);
@@ -182,10 +158,10 @@ int agree_rounds(ctmr_ctx* c, uint64_t mine, uint64_t* agreed) {
 
 // Upload of one member's slice to stage `sidx`, and the slice's description for run_round.  chain: the round follows
 // another, whose owner passes (and string identities) this round's must follow.
-int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Slice& sl, const uint32_t* map_dev, bool want_meta,
+int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Slice& sl, const uint32_t* map_dev, bool meta,
                 RoundMember& x) {
     Stage& s = c->stages[sidx];
-    const uint64_t cnt = sl.hi - sl.lo, E = c->stage_entries;
+    const uint64_t cnt = sl.hi - sl.lo;
     CU(c, cudaSetDevice(c->device));
     x = RoundMember{};
     x.c = c;
@@ -205,30 +181,15 @@ int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Sli
         db.first_index = sl.first_index;
         db.now_unix_ns = a.now_unix_ns;
     }
-    ctmr_dev_out& dout = x.dout;
-    dout.status = s.status;
-    dout.sha256 = a.out->sha256 ? s.sha.get() : nullptr;
-    dout.exp_hour = s.exp_hour;
-    dout.serial_off = s.serial_off;
-    dout.serial_len = s.serial_len;
-    dout.was_unknown = s.was_unknown;
-    dout.first_issuer_hour = s.first;
-    dout.keys = s.keys;
-    if (want_meta) {
-        dout.issuer_name_off = s.spans;
-        dout.issuer_name_len = s.spans + E;
-        dout.crldp_off = s.spans + 2 * E;
-        dout.crldp_len = s.spans + 3 * E;
-        dout.first_issuer_dn = s.first_meta;
-        dout.first_crldp = s.first_meta + E;
-    }
+    x.dout = s.out.dev_out(a.out->sha256 != nullptr, meta);
+    x.dout.keys = s.keys;
     x.slot_of = s.slot_of; x.pair_slot = s.pair_slot; x.order = s.order; x.len_hist = s.len_hist; x.meta_slots = s.meta_slots;
     x.map_stream = x.reduce_stream = s.stream;
-    x.mapped = s.mapped; x.reduced = s.reduced; x.meta_done = s.meta_done;
+    x.mapped = s.out.mapped; x.reduced = s.out.reduced; x.meta_done = s.out.meta_done;
     if (chain) {
         const Stage& prev = c->stages[(sidx + kStages - 1) % kStages];
-        x.prev_reduced = prev.reduced;
-        x.prev_meta_done = prev.meta_done;
+        x.prev_reduced = prev.out.reduced;
+        x.prev_meta_done = prev.out.meta_done;
     }
     x.ch_map = CH_STAGE_MAP + sidx;
     x.ch_resolve = CH_STAGE_RESOLVE + sidx;
@@ -256,7 +217,7 @@ int stage_out(const RoundMember& x, int sidx, const BatchArgs& a, const Slice& s
 int run_rounds(ctmr_ctx** m, uint32_t W, const BatchArgs& a, const std::vector<std::vector<Slice>>& plan,
                const std::vector<const uint32_t*>& map_dev, ctmr_ctx** failed) {
     const ctmr_out* out = a.out;
-    const bool want_meta = out->first_issuer_dn || out->first_crldp || out->issuer_name_off || out->crldp_off;
+    const bool meta = want_meta(out);
     const bool want_pem = out->pem != nullptr || out->pem_off != nullptr;
     uint64_t pem_base = 0;
     int rc = CTMR_OK;
@@ -271,8 +232,8 @@ int run_rounds(ctmr_ctx** m, uint32_t W, const BatchArgs& a, const std::vector<s
     RoundMember rm[kMaxWorld];
     for (size_t k = 0; k < plan.size(); ++k) {
         const int sidx = (int)(k % kStages);
-        for (uint32_t r = 0; r < W; ++r) RR(r, stage_slice(m[r], sidx, k > 0, a, plan[k][r], map_dev[r], want_meta, rm[r]));
-        rc = run_round(rm, W, sidx, m[0]->stage_entries, want_meta, failed);
+        for (uint32_t r = 0; r < W; ++r) RR(r, stage_slice(m[r], sidx, k > 0, a, plan[k][r], map_dev[r], meta, rm[r]));
+        rc = run_round(rm, W, sidx, m[0]->stage_entries, meta, failed);
         if (rc) return rc;
         for (uint32_t r = 0; r < W; ++r) RR(r, stage_out(rm[r], sidx, a, plan[k][r], want_pem, &pem_base));
     }
@@ -292,15 +253,13 @@ int run_rounds(ctmr_ctx** m, uint32_t W, const BatchArgs& a, const std::vector<s
     return CTMR_OK;
 }
 
-// no copy from / into the caller's buffers may outlive a failed call
+// drain_streams over every member's stage streams
 void drain(ctmr_ctx** m, uint32_t W) {
     for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = m[r];
-        if (!c->stages) continue;
-        const std::string keep = c->err;
-        cudaSetDevice(c->device);
-        for (int k = 0; k < kStages; ++k) cudaStreamSynchronize(c->stages[k].stream);
-        c->err = keep;
+        if (!m[r]->stages) continue;
+        cudaStream_t s[kStages];
+        for (int k = 0; k < kStages; ++k) s[k] = m[r]->stages[k].stream;
+        drain_streams(m[r], s, kStages);
     }
 }
 
@@ -315,8 +274,8 @@ int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, const 
         *failed = nullptr;
         return CTMR_OK;
     }
-    if ((out->pem != nullptr) != (out->pem_off != nullptr)) return fail(c0, CTMR_E_INVALID, "pem and pem_off go together");
-    int rc;
+    int rc = check_pem(c0, out);
+    if (rc) return rc;
     for (uint32_t r = 0; r < W; ++r) {
         *failed = m[r];
         CU(m[r], cudaSetDevice(m[r]->device));

@@ -335,23 +335,11 @@ __device__ __forceinline__ uint32_t pair_hash(const uint32_t (&w)[11]) {
     return (uint32_t)(h >> 32);
 }
 
-__global__ void __launch_bounds__(256) crl_set_insert_kernel(const uint8_t* __restrict__ stage, const CrlDesc* __restrict__ desc,
-                                                             const CrlRes* __restrict__ res, const uint32_t* __restrict__ ecrl,
-                                                             const uint64_t* __restrict__ serial_off, const uint8_t* __restrict__ serial_len,
-                                                             const uint8_t* __restrict__ status, uint32_t ne, CrlSetSlot* set, uint64_t mask,
-                                                             uint32_t* __restrict__ slot) {
-    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= ne) return;
-    const uint32_t k = ecrl[e];
-    const CrlDesc cd = desc[k];
-    if (status[e] != CTMR_RV_OK || res[k].status != CTMR_CRL_OK) {
-        slot[e] = kNone;
-        return;
-    }
-    uint32_t w[11];
+// an entry's pair as the words w: issuer, then {serial_len, serial[39]} read from the staged CRL (len <= 255: at most 39
+// serial bytes are read, all inside the serial)
+__device__ __forceinline__ void pair_words(const uint8_t* stage, const CrlDesc& cd, uint64_t serial_off, uint32_t len, uint32_t (&w)[11]) {
     w[0] = cd.issuer;
-    const uint32_t len = serial_len[e];
-    const uint8_t* s = stage + cd.staged + (uint32_t)(serial_off[e] - cd.data_off) - 1;  // s[at]: serial byte at - 1
+    const uint8_t* s = stage + cd.staged + (uint32_t)(serial_off - cd.data_off) - 1;  // s[at]: serial byte at - 1
 #pragma unroll
     for (uint32_t q = 0; q < 10u; ++q) {  // static register indices
         uint32_t v = q == 0u ? len : 0u;
@@ -362,6 +350,10 @@ __global__ void __launch_bounds__(256) crl_set_insert_kernel(const uint8_t* __re
         }
         w[1 + q] = v;
     }
+}
+
+// find-or-insert of the pair w: its slot; equal pairs share one
+__device__ __forceinline__ uint32_t set_insert(CrlSetSlot* set, uint64_t mask, const uint32_t (&w)[11]) {
     const uint32_t h = pair_hash(w);
     const uint32_t ready = (h & ~3u) | 2u, pending = (h & ~3u) | 1u;
     uint64_t pos = h & mask;
@@ -383,9 +375,27 @@ __global__ void __launch_bounds__(256) crl_set_insert_kernel(const uint8_t* __re
             for (int i = 0; i < 11; ++i) same &= *reinterpret_cast<volatile uint32_t*>(&sl->key[i]) == w[i];
             if (same) break;
         }
-        pos = (pos + 1) & mask;  // the set has twice the entries' slots: a free one always exists
+        pos = (pos + 1) & mask;  // the set has twice the pairs' slots: a free one always exists
     }
-    slot[e] = (uint32_t)pos;
+    return (uint32_t)pos;
+}
+
+__global__ void __launch_bounds__(256) crl_set_insert_kernel(const uint8_t* __restrict__ stage, const CrlDesc* __restrict__ desc,
+                                                             const CrlRes* __restrict__ res, const uint32_t* __restrict__ ecrl,
+                                                             const uint64_t* __restrict__ serial_off, const uint8_t* __restrict__ serial_len,
+                                                             const uint8_t* __restrict__ status, uint32_t ne, CrlSetSlot* set, uint64_t mask,
+                                                             uint32_t* __restrict__ slot) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= ne) return;
+    const uint32_t k = ecrl[e];
+    const CrlDesc cd = desc[k];
+    if (status[e] != CTMR_RV_OK || res[k].status != CTMR_CRL_OK) {
+        slot[e] = kNone;
+        return;
+    }
+    uint32_t w[11];
+    pair_words(stage, cd, serial_off[e], serial_len[e], w);
+    slot[e] = set_insert(set, mask, w);
 }
 
 // one pass over the table: every ready key probes the set with its (issuer, serial); a hit records the key's hour
@@ -438,6 +448,114 @@ __global__ void __launch_bounds__(256) crl_finish_kernel(const uint32_t* __restr
     o.sets[e] = n;
 }
 
+// ---- one process per GPU: every rank's entries against every rank's shard, through the exchange area's inbox regions.
+// Region of source s on owner o: px.inbox[o] + s X (parity 0), its record count px.counts[o][s].
+
+// What every rank agreed a source sends in this round (the mailbox row).  The owner never reads more records of a source
+// than this, whatever the source's published count says: a source that missed its send (a failure, or a barrier that timed
+// out) leaves an earlier round's count behind, and the union set is sized for the agreed total only.
+struct CrlRoundCounts {
+    unsigned long long n[kMaxWorld];
+};
+
+__device__ __forceinline__ uint64_t crl_received(const PeerExchange& px, const CrlRoundCounts& agreed, uint32_t src) {
+    unsigned long long a = 0;
+#pragma unroll
+    for (uint32_t r = 0; r < kMaxWorld; ++r)  // static indices: the counts stay in parameter space, no local copy
+        if (r == src) a = agreed.n[r];
+    return min(min((unsigned long long)px.X, ld_volatile_u64(px.counts[px.rank] + src)), a);
+}
+
+// thread per entry lo + t of the chunk, t < n: its 64-byte record (ctmr_key layout) into rec[t]: index = the entry's
+// position in the chunk, issuer, {serial_len, serial}, valid = 1 only for a CTMR_RV_OK entry of a CTMR_CRL_OK CRL; exp_hour
+// and pad carry the answer later
+__global__ void __launch_bounds__(256) crl_peer_records_kernel(const uint8_t* __restrict__ stage, const CrlDesc* __restrict__ desc,
+                                                               const CrlRes* __restrict__ res, const uint32_t* __restrict__ ecrl,
+                                                               const uint64_t* __restrict__ serial_off, const uint8_t* __restrict__ serial_len,
+                                                               const uint8_t* __restrict__ status, uint32_t lo, uint32_t n,
+                                                               ctmr_key* __restrict__ rec) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const uint32_t e = lo + t;
+    const uint32_t k = ecrl[e];
+    const CrlDesc cd = desc[k];
+    uint32_t w[11];
+    pair_words(stage, cd, serial_off[e], serial_len[e], w);
+    const uint32_t valid = status[e] == CTMR_RV_OK && res[k].status == CTMR_CRL_OK ? 1u : 0u;
+    uint4* dst = reinterpret_cast<uint4*>(rec + t);
+    dst[0] = make_uint4(e, 0u, 0u, w[0]);
+    dst[1] = make_uint4(w[1], w[2], w[3], w[4]);
+    dst[2] = make_uint4(w[5], w[6], w[7], w[8]);
+    dst[3] = make_uint4(w[9], w[10], valid, 0u);
+}
+
+// Source side, grid (records x 4 / 256, world): records [0, n) into this source's region on every rank, its own among
+// them, four lanes per record so that a warp writes 512 contiguous bytes of posted stores; then the count.
+__global__ void __launch_bounds__(256) crl_peer_send_kernel(PeerExchange px, const ctmr_key* __restrict__ rec, uint64_t n) {
+    const uint32_t owner = blockIdx.y;
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < 4u * n) {
+        const uint4 v = reinterpret_cast<const uint4*>(rec)[t];
+        reinterpret_cast<uint4*>(px.inbox[owner] + (uint64_t)px.rank * px.X)[t] = v;
+    }
+    if (t == 0) px.counts[owner][px.rank] = n;  // the barrier after this kernel publishes both
+}
+
+// Owner side, grid (the most records of a source / 256, world): every valid record received into the union set; equal
+// keys of several sources share a slot.  in_slot[s X + j] = the record's slot, NONE for an invalid one.  The set has at
+// least twice the agreed total's slots, so a free one always exists.
+__global__ void __launch_bounds__(256) crl_union_insert_kernel(PeerExchange px, CrlRoundCounts agreed, CrlSetSlot* set, uint64_t mask,
+                                                               uint32_t* __restrict__ in_slot) {
+    const uint32_t src = blockIdx.y;
+    const uint64_t m = crl_received(px, agreed, src);
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const uint4* r = reinterpret_cast<const uint4*>(px.inbox[px.rank] + (uint64_t)src * px.X + j);
+    const uint4 q0 = __ldcg(r), q1 = __ldcg(r + 1), q2 = __ldcg(r + 2), q3 = __ldcg(r + 3);
+    if (q3.z != 1u) {
+        in_slot[(uint64_t)src * px.X + j] = kNone;
+        return;
+    }
+    const uint32_t w[11] = {q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y};
+    in_slot[(uint64_t)src * px.X + j] = set_insert(set, mask, w);
+}
+
+// Owner side, after the scan of its shard: each received record's answer in place, exp_hour = the lowest hour of this
+// shard's sets that hold it and pad = how many (0: none, or an invalid record)
+__global__ void __launch_bounds__(256) crl_peer_answer_kernel(PeerExchange px, CrlRoundCounts agreed, const uint32_t* __restrict__ in_slot,
+                                                              const int32_t* __restrict__ hour, const uint32_t* __restrict__ count) {
+    const uint32_t src = blockIdx.y;
+    const uint64_t m = crl_received(px, agreed, src);
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    const uint32_t s = in_slot[(uint64_t)src * px.X + j];
+    const uint32_t n = s < kNone ? count[s] : 0u;
+    ctmr_key* r = px.inbox[px.rank] + (uint64_t)src * px.X + j;
+    r->exp_hour = n ? hour[s] : 0;
+    r->pad = n;
+}
+
+// Source side, thread per record of the round: the answers of all owners for records [0, n) of this source, read from its
+// region on each owner; entry lo + i gets the lowest hour where an owner counted sets, and the sum of the counts
+__global__ void __launch_bounds__(256) crl_peer_pull_kernel(PeerExchange px, uint64_t n, uint64_t lo, uint8_t* __restrict__ known,
+                                                            int64_t* __restrict__ hour, uint32_t* __restrict__ sets) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    int32_t h = INT32_MAX;
+    uint32_t total = 0;
+    for (uint32_t o = 0; o < px.world; ++o) {
+        const ctmr_key* r = px.inbox[o] + (uint64_t)px.rank * px.X + i;
+        const uint32_t c = __ldcv(&r->pad);
+        if (c) {
+            h = min(h, __ldcv(&r->exp_hour));
+            total += c;
+        }
+    }
+    known[lo + i] = total ? 1 : 0;
+    hour[lo + i] = total ? (int64_t)h : 0;
+    sets[lo + i] = total;
+}
+
 inline unsigned grid(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
 }  // namespace
@@ -448,13 +566,16 @@ namespace {
 constexpr uint64_t kCrlBudgetMax = 256ull << 20;  // staged CRL bytes per chunk
 constexpr uint64_t kCrlsPerChunk = 1ull << 16;
 
+// staged CRL bytes per chunk
+uint64_t crl_budget(const ctmr_ctx* c) { return ((c->stage_bytes < kCrlBudgetMax ? c->stage_bytes : kCrlBudgetMax) + 15) / 16 * 16; }
+
 // The split's buffers on first use, for chunks of the ctx's budget: built into a local, moved in only when every
 // allocation succeeded.
 int crl_ensure(ctmr_ctx* c) {
     if (c->crl && c->crl->budget) return CTMR_OK;
     std::unique_ptr<CrlState> s(new (std::nothrow) CrlState());
     if (!s) return fail(c, CTMR_E_NOMEM, "host allocation failed");
-    const uint64_t B = ((c->stage_bytes < kCrlBudgetMax ? c->stage_bytes : kCrlBudgetMax) + 15) / 16 * 16;
+    const uint64_t B = crl_budget(c);
     s->budget = B;
     s->cap_crls = kCrlsPerChunk;
     // Candidates of any input: map a candidate p to p + 2 when its length is short (that byte is 02, no candidate) and to
@@ -531,6 +652,28 @@ int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
     return CTMR_OK;
 }
 
+// A rank attached to peers, after crl_ensure: the records of one round (X) and the union set of a round (2 world X
+// slots, so that a free slot always exists), all or nothing
+int crl_peer_ensure(ctmr_ctx* c) {
+    CrlState* s = c->crl.get();
+    if (s->records) return CTMR_OK;
+    const uint64_t cap = pow2_at_least(2ull * c->px.world * c->px.X);
+    DevBuf<ctmr_key> records;
+    DevBuf<CrlSetSlot> set;
+    DevBuf<int32_t> hour;
+    DevBuf<uint32_t> count;
+    CU(c, alloc(records, c->px.X));
+    CU(c, alloc(set, cap));
+    CU(c, alloc(hour, cap));
+    CU(c, alloc(count, cap));
+    s->union_set = std::move(set);
+    s->union_hour = std::move(hour);
+    s->union_count = std::move(count);
+    s->union_cap = cap;
+    s->records = std::move(records);  // last: a state with records has all of it
+    return CTMR_OK;
+}
+
 struct CrlChunk {
     uint64_t lo = 0, hi = 0;  // CRLs of the batch
     uint64_t bytes = 0;
@@ -594,11 +737,8 @@ int crl_scan_members(ctmr_ctx* const* m, uint32_t W, uint64_t slots, ctmr_group*
     return CTMR_OK;
 }
 
-// One chunk on member 0 (`c`): split, parse, join (every member's table), copy back.  *base: entries placed so far; with
-// `count_only` (the caller's entry_cap is already exceeded) only the count advances.
-int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, ctmr_crl_out* out, const CrlChunk& ch, int st,
-              uint64_t* base, bool* count_only) {
-    ctmr_ctx* c = m[0];
+// The split of chunk `ch` in stage[st] on the ctx's stream, up to the compaction: *ne = the chunk's entries (epos, ecrl)
+int crl_split(ctmr_ctx* c, const CrlChunk& ch, int st, uint32_t* ne_out) {
     CrlState* s = c->crl.get();
     cudaStream_t q = c->stream;
     const uint32_t n = (uint32_t)(ch.hi - ch.lo);
@@ -644,39 +784,15 @@ int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batc
         CU(c, cudaStreamSynchronize(q));
         ne = last[0] + last[1];
     }
-    if (*count_only || *base + ne > out->entry_cap) {
-        *count_only = true;
-        *base += ne;
-        CU(c, cudaEventRecord(s->consumed[st], q));
-        return CTMR_OK;
-    }
-    EntryOut eo{s->eserial_off, s->eserial_len, s->ereason, s->estatus, s->eknown, s->erevoked, s->ehour, s->eslot, s->esets};
-    if (ne) {
-        crl_entry_kernel<<<grid(ne, 256), 256, 0, q>>>(stage, s->desc[st], s->res, s->epos, s->ecrl, ne, eo);
-        CU(c, cudaGetLastError());
-        uint64_t slots = 64;
-        while (slots < 2ull * ne) slots <<= 1;
-        int rc = crl_set_ensure(c, slots, W > 1);
-        if (rc) return group_fail(g, c, rc);
-        slots = s->set_cap;  // the set spans its whole allocation: every member probes with the same mask
-        CU(c, cudaMemsetAsync(s->set, 0, slots * sizeof(CrlSetSlot), q));
-        CU(c, cudaMemsetAsync(s->set_hour, 0x7f, slots * sizeof(int32_t), q));
-        CU(c, cudaMemsetAsync(s->set_count, 0, slots * sizeof(uint32_t), q));
-        crl_set_insert_kernel<<<grid(ne, 256), 256, 0, q>>>(stage, s->desc[st], s->res, s->ecrl, s->eserial_off, s->eserial_len, s->estatus, ne,
-                                                           s->set, slots - 1, s->eslot);
-        CU(c, cudaGetLastError());
-        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->set, slots - 1, s->set_hour, s->set_count);
-        CU(c, cudaGetLastError());
-        if (W > 1) {
-            rc = crl_scan_members(m, W, slots, g);
-            if (rc) return rc;
-        }
-        crl_finish_kernel<<<grid(ne, 256), 256, 0, q>>>(s->eslot, s->set_hour, s->set_count, ne, eo);
-        CU(c, cudaGetLastError());
-    }
-    CU(c, cudaEventRecord(s->consumed[st], q));
-    // per-entry outputs straight into the caller's arrays
-    const uint64_t at = *base;
+    *ne_out = ne;
+    return CTMR_OK;
+}
+
+// the per-entry outputs of the chunk's ne entries to the caller's entries [at, at + ne), then its per-CRL fields; waits
+int crl_copy_back(ctmr_ctx* c, ctmr_crl_out* out, const CrlChunk& ch, uint64_t at, uint32_t ne) {
+    CrlState* s = c->crl.get();
+    cudaStream_t q = c->stream;
+    const uint32_t n = (uint32_t)(ch.hi - ch.lo);
     auto back = [&](void* dst, const void* src, size_t per) -> cudaError_t {
         if (!dst || !ne) return cudaSuccess;
         return cudaMemcpyAsync(static_cast<uint8_t*>(dst) + at * per, src, (size_t)ne * per, cudaMemcpyDeviceToHost, q);
@@ -709,39 +825,95 @@ int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batc
         if (out->crl_first) out->crl_first[i] = first;
         first += listed ? r.count : 0u;
     }
+    return CTMR_OK;
+}
+
+EntryOut entry_out(CrlState* s) {
+    return EntryOut{s->eserial_off, s->eserial_len, s->ereason, s->estatus, s->eknown, s->erevoked, s->ehour, s->eslot, s->esets};
+}
+
+// One chunk on member 0 (`c`): split, parse, join (every member's table), copy back.  *base: entries placed so far; with
+// `count_only` (the caller's entry_cap is already exceeded) only the count advances.
+int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, ctmr_crl_out* out, const CrlChunk& ch, int st, uint64_t* base,
+              bool* count_only) {
+    ctmr_ctx* c = m[0];
+    CrlState* s = c->crl.get();
+    cudaStream_t q = c->stream;
+    const uint8_t* stage = s->stage[st];
+    uint32_t ne = 0;
+    int rc = crl_split(c, ch, st, &ne);
+    if (rc) return rc;
+    if (*count_only || *base + ne > out->entry_cap) {
+        *count_only = true;
+        *base += ne;
+        CU(c, cudaEventRecord(s->consumed[st], q));
+        return CTMR_OK;
+    }
+    const EntryOut eo = entry_out(s);
+    if (ne) {
+        crl_entry_kernel<<<grid(ne, 256), 256, 0, q>>>(stage, s->desc[st], s->res, s->epos, s->ecrl, ne, eo);
+        CU(c, cudaGetLastError());
+        uint64_t slots = 64;
+        while (slots < 2ull * ne) slots <<= 1;
+        int rc = crl_set_ensure(c, slots, W > 1);
+        if (rc) return group_fail(g, c, rc);
+        slots = s->set_cap;  // the set spans its whole allocation: every member probes with the same mask
+        CU(c, cudaMemsetAsync(s->set, 0, slots * sizeof(CrlSetSlot), q));
+        CU(c, cudaMemsetAsync(s->set_hour, 0x7f, slots * sizeof(int32_t), q));
+        CU(c, cudaMemsetAsync(s->set_count, 0, slots * sizeof(uint32_t), q));
+        crl_set_insert_kernel<<<grid(ne, 256), 256, 0, q>>>(stage, s->desc[st], s->res, s->ecrl, s->eserial_off, s->eserial_len, s->estatus, ne,
+                                                           s->set, slots - 1, s->eslot);
+        CU(c, cudaGetLastError());
+        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->set, slots - 1, s->set_hour, s->set_count);
+        CU(c, cudaGetLastError());
+        if (W > 1) {
+            rc = crl_scan_members(m, W, slots, g);
+            if (rc) return rc;
+        }
+        crl_finish_kernel<<<grid(ne, 256), 256, 0, q>>>(s->eslot, s->set_hour, s->set_count, ne, eo);
+        CU(c, cudaGetLastError());
+    }
+    CU(c, cudaEventRecord(s->consumed[st], q));
+    // per-entry outputs straight into the caller's arrays
+    rc = crl_copy_back(c, out, ch, *base, ne);
+    if (rc) return rc;
     *base += ne;
     return CTMR_OK;
 }
 
-// the call on member 0 of `W` members (W == 1: one ctx)
-int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, ctmr_crl_out* out) {
-    ctmr_ctx* c = m[0];
-    CU(c, cudaSetDevice(c->device));
-    if (!b || !out) return group_fail(g, c, fail(c, CTMR_E_INVALID, "ctmr_revoked_known: NULL batch or output"));
+// The checks every call makes before any work: the arguments, and each CRL inside data and no larger than a chunk
+int crl_check_batch(ctmr_ctx* c, const ctmr_crl_batch* b, const ctmr_crl_out* out) {
+    if (!b || !out) return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: NULL batch or output");
     if (b->n_crls && (!b->data || !b->crl_off || !b->crl_len || !b->issuer_digest))
-        return group_fail(g, c, fail(c, CTMR_E_INVALID, "ctmr_revoked_known: NULL input array"));
-    const uint64_t B = ((c->stage_bytes < kCrlBudgetMax ? c->stage_bytes : kCrlBudgetMax) + 15) / 16 * 16;
+        return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: NULL input array");
+    const uint64_t B = crl_budget(c);
     for (uint64_t k = 0; k < b->n_crls; ++k) {
         const uint64_t off = b->crl_off[k], len = b->crl_len[k];
         if (off > b->data_bytes || len > b->data_bytes - off)
-            return group_fail(g, c, fail(c, CTMR_E_INVALID, "ctmr_revoked_known: CRL " + std::to_string(k) + " lies outside data"));
+            return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: CRL " + std::to_string(k) + " lies outside data");
         if (len > B)
-            return group_fail(g, c, fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: CRL " + std::to_string(k) + " (" + std::to_string(len) +
-                                                                    " bytes) exceeds the staging budget of " + std::to_string(B) + " bytes"));
+            return fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: CRL " + std::to_string(k) + " (" + std::to_string(len) +
+                                                       " bytes) exceeds the staging budget of " + std::to_string(B) + " bytes");
     }
-    out->n_entries = 0;
-    if (b->n_crls == 0) return CTMR_OK;
-    // the issuers' dense indices: read from the registry, never registered here
-    std::vector<uint32_t> issuer(b->n_crls);
+    return CTMR_OK;
+}
+
+// the issuers' dense indices: read from the registry, never registered here
+int crl_issuers(ctmr_ctx* c, const ctmr_crl_batch* b, std::vector<uint32_t>& issuer) {
+    issuer.assign(b->n_crls, CTMR_ISSUER_NONE);
     for (uint64_t k = 0; k < b->n_crls; ++k) {
         uint32_t idx = 0;
         bool found = false;
-        int rc = lookup_digest(c, b->issuer_digest + 32 * k, false, &idx, &found);
-        if (rc) return group_fail(g, c, rc);
+        const int rc = lookup_digest(c, b->issuer_digest + 32 * k, false, &idx, &found);
+        if (rc) return rc;
         issuer[k] = found ? idx : CTMR_ISSUER_NONE;
     }
-    int rc = crl_ensure(c);
-    if (rc) return group_fail(g, c, rc);
+    return CTMR_OK;
+}
+
+// the batch cut into chunks of whole CRLs of at most the budget's bytes
+std::vector<CrlChunk> crl_cut(ctmr_ctx* c, const ctmr_crl_batch* b) {
+    const uint64_t B = crl_budget(c);
     std::vector<CrlChunk> chunks;
     for (uint64_t k = 0; k < b->n_crls;) {
         CrlChunk ch;
@@ -757,6 +929,23 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
         while ((1ull << ch.rounds) < chain) ++ch.rounds;
         chunks.push_back(ch);
     }
+    return chunks;
+}
+
+// the call on member 0 of `W` members (W == 1: one ctx)
+int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, ctmr_crl_out* out) {
+    ctmr_ctx* c = m[0];
+    CU(c, cudaSetDevice(c->device));
+    int rc = crl_check_batch(c, b, out);
+    if (rc) return group_fail(g, c, rc);
+    out->n_entries = 0;
+    if (b->n_crls == 0) return CTMR_OK;
+    std::vector<uint32_t> issuer;
+    rc = crl_issuers(c, b, issuer);
+    if (rc) return group_fail(g, c, rc);
+    rc = crl_ensure(c);
+    if (rc) return group_fail(g, c, rc);
+    const std::vector<CrlChunk> chunks = crl_cut(c, b);
     uint64_t base = 0;
     bool count_only = false;
     rc = crl_upload(c, b, issuer, chunks[0], 0);
@@ -766,7 +955,7 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
             rc = crl_upload(c, b, issuer, chunks[i + 1], (int)((i + 1) & 1));
             if (rc) return group_fail(g, c, rc);
         }
-        rc = crl_chunk(m, W, g, b, out, chunks[i], (int)(i & 1), &base, &count_only);
+        rc = crl_chunk(m, W, g, out, chunks[i], (int)(i & 1), &base, &count_only);
         if (rc) {
             cudaStreamSynchronize(c->crl->copy_stream);
             return group_fail(g, c, rc);
@@ -780,6 +969,186 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
     return CTMR_OK;
 }
 
+// ---- one process per GPU: the collective call on a ctx attached to peers (include/ctmr.h states the rules) -----------
+// Every rank checks its batch and builds its buffers, then agreement 1 posts its chunk count (or that it failed).  For
+// each step k below the most chunks any rank has, a rank with a chunk k parses it (one without has no entries),
+// agreement 2 posts how many entries it sends, and ceil(the largest count / X) rounds follow:
+//     send:  each rank's next <= X entries as records, built from the staged chunk, into its region on EVERY rank (the
+//            hour is unknown: no owner routing) + count
+//     -- barrier: every region of the round has landed --
+//     owner: the valid records received into the union set, one pass over the own shard, each record's answer in place
+//     -- barrier: every owner's answers are in --
+//     pull:  each rank reads its records' answers from every owner: the lowest hour, the sum of the counts
+// One parity of the regions is enough because the rounds are synchronous: a source writes round j + 1 into its regions
+// only after its own pull of round j (stream order), and every owner's reads and answers of round j came before the
+// second barrier of round j, which the source has passed.  A final agreement makes any later failure every rank's.
+constexpr uint64_t kPeerFailed = 1ull << 63;
+
+// One agreement: every rank's word in row (kPeerFailed: that rank failed).  Returns this rank's own error `mine`,
+// CTMR_E_PEER_FAILED when only another rank failed, or a barrier's timeout.
+int crl_agree(ctmr_ctx* c, int mine, uint64_t word, uint64_t* row) {
+    const std::string err = c->err;
+    int rc = peer_mailbox(c, mine ? kPeerFailed : word, row);
+    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
+    if (rc) return rc;
+    if (mine) {
+        c->err = err;
+        return mine;
+    }
+    for (uint32_t r = 0; r < c->st.peer.world; ++r)
+        if (row[r] & kPeerFailed)
+            return fail(c, CTMR_E_PEER_FAILED, "ctmr_revoked_known: rank " + std::to_string(r) + "'s part of this collective call failed");
+    return CTMR_OK;
+}
+
+// the per-entry outputs of a parsed chunk's ne entries
+int crl_peer_entries(ctmr_ctx* c, int st, uint32_t ne) {
+    CrlState* s = c->crl.get();
+    crl_entry_kernel<<<grid(ne, 256), 256, 0, c->stream>>>(s->stage[st], s->desc[st], s->res, s->epos, s->ecrl, ne, entry_out(s));
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
+}
+
+// entries [lo, lo + n) of the chunk in stage[st] as records, sent to every rank with the count (n == 0: the count only)
+int crl_peer_send(ctmr_ctx* c, int st, uint64_t lo, uint64_t n) {
+    CrlState* s = c->crl.get();
+    if (n) {
+        crl_peer_records_kernel<<<grid(n, 256), 256, 0, c->stream>>>(s->stage[st], s->desc[st], s->res, s->ecrl, s->eserial_off,
+                                                                     s->eserial_len, s->estatus, (uint32_t)lo, (uint32_t)n, s->records);
+        CU(c, cudaGetLastError());
+    }
+    crl_peer_send_kernel<<<dim3(grid(4 * (n ? n : 1), 256), c->px.world), 256, 0, c->stream>>>(c->px, s->records, n);
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
+}
+
+// the owner's part of a round: agreed.n[s] records from source s, `total` of them, at most `most` from one source
+int crl_peer_owner(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uint64_t total) {
+    CrlState* s = c->crl.get();
+    const cudaStream_t q = c->stream;
+    const uint64_t slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
+    CU(c, cudaMemsetAsync(s->union_set, 0, slots * sizeof(CrlSetSlot), q));
+    CU(c, cudaMemsetAsync(s->union_hour, 0x7f, slots * sizeof(int32_t), q));
+    CU(c, cudaMemsetAsync(s->union_count, 0, slots * sizeof(uint32_t), q));
+    const dim3 g(grid(most, 256), c->px.world);
+    crl_union_insert_kernel<<<g, 256, 0, q>>>(c->px, agreed, s->union_set, slots - 1, c->in_slot);
+    CU(c, cudaGetLastError());
+    crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->union_set, slots - 1, s->union_hour,
+                                                          s->union_count);
+    CU(c, cudaGetLastError());
+    crl_peer_answer_kernel<<<g, 256, 0, q>>>(c->px, agreed, c->in_slot, s->union_hour, s->union_count);
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
+}
+
+// Round j of a step whose sent entries are row[0..world), this rank's chunk in stage[st].  `work` false (this rank
+// failed): nothing but the two barriers, which every rank issues whatever happens, so that a failure never leaves another
+// rank waiting.
+int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int st) {
+    const uint64_t X = c->px.X, lo = j * X;
+    const auto in_round = [&](uint64_t n) -> uint64_t { return n > lo ? std::min(X, n - lo) : 0; };
+    CrlRoundCounts agreed{};
+    uint64_t most = 0, total = 0;
+    for (uint32_t r = 0; r < c->px.world; ++r) {
+        agreed.n[r] = in_round(row[r]);
+        most = std::max<uint64_t>(most, agreed.n[r]);
+        total += agreed.n[r];
+    }
+    const uint64_t mine = agreed.n[c->px.rank];
+    int rc = work ? crl_peer_send(c, st, lo, mine) : CTMR_OK;
+    int brc = peer_barrier(c, CH_CRL, c->stream);
+    if (rc == CTMR_OK) rc = brc;
+    if (rc == CTMR_OK && work && total) rc = crl_peer_owner(c, agreed, most, total);
+    brc = peer_barrier(c, CH_CRL, c->stream);
+    if (rc == CTMR_OK) rc = brc;
+    if (rc == CTMR_OK && work && mine) {
+        CrlState* s = c->crl.get();
+        crl_peer_pull_kernel<<<grid(mine, 256), 256, 0, c->stream>>>(c->px, mine, lo, s->eknown, s->ehour, s->esets);
+        CU(c, cudaGetLastError());
+    }
+    return rc;
+}
+
+// this rank's part of the collective call
+int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) {
+    CU(c, cudaSetDevice(c->device));
+    if (out) out->n_entries = 0;
+    std::vector<uint32_t> issuer;
+    std::vector<CrlChunk> chunks;
+    // everything that can fail before any work, allocations included, so that it travels in agreement 1
+    int rc = crl_check_batch(c, b, out);
+    if (rc == CTMR_OK) rc = crl_issuers(c, b, issuer);
+    if (rc == CTMR_OK) rc = crl_ensure(c);
+    if (rc == CTMR_OK) rc = crl_peer_ensure(c);
+    if (rc == CTMR_OK) chunks = crl_cut(c, b);
+    uint64_t row[kMaxWorld] = {};
+    rc = crl_agree(c, rc, chunks.size(), row);
+    if (rc) return rc;
+    const uint32_t W = c->st.peer.world;
+    uint64_t steps = 0;
+    for (uint32_t r = 0; r < W; ++r) steps = std::max(steps, row[r]);
+    CrlState* s = c->crl.get();
+    uint64_t base = 0;
+    bool count_only = false;  // entry_cap is exceeded: the rank still answers the others' records, and sends none of its own
+    int local = CTMR_OK;      // this rank's error after agreement 1: it does no more work, and the ranks stop at the next agreement
+    std::string local_err;
+    const auto fail_locally = [&](int code) {
+        if (local) return;
+        local = code;
+        local_err = c->err;
+    };
+    if (!chunks.empty() && (rc = crl_upload(c, b, issuer, chunks[0], 0))) fail_locally(rc);
+    for (uint64_t k = 0; k < steps; ++k) {
+        const int st = (int)(k & 1);
+        const bool mine = k < chunks.size() && !local;
+        uint32_t ne = 0;
+        uint64_t send = 0;
+        if (mine) {
+            rc = k + 1 < chunks.size() ? crl_upload(c, b, issuer, chunks[k + 1], st ^ 1) : CTMR_OK;
+            if (rc == CTMR_OK) rc = crl_split(c, chunks[k], st, &ne);
+            if (rc == CTMR_OK && (count_only || base + ne > out->entry_cap)) {
+                count_only = true;
+            } else if (rc == CTMR_OK && ne) {
+                rc = crl_peer_entries(c, st, ne);
+                send = ne;
+            }
+            if (rc) fail_locally(rc);
+        }
+        rc = peer_mailbox(c, local ? kPeerFailed : send, row);  // agreement 2
+        if (rc) {
+            fail_locally(rc);
+            break;
+        }
+        uint64_t most = 0;
+        bool stop = false;
+        for (uint32_t r = 0; r < W; ++r) {
+            stop |= (row[r] & kPeerFailed) != 0;
+            most = std::max(most, row[r] & ~kPeerFailed);
+        }
+        if (stop) break;  // every rank saw the same row: all go to the final agreement
+        for (uint64_t j = 0; j * c->px.X < most; ++j)  // the rounds build their records from the staged chunk
+            if ((rc = crl_peer_round(c, row, j, !local, st))) fail_locally(rc);
+        if (!mine || local) continue;
+        if (cudaEventRecord(s->consumed[st], c->stream) != cudaSuccess) {  // the rounds' last read of stage[st] is issued
+            fail_locally(fail(c, CTMR_E_CUDA, "cudaEventRecord failed"));
+            continue;
+        }
+        if (!count_only && (rc = crl_copy_back(c, out, chunks[k], base, ne))) fail_locally(rc);
+        base += ne;
+    }
+    const cudaStream_t drain[] = {s->copy_stream, c->stream};
+    drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
+    if (!local && (rc = ctmr_check_device(c, nullptr))) fail_locally(rc);  // a barrier of a round that timed out
+    if (local) c->err = local_err;
+    rc = crl_agree(c, local, 0, row);
+    if (rc) return rc;
+    out->n_entries = base;
+    if (count_only)
+        return fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: entry_cap " + std::to_string(out->entry_cap) + " < " + std::to_string(base) +
+                                                   " entries");
+    return CTMR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -787,7 +1156,7 @@ extern "C" {
 int ctmr_revoked_known(ctmr_ctx* c, const ctmr_crl_batch* batch, ctmr_crl_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: a member of a group; use ctmr_group_revoked_known");
-    if (c->peer_mode == PEER_IPC) return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: a ctx attached to peers holds part of the table");
+    if (c->peer_mode == PEER_IPC && c->st.peer.world > 1) return revoked_known_peer(c, batch, out);
     ctmr_ctx* m[1] = {c};
     return revoked_known(m, 1, nullptr, batch, out);
 }

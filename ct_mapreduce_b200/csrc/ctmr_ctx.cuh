@@ -339,6 +339,13 @@ struct CrlState {
     DevBuf<CrlSetSlot> set;
     DevBuf<int32_t> set_hour, recv_hour;   // recv_*: a group's member 0 receives the other members' answers there
     DevBuf<uint32_t> set_count, recv_count;
+    // a rank attached to peers (crl_peer_ensure): the 64-byte records it sends in a round [X], and the owner side's union
+    // set of the records every rank sends in a round [union_cap = 2 world X, a power of two] with its answers
+    DevBuf<ctmr_key> records;
+    uint64_t union_cap = 0;
+    DevBuf<CrlSetSlot> union_set;
+    DevBuf<int32_t> union_hour;
+    DevBuf<uint32_t> union_count;
 };
 
 // the ctx's private device words (one allocation)
@@ -382,6 +389,7 @@ enum : uint32_t {
     CH_DEV_MAP = 6, CH_DEV_RESOLVE = 7,  // ctmr_process_device
     CH_USER = 8, CH_HIST_A = 9, CH_HIST_B = 10, CH_RESET_A = 11, CH_RESET_B = 12, CH_MAILBOX = 13,
     CH_CKPT = 14,                        // ctmr_checkpoint_*: every barrier and agreement of the collective size, save and load
+    CH_CRL = 15,                         // ctmr_revoked_known: the two barriers of each round of a collective call
     CH_STAGE_META = 16                   // + stage index (3): after the string-identity insert of a host-pipeline round
 };
 

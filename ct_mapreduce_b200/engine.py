@@ -652,7 +652,8 @@ class GpuCertDatabase:
 
     def peer_attach(self, rank: int, world: int, handles: list):
         """handles[r] = rank r's peer_export().  Afterwards process_device / store_batch / reset_device and the front end
-        (store_raw_entries, store_tiles, with or without trees) are collective."""
+        (store_raw_entries, store_tiles, with or without trees), checkpoint / load_checkpoint and revoked_known are
+        collective."""
         buf = (C.c_uint8 * (capi.PEER_HANDLE_BYTES * world)).from_buffer_copy(b"".join(handles))
         self._check(self._lib.ctmr_peer_attach(self._h, rank, world, buf))
         self._peers = world > 1
@@ -671,15 +672,19 @@ class GpuCertDatabase:
         return n.value
 
     @contextlib.contextmanager
-    def _peer_refusal(self):
-        """On a db attached to peers the front end is collective: a rank that gives up on a call before making it
-        (an argument its binding refuses, a failed fetch) still makes it with no batch, so that the other ranks return
-        CTMR_E_PEER_FAILED instead of waiting at a barrier."""
+    def _peer_refusal(self, call=None):
+        """On a db attached to peers the front end and revoked_known are collective: a rank that gives up on a call
+        before making it (an argument its binding refuses, a failed fetch) still makes it with no batch, so that the other
+        ranks return CTMR_E_PEER_FAILED instead of waiting at a barrier.  `call` makes that call (default: the front
+        end's ctmr_process_raw)."""
         try:
             yield
         except Exception:
             if self._peers:
-                self._lib.ctmr_process_raw(self._h, None, None)
+                if call is None:
+                    self._lib.ctmr_process_raw(self._h, None, None)
+                else:
+                    call()
             raise
 
     def _join_resumes(self):
@@ -725,21 +730,26 @@ class GpuCertDatabase:
     def revoked_known(self, crls, issuer_digests, entry_cap: int | None = None) -> RevokedResult:
         """Which revoked serials of these CRLs are known certificates (ctmr_revoked_known).  `crls`: a list of DER CRLs,
         or (data, crl_off, crl_len); `issuer_digests`: per CRL the 32-byte Issuer.ID() digest whose crl:: set named it.
-        Read-only.  entry_cap defaults to the bound that always suffices (total bytes // 18)."""
-        if isinstance(crls, tuple):
-            data, offs, lens = (np.ascontiguousarray(a) for a in crls)
-            data, offs, lens = data.astype(np.uint8, copy=False), offs.astype(np.uint64), lens.astype(np.uint64)
-        else:
-            data, offs, lens = pack_crls(crls)
-        n = len(offs)
-        dig = np.frombuffer(b"".join(bytes(d) for d in issuer_digests), np.uint8) if n else np.zeros(32, np.uint8)
-        if dig.size != 32 * n:
-            raise ValueError("one 32-byte issuer digest per CRL")
-        cap = int(lens.sum()) // capi.CRL_MIN_ENTRY if entry_cap is None else int(entry_cap)
-        res = RevokedResult(n, cap)
-        b = capi.CrlBatch(capi.ptr(data) if data.size else None, data.size, capi.ptr(offs) if n else None,
-                          capi.ptr(lens) if n else None, capi.ptr(dig) if n else None, n)
-        o = res.to_c()
+        Read-only.  entry_cap defaults to the bound that always suffices (total bytes // 18).  An empty list of CRLs
+        (and of digests) returns an empty result.
+        On a db attached to peers the call is collective: every rank calls it with its own CRLs (an empty list will do)
+        and gets the answers for its own CRLs against every rank's shard.  A rank whose arguments are refused here
+        still makes the call, with no batch, so that the other ranks return CTMR_E_PEER_FAILED, and then raises."""
+        with self._peer_refusal(lambda: self._revoked_known_fn()(self._h, None, None)):
+            if isinstance(crls, tuple):
+                data, offs, lens = (np.ascontiguousarray(a) for a in crls)
+                data, offs, lens = data.astype(np.uint8, copy=False), offs.astype(np.uint64), lens.astype(np.uint64)
+            else:
+                data, offs, lens = pack_crls(crls)
+            n = len(offs)
+            dig = np.frombuffer(b"".join(bytes(d) for d in issuer_digests), np.uint8) if n else np.zeros(32, np.uint8)
+            if n and dig.size != 32 * n:
+                raise ValueError("one 32-byte issuer digest per CRL")
+            cap = int(lens.sum()) // capi.CRL_MIN_ENTRY if entry_cap is None else int(entry_cap)
+            res = RevokedResult(n, cap)
+            b = capi.CrlBatch(capi.ptr(data) if data.size else None, data.size, capi.ptr(offs) if n else None,
+                              capi.ptr(lens) if n else None, capi.ptr(dig) if n else None, n)
+            o = res.to_c()
         rc = self._revoked_known_fn()(self._h, C.byref(b), C.byref(o))
         res.n_entries = int(o.n_entries)
         try:

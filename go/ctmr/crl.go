@@ -7,6 +7,7 @@ package ctmr
 import "C"
 
 import (
+	"fmt"
 	"unsafe"
 )
 
@@ -34,11 +35,24 @@ type CRLResult struct {
 
 // RevokedKnown parses DER CRLs on the GPU and answers, per entry, whether the serial is a known certificate of the
 // issuer whose crl:: set named the CRL (issuerIDs[i] is that Issuer.ID() digest, 32 bytes).  Read-only.  On a DB
-// attached to peers the library refuses the call.
+// attached to peers the call is collective: every rank calls it with its own CRLs, none included, and gets the
+// answers for its own CRLs against every rank's shard; a rank whose arguments are refused still makes the call.  Fewer
+// issuer IDs than CRLs is an error (it used to be an index-out-of-range panic).
 func (d *DB) RevokedKnown(crls [][]byte, issuerIDs [][32]byte) ([]CRLResult, error) {
 	n := len(crls)
 	if n == 0 {
-		return nil, nil
+		if !d.peer {
+			return nil, nil
+		}
+		b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
+		defer C.free(unsafe.Pointer(b))
+		out := (*C.ctmr_crl_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_out{}))))
+		defer C.free(unsafe.Pointer(out))
+		return nil, d.err(C.ctmr_revoked_known(d.h, b, out), "ctmr_revoked_known")
+	}
+	if len(issuerIDs) < n { // one issuer ID per CRL; extra IDs are ignored, as before
+		err := fmt.Errorf("RevokedKnown: %d issuer IDs for %d CRLs", len(issuerIDs), n)
+		return nil, d.peerRefuseWith(err, func() { C.ctmr_revoked_known(d.h, nil, nil) })
 	}
 	total := 0
 	for _, c := range crls {

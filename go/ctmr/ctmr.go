@@ -151,8 +151,13 @@ func (d *DB) peerStopped() (uint32, error) {
 // peerRefuse: a peer DB that gives up on a front-end call before making it still makes it, with no batch, so that the
 // other ranks return CTMR_E_PEER_FAILED instead of waiting at a barrier.  It returns err.
 func (d *DB) peerRefuse(err error) error {
+	return d.peerRefuseWith(err, func() { C.ctmr_process_raw(d.h, nil, nil) })
+}
+
+// peerRefuseWith: the same for any collective call; call makes it with no batch.  It returns err.
+func (d *DB) peerRefuseWith(err error, call func()) error {
 	if d.peer {
-		C.ctmr_process_raw(d.h, nil, nil)
+		call()
 	}
 	return err
 }

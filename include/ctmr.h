@@ -252,7 +252,26 @@ int ctmr_checkpoint_load(ctmr_ctx* ctx, const uint8_t* const* parts, const uint6
  * CTMR_E_BATCH_TOO_LARGE before any work.
  *
  * Read-only: no index is taken and no table, counter or registry changes, so the call may come between any other calls.
- * A member ctx of a group (use ctmr_group_revoked_known) and a ctx attached to peers are refused with CTMR_E_INVALID.
+ * A member ctx of a group is refused with CTMR_E_INVALID: use ctmr_group_revoked_known.
+ *
+ * On a ctx attached to peers (ctmr_peer_attach, world > 1) the call is COLLECTIVE: every rank makes the same sequence of
+ * collective calls (a mismatch is undefined), each with its OWN batch, which may be empty (n_crls == 0).  Each rank gets
+ * the answers for its own CRLs only, and every output is what the call on one ctx holding the union of all ranks' tables
+ * gives for that batch: known_exp_hour is the lowest hour over every rank's sets and known_sets the sum over the ranks.
+ * The other ranks' batches make no difference to it.  Issuer digests are looked up in the shared registry (one that
+ * only another rank registered is found), and the call stays read-only on every rank.  Failures:
+ *   - the checks above (a NULL batch or output, a CRL outside data or larger than a chunk) run on every rank before any
+ *     work; if one fails anywhere, that rank returns its error and the others CTMR_E_PEER_FAILED, n_entries is 0 and
+ *     nothing else is written;
+ *   - a later failure on any rank (CUDA, an allocation, a barrier that timed out) is every rank's: that rank returns its
+ *     error, the others CTMR_E_PEER_FAILED, and the outputs are undefined;
+ *   - entry_cap too small is the rank's own: it still answers the other ranks' entries and returns
+ *     CTMR_E_BATCH_TOO_LARGE with the count needed, while the others succeed.
+ * A rank whose binding refuses its arguments before calling must still make the call (a NULL batch will do).  Cost: a
+ * CRL entry has no expiry, so an entry's sets may lie on any rank; every rank's records go to every rank, config.
+ * max_round_entries (X, at least max_batch_entries) per rank and round, and each round is one pass over each rank's
+ * shard.  A chunk takes ceil(the most entries any rank has in its chunk at that step / X) rounds (DESIGN.md "Revoked
+ * known certificates").
  * Out of scope: signature verification, fetching, and the semantics of delta and indirect CRLs beyond crl_flags and
  * CTMR_RV_INDIRECT. */
 enum { CTMR_CRL_OK = 0, CTMR_CRL_BAD = 1,          /* CertificateList / TBSCertList framing or fields */

@@ -425,6 +425,21 @@ int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row) {
     return CTMR_OK;
 }
 
+int peer_agree(ctmr_ctx* c, int mine, uint64_t payload, uint64_t* row, const char* call, const char* part, bool their_code) {
+    const std::string err = c->err;
+    int rc = peer_mailbox(c, peer_word(mine, payload), row);
+    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
+    if (rc) return rc;
+    if (mine) {
+        c->err = err;
+        return mine;
+    }
+    const uint32_t r = peer_row_failed(row, c->st.peer.world);
+    if (r == c->st.peer.world) return CTMR_OK;
+    return fail(c, their_code ? peer_word_code(row[r]) : CTMR_E_PEER_FAILED,
+                std::string(call) + "rank " + std::to_string(r) + "'s part of this " + part);
+}
+
 int PathOut::allocate(ctmr_ctx* c, uint64_t entries) {
     cap = entries;
     CU(c, alloc(status, entries)); CU(c, alloc(sha, entries * 32)); CU(c, alloc(was_unknown, entries)); CU(c, alloc(first, entries));
@@ -857,7 +872,7 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     // and meets the others at two barriers per round; round k of rank r carries the global indices
     // first_index + (k * world + r) * E .. , i.e. the rounds are ordered, and inside a round the ranks.
     const uint32_t world = c->st.peer.world, rank = c->st.peer.rank;
-    const bool coll = c->peer_mode == PEER_IPC && world > 1;
+    const bool coll = peer_call(c);
     if (c->peer_mode == PEER_GROUP && world > 1)
         return fail(c, CTMR_E_INVALID, "members of an in-process group are driven through ctmr_group_process_batch");
     if (want_meta && world > 1) return fail(c, CTMR_E_INVALID, "first_issuer_dn / first_crldp of a group come from the host-buffer call");

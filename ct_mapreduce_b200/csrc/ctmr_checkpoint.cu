@@ -24,8 +24,6 @@ static_assert(sizeof(CkptHeader) == 128, "checkpoint header layout");
 
 constexpr int64_t kEveryKey = INT64_MIN;  // compaction filter: no key is expired
 
-bool peer_call(const ctmr_ctx* c) { return c->peer_mode == PEER_IPC && c->st.peer.world > 1; }
-
 // the live records of one member's three tables
 struct MemberPlan {
     CompactPlan keys, pairs, meta;
@@ -258,45 +256,23 @@ int load_members(ctmr_ctx** m, uint32_t W, const uint8_t* const* parts, const ui
     return CTMR_OK;
 }
 
-// The mailbox word of a rank: 0, or its error code with the top bit set.
-constexpr uint64_t kFailed = 1ull << 63;
-uint64_t word_of(int rc) { return rc ? kFailed | (uint32_t)(-rc) : 0; }
-
-// One agreement of a collective load: every rank's word.  Returns CTMR_OK when no rank failed; otherwise this rank's own
-// error, or CTMR_E_PEER_FAILED (peer_failed_code) or the code of the lowest rank that failed.
-int peer_outcome(ctmr_ctx* c, int mine, bool peer_failed_code) {
-    const std::string err = c->err;
-    uint64_t row[kMaxWorld] = {};
-    int rc = peer_mailbox(c, word_of(mine), row);
-    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
-    if (rc) return rc;
-    if (mine) {
-        c->err = err;
-        return mine;
-    }
-    for (uint32_t r = 0; r < c->st.peer.world; ++r)
-        if (row[r] & kFailed) {
-            const int code = peer_failed_code ? CTMR_E_PEER_FAILED : -(int)(uint32_t)row[r];
-            return fail(c, code, "rank " + std::to_string(r) + "'s part of this checkpoint load failed");
-        }
-    return CTMR_OK;
-}
-
 // a rank attached to peers: its part of the collective load
 int load_peer(ctmr_ctx* c, const uint8_t* const* parts, const uint64_t* bytes, uint32_t n_parts) {
     std::vector<CkptHeader> hs;
     RegistryUpload u;
     const bool reg = c->st.peer.rank == 0;
+    uint64_t row[kMaxWorld] = {};
     int rc = check_parts(c, parts, bytes, n_parts, hs);
     if (rc == CTMR_OK) rc = load_prepare(c, reg, hs[0].n_issuers, u);
-    rc = peer_outcome(c, rc, true);  // every rank's checks passed, or every rank returns unchanged
+    // every rank's checks passed, or every rank returns unchanged
+    rc = peer_agree(c, rc, 0, row, "", "checkpoint load failed");
     if (rc) return rc;
     rc = load_clear(c);
     if (rc == CTMR_OK && reg) rc = snap_registry_restore(c, parts[0] + sizeof(CkptHeader), hs[0].n_issuers, u);
     const int brc = peer_barrier(c, CH_CKPT, c->stream);  // the registry is whole before any rank goes on
     if (rc == CTMR_OK) rc = brc;
     if (rc == CTMR_OK) rc = load_records(c, parts, hs);  // checks the device: a barrier that timed out too
-    rc = peer_outcome(c, rc, false);
+    rc = peer_agree(c, rc, 0, row, "", "checkpoint load failed", true);  // the failed rank's own code on every rank
     if (rc) {
         load_undo(&c, 1);
         return rc;

@@ -982,24 +982,6 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
 // One parity of the regions is enough because the rounds are synchronous: a source writes round j + 1 into its regions
 // only after its own pull of round j (stream order), and every owner's reads and answers of round j came before the
 // second barrier of round j, which the source has passed.  A final agreement makes any later failure every rank's.
-constexpr uint64_t kPeerFailed = 1ull << 63;
-
-// One agreement: every rank's word in row (kPeerFailed: that rank failed).  Returns this rank's own error `mine`,
-// CTMR_E_PEER_FAILED when only another rank failed, or a barrier's timeout.
-int crl_agree(ctmr_ctx* c, int mine, uint64_t word, uint64_t* row) {
-    const std::string err = c->err;
-    int rc = peer_mailbox(c, mine ? kPeerFailed : word, row);
-    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
-    if (rc) return rc;
-    if (mine) {
-        c->err = err;
-        return mine;
-    }
-    for (uint32_t r = 0; r < c->st.peer.world; ++r)
-        if (row[r] & kPeerFailed)
-            return fail(c, CTMR_E_PEER_FAILED, "ctmr_revoked_known: rank " + std::to_string(r) + "'s part of this collective call failed");
-    return CTMR_OK;
-}
 
 // the per-entry outputs of a parsed chunk's ne entries
 int crl_peer_entries(ctmr_ctx* c, int st, uint32_t ne) {
@@ -1082,7 +1064,7 @@ int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) 
     if (rc == CTMR_OK) rc = crl_peer_ensure(c);
     if (rc == CTMR_OK) chunks = crl_cut(c, b);
     uint64_t row[kMaxWorld] = {};
-    rc = crl_agree(c, rc, chunks.size(), row);
+    rc = peer_agree(c, rc, chunks.size(), row, "ctmr_revoked_known: ", "collective call failed");  // agreement 1
     if (rc) return rc;
     const uint32_t W = c->st.peer.world;
     uint64_t steps = 0;
@@ -1114,18 +1096,14 @@ int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) 
             }
             if (rc) fail_locally(rc);
         }
-        rc = peer_mailbox(c, local ? kPeerFailed : send, row);  // agreement 2
+        rc = peer_mailbox(c, peer_word(local, send), row);  // agreement 2
         if (rc) {
             fail_locally(rc);
             break;
         }
+        if (peer_row_failed(row, W) < W) break;  // every rank saw the same row: all go to the final agreement
         uint64_t most = 0;
-        bool stop = false;
-        for (uint32_t r = 0; r < W; ++r) {
-            stop |= (row[r] & kPeerFailed) != 0;
-            most = std::max(most, row[r] & ~kPeerFailed);
-        }
-        if (stop) break;  // every rank saw the same row: all go to the final agreement
+        for (uint32_t r = 0; r < W; ++r) most = std::max(most, row[r]);
         for (uint64_t j = 0; j * c->px.X < most; ++j)  // the rounds build their records from the staged chunk
             if ((rc = crl_peer_round(c, row, j, !local, st))) fail_locally(rc);
         if (!mine || local) continue;
@@ -1140,7 +1118,7 @@ int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) 
     drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
     if (!local && (rc = ctmr_check_device(c, nullptr))) fail_locally(rc);  // a barrier of a round that timed out
     if (local) c->err = local_err;
-    rc = crl_agree(c, local, 0, row);
+    rc = peer_agree(c, local, 0, row, "ctmr_revoked_known: ", "collective call failed");
     if (rc) return rc;
     out->n_entries = base;
     if (count_only)
@@ -1156,7 +1134,7 @@ extern "C" {
 int ctmr_revoked_known(ctmr_ctx* c, const ctmr_crl_batch* batch, ctmr_crl_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: a member of a group; use ctmr_group_revoked_known");
-    if (c->peer_mode == PEER_IPC && c->st.peer.world > 1) return revoked_known_peer(c, batch, out);
+    if (peer_call(c)) return revoked_known_peer(c, batch, out);
     ctmr_ctx* m[1] = {c};
     return revoked_known(m, 1, nullptr, batch, out);
 }

@@ -545,9 +545,16 @@ int group_fail(ctmr_group* g, ctmr_ctx* c, int rc);   // c's error becomes g's l
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise
+// c is one rank of a group of processes (ctmr_peer_attach): its front-end, checkpoint, CRL and batch calls are collective
+inline bool peer_call(const ctmr_ctx* c) { return c->peer_mode == PEER_IPC && c->st.peer.world > 1; }
 // one word from every rank through the mailbox, row[r] = rank r's; the caller then checks the device for a barrier that
 // timed out
 int peer_mailbox(ctmr_ctx* c, uint64_t mine, uint64_t* row);
+// One agreement of a collective call: posts peer_word(mine, payload) and reads every rank's word into row.  Returns, in
+// this order: a failed exchange or a barrier that timed out; this rank's own error `mine`, with its error text; the
+// failure of the lowest rank whose word failed, CTMR_E_PEER_FAILED (their_code: that rank's own code) with the text
+// "<call>rank r's part of this <part>"; CTMR_OK, row then holding every rank's payload.
+int peer_agree(ctmr_ctx* c, int mine, uint64_t payload, uint64_t* row, const char* call, const char* part, bool their_code = false);
 int refresh_digests(ctmr_ctx* c);                                   // host memo <- device registry
 int lookup_digest(ctmr_ctx* c, const uint8_t digest[32], bool insert, uint32_t* idx_out, bool* found);
 int upload_issuer_map(ctmr_ctx* c, const uint32_t* dense, uint32_t n);

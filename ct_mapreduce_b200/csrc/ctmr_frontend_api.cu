@@ -1233,7 +1233,6 @@ int fe_member(ctmr_ctx* c, const ctmr_dev_batch& db, const ctmr_dev_out& dout, i
 // and on whether every rank's checks passed.  Then every rank runs R rounds of the key exchange over its own chunks (an
 // empty chunk when it has none left, has stopped or has failed), and a last mailbox exchange tells every rank how many
 // ranks stopped at an unknown Chain[0] fingerprint: they resume with another collective call.
-bool peer_call(const ctmr_ctx* c) { return c->peer_mode == PEER_IPC && c->st.peer.world > 1; }
 
 // What the ranks of a collective call agreed on.
 struct PeerCall {
@@ -1243,36 +1242,10 @@ struct PeerCall {
     uint64_t span = 0;    // R * world * E: the indices the call takes once agreed
 };
 
-// The agreement word: the rank's chunk count, its E and whether it wants string identities, or that its checks failed.
-constexpr uint64_t kAgreeFailed = 1ull << 63, kAgreeMeta = 1ull << 62;
+// The agreement's payload (peer_word): the rank's chunk count, its E and whether it wants string identities.
+constexpr uint64_t kAgreeMeta = 1ull << 62;
 constexpr int kAgreeEShift = 40;  // E <= kStageEntries < 2^22 in bits 40..61, the chunk count below 2^40
 static_assert(kStageEntries < (1ull << 22), "agreement word layout");
-
-// Posts this rank's part (`mine_rc`: the result of its checks) and reads every rank's.  Returns the rank's own error,
-// CTMR_E_PEER_FAILED when only another rank failed, or CTMR_OK with *pc filled in.
-int peer_agree(ctmr_ctx* c, int mine_rc, uint64_t chunks, uint64_t E, bool meta, PeerCall* pc, bool* meta_out) {
-    const std::string err = c->err;
-    uint64_t row[kMaxWorld] = {};
-    const uint64_t mine = mine_rc ? kAgreeFailed : chunks | E << kAgreeEShift | (meta ? kAgreeMeta : 0);
-    int rc = peer_mailbox(c, mine, row);
-    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
-    if (rc) return rc;
-    if (mine_rc) {
-        c->err = err;
-        return mine_rc;
-    }
-    const uint32_t world = c->st.peer.world;
-    for (uint32_t r = 0; r < world; ++r) {
-        if (row[r] & kAgreeFailed) return fail(c, CTMR_E_PEER_FAILED, "rank " + std::to_string(r) + "'s part of this collective call failed before any work");
-        pc->rounds = std::max<uint64_t>(pc->rounds, row[r] & ((1ull << kAgreeEShift) - 1));
-        pc->E = std::max<uint64_t>(pc->E, (row[r] >> kAgreeEShift) & ((1ull << 22) - 1));
-        meta |= (row[r] & kAgreeMeta) != 0;
-    }
-    pc->rounds = std::max<uint64_t>(pc->rounds, 1);  // at least one round: its barriers fence the next call's post
-    pc->span = pc->rounds * world * pc->E;
-    *meta_out = meta;
-    return CTMR_OK;
-}
 
 // the chunks of the whole batch, cut by fit before the agreement exactly as the upload loop cuts them
 template <class Format>
@@ -1380,18 +1353,27 @@ int process_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format& fm, 
         return pc.on ? count_chunks(m[0], fm, &chunks) : CTMR_OK;
     };
     if (rc == CTMR_OK) rc = setup();
+    const uint64_t world = m[0]->st.peer.world, rank = m[0]->st.peer.rank;
     if (pc.on) {  // every check of every rank is done and no table has changed: the ranks go on together, or all return
-        bool meta = false;
         // E <= the key-exchange region X: alloc_exchange sizes X to at least the stage size, the front end's entry budget
-        rc = peer_agree(m[0], rc, chunks, rc ? 0 : m[0]->fe->cap_entries, rc ? false : want_meta(po), &pc, &meta);
+        const uint64_t mine = rc ? 0 : chunks | m[0]->fe->cap_entries << kAgreeEShift | (want_meta(po) ? kAgreeMeta : 0);
+        uint64_t row[kMaxWorld] = {};
+        rc = peer_agree(m[0], rc, mine, row, "", "collective call failed before any work");
         if (rc) return rc;
+        bool meta = false;
+        for (uint32_t r = 0; r < world; ++r) {
+            pc.rounds = std::max<uint64_t>(pc.rounds, row[r] & ((1ull << kAgreeEShift) - 1));
+            pc.E = std::max<uint64_t>(pc.E, (row[r] >> kAgreeEShift) & ((1ull << 22) - 1));
+            meta |= (row[r] & kAgreeMeta) != 0;
+        }
+        pc.rounds = std::max<uint64_t>(pc.rounds, 1);  // at least one round: its barriers fence the next call's post
+        pc.span = pc.rounds * world * pc.E;
         fm.meta = meta;
     } else {
         if (rc) return rc;
         fm.meta = want_meta(po);
         if (tree && total == 0) return tree_end(m[0], tree);
     }
-    const uint64_t world = m[0]->st.peer.world, rank = m[0]->st.peer.rank;
     uint64_t pem_base = 0;
     std::vector<Chunk> ch[2];  // round k's chunks in ch[k & 1], uploaded into stage k & 1
     rc = plan_round(m, W, fm, 0, 0, ch[0], failed);

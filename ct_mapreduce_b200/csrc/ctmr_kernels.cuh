@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cassert>
+
 #include "../../include/ctmr.h"
 #include "../../include/ctmr_frontend.h"
 
@@ -53,6 +55,24 @@ struct __align__(16) MetaSlot {      // IssuerMetadata string sets: identity = t
 // in one process, CUDA IPC across processes).
 constexpr uint32_t kMaxWorld = 8;
 constexpr uint32_t kParities = 3;   // exchange buffers in flight: the host pipeline's three stages / two rounds of the device path
+
+// The mailbox word a rank posts in an agreement of a collective call (peer_agree, ctmr_api.cu): its payload, below 2^63,
+// or, with bit 63 set, that its part failed and its error code.  Host functions of the word alone, so that a host test
+// compiles them.
+constexpr uint64_t kPeerWordFailed = 1ull << 63;
+inline uint64_t peer_word(int rc, uint64_t payload) {
+    if (rc != CTMR_OK) return kPeerWordFailed | (uint32_t)(-rc);
+    assert(payload < kPeerWordFailed);
+    return payload;
+}
+inline bool peer_word_failed(uint64_t w) { return (w & kPeerWordFailed) != 0; }
+inline int peer_word_code(uint64_t w) { return -(int)(uint32_t)w; }  // of a failed word
+// the lowest rank of row[0..world) whose word failed; world when none did
+inline uint32_t peer_row_failed(const uint64_t* row, uint32_t world) {
+    uint32_t r = 0;
+    while (r < world && !peer_word_failed(row[r])) ++r;
+    return r;
+}
 
 // exchange areas of every rank (peer visible).  Region of (parity p, source s) = element offset (p * world + s) * X.
 struct PeerExchange {

@@ -144,18 +144,6 @@ int plan_rounds(ctmr_ctx* c0, uint32_t W, const BatchArgs& a, std::vector<std::v
     return CTMR_OK;
 }
 
-// multi-process group: the ranks agree on the number of rounds of this collective call (the largest any rank needs)
-int agree_rounds(ctmr_ctx* c, uint64_t mine, uint64_t* agreed) {
-    uint64_t row[kMaxWorld] = {};
-    int rc = peer_mailbox(c, mine, row);
-    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
-    if (rc) return rc;
-    uint64_t mx = mine;
-    for (uint32_t r = 0; r < c->pf.world; ++r) mx = std::max<uint64_t>(mx, row[r]);
-    *agreed = mx ? mx : 1;  // at least one round: its barriers also fence the mailbox against the next call
-    return CTMR_OK;
-}
-
 // Upload of one member's slice to stage `sidx`, and the slice's description for run_round.  chain: the round follows
 // another, whose owner passes (and string identities) this round's must follow.
 int stage_slice(ctmr_ctx* c, int sidx, bool chain, const BatchArgs& a, const Slice& sl, const uint32_t* map_dev, bool meta,
@@ -269,7 +257,7 @@ int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, const 
     ctmr_ctx* c0 = m[0];
     *failed = c0;
     if (!out || (n && (!blob || !offsets))) return fail(c0, CTMR_E_INVALID, "bad argument");
-    const bool ipc = c0->peer_mode == PEER_IPC && c0->st.peer.world > 1;
+    const bool ipc = peer_call(c0);
     if (n == 0 && !ipc) {
         *failed = nullptr;
         return CTMR_OK;
@@ -316,11 +304,14 @@ int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, const 
     }
     uint64_t advance = n;
     if (ipc) {
-        // collective call: the agreed number of rounds, each rank's round k at (k * world + rank) * E above the base
+        // collective call: the agreed number of rounds, the most any rank needs, each rank's round k at
+        // (k * world + rank) * E above the base
         const uint32_t world = c0->st.peer.world, rank = c0->st.peer.rank;
-        uint64_t rounds = 0;
-        rc = agree_rounds(c0, plan.size(), &rounds);
+        uint64_t row[kMaxWorld] = {};
+        rc = peer_agree(c0, CTMR_OK, plan.size(), row, "", "collective call failed before any work");
         if (rc) return rc;
+        uint64_t rounds = 1;  // at least one round: its barriers also fence the mailbox against the next call
+        for (uint32_t r = 0; r < world; ++r) rounds = std::max(rounds, row[r]);
         plan.resize(rounds, std::vector<Slice>(1));
         for (uint64_t k = 0; k < rounds; ++k) {
             if (plan[k][0].hi == plan[k][0].lo) plan[k][0].lo = plan[k][0].hi = n;  // an empty round

@@ -6,15 +6,13 @@ library cuts (at most E requested entries each).  The entries each rank's bodies
 finds; the front-end fields come from oracle.raw_process on those strings.  Covered: a rank with no bodies, twins
 across ranks and rounds, PEM and string identities on one rank only, and a rank whose check fails (the other returns
 CTMR_E_PEER_FAILED, nothing changes, no index is taken).  Marked gpu."""
-import os
-import socket
-import sys
 
 import numpy as np
 import pytest
 
 import bodies_oracle as bo
-from conftest import NOW_NS, README_FILTER, ROOT
+from conftest import NOW_NS, README_FILTER
+from peer_ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -58,14 +56,6 @@ def chunks_of(maxes, counts):
     return out
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _keep(r, pem):
     p = r.path
     out = {f: getattr(p, f) for f in FIELDS + PARSED + META if getattr(p, f, None) is not None}
@@ -77,69 +67,60 @@ def _keep(r, pem):
     return out
 
 
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
+def _worker(rank, world):
+    import torch
+    import torch.distributed as dist
+    torch.cuda.set_device(0)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from ct_mapreduce_b200 import capi, engine, sharded
+    inp = inputs()
+    db = engine.GpuCertDatabase(device=0, table_capacity=1 << 16, issuer_cn_filter=README_FILTER, max_issuers=1024,
+                                max_batch_entries=E)
+    sharded.attach_peers(db)
+
+    def bodies(k, **kw):
+        bs, ms = inp[k]
+        offs = np.cumsum([0] + [len(b) for b in bs[:-1]]).astype(np.uint64)
+        return db.store_raw_bodies(b"".join(bs), offs, [len(b) for b in bs], ms, NOW_NS, **kw)
+
+    def nothing():
+        return db.store_raw_bodies(b"", np.zeros(0, np.uint64), [], [], NOW_NS)
+
+    res = {("idx", 0): db.next_index()}
+    dist.barrier()
+    # 1. ragged: rank 0 has three chunks, rank 1 none
+    r = bodies("A", want_meta=True) if rank == 0 else nothing()
+    res[1] = _keep(r, False)
+    res["idx", 1] = db.next_index()
+    # 2. both ranks; string identities on rank 1 only, PEM on rank 0 only
+    r = bodies("B", want_pem=True) if rank == 0 else bodies("A", want_meta=True)
+    res[2] = _keep(r, rank == 0)
+    res["idx", 2] = db.next_index()
+    # 3. twins across ranks and rounds
+    r = bodies("C%d" % rank)
+    res[3] = _keep(r, False)
+    res["idx", 3] = db.next_index()
+    # 4. rank 1 passes a body outside its text: it fails, rank 0 returns CTMR_E_PEER_FAILED, nothing changes
+    before = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts())
+    code = None
     try:
-        import torch
-        import torch.distributed as dist
-        torch.cuda.set_device(0)
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        from ct_mapreduce_b200 import capi, engine, sharded
-        inp = inputs()
-        db = engine.GpuCertDatabase(device=0, table_capacity=1 << 16, issuer_cn_filter=README_FILTER, max_issuers=1024,
-                                    max_batch_entries=E)
-        sharded.attach_peers(db)
-
-        def bodies(k, **kw):
-            bs, ms = inp[k]
-            offs = np.cumsum([0] + [len(b) for b in bs[:-1]]).astype(np.uint64)
-            return db.store_raw_bodies(b"".join(bs), offs, [len(b) for b in bs], ms, NOW_NS, **kw)
-
-        def nothing():
-            return db.store_raw_bodies(b"", np.zeros(0, np.uint64), [], [], NOW_NS)
-
-        res = {("idx", 0): db.next_index()}
-        dist.barrier()
-        # 1. ragged: rank 0 has three chunks, rank 1 none
-        r = bodies("A", want_meta=True) if rank == 0 else nothing()
-        res[1] = _keep(r, False)
-        res["idx", 1] = db.next_index()
-        # 2. both ranks; string identities on rank 1 only, PEM on rank 0 only
-        r = bodies("B", want_pem=True) if rank == 0 else bodies("A", want_meta=True)
-        res[2] = _keep(r, rank == 0)
-        res["idx", 2] = db.next_index()
-        # 3. twins across ranks and rounds
-        r = bodies("C%d" % rank)
-        res[3] = _keep(r, False)
-        res["idx", 3] = db.next_index()
-        # 4. rank 1 passes a body outside its text: it fails, rank 0 returns CTMR_E_PEER_FAILED, nothing changes
-        before = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts())
-        code = None
-        try:
-            if rank == 1:
-                db.store_raw_bodies(b"{}", [1], [2], [1], NOW_NS)
-            else:
-                bodies("A")
-        except capi.CtmrError as e:
-            code = e.code
-        res[4] = (code, before == (db.table_stats(), db.status_counters().tolist(), db.issuer_counts()))
-        res["idx", 4] = db.next_index()
-        # 5. the next good call
-        r = bodies("B") if rank == 1 else nothing()
-        res[5] = _keep(r, False)
-        res["idx", 5] = db.next_index()
-        res["counts"] = db.issuer_counts()
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        db.close()
-        dist.destroy_process_group()
-    except Exception:  # surface the failure instead of a silent hang of the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+        if rank == 1:
+            db.store_raw_bodies(b"{}", [1], [2], [1], NOW_NS)
+        else:
+            bodies("A")
+    except capi.CtmrError as e:
+        code = e.code
+    res[4] = (code, before == (db.table_stats(), db.status_counters().tolist(), db.issuer_counts()))
+    res["idx", 4] = db.next_index()
+    # 5. the next good call
+    r = bodies("B") if rank == 1 else nothing()
+    res[5] = _keep(r, False)
+    res["idx", 5] = db.next_index()
+    res["counts"] = db.issuer_counts()
+    dist.barrier()
+    db.close()
+    dist.destroy_process_group()
+    return res
 
 
 def _part(ora, inp, k):
@@ -216,22 +197,8 @@ def _check(got, want, part, meta=False, pem=False):
 
 @pytest.mark.timeout(1200)
 def test_collective_bodies_match_sequential_oracle(ora):
-    import torch.multiprocessing as mp
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=1100)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    outs = run_ranks(_worker, world, timeout=1100)
     from ct_mapreduce_b200 import capi
     inp = inputs()
     odb = ora.DB(README_FILTER, False)

@@ -6,9 +6,6 @@ trees must be equal bit for bit.  The roots are also checked against merkle_mode
 must equal the one-ctx call, and two processes on one GPU fold each rank's own trees.  Marked gpu."""
 import base64
 import ctypes as C
-import os
-import socket
-import sys
 
 import numpy as np
 import pytest
@@ -16,7 +13,8 @@ import pytest
 import bodies_oracle as bo
 import bodyfold_model as bm
 import merkle_model as mm
-from conftest import NOW_NS, ROOT
+from conftest import NOW_NS
+from peer_ranks import run_ranks
 from test_gpu_bodies import PATH_FIELDS, RAW_FIELDS, corpus, next_idx, synth_bodies
 
 pytestmark = pytest.mark.gpu
@@ -374,76 +372,45 @@ def peer_inputs():
             1: (c, [0] * 12, [k * 10 - (5 if k >= 6 else 0) for k in range(12)])}   # body 6 refetches 5 entries
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
+def _worker(rank, world):
+    import torch
+    import torch.distributed as dist
+    torch.cuda.set_device(0)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from ct_mapreduce_b200 import capi, engine, sharded
+    db = engine.GpuCertDatabase(device=0, table_capacity=1 << 15, max_batch_entries=E, log_expired_entries=True)
+    sharded.attach_peers(db)
+    bodies, logs, starts = peer_inputs()[rank]
+    text, offs, lens = text_of(bodies)
+    res = {}
+    n_trees = max(logs) + 1
+    r = db.store_raw_bodies(text, offs, lens, [10] * len(bodies), NOW_NS, trees=[engine.LogTree() for _ in range(n_trees)],
+                            body_log=logs, body_start=starts)
+    res[1] = [(t.size, t.edge.tobytes(), t.root) for t in r.trees]
+    res["idx", 1] = db.next_index()
+    # rank 1 breaks a tree rule (its starts decrease): rank 0 returns CTMR_E_PEER_FAILED, nothing is taken
+    bad = list(starts)
+    if rank == 1:
+        bad[3] = 0
+    trees = [engine.LogTree(size=7, edge=np.full((64, 32), 9, np.uint8)) for _ in range(n_trees)]
+    code = None
     try:
-        import torch
-        import torch.distributed as dist
-        torch.cuda.set_device(0)
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        from ct_mapreduce_b200 import capi, engine, sharded
-        db = engine.GpuCertDatabase(device=0, table_capacity=1 << 15, max_batch_entries=E, log_expired_entries=True)
-        sharded.attach_peers(db)
-        bodies, logs, starts = peer_inputs()[rank]
-        text, offs, lens = text_of(bodies)
-        res = {}
-        n_trees = max(logs) + 1
-        r = db.store_raw_bodies(text, offs, lens, [10] * len(bodies), NOW_NS, trees=[engine.LogTree() for _ in range(n_trees)],
-                                body_log=logs, body_start=starts)
-        res[1] = [(t.size, t.edge.tobytes(), t.root) for t in r.trees]
-        res["idx", 1] = db.next_index()
-        # rank 1 breaks a tree rule (its starts decrease): rank 0 returns CTMR_E_PEER_FAILED, nothing is taken
-        bad = list(starts)
-        if rank == 1:
-            bad[3] = 0
-        trees = [engine.LogTree(size=7, edge=np.full((64, 32), 9, np.uint8)) for _ in range(n_trees)]
-        code = None
-        try:
-            db.store_raw_bodies(text, offs, lens, [10] * len(bodies), NOW_NS, trees=trees, body_log=logs,
-                                body_start=[s + 7 for s in bad] if rank == 0 else bad)
-        except capi.CtmrError as e:
-            code = e.code
-        res[2] = (code, db.next_index())
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        db.close()
-        dist.destroy_process_group()
-    except Exception:
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+        db.store_raw_bodies(text, offs, lens, [10] * len(bodies), NOW_NS, trees=trees, body_log=logs,
+                            body_start=[s + 7 for s in bad] if rank == 0 else bad)
+    except capi.CtmrError as e:
+        code = e.code
+    res[2] = (code, db.next_index())
+    dist.barrier()
+    db.close()
+    dist.destroy_process_group()
+    return res
 
 
 @pytest.mark.timeout(1200)
 def test_collective_two_ranks_fold_their_own_trees(eng):
-    import torch.multiprocessing as mp
     from ct_mapreduce_b200 import capi
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=1100)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    outs = run_ranks(_worker, world, timeout=1100)
     for rank in range(world):
         bodies, logs, starts = peer_inputs()[rank]
         with eng.GpuCertDatabase(table_capacity=1 << 15, max_batch_entries=E, log_expired_entries=True) as one:

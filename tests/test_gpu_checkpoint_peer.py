@@ -4,15 +4,13 @@ one-ctx checkpoint loads into two ranks.  Every continuation is compared with th
 collective index rule defines (each rank's batch fits one round: rank 0's entries, then rank 1's).  A rank that passes a
 truncated part gets CTMR_E_INVALID, the other CTMR_E_PEER_FAILED, neither changes, and the next collective call returns
 normally.  Marked gpu."""
-import os
-import socket
-import sys
 
 import numpy as np
 import pytest
 
 import checkpoint_model as CM
-from conftest import NOW_NS, README_FILTER, ROOT
+from conftest import NOW_NS, README_FILTER
+from peer_ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -39,97 +37,80 @@ def batch(c, k):
     return blob, offs[lo:hi + 1], iblob, ioffs, idx[lo:hi]
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _keep(r):
     return {f: getattr(r, f) for f in FIELDS}
 
 
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
+def _worker(rank, world):
+    import torch
+    import torch.distributed as dist
+    torch.cuda.set_device(0)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from ct_mapreduce_b200 import capi, engine, sharded
+    c = corpus()
+    iblob, ioffs = c[3], c[4]
+    res = {}
+
+    def peer_db():
+        db = engine.GpuCertDatabase(device=0, **KW)
+        sharded.attach_peers(db)
+        return db
+
+    db = peer_db()
+    if rank == 0:  # the registry in reverse order first
+        ni = ioffs.size - 1
+        ders = [iblob[ioffs[k]:ioffs[k + 1]].tobytes() for k in range(ni)][::-1]
+        ro = np.zeros(ni + 1, np.uint64)
+        ro[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
+        db.register_issuers(np.frombuffer(b"".join(ders), np.uint8), ro)
+    dist.barrier()
+    res["dense"] = db.register_issuers(iblob, ioffs)
+    res["a"] = _keep(db.store_batch(*batch(c, rank), NOW_NS))
+    part = db.checkpoint().copy()
+    assert np.array_equal(part, db.checkpoint())
+    res["next"] = db.next_index()
+    parts = [None] * world
+    dist.all_gather_object(parts, part)
+    res["parts"] = parts
+    # truncated part on rank 1: it fails, rank 0 gets CTMR_E_PEER_FAILED, nothing changes on either rank
+    before = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts(), db.next_index())
+    code = None
     try:
-        import torch
-        import torch.distributed as dist
-        torch.cuda.set_device(0)
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        from ct_mapreduce_b200 import capi, engine, sharded
-        c = corpus()
-        iblob, ioffs = c[3], c[4]
-        res = {}
-
-        def peer_db():
-            db = engine.GpuCertDatabase(device=0, **KW)
-            sharded.attach_peers(db)
-            return db
-
+        db.load_checkpoint([parts[0][:-1], parts[1]] if rank == 1 else parts)
+    except capi.CtmrError as e:
+        code = e.code
+    res["fail"] = (code, before == (db.table_stats(), db.status_counters().tolist(), db.issuer_counts(), db.next_index()))
+    r = db.store_batch(*batch(c, 2 + rank), NOW_NS)   # the next collective call returns normally (state unchanged)
+    res["after_fail"] = _keep(r)
+    db.close()
+    # the two parts into one ctx and a group of three shards (rank 0 alone), continued over both second halves
+    one = None
+    if rank == 0:
+        second = (c[0], c[1][2 * N:4 * N + 1], iblob, ioffs, c[2][2 * N:4 * N])
+        with engine.GpuCertDatabase(device=0, **dict(KW, table_capacity=1 << 14)) as t:
+            t.load_checkpoint(parts[::-1])
+            res["ctx_next"] = t.next_index()
+            res["ctx_counts"] = t.issuer_counts()
+            one = t.checkpoint().copy()
+            res["ctx_b"] = _keep(t.store_batch(*second, NOW_NS))
+        with engine.GpuCertGroup([0, 0, 0], **dict(KW, table_capacity=1 << 13)) as t:
+            t.load_checkpoint(parts)
+            res["group_counts"] = t.issuer_counts()
+            res["group_b"] = _keep(t.store_batch(*second, NOW_NS))
+    ones = [None] * world
+    dist.all_gather_object(ones, one)
+    # the two parts, then the one-ctx checkpoint, into two ranks again; each continued collectively
+    for name, ck in (("peer2", parts[::-1]), ("peer1", [ones[0]])):
         db = peer_db()
-        if rank == 0:  # the registry in reverse order first
-            ni = ioffs.size - 1
-            ders = [iblob[ioffs[k]:ioffs[k + 1]].tobytes() for k in range(ni)][::-1]
-            ro = np.zeros(ni + 1, np.uint64)
-            ro[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
-            db.register_issuers(np.frombuffer(b"".join(ders), np.uint8), ro)
-        dist.barrier()
-        res["dense"] = db.register_issuers(iblob, ioffs)
-        res["a"] = _keep(db.store_batch(*batch(c, rank), NOW_NS))
-        part = db.checkpoint().copy()
-        assert np.array_equal(part, db.checkpoint())
-        res["next"] = db.next_index()
-        parts = [None] * world
-        dist.all_gather_object(parts, part)
-        res["parts"] = parts
-        # truncated part on rank 1: it fails, rank 0 gets CTMR_E_PEER_FAILED, nothing changes on either rank
-        before = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts(), db.next_index())
-        code = None
-        try:
-            db.load_checkpoint([parts[0][:-1], parts[1]] if rank == 1 else parts)
-        except capi.CtmrError as e:
-            code = e.code
-        res["fail"] = (code, before == (db.table_stats(), db.status_counters().tolist(), db.issuer_counts(), db.next_index()))
-        r = db.store_batch(*batch(c, 2 + rank), NOW_NS)   # the next collective call returns normally (state unchanged)
-        res["after_fail"] = _keep(r)
+        db.load_checkpoint(ck)
+        res[name + "_next"] = db.next_index()
+        res[name + "_counts"] = db.issuer_counts()
+        res[name + "_status"] = db.status_counters()
+        res[name + "_b"] = _keep(db.store_batch(*batch(c, 2 + rank), NOW_NS))
         db.close()
-        # the two parts into one ctx and a group of three shards (rank 0 alone), continued over both second halves
-        one = None
-        if rank == 0:
-            second = (c[0], c[1][2 * N:4 * N + 1], iblob, ioffs, c[2][2 * N:4 * N])
-            with engine.GpuCertDatabase(device=0, **dict(KW, table_capacity=1 << 14)) as t:
-                t.load_checkpoint(parts[::-1])
-                res["ctx_next"] = t.next_index()
-                res["ctx_counts"] = t.issuer_counts()
-                one = t.checkpoint().copy()
-                res["ctx_b"] = _keep(t.store_batch(*second, NOW_NS))
-            with engine.GpuCertGroup([0, 0, 0], **dict(KW, table_capacity=1 << 13)) as t:
-                t.load_checkpoint(parts)
-                res["group_counts"] = t.issuer_counts()
-                res["group_b"] = _keep(t.store_batch(*second, NOW_NS))
-        ones = [None] * world
-        dist.all_gather_object(ones, one)
-        # the two parts, then the one-ctx checkpoint, into two ranks again; each continued collectively
-        for name, ck in (("peer2", parts[::-1]), ("peer1", [ones[0]])):
-            db = peer_db()
-            db.load_checkpoint(ck)
-            res[name + "_next"] = db.next_index()
-            res[name + "_counts"] = db.issuer_counts()
-            res[name + "_status"] = db.status_counters()
-            res[name + "_b"] = _keep(db.store_batch(*batch(c, 2 + rank), NOW_NS))
-            db.close()
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        dist.destroy_process_group()
-    except Exception:  # surface the failure instead of a silent hang of the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+    dist.barrier()
+    dist.destroy_process_group()
+    return res
 
 
 def _same(got, want, lo, hi):
@@ -141,24 +122,10 @@ def _same(got, want, lo, hi):
 
 @pytest.mark.timeout(1200)
 def test_collective_checkpoint_moves_between_shapes(ora):
-    import torch.multiprocessing as mp
     from ct_mapreduce_b200 import build, capi
     build.build()
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=1100)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    outs = run_ranks(_worker, world, timeout=1100)
     blob, offs, idx, iblob, ioffs = corpus()
     odb = ora.DB(README_FILTER, False)
     wa = odb.process(blob, offs[:2 * N + 1], iblob, ioffs, idx[:2 * N], NOW_NS)  # rank 0's first half, then rank 1's

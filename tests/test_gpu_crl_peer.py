@@ -4,9 +4,6 @@ joins its own CRLs in collective calls.  Every output of every rank must equal c
 that loads both ranks' checkpoint parts and runs the same rank's CRLs, and must pass the crl_oracle checks over the union
 of the sets.  Also covered: round and chunk edges with 512 records per round, the read-only property, each failure rule
 and the next call after it, and one rank joining a 2 M-entry CRL while the other joins 10,000 small CRLs.  Marked gpu."""
-import os
-import socket
-import sys
 
 import numpy as np
 import pytest
@@ -14,7 +11,8 @@ import pytest
 import crl_build as cb
 import crl_oracle as co
 import xchg_model as XM
-from conftest import NOW_NS, ROOT
+from conftest import NOW_NS
+from peer_ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -117,14 +115,6 @@ def capped(cases_, need0):
     return ("cap_short", (a[0], a[1], need0 - 1), b)
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _join(db, crls, digs, cap):
     """{code, n_entries, every output array} of one call"""
     from ct_mapreduce_b200 import capi
@@ -141,116 +131,107 @@ def _state(db):
     return (db.checkpoint().tobytes(), db.next_index(), db.status_counters().tolist(), db.issuer_counts(), db.table_stats())
 
 
-def _worker(rank, world, port, q, same_gpu):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    try:
-        import torch
-        import torch.distributed as dist
-        dev = 0 if same_gpu else rank
-        torch.cuda.set_device(dev)
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        from ct_mapreduce_b200 import capi, engine, sharded
-        c = corpus()
-        res = {}
-        db = engine.GpuCertDatabase(device=dev, **KW)
-        sharded.attach_peers(db)
-        dense = db.register_issuers(c[3], c[4])
-        dig = [db.issuer_digest(int(d)) for d in dense]
-        x = None
-        if rank == 0:  # an issuer only rank 0 registers
-            der = np.frombuffer(XM.ca(3).der, np.uint8)
-            xd = int(db.register_issuers(der, np.array([0, der.size], np.uint64))[0])
-            x = (xd, db.issuer_digest(xd))
-        xs = [None] * world
-        dist.all_gather_object(xs, x)
-        x_dense, x_dig = xs[0]
-        db.store_batch(*part(c, rank * H, (rank + 1) * H), NOW_NS)
-        for owner, hour, d, serials in crafted(dense, dig, x_dense, x_dig):
-            if owner == rank:
-                db.preload_known(hour, d, serials)
-        dist.barrier()
-        sets = corpus_sets(c, dig)
-        cs = cases(dig, x_dig, sets)
-        res["parts"] = db.checkpoint().copy()
-        res["dig"], res["x_dig"] = dig, x_dig
-        before = _state(db)
-        res["calls"] = {}
-        for name, a, b in cs:
-            crls, digs, cap = (a, b)[rank]
-            res["calls"][name] = _join(db, crls, digs, cap)
-        res["read_only"] = _state(db) == before
-        need0 = [None] * world
-        dist.all_gather_object(need0, res["calls"]["mix"]["n_entries"])
-        name, a, b = capped(cs, need0[0])
-        res["calls"][name] = _join(db, *(a, b)[rank])
-        # failures, each followed by the mix again: a CRL outside data, a CRL above the staging budget, and a digest count
-        # the binding refuses (the call is made anyway, with no batch)
-        mix = cs[0][1 + rank]
-        data, offs, lens = engine.pack_crls(mix[0])
-        fails = {
-            "outside": ((data, offs, lens + np.uint64(1) * (np.arange(lens.size) == lens.size - 1)), mix[1]),
-            "too_large": ([cb.crl(entries=[cb.entry(bytes([1, i >> 8, i & 255]), 1767000000) for i in range(7000)])], [dig[0]]),
-            "refused": (mix[0], mix[1][:-1]),
-        }
-        res["fail"] = {}
-        for fname, (crls, digs) in fails.items():
-            got = None
-            if rank == 1:
-                try:
-                    db.revoked_known(crls, digs)
-                except capi.CtmrError as ex:
-                    got = (ex.code, ex.n_entries)
-                except ValueError:
-                    got = ("ValueError", None)
-            else:
-                got = _join(db, *mix)
-                got = (got["code"], got["n_entries"])
-            res["fail"][fname] = (got, _join(db, *mix))
-        after = db.store_batch(*part(c, 2 * H + rank * TAIL, 2 * H + (rank + 1) * TAIL), NOW_NS)
-        res["after"] = {f: getattr(after, f) for f in ("status", "was_unknown", "first_issuer_hour")}
-        db.close()
-        # scale: a 2 M-entry CRL on rank 0, 10,000 small CRLs on rank 1, hits seeded in sets of both ranks' shards
-        db = engine.GpuCertDatabase(device=dev, **SCALE_KW)
-        sharded.attach_peers(db)
-        dense = db.register_issuers(c[3], c[4])
-        dig = [db.issuer_digest(int(d)) for d in dense]
-        rng = np.random.default_rng(11)
-        rows = rng.integers(0, 256, (SCALE_N, 16), dtype=np.uint8)
-        rows[:, 0] = rng.integers(1, 0x80, SCALE_N, dtype=np.uint8)
-        seeded = list(range(0, SCALE_N, SCALE_STRIDE))
-        i2 = int(dense[2])
-        small_seed = [7, 1234, 5555, 9999]
-        for j, pos in enumerate(seeded):  # alternate owners
-            owner = j & 1
-            if owner == rank:
-                db.preload_known(XM.hour_for(i2, 2, owner, FAR + j), dig[2], [rows[pos].tobytes()])
-        small_serial = lambda i: bytes([1 + i % 100, i >> 8 & 0x7F])  # noqa: E731
-        for j, i in enumerate(small_seed):
-            owner = j & 1
-            if owner == rank:
-                ii = int(dense[i % 3])
-                db.preload_known(XM.hour_for(ii, 2, owner, FAR + j), dig[i % 3], [small_serial(i)])
-        dist.barrier()
-        if rank == 0:
-            r = db.revoked_known([cb.bulk_crl(rows)], [dig[2]])
-            res["scale"] = (int(r.crl_status[0]), r.n_entries, sorted(np.nonzero(r.known)[0].tolist()), seeded)
+def _worker(rank, world, same_gpu):
+    import torch
+    import torch.distributed as dist
+    dev = 0 if same_gpu else rank
+    torch.cuda.set_device(dev)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from ct_mapreduce_b200 import capi, engine, sharded
+    c = corpus()
+    res = {}
+    db = engine.GpuCertDatabase(device=dev, **KW)
+    sharded.attach_peers(db)
+    dense = db.register_issuers(c[3], c[4])
+    dig = [db.issuer_digest(int(d)) for d in dense]
+    x = None
+    if rank == 0:  # an issuer only rank 0 registers
+        der = np.frombuffer(XM.ca(3).der, np.uint8)
+        xd = int(db.register_issuers(der, np.array([0, der.size], np.uint64))[0])
+        x = (xd, db.issuer_digest(xd))
+    xs = [None] * world
+    dist.all_gather_object(xs, x)
+    x_dense, x_dig = xs[0]
+    db.store_batch(*part(c, rank * H, (rank + 1) * H), NOW_NS)
+    for owner, hour, d, serials in crafted(dense, dig, x_dense, x_dig):
+        if owner == rank:
+            db.preload_known(hour, d, serials)
+    dist.barrier()
+    sets = corpus_sets(c, dig)
+    cs = cases(dig, x_dig, sets)
+    res["parts"] = db.checkpoint().copy()
+    res["dig"], res["x_dig"] = dig, x_dig
+    before = _state(db)
+    res["calls"] = {}
+    for name, a, b in cs:
+        crls, digs, cap = (a, b)[rank]
+        res["calls"][name] = _join(db, crls, digs, cap)
+    res["read_only"] = _state(db) == before
+    need0 = [None] * world
+    dist.all_gather_object(need0, res["calls"]["mix"]["n_entries"])
+    name, a, b = capped(cs, need0[0])
+    res["calls"][name] = _join(db, *(a, b)[rank])
+    # failures, each followed by the mix again: a CRL outside data, a CRL above the staging budget, and a digest count
+    # the binding refuses (the call is made anyway, with no batch)
+    mix = cs[0][1 + rank]
+    data, offs, lens = engine.pack_crls(mix[0])
+    fails = {
+        "outside": ((data, offs, lens + np.uint64(1) * (np.arange(lens.size) == lens.size - 1)), mix[1]),
+        "too_large": ([cb.crl(entries=[cb.entry(bytes([1, i >> 8, i & 255]), 1767000000) for i in range(7000)])], [dig[0]]),
+        "refused": (mix[0], mix[1][:-1]),
+    }
+    res["fail"] = {}
+    for fname, (crls, digs) in fails.items():
+        got = None
+        if rank == 1:
+            try:
+                db.revoked_known(crls, digs)
+            except capi.CtmrError as ex:
+                got = (ex.code, ex.n_entries)
+            except ValueError:
+                got = ("ValueError", None)
         else:
-            small = [cb.crl(entries=[cb.entry(small_serial(i), 1767000000)]) for i in range(10_000)]
-            r = db.revoked_known(small, [dig[i % 3] for i in range(10_000)])
-            res["scale"] = (bool((r.crl_status == co.CRL_OK).all()), r.n_entries, sorted(np.nonzero(r.known)[0].tolist()), small_seed)
-        db.close()
-        if rank == 0:
-            res["cases"] = cs + [capped(cs, need0[0])]
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        dist.destroy_process_group()
-    except Exception:  # surface the failure instead of a silent hang of the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+            got = _join(db, *mix)
+            got = (got["code"], got["n_entries"])
+        res["fail"][fname] = (got, _join(db, *mix))
+    after = db.store_batch(*part(c, 2 * H + rank * TAIL, 2 * H + (rank + 1) * TAIL), NOW_NS)
+    res["after"] = {f: getattr(after, f) for f in ("status", "was_unknown", "first_issuer_hour")}
+    db.close()
+    # scale: a 2 M-entry CRL on rank 0, 10,000 small CRLs on rank 1, hits seeded in sets of both ranks' shards
+    db = engine.GpuCertDatabase(device=dev, **SCALE_KW)
+    sharded.attach_peers(db)
+    dense = db.register_issuers(c[3], c[4])
+    dig = [db.issuer_digest(int(d)) for d in dense]
+    rng = np.random.default_rng(11)
+    rows = rng.integers(0, 256, (SCALE_N, 16), dtype=np.uint8)
+    rows[:, 0] = rng.integers(1, 0x80, SCALE_N, dtype=np.uint8)
+    seeded = list(range(0, SCALE_N, SCALE_STRIDE))
+    i2 = int(dense[2])
+    small_seed = [7, 1234, 5555, 9999]
+    for j, pos in enumerate(seeded):  # alternate owners
+        owner = j & 1
+        if owner == rank:
+            db.preload_known(XM.hour_for(i2, 2, owner, FAR + j), dig[2], [rows[pos].tobytes()])
+    small_serial = lambda i: bytes([1 + i % 100, i >> 8 & 0x7F])  # noqa: E731
+    for j, i in enumerate(small_seed):
+        owner = j & 1
+        if owner == rank:
+            ii = int(dense[i % 3])
+            db.preload_known(XM.hour_for(ii, 2, owner, FAR + j), dig[i % 3], [small_serial(i)])
+    dist.barrier()
+    if rank == 0:
+        r = db.revoked_known([cb.bulk_crl(rows)], [dig[2]])
+        res["scale"] = (int(r.crl_status[0]), r.n_entries, sorted(np.nonzero(r.known)[0].tolist()), seeded)
+    else:
+        small = [cb.crl(entries=[cb.entry(small_serial(i), 1767000000)]) for i in range(10_000)]
+        r = db.revoked_known(small, [dig[i % 3] for i in range(10_000)])
+        res["scale"] = (bool((r.crl_status == co.CRL_OK).all()), r.n_entries, sorted(np.nonzero(r.known)[0].tolist()), small_seed)
+    db.close()
+    if rank == 0:
+        res["cases"] = cs + [capped(cs, need0[0])]
+    dist.barrier()
+    dist.destroy_process_group()
+    return res
 
 
 def _oracle_check(got, crls, digs, sets, registered):
@@ -277,25 +258,10 @@ def _oracle_check(got, crls, digs, sets, registered):
 
 
 def _run(same_gpu):
-    import torch.multiprocessing as mp
     from ct_mapreduce_b200 import build
     build.build()
     world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q, same_gpu)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=1700)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
-    return outs
+    return run_ranks(_worker, world, (same_gpu,), timeout=1700)
 
 
 @pytest.mark.timeout(1800)

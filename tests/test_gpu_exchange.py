@@ -13,7 +13,6 @@ the cardinality of every set, and the group's sums.
 The last test runs the collective ctmr_process_device in two processes on one GPU, with rounds of exactly X entries and
 a refusal one entry above."""
 import os
-import sys
 
 import numpy as np
 import pytest
@@ -22,7 +21,8 @@ import der_build as D
 import keymodel as K
 import metamodel as M
 import xchg_model as X
-from conftest import NOW_NS, ROOT, pack
+from conftest import NOW_NS, pack
+from peer_ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -410,98 +410,70 @@ def _peer_corpus(rank, n, m):
     return out
 
 
-def _peer_worker(rank, world, port, n, n_big, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      CTMR_PEER_TIMEOUT_MS="20000")
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
+def _peer_worker(rank, world, n, n_big):
+    os.environ["CTMR_PEER_TIMEOUT_MS"] = "20000"
+    import torch
+    import torch.distributed as dist
+    torch.cuda.set_device(0)
+    dev = torch.device("cuda", 0)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from ct_mapreduce_b200 import capi, engine, sharded
+    assert capi.peer_rounds() == 8 and sharded.round_entries(n) == X_ENTRIES and sharded.round_entries(n_big) == X_ENTRIES + 1
+    iblob, ioffs = pack(X.issuers())
+    db = engine.GpuCertDatabase(device=0, table_capacity=1 << 13, issuer_cn_filter=X.CN_FILTER, max_issuers=64,
+                                max_batch_entries=STAGE, max_round_entries=X_ENTRIES, pair_capacity_log2=PAIR_LOG2,
+                                meta_capacity_log2=META_LOG2)
+    sharded.attach_peers(db)
+    dense = db.register_issuers(iblob, ioffs)
+    es = _peer_corpus(rank, n, n_big)
+    blob, offs = pack([e[0] for e in es])
+    dblob = torch.from_numpy(np.concatenate([blob, np.zeros(64, np.uint8)])).to(dev)
+    doffs = torch.from_numpy(offs.astype(np.int64)).to(dev)
+    didx = torch.from_numpy(np.array([dense[e[1]] for e in es], np.int32)).to(dev)
+    t = {k: torch.zeros((n_big,) + sh, dtype=dt, device=dev) for k, sh, dt in (
+        ("status", (), torch.uint8), ("sha", (32,), torch.uint8), ("exp_hour", (), torch.int64), ("wu", (), torch.uint8),
+        ("fi", (), torch.uint8))}
+    o = capi.DevOut(t["status"].data_ptr(), t["sha"].data_ptr(), t["exp_hour"].data_ptr(), None, None, t["wu"].data_ptr(),
+                    t["fi"].data_ptr(), None)
+
+    def batch(m):
+        b = capi.DevBatch()
+        b.blob, b.blob_bytes, b.offsets, b.n = dblob.data_ptr(), int(offs[m]), doffs.data_ptr(), m
+        b.issuer_idx, b.issuer_map, b.issuer_map_len = didx.data_ptr(), None, 0
+        b.first_index, b.now_unix_ns = 0, NOW_NS
+        return b
+
+    torch.cuda.synchronize(dev)
+    dist.barrier()
+    db.process_device(batch(n), o)
+    torch.cuda.synchronize(dev)
+    db.check_device()
+    res = {k: v[:n].cpu().numpy() for k, v in t.items()}
+    res["counts"] = db.issuer_counts()
+    res["status_counts"] = db.status_counters()
+    res["used"] = db.table_stats()[0]
+    dist.barrier()
+    # one entry more per round than the regions hold: both ranks refuse before any barrier, nothing changes
     try:
-        import torch
-        import torch.distributed as dist
-        torch.cuda.set_device(0)
-        dev = torch.device("cuda", 0)
-        dist.init_process_group("gloo", rank=rank, world_size=world)
-        from ct_mapreduce_b200 import capi, engine, sharded
-        assert capi.peer_rounds() == 8 and sharded.round_entries(n) == X_ENTRIES and sharded.round_entries(n_big) == X_ENTRIES + 1
-        iblob, ioffs = pack(X.issuers())
-        db = engine.GpuCertDatabase(device=0, table_capacity=1 << 13, issuer_cn_filter=X.CN_FILTER, max_issuers=64,
-                                    max_batch_entries=STAGE, max_round_entries=X_ENTRIES, pair_capacity_log2=PAIR_LOG2,
-                                    meta_capacity_log2=META_LOG2)
-        sharded.attach_peers(db)
-        dense = db.register_issuers(iblob, ioffs)
-        es = _peer_corpus(rank, n, n_big)
-        blob, offs = pack([e[0] for e in es])
-        dblob = torch.from_numpy(np.concatenate([blob, np.zeros(64, np.uint8)])).to(dev)
-        doffs = torch.from_numpy(offs.astype(np.int64)).to(dev)
-        didx = torch.from_numpy(np.array([dense[e[1]] for e in es], np.int32)).to(dev)
-        t = {k: torch.zeros((n_big,) + sh, dtype=dt, device=dev) for k, sh, dt in (
-            ("status", (), torch.uint8), ("sha", (32,), torch.uint8), ("exp_hour", (), torch.int64), ("wu", (), torch.uint8),
-            ("fi", (), torch.uint8))}
-        o = capi.DevOut(t["status"].data_ptr(), t["sha"].data_ptr(), t["exp_hour"].data_ptr(), None, None, t["wu"].data_ptr(),
-                        t["fi"].data_ptr(), None)
-
-        def batch(m):
-            b = capi.DevBatch()
-            b.blob, b.blob_bytes, b.offsets, b.n = dblob.data_ptr(), int(offs[m]), doffs.data_ptr(), m
-            b.issuer_idx, b.issuer_map, b.issuer_map_len = didx.data_ptr(), None, 0
-            b.first_index, b.now_unix_ns = 0, NOW_NS
-            return b
-
-        torch.cuda.synchronize(dev)
-        dist.barrier()
-        db.process_device(batch(n), o)
-        torch.cuda.synchronize(dev)
-        db.check_device()
-        res = {k: v[:n].cpu().numpy() for k, v in t.items()}
-        res["counts"] = db.issuer_counts()
-        res["status_counts"] = db.status_counters()
-        res["used"] = db.table_stats()[0]
-        dist.barrier()
-        # one entry more per round than the regions hold: both ranks refuse before any barrier, nothing changes
-        try:
-            db.process_device(batch(n_big), o)
-            res["refused"] = None
-        except capi.CtmrError as e:
-            res["refused"] = e.code
-        torch.cuda.synchronize(dev)
-        res["after"] = (db.issuer_counts(), db.status_counters(), db.table_stats()[0])
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        db.close()
-        dist.destroy_process_group()
-    except Exception:
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+        db.process_device(batch(n_big), o)
+        res["refused"] = None
+    except capi.CtmrError as e:
+        res["refused"] = e.code
+    torch.cuda.synchronize(dev)
+    res["after"] = (db.issuer_counts(), db.status_counters(), db.table_stats()[0])
+    dist.barrier()
+    db.close()
+    dist.destroy_process_group()
+    return res
 
 
 @pytest.mark.timeout(600)
 def test_collective_device_call_rounds_of_exactly_x(ora):
-    import socket
-
-    import torch.multiprocessing as mp
     from ct_mapreduce_b200 import capi, sharded
     world = 2
     n = next(m for m in range(1, 4000) if X.device_round_entries(m, 8) == X_ENTRIES)
     n_big = next(m for m in range(n, 4000) if X.device_round_entries(m, 8) == X_ENTRIES + 1)
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_peer_worker, args=(r, world, port, n, n_big, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=500)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    outs = run_ranks(_peer_worker, world, (n, n_big), timeout=500)
     # the oracle over the order the collective call defines
     shard = [_peer_corpus(r, n, n) for r in range(world)]
     slices = list(sharded.sequential_order(n, world, 8))

@@ -5,14 +5,12 @@ and one rank per GPU over NCCL when the box has two or more.  Every output of ev
 the oracle run SEQUENTIALLY over the order the collective calls define (sharded.frontend_indices), the front-end fields
 with oracle.raw_process / tiles_oracle, the merged histogram and the per-rank counts with the oracle's.  Marked gpu."""
 import base64
-import os
-import socket
-import sys
 
 import numpy as np
 import pytest
 
-from conftest import NOW_NS, README_FILTER, ROOT
+from conftest import NOW_NS, README_FILTER
+from peer_ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -71,14 +69,6 @@ class Inputs:
         return text, lo[sl].copy(), ll[sl].copy(), xo[sl].copy(), xl[sl].copy()
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _keep(r, fields):
     return {f: getattr(r, f) for f in fields if getattr(r, f, None) is not None}
 
@@ -95,146 +85,137 @@ def _frontend(r):
     return _keep(r, ("entry_status", "entry_type", "tiles_done", "leaf_hash"))
 
 
-def _worker(rank, world, port, backend, same_gpu, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
+def _worker(rank, world, backend, same_gpu):
+    import torch
+    import torch.distributed as dist
+    devno = 0 if same_gpu else rank
+    torch.cuda.set_device(devno)
+    dev = torch.device("cuda", devno)
+    if backend == "nccl":
+        dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
+    else:
+        dist.init_process_group("gloo", rank=rank, world_size=world)
+    from conftest import pack
+    from ct_mapreduce_b200 import capi, engine, sharded
+    from oracle import oracle as ora
+    inp = Inputs(ora)
+    kw = dict(device=devno, table_capacity=1 << 16, issuer_cn_filter=README_FILTER, max_issuers=1024, max_batch_entries=E)
+    db = engine.GpuCertDatabase(**kw)
+    sharded.attach_peers(db)
+    # every rank registers its own chain certificates (the registry behind them is the group's)
+    def register(k):
+        db.register_chain_certs(*pack([inp.tiles[k].by_fp[fp] for fp in inp.known(k)]))
+
+    for k in {0: ["T3"], 1: ["T1", "T2", "T5"]}.get(rank, []):   # T4's own issuers come later: they hold T2's missing one
+        register(k)
+    z64, z32 = np.zeros(0, np.uint64), np.zeros(0, np.uint32)
+    empty_pages = (b"x", z64, z32, z64, z32)
+    res = {("idx", 0): db.next_index()}
+    dist.barrier()
+
+    def pages(k, sl=slice(None), **a):
+        return db.store_raw_entries(*inp.page_args(k, sl), NOW_NS, **a)
+
+    def tiles(k, sl=slice(None), **a):
+        return db.store_tiles(*inp.tiles[k].args(sl), NOW_NS, **a)
+
+    def fetch_of(k):
+        return lambda fps: [inp.tiles[k].by_fp[fp] for fp in fps]
+
+    # 1. ragged: rank 0 has six chunks, every other rank none.  String identities are computed only by calls that
+    # want them (as on one GPU), and the oracle computes them always: every call up to the last one that compares
+    # them asks for them on some rank.
+    r = pages("A", want_meta=True) if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
+    res[1] = (_path(r), _frontend(r))
+    res["idx", 1] = db.next_index()
+    # 2. certificates nothing earlier has seen, on every rank: twins across ranks and rounds, rank 1's in another order;
+    # PEM on rank 0, string identities on rank 1 only
+    r = pages("C", TWIN_ORDER if rank == 1 else slice(None), want_pem=rank == 0, want_meta=rank == 1)
+    res[2] = (_path(r, pem=rank == 0), _frontend(r))
+    res["idx", 2] = db.next_index()
+    # 3. pages on rank 0 (with string identities), tiles on rank 1
+    if rank == 1:
+        r = tiles("T1", want_leaf_hash=True)
+    else:
+        r = pages("D", want_meta=rank == 0) if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
+    res[3] = (_path(r), _frontend(r))
+    res["idx", 3] = db.next_index()
+    # 4. a stop on rank 1: every rank learns of it; 5. the resume, the other ranks with empty batches
+    r = tiles("T2") if rank == 1 else (pages("E") if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS))
+    res[4] = (_path(r), _frontend(r), db.peer_frontend_stopped(), getattr(r, "missing", None))
+    res["idx", 4] = db.next_index()
+    if rank == 1:
+        done = r.tiles_done
+        db.register_chain_certs(*pack([inp.tiles["T2"].by_fp[fp] for fp in r.missing]))
+        r = tiles("T2", slice(done, None))
+    else:
+        r = db.store_raw_entries(*empty_pages, NOW_NS)
+    res[5] = (_path(r), _frontend(r), db.peer_frontend_stopped())
+    res["idx", 5] = db.next_index()
+    if rank == 1:
+        register("T4")
+    # 6. the engine's fetch loop on every rank: rank 1 stops, fetches and resumes; the others join with nothing left
+    if rank in (0, 1):
+        r = tiles("T3" if rank == 0 else "T4", fetch=fetch_of("T3" if rank == 0 else "T4"))
+    else:
+        r = db.store_tiles(b"", z64, z32, z64, np.zeros(0, np.uint16), NOW_NS, fetch=lambda fps: [])
+    res[6] = (_path(r), _frontend(r), db.peer_frontend_stopped())
+    res["idx", 6] = db.next_index()
+    # 7. trees: two logs through ctmr_process_raw_trees on rank 0, one log through ctmr_process_tiles_tree on rank 1
+    log_f = (np.arange(PAGES["F"][0]) // 100 % 2).astype(np.uint32)
+    if rank == 0:
+        r = pages("F", trees=[engine.LogTree(), engine.LogTree()], entry_log=log_f)
+        trees = [(t.size, t.edge.tobytes(), t.root) for t in r.trees]
+    elif rank == 1:
+        r = tiles("T5", tree=engine.LogTree())
+        trees = [(r.tree.size, r.tree.edge.tobytes(), r.tree.root)]
+    else:
+        r, trees = db.store_raw_entries(*empty_pages, NOW_NS), []
+    res[7] = (_path(r), _frontend(r), trees)
+    res["idx", 7] = db.next_index()
+    # 8. rank 1 passes a span outside its text: it fails, every other rank returns CTMR_E_PEER_FAILED, nothing changes
+    before = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts())
+    codes = None
     try:
-        import torch
-        import torch.distributed as dist
-        devno = 0 if same_gpu else rank
-        torch.cuda.set_device(devno)
-        dev = torch.device("cuda", devno)
-        if backend == "nccl":
-            dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
-        else:
-            dist.init_process_group("gloo", rank=rank, world_size=world)
-        from conftest import pack
-        from ct_mapreduce_b200 import capi, engine, sharded
-        from oracle import oracle as ora
-        inp = Inputs(ora)
-        kw = dict(device=devno, table_capacity=1 << 16, issuer_cn_filter=README_FILTER, max_issuers=1024, max_batch_entries=E)
-        db = engine.GpuCertDatabase(**kw)
-        sharded.attach_peers(db)
-        # every rank registers its own chain certificates (the registry behind them is the group's)
-        def register(k):
-            db.register_chain_certs(*pack([inp.tiles[k].by_fp[fp] for fp in inp.known(k)]))
-
-        for k in {0: ["T3"], 1: ["T1", "T2", "T5"]}.get(rank, []):   # T4's own issuers come later: they hold T2's missing one
-            register(k)
-        z64, z32 = np.zeros(0, np.uint64), np.zeros(0, np.uint32)
-        empty_pages = (b"x", z64, z32, z64, z32)
-        res = {("idx", 0): db.next_index()}
-        dist.barrier()
-
-        def pages(k, sl=slice(None), **a):
-            return db.store_raw_entries(*inp.page_args(k, sl), NOW_NS, **a)
-
-        def tiles(k, sl=slice(None), **a):
-            return db.store_tiles(*inp.tiles[k].args(sl), NOW_NS, **a)
-
-        def fetch_of(k):
-            return lambda fps: [inp.tiles[k].by_fp[fp] for fp in fps]
-
-        # 1. ragged: rank 0 has six chunks, every other rank none.  String identities are computed only by calls that
-        # want them (as on one GPU), and the oracle computes them always: every call up to the last one that compares
-        # them asks for them on some rank.
-        r = pages("A", want_meta=True) if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
-        res[1] = (_path(r), _frontend(r))
-        res["idx", 1] = db.next_index()
-        # 2. certificates nothing earlier has seen, on every rank: twins across ranks and rounds, rank 1's in another order;
-        # PEM on rank 0, string identities on rank 1 only
-        r = pages("C", TWIN_ORDER if rank == 1 else slice(None), want_pem=rank == 0, want_meta=rank == 1)
-        res[2] = (_path(r, pem=rank == 0), _frontend(r))
-        res["idx", 2] = db.next_index()
-        # 3. pages on rank 0 (with string identities), tiles on rank 1
         if rank == 1:
-            r = tiles("T1", want_leaf_hash=True)
+            text, lo, ll, xo, xl = inp.page_args("G")
+            lo = lo.copy()
+            lo[-1] = len(text)
+            db.store_raw_entries(text, lo, ll, xo, xl, NOW_NS)
         else:
-            r = pages("D", want_meta=rank == 0) if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
-        res[3] = (_path(r), _frontend(r))
-        res["idx", 3] = db.next_index()
-        # 4. a stop on rank 1: every rank learns of it; 5. the resume, the other ranks with empty batches
-        r = tiles("T2") if rank == 1 else (pages("E") if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS))
-        res[4] = (_path(r), _frontend(r), db.peer_frontend_stopped(), getattr(r, "missing", None))
-        res["idx", 4] = db.next_index()
-        if rank == 1:
-            done = r.tiles_done
-            db.register_chain_certs(*pack([inp.tiles["T2"].by_fp[fp] for fp in r.missing]))
-            r = tiles("T2", slice(done, None))
-        else:
-            r = db.store_raw_entries(*empty_pages, NOW_NS)
-        res[5] = (_path(r), _frontend(r), db.peer_frontend_stopped())
-        res["idx", 5] = db.next_index()
-        if rank == 1:
-            register("T4")
-        # 6. the engine's fetch loop on every rank: rank 1 stops, fetches and resumes; the others join with nothing left
-        if rank in (0, 1):
-            r = tiles("T3" if rank == 0 else "T4", fetch=fetch_of("T3" if rank == 0 else "T4"))
-        else:
-            r = db.store_tiles(b"", z64, z32, z64, np.zeros(0, np.uint16), NOW_NS, fetch=lambda fps: [])
-        res[6] = (_path(r), _frontend(r), db.peer_frontend_stopped())
-        res["idx", 6] = db.next_index()
-        # 7. trees: two logs through ctmr_process_raw_trees on rank 0, one log through ctmr_process_tiles_tree on rank 1
-        log_f = (np.arange(PAGES["F"][0]) // 100 % 2).astype(np.uint32)
+            pages("G") if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
+    except capi.CtmrError as e:
+        codes = e.code
+    after = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts())
+    res[8] = (codes, before == after, db.peer_frontend_stopped())
+    res["idx", 8] = db.next_index()
+    # 9. the next good call
+    r = pages("G") if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
+    res[9] = (_path(r), _frontend(r))
+    res["idx", 9] = db.next_index()
+    # the merged histogram and this rank's own counts
+    ni = 1024
+    counts = torch.zeros(ni, dtype=torch.int64, device=dev)
+    stat = torch.zeros(capi.ST_COUNT, dtype=torch.int64, device=dev)
+    db.peer_allreduce_histogram_device(counts, ni, stat)
+    torch.cuda.synchronize(dev)
+    db.check_device()
+    res["hist"] = (counts.cpu().numpy(), stat.cpu().numpy())
+    res["counts"] = db.issuer_counts()
+    dist.barrier()
+    # the tree calls on one GPU, same batches (a plain ctx of its own)
+    with engine.GpuCertDatabase(**kw) as one:
         if rank == 0:
-            r = pages("F", trees=[engine.LogTree(), engine.LogTree()], entry_log=log_f)
-            trees = [(t.size, t.edge.tobytes(), t.root) for t in r.trees]
+            r1 = one.store_raw_entries(*inp.page_args("F"), NOW_NS, trees=[engine.LogTree(), engine.LogTree()], entry_log=log_f)
+            res["one_trees"] = [(t.size, t.edge.tobytes(), t.root) for t in r1.trees]
         elif rank == 1:
-            r = tiles("T5", tree=engine.LogTree())
-            trees = [(r.tree.size, r.tree.edge.tobytes(), r.tree.root)]
-        else:
-            r, trees = db.store_raw_entries(*empty_pages, NOW_NS), []
-        res[7] = (_path(r), _frontend(r), trees)
-        res["idx", 7] = db.next_index()
-        # 8. rank 1 passes a span outside its text: it fails, every other rank returns CTMR_E_PEER_FAILED, nothing changes
-        before = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts())
-        codes = None
-        try:
-            if rank == 1:
-                text, lo, ll, xo, xl = inp.page_args("G")
-                lo = lo.copy()
-                lo[-1] = len(text)
-                db.store_raw_entries(text, lo, ll, xo, xl, NOW_NS)
-            else:
-                pages("G") if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
-        except capi.CtmrError as e:
-            codes = e.code
-        after = (db.table_stats(), db.status_counters().tolist(), db.issuer_counts())
-        res[8] = (codes, before == after, db.peer_frontend_stopped())
-        res["idx", 8] = db.next_index()
-        # 9. the next good call
-        r = pages("G") if rank == 0 else db.store_raw_entries(*empty_pages, NOW_NS)
-        res[9] = (_path(r), _frontend(r))
-        res["idx", 9] = db.next_index()
-        # the merged histogram and this rank's own counts
-        ni = 1024
-        counts = torch.zeros(ni, dtype=torch.int64, device=dev)
-        stat = torch.zeros(capi.ST_COUNT, dtype=torch.int64, device=dev)
-        db.peer_allreduce_histogram_device(counts, ni, stat)
-        torch.cuda.synchronize(dev)
-        db.check_device()
-        res["hist"] = (counts.cpu().numpy(), stat.cpu().numpy())
-        res["counts"] = db.issuer_counts()
-        dist.barrier()
-        # the tree calls on one GPU, same batches (a plain ctx of its own)
-        with engine.GpuCertDatabase(**kw) as one:
-            if rank == 0:
-                r1 = one.store_raw_entries(*inp.page_args("F"), NOW_NS, trees=[engine.LogTree(), engine.LogTree()], entry_log=log_f)
-                res["one_trees"] = [(t.size, t.edge.tobytes(), t.root) for t in r1.trees]
-            elif rank == 1:
-                one.register_chain_certs(*pack(inp.tiles["T5"].certs))
-                r1 = one.store_tiles(*inp.tiles["T5"].args(), NOW_NS, tree=engine.LogTree())
-                res["one_trees"] = [(r1.tree.size, r1.tree.edge.tobytes(), r1.tree.root)]
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        db.close()
-        dist.destroy_process_group()
-    except Exception:  # surface the failure instead of a silent hang of the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+            one.register_chain_certs(*pack(inp.tiles["T5"].certs))
+            r1 = one.store_tiles(*inp.tiles["T5"].args(), NOW_NS, tree=engine.LogTree())
+            res["one_trees"] = [(r1.tree.size, r1.tree.edge.tobytes(), r1.tree.root)]
+    dist.barrier()
+    db.close()
+    dist.destroy_process_group()
+    return res
 
 
 # ---------------------------------------------------------------------------------------------------------- the oracle
@@ -315,7 +296,6 @@ def _check_frontend(got, part, lo=0):
 @pytest.mark.parametrize("mode", ["two_processes_one_gpu", "one_process_per_gpu"])
 def test_collective_front_end_matches_sequential_oracle(ora, mode):
     import torch
-    import torch.multiprocessing as mp
     import merkle_model as mm
     if mode == "one_process_per_gpu":
         if torch.cuda.device_count() < 2:
@@ -323,20 +303,7 @@ def test_collective_front_end_matches_sequential_oracle(ora, mode):
         world, backend, same = min(torch.cuda.device_count(), 4), "nccl", False
     else:
         world, backend, same = 2, "gloo", True
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, backend, same, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=1100)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    outs = run_ranks(_worker, world, (backend, same), timeout=1100)
     from ct_mapreduce_b200 import capi, sharded
     inp = Inputs(ora)
     odb = ora.DB(README_FILTER, False)

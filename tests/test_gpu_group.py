@@ -8,14 +8,12 @@ Two forms of the same device code:
     processes on one GPU (gloo plumbing) and, with >= 2 GPUs, one process per GPU (NCCL plumbing).
 Every comparison is against the oracle run SEQUENTIALLY over the same entries in the order the group defines.
 """
-import os
-import socket
-import sys
 
 import numpy as np
 import pytest
 
-from conftest import NOW_NS, NOW_SEC, README_FILTER, ROOT, go_pem
+from conftest import NOW_NS, NOW_SEC, README_FILTER, go_pem
+from peer_ranks import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -234,91 +232,74 @@ def test_group_snapshot_and_restore(eng, ora):
 
 
 # ------------------------------------------------------------------------------------------------ one process per GPU
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _peer_worker(rank, world, port, backend, same_gpu, n, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
-    try:
-        import torch
-        import torch.distributed as dist
-        devno = 0 if same_gpu else rank
-        torch.cuda.set_device(devno)
-        dev = torch.device("cuda", devno)
-        if backend == "nccl":
-            dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
-        else:
-            dist.init_process_group("gloo", rank=rank, world_size=world)
-        from ct_mapreduce_b200 import capi, engine, sharded
-        cfg = capi.synth_cfg(world * n * 2, len_mode=1, len_lo=512, len_hi=3000, dup_mode=1)
-        iblob, ioffs = engine.synth_issuers(cfg)
-        db = engine.GpuCertDatabase(device=devno, table_capacity=1 << 16, issuer_cn_filter=README_FILTER, max_issuers=1024,
-                                    max_batch_entries=1500)
-        sharded.attach_peers(db)
-        # issuers registered in a rank-dependent order: the indices must agree anyway (shared device registry)
-        ni = ioffs.size - 1
-        perm = np.roll(np.arange(ni), 37 * rank)
-        ders = [iblob[ioffs[k]:ioffs[k + 1]].tobytes() for k in perm]
-        po = np.zeros(ni + 1, np.uint64)
-        po[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
-        dense_perm = db.register_issuers(np.frombuffer(b"".join(ders), np.uint8), po)
-        dense = np.zeros(ni, np.uint32)
-        dense[perm] = dense_perm
-        res = {"dense": dense}
-        # everything the host has to prepare happens BEFORE the collective calls (a rank waiting at a barrier spins on the GPU)
-        from oracle import oracle as ora
-        m = n - 400 * (world - 1 - rank)   # ragged: the ranks pass different sizes to the host-buffer call
-        hb, ho, hi = ora.synth_corpus(ora.synth_cfg(world * n * 2, len_mode=1, len_lo=512, len_hi=3000, dup_mode=1), world * n + rank * n, m)
-        blob, offsets, idx, total = engine.synth_corpus_device(cfg, rank * n, n, dev)
-        idx_dense = torch.from_numpy(dense.astype(np.int32)).to(dev)[idx.long()]
-        status = torch.empty(n, dtype=torch.uint8, device=dev)
-        sha = torch.empty((n, 32), dtype=torch.uint8, device=dev)
-        exp_hour = torch.empty(n, dtype=torch.int64, device=dev)
-        wu = torch.empty(n, dtype=torch.uint8, device=dev)
-        fi = torch.empty(n, dtype=torch.uint8, device=dev)
-        counts = torch.zeros(ni, dtype=torch.int64, device=dev)
-        stat = torch.zeros(capi.ST_COUNT, dtype=torch.int64, device=dev)
-        torch.cuda.synchronize(dev)
-        dist.barrier()
-        # ---- collective HOST-buffer call on the second half of the corpus
-        got = db.store_batch(hb, ho, iblob, ioffs, hi, NOW_NS, want_meta=True)
-        res["host"] = (m, got.status, got.sha256, got.was_unknown, got.first_issuer_hour, got.first_issuer_dn, got.first_crldp)
-        dist.barrier()
-        # ---- collective device-resident call: this rank's shard = entries [rank*n, (rank+1)*n) of the corpus; its global
-        # indices start above everything the host-buffer call used
-        b = capi.DevBatch()
-        b.blob, b.blob_bytes, b.offsets, b.n = blob.data_ptr(), total, offsets.data_ptr(), n
-        b.issuer_idx, b.issuer_map, b.issuer_map_len = idx_dense.data_ptr(), None, 0
-        b.first_index, b.now_unix_ns = 1 << 40, NOW_NS
-        o = capi.DevOut(status.data_ptr(), sha.data_ptr(), exp_hour.data_ptr(), None, None, wu.data_ptr(), fi.data_ptr(), None)
-        db.process_device(b, o)
-        db.peer_allreduce_histogram_device(counts, ni, stat)
-        torch.cuda.synchronize(dev)
-        db.check_device()
-        res["dev"] = (status.cpu().numpy(), sha.cpu().numpy(), wu.cpu().numpy(), fi.cpu().numpy(), counts.cpu().numpy(), stat.cpu().numpy())
-        res["counts"] = db.issuer_counts()
-        dist.barrier()
-        q.put((rank, res, None))
-        dist.barrier()
-        db.close()
-        dist.destroy_process_group()
-    except Exception as e:  # surface the failure instead of a silent hang of the parent
-        import traceback
-        q.put((rank, None, traceback.format_exc()))
-        raise
+def _peer_worker(rank, world, backend, same_gpu, n):
+    import torch
+    import torch.distributed as dist
+    devno = 0 if same_gpu else rank
+    torch.cuda.set_device(devno)
+    dev = torch.device("cuda", devno)
+    if backend == "nccl":
+        dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
+    else:
+        dist.init_process_group("gloo", rank=rank, world_size=world)
+    from ct_mapreduce_b200 import capi, engine, sharded
+    cfg = capi.synth_cfg(world * n * 2, len_mode=1, len_lo=512, len_hi=3000, dup_mode=1)
+    iblob, ioffs = engine.synth_issuers(cfg)
+    db = engine.GpuCertDatabase(device=devno, table_capacity=1 << 16, issuer_cn_filter=README_FILTER, max_issuers=1024,
+                                max_batch_entries=1500)
+    sharded.attach_peers(db)
+    # issuers registered in a rank-dependent order: the indices must agree anyway (shared device registry)
+    ni = ioffs.size - 1
+    perm = np.roll(np.arange(ni), 37 * rank)
+    ders = [iblob[ioffs[k]:ioffs[k + 1]].tobytes() for k in perm]
+    po = np.zeros(ni + 1, np.uint64)
+    po[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
+    dense_perm = db.register_issuers(np.frombuffer(b"".join(ders), np.uint8), po)
+    dense = np.zeros(ni, np.uint32)
+    dense[perm] = dense_perm
+    res = {"dense": dense}
+    # everything the host has to prepare happens BEFORE the collective calls (a rank waiting at a barrier spins on the GPU)
+    from oracle import oracle as ora
+    m = n - 400 * (world - 1 - rank)   # ragged: the ranks pass different sizes to the host-buffer call
+    hb, ho, hi = ora.synth_corpus(ora.synth_cfg(world * n * 2, len_mode=1, len_lo=512, len_hi=3000, dup_mode=1), world * n + rank * n, m)
+    blob, offsets, idx, total = engine.synth_corpus_device(cfg, rank * n, n, dev)
+    idx_dense = torch.from_numpy(dense.astype(np.int32)).to(dev)[idx.long()]
+    status = torch.empty(n, dtype=torch.uint8, device=dev)
+    sha = torch.empty((n, 32), dtype=torch.uint8, device=dev)
+    exp_hour = torch.empty(n, dtype=torch.int64, device=dev)
+    wu = torch.empty(n, dtype=torch.uint8, device=dev)
+    fi = torch.empty(n, dtype=torch.uint8, device=dev)
+    counts = torch.zeros(ni, dtype=torch.int64, device=dev)
+    stat = torch.zeros(capi.ST_COUNT, dtype=torch.int64, device=dev)
+    torch.cuda.synchronize(dev)
+    dist.barrier()
+    # ---- collective HOST-buffer call on the second half of the corpus
+    got = db.store_batch(hb, ho, iblob, ioffs, hi, NOW_NS, want_meta=True)
+    res["host"] = (m, got.status, got.sha256, got.was_unknown, got.first_issuer_hour, got.first_issuer_dn, got.first_crldp)
+    dist.barrier()
+    # ---- collective device-resident call: this rank's shard = entries [rank*n, (rank+1)*n) of the corpus; its global
+    # indices start above everything the host-buffer call used
+    b = capi.DevBatch()
+    b.blob, b.blob_bytes, b.offsets, b.n = blob.data_ptr(), total, offsets.data_ptr(), n
+    b.issuer_idx, b.issuer_map, b.issuer_map_len = idx_dense.data_ptr(), None, 0
+    b.first_index, b.now_unix_ns = 1 << 40, NOW_NS
+    o = capi.DevOut(status.data_ptr(), sha.data_ptr(), exp_hour.data_ptr(), None, None, wu.data_ptr(), fi.data_ptr(), None)
+    db.process_device(b, o)
+    db.peer_allreduce_histogram_device(counts, ni, stat)
+    torch.cuda.synchronize(dev)
+    db.check_device()
+    res["dev"] = (status.cpu().numpy(), sha.cpu().numpy(), wu.cpu().numpy(), fi.cpu().numpy(), counts.cpu().numpy(), stat.cpu().numpy())
+    res["counts"] = db.issuer_counts()
+    dist.barrier()
+    db.close()
+    dist.destroy_process_group()
+    return res
 
 
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("mode", ["two_processes_one_gpu", "one_process_per_gpu"])
 def test_peer_processes_match_sequential_oracle(ora, mode):
     import torch
-    import torch.multiprocessing as mp
     from ct_mapreduce_b200 import sharded
     if mode == "one_process_per_gpu":
         if torch.cuda.device_count() < 2:
@@ -327,20 +308,7 @@ def test_peer_processes_match_sequential_oracle(ora, mode):
     else:
         world, backend, same = 2, "gloo", True
     n = 6000
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_peer_worker, args=(r, world, port, backend, same, n, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, res, err = q.get(timeout=800)
-        assert err is None, err
-        outs[rank] = res
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    outs = run_ranks(_peer_worker, world, (backend, same, n), timeout=800)
     # the registry gave every rank the same dense index for the same issuer, whatever the registration order
     for r in range(1, world):
         assert np.array_equal(outs[0]["dense"], outs[r]["dense"])

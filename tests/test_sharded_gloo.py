@@ -12,16 +12,12 @@
     first_index + (round * world + rank) * E + j the result must equal the oracle run sequentially over
     sequential_order() -- and a deliberately broken variant (resolve before every rank's appends have landed) must not.
 """
-import os
-import socket
-import sys
-
 import numpy as np
 import pytest
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
-from conftest import NOW_NS, README_FILTER, ROOT
+from conftest import NOW_NS, README_FILTER
+from peer_ranks import run_ranks
 
 M64 = (1 << 64) - 1
 
@@ -38,14 +34,6 @@ def key_owner(exp_hour, issuer, world):
     return mix64(((issuer & 0xFFFFFFFF) << 32) | (exp_hour & 0xFFFFFFFF)) % world
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 class RecordingCtx:
     """Stand-in for engine.GpuCertDatabase in attach_peers: records what the host logic hands to the C ABI."""
 
@@ -59,9 +47,7 @@ class RecordingCtx:
         self.attached = (rank, world, [h[0] for h in handles], [h[1] for h in handles])
 
 
-def _model_worker(rank, world, port, n, rounds, broken, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    sys.path.insert(0, ROOT)
+def _model_worker(rank, world, n, rounds, broken):
     from ct_mapreduce_b200 import sharded
     from oracle import oracle as ora
     dist.init_process_group("gloo", rank=rank, world_size=world)
@@ -142,12 +128,8 @@ def _model_worker(rank, world, port, n, rounds, broken, q):
         for c in tot:
             for i, v in c.items():
                 merged[i] = merged.get(i, 0) + v
-        q.put((rank, was_unknown, first, merged, None))
         dist.barrier()
-    except Exception:
-        import traceback
-        q.put((rank, None, None, None, traceback.format_exc()))
-        raise
+        return was_unknown, first, merged
     finally:
         dist.destroy_process_group()
 
@@ -155,20 +137,7 @@ def _model_worker(rank, world, port, n, rounds, broken, q):
 def _run_model(ora, broken):
     from ct_mapreduce_b200 import sharded
     world, n, rounds = 2, 3000, 4
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_model_worker, args=(r, world, port, n, rounds, broken, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    outs = {}
-    for _ in range(world):
-        rank, wu, fi, merged, err = q.get(timeout=300)
-        assert err is None, err
-        outs[rank] = (wu, fi, merged)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    outs = run_ranks(_model_worker, world, (n, rounds, broken), timeout=300)
     cfg = ora.synth_cfg(world * n, len_mode=1, len_lo=512, len_hi=2048, dup_mode=1)
     iblob, ioffs = ora.synth_issuers(cfg)
     shards = [ora.synth_corpus(cfg, r * n, n) for r in range(world)]

@@ -51,6 +51,7 @@ EXPORTS = [
     "ctmr_bind_host_to_device", "ctmr_peer_rounds", "ctmr_peer_round_entries", "ctmr_peer_frontend_stopped",
     "ctmr_next_index",
     "ctmr_revoked_known", "ctmr_group_revoked_known",   # CRLs joined with the known-certificate sets
+    "ctmr_revoked_cascade", "ctmr_group_revoked_cascade",   # CRLite's filter cascade of the covered issuers
 ]
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -162,6 +163,15 @@ class CrlOut(C.Structure):
                  "issuer_name_len", "crl_first", "crl_entries", "serial_off", "serial_len", "revoked_at", "reason",
                  "entry_status", "known", "known_exp_hour", "known_sets")] + \
                [("entry_cap", C.c_uint64), ("n_entries", C.c_uint64)]
+
+
+class CascadeOut(C.Structure):
+    """ctmr_cascade_out (include/ctmr.h)."""
+    _fields_ = [("buf", C.c_void_p), ("cap", C.c_uint64), ("bytes", C.c_uint64), ("crl_status", C.c_void_p),
+                ("issuers", C.c_uint32), ("levels", C.c_uint32), ("revoked", C.c_uint64), ("valid", C.c_uint64)]
+
+
+CASCADE_MAX_SALT = 32   # salt_len of ctmr_revoked_cascade
 
 
 class SynthCfg(C.Structure):
@@ -299,6 +309,8 @@ def load():
     L.ctmr_next_index.argtypes = [vp, C.POINTER(u64)]
     L.ctmr_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
     L.ctmr_group_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
+    L.ctmr_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
+    L.ctmr_group_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
     for name in EXPORTS:
         getattr(L, name)  # every symbol include/ctmr.h declares must resolve
     _lib = L

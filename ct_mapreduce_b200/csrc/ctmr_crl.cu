@@ -327,14 +327,6 @@ __global__ void __launch_bounds__(256) crl_entry_kernel(const uint8_t* __restric
     o.status[e] = ce.indirect ? CTMR_RV_INDIRECT : ce.serial_len > CTMR_MAX_SERIAL ? CTMR_RV_SERIAL_TOO_LONG : CTMR_RV_OK;
 }
 
-// the pair's key exactly as words 1..11 of a KnownSlot body: issuer, then {serial_len, serial[39]} little-endian
-__device__ __forceinline__ uint32_t pair_hash(const uint32_t (&w)[11]) {
-    uint64_t h = 0x9E3779B97F4A7C15ull;
-#pragma unroll
-    for (int i = 0; i < 11; ++i) h = mix64(h ^ ((uint64_t)w[i] << (i & 1 ? 32 : 0))) + (uint64_t)i;
-    return (uint32_t)(h >> 32);
-}
-
 // an entry's pair as the words w: issuer, then {serial_len, serial[39]} read from the staged CRL (len <= 255: at most 39
 // serial bytes are read, all inside the serial)
 __device__ __forceinline__ void pair_words(const uint8_t* stage, const CrlDesc& cd, uint64_t serial_off, uint32_t len, uint32_t (&w)[11]) {
@@ -624,8 +616,10 @@ int crl_ensure(ctmr_ctx* c) {
     return CTMR_OK;
 }
 
+}  // namespace
+
 // the set arrays for `slots` pairs (a power of two), all or nothing; `recv`: also the receive side of a group's member 0
-int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
+int ctmr_host::crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
     if (!c->crl) {
         c->crl.reset(new (std::nothrow) CrlState());
         if (!c->crl) return fail(c, CTMR_E_NOMEM, "host allocation failed");
@@ -651,6 +645,8 @@ int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
     s->set_cap = cap;
     return CTMR_OK;
 }
+
+namespace {
 
 // A rank attached to peers, after crl_ensure: the records of one round (X) and the union set of a round (2 world X
 // slots, so that a free slot always exists), all or nothing
@@ -832,6 +828,29 @@ EntryOut entry_out(CrlState* s) {
     return EntryOut{s->eserial_off, s->eserial_len, s->ereason, s->estatus, s->eknown, s->erevoked, s->ehour, s->eslot, s->esets};
 }
 
+// The entries of the chunk in stage[st] (ne of them, ne > 0) parsed, and the set of their (issuer, serial) pairs built on
+// c's stream, with its hour and count answers reset; *slots = the set's slots (its whole allocation: every member of a
+// group probes with the same mask).  `recv`: a group's member 0 also receives the other members' answers.
+int crl_set_build(ctmr_ctx* c, int st, uint32_t ne, bool recv, uint64_t* slots) {
+    CrlState* s = c->crl.get();
+    const cudaStream_t q = c->stream;
+    crl_entry_kernel<<<grid(ne, 256), 256, 0, q>>>(s->stage[st], s->desc[st], s->res, s->epos, s->ecrl, ne, entry_out(s));
+    CU(c, cudaGetLastError());
+    uint64_t n = 64;
+    while (n < 2ull * ne) n <<= 1;
+    const int rc = crl_set_ensure(c, n, recv);
+    if (rc) return rc;
+    n = s->set_cap;
+    CU(c, cudaMemsetAsync(s->set, 0, n * sizeof(CrlSetSlot), q));
+    CU(c, cudaMemsetAsync(s->set_hour, 0x7f, n * sizeof(int32_t), q));
+    CU(c, cudaMemsetAsync(s->set_count, 0, n * sizeof(uint32_t), q));
+    crl_set_insert_kernel<<<grid(ne, 256), 256, 0, q>>>(s->stage[st], s->desc[st], s->res, s->ecrl, s->eserial_off, s->eserial_len,
+                                                       s->estatus, ne, s->set, n - 1, s->eslot);
+    CU(c, cudaGetLastError());
+    *slots = n;
+    return CTMR_OK;
+}
+
 // One chunk on member 0 (`c`): split, parse, join (every member's table), copy back.  *base: entries placed so far; with
 // `count_only` (the caller's entry_cap is already exceeded) only the count advances.
 int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, ctmr_crl_out* out, const CrlChunk& ch, int st, uint64_t* base,
@@ -839,7 +858,6 @@ int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, ctmr_crl_out* out, 
     ctmr_ctx* c = m[0];
     CrlState* s = c->crl.get();
     cudaStream_t q = c->stream;
-    const uint8_t* stage = s->stage[st];
     uint32_t ne = 0;
     int rc = crl_split(c, ch, st, &ne);
     if (rc) return rc;
@@ -851,19 +869,9 @@ int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, ctmr_crl_out* out, 
     }
     const EntryOut eo = entry_out(s);
     if (ne) {
-        crl_entry_kernel<<<grid(ne, 256), 256, 0, q>>>(stage, s->desc[st], s->res, s->epos, s->ecrl, ne, eo);
-        CU(c, cudaGetLastError());
-        uint64_t slots = 64;
-        while (slots < 2ull * ne) slots <<= 1;
-        int rc = crl_set_ensure(c, slots, W > 1);
+        uint64_t slots = 0;
+        rc = crl_set_build(c, st, ne, W > 1, &slots);
         if (rc) return group_fail(g, c, rc);
-        slots = s->set_cap;  // the set spans its whole allocation: every member probes with the same mask
-        CU(c, cudaMemsetAsync(s->set, 0, slots * sizeof(CrlSetSlot), q));
-        CU(c, cudaMemsetAsync(s->set_hour, 0x7f, slots * sizeof(int32_t), q));
-        CU(c, cudaMemsetAsync(s->set_count, 0, slots * sizeof(uint32_t), q));
-        crl_set_insert_kernel<<<grid(ne, 256), 256, 0, q>>>(stage, s->desc[st], s->res, s->ecrl, s->eserial_off, s->eserial_len, s->estatus, ne,
-                                                           s->set, slots - 1, s->eslot);
-        CU(c, cudaGetLastError());
         crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->set, slots - 1, s->set_hour, s->set_count);
         CU(c, cudaGetLastError());
         if (W > 1) {
@@ -882,17 +890,17 @@ int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, ctmr_crl_out* out, 
 }
 
 // The checks every call makes before any work: the arguments, and each CRL inside data and no larger than a chunk
-int crl_check_batch(ctmr_ctx* c, const ctmr_crl_batch* b, const ctmr_crl_out* out) {
-    if (!b || !out) return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: NULL batch or output");
+int crl_check_batch(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const std::string& call = "ctmr_revoked_known: ") {
+    if (!b || !out) return fail(c, CTMR_E_INVALID, call + "NULL batch or output");
     if (b->n_crls && (!b->data || !b->crl_off || !b->crl_len || !b->issuer_digest))
-        return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: NULL input array");
+        return fail(c, CTMR_E_INVALID, call + "NULL input array");
     const uint64_t B = crl_budget(c);
     for (uint64_t k = 0; k < b->n_crls; ++k) {
         const uint64_t off = b->crl_off[k], len = b->crl_len[k];
         if (off > b->data_bytes || len > b->data_bytes - off)
-            return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: CRL " + std::to_string(k) + " lies outside data");
+            return fail(c, CTMR_E_INVALID, call + "CRL " + std::to_string(k) + " lies outside data");
         if (len > B)
-            return fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: CRL " + std::to_string(k) + " (" + std::to_string(len) +
+            return fail(c, CTMR_E_BATCH_TOO_LARGE, call + "CRL " + std::to_string(k) + " (" + std::to_string(len) +
                                                        " bytes) exceeds the staging budget of " + std::to_string(B) + " bytes");
     }
     return CTMR_OK;
@@ -932,6 +940,23 @@ std::vector<CrlChunk> crl_cut(ctmr_ctx* c, const ctmr_crl_batch* b) {
     return chunks;
 }
 
+// Every chunk of the batch (n_crls > 0) staged on the copy stream, the next one while chunk(ch, st) works on the current
+// one in stage[st] on c's stream.  No upload outlives the call, whatever chunk returns.
+int crl_for_chunks(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer,
+                   const std::function<int(const CrlChunk&, int)>& chunk) {
+    int rc = crl_ensure(c);
+    if (rc) return rc;
+    const std::vector<CrlChunk> chunks = crl_cut(c, b);
+    rc = crl_upload(c, b, issuer, chunks[0], 0);
+    for (size_t i = 0; i < chunks.size() && rc == CTMR_OK; ++i) {
+        if (i + 1 < chunks.size()) rc = crl_upload(c, b, issuer, chunks[i + 1], (int)((i + 1) & 1));
+        if (rc == CTMR_OK) rc = chunk(chunks[i], (int)(i & 1));
+    }
+    const cudaError_t e = cudaStreamSynchronize(c->crl->copy_stream);
+    if (rc == CTMR_OK && e != cudaSuccess) rc = fail(c, CTMR_E_CUDA, std::string("cudaStreamSynchronize: ") + cudaGetErrorString(e));
+    return rc;
+}
+
 // the call on member 0 of `W` members (W == 1: one ctx)
 int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, ctmr_crl_out* out) {
     ctmr_ctx* c = m[0];
@@ -943,25 +968,10 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
     std::vector<uint32_t> issuer;
     rc = crl_issuers(c, b, issuer);
     if (rc) return group_fail(g, c, rc);
-    rc = crl_ensure(c);
-    if (rc) return group_fail(g, c, rc);
-    const std::vector<CrlChunk> chunks = crl_cut(c, b);
     uint64_t base = 0;
     bool count_only = false;
-    rc = crl_upload(c, b, issuer, chunks[0], 0);
+    rc = crl_for_chunks(c, b, issuer, [&](const CrlChunk& ch, int st) { return crl_chunk(m, W, g, out, ch, st, &base, &count_only); });
     if (rc) return group_fail(g, c, rc);
-    for (size_t i = 0; i < chunks.size(); ++i) {
-        if (i + 1 < chunks.size()) {
-            rc = crl_upload(c, b, issuer, chunks[i + 1], (int)((i + 1) & 1));
-            if (rc) return group_fail(g, c, rc);
-        }
-        rc = crl_chunk(m, W, g, out, chunks[i], (int)(i & 1), &base, &count_only);
-        if (rc) {
-            cudaStreamSynchronize(c->crl->copy_stream);
-            return group_fail(g, c, rc);
-        }
-    }
-    CU(c, cudaStreamSynchronize(c->crl->copy_stream));
     out->n_entries = base;
     if (count_only)
         return group_fail(g, c, fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: entry_cap " + std::to_string(out->entry_cap) + " < " +
@@ -1128,6 +1138,40 @@ int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) 
 }
 
 }  // namespace
+
+// ---- the chunk path as ctmr_revoked_cascade uses it (ctmr_cascade.cu) -------------------------------------------------
+namespace ctmr_host {
+
+int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer) {
+    int rc = crl_check_batch(c, b, out, call);
+    if (rc == CTMR_OK) rc = crl_issuers(c, b, issuer);
+    return rc;
+}
+
+int crl_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit) {
+    if (b->n_crls == 0) return CTMR_OK;
+    std::vector<CrlRes> res;
+    std::vector<uint8_t> status;
+    return crl_for_chunks(c, b, issuer, [&](const CrlChunk& ch, int st) -> int {
+        CrlState* s = c->crl.get();
+        const cudaStream_t q = c->stream;
+        uint32_t ne = 0;
+        uint64_t slots = 0;
+        int rc = crl_split(c, ch, st, &ne);
+        if (rc == CTMR_OK && ne) rc = crl_set_build(c, st, ne, false, &slots);
+        if (rc) return rc;
+        CU(c, cudaEventRecord(s->consumed[st], q));
+        const uint32_t n = (uint32_t)(ch.hi - ch.lo);
+        res.resize(n);
+        CU(c, cudaMemcpyAsync(res.data(), s->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, q));
+        CU(c, cudaStreamSynchronize(q));
+        status.resize(n);
+        for (uint32_t k = 0; k < n; ++k) status[k] = (uint8_t)res[k].status;
+        return visit(ch.lo, status, ne ? s->set.get() : nullptr, slots ? slots - 1 : 0);
+    });
+}
+
+}  // namespace ctmr_host
 
 extern "C" {
 

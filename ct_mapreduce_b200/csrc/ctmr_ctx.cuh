@@ -15,6 +15,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -348,6 +349,24 @@ struct CrlState {
     DevBuf<uint32_t> union_count;
 };
 
+// ctmr_revoked_cascade (ctmr_cascade.cu): one bit per table slot (revoked: the slot's pair is in a chunk's set), the
+// registry's digests and the covered-issuer bitmap over dense indices, the three include / test lists of slot indices
+// [list_cap] each, one level's bits [bit_words] and on a group's member 0 the receive side of the merge [bit_words].
+// Built on first use and grown, all or nothing.
+struct CascadeState {
+    uint64_t slot_words = 0;
+    DevBuf<uint32_t> revoked;            // [slot_words]
+    uint32_t issuer_cap = 0;
+    DevBuf<uint8_t> dig;                 // [issuer_cap][32]
+    DevBuf<uint32_t> covered;            // [issuer_cap / 32 + 1]
+    DevBuf<unsigned long long> counters; // [2]: records appended to a list, records counted
+    uint64_t list_cap = 0;
+    DevBuf<uint32_t> list[3];
+    uint64_t bit_words = 0;
+    DevBuf<uint32_t> bits, recv;         // recv: a group's member 0 only (0 words elsewhere)
+    uint64_t recv_words = 0;
+};
+
 // the ctx's private device words (one allocation)
 struct SmallDev {
     unsigned long long slots_used;   // DeviceState::slots_used points here (no kernel reads it)
@@ -443,6 +462,7 @@ struct ctmr_ctx {
     std::unique_ptr<FrontEnd> fe;
     uint32_t fe_peer_stopped = 0;  // ranks that stopped (tiles) in the last collective front-end call
     std::unique_ptr<CrlState> crl;  // ctmr_revoked_known (ctmr_crl.cu)
+    std::unique_ptr<CascadeState> cascade;  // ctmr_revoked_cascade (ctmr_cascade.cu)
     std::string err;
 };
 
@@ -584,6 +604,17 @@ int ensure_device_path(ctmr_ctx* c, uint64_t n);   // what ctmr_process_device n
 int reset_tables(ctmr_ctx* c, cudaStream_t s);
 // after the registry was replaced: the host memos of it go, and so do the Chain[0] mirror and the tiles' fingerprints
 int clear_issuer_memos(ctmr_ctx* c);
+
+// ctmr_revoked_cascade's use of the CRL path (ctmr_crl.cu).  crl_prepare: ctmr_revoked_known's checks before any work
+// (`out` is only tested for NULL; `call` opens the error text), then each CRL's dense issuer (CTMR_ISSUER_NONE when the
+// digest is not registered).  crl_each_set: every chunk through the split, the entries and the set of its (issuer,
+// serial) pairs on c's stream; after each, visit(first CRL of the chunk, CTMR_CRL_* of its CRLs, the set or NULL when the
+// chunk has no entries, mask) while the set is intact.  Synchronous; no upload outlives it.
+using CrlSetVisit = std::function<int(uint64_t, const std::vector<uint8_t>&, const CrlSetSlot*, uint64_t)>;
+int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer);
+int crl_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit);
+// the set arrays for `slots` pairs (a power of two), all or nothing; `recv`: also the receive side of a group's member 0
+int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv);
 
 // Where a table's live slots go when they are compacted in slot order (launch_evict_compact): the exclusive prefix of the
 // live slots per tile of kCompactTile, on the host and on the device.  host[tiles()] = the live slots of the table.

@@ -12,6 +12,8 @@ points, and exposes the results under the reference's names:
     GpuCertDatabase.status_counters    <- metrics certIsFilteredOut.{CA,expired,cn-filtered}, insertCTWorker.Inserted
     GpuCertDatabase.revoked_known      <- the join CRLite makes of an issuer's CRLs (crl::<issuer>) with its
                                           serials::<expDate>::<issuer> sets (storage/knowncertificates.go:28-55)
+    GpuCertDatabase.revoked_cascade    <- CRLite's filter cascade of the covered issuers' revoked and valid known
+                                          certificates, built on the GPU next to the table
 
 All arithmetic happens in the CUDA kernels; nothing here parses, hashes or de-duplicates.
 """
@@ -221,6 +223,32 @@ class RevokedResult:
     def serial(self, data: np.ndarray, e: int) -> bytes:
         o = int(self.serial_off[e])
         return bytes(data[o:o + int(self.serial_len[e])])
+
+
+class CascadeResult:
+    """Outputs of ctmr_revoked_cascade (include/ctmr.h ctmr_cascade_out): the serialized filter cascade, each CRL's
+    status, and the covered issuers, levels and key records in R (revoked) and S (valid)."""
+
+    def __init__(self, data: bytes, crl_status: np.ndarray, o):
+        self.bytes = data
+        self.crl_status = crl_status
+        self.issuers, self.levels, self.revoked, self.valid = int(o.issuers), int(o.levels), int(o.revoked), int(o.valid)
+
+
+def _crl_batch(crls, issuer_digests):
+    """(ctmr_crl_batch, the arrays it points into) of a list of DER CRLs or (data, crl_off, crl_len)"""
+    if isinstance(crls, tuple):
+        data, offs, lens = (np.ascontiguousarray(a) for a in crls)
+        data, offs, lens = data.astype(np.uint8, copy=False), offs.astype(np.uint64), lens.astype(np.uint64)
+    else:
+        data, offs, lens = pack_crls(crls)
+    n = len(offs)
+    dig = np.frombuffer(b"".join(bytes(d) for d in issuer_digests), np.uint8) if n else np.zeros(32, np.uint8)
+    if n and dig.size != 32 * n:
+        raise ValueError("one 32-byte issuer digest per CRL")
+    b = capi.CrlBatch(capi.ptr(data) if data.size else None, data.size, capi.ptr(offs) if n else None,
+                      capi.ptr(lens) if n else None, capi.ptr(dig) if n else None, n)
+    return b, (data, offs, lens, dig)
 
 
 def pack_crls(crls):
@@ -736,19 +764,10 @@ class GpuCertDatabase:
         and gets the answers for its own CRLs against every rank's shard.  A rank whose arguments are refused here
         still makes the call, with no batch, so that the other ranks return CTMR_E_PEER_FAILED, and then raises."""
         with self._peer_refusal(lambda: self._revoked_known_fn()(self._h, None, None)):
-            if isinstance(crls, tuple):
-                data, offs, lens = (np.ascontiguousarray(a) for a in crls)
-                data, offs, lens = data.astype(np.uint8, copy=False), offs.astype(np.uint64), lens.astype(np.uint64)
-            else:
-                data, offs, lens = pack_crls(crls)
-            n = len(offs)
-            dig = np.frombuffer(b"".join(bytes(d) for d in issuer_digests), np.uint8) if n else np.zeros(32, np.uint8)
-            if n and dig.size != 32 * n:
-                raise ValueError("one 32-byte issuer digest per CRL")
+            b, keep = _crl_batch(crls, issuer_digests)
+            lens = keep[2]
             cap = int(lens.sum()) // capi.CRL_MIN_ENTRY if entry_cap is None else int(entry_cap)
-            res = RevokedResult(n, cap)
-            b = capi.CrlBatch(capi.ptr(data) if data.size else None, data.size, capi.ptr(offs) if n else None,
-                              capi.ptr(lens) if n else None, capi.ptr(dig) if n else None, n)
+            res = RevokedResult(int(b.n_crls), cap)
             o = res.to_c()
         rc = self._revoked_known_fn()(self._h, C.byref(b), C.byref(o))
         res.n_entries = int(o.n_entries)
@@ -759,6 +778,37 @@ class GpuCertDatabase:
             raise
         res.trim(int(o.n_entries))
         return res
+
+    def _revoked_cascade_fn(self):
+        return self._lib.ctmr_revoked_cascade
+
+    _cascade_bytes = 0   # size of the last cascade this db built: the next call's first buffer holds twice that
+
+    def revoked_cascade(self, crls, issuer_digests, now_unix_sec: int, salt: bytes = b"", cap: int | None = None) -> CascadeResult:
+        """CRLite's filter cascade (ctmr_revoked_cascade): it includes the live known certificates of the covered issuers
+        that these CRLs revoke and excludes every other live known certificate of those issuers.  An issuer is covered
+        when it is registered and every one of its CRLs here parses (CRL_OK).  `crls` and `issuer_digests` as for
+        revoked_known; `salt`: at most 32 bytes.  Read-only.  Returns .bytes (the serialized cascade), .crl_status,
+        .issuers, .levels, .revoked and .valid.
+        The output buffer holds `cap` bytes; by default 16 MiB, or twice the last cascade this db built if that is more.
+        A cascade larger than the buffer is built twice: the first build only reports its size (the library writes
+        nothing else when the buffer is too small), the second fills a buffer of that size."""
+        b, keep = _crl_batch(crls, issuer_digests)
+        salt = bytes(salt)
+        sbuf = (C.c_uint8 * max(len(salt), 1)).from_buffer_copy(salt or b"\0")
+        status = np.zeros(max(int(b.n_crls), 1), np.uint8)
+        size = int(cap) if cap is not None else max(16 << 20, 2 * self._cascade_bytes)
+        buf = np.empty(max(size, 1), np.uint8)
+        o = capi.CascadeOut(capi.ptr(buf), size, 0, capi.ptr(status))
+        fn = self._revoked_cascade_fn()
+        rc = fn(self._h, C.byref(b), int(now_unix_sec), sbuf, len(salt), C.byref(o))
+        if rc == capi.E_BATCH_TOO_LARGE and o.bytes:  # larger than the buffer: again into one of the size it reported
+            buf = np.empty(int(o.bytes), np.uint8)
+            o = capi.CascadeOut(capi.ptr(buf), buf.size, 0, capi.ptr(status))
+            rc = fn(self._h, C.byref(b), int(now_unix_sec), sbuf, len(salt), C.byref(o))
+        self._check(rc)
+        self._cascade_bytes = int(o.bytes)
+        return CascadeResult(buf[:o.bytes].tobytes(), status[:b.n_crls].copy(), o)
 
     def checkpoint(self) -> np.ndarray:
         """This db's part of a portable checkpoint (ctmr_checkpoint_save): loads into any table size, group size or number
@@ -954,6 +1004,9 @@ class GpuCertGroup(GpuCertDatabase):
 
     def _revoked_known_fn(self):
         return self._lib.ctmr_group_revoked_known
+
+    def _revoked_cascade_fn(self):
+        return self._lib.ctmr_group_revoked_cascade
 
     def get_known_certificates(self, exp_hour: int, issuer_digest: bytes):
         grp = self

@@ -138,3 +138,90 @@ func (d *DB) RevokedKnown(crls [][]byte, issuerIDs [][32]byte) ([]CRLResult, err
 	}
 	return res, nil
 }
+
+// Cascade is CRLite's filter cascade as RevokedCascade builds it (include/ctmr.h "CRLite filter cascade" states the
+// layout and the query rule).
+type Cascade struct {
+	Bytes     []byte  // the serialized cascade
+	CRLStatus []uint8 // per CRL, CTMR_CRL_*
+	Issuers   uint32  // issuers covered: registered, in the batch, every CRL of theirs CTMR_CRL_OK
+	Levels    uint32
+	Revoked   uint64 // key records included (R)
+	Valid     uint64 // key records excluded (S)
+}
+
+// RevokedCascade builds the filter cascade of the covered issuers' live known certificates on the GPU: the revoked
+// ones included, every other one excluded.  crls and issuerIDs as for RevokedKnown, verified CRLs only; salt is at most
+// 32 bytes.  Read-only.  A DB attached to peers has no collective form yet: the library refuses the call.  The output
+// buffer holds 16 MiB, or twice the DB's last cascade if that is more; a larger cascade is built twice (the first build
+// only reports its size).
+func (d *DB) RevokedCascade(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int64, salt []byte) (*Cascade, error) {
+	n := len(crls)
+	if len(issuerIDs) < n {
+		return nil, fmt.Errorf("RevokedCascade: %d issuer IDs for %d CRLs", len(issuerIDs), n)
+	}
+	total := 0
+	for _, c := range crls {
+		total += len(c)
+	}
+	data := C.malloc(C.size_t(total + 1))
+	defer C.free(data)
+	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
+	lens := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
+	dig := C.malloc(C.size_t(32*n + 32))
+	defer C.free(unsafe.Pointer(&offs[0]))
+	defer C.free(unsafe.Pointer(&lens[0]))
+	defer C.free(dig)
+	flat := unsafe.Slice((*byte)(data), total+1)
+	o := 0
+	for i, c := range crls {
+		copy(flat[o:], c)
+		offs[i], lens[i] = C.uint64_t(o), C.uint64_t(len(c))
+		copy(unsafe.Slice((*byte)(dig), 32*n)[32*i:], issuerIDs[i][:])
+		o += len(c)
+	}
+	b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
+	defer C.free(unsafe.Pointer(b))
+	b.data, b.data_bytes = (*C.uint8_t)(data), C.uint64_t(total)
+	b.crl_off, b.crl_len = &offs[0], &lens[0]
+	b.issuer_digest, b.n_crls = (*C.uint8_t)(dig), C.uint64_t(n)
+	cs := C.malloc(C.size_t(len(salt) + 1))
+	defer C.free(cs)
+	copy(unsafe.Slice((*byte)(cs), len(salt)+1), salt)
+	status := C.calloc(C.size_t(n+1), 1)
+	defer C.free(status)
+	out := (*C.ctmr_cascade_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_cascade_out{}))))
+	defer C.free(unsafe.Pointer(out))
+	call := func() C.int {
+		if d.g != nil {
+			return C.ctmr_group_revoked_cascade(d.g, b, C.int64_t(nowUnixSec), (*C.uint8_t)(cs), C.uint32_t(len(salt)), out)
+		}
+		return C.ctmr_revoked_cascade(d.h, b, C.int64_t(nowUnixSec), (*C.uint8_t)(cs), C.uint32_t(len(salt)), out)
+	}
+	size := uint64(16 << 20)
+	if 2*d.cascadeBytes > size {
+		size = 2 * d.cascadeBytes
+	}
+	buf := C.malloc(C.size_t(size)) // a larger cascade is built again into a buffer of the size it reported
+	out.buf, out.cap, out.crl_status = (*C.uint8_t)(buf), C.uint64_t(size), (*C.uint8_t)(status)
+	rc := call()
+	if rc == C.CTMR_E_BATCH_TOO_LARGE && out.bytes > 0 {
+		C.free(buf)
+		buf = C.malloc(C.size_t(out.bytes))
+		out.buf, out.cap = (*C.uint8_t)(buf), out.bytes
+		rc = call()
+	}
+	defer C.free(buf)
+	if err := d.err(rc, "ctmr_revoked_cascade"); err != nil {
+		return nil, err
+	}
+	d.cascadeBytes = uint64(out.bytes)
+	return &Cascade{
+		Bytes:     C.GoBytes(buf, C.int(out.bytes)),
+		CRLStatus: C.GoBytes(status, C.int(n)),
+		Issuers:   uint32(out.issuers),
+		Levels:    uint32(out.levels),
+		Revoked:   uint64(out.revoked),
+		Valid:     uint64(out.valid),
+	}, nil
+}

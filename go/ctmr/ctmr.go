@@ -59,9 +59,10 @@ type Config struct {
 // DB is one ctx (one GPU) or one group (several GPUs of the box behind one handle): the fan-out is
 // inside the library, invisible here (SURVEY.md §8(b)).
 type DB struct {
-	h    *C.ctmr_ctx
-	g    *C.ctmr_group
-	peer bool // attached to the DBs of other processes (PeerAttach): the batch calls and the front end are collective
+	h            *C.ctmr_ctx
+	g            *C.ctmr_group
+	peer         bool   // attached to the DBs of other processes (PeerAttach): the batch calls and the front end are collective
+	cascadeBytes uint64 // size of the last RevokedCascade: the next call's first buffer holds twice that
 }
 
 func New(c Config) (*DB, error) {

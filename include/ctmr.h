@@ -309,6 +309,62 @@ typedef struct ctmr_crl_out {                      /* caller-allocated, any poin
  * On a failed call (rc != 0) the outputs other than n_entries are undefined. */
 int ctmr_revoked_known(ctmr_ctx* ctx, const ctmr_crl_batch* batch, ctmr_crl_out* out);
 
+/* ---- CRLite filter cascade (the revoked / not-revoked Bloom cascade of the covered issuers) ------------------------- */
+/* Builds CRLite's filter cascade straight from the table: only the serialized filter reaches the host (DESIGN.md
+ * "Revoked cascade").  Same batch and match rule as ctmr_revoked_known; the batch holds the CRLs the caller accepts (their
+ * signatures already verified, INTEGRATION.md §2d).
+ *
+ * Sets.  An issuer is COVERED when its digest appears in the batch, it is in the registry, and every one of its CRLs in the
+ * batch is CTMR_CRL_OK (an issuer with a bad CRL must not claim its certificates valid).  A LIVE key record is a ready key
+ * whose set has exp_hour * 3600 > now_unix_sec (the sets ctmr_evict_expired(now) keeps).  Of the live records of covered
+ * issuers, R = those whose (issuer, raw serial) equals a CTMR_RV_OK entry of a CTMR_CRL_OK CRL (byte for byte, under
+ * every hour), S = all the others.  Sizes count key records: a serial under two hours counts twice (a group's counts are
+ * sums over its shards).
+ *
+ * Key and hash.  x = digest(32) || serial content octets (Issuer.ID()'s digest, then NewSerial's bytes).  Level l
+ * (1-based) with m_l bits and k_l functions sets or tests the bits
+ *     b_i = LE32(SHA-256(salt || LE32(i) || u8(l) || x)[0..4]) mod m_l,   i = 0 .. k_l - 1.
+ * salt_len <= 32 (every message fits two SHA-256 blocks); a longer salt is CTMR_E_INVALID.
+ *
+ * Sizing: host IEEE double, in exactly this order, with C log, pow, sqrt and ceil:
+ *     p_1 = 0.5 if |R| == 0 or |S| == 0, else min(0.5, |R| / (sqrt(2) * |S|));   p_l = 0.5 for l >= 2
+ *     k_l = max(1, ceil(log(1 / p_l) / log(2)))
+ *     m_l = max(8, ceil(-k_l * n_l / log(1 - pow(p_l, 1.0 / k_l))))   n_l = records included at level l
+ * m_l >= 2^32 is CTMR_E_BATCH_TOO_LARGE (with bytes = 0).
+ *
+ * Build.  Level 1 includes I_1 = R and is tested against E_1 = S.  F_l = the records of E_l that level l contains (all
+ * k_l bits set).  The cascade stops at the first empty F_l; otherwise I_{l+1} = F_l, E_{l+1} = I_l.  More than 255 levels
+ * is CTMR_E_INVALID (the level is one octet): build again with another salt.
+ *
+ * Layout, integers little-endian:
+ *     header      u16 2 (version), u8 0 (not inverted), u8 salt_len, salt[salt_len]
+ *     each level  u8 2 (hash: SHA-256, first 32 bits), u32 m_l, u32 k_l, u8 l, ceil(m_l / 8) bytes of bits
+ * Bit j is (byte[j >> 3] >> (j & 7)) & 1; the unused high bits of the last byte are zero.
+ *
+ * Query.  Walk the levels from 1 and stop at the first that does not contain x: x is revoked iff that level's number is
+ * even.  If all L levels contain x, it is revoked iff L is odd.
+ *
+ * This follows Mozilla's filter-cascade version 2 as restated here.  Byte parity with filter-cascade or rust-cascade is
+ * NOT pinned (neither is available to this build): this header and tests/cascade_model.py pin the format.
+ *
+ * The output is deterministic: it depends neither on table layout, group size nor thread order.  With cap too small (buf
+ * may be NULL) the call returns CTMR_E_BATCH_TOO_LARGE and writes `bytes` and nothing else; a second call with that cap
+ * returns exactly those bytes.  Read-only, like ctmr_revoked_known: no index is taken and no table, counter or registry
+ * changes.  Argument checks are ctmr_revoked_known's (a NULL batch or output, a CRL outside data or larger than a chunk),
+ * plus the salt's.  A member ctx of a group is refused with CTMR_E_INVALID (use ctmr_group_revoked_cascade), and so is a
+ * ctx attached to peers (no collective form yet).  Cost: one pass over the table per CRL chunk, two more for level 1, and
+ * device scratch of one bit per table slot plus the include lists and one level's bits (DESIGN.md "Revoked cascade"). */
+typedef struct ctmr_cascade_out {   /* caller-allocated; HOST buffers */
+    uint8_t* buf; uint64_t cap;     /* the serialized cascade */
+    uint64_t bytes;                 /* written; on CTMR_E_BATCH_TOO_LARGE the bytes needed */
+    uint8_t* crl_status;            /* [n_crls] CTMR_CRL_*, as ctmr_revoked_known; may be NULL */
+    uint32_t issuers;               /* issuers covered */
+    uint32_t levels;
+    uint64_t revoked, valid;        /* key records in R and in S */
+} ctmr_cascade_out;
+int ctmr_revoked_cascade(ctmr_ctx* ctx, const ctmr_crl_batch* batch, int64_t now_unix_sec,
+                         const uint8_t* salt, uint32_t salt_len, ctmr_cascade_out* out);
+
 /* ---- device-resident entry points ---------------------------------------------------------- */
 /* Same path with every buffer already in HBM on ctx's device (benchmarks, multi-GPU orchestration,
  * hosts that receive entries by GPUDirect).  `stream` is a cudaStream_t passed as void*; NULL =
@@ -420,6 +476,11 @@ int ctmr_group_checkpoint_load(ctmr_group* g, const uint8_t* const* parts, const
 /* ctmr_revoked_known over every shard: member 0 parses the CRLs and builds the set of (issuer, serial) pairs, each member
  * scans its own table against a bulk copy of it, and member 0 merges the answers (lowest hour, sum of sets). */
 int ctmr_group_revoked_known(ctmr_group* g, const ctmr_crl_batch* batch, ctmr_crl_out* out);
+/* ctmr_revoked_cascade over every shard, the same bytes as one ctx: member 0 parses the CRLs and builds the set, each
+ * member marks and compacts its own shard, and each level's partial bit arrays are merged on member 0 with peer copies
+ * and copied back to every member before the members test their own records.  No atomic crosses a GPU. */
+int ctmr_group_revoked_cascade(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* salt,
+                               uint32_t salt_len, ctmr_cascade_out* out);
 
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the

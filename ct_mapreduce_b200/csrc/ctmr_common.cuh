@@ -102,7 +102,7 @@ __device__ __forceinline__ uint32_t known_insert(KnownSlot* __restrict__ table, 
 
 // a CRL join's (issuer, serial) pair exactly as words 1..11 of a KnownSlot body: issuer, then {serial_len, serial[39]}
 // little-endian (ctmr_crl.cu's set, probed by ctmr_cascade.cu too)
-__device__ __forceinline__ uint32_t pair_hash(const uint32_t (&w)[11]) {
+__device__ __host__ __forceinline__ uint32_t pair_hash(const uint32_t (&w)[11]) {
     uint64_t h = 0x9E3779B97F4A7C15ull;
 #pragma unroll
     for (int i = 0; i < 11; ++i) h = mix64(h ^ ((uint64_t)w[i] << (i & 1 ? 32 : 0))) + (uint64_t)i;

@@ -192,7 +192,9 @@ class TileBatchResult(RawBatchResult):
 
 
 class RevokedResult:
-    """Outputs of ctmr_revoked_known (include/ctmr.h ctmr_crl_out): per CRL, and per entry of the listed CRLs."""
+    """Outputs of ctmr_revoked_known (include/ctmr.h ctmr_crl_out): per CRL, and per entry of the listed CRLs.
+    serial_len saturates at 255, so serial() of an entry whose serial has 256 or more octets (CTMR_RV_SERIAL_TOO_LONG,
+    never joined) returns only its first 255 octets; serial_off is exact."""
 
     _CRL = (("crl_status", np.uint8), ("crl_flags", np.uint8), ("this_update", np.int64), ("next_update", np.int64),
             ("tbs_off", np.uint64), ("tbs_len", np.uint32), ("issuer_name_off", np.uint64), ("issuer_name_len", np.uint32),

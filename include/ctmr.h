@@ -306,6 +306,8 @@ typedef struct ctmr_crl_out {                      /* caller-allocated, any poin
 } ctmr_crl_out;
 /* Per CRL: CTMR_CRL_BAD and CTMR_CRL_BAD_ENTRIES CRLs have no entries (crl_entries 0) and only crl_status is meaningful;
  * CTMR_CRL_OK and CTMR_CRL_UNKNOWN_ISSUER CRLs list every entry in order, entries of the CRLs back to back in CRL order.
+ * serial_len saturates at 255: a serial of 256 or more content octets (always CTMR_RV_SERIAL_TOO_LONG, never joined)
+ * reports 255, and its serial_off is still exact.
  * On a failed call (rc != 0) the outputs other than n_entries are undefined. */
 int ctmr_revoked_known(ctmr_ctx* ctx, const ctmr_crl_batch* batch, ctmr_crl_out* out);
 

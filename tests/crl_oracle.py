@@ -253,6 +253,7 @@ def parse_crl(d: bytes) -> dict:
         r["flags"] = 0
         return r
     r["status"] = CRL_OK
+    r["content"] = content  # the revokedCertificates content span, None when absent
     if content:  # the serial walk the GPU's split must agree with
         p, ce = content
         try:

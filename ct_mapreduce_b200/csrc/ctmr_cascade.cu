@@ -214,6 +214,22 @@ __global__ void __launch_bounds__(256) cascade_or_kernel(uint32_t* bits, const u
     if (i < words) bits[i] |= other[i];
 }
 
+// One process per GPU, a slice of the OR all-reduce.  Source side, grid (n / 256, world): words [0, n) of the rank's
+// bits into its region on every rank, its own among them (posted stores; the barrier after publishes them).
+__global__ void __launch_bounds__(256) cascade_peer_send_kernel(PeerExchange px, const uint32_t* __restrict__ bits, uint64_t n) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n) reinterpret_cast<uint32_t*>(px.inbox[blockIdx.y] + (uint64_t)px.rank * px.X)[j] = bits[j];
+}
+
+// Owner side, thread per word: the OR of every source's region, its own included, into words [0, n) of the rank's bits
+__global__ void __launch_bounds__(256) cascade_peer_or_kernel(PeerExchange px, uint32_t* bits, uint64_t n) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    uint32_t v = 0;
+    for (uint32_t s = 0; s < px.world; ++s) v |= __ldcg(reinterpret_cast<const uint32_t*>(px.inbox[px.rank] + (uint64_t)s * px.X) + j);
+    bits[j] = v;
+}
+
 inline unsigned grid(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
 }  // namespace
@@ -565,6 +581,246 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
     return CTMR_OK;
 }
 
+// ---- one process per GPU: the collective call on a ctx attached to peers (include/ctmr.h states the rules) -----------
+// Every rank checks its arguments and builds its buffers; agreement 1 posts its chunk count (or that it failed), and one
+// more mailbox word a hash of (now, salt), which must equal rank 0's.  Then:
+//   mark      the steps and rounds of the collective ctmr_revoked_known (crl_peer_each_set): in each round every rank
+//             marks its own shard against the union set of every rank's valid records of the round
+//   coverage  each rank's seen and bad bitmaps over dense indices from its own CRLs, OR-reduced; covered = seen & ~bad;
+//             each rank splits its own shard, and |R| and |S| are mailbox sums
+//   levels    each rank inserts its own include list into partial bits, the OR all-reduce merges them on every rank, each
+//             rank tests its own exclude list (level 1: S straight from its table); |F_l| is a mailbox sum, and every rank
+//             reads the merged level into its own image
+// The OR all-reduce goes through the parity-0 region of source `rank` on every rank, 16 X words a slice: the rank's words
+// of the slice into that region on every rank, a barrier, the OR of the world regions into the rank's bits, a barrier.
+// Every decision after agreement 1 is made from agreed sizes or from a mailbox row that every rank reads alike, so a rank
+// that failed still issues every barrier and exchange the others do.  A final agreement makes its failure every rank's,
+// and then a cap too small on any rank every rank's CTMR_E_BATCH_TOO_LARGE.
+
+int launched(ctmr_ctx* c) {
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
+}
+
+// the OR all-reduce of words [0, words) of every rank's bits, slice by slice; `work` false (this rank failed): the
+// barriers only
+int cascade_peer_or(ctmr_ctx* c, uint32_t* bits, uint64_t words, bool work) {
+    const uint64_t per = c->px.X * (sizeof(ctmr_key) / sizeof(uint32_t));
+    int rc = CTMR_OK;
+    for (uint64_t lo = 0; lo < words; lo += per) {
+        const uint64_t n = std::min(per, words - lo);
+        work = work && rc == CTMR_OK;
+        if (work) {
+            cascade_peer_send_kernel<<<dim3(grid(n, 256), c->px.world), 256, 0, c->stream>>>(c->px, bits + lo, n);
+            rc = launched(c);
+        }
+        int brc = peer_barrier(c, CH_CRL, c->stream);  // every region of the slice has landed
+        if (rc == CTMR_OK) rc = brc;
+        if (rc == CTMR_OK && work) {
+            cascade_peer_or_kernel<<<grid(n, 256), 256, 0, c->stream>>>(c->px, bits + lo, n);
+            rc = launched(c);
+        }
+        brc = peer_barrier(c, CH_CRL, c->stream);  // every rank has read the slice: the regions are free again
+        if (rc == CTMR_OK) rc = brc;
+    }
+    return rc;
+}
+
+// One mailbox exchange of this rank's payload, or of its failure.  false: some rank failed (every rank reads the same
+// row and goes to the final agreement); else *sum = the sum of the payloads.
+bool peer_sum(ctmr_ctx* c, PeerLocal& local, uint64_t mine, uint64_t* sum) {
+    uint64_t row[kMaxWorld] = {};
+    const int rc = peer_mailbox(c, peer_word(local.code, mine), row);
+    if (rc) {
+        local.fail(c, rc);
+        return false;
+    }
+    const uint32_t W = c->st.peer.world;
+    if (peer_row_failed(row, W) < W) return false;
+    *sum = 0;
+    for (uint32_t r = 0; r < W; ++r) *sum += row[r];
+    return true;
+}
+
+// 63 bits of FNV-1a over (now, salt_len, salt): equal on every rank that passes the same arguments
+uint64_t args_hash(int64_t now, const uint8_t* salt, uint32_t salt_len) {
+    uint64_t h = 14695981039346656037ull;
+    const auto put = [&](uint8_t v) { h = (h ^ v) * 1099511628211ull; };
+    for (int i = 0; i < 8; ++i) put((uint8_t)((uint64_t)now >> (8 * i)));
+    put((uint8_t)salt_len);
+    for (uint32_t j = 0; j < salt_len; ++j) put(salt[j]);
+    return h >> 1;
+}
+
+// this rank's part of the collective call
+int revoked_cascade_peer(ctmr_ctx* c, const ctmr_crl_batch* b, int64_t now, const uint8_t* salt, uint32_t salt_len, ctmr_cascade_out* out) {
+    const char* call = "ctmr_revoked_cascade: ";
+    CU(c, cudaSetDevice(c->device));
+    if (out) out->bytes = 0;
+    const uint32_t W = c->st.peer.world;
+    const uint64_t IW = c->st.max_issuers / 32 + 1;  // words of the seen bitmap, and of the bad one after it
+    std::vector<uint32_t> issuer;
+    uint64_t n_chunks = 0;
+    // everything that can fail before any work, allocations included, so that it travels in agreement 1
+    int rc = salt_len > kMaxSalt ? fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: salt_len > 32")
+             : salt_len && !salt ? fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: NULL salt")
+                                 : CTMR_OK;
+    if (rc == CTMR_OK) rc = crl_peer_prepare(c, b, out, call, issuer, &n_chunks);
+    if (rc == CTMR_OK) rc = cascade_ensure(c, 0, 2 * IW, false);
+    if (rc == CTMR_OK) rc = refresh_digests(c);
+    uint64_t row[kMaxWorld] = {};
+    rc = peer_agree(c, rc, n_chunks, row, call, "collective call failed");  // agreement 1
+    if (rc) return rc;
+    {  // now and salt define R, S and every bit: they must be rank 0's
+        uint64_t hrow[kMaxWorld] = {};
+        const uint64_t h = args_hash(now, salt, salt_len);
+        rc = peer_mailbox(c, h, hrow);
+        if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
+        if (rc) return rc;
+        if (h != hrow[0]) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: now_unix_sec or salt differs from rank 0's");
+        for (uint32_t r = 1; r < W; ++r)
+            if (hrow[r] != hrow[0])
+                return fail(c, CTMR_E_PEER_FAILED, "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s now_unix_sec or salt differs from rank 0's");
+    }
+    const uint32_t n_issuers = (uint32_t)c->digests.size();
+    ctmr_ctx* m[1] = {c};
+    Cascade cs{m, 1, nullptr};
+    cs.p.n_issuers = n_issuers;
+    cs.p.salt_len = salt_len;
+    cs.p.now = now;
+    for (uint32_t j = 0; j < salt_len; ++j) cs.p.salt[j >> 2] |= (uint32_t)salt[j] << (8 * (j & 3));
+    cs.p.one = 1;
+    cs.ml.assign(1, MemberLevel{});
+    CascadeState* s = c->cascade.get();
+    PeerLocal local;  // this rank's error after agreement 1: it does no more work, and the ranks stop at the next exchange
+    // the slot bits cleared, the registry's digests
+    local.fail(c, [&]() -> int {
+        CU(c, cudaMemsetAsync(s->revoked, 0, s->slot_words * 4, c->stream));
+        if (n_issuers) CU(c, cudaMemcpyAsync(s->dig, c->digests.data(), (size_t)n_issuers * 32, cudaMemcpyHostToDevice, c->stream));
+        return CTMR_OK;
+    }());
+    // mark: every round's union set against the own shard
+    std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
+    const bool going = crl_peer_each_set(c, b, issuer, row, [&](const CrlSetSlot* set, uint64_t mask) -> int {
+        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set, mask, s->revoked);
+        return launched(c);
+    }, crl_status, local);
+
+    std::vector<uint8_t> img;
+    uint32_t n_covered = 0, level = 0;
+    const auto build = [&]() {  // every return is one that all ranks take together, to the final agreement
+        if (!going) return;
+        // coverage: seen and bad bitmaps of the rank's own CRLs, OR-reduced over the ranks
+        std::vector<uint32_t> sb(2 * IW, 0);
+        for (uint64_t k = 0; k < b->n_crls; ++k) {
+            const uint32_t i = issuer[k];
+            if (i >= n_issuers) continue;
+            sb[i >> 5] |= 1u << (i & 31);
+            if (crl_status[k] != CTMR_CRL_OK) sb[IW + (i >> 5)] |= 1u << (i & 31);
+        }
+        if (!local.code) local.fail(c, [&]() -> int {
+            CU(c, cudaMemcpyAsync(s->bits, sb.data(), sb.size() * 4, cudaMemcpyHostToDevice, c->stream));
+            return CTMR_OK;
+        }());
+        local.fail(c, cascade_peer_or(c, s->bits, 2 * IW, !local.code));
+        std::vector<uint32_t> covered(n_issuers / 32 + 1, 0);
+        uint64_t nr = 0, ns = 0;
+        if (!local.code) local.fail(c, [&]() -> int {
+            CU(c, cudaMemcpyAsync(sb.data(), s->bits, sb.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+            CU(c, cudaStreamSynchronize(c->stream));
+            for (uint32_t i = 0; i < n_issuers; ++i)
+                if ((sb[i >> 5] & ~sb[IW + (i >> 5)]) >> (i & 31) & 1u) {
+                    covered[i >> 5] |= 1u << (i & 31);
+                    ++n_covered;
+                }
+            CU(c, cudaMemcpyAsync(s->covered, covered.data(), covered.size() * 4, cudaMemcpyHostToDevice, c->stream));
+            int rc2 = cs.split(0, s->list_cap, &nr, &ns);  // R and S of the own shard
+            if (rc2 == CTMR_OK && nr > s->list_cap) rc2 = cs.split(0, nr, &nr, &ns);
+            return rc2;
+        }());
+        if (!peer_sum(c, local, nr, &cs.R) || !peer_sum(c, local, ns, &cs.S)) return;
+        cs.ml[0].n_inc = nr;
+        cs.ml[0].n_exc = ns;
+
+        // the levels, each merged on every rank and read back into the image behind the header
+        img = {2, 0, 0, (uint8_t)salt_len};
+        img.insert(img.end(), salt, salt + salt_len);
+        uint64_t n_inc = cs.R;
+        for (;;) {
+            if (++level > kMaxLevels) {
+                local.fail(c, fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: more than 255 levels; build with another salt"));
+                return;
+            }
+            const double p = level == 1 ? (cs.R == 0 || cs.S == 0 ? 0.5 : std::min(0.5, (double)cs.R / (std::sqrt(2.0) * (double)cs.S))) : 0.5;
+            const LevelSize ls = level_size(n_inc, p);
+            if (ls.m >= 4294967296.0) {
+                local.fail(c, fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_cascade: level " + std::to_string(level) + " needs 2^32 bits or more"));
+                return;
+            }
+            const uint32_t mbits = (uint32_t)ls.m;
+            const uint64_t words = ((uint64_t)mbits + 31) / 32;
+            cs.p.level = level;
+            cs.p.k = ls.k;
+            cs.p.m = mbits;
+            if (!local.code) local.fail(c, cs.insert(words));  // the own include list into partial bits
+            local.fail(c, cascade_peer_or(c, s->bits, words, !local.code));
+            uint64_t f = 0;
+            if (!local.code) {
+                int rc2 = cs.test(0, &f);
+                if (rc2 == CTMR_OK && f > s->list_cap) {  // level 1 only: F_1 outgrew the lists, which hold R; make room and run again
+                    rc2 = cs.split(0, f, &nr, &ns);
+                    if (rc2 == CTMR_OK) rc2 = cs.test(0, &f);
+                }
+                local.fail(c, rc2);
+            }
+            uint64_t F = 0;
+            if (!peer_sum(c, local, f, &F)) return;
+            const uint64_t nbytes = ((uint64_t)mbits + 7) / 8;
+            const size_t at = img.size();
+            img.resize(at + 10 + nbytes);
+            img[at] = 2;
+            std::memcpy(&img[at + 1], &mbits, 4);
+            std::memcpy(&img[at + 5], &ls.k, 4);
+            img[at + 9] = (uint8_t)level;
+            if (!local.code) local.fail(c, [&]() -> int {
+                CU(c, cudaMemcpyAsync(&img[at + 10], s->bits, nbytes, cudaMemcpyDeviceToHost, c->stream));
+                CU(c, cudaStreamSynchronize(c->stream));
+                return CTMR_OK;
+            }());
+            if (F == 0) return;
+            MemberLevel& l = cs.ml[0];  // I_{l+1} = F_l, E_{l+1} = I_l
+            const uint32_t free_list = l.exc == kNoList ? 3 - l.inc - l.out : l.exc;
+            l.exc = l.inc;
+            l.n_exc = l.n_inc;
+            l.inc = l.out;
+            l.n_inc = f;
+            l.out = free_list;
+            n_inc = F;
+        }
+    };
+    build();
+
+    const cudaStream_t drain[] = {c->crl->copy_stream, c->stream};
+    drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
+    if (!local.code && (rc = ctmr_check_device(c, nullptr))) local.fail(c, rc);  // a barrier that timed out
+    if (local.code) c->err = local.err;
+    const bool short_cap = img.size() > out->cap || !out->buf;
+    rc = peer_agree(c, local.code, short_cap ? 1 : 0, row, call, "collective call failed");  // the final agreement
+    if (rc) return rc;
+    out->bytes = img.size();
+    for (uint32_t r = 0; r < W; ++r)
+        if (row[r])
+            return fail(c, CTMR_E_BATCH_TOO_LARGE, r == c->px.rank ? "ctmr_revoked_cascade: cap " + std::to_string(out->cap) + " < " + std::to_string(img.size()) + " bytes"
+                                                                  : "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s cap < " + std::to_string(img.size()) + " bytes");
+    std::memcpy(out->buf, img.data(), img.size());
+    if (out->crl_status) std::memcpy(out->crl_status, crl_status.data(), crl_status.size());
+    out->issuers = n_covered;
+    out->levels = level;
+    out->revoked = cs.R;
+    out->valid = cs.S;
+    return CTMR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -573,7 +829,7 @@ int ctmr_revoked_cascade(ctmr_ctx* c, const ctmr_crl_batch* batch, int64_t now_u
                          ctmr_cascade_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: a member of a group; use ctmr_group_revoked_cascade");
-    if (peer_call(c)) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: a ctx attached to peers has no collective form yet");
+    if (peer_call(c)) return revoked_cascade_peer(c, batch, now_unix_sec, salt, salt_len, out);
     ctmr_ctx* m[1] = {c};
     return revoked_cascade(m, 1, nullptr, batch, now_unix_sec, salt, salt_len, out);
 }

@@ -1033,10 +1033,22 @@ int crl_peer_owner(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uin
     return CTMR_OK;
 }
 
+// What a collective call does around the shared step and round driver (crl_peer_steps): ctmr_revoked_known answers
+// each rank's entries and pulls the answers back, ctmr_revoked_cascade marks its shard against each round's union set.
+struct CrlPeerActions {
+    std::function<bool(uint32_t ne)> send;  // the rank's chunk parsed with ne entries: does it send them (false: it only serves)
+    // the owner's part of a round, between its two barriers: agreed.n[s] records from source s, `total` in all, at most
+    // `most` from one source
+    std::function<int(const CrlRoundCounts& agreed, uint64_t most, uint64_t total)> owner;
+    std::function<int(uint64_t lo, uint64_t mine)> pull;  // after a round in which the rank sent entries [lo, lo + mine); may be empty
+    // after the rounds of the rank's own chunk `ch` (ne entries, parsed in stage[st]), whose last read of the stage is issued
+    std::function<int(const CrlChunk& ch, int st, uint32_t ne)> done;
+};
+
 // Round j of a step whose sent entries are row[0..world), this rank's chunk in stage[st].  `work` false (this rank
 // failed): nothing but the two barriers, which every rank issues whatever happens, so that a failure never leaves another
 // rank waiting.
-int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int st) {
+int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int st, const CrlPeerActions& a) {
     const uint64_t X = c->px.X, lo = j * X;
     const auto in_round = [&](uint64_t n) -> uint64_t { return n > lo ? std::min(X, n - lo) : 0; };
     CrlRoundCounts agreed{};
@@ -1050,15 +1062,56 @@ int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int 
     int rc = work ? crl_peer_send(c, st, lo, mine) : CTMR_OK;
     int brc = peer_barrier(c, CH_CRL, c->stream);
     if (rc == CTMR_OK) rc = brc;
-    if (rc == CTMR_OK && work && total) rc = crl_peer_owner(c, agreed, most, total);
+    if (rc == CTMR_OK && work && total) rc = a.owner(agreed, most, total);
     brc = peer_barrier(c, CH_CRL, c->stream);
     if (rc == CTMR_OK) rc = brc;
-    if (rc == CTMR_OK && work && mine) {
-        CrlState* s = c->crl.get();
-        crl_peer_pull_kernel<<<grid(mine, 256), 256, 0, c->stream>>>(c->px, mine, lo, s->eknown, s->ehour, s->esets);
-        CU(c, cudaGetLastError());
-    }
+    if (rc == CTMR_OK && work && mine && a.pull) rc = a.pull(lo, mine);
     return rc;
+}
+
+// The steps after agreement 1 (row: every rank's chunk count), up to the final agreement, which the caller makes after
+// draining the streams.  A failure of this rank goes to `local`; false: a rank's failure stopped the steps early (every
+// rank saw it in the same agreement 2), and the ranks go straight to the final agreement.
+bool crl_peer_steps(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const std::vector<CrlChunk>& chunks,
+                    uint64_t* row, const CrlPeerActions& a, PeerLocal& local) {
+    const uint32_t W = c->st.peer.world;
+    uint64_t steps = 0;
+    for (uint32_t r = 0; r < W; ++r) steps = std::max(steps, row[r]);
+    CrlState* s = c->crl.get();
+    int rc = CTMR_OK;
+    if (!chunks.empty() && !local.code && (rc = crl_upload(c, b, issuer, chunks[0], 0))) local.fail(c, rc);
+    for (uint64_t k = 0; k < steps; ++k) {
+        const int st = (int)(k & 1);
+        const bool mine = k < chunks.size() && !local.code;
+        uint32_t ne = 0;
+        uint64_t send = 0;
+        if (mine) {
+            rc = k + 1 < chunks.size() ? crl_upload(c, b, issuer, chunks[k + 1], st ^ 1) : CTMR_OK;
+            if (rc == CTMR_OK) rc = crl_split(c, chunks[k], st, &ne);
+            if (rc == CTMR_OK && a.send(ne) && ne) {
+                rc = crl_peer_entries(c, st, ne);
+                send = ne;
+            }
+            if (rc) local.fail(c, rc);
+        }
+        rc = peer_mailbox(c, peer_word(local.code, send), row);  // agreement 2
+        if (rc) {
+            local.fail(c, rc);
+            return false;
+        }
+        if (peer_row_failed(row, W) < W) return false;  // every rank saw the same row: all go to the final agreement
+        uint64_t most = 0;
+        for (uint32_t r = 0; r < W; ++r) most = std::max(most, row[r]);
+        for (uint64_t j = 0; j * c->px.X < most; ++j)  // the rounds build their records from the staged chunk
+            if ((rc = crl_peer_round(c, row, j, !local.code, st, a))) local.fail(c, rc);
+        if (!mine || local.code) continue;
+        if (cudaEventRecord(s->consumed[st], c->stream) != cudaSuccess) {  // the rounds' last read of stage[st] is issued
+            local.fail(c, fail(c, CTMR_E_CUDA, "cudaEventRecord failed"));
+            continue;
+        }
+        if ((rc = a.done(chunks[k], st, ne))) local.fail(c, rc);
+    }
+    return true;
 }
 
 // this rank's part of the collective call
@@ -1076,59 +1129,32 @@ int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) 
     uint64_t row[kMaxWorld] = {};
     rc = peer_agree(c, rc, chunks.size(), row, "ctmr_revoked_known: ", "collective call failed");  // agreement 1
     if (rc) return rc;
-    const uint32_t W = c->st.peer.world;
-    uint64_t steps = 0;
-    for (uint32_t r = 0; r < W; ++r) steps = std::max(steps, row[r]);
     CrlState* s = c->crl.get();
     uint64_t base = 0;
     bool count_only = false;  // entry_cap is exceeded: the rank still answers the others' records, and sends none of its own
-    int local = CTMR_OK;      // this rank's error after agreement 1: it does no more work, and the ranks stop at the next agreement
-    std::string local_err;
-    const auto fail_locally = [&](int code) {
-        if (local) return;
-        local = code;
-        local_err = c->err;
+    PeerLocal local;          // this rank's error after agreement 1: it does no more work, and the ranks stop at the next agreement
+    CrlPeerActions a;
+    a.send = [&](uint32_t ne) {
+        if (count_only || base + ne > out->entry_cap) count_only = true;
+        return !count_only;
     };
-    if (!chunks.empty() && (rc = crl_upload(c, b, issuer, chunks[0], 0))) fail_locally(rc);
-    for (uint64_t k = 0; k < steps; ++k) {
-        const int st = (int)(k & 1);
-        const bool mine = k < chunks.size() && !local;
-        uint32_t ne = 0;
-        uint64_t send = 0;
-        if (mine) {
-            rc = k + 1 < chunks.size() ? crl_upload(c, b, issuer, chunks[k + 1], st ^ 1) : CTMR_OK;
-            if (rc == CTMR_OK) rc = crl_split(c, chunks[k], st, &ne);
-            if (rc == CTMR_OK && (count_only || base + ne > out->entry_cap)) {
-                count_only = true;
-            } else if (rc == CTMR_OK && ne) {
-                rc = crl_peer_entries(c, st, ne);
-                send = ne;
-            }
-            if (rc) fail_locally(rc);
-        }
-        rc = peer_mailbox(c, peer_word(local, send), row);  // agreement 2
-        if (rc) {
-            fail_locally(rc);
-            break;
-        }
-        if (peer_row_failed(row, W) < W) break;  // every rank saw the same row: all go to the final agreement
-        uint64_t most = 0;
-        for (uint32_t r = 0; r < W; ++r) most = std::max(most, row[r]);
-        for (uint64_t j = 0; j * c->px.X < most; ++j)  // the rounds build their records from the staged chunk
-            if ((rc = crl_peer_round(c, row, j, !local, st))) fail_locally(rc);
-        if (!mine || local) continue;
-        if (cudaEventRecord(s->consumed[st], c->stream) != cudaSuccess) {  // the rounds' last read of stage[st] is issued
-            fail_locally(fail(c, CTMR_E_CUDA, "cudaEventRecord failed"));
-            continue;
-        }
-        if (!count_only && (rc = crl_copy_back(c, out, chunks[k], base, ne))) fail_locally(rc);
+    a.owner = [&](const CrlRoundCounts& agreed, uint64_t most, uint64_t total) { return crl_peer_owner(c, agreed, most, total); };
+    a.pull = [&](uint64_t lo, uint64_t mine) -> int {
+        crl_peer_pull_kernel<<<grid(mine, 256), 256, 0, c->stream>>>(c->px, mine, lo, s->eknown, s->ehour, s->esets);
+        CU(c, cudaGetLastError());
+        return CTMR_OK;
+    };
+    a.done = [&](const CrlChunk& ch, int, uint32_t ne) {
+        const int rc2 = count_only ? CTMR_OK : crl_copy_back(c, out, ch, base, ne);
         base += ne;
-    }
+        return rc2;
+    };
+    crl_peer_steps(c, b, issuer, chunks, row, a, local);
     const cudaStream_t drain[] = {s->copy_stream, c->stream};
     drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
-    if (!local && (rc = ctmr_check_device(c, nullptr))) fail_locally(rc);  // a barrier of a round that timed out
-    if (local) c->err = local_err;
-    rc = peer_agree(c, local, 0, row, "ctmr_revoked_known: ", "collective call failed");
+    if (!local.code && (rc = ctmr_check_device(c, nullptr))) local.fail(c, rc);  // a barrier of a round that timed out
+    if (local.code) c->err = local.err;
+    rc = peer_agree(c, local.code, 0, row, "ctmr_revoked_known: ", "collective call failed");
     if (rc) return rc;
     out->n_entries = base;
     if (count_only)
@@ -1169,6 +1195,42 @@ int crl_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_
         for (uint32_t k = 0; k < n; ++k) status[k] = (uint8_t)res[k].status;
         return visit(ch.lo, status, ne ? s->set.get() : nullptr, slots ? slots - 1 : 0);
     });
+}
+
+int crl_peer_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
+                     uint64_t* n_chunks) {
+    *n_chunks = 0;
+    int rc = crl_prepare(c, b, out, call, issuer);
+    if (rc == CTMR_OK) rc = crl_ensure(c);
+    if (rc == CTMR_OK) rc = crl_peer_ensure(c);
+    if (rc == CTMR_OK) *n_chunks = crl_cut(c, b).size();
+    return rc;
+}
+
+bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlUnionVisit& visit,
+                       std::vector<uint8_t>& status, PeerLocal& local) {
+    CrlState* s = c->crl.get();
+    const std::vector<CrlChunk> chunks = crl_cut(c, b);
+    std::vector<CrlRes> res;
+    CrlPeerActions a;
+    a.send = [](uint32_t) { return true; };
+    a.owner = [&](const CrlRoundCounts& agreed, uint64_t most, uint64_t total) -> int {  // the valid records of the round, then the visit
+        const cudaStream_t q = c->stream;
+        const uint64_t slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
+        CU(c, cudaMemsetAsync(s->union_set, 0, slots * sizeof(CrlSetSlot), q));
+        crl_union_insert_kernel<<<dim3(grid(most, 256), c->px.world), 256, 0, q>>>(c->px, agreed, s->union_set, slots - 1, c->in_slot);
+        CU(c, cudaGetLastError());
+        return visit(s->union_set, slots - 1);
+    };
+    a.done = [&](const CrlChunk& ch, int, uint32_t) -> int {
+        const uint32_t n = (uint32_t)(ch.hi - ch.lo);
+        res.resize(n);
+        CU(c, cudaMemcpyAsync(res.data(), s->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        for (uint32_t k = 0; k < n; ++k) status[ch.lo + k] = (uint8_t)res[k].status;
+        return CTMR_OK;
+    };
+    return crl_peer_steps(c, b, issuer, chunks, row, a, local);
 }
 
 }  // namespace ctmr_host

@@ -408,7 +408,8 @@ enum : uint32_t {
     CH_DEV_MAP = 6, CH_DEV_RESOLVE = 7,  // ctmr_process_device
     CH_USER = 8, CH_HIST_A = 9, CH_HIST_B = 10, CH_RESET_A = 11, CH_RESET_B = 12, CH_MAILBOX = 13,
     CH_CKPT = 14,                        // ctmr_checkpoint_*: every barrier and agreement of the collective size, save and load
-    CH_CRL = 15,                         // ctmr_revoked_known: the two barriers of each round of a collective call
+    CH_CRL = 15,                         // ctmr_revoked_known and ctmr_revoked_cascade: the two barriers of each round of a
+                                         // collective call, and of each slice of the cascade's OR all-reduce
     CH_STAGE_META = 16                   // + stage index (3): after the string-identity insert of a host-pipeline round
 };
 
@@ -615,6 +616,31 @@ int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const cha
 int crl_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit);
 // the set arrays for `slots` pairs (a power of two), all or nothing; `recv`: also the receive side of a group's member 0
 int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv);
+
+// A rank's own failure in a collective call after its first agreement: it does no more work but still meets every barrier
+// and agreement of the call, and the first failure's code and text are kept for the final agreement.
+struct PeerLocal {
+    int code = CTMR_OK;
+    std::string err;
+    void fail(const ctmr_ctx* c, int rc) {
+        if (code || rc == CTMR_OK) return;
+        code = rc;
+        err = c->err;
+    }
+};
+
+// ctmr_revoked_cascade's collective use of the CRL exchange (ctmr_crl.cu).  crl_peer_prepare: crl_prepare, then the
+// split's and the exchange's buffers and the number of chunks, so that every failure before any work travels in
+// agreement 1.  crl_peer_each_set: after agreement 1 (row: every rank's chunk count), the step and round driver of the
+// collective ctmr_revoked_known; in each round, visit(the union set of every rank's valid records of the round, mask)
+// is issued on c's stream between the round's two barriers, and status[] gets the CTMR_CRL_* of the rank's own CRLs.
+// This rank's failures go to `local`; false: a rank's failure stopped the steps, and the ranks go to the final agreement.
+// The caller drains c's streams (the copy stream too) before that agreement.
+using CrlUnionVisit = std::function<int(const CrlSetSlot*, uint64_t)>;
+int crl_peer_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
+                     uint64_t* n_chunks);
+bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlUnionVisit& visit,
+                       std::vector<uint8_t>& status, PeerLocal& local);
 
 // Where a table's live slots go when they are compacted in slot order (launch_evict_compact): the exclusive prefix of the
 // live slots per tile of kCompactTile, on the host and on the device.  host[tiles()] = the live slots of the table.

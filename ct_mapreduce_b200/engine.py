@@ -794,20 +794,28 @@ class GpuCertDatabase:
         .issuers, .levels, .revoked and .valid.
         The output buffer holds `cap` bytes; by default 16 MiB, or twice the last cascade this db built if that is more.
         A cascade larger than the buffer is built twice: the first build only reports its size (the library writes
-        nothing else when the buffer is too small), the second fills a buffer of that size."""
-        b, keep = _crl_batch(crls, issuer_digests)
-        salt = bytes(salt)
-        sbuf = (C.c_uint8 * max(len(salt), 1)).from_buffer_copy(salt or b"\0")
-        status = np.zeros(max(int(b.n_crls), 1), np.uint8)
-        size = int(cap) if cap is not None else max(16 << 20, 2 * self._cascade_bytes)
-        buf = np.empty(max(size, 1), np.uint8)
-        o = capi.CascadeOut(capi.ptr(buf), size, 0, capi.ptr(status))
+        nothing else when the buffer is too small), the second fills a buffer of that size.
+        On a db attached to peers the call is collective: every rank calls it with its own CRLs (an empty list will do) and
+        the same now_unix_sec and salt, and every rank gets the cascade of every rank's shard and every rank's CRLs, as
+        one db holding all the shards would build it from the ranks' CRLs in rank order; .crl_status covers the rank's own
+        CRLs.  A buffer too small on any rank is too small on every rank, so every rank builds it the second time together.
+        A rank whose arguments are refused here still makes the call, with no batch, so that the other ranks return
+        CTMR_E_PEER_FAILED, and then raises."""
         fn = self._revoked_cascade_fn()
-        rc = fn(self._h, C.byref(b), int(now_unix_sec), sbuf, len(salt), C.byref(o))
+        with self._peer_refusal(lambda: fn(self._h, None, 0, None, 0, None)):
+            b, keep = _crl_batch(crls, issuer_digests)
+            salt = bytes(salt)
+            sbuf = (C.c_uint8 * max(len(salt), 1)).from_buffer_copy(salt or b"\0")
+            status = np.zeros(max(int(b.n_crls), 1), np.uint8)
+            size = int(cap) if cap is not None else max(16 << 20, 2 * self._cascade_bytes)
+            buf = np.empty(max(size, 1), np.uint8)
+            o = capi.CascadeOut(capi.ptr(buf), size, 0, capi.ptr(status))
+            now_unix_sec = int(now_unix_sec)
+        rc = fn(self._h, C.byref(b), now_unix_sec, sbuf, len(salt), C.byref(o))
         if rc == capi.E_BATCH_TOO_LARGE and o.bytes:  # larger than the buffer: again into one of the size it reported
             buf = np.empty(int(o.bytes), np.uint8)
             o = capi.CascadeOut(capi.ptr(buf), buf.size, 0, capi.ptr(status))
-            rc = fn(self._h, C.byref(b), int(now_unix_sec), sbuf, len(salt), C.byref(o))
+            rc = fn(self._h, C.byref(b), now_unix_sec, sbuf, len(salt), C.byref(o))
         self._check(rc)
         self._cascade_bytes = int(o.bytes)
         return CascadeResult(buf[:o.bytes].tobytes(), status[:b.n_crls].copy(), o)

@@ -152,13 +152,17 @@ type Cascade struct {
 
 // RevokedCascade builds the filter cascade of the covered issuers' live known certificates on the GPU: the revoked
 // ones included, every other one excluded.  crls and issuerIDs as for RevokedKnown, verified CRLs only; salt is at most
-// 32 bytes.  Read-only.  A DB attached to peers has no collective form yet: the library refuses the call.  The output
-// buffer holds 16 MiB, or twice the DB's last cascade if that is more; a larger cascade is built twice (the first build
-// only reports its size).
+// 32 bytes.  Read-only.  The output buffer holds 16 MiB, or twice the DB's last cascade if that is more; a larger cascade
+// is built twice (the first build only reports its size).  On a DB attached to peers the call is collective: every rank
+// calls it with its own CRLs (none will do) and the same nowUnixSec and salt, and every rank gets the cascade of every
+// shard and every rank's CRLs; CRLStatus covers the rank's own CRLs.  A buffer too small on any rank is too small on
+// every rank, so every rank builds it the second time together.  A rank whose arguments are refused here still makes
+// the call, with no batch, so that the other ranks fail instead of waiting.
 func (d *DB) RevokedCascade(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int64, salt []byte) (*Cascade, error) {
 	n := len(crls)
 	if len(issuerIDs) < n {
-		return nil, fmt.Errorf("RevokedCascade: %d issuer IDs for %d CRLs", len(issuerIDs), n)
+		err := fmt.Errorf("RevokedCascade: %d issuer IDs for %d CRLs", len(issuerIDs), n)
+		return nil, d.peerRefuseWith(err, func() { C.ctmr_revoked_cascade(d.h, nil, 0, nil, 0, nil) })
 	}
 	total := 0
 	for _, c := range crls {

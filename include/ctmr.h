@@ -353,9 +353,30 @@ int ctmr_revoked_known(ctmr_ctx* ctx, const ctmr_crl_batch* batch, ctmr_crl_out*
  * may be NULL) the call returns CTMR_E_BATCH_TOO_LARGE and writes `bytes` and nothing else; a second call with that cap
  * returns exactly those bytes.  Read-only, like ctmr_revoked_known: no index is taken and no table, counter or registry
  * changes.  Argument checks are ctmr_revoked_known's (a NULL batch or output, a CRL outside data or larger than a chunk),
- * plus the salt's.  A member ctx of a group is refused with CTMR_E_INVALID (use ctmr_group_revoked_cascade), and so is a
- * ctx attached to peers (no collective form yet).  Cost: one pass over the table per CRL chunk, two more for level 1, and
- * device scratch of one bit per table slot plus the include lists and one level's bits (DESIGN.md "Revoked cascade"). */
+ * plus the salt's.  A member ctx of a group is refused with CTMR_E_INVALID (use ctmr_group_revoked_cascade).  Cost: one
+ * pass over the table per CRL chunk, two more for level 1, and device scratch of one bit per table slot plus the include
+ * lists and one level's bits (DESIGN.md "Revoked cascade").
+ *
+ * On a ctx attached to peers (world > 1) the call is COLLECTIVE: every rank makes it with its own batch, which may be
+ * empty (n_crls == 0), and every rank passes the same now_unix_sec and the same salt.  The result is what the call on one
+ * ctx would give that holds the union of every rank's table (every rank's checkpoint part loaded) and is passed the
+ * concatenated batch, rank 0's CRLs first, then rank 1's, and so on: bytes, buf, issuers, levels, revoked and valid are
+ * identical on every rank, and crl_status covers the rank's own CRLs.  Coverage is global: an issuer is covered when it
+ * is registered, its digest appears in some rank's batch, and every CRL of it in every rank's batch is CTMR_CRL_OK (a
+ * bad CRL on one rank uncovers its issuer on every rank); an issuer registered only by another rank is found, as in
+ * ctmr_revoked_known.  Read-only on every rank.  Failures follow ctmr_revoked_known's peer rules:
+ *   - the checks before any work (a NULL batch or output, a CRL outside data or larger than a chunk, salt_len > 32, a
+ *     NULL salt with salt_len > 0) run on every rank: a rank that fails one returns its error, the others return
+ *     CTMR_E_PEER_FAILED, and bytes is 0; nothing else is written;
+ *   - a now_unix_sec or salt not equal to rank 0's: that rank returns CTMR_E_INVALID and the others CTMR_E_PEER_FAILED,
+ *     before any work (R, S and every bit depend on them);
+ *   - a later failure on any rank (CUDA, an allocation, a barrier timeout) is every rank's; outputs are undefined;
+ *   - a cap too small on any rank (or a NULL buf) is CTMR_E_BATCH_TOO_LARGE on every rank, and every rank writes only
+ *     bytes, which is the same everywhere.  Unlike ctmr_revoked_known's entry_cap, which only affects its own rank: the
+ *     retry with the reported size is a collective call, so every rank retries together;
+ *   - m_l >= 2^32 and more than 255 levels are as above; the sizes are agreed, so every rank reaches them together.
+ * The collective form moves every rank's CRL entries to every rank through the exchange area and merges each level's
+ * bits with an OR all-reduce there; DESIGN.md "Revoked cascade" gives its cost. */
 typedef struct ctmr_cascade_out {   /* caller-allocated; HOST buffers */
     uint8_t* buf; uint64_t cap;     /* the serialized cascade */
     uint64_t bytes;                 /* written; on CTMR_E_BATCH_TOO_LARGE the bytes needed */

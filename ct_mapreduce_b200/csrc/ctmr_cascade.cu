@@ -295,15 +295,6 @@ int cascade_ensure(ctmr_ctx* c, uint64_t list_cap, uint64_t bit_words, bool recv
     return CTMR_OK;
 }
 
-// CU for the code that serves a group too: the failing ctx's error text also becomes the group's
-#define CUG(g, ctx, call)                                                                                                      \
-    do {                                                                                                                       \
-        const cudaError_t e_ = (call);                                                                                         \
-        if (e_ != cudaSuccess)                                                                                                 \
-            return group_fail((g), (ctx), fail((ctx), e_ == cudaErrorMemoryAllocation ? CTMR_E_NOMEM : CTMR_E_CUDA,             \
-                                               std::string(#call) + ": " + cudaGetErrorString(e_)));                           \
-    } while (0)
-
 // The sizing of include/ctmr.h, host IEEE double in exactly that order
 struct LevelSize {
     uint32_t k;
@@ -322,30 +313,36 @@ struct MemberLevel {
     uint64_t n_inc = 0, n_exc = 0;
 };
 
+// The work of a build on its W members.  The first failure goes to `local`, and run() skips every step after it (a peer
+// rank's exchanges still run).
 struct Cascade {
     ctmr_ctx* const* m;
     uint32_t W;
-    ctmr_group* g;
     CascadeParams p{};
     std::vector<MemberLevel> ml;
     uint64_t R = 0, S = 0;
+    PeerLocal local;
 
-    int gfail(ctmr_ctx* c, int rc) { return group_fail(g, c, rc); }
+    // f() on member c unless the call has failed; a failure of f is c's
+    template <class F>
+    void run(ctmr_ctx* c, F&& f) {
+        if (!local.code) local.fail(c, f());
+    }
 
     // member r's R list (list 0) and counts; the list grown first to `cap`
     int split(uint32_t r, uint64_t cap, uint64_t* nr, uint64_t* ns) {
         ctmr_ctx* c = m[r];
-        CUG(g, c, cudaSetDevice(c->device));
+        CU(c, cudaSetDevice(c->device));
         int rc = cascade_ensure(c, cap, 0, false);
         if (rc) return rc;
         CascadeState* s = c->cascade.get();
         CascadeParams q = params(c);
-        CUG(g, c, cudaMemsetAsync(s->counters, 0, 2 * sizeof(unsigned long long), c->stream));
+        CU(c, cudaMemsetAsync(s->counters, 0, 2 * sizeof(unsigned long long), c->stream));
         cascade_split_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(q, s->revoked, s->list[0], s->list_cap, s->counters);
-        CUG(g, c, cudaGetLastError());
+        CU(c, cudaGetLastError());
         unsigned long long h[2] = {0, 0};
-        CUG(g, c, cudaMemcpyAsync(h, s->counters, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
-        CUG(g, c, cudaStreamSynchronize(c->stream));
+        CU(c, cudaMemcpyAsync(h, s->counters, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
         *nr = h[0];
         *ns = h[1];
         return CTMR_OK;
@@ -363,11 +360,11 @@ struct Cascade {
     // member r's test of level p.level: F into its out list; *f = how many
     int test(uint32_t r, uint64_t* f) {
         ctmr_ctx* c = m[r];
-        CUG(g, c, cudaSetDevice(c->device));
+        CU(c, cudaSetDevice(c->device));
         CascadeState* s = c->cascade.get();
         const MemberLevel& l = ml[r];
         const CascadeParams q = params(c);
-        CUG(g, c, cudaMemsetAsync(s->counters, 0, sizeof(unsigned long long), c->stream));
+        CU(c, cudaMemsetAsync(s->counters, 0, sizeof(unsigned long long), c->stream));
         if (l.exc == kNoList) {
             cascade_test_table_kernel<<<c->sm_count * 8, kCascadeThreads, 0, c->stream>>>(q, s->revoked, s->bits, s->list[l.out], s->list_cap,
                                                                                          s->counters);
@@ -375,230 +372,66 @@ struct Cascade {
             cascade_test_kernel<<<grid(l.n_exc, kCascadeThreads), kCascadeThreads, 0, c->stream>>>(q, s->list[l.exc], l.n_exc, s->bits,
                                                                                                   s->list[l.out], s->list_cap, s->counters);
         }
-        CUG(g, c, cudaGetLastError());
+        CU(c, cudaGetLastError());
         unsigned long long h = 0;
-        CUG(g, c, cudaMemcpyAsync(&h, s->counters, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
-        CUG(g, c, cudaStreamSynchronize(c->stream));
+        CU(c, cudaMemcpyAsync(&h, s->counters, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
         *f = h;
         return CTMR_OK;
     }
 
-    // level p.level with words of bits: every member's partial bits, merged on member 0 and copied back to every member
-    int insert(uint64_t words) {
-        for (uint32_t r = 0; r < W; ++r) {
-            ctmr_ctx* c = m[r];
-            CUG(g, c, cudaSetDevice(c->device));
-            int rc = cascade_ensure(c, 0, words, r == 0 && W > 1);
-            if (rc) return gfail(c, rc);
-            CascadeState* s = c->cascade.get();
-            const CascadeParams q = params(c);
-            CUG(g, c, cudaMemsetAsync(s->bits, 0, words * 4, c->stream));
-            if (ml[r].n_inc) {
-                cascade_insert_kernel<<<grid(ml[r].n_inc, kCascadeThreads), kCascadeThreads, 0, c->stream>>>(q, s->list[ml[r].inc], ml[r].n_inc,
-                                                                                                            s->bits);
-                CUG(g, c, cudaGetLastError());
-            }
-        }
-        if (W == 1) return CTMR_OK;
-        ctmr_ctx* c0 = m[0];
-        CascadeState* s0 = c0->cascade.get();
-        for (uint32_t r = 1; r < W; ++r) {
-            ctmr_ctx* c = m[r];
-            CUG(g, c, cudaSetDevice(c->device));
-            CUG(g, c, cudaStreamSynchronize(c->stream));
-            CUG(g, c0, cudaSetDevice(c0->device));
-            CUG(g, c0, cudaMemcpyPeerAsync(s0->recv, c0->device, c->cascade->bits, c->device, words * 4, c0->stream));
-            cascade_or_kernel<<<grid(words, 256), 256, 0, c0->stream>>>(s0->bits, s0->recv, words);
-            CUG(g, c0, cudaGetLastError());
-        }
-        CUG(g, c0, cudaStreamSynchronize(c0->stream));
-        for (uint32_t r = 1; r < W; ++r) {
-            ctmr_ctx* c = m[r];
-            CUG(g, c, cudaSetDevice(c->device));
-            CUG(g, c, cudaMemcpyPeerAsync(c->cascade->bits, c->device, s0->bits, c0->device, words * 4, c->stream));
+    // member r's included records into its partial bits of level p.level, `words` of them
+    int insert(uint32_t r, uint64_t words) {
+        ctmr_ctx* c = m[r];
+        CU(c, cudaSetDevice(c->device));
+        const int rc = cascade_ensure(c, 0, words, r == 0 && W > 1);
+        if (rc) return rc;
+        CascadeState* s = c->cascade.get();
+        CU(c, cudaMemsetAsync(s->bits, 0, words * 4, c->stream));
+        if (ml[r].n_inc) {
+            cascade_insert_kernel<<<grid(ml[r].n_inc, kCascadeThreads), kCascadeThreads, 0, c->stream>>>(params(c), s->list[ml[r].inc],
+                                                                                                        ml[r].n_inc, s->bits);
+            CU(c, cudaGetLastError());
         }
         return CTMR_OK;
+    }
+
+    // a group's level (W > 1): member 0 pulls every other member's partial bits and ORs them into its own, then copies
+    // the merged level back to every member
+    void merge(uint64_t words) {
+        if (W == 1 || local.code) return;
+        ctmr_ctx *c0 = m[0], *at = c0;
+        CascadeState* s0 = c0->cascade.get();
+        const int rc = [&]() -> int {
+            for (uint32_t r = 1; r < W; ++r) {
+                ctmr_ctx* c = at = m[r];
+                CU(c, cudaSetDevice(c->device));
+                CU(c, cudaStreamSynchronize(c->stream));
+                at = c0;
+                CU(c0, cudaSetDevice(c0->device));
+                CU(c0, cudaMemcpyPeerAsync(s0->recv, c0->device, c->cascade->bits, c->device, words * 4, c0->stream));
+                cascade_or_kernel<<<grid(words, 256), 256, 0, c0->stream>>>(s0->bits, s0->recv, words);
+                CU(c0, cudaGetLastError());
+            }
+            CU(c0, cudaStreamSynchronize(c0->stream));
+            for (uint32_t r = 1; r < W; ++r) {
+                ctmr_ctx* c = at = m[r];
+                CU(c, cudaSetDevice(c->device));
+                CU(c, cudaMemcpyPeerAsync(c->cascade->bits, c->device, s0->bits, c0->device, words * 4, c->stream));
+            }
+            return CTMR_OK;
+        }();
+        local.fail(at, rc);
     }
 };
 
-// the call on member 0 of `W` members (W == 1: one ctx)
-int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, int64_t now, const uint8_t* salt,
-                    uint32_t salt_len, ctmr_cascade_out* out) {
-    ctmr_ctx* c0 = m[0];
-    const auto gf = [&](ctmr_ctx* c, int rc) { return group_fail(g, c, rc); };
-    CUG(g, c0, cudaSetDevice(c0->device));
-    if (salt_len > kMaxSalt) return gf(c0, fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: salt_len > 32"));
-    if (salt_len && !salt) return gf(c0, fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: NULL salt"));
-    std::vector<uint32_t> issuer;
-    int rc = crl_prepare(c0, b, out, "ctmr_revoked_cascade: ", issuer);
-    if (rc) return gf(c0, rc);
-    if ((rc = refresh_digests(c0))) return gf(c0, rc);
-    const uint32_t n_issuers = (uint32_t)c0->digests.size();
-
-    Cascade cs{m, W, g};
-    cs.p.n_issuers = n_issuers;
-    cs.p.salt_len = salt_len;
-    cs.p.now = now;
-    for (uint32_t j = 0; j < salt_len; ++j) cs.p.salt[j >> 2] |= (uint32_t)salt[j] << (8 * (j & 3));
-    cs.p.one = 1;
-    cs.ml.assign(W, MemberLevel{});
-
-    // every member's scratch, its slot bits cleared, the registry's digests
-    for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = m[r];
-        CUG(g, c, cudaSetDevice(c->device));
-        if ((rc = cascade_ensure(c, 0, 0, false))) return gf(c, rc);
-        CascadeState* s = c->cascade.get();
-        CUG(g, c, cudaMemsetAsync(s->revoked, 0, s->slot_words * 4, c->stream));
-        if (n_issuers) CUG(g, c, cudaMemcpyAsync(s->dig, c0->digests.data(), (size_t)n_issuers * 32, cudaMemcpyHostToDevice, c->stream));
-        CUG(g, c, cudaStreamSynchronize(c->stream));
-    }
-
-    // the chunks: member 0 builds each chunk's set, every member marks its own shard against it
-    std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
-    CUG(g, c0, cudaSetDevice(c0->device));
-    uint32_t at = 0;  // the member the chunk path is working on: a failure's text is on it
-    rc = crl_each_set(c0, b, issuer, [&](uint64_t lo, const std::vector<uint8_t>& st, const CrlSetSlot* set, uint64_t mask) -> int {
-        std::copy(st.begin(), st.end(), crl_status.begin() + lo);
-        if (!set) return CTMR_OK;
-        for (uint32_t r = 0; r < W; ++r) {
-            ctmr_ctx* c = m[at = r];
-            CUG(g, c, cudaSetDevice(c->device));
-            const CrlSetSlot* probe = set;
-            if (r) {
-                int rc2 = crl_set_ensure(c, mask + 1, false);
-                if (rc2) return gf(c, rc2);
-                CUG(g, c, cudaMemcpyPeerAsync(c->crl->set, c->device, set, c0->device, (mask + 1) * sizeof(CrlSetSlot), c->stream));
-                probe = c->crl->set;
-            }
-            cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, probe, mask, c->cascade->revoked);
-            CUG(g, c, cudaGetLastError());
-        }
-        for (uint32_t r = W; r-- > 1;) {  // the next chunk rewrites member 0's set
-            at = r;
-            CUG(g, m[r], cudaSetDevice(m[r]->device));
-            CUG(g, m[r], cudaStreamSynchronize(m[r]->stream));
-        }
-        at = 0;
-        CUG(g, c0, cudaSetDevice(c0->device));
-        return CTMR_OK;
-    });
-    if (rc) return gf(m[at], rc);
-
-    // coverage: every CRL of an issuer in the batch is CTMR_CRL_OK
-    std::vector<uint8_t> seen(n_issuers, 0), bad(n_issuers, 0);
-    for (uint64_t k = 0; k < b->n_crls; ++k) {
-        if (issuer[k] >= n_issuers) continue;
-        seen[issuer[k]] = 1;
-        if (crl_status[k] != CTMR_CRL_OK) bad[issuer[k]] = 1;
-    }
-    std::vector<uint32_t> covered(n_issuers / 32 + 1, 0);
-    uint32_t n_covered = 0;
-    for (uint32_t i = 0; i < n_issuers; ++i)
-        if (seen[i] && !bad[i]) {
-            covered[i >> 5] |= 1u << (i & 31);
-            ++n_covered;
-        }
-
-    // R and S: each member's R list and counts
-    for (uint32_t r = 0; r < W; ++r) {
-        ctmr_ctx* c = m[r];
-        CUG(g, c, cudaSetDevice(c->device));
-        CUG(g, c, cudaMemcpyAsync(c->cascade->covered, covered.data(), covered.size() * 4, cudaMemcpyHostToDevice, c->stream));
-        uint64_t nr = 0, ns = 0;
-        if ((rc = cs.split(r, c->cascade->list_cap, &nr, &ns))) return gf(c, rc);
-        if (nr > c->cascade->list_cap && (rc = cs.split(r, nr, &nr, &ns))) return gf(c, rc);
-        cs.ml[r].n_inc = nr;
-        cs.ml[r].n_exc = ns;
-        cs.R += nr;
-        cs.S += ns;
-    }
-
-    // the levels, each read back into the image behind the header
-    std::vector<uint8_t> img = {2, 0, 0, (uint8_t)salt_len};
-    img.insert(img.end(), salt, salt + salt_len);
-    uint64_t n_inc = cs.R;
-    uint32_t level = 0;
-    std::vector<uint64_t> fr(W, 0);  // each member's F_l
-    for (;;) {
-        if (++level > kMaxLevels)
-            return gf(c0, fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: more than 255 levels; build with another salt"));
-        const double p = level == 1 ? (cs.R == 0 || cs.S == 0 ? 0.5 : std::min(0.5, (double)cs.R / (std::sqrt(2.0) * (double)cs.S))) : 0.5;
-        const LevelSize ls = level_size(n_inc, p);
-        if (ls.m >= 4294967296.0) {
-            out->bytes = 0;
-            return gf(c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_cascade: level " + std::to_string(level) + " needs 2^32 bits or more"));
-        }
-        const uint32_t mbits = (uint32_t)ls.m;
-        const uint64_t words = ((uint64_t)mbits + 31) / 32;
-        cs.p.level = level;
-        cs.p.k = ls.k;
-        cs.p.m = mbits;
-        if ((rc = cs.insert(words))) return rc;
-        uint64_t F = 0;
-        for (uint32_t r = 0; r < W; ++r) {
-            uint64_t& f = fr[r];
-            if ((rc = cs.test(r, &f))) return gf(m[r], rc);
-            if (f > m[r]->cascade->list_cap) {  // level 1 only: F_1 outgrew the lists, which hold R; make room and run again
-                uint64_t nr = 0, ns = 0;
-                if ((rc = cs.split(r, f, &nr, &ns)) || (rc = cs.test(r, &f))) return gf(m[r], rc);
-            }
-            F += f;
-        }
-        const uint64_t nbytes = ((uint64_t)mbits + 7) / 8;
-        const size_t at = img.size();
-        img.resize(at + 10 + nbytes);
-        img[at] = 2;
-        std::memcpy(&img[at + 1], &mbits, 4);
-        std::memcpy(&img[at + 5], &ls.k, 4);
-        img[at + 9] = (uint8_t)level;
-        CUG(g, c0, cudaSetDevice(c0->device));
-        CUG(g, c0, cudaMemcpyAsync(&img[at + 10], c0->cascade->bits, nbytes, cudaMemcpyDeviceToHost, c0->stream));
-        CUG(g, c0, cudaStreamSynchronize(c0->stream));
-        if (F == 0) break;
-        for (uint32_t r = 0; r < W; ++r) {  // I_{l+1} = F_l, E_{l+1} = I_l
-            MemberLevel& l = cs.ml[r];
-            const uint32_t free_list = l.exc == kNoList ? 3 - l.inc - l.out : l.exc;
-            l.exc = l.inc;
-            l.n_exc = l.n_inc;
-            l.inc = l.out;
-            l.n_inc = fr[r];
-            l.out = free_list;
-        }
-        n_inc = F;
-    }
-    CUG(g, c0, cudaSetDevice(c0->device));
-    out->bytes = img.size();
-    if (img.size() > out->cap || !out->buf)
-        return gf(c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_cascade: cap " + std::to_string(out->cap) + " < " +
-                                                           std::to_string(img.size()) + " bytes"));
-    std::memcpy(out->buf, img.data(), img.size());
-    if (out->crl_status) std::memcpy(out->crl_status, crl_status.data(), crl_status.size());
-    out->issuers = n_covered;
-    out->levels = level;
-    out->revoked = cs.R;
-    out->valid = cs.S;
+int launched(ctmr_ctx* c) {
+    CU(c, cudaGetLastError());
     return CTMR_OK;
 }
 
-// ---- one process per GPU: the collective call on a ctx attached to peers (include/ctmr.h states the rules) -----------
-// Every rank checks its arguments and builds its buffers; agreement 1 posts its chunk count (or that it failed), and one
-// more mailbox word a hash of (now, salt), which must equal rank 0's.  Then:
-//   mark      the steps and rounds of the collective ctmr_revoked_known (crl_peer_each_set): in each round every rank
-//             marks its own shard against the union set of every rank's valid records of the round
-//   coverage  each rank's seen and bad bitmaps over dense indices from its own CRLs, OR-reduced; covered = seen & ~bad;
-//             each rank splits its own shard, and |R| and |S| are mailbox sums
-//   levels    each rank inserts its own include list into partial bits, the OR all-reduce merges them on every rank, each
-//             rank tests its own exclude list (level 1: S straight from its table); |F_l| is a mailbox sum, and every rank
-//             reads the merged level into its own image
-// The OR all-reduce goes through the parity-0 region of source `rank` on every rank, 16 X words a slice: the rank's words
-// of the slice into that region on every rank, a barrier, the OR of the world regions into the rank's bits, a barrier.
-// Every decision after agreement 1 is made from agreed sizes or from a mailbox row that every rank reads alike, so a rank
-// that failed still issues every barrier and exchange the others do.  A final agreement makes its failure every rank's,
-// and then a cap too small on any rank every rank's CTMR_E_BATCH_TOO_LARGE.
-
-int launched(ctmr_ctx* c) {
-    CU(c, cudaGetLastError());
+int set_device(ctmr_ctx* c) {
+    CU(c, cudaSetDevice(c->device));
     return CTMR_OK;
 }
 
@@ -642,119 +475,177 @@ bool peer_sum(ctmr_ctx* c, PeerLocal& local, uint64_t mine, uint64_t* sum) {
     return true;
 }
 
-// 63 bits of FNV-1a over (now, salt_len, salt): equal on every rank that passes the same arguments
-uint64_t args_hash(int64_t now, const uint8_t* salt, uint32_t salt_len) {
+// now and salt define R, S and every bit, so every rank's must be rank 0's: one mailbox word each, 63 bits of FNV-1a over
+// (now, salt_len, salt)
+int peer_same_args(ctmr_ctx* c, int64_t now, const uint8_t* salt, uint32_t salt_len) {
     uint64_t h = 14695981039346656037ull;
     const auto put = [&](uint8_t v) { h = (h ^ v) * 1099511628211ull; };
     for (int i = 0; i < 8; ++i) put((uint8_t)((uint64_t)now >> (8 * i)));
     put((uint8_t)salt_len);
     for (uint32_t j = 0; j < salt_len; ++j) put(salt[j]);
-    return h >> 1;
+    h >>= 1;
+    uint64_t row[kMaxWorld] = {};
+    int rc = peer_mailbox(c, h, row);
+    if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
+    if (rc) return rc;
+    if (h != row[0]) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: now_unix_sec or salt differs from rank 0's");
+    for (uint32_t r = 1; r < c->st.peer.world; ++r)
+        if (row[r] != row[0])
+            return fail(c, CTMR_E_PEER_FAILED, "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s now_unix_sec or salt differs from rank 0's");
+    return CTMR_OK;
 }
 
-// this rank's part of the collective call
-int revoked_cascade_peer(ctmr_ctx* c, const ctmr_crl_batch* b, int64_t now, const uint8_t* salt, uint32_t salt_len, ctmr_cascade_out* out) {
+// ---- the call ---------------------------------------------------------------------------------------------------------
+// One driver builds the cascade on the members this process holds: a group's W members, one ctx (W == 1), or one rank
+// of a group of processes (W == 1; the call is collective, include/ctmr.h states the rules).  The phases run in the same
+// order in every form, and only these steps differ:
+//   checks    one ctx or a group: the arguments and crl_prepare, and a failure returns at once.  A peer rank: the same
+//             checks and every allocation of the call, carried in agreement 1 with the rank's chunk count; then one more
+//             mailbox word, a hash of (now, salt), which must equal rank 0's.
+//   mark      one ctx or a group: member 0 builds each chunk's set, and every member marks its shard against its copy of
+//             it (crl_each_set).  A peer rank: the steps and rounds of the collective ctmr_revoked_known
+//             (crl_peer_each_set); in each round the rank marks its shard against the union set of every rank's valid
+//             records of the round.
+//   coverage  seen and bad bitmaps over dense indices from the CRLs' statuses (peer ranks: each from its own CRLs, then
+//             OR-reduced over the ranks); covered = seen & ~bad
+//   counts    |R|, |S| and |F_l| are sums over the members, or mailbox sums over the ranks
+//   merge     each member inserts its own include list into partial bits; a group's member 0 pulls them, ORs them
+//             (cascade_or) and copies the merged level back; peer ranks OR-reduce them on every rank (cascade_peer_or)
+//   finish    one ctx or a group: the cap check.  A peer rank: the streams drained and a final agreement, which makes a
+//             failure on any rank every rank's, and then a cap too small on any rank every rank's CTMR_E_BATCH_TOO_LARGE.
+// The OR all-reduce goes through the parity-0 region of source `rank` on every rank, 16 X words a slice: the rank's words
+// of the slice into that region on every rank, a barrier, the OR of the world regions into the rank's bits, a barrier.
+// One ctx or a group stops at its first failure.  A peer rank that failed after agreement 1 does no more work, but every
+// decision is made from agreed sizes or from a mailbox row that every rank reads alike, so it still issues every barrier
+// and exchange the others do.
+int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, int64_t now, const uint8_t* salt,
+                    uint32_t salt_len, ctmr_cascade_out* out) {
+    ctmr_ctx* c0 = m[0];
+    const bool peer = peer_call(c0);
     const char* call = "ctmr_revoked_cascade: ";
-    CU(c, cudaSetDevice(c->device));
-    if (out) out->bytes = 0;
-    const uint32_t W = c->st.peer.world;
-    const uint64_t IW = c->st.max_issuers / 32 + 1;  // words of the seen bitmap, and of the bad one after it
+    int rc = set_device(c0);
+    if (rc) return group_fail(g, c0, rc);
+    if (peer && out) out->bytes = 0;
+    const uint64_t IW = c0->st.max_issuers / 32 + 1;  // words of the seen bitmap, and of the bad one after it
     std::vector<uint32_t> issuer;
-    uint64_t n_chunks = 0;
-    // everything that can fail before any work, allocations included, so that it travels in agreement 1
-    int rc = salt_len > kMaxSalt ? fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: salt_len > 32")
-             : salt_len && !salt ? fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: NULL salt")
+    uint64_t n_chunks = 0, row[kMaxWorld] = {};
+    rc = salt_len > kMaxSalt ? fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: salt_len > 32")
+             : salt_len && !salt ? fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: NULL salt")
                                  : CTMR_OK;
-    if (rc == CTMR_OK) rc = crl_peer_prepare(c, b, out, call, issuer, &n_chunks);
-    if (rc == CTMR_OK) rc = cascade_ensure(c, 0, 2 * IW, false);
-    if (rc == CTMR_OK) rc = refresh_digests(c);
-    uint64_t row[kMaxWorld] = {};
-    rc = peer_agree(c, rc, n_chunks, row, call, "collective call failed");  // agreement 1
-    if (rc) return rc;
-    {  // now and salt define R, S and every bit: they must be rank 0's
-        uint64_t hrow[kMaxWorld] = {};
-        const uint64_t h = args_hash(now, salt, salt_len);
-        rc = peer_mailbox(c, h, hrow);
-        if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
-        if (rc) return rc;
-        if (h != hrow[0]) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: now_unix_sec or salt differs from rank 0's");
-        for (uint32_t r = 1; r < W; ++r)
-            if (hrow[r] != hrow[0])
-                return fail(c, CTMR_E_PEER_FAILED, "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s now_unix_sec or salt differs from rank 0's");
-    }
-    const uint32_t n_issuers = (uint32_t)c->digests.size();
-    ctmr_ctx* m[1] = {c};
-    Cascade cs{m, 1, nullptr};
+    if (rc == CTMR_OK) rc = peer ? crl_peer_prepare(c0, b, out, call, issuer, &n_chunks) : crl_prepare(c0, b, out, call, issuer);
+    if (rc == CTMR_OK && peer) rc = cascade_ensure(c0, 0, 2 * IW, false);
+    if (rc == CTMR_OK) rc = refresh_digests(c0);
+    if (peer && (rc = peer_agree(c0, rc, n_chunks, row, call, "collective call failed")) == CTMR_OK)  // agreement 1
+        rc = peer_same_args(c0, now, salt, salt_len);
+    if (rc) return group_fail(g, c0, rc);
+
+    const uint32_t n_issuers = (uint32_t)c0->digests.size();
+    Cascade cs{m, W};
     cs.p.n_issuers = n_issuers;
     cs.p.salt_len = salt_len;
     cs.p.now = now;
     for (uint32_t j = 0; j < salt_len; ++j) cs.p.salt[j >> 2] |= (uint32_t)salt[j] << (8 * (j & 3));
     cs.p.one = 1;
-    cs.ml.assign(1, MemberLevel{});
-    CascadeState* s = c->cascade.get();
-    PeerLocal local;  // this rank's error after agreement 1: it does no more work, and the ranks stop at the next exchange
-    // the slot bits cleared, the registry's digests
-    local.fail(c, [&]() -> int {
-        CU(c, cudaMemsetAsync(s->revoked, 0, s->slot_words * 4, c->stream));
-        if (n_issuers) CU(c, cudaMemcpyAsync(s->dig, c->digests.data(), (size_t)n_issuers * 32, cudaMemcpyHostToDevice, c->stream));
-        return CTMR_OK;
-    }());
-    // mark: every round's union set against the own shard
-    std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
-    const bool going = crl_peer_each_set(c, b, issuer, row, [&](const CrlSetSlot* set, uint64_t mask) -> int {
-        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set, mask, s->revoked);
-        return launched(c);
-    }, crl_status, local);
+    cs.ml.assign(W, MemberLevel{});
+    PeerLocal& local = cs.local;
 
+    // every member's scratch, its slot bits cleared, the registry's digests
+    for (uint32_t r = 0; r < W; ++r)
+        cs.run(m[r], [&, c = m[r]]() -> int {
+            CU(c, cudaSetDevice(c->device));
+            const int rc2 = cascade_ensure(c, 0, 0, false);
+            if (rc2) return rc2;
+            CascadeState* s = c->cascade.get();
+            CU(c, cudaMemsetAsync(s->revoked, 0, s->slot_words * 4, c->stream));
+            if (n_issuers) CU(c, cudaMemcpyAsync(s->dig, c0->digests.data(), (size_t)n_issuers * 32, cudaMemcpyHostToDevice, c->stream));
+            CU(c, cudaStreamSynchronize(c->stream));
+            return CTMR_OK;
+        });
+
+    // mark: every member's shard against each chunk's set, or a peer rank's against each round's union set
+    std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
+    const CrlSetVisit mark = [&](ctmr_ctx* c, const CrlSetSlot* set, uint64_t mask) -> int {
+        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set, mask, c->cascade->revoked);
+        return launched(c);
+    };
+    bool going = peer ? crl_peer_each_set(c0, b, issuer, row, mark, crl_status, local) : !local.code;
+    if (!peer && going) {
+        ctmr_ctx* at = c0;
+        rc = crl_each_set(m, W, b, issuer, mark, crl_status, &at);
+        local.fail(at, rc);
+        going = rc == CTMR_OK;
+    }
+
+    // a count summed over the members, or over the ranks; false: the build stops (it failed here, or on a peer rank)
+    const auto total = [&](const std::vector<uint64_t>& v, uint64_t* sum) {
+        if (peer) return peer_sum(c0, local, v[0], sum);
+        *sum = 0;
+        for (const uint64_t x : v) *sum += x;
+        return !local.code;
+    };
     std::vector<uint8_t> img;
     uint32_t n_covered = 0, level = 0;
-    const auto build = [&]() {  // every return is one that all ranks take together, to the final agreement
+    const auto build = [&]() {  // every return is one that all peer ranks take together, to the finish
         if (!going) return;
-        // coverage: seen and bad bitmaps of the rank's own CRLs, OR-reduced over the ranks
-        std::vector<uint32_t> sb(2 * IW, 0);
+        // coverage: every CRL of an issuer in the batch is CTMR_CRL_OK
+        std::vector<uint32_t> sb(2 * IW, 0);  // seen, then bad
         for (uint64_t k = 0; k < b->n_crls; ++k) {
             const uint32_t i = issuer[k];
             if (i >= n_issuers) continue;
             sb[i >> 5] |= 1u << (i & 31);
             if (crl_status[k] != CTMR_CRL_OK) sb[IW + (i >> 5)] |= 1u << (i & 31);
         }
-        if (!local.code) local.fail(c, [&]() -> int {
-            CU(c, cudaMemcpyAsync(s->bits, sb.data(), sb.size() * 4, cudaMemcpyHostToDevice, c->stream));
-            return CTMR_OK;
-        }());
-        local.fail(c, cascade_peer_or(c, s->bits, 2 * IW, !local.code));
+        if (peer) {
+            uint32_t* bits = c0->cascade->bits;
+            cs.run(c0, [&]() -> int {
+                CU(c0, cudaMemcpyAsync(bits, sb.data(), sb.size() * 4, cudaMemcpyHostToDevice, c0->stream));
+                return CTMR_OK;
+            });
+            local.fail(c0, cascade_peer_or(c0, bits, 2 * IW, !local.code));
+            cs.run(c0, [&]() -> int {
+                CU(c0, cudaMemcpyAsync(sb.data(), bits, sb.size() * 4, cudaMemcpyDeviceToHost, c0->stream));
+                CU(c0, cudaStreamSynchronize(c0->stream));
+                return CTMR_OK;
+            });
+        }
         std::vector<uint32_t> covered(n_issuers / 32 + 1, 0);
-        uint64_t nr = 0, ns = 0;
-        if (!local.code) local.fail(c, [&]() -> int {
-            CU(c, cudaMemcpyAsync(sb.data(), s->bits, sb.size() * 4, cudaMemcpyDeviceToHost, c->stream));
-            CU(c, cudaStreamSynchronize(c->stream));
-            for (uint32_t i = 0; i < n_issuers; ++i)
-                if ((sb[i >> 5] & ~sb[IW + (i >> 5)]) >> (i & 31) & 1u) {
-                    covered[i >> 5] |= 1u << (i & 31);
-                    ++n_covered;
-                }
-            CU(c, cudaMemcpyAsync(s->covered, covered.data(), covered.size() * 4, cudaMemcpyHostToDevice, c->stream));
-            int rc2 = cs.split(0, s->list_cap, &nr, &ns);  // R and S of the own shard
-            if (rc2 == CTMR_OK && nr > s->list_cap) rc2 = cs.split(0, nr, &nr, &ns);
-            return rc2;
-        }());
-        if (!peer_sum(c, local, nr, &cs.R) || !peer_sum(c, local, ns, &cs.S)) return;
-        cs.ml[0].n_inc = nr;
-        cs.ml[0].n_exc = ns;
+        for (uint32_t i = 0; i < n_issuers; ++i)
+            if ((sb[i >> 5] & ~sb[IW + (i >> 5)]) >> (i & 31) & 1u) {
+                covered[i >> 5] |= 1u << (i & 31);
+                ++n_covered;
+            }
 
-        // the levels, each merged on every rank and read back into the image behind the header
+        // R and S: each member's R list and counts
+        std::vector<uint64_t> nr(W, 0), ns(W, 0);
+        for (uint32_t r = 0; r < W; ++r)
+            cs.run(m[r], [&, c = m[r]]() -> int {
+                CU(c, cudaSetDevice(c->device));
+                CU(c, cudaMemcpyAsync(c->cascade->covered, covered.data(), covered.size() * 4, cudaMemcpyHostToDevice, c->stream));
+                int rc2 = cs.split(r, c->cascade->list_cap, &nr[r], &ns[r]);
+                if (rc2 == CTMR_OK && nr[r] > c->cascade->list_cap) rc2 = cs.split(r, nr[r], &nr[r], &ns[r]);
+                return rc2;
+            });
+        if (!total(nr, &cs.R) || !total(ns, &cs.S)) return;
+        for (uint32_t r = 0; r < W; ++r) {
+            cs.ml[r].n_inc = nr[r];
+            cs.ml[r].n_exc = ns[r];
+        }
+
+        // the levels, each merged and read back into the image behind the header
         img = {2, 0, 0, (uint8_t)salt_len};
         img.insert(img.end(), salt, salt + salt_len);
         uint64_t n_inc = cs.R;
+        std::vector<uint64_t> fr(W, 0);  // each member's F_l
         for (;;) {
             if (++level > kMaxLevels) {
-                local.fail(c, fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: more than 255 levels; build with another salt"));
+                local.fail(c0, fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: more than 255 levels; build with another salt"));
                 return;
             }
             const double p = level == 1 ? (cs.R == 0 || cs.S == 0 ? 0.5 : std::min(0.5, (double)cs.R / (std::sqrt(2.0) * (double)cs.S))) : 0.5;
             const LevelSize ls = level_size(n_inc, p);
             if (ls.m >= 4294967296.0) {
-                local.fail(c, fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_cascade: level " + std::to_string(level) + " needs 2^32 bits or more"));
+                out->bytes = 0;
+                local.fail(c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_cascade: level " + std::to_string(level) + " needs 2^32 bits or more"));
                 return;
             }
             const uint32_t mbits = (uint32_t)ls.m;
@@ -762,19 +653,21 @@ int revoked_cascade_peer(ctmr_ctx* c, const ctmr_crl_batch* b, int64_t now, cons
             cs.p.level = level;
             cs.p.k = ls.k;
             cs.p.m = mbits;
-            if (!local.code) local.fail(c, cs.insert(words));  // the own include list into partial bits
-            local.fail(c, cascade_peer_or(c, s->bits, words, !local.code));
-            uint64_t f = 0;
-            if (!local.code) {
-                int rc2 = cs.test(0, &f);
-                if (rc2 == CTMR_OK && f > s->list_cap) {  // level 1 only: F_1 outgrew the lists, which hold R; make room and run again
-                    rc2 = cs.split(0, f, &nr, &ns);
-                    if (rc2 == CTMR_OK) rc2 = cs.test(0, &f);
-                }
-                local.fail(c, rc2);
-            }
+            for (uint32_t r = 0; r < W; ++r) cs.run(m[r], [&] { return cs.insert(r, words); });
+            if (peer) local.fail(c0, cascade_peer_or(c0, c0->cascade->bits, words, !local.code));
+            else cs.merge(words);
+            for (uint32_t r = 0; r < W; ++r)
+                cs.run(m[r], [&]() -> int {
+                    int rc2 = cs.test(r, &fr[r]);
+                    if (rc2 == CTMR_OK && fr[r] > m[r]->cascade->list_cap) {  // level 1 only: F_1 outgrew the lists, which hold R; make room and run again
+                        uint64_t nr2 = 0, ns2 = 0;
+                        rc2 = cs.split(r, fr[r], &nr2, &ns2);
+                        if (rc2 == CTMR_OK) rc2 = cs.test(r, &fr[r]);
+                    }
+                    return rc2;
+                });
             uint64_t F = 0;
-            if (!peer_sum(c, local, f, &F)) return;
+            if (!total(fr, &F)) return;
             const uint64_t nbytes = ((uint64_t)mbits + 7) / 8;
             const size_t at = img.size();
             img.resize(at + 10 + nbytes);
@@ -782,36 +675,48 @@ int revoked_cascade_peer(ctmr_ctx* c, const ctmr_crl_batch* b, int64_t now, cons
             std::memcpy(&img[at + 1], &mbits, 4);
             std::memcpy(&img[at + 5], &ls.k, 4);
             img[at + 9] = (uint8_t)level;
-            if (!local.code) local.fail(c, [&]() -> int {
-                CU(c, cudaMemcpyAsync(&img[at + 10], s->bits, nbytes, cudaMemcpyDeviceToHost, c->stream));
-                CU(c, cudaStreamSynchronize(c->stream));
+            cs.run(c0, [&]() -> int {
+                CU(c0, cudaSetDevice(c0->device));
+                CU(c0, cudaMemcpyAsync(&img[at + 10], c0->cascade->bits, nbytes, cudaMemcpyDeviceToHost, c0->stream));
+                CU(c0, cudaStreamSynchronize(c0->stream));
                 return CTMR_OK;
-            }());
-            if (F == 0) return;
-            MemberLevel& l = cs.ml[0];  // I_{l+1} = F_l, E_{l+1} = I_l
-            const uint32_t free_list = l.exc == kNoList ? 3 - l.inc - l.out : l.exc;
-            l.exc = l.inc;
-            l.n_exc = l.n_inc;
-            l.inc = l.out;
-            l.n_inc = f;
-            l.out = free_list;
+            });
+            if (F == 0 || (local.code && !peer)) return;  // one ctx or a group stops at its first failure
+            for (uint32_t r = 0; r < W; ++r) {  // I_{l+1} = F_l, E_{l+1} = I_l
+                MemberLevel& l = cs.ml[r];
+                const uint32_t free_list = l.exc == kNoList ? 3 - l.inc - l.out : l.exc;
+                l.exc = l.inc;
+                l.n_exc = l.n_inc;
+                l.inc = l.out;
+                l.n_inc = fr[r];
+                l.out = free_list;
+            }
             n_inc = F;
         }
     };
     build();
 
-    const cudaStream_t drain[] = {c->crl->copy_stream, c->stream};
-    drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
-    if (!local.code && (rc = ctmr_check_device(c, nullptr))) local.fail(c, rc);  // a barrier that timed out
-    if (local.code) c->err = local.err;
     const bool short_cap = img.size() > out->cap || !out->buf;
-    rc = peer_agree(c, local.code, short_cap ? 1 : 0, row, call, "collective call failed");  // the final agreement
-    if (rc) return rc;
+    if (peer) {
+        const cudaStream_t drain[] = {c0->crl->copy_stream, c0->stream};
+        drain_streams(c0, drain, 2);  // no upload may read the caller's data after the call
+        if (!local.code && (rc = ctmr_check_device(c0, nullptr))) local.fail(c0, rc);  // a barrier that timed out
+        if (local.code) c0->err = local.err;
+        rc = peer_agree(c0, local.code, short_cap ? 1 : 0, row, call, "collective call failed");  // the final agreement
+        if (rc) return rc;
+    } else {
+        if (local.code) {
+            if (g) g->err = local.err;  // the failing member's text is the group's
+            return local.code;
+        }
+        row[0] = short_cap;  // as the only rank
+    }
     out->bytes = img.size();
-    for (uint32_t r = 0; r < W; ++r)
+    const uint32_t world = peer ? c0->st.peer.world : 1, me = peer ? c0->px.rank : 0;
+    for (uint32_t r = 0; r < world; ++r)
         if (row[r])
-            return fail(c, CTMR_E_BATCH_TOO_LARGE, r == c->px.rank ? "ctmr_revoked_cascade: cap " + std::to_string(out->cap) + " < " + std::to_string(img.size()) + " bytes"
-                                                                  : "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s cap < " + std::to_string(img.size()) + " bytes");
+            return group_fail(g, c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, r == me ? "ctmr_revoked_cascade: cap " + std::to_string(out->cap) + " < " + std::to_string(img.size()) + " bytes"
+                                                                             : "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s cap < " + std::to_string(img.size()) + " bytes"));
     std::memcpy(out->buf, img.data(), img.size());
     if (out->crl_status) std::memcpy(out->crl_status, crl_status.data(), crl_status.size());
     out->issuers = n_covered;
@@ -829,7 +734,6 @@ int ctmr_revoked_cascade(ctmr_ctx* c, const ctmr_crl_batch* batch, int64_t now_u
                          ctmr_cascade_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: a member of a group; use ctmr_group_revoked_cascade");
-    if (peer_call(c)) return revoked_cascade_peer(c, batch, now_unix_sec, salt, salt_len, out);
     ctmr_ctx* m[1] = {c};
     return revoked_cascade(m, 1, nullptr, batch, now_unix_sec, salt, salt_len, out);
 }

@@ -616,10 +616,8 @@ int crl_ensure(ctmr_ctx* c) {
     return CTMR_OK;
 }
 
-}  // namespace
-
 // the set arrays for `slots` pairs (a power of two), all or nothing; `recv`: also the receive side of a group's member 0
-int ctmr_host::crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
+int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
     if (!c->crl) {
         c->crl.reset(new (std::nothrow) CrlState());
         if (!c->crl) return fail(c, CTMR_E_NOMEM, "host allocation failed");
@@ -645,8 +643,6 @@ int ctmr_host::crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv) {
     s->set_cap = cap;
     return CTMR_OK;
 }
-
-namespace {
 
 // A rank attached to peers, after crl_ensure: the records of one round (X) and the union set of a round (2 world X
 // slots, so that a free slot always exists), all or nothing
@@ -704,6 +700,14 @@ int crl_upload(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>
     return CTMR_OK;
 }
 
+// A group's member c (its device current) gets a bulk copy of the `slots` slots of member 0's set, on c's stream
+int crl_set_copy(ctmr_ctx* c0, ctmr_ctx* c, uint64_t slots) {
+    const int rc = crl_set_ensure(c, slots, false);
+    if (rc) return rc;
+    CU(c, cudaMemcpyPeerAsync(c->crl->set, c->device, c0->crl->set, c0->device, slots * sizeof(CrlSetSlot), c->stream));
+    return CTMR_OK;
+}
+
 // The other members' part of a group's join: each scans its own table against a bulk copy of member 0's set, and member 0
 // merges the answers.  Synchronous; no atomics cross GPUs.
 int crl_scan_members(ctmr_ctx* const* m, uint32_t W, uint64_t slots, ctmr_group* g) {
@@ -713,10 +717,9 @@ int crl_scan_members(ctmr_ctx* const* m, uint32_t W, uint64_t slots, ctmr_group*
     for (uint32_t r = 1; r < W; ++r) {
         ctmr_ctx* c = m[r];
         CU(c, cudaSetDevice(c->device));
-        int rc = crl_set_ensure(c, slots, false);
+        const int rc = crl_set_copy(c0, c, slots);
         if (rc) return group_fail(g, c, rc);
         CrlState* s = c->crl.get();
-        CU(c, cudaMemcpyPeerAsync(s->set, c->device, s0->set, c0->device, slots * sizeof(CrlSetSlot), c->stream));
         CU(c, cudaMemsetAsync(s->set_hour, 0x7f, slots * sizeof(int32_t), c->stream));
         CU(c, cudaMemsetAsync(s->set_count, 0, slots * sizeof(uint32_t), c->stream));
         const uint64_t n_slots = c->st.table_mask + 1;
@@ -1014,20 +1017,30 @@ int crl_peer_send(ctmr_ctx* c, int st, uint64_t lo, uint64_t n) {
     return CTMR_OK;
 }
 
-// the owner's part of a round: agreed.n[s] records from source s, `total` of them, at most `most` from one source
+// The union set of a round's valid records (agreed.n[s] from source s, `total` of them, at most `most` from one source),
+// cleared and filled on c's stream; *slots = its slots
+int crl_union_build(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uint64_t total, uint64_t* slots) {
+    CrlState* s = c->crl.get();
+    *slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
+    CU(c, cudaMemsetAsync(s->union_set, 0, *slots * sizeof(CrlSetSlot), c->stream));
+    crl_union_insert_kernel<<<dim3(grid(most, 256), c->px.world), 256, 0, c->stream>>>(c->px, agreed, s->union_set, *slots - 1, c->in_slot);
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
+}
+
+// the owner's part of a round: the union set, then every record's answer from the own shard
 int crl_peer_owner(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uint64_t total) {
     CrlState* s = c->crl.get();
     const cudaStream_t q = c->stream;
-    const uint64_t slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
-    CU(c, cudaMemsetAsync(s->union_set, 0, slots * sizeof(CrlSetSlot), q));
+    uint64_t slots = 0;
+    const int rc = crl_union_build(c, agreed, most, total, &slots);
+    if (rc) return rc;
     CU(c, cudaMemsetAsync(s->union_hour, 0x7f, slots * sizeof(int32_t), q));
     CU(c, cudaMemsetAsync(s->union_count, 0, slots * sizeof(uint32_t), q));
-    const dim3 g(grid(most, 256), c->px.world);
-    crl_union_insert_kernel<<<g, 256, 0, q>>>(c->px, agreed, s->union_set, slots - 1, c->in_slot);
-    CU(c, cudaGetLastError());
     crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->union_set, slots - 1, s->union_hour,
                                                           s->union_count);
     CU(c, cudaGetLastError());
+    const dim3 g(grid(most, 256), c->px.world);
     crl_peer_answer_kernel<<<g, 256, 0, q>>>(c->px, agreed, c->in_slot, s->union_hour, s->union_count);
     CU(c, cudaGetLastError());
     return CTMR_OK;
@@ -1163,6 +1176,16 @@ int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) 
     return CTMR_OK;
 }
 
+// the CTMR_CRL_* of chunk ch's CRLs, parsed on c, into status[ch.lo, ch.hi); waits for c's stream
+int crl_read_status(ctmr_ctx* c, const CrlChunk& ch, std::vector<uint8_t>& status) {
+    const uint32_t n = (uint32_t)(ch.hi - ch.lo);
+    std::vector<CrlRes> res(n);
+    CU(c, cudaMemcpyAsync(res.data(), c->crl->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    for (uint32_t k = 0; k < n; ++k) status[ch.lo + k] = (uint8_t)res[k].status;
+    return CTMR_OK;
+}
+
 }  // namespace
 
 // ---- the chunk path as ctmr_revoked_cascade uses it (ctmr_cascade.cu) -------------------------------------------------
@@ -1174,26 +1197,32 @@ int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const cha
     return rc;
 }
 
-int crl_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit) {
+int crl_each_set(ctmr_ctx* const* m, uint32_t W, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit,
+                 std::vector<uint8_t>& status, ctmr_ctx** failed) {
+    ctmr_ctx* c0 = *failed = m[0];
     if (b->n_crls == 0) return CTMR_OK;
-    std::vector<CrlRes> res;
-    std::vector<uint8_t> status;
-    return crl_for_chunks(c, b, issuer, [&](const CrlChunk& ch, int st) -> int {
-        CrlState* s = c->crl.get();
-        const cudaStream_t q = c->stream;
+    return crl_for_chunks(c0, b, issuer, [&](const CrlChunk& ch, int st) -> int {
         uint32_t ne = 0;
         uint64_t slots = 0;
-        int rc = crl_split(c, ch, st, &ne);
-        if (rc == CTMR_OK && ne) rc = crl_set_build(c, st, ne, false, &slots);
+        int rc = crl_split(c0, ch, st, &ne);
+        if (rc == CTMR_OK && ne) rc = crl_set_build(c0, st, ne, false, &slots);
         if (rc) return rc;
-        CU(c, cudaEventRecord(s->consumed[st], q));
-        const uint32_t n = (uint32_t)(ch.hi - ch.lo);
-        res.resize(n);
-        CU(c, cudaMemcpyAsync(res.data(), s->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, q));
-        CU(c, cudaStreamSynchronize(q));
-        status.resize(n);
-        for (uint32_t k = 0; k < n; ++k) status[k] = (uint8_t)res[k].status;
-        return visit(ch.lo, status, ne ? s->set.get() : nullptr, slots ? slots - 1 : 0);
+        CU(c0, cudaEventRecord(c0->crl->consumed[st], c0->stream));
+        if ((rc = crl_read_status(c0, ch, status)) || !ne) return rc;
+        for (uint32_t r = 0; r < W; ++r) {
+            ctmr_ctx* c = *failed = m[r];
+            CU(c, cudaSetDevice(c->device));
+            if (r && (rc = crl_set_copy(c0, c, slots))) return rc;
+            if ((rc = visit(c, c->crl->set, slots - 1))) return rc;
+        }
+        for (uint32_t r = W; r-- > 1;) {  // the next chunk rewrites member 0's set
+            ctmr_ctx* c = *failed = m[r];
+            CU(c, cudaSetDevice(c->device));
+            CU(c, cudaStreamSynchronize(c->stream));
+        }
+        *failed = c0;
+        CU(c0, cudaSetDevice(c0->device));
+        return CTMR_OK;
     });
 }
 
@@ -1207,30 +1236,17 @@ int crl_peer_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, cons
     return rc;
 }
 
-bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlUnionVisit& visit,
+bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlSetVisit& visit,
                        std::vector<uint8_t>& status, PeerLocal& local) {
-    CrlState* s = c->crl.get();
-    const std::vector<CrlChunk> chunks = crl_cut(c, b);
-    std::vector<CrlRes> res;
     CrlPeerActions a;
     a.send = [](uint32_t) { return true; };
-    a.owner = [&](const CrlRoundCounts& agreed, uint64_t most, uint64_t total) -> int {  // the valid records of the round, then the visit
-        const cudaStream_t q = c->stream;
-        const uint64_t slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
-        CU(c, cudaMemsetAsync(s->union_set, 0, slots * sizeof(CrlSetSlot), q));
-        crl_union_insert_kernel<<<dim3(grid(most, 256), c->px.world), 256, 0, q>>>(c->px, agreed, s->union_set, slots - 1, c->in_slot);
-        CU(c, cudaGetLastError());
-        return visit(s->union_set, slots - 1);
+    a.owner = [&](const CrlRoundCounts& agreed, uint64_t most, uint64_t total) -> int {
+        uint64_t slots = 0;
+        const int rc = crl_union_build(c, agreed, most, total, &slots);
+        return rc ? rc : visit(c, c->crl->union_set, slots - 1);
     };
-    a.done = [&](const CrlChunk& ch, int, uint32_t) -> int {
-        const uint32_t n = (uint32_t)(ch.hi - ch.lo);
-        res.resize(n);
-        CU(c, cudaMemcpyAsync(res.data(), s->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, c->stream));
-        CU(c, cudaStreamSynchronize(c->stream));
-        for (uint32_t k = 0; k < n; ++k) status[ch.lo + k] = (uint8_t)res[k].status;
-        return CTMR_OK;
-    };
-    return crl_peer_steps(c, b, issuer, chunks, row, a, local);
+    a.done = [&](const CrlChunk& ch, int, uint32_t) { return crl_read_status(c, ch, status); };
+    return crl_peer_steps(c, b, issuer, crl_cut(c, b), row, a, local);
 }
 
 }  // namespace ctmr_host

@@ -608,14 +608,15 @@ int clear_issuer_memos(ctmr_ctx* c);
 
 // ctmr_revoked_cascade's use of the CRL path (ctmr_crl.cu).  crl_prepare: ctmr_revoked_known's checks before any work
 // (`out` is only tested for NULL; `call` opens the error text), then each CRL's dense issuer (CTMR_ISSUER_NONE when the
-// digest is not registered).  crl_each_set: every chunk through the split, the entries and the set of its (issuer,
-// serial) pairs on c's stream; after each, visit(first CRL of the chunk, CTMR_CRL_* of its CRLs, the set or NULL when the
-// chunk has no entries, mask) while the set is intact.  Synchronous; no upload outlives it.
-using CrlSetVisit = std::function<int(uint64_t, const std::vector<uint8_t>&, const CrlSetSlot*, uint64_t)>;
+// digest is not registered).  crl_each_set, on member 0 of W members (a group, or one ctx): every chunk through the
+// split, the entries and the set of its (issuer, serial) pairs, and status[] gets the CTMR_CRL_* of its CRLs; then each
+// member, its device current, gets visit(member, a copy of the set on its device (member 0: the set), mask) on its
+// stream while the set is intact (a chunk with no entries: no visit).  Synchronous; no upload outlives it.  On error
+// *failed names the member that failed.
+using CrlSetVisit = std::function<int(ctmr_ctx* c, const CrlSetSlot* set, uint64_t mask)>;
 int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer);
-int crl_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit);
-// the set arrays for `slots` pairs (a power of two), all or nothing; `recv`: also the receive side of a group's member 0
-int crl_set_ensure(ctmr_ctx* c, uint64_t slots, bool recv);
+int crl_each_set(ctmr_ctx* const* m, uint32_t W, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit,
+                 std::vector<uint8_t>& status, ctmr_ctx** failed);
 
 // A rank's own failure in a collective call after its first agreement: it does no more work but still meets every barrier
 // and agreement of the call, and the first failure's code and text are kept for the final agreement.
@@ -632,14 +633,13 @@ struct PeerLocal {
 // ctmr_revoked_cascade's collective use of the CRL exchange (ctmr_crl.cu).  crl_peer_prepare: crl_prepare, then the
 // split's and the exchange's buffers and the number of chunks, so that every failure before any work travels in
 // agreement 1.  crl_peer_each_set: after agreement 1 (row: every rank's chunk count), the step and round driver of the
-// collective ctmr_revoked_known; in each round, visit(the union set of every rank's valid records of the round, mask)
+// collective ctmr_revoked_known; in each round, visit(c, the union set of every rank's valid records of the round, mask)
 // is issued on c's stream between the round's two barriers, and status[] gets the CTMR_CRL_* of the rank's own CRLs.
 // This rank's failures go to `local`; false: a rank's failure stopped the steps, and the ranks go to the final agreement.
 // The caller drains c's streams (the copy stream too) before that agreement.
-using CrlUnionVisit = std::function<int(const CrlSetSlot*, uint64_t)>;
 int crl_peer_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
                      uint64_t* n_chunks);
-bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlUnionVisit& visit,
+bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlSetVisit& visit,
                        std::vector<uint8_t>& status, PeerLocal& local);
 
 // Where a table's live slots go when they are compacted in slot order (launch_evict_compact): the exclusive prefix of the

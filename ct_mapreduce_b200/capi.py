@@ -52,6 +52,7 @@ EXPORTS = [
     "ctmr_next_index",
     "ctmr_revoked_known", "ctmr_group_revoked_known",   # CRLs joined with the known-certificate sets
     "ctmr_revoked_cascade", "ctmr_group_revoked_cascade",   # CRLite's filter cascade of the covered issuers
+    "ctmr_revoked_stash", "ctmr_group_revoked_stash",   # CRLite's stash: what a published filter and its stashes miss
 ]
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -172,6 +173,13 @@ class CascadeOut(C.Structure):
 
 
 CASCADE_MAX_SALT = 32   # salt_len of ctmr_revoked_cascade
+
+
+class StashOut(C.Structure):
+    """ctmr_stash_out (include/ctmr.h)."""
+    _fields_ = [("buf", C.c_void_p), ("cap", C.c_uint64), ("bytes", C.c_uint64), ("crl_status", C.c_void_p),
+                ("issuers", C.c_uint32), ("stash_issuers", C.c_uint32), ("revoked", C.c_uint64), ("in_filter", C.c_uint64),
+                ("in_stashes", C.c_uint64), ("serials", C.c_uint64)]
 
 
 class SynthCfg(C.Structure):
@@ -311,6 +319,8 @@ def load():
     L.ctmr_group_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
     L.ctmr_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
     L.ctmr_group_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
+    L.ctmr_revoked_stash.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u64, vp, u64, C.POINTER(StashOut)]
+    L.ctmr_group_revoked_stash.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u64, vp, u64, C.POINTER(StashOut)]
     for name in EXPORTS:
         getattr(L, name)  # every symbol include/ctmr.h declares must resolve
     _lib = L

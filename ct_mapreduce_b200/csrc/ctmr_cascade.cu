@@ -10,7 +10,12 @@
 //   cascade_test     thread per excluded record (level 1: grid-stride over the table for S): hashes until the first
 //                    clear bit; a record the level contains goes to the next include list
 // The host reads one count per level, sizes the next level and reads each finished level back.
+// ctmr_revoked_stash / ctmr_group_revoked_stash share the work up to the split (cascade_front), then
+//   stash_query      thread per R record: the published filter's query; the records it misses go to the host
+#include <algorithm>
 #include <cmath>
+#include <string>
+#include <unordered_set>
 
 #include "ctmr_common.cuh"
 #include "ctmr_ctx.cuh"
@@ -230,6 +235,38 @@ __global__ void __launch_bounds__(256) cascade_peer_or_kernel(PeerExchange px, u
     bits[j] = v;
 }
 
+// ctmr_revoked_stash, thread per record of the R list: the published filter's query (p: its salt; levels[l]: level l + 1's
+// first word in `words`, m and k).  The message is built once and only its level byte changes between levels.  A record
+// the filter calls revoked is counted in counters[1]; the key body words 1..11 of any other go to `bodies`, which holds
+// n of them, at counters[0].
+__global__ void __launch_bounds__(kCascadeThreads) stash_query_kernel(CascadeParams p, const uint32_t* __restrict__ list, uint64_t n,
+                                                                      const uint32_t* __restrict__ words, const StashLevel* __restrict__ levels,
+                                                                      uint32_t n_levels, uint32_t* bodies, unsigned long long* counters) {
+    __shared__ uint32_t smem[32 * kCascadeThreads];
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    uint32_t b[12];
+    load_body(p.table, list[t], b);
+    CascadeMsg msg{smem + threadIdx.x, 0u};
+    msg.build(p, b);
+    uint32_t l = 0;
+    for (; l < n_levels; ++l) {
+        const StashLevel lv = levels[l];
+        p.m = lv.m;
+        p.k = lv.k;
+        msg.put(p.salt_len + 4u, l + 1u);
+        if (!contains(p, msg, words + lv.word)) break;
+    }
+    // stopped at level l + 1: revoked iff that number is even; contained in all: iff n_levels is odd
+    if (l < n_levels ? (l & 1u) : (n_levels & 1u)) {
+        atomicAdd(counters + 1, 1ull);
+        return;
+    }
+    uint32_t* o = bodies + 11ull * atomicAdd(counters, 1ull);
+#pragma unroll
+    for (int j = 0; j < 11; ++j) o[j] = b[1 + j];
+}
+
 inline unsigned grid(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
 
 }  // namespace
@@ -318,6 +355,7 @@ struct MemberLevel {
 struct Cascade {
     ctmr_ctx* const* m;
     uint32_t W;
+    bool peer;  // one rank of a group of processes (W == 1)
     CascadeParams p{};
     std::vector<MemberLevel> ml;
     uint64_t R = 0, S = 0;
@@ -495,6 +533,102 @@ int peer_same_args(ctmr_ctx* c, int64_t now, const uint8_t* salt, uint32_t salt_
     return CTMR_OK;
 }
 
+// a count summed over the members, or over the ranks; false: the build stops (it failed here, or on a peer rank)
+bool cascade_total(Cascade& cs, const std::vector<uint64_t>& v, uint64_t* sum) {
+    if (cs.peer) return peer_sum(cs.m[0], cs.local, v[0], sum);
+    *sum = 0;
+    for (const uint64_t x : v) *sum += x;
+    return !cs.local.code;
+}
+
+// The front half of the cascade, which the stash shares: every member's scratch (slot bits cleared, the registry's
+// digests), the mark, the coverage and the split.  cs.p holds n_issuers, now and the salt; issuer[] is each CRL's dense
+// issuer, row agreement 1's row (peer ranks).  Afterwards crl_status[] holds each CRL's status, *n_covered the covered
+// issuers, cs.R and cs.S the sizes, and each member's R list is list 0 (ml[r].n_inc records; n_exc: its |S|).  false:
+// the build stops (it failed here, or on a peer rank).
+bool cascade_front(Cascade& cs, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row,
+                   std::vector<uint8_t>& crl_status, uint32_t* n_covered) {
+    ctmr_ctx* const* m = cs.m;
+    ctmr_ctx* c0 = m[0];
+    const uint32_t W = cs.W, n_issuers = cs.p.n_issuers;
+    const bool peer = cs.peer;
+    const int64_t now = cs.p.now;
+    const uint64_t IW = c0->st.max_issuers / 32 + 1;  // words of the seen bitmap, and of the bad one after it
+    PeerLocal& local = cs.local;
+
+    // every member's scratch, its slot bits cleared, the registry's digests
+    for (uint32_t r = 0; r < W; ++r)
+        cs.run(m[r], [&, c = m[r]]() -> int {
+            CU(c, cudaSetDevice(c->device));
+            const int rc2 = cascade_ensure(c, 0, 0, false);
+            if (rc2) return rc2;
+            CascadeState* s = c->cascade.get();
+            CU(c, cudaMemsetAsync(s->revoked, 0, s->slot_words * 4, c->stream));
+            if (n_issuers) CU(c, cudaMemcpyAsync(s->dig, c0->digests.data(), (size_t)n_issuers * 32, cudaMemcpyHostToDevice, c->stream));
+            CU(c, cudaStreamSynchronize(c->stream));
+            return CTMR_OK;
+        });
+
+    // mark: every member's shard against each chunk's set, or a peer rank's against each round's union set
+    const CrlSetVisit mark = [&](ctmr_ctx* c, const CrlSetSlot* set, uint64_t mask) -> int {
+        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set, mask, c->cascade->revoked);
+        return launched(c);
+    };
+    bool going = peer ? crl_peer_each_set(c0, b, issuer, row, mark, crl_status, local) : !local.code;
+    if (!peer && going) {
+        ctmr_ctx* at = c0;
+        const int rc = crl_each_set(m, W, b, issuer, mark, crl_status, &at);
+        local.fail(at, rc);
+        going = rc == CTMR_OK;
+    }
+    if (!going) return false;
+
+    // coverage: every CRL of an issuer in the batch is CTMR_CRL_OK
+    std::vector<uint32_t> sb(2 * IW, 0);  // seen, then bad
+    for (uint64_t k = 0; k < b->n_crls; ++k) {
+        const uint32_t i = issuer[k];
+        if (i >= n_issuers) continue;
+        sb[i >> 5] |= 1u << (i & 31);
+        if (crl_status[k] != CTMR_CRL_OK) sb[IW + (i >> 5)] |= 1u << (i & 31);
+    }
+    if (peer) {
+        uint32_t* bits = c0->cascade->bits;
+        cs.run(c0, [&]() -> int {
+            CU(c0, cudaMemcpyAsync(bits, sb.data(), sb.size() * 4, cudaMemcpyHostToDevice, c0->stream));
+            return CTMR_OK;
+        });
+        local.fail(c0, cascade_peer_or(c0, bits, 2 * IW, !local.code));
+        cs.run(c0, [&]() -> int {
+            CU(c0, cudaMemcpyAsync(sb.data(), bits, sb.size() * 4, cudaMemcpyDeviceToHost, c0->stream));
+            CU(c0, cudaStreamSynchronize(c0->stream));
+            return CTMR_OK;
+        });
+    }
+    std::vector<uint32_t> covered(n_issuers / 32 + 1, 0);
+    for (uint32_t i = 0; i < n_issuers; ++i)
+        if ((sb[i >> 5] & ~sb[IW + (i >> 5)]) >> (i & 31) & 1u) {
+            covered[i >> 5] |= 1u << (i & 31);
+            ++*n_covered;
+        }
+
+    // R and S: each member's R list and counts
+    std::vector<uint64_t> nr(W, 0), ns(W, 0);
+    for (uint32_t r = 0; r < W; ++r)
+        cs.run(m[r], [&, c = m[r]]() -> int {
+            CU(c, cudaSetDevice(c->device));
+            CU(c, cudaMemcpyAsync(c->cascade->covered, covered.data(), covered.size() * 4, cudaMemcpyHostToDevice, c->stream));
+            int rc2 = cs.split(r, c->cascade->list_cap, &nr[r], &ns[r]);
+            if (rc2 == CTMR_OK && nr[r] > c->cascade->list_cap) rc2 = cs.split(r, nr[r], &nr[r], &ns[r]);
+            return rc2;
+        });
+    if (!cascade_total(cs, nr, &cs.R) || !cascade_total(cs, ns, &cs.S)) return false;
+    for (uint32_t r = 0; r < W; ++r) {
+        cs.ml[r].n_inc = nr[r];
+        cs.ml[r].n_exc = ns[r];
+    }
+    return true;
+}
+
 // ---- the call ---------------------------------------------------------------------------------------------------------
 // One driver builds the cascade on the members this process holds: a group's W members, one ctx (W == 1), or one rank
 // of a group of processes (W == 1; the call is collective, include/ctmr.h states the rules).  The phases run in the same
@@ -539,9 +673,8 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
         rc = peer_same_args(c0, now, salt, salt_len);
     if (rc) return group_fail(g, c0, rc);
 
-    const uint32_t n_issuers = (uint32_t)c0->digests.size();
-    Cascade cs{m, W};
-    cs.p.n_issuers = n_issuers;
+    Cascade cs{m, W, peer};
+    cs.p.n_issuers = (uint32_t)c0->digests.size();
     cs.p.salt_len = salt_len;
     cs.p.now = now;
     for (uint32_t j = 0; j < salt_len; ++j) cs.p.salt[j >> 2] |= (uint32_t)salt[j] << (8 * (j & 3));
@@ -549,87 +682,11 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
     cs.ml.assign(W, MemberLevel{});
     PeerLocal& local = cs.local;
 
-    // every member's scratch, its slot bits cleared, the registry's digests
-    for (uint32_t r = 0; r < W; ++r)
-        cs.run(m[r], [&, c = m[r]]() -> int {
-            CU(c, cudaSetDevice(c->device));
-            const int rc2 = cascade_ensure(c, 0, 0, false);
-            if (rc2) return rc2;
-            CascadeState* s = c->cascade.get();
-            CU(c, cudaMemsetAsync(s->revoked, 0, s->slot_words * 4, c->stream));
-            if (n_issuers) CU(c, cudaMemcpyAsync(s->dig, c0->digests.data(), (size_t)n_issuers * 32, cudaMemcpyHostToDevice, c->stream));
-            CU(c, cudaStreamSynchronize(c->stream));
-            return CTMR_OK;
-        });
-
-    // mark: every member's shard against each chunk's set, or a peer rank's against each round's union set
     std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
-    const CrlSetVisit mark = [&](ctmr_ctx* c, const CrlSetSlot* set, uint64_t mask) -> int {
-        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set, mask, c->cascade->revoked);
-        return launched(c);
-    };
-    bool going = peer ? crl_peer_each_set(c0, b, issuer, row, mark, crl_status, local) : !local.code;
-    if (!peer && going) {
-        ctmr_ctx* at = c0;
-        rc = crl_each_set(m, W, b, issuer, mark, crl_status, &at);
-        local.fail(at, rc);
-        going = rc == CTMR_OK;
-    }
-
-    // a count summed over the members, or over the ranks; false: the build stops (it failed here, or on a peer rank)
-    const auto total = [&](const std::vector<uint64_t>& v, uint64_t* sum) {
-        if (peer) return peer_sum(c0, local, v[0], sum);
-        *sum = 0;
-        for (const uint64_t x : v) *sum += x;
-        return !local.code;
-    };
     std::vector<uint8_t> img;
     uint32_t n_covered = 0, level = 0;
     const auto build = [&]() {  // every return is one that all peer ranks take together, to the finish
-        if (!going) return;
-        // coverage: every CRL of an issuer in the batch is CTMR_CRL_OK
-        std::vector<uint32_t> sb(2 * IW, 0);  // seen, then bad
-        for (uint64_t k = 0; k < b->n_crls; ++k) {
-            const uint32_t i = issuer[k];
-            if (i >= n_issuers) continue;
-            sb[i >> 5] |= 1u << (i & 31);
-            if (crl_status[k] != CTMR_CRL_OK) sb[IW + (i >> 5)] |= 1u << (i & 31);
-        }
-        if (peer) {
-            uint32_t* bits = c0->cascade->bits;
-            cs.run(c0, [&]() -> int {
-                CU(c0, cudaMemcpyAsync(bits, sb.data(), sb.size() * 4, cudaMemcpyHostToDevice, c0->stream));
-                return CTMR_OK;
-            });
-            local.fail(c0, cascade_peer_or(c0, bits, 2 * IW, !local.code));
-            cs.run(c0, [&]() -> int {
-                CU(c0, cudaMemcpyAsync(sb.data(), bits, sb.size() * 4, cudaMemcpyDeviceToHost, c0->stream));
-                CU(c0, cudaStreamSynchronize(c0->stream));
-                return CTMR_OK;
-            });
-        }
-        std::vector<uint32_t> covered(n_issuers / 32 + 1, 0);
-        for (uint32_t i = 0; i < n_issuers; ++i)
-            if ((sb[i >> 5] & ~sb[IW + (i >> 5)]) >> (i & 31) & 1u) {
-                covered[i >> 5] |= 1u << (i & 31);
-                ++n_covered;
-            }
-
-        // R and S: each member's R list and counts
-        std::vector<uint64_t> nr(W, 0), ns(W, 0);
-        for (uint32_t r = 0; r < W; ++r)
-            cs.run(m[r], [&, c = m[r]]() -> int {
-                CU(c, cudaSetDevice(c->device));
-                CU(c, cudaMemcpyAsync(c->cascade->covered, covered.data(), covered.size() * 4, cudaMemcpyHostToDevice, c->stream));
-                int rc2 = cs.split(r, c->cascade->list_cap, &nr[r], &ns[r]);
-                if (rc2 == CTMR_OK && nr[r] > c->cascade->list_cap) rc2 = cs.split(r, nr[r], &nr[r], &ns[r]);
-                return rc2;
-            });
-        if (!total(nr, &cs.R) || !total(ns, &cs.S)) return;
-        for (uint32_t r = 0; r < W; ++r) {
-            cs.ml[r].n_inc = nr[r];
-            cs.ml[r].n_exc = ns[r];
-        }
+        if (!cascade_front(cs, b, issuer, row, crl_status, &n_covered)) return;
 
         // the levels, each merged and read back into the image behind the header
         img = {2, 0, 0, (uint8_t)salt_len};
@@ -667,7 +724,7 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
                     return rc2;
                 });
             uint64_t F = 0;
-            if (!total(fr, &F)) return;
+            if (!cascade_total(cs, fr, &F)) return;
             const uint64_t nbytes = ((uint64_t)mbits + 7) / 8;
             const size_t at = img.size();
             img.resize(at + 10 + nbytes);
@@ -726,6 +783,215 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
     return CTMR_OK;
 }
 
+// ---- the stash ------------------------------------------------------------------------------------------------------
+constexpr uint32_t kMaxStashK = 64;  // a bound on each thread's hashes per level; the build's k is far below it
+
+// A published filter checked against include/ctmr.h's layout: its salt, and each level's bits laid out again in words
+// from a 16-byte boundary (bit j stays (byte[j >> 3] >> (j & 7)) & 1: words are little-endian), with its level table.
+struct StashFilter {
+    uint32_t salt_len = 0;
+    const uint8_t* salt = nullptr;
+    std::vector<StashLevel> levels;
+    std::vector<uint32_t> words;
+};
+
+// nullptr, or what is wrong with the filter
+const char* stash_filter(const uint8_t* f, uint64_t n, StashFilter& out) {
+    if (n < 4) return "filter shorter than its header";
+    if (f[0] != 2 || f[1] != 0) return "filter version is not 2";
+    if (f[2] != 0) return "filter is inverted";
+    out.salt_len = f[3];
+    out.salt = f + 4;
+    if (out.salt_len > kMaxSalt) return "filter salt_len > 32";
+    if (n - 4 < out.salt_len) return "filter truncated in its salt";
+    for (uint64_t o = 4 + out.salt_len; o < n;) {
+        if (n - o < 10) return "filter truncated in a level header";
+        uint32_t m, k;
+        std::memcpy(&m, f + o + 1, 4);
+        std::memcpy(&k, f + o + 5, 4);
+        if (f[o] != 2) return "filter level hash is not 2";
+        if (k < 1 || k > kMaxStashK) return "filter level k is not in [1, 64]";
+        if (m < 8) return "filter level m < 8";
+        if (f[o + 9] != out.levels.size() + 1) return "filter level number is not its position";
+        const uint64_t nbytes = ((uint64_t)m + 7) / 8;
+        o += 10;
+        if (n - o < nbytes) return "filter truncated in a level's bits";
+        if ((m & 7u) && f[o + nbytes - 1] >> (m & 7u)) return "filter level has unused high bits set";
+        const uint64_t at = out.words.size();
+        out.levels.push_back(StashLevel{at, m, k});
+        out.words.resize(at + ((nbytes + 15) / 16) * 4, 0u);
+        std::memcpy(out.words.data() + at, f + o, nbytes);
+        o += nbytes;
+    }
+    return out.levels.empty() ? "filter has no level" : nullptr;
+}
+
+// nullptr, or what is wrong with the stashes; every listed (digest || serial) into `listed`
+const char* stash_parse(const uint8_t* s, uint64_t n, std::unordered_set<std::string>& listed) {
+    for (uint64_t o = 0; o < n;) {
+        if (n - o < 37) return "stash truncated in a unit header";
+        uint32_t cnt;
+        std::memcpy(&cnt, s + o, 4);
+        if (s[o + 4] != 32) return "stash unit hash length is not 32";
+        const char* dig = reinterpret_cast<const char*>(s + o + 5);
+        o += 37;
+        for (uint32_t e = 0; e < cnt; ++e) {
+            if (o >= n || n - o - 1 < s[o]) return "stash truncated in an entry";
+            std::string key(dig, 32);
+            key.append(reinterpret_cast<const char*>(s + o + 1), s[o]);
+            listed.insert(std::move(key));
+            o += 1 + s[o];
+        }
+    }
+    return nullptr;
+}
+
+// all or nothing, like cascade_ensure: the filter words, the level table and the bodies of `records` R records
+int stash_ensure(ctmr_ctx* c, uint64_t words, uint64_t levels, uint64_t records) {
+    StashState* have = c->stash.get();
+    const bool w = !have || have->word_cap < words;
+    const bool l = !have || have->level_cap < levels;
+    const bool bd = !have || have->body_cap < records;
+    if (!w && !l && !bd) return CTMR_OK;
+    DevBuf<uint32_t> nw, nb;
+    DevBuf<StashLevel> nl;
+    if (w) CU(c, alloc(nw, std::max<uint64_t>(words, 1)));
+    if (l) CU(c, alloc(nl, std::max<uint64_t>(levels, 1)));
+    if (bd) CU(c, alloc(nb, 11 * std::max<uint64_t>(records, 1)));
+    if (!have) {
+        c->stash.reset(new (std::nothrow) StashState());
+        if (!c->stash) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    }
+    StashState* s = c->stash.get();
+    if (w) {
+        s->words = std::move(nw);
+        s->word_cap = words;
+    }
+    if (l) {
+        s->levels = std::move(nl);
+        s->level_cap = levels;
+    }
+    if (bd) {
+        s->bodies = std::move(nb);
+        s->body_cap = records;
+    }
+    return CTMR_OK;
+}
+
+// member r's query of its R list (list 0 after cascade_front) against the filter: the records it calls revoked are
+// counted in *in_filter, the others' (digest || serial) appended to `cand`
+int stash_query(Cascade& cs, uint32_t r, const StashFilter& f, uint64_t* in_filter, std::vector<std::string>& cand) {
+    ctmr_ctx* c = cs.m[r];
+    const uint64_t n = cs.ml[r].n_inc;
+    if (n == 0) return CTMR_OK;
+    CU(c, cudaSetDevice(c->device));
+    const int rc = stash_ensure(c, f.words.size(), f.levels.size(), n);
+    if (rc) return rc;
+    StashState* s = c->stash.get();
+    CascadeState* cst = c->cascade.get();
+    CU(c, cudaMemcpyAsync(s->words, f.words.data(), f.words.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(s->levels, f.levels.data(), f.levels.size() * sizeof(StashLevel), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemsetAsync(cst->counters, 0, 2 * sizeof(unsigned long long), c->stream));
+    stash_query_kernel<<<grid(n, kCascadeThreads), kCascadeThreads, 0, c->stream>>>(cs.params(c), cst->list[0], n, s->words, s->levels,
+                                                                                  (uint32_t)f.levels.size(), s->bodies, cst->counters);
+    CU(c, cudaGetLastError());
+    unsigned long long h[2] = {0, 0};
+    CU(c, cudaMemcpyAsync(h, cst->counters, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    std::vector<uint32_t> body(11 * h[0]);
+    if (h[0]) {
+        CU(c, cudaMemcpyAsync(body.data(), s->bodies, body.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+    }
+    *in_filter += h[1];
+    const auto& dig = cs.m[0]->digests;
+    for (uint64_t i = 0; i < h[0]; ++i) {
+        const uint32_t* b = &body[11 * i];  // issuer, then serial_len and serial[39] from byte 4
+        const uint8_t* sb = reinterpret_cast<const uint8_t*>(b + 1);
+        std::string key(reinterpret_cast<const char*>(dig[b[0]].data()), 32);
+        key.append(reinterpret_cast<const char*>(sb + 1), sb[0]);
+        cand.push_back(std::move(key));
+    }
+    return CTMR_OK;
+}
+
+// ctmr_revoked_stash on one ctx or a group: the checks, cascade_front, each member's query, and on the host the drop of
+// the pairs the earlier stashes list, the sort and the serialization (include/ctmr.h states the rules)
+int revoked_stash(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, int64_t now, const uint8_t* filter,
+                  uint64_t filter_bytes, const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out) {
+    ctmr_ctx* c0 = m[0];
+    const char* call = "ctmr_revoked_stash: ";
+    int rc = set_device(c0);
+    if (rc) return group_fail(g, c0, rc);
+    std::vector<uint32_t> issuer;
+    StashFilter f;
+    std::unordered_set<std::string> listed;
+    const char* bad = !filter && filter_bytes ? "NULL filter" : !stashes && stash_bytes ? "NULL stashes" : nullptr;
+    if (!bad) bad = stash_filter(filter, filter_bytes, f);
+    if (!bad) bad = stash_parse(stashes, stash_bytes, listed);
+    rc = bad ? fail(c0, CTMR_E_INVALID, std::string(call) + bad) : crl_prepare(c0, b, out, call, issuer);
+    if (rc == CTMR_OK) rc = refresh_digests(c0);
+    if (rc) return group_fail(g, c0, rc);
+
+    Cascade cs{m, W, false};
+    cs.p.n_issuers = (uint32_t)c0->digests.size();
+    cs.p.salt_len = f.salt_len;
+    cs.p.now = now;
+    for (uint32_t j = 0; j < f.salt_len; ++j) cs.p.salt[j >> 2] |= (uint32_t)f.salt[j] << (8 * (j & 3));
+    cs.p.one = 1;
+    cs.ml.assign(W, MemberLevel{});
+    std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
+    uint32_t n_covered = 0;
+    uint64_t in_filter = 0;
+    std::vector<std::string> cand;
+    if (cascade_front(cs, b, issuer, nullptr, crl_status, &n_covered))
+        for (uint32_t r = 0; r < W; ++r) cs.run(m[r], [&] { return stash_query(cs, r, f, &in_filter, cand); });
+    if (cs.local.code) {
+        if (g) g->err = cs.local.err;  // the failing member's text is the group's
+        return cs.local.code;
+    }
+
+    // the new records: those no earlier stash lists; then their distinct pairs by digest, then serial
+    uint64_t in_stashes = 0;
+    std::vector<std::string> fresh;
+    for (std::string& k : cand) {
+        if (listed.count(k)) ++in_stashes;
+        else fresh.push_back(std::move(k));
+    }
+    std::sort(fresh.begin(), fresh.end());  // std::string orders bytes as unsigned, a prefix first
+    fresh.erase(std::unique(fresh.begin(), fresh.end()), fresh.end());
+    std::vector<uint8_t> img;
+    uint32_t units = 0;
+    for (size_t i = 0; i < fresh.size();) {
+        size_t j = i;
+        while (j < fresh.size() && fresh[j].compare(0, 32, fresh[i], 0, 32) == 0) ++j;
+        const uint32_t cnt = (uint32_t)(j - i);
+        const size_t at = img.size();
+        img.resize(at + 37);
+        std::memcpy(&img[at], &cnt, 4);
+        img[at + 4] = 32;
+        std::memcpy(&img[at + 5], fresh[i].data(), 32);
+        for (; i < j; ++i) {
+            img.push_back((uint8_t)(fresh[i].size() - 32));
+            img.insert(img.end(), fresh[i].begin() + 32, fresh[i].end());
+        }
+        ++units;
+    }
+
+    out->bytes = img.size();
+    if (img.size() > out->cap || (!out->buf && !img.empty()))
+        return group_fail(g, c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_stash: cap " + std::to_string(out->cap) + " < " + std::to_string(img.size()) + " bytes"));
+    if (!img.empty()) std::memcpy(out->buf, img.data(), img.size());
+    if (out->crl_status) std::memcpy(out->crl_status, crl_status.data(), crl_status.size());
+    out->issuers = n_covered;
+    out->stash_issuers = units;
+    out->revoked = cs.R;
+    out->in_filter = in_filter;
+    out->in_stashes = in_stashes;
+    out->serials = fresh.size();
+    return CTMR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -742,6 +1008,23 @@ int ctmr_group_revoked_cascade(ctmr_group* g, const ctmr_crl_batch* batch, int64
                                ctmr_cascade_out* out) {
     if (!g || g->m.empty()) return CTMR_E_INVALID;
     const int rc = revoked_cascade(g->m.data(), (uint32_t)g->m.size(), g, batch, now_unix_sec, salt, salt_len, out);
+    cudaSetDevice(g->m[0]->device);
+    return rc;
+}
+
+int ctmr_revoked_stash(ctmr_ctx* c, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter, uint64_t filter_bytes,
+                       const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_stash: a member of a group; use ctmr_group_revoked_stash");
+    if (peer_call(c)) return fail(c, CTMR_E_INVALID, "ctmr_revoked_stash: not a collective call; load the ranks' checkpoint parts into one ctx or a group");
+    ctmr_ctx* m[1] = {c};
+    return revoked_stash(m, 1, nullptr, batch, now_unix_sec, filter, filter_bytes, stashes, stash_bytes, out);
+}
+
+int ctmr_group_revoked_stash(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter, uint64_t filter_bytes,
+                             const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const int rc = revoked_stash(g->m.data(), (uint32_t)g->m.size(), g, batch, now_unix_sec, filter, filter_bytes, stashes, stash_bytes, out);
     cudaSetDevice(g->m[0]->device);
     return rc;
 }

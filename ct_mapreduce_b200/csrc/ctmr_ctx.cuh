@@ -367,6 +367,22 @@ struct CascadeState {
     uint64_t recv_words = 0;
 };
 
+// ctmr_revoked_stash (ctmr_cascade.cu): the published filter laid out again in words, each level from a 16-byte boundary,
+// its level table, and the 44-byte key bodies of the R records the filter calls not revoked.  Built on first use and
+// grown, all or nothing.
+struct StashLevel {
+    uint64_t word;  // the level's first word in the filter words
+    uint32_t m, k;
+};
+struct StashState {
+    uint64_t word_cap = 0;
+    DevBuf<uint32_t> words;              // [word_cap]
+    uint64_t level_cap = 0;
+    DevBuf<StashLevel> levels;           // [level_cap]
+    uint64_t body_cap = 0;
+    DevBuf<uint32_t> bodies;             // [body_cap][11]: issuer, serial_len, serial[39]
+};
+
 // the ctx's private device words (one allocation)
 struct SmallDev {
     unsigned long long slots_used;   // DeviceState::slots_used points here (no kernel reads it)
@@ -464,6 +480,7 @@ struct ctmr_ctx {
     uint32_t fe_peer_stopped = 0;  // ranks that stopped (tiles) in the last collective front-end call
     std::unique_ptr<CrlState> crl;  // ctmr_revoked_known (ctmr_crl.cu)
     std::unique_ptr<CascadeState> cascade;  // ctmr_revoked_cascade (ctmr_cascade.cu)
+    std::unique_ptr<StashState> stash;      // ctmr_revoked_stash (ctmr_cascade.cu)
     std::string err;
 };
 

@@ -14,6 +14,8 @@ points, and exposes the results under the reference's names:
                                           serials::<expDate>::<issuer> sets (storage/knowncertificates.go:28-55)
     GpuCertDatabase.revoked_cascade    <- CRLite's filter cascade of the covered issuers' revoked and valid known
                                           certificates, built on the GPU next to the table
+    GpuCertDatabase.revoked_stash      <- CRLite's stash: the revoked known certificates a published filter and the
+                                          stashes since it miss
 
 All arithmetic happens in the CUDA kernels; nothing here parses, hashes or de-duplicates.
 """
@@ -235,6 +237,18 @@ class CascadeResult:
         self.bytes = data
         self.crl_status = crl_status
         self.issuers, self.levels, self.revoked, self.valid = int(o.issuers), int(o.levels), int(o.revoked), int(o.valid)
+
+
+class StashResult:
+    """Outputs of ctmr_revoked_stash (include/ctmr.h ctmr_stash_out): the serialized stash, each CRL's status, the
+    covered issuers, the issuer units written, the key records in R, those the filter and the earlier stashes already
+    answer, and the (issuer, serial) entries written."""
+
+    def __init__(self, data: bytes, crl_status: np.ndarray, o):
+        self.bytes = data
+        self.crl_status = crl_status
+        self.issuers, self.stash_issuers = int(o.issuers), int(o.stash_issuers)
+        self.revoked, self.in_filter, self.in_stashes, self.serials = int(o.revoked), int(o.in_filter), int(o.in_stashes), int(o.serials)
 
 
 def _crl_batch(crls, issuer_digests):
@@ -820,6 +834,39 @@ class GpuCertDatabase:
         self._cascade_bytes = int(o.bytes)
         return CascadeResult(buf[:o.bytes].tobytes(), status[:b.n_crls].copy(), o)
 
+    def _revoked_stash_fn(self):
+        return self._lib.ctmr_revoked_stash
+
+    _stash_bytes = 0   # size of the last stash this db computed: the next call's first buffer holds twice that
+
+    def revoked_stash(self, crls, issuer_digests, now_unix_sec: int, filter: bytes, stashes: bytes = b"",
+                      cap: int | None = None) -> StashResult:
+        """CRLite's next stash (ctmr_revoked_stash): every (issuer, serial) of the cascade's revoked set R for these CRLs
+        and now_unix_sec that the published `filter` answers "not revoked" and that none of `stashes` (every stash
+        published since the filter, back to back) lists.  `crls` and `issuer_digests` as for revoked_cascade.  Read-only.
+        Returns .bytes (the serialized stash), .crl_status, .issuers, .stash_issuers, .revoked, .in_filter, .in_stashes
+        and .serials.  The output buffer holds `cap` bytes; by default 1 MiB, or twice the last stash this db computed if
+        that is more.  A larger stash is computed twice: the first call only reports its size.  Not on a db attached to
+        peers (CTMR_E_INVALID on every rank)."""
+        fn = self._revoked_stash_fn()
+        b, keep = _crl_batch(crls, issuer_digests)
+        filter, stashes = bytes(filter), bytes(stashes)
+        fbuf = (C.c_uint8 * max(len(filter), 1)).from_buffer_copy(filter or b"\0")
+        sbuf = (C.c_uint8 * max(len(stashes), 1)).from_buffer_copy(stashes or b"\0")
+        status = np.zeros(max(int(b.n_crls), 1), np.uint8)
+        size = int(cap) if cap is not None else max(1 << 20, 2 * self._stash_bytes)
+        buf = np.empty(max(size, 1), np.uint8)
+        o = capi.StashOut(capi.ptr(buf), size, 0, capi.ptr(status))
+        now_unix_sec = int(now_unix_sec)
+        rc = fn(self._h, C.byref(b), now_unix_sec, fbuf, len(filter), sbuf, len(stashes), C.byref(o))
+        if rc == capi.E_BATCH_TOO_LARGE and o.bytes:  # larger than the buffer: again into one of the size it reported
+            buf = np.empty(int(o.bytes), np.uint8)
+            o = capi.StashOut(capi.ptr(buf), buf.size, 0, capi.ptr(status))
+            rc = fn(self._h, C.byref(b), now_unix_sec, fbuf, len(filter), sbuf, len(stashes), C.byref(o))
+        self._check(rc)
+        self._stash_bytes = int(o.bytes)
+        return StashResult(buf[:o.bytes].tobytes(), status[:b.n_crls].copy(), o)
+
     def checkpoint(self) -> np.ndarray:
         """This db's part of a portable checkpoint (ctmr_checkpoint_save): loads into any table size, group size or number
         of ranks.  On a db attached to peers it is collective, and every rank returns its own part."""
@@ -1017,6 +1064,9 @@ class GpuCertGroup(GpuCertDatabase):
 
     def _revoked_cascade_fn(self):
         return self._lib.ctmr_group_revoked_cascade
+
+    def _revoked_stash_fn(self):
+        return self._lib.ctmr_group_revoked_stash
 
     def get_known_certificates(self, exp_hour: int, issuer_digest: bytes):
         grp = self

@@ -150,6 +150,18 @@ type Cascade struct {
 	Valid     uint64 // key records excluded (S)
 }
 
+// Stash is CRLite's stash as RevokedStash computes it (include/ctmr.h "CRLite stash" states the layout and the rules).
+type Stash struct {
+	Bytes        []byte  // the serialized stash: units of u32 n, u8 32, digest, n entries of u8 len, serial
+	CRLStatus    []uint8 // per CRL, CTMR_CRL_*
+	Issuers      uint32  // issuers covered (RevokedCascade's rule)
+	StashIssuers uint32  // issuer units written
+	Revoked      uint64  // key records in R
+	InFilter     uint64  // of them: the filter answers revoked
+	InStashes    uint64  // of the rest: an earlier stash lists their (issuer, serial)
+	Serials      uint64  // (issuer, serial) entries written
+}
+
 // RevokedCascade builds the filter cascade of the covered issuers' live known certificates on the GPU: the revoked
 // ones included, every other one excluded.  crls and issuerIDs as for RevokedKnown, verified CRLs only; salt is at most
 // 32 bytes.  Read-only.  The output buffer holds 16 MiB, or twice the DB's last cascade if that is more; a larger cascade
@@ -227,5 +239,88 @@ func (d *DB) RevokedCascade(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int6
 		Levels:    uint32(out.levels),
 		Revoked:   uint64(out.revoked),
 		Valid:     uint64(out.valid),
+	}, nil
+}
+
+// RevokedStash computes CRLite's next stash on the GPU: every (issuer, serial) of RevokedCascade's revoked set for these
+// CRLs and nowUnixSec that the published filter answers "not revoked" and that none of stashes lists (every stash
+// published since the filter, back to back; may be empty).  crls and issuerIDs as for RevokedCascade.  Read-only.  The
+// output buffer holds 1 MiB, or twice the DB's last stash if that is more; a larger stash is computed twice (the first
+// call only reports its size).  Not on a DB attached to peers: every rank gets CTMR_E_INVALID.
+func (d *DB) RevokedStash(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int64, filter, stashes []byte) (*Stash, error) {
+	n := len(crls)
+	if len(issuerIDs) < n {
+		return nil, fmt.Errorf("RevokedStash: %d issuer IDs for %d CRLs", len(issuerIDs), n)
+	}
+	total := 0
+	for _, c := range crls {
+		total += len(c)
+	}
+	data := C.malloc(C.size_t(total + 1))
+	defer C.free(data)
+	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
+	lens := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
+	dig := C.malloc(C.size_t(32*n + 32))
+	defer C.free(unsafe.Pointer(&offs[0]))
+	defer C.free(unsafe.Pointer(&lens[0]))
+	defer C.free(dig)
+	flat := unsafe.Slice((*byte)(data), total+1)
+	o := 0
+	for i, c := range crls {
+		copy(flat[o:], c)
+		offs[i], lens[i] = C.uint64_t(o), C.uint64_t(len(c))
+		copy(unsafe.Slice((*byte)(dig), 32*n)[32*i:], issuerIDs[i][:])
+		o += len(c)
+	}
+	b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
+	defer C.free(unsafe.Pointer(b))
+	b.data, b.data_bytes = (*C.uint8_t)(data), C.uint64_t(total)
+	b.crl_off, b.crl_len = &offs[0], &lens[0]
+	b.issuer_digest, b.n_crls = (*C.uint8_t)(dig), C.uint64_t(n)
+	cf := C.malloc(C.size_t(len(filter) + 1))
+	defer C.free(cf)
+	copy(unsafe.Slice((*byte)(cf), len(filter)+1), filter)
+	cst := C.malloc(C.size_t(len(stashes) + 1))
+	defer C.free(cst)
+	copy(unsafe.Slice((*byte)(cst), len(stashes)+1), stashes)
+	status := C.calloc(C.size_t(n+1), 1)
+	defer C.free(status)
+	out := (*C.ctmr_stash_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_stash_out{}))))
+	defer C.free(unsafe.Pointer(out))
+	call := func() C.int {
+		f, fn := (*C.uint8_t)(cf), C.uint64_t(len(filter))
+		s, sn := (*C.uint8_t)(cst), C.uint64_t(len(stashes))
+		if d.g != nil {
+			return C.ctmr_group_revoked_stash(d.g, b, C.int64_t(nowUnixSec), f, fn, s, sn, out)
+		}
+		return C.ctmr_revoked_stash(d.h, b, C.int64_t(nowUnixSec), f, fn, s, sn, out)
+	}
+	size := uint64(1 << 20)
+	if 2*d.stashBytes > size {
+		size = 2 * d.stashBytes
+	}
+	buf := C.malloc(C.size_t(size)) // a larger stash is computed again into a buffer of the size it reported
+	out.buf, out.cap, out.crl_status = (*C.uint8_t)(buf), C.uint64_t(size), (*C.uint8_t)(status)
+	rc := call()
+	if rc == C.CTMR_E_BATCH_TOO_LARGE && out.bytes > 0 {
+		C.free(buf)
+		buf = C.malloc(C.size_t(out.bytes))
+		out.buf, out.cap = (*C.uint8_t)(buf), out.bytes
+		rc = call()
+	}
+	defer C.free(buf)
+	if err := d.err(rc, "ctmr_revoked_stash"); err != nil {
+		return nil, err
+	}
+	d.stashBytes = uint64(out.bytes)
+	return &Stash{
+		Bytes:        C.GoBytes(buf, C.int(out.bytes)),
+		CRLStatus:    C.GoBytes(status, C.int(n)),
+		Issuers:      uint32(out.issuers),
+		StashIssuers: uint32(out.stash_issuers),
+		Revoked:      uint64(out.revoked),
+		InFilter:     uint64(out.in_filter),
+		InStashes:    uint64(out.in_stashes),
+		Serials:      uint64(out.serials),
 	}, nil
 }

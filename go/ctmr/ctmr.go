@@ -63,6 +63,7 @@ type DB struct {
 	g            *C.ctmr_group
 	peer         bool   // attached to the DBs of other processes (PeerAttach): the batch calls and the front end are collective
 	cascadeBytes uint64 // size of the last RevokedCascade: the next call's first buffer holds twice that
+	stashBytes   uint64 // size of the last RevokedStash: the next call's first buffer holds twice that
 }
 
 func New(c Config) (*DB, error) {

@@ -388,6 +388,60 @@ typedef struct ctmr_cascade_out {   /* caller-allocated; HOST buffers */
 int ctmr_revoked_cascade(ctmr_ctx* ctx, const ctmr_crl_batch* batch, int64_t now_unix_sec,
                          const uint8_t* salt, uint32_t salt_len, ctmr_cascade_out* out);
 
+/* ---- CRLite stash (the revoked known certificates a published filter and its stashes miss) ------------------------- */
+/* Between full filters CRLite publishes stashes: per issuer, the serials revoked since the filter.  This call computes the
+ * next stash from the table and what was already published, with no state kept between runs; only the candidates the
+ * filter misses reach the host (DESIGN.md "Revoked stash").
+ *
+ * Sets.  Covered issuers, live records and R are ctmr_revoked_cascade's with the same batch and now_unix_sec.  For each
+ * key record of R, with x = digest || serial:
+ *   in_filter   query(filter, x) is revoked (the query rule above, with the filter's own salt);
+ *   in_stashes  otherwise, and an earlier stash lists (digest, serial);
+ *   new         every other record of R.  The stash lists the distinct (digest, serial) pairs of the new records: a serial
+ *               under two hours is one entry.
+ * Counts are key records, as in the cascade: revoked == in_filter + in_stashes + (new key records).
+ *
+ * Stash layout, integers little-endian: any number of units back to back, each
+ *     u32 n, u8 32 (hash length), digest[32], then n entries of u8 len, serial[len].
+ * Byte parity with Firefox's cert_storage loader is NOT pinned: this header and tests/stash_model.py pin the format.  The
+ * concatenation of stashes is a stash, so `stashes` is every stash published since `filter`, back to back (may be empty).
+ * The output is deterministic: units in ascending order of digest bytes, only issuers with at least one entry; each
+ * issuer's serials in ascending lexicographic byte order, a serial before any longer one it is a prefix of.  An empty
+ * stash is 0 bytes and succeeds with any cap and a NULL buf.
+ *
+ * Checks before any work, each CTMR_E_INVALID (both inputs come from outside the library):
+ *   - the filter must follow the layout above exactly: at least 4 bytes; version 2, not inverted, salt_len <= 32; at least
+ *     one level; each level hash byte 2, 1 <= k <= 64, m >= 8, a level byte equal to its 1-based position, all
+ *     ceil(m / 8) bytes present with the unused high bits of the last zero; nothing after the last level.  k <= 64 is a
+ *     bound the build never reaches (its p_1 >= 1 / (sqrt(2) * slots)); it stops a crafted filter from making each
+ *     thread hash without limit;
+ *   - a stash unit whose hash length is not 32, and a stash truncated anywhere; a NULL filter or stashes with a nonzero
+ *     length.  Entries longer than CTMR_MAX_SERIAL and digests not in the registry are accepted: they never match;
+ *   - ctmr_revoked_cascade's: a NULL batch or output, a CRL outside data or larger than a chunk.
+ *
+ * The cap rule is the cascade's: with cap too small (buf may be NULL) the call returns CTMR_E_BATCH_TOO_LARGE and writes
+ * `bytes` and nothing else; a second call with that cap returns exactly those bytes.  Read-only, like the other CRL calls.
+ * A member ctx of a group is refused with CTMR_E_INVALID (use ctmr_group_revoked_stash), and so is a ctx attached to
+ * peers (world > 1): every rank refuses before any barrier, so none waits.  Cost: the cascade's mark and split, then one
+ * thread per record of R walking the filter's levels, and the candidates the filter misses read back and sorted on the
+ * host (DESIGN.md "Revoked stash").
+ * Out of scope: un-revocations (a stash only adds); which issuers the old filter covered (every issuer covered now is
+ * answered by the filter's query, and a newly enrolled issuer wants a new full filter); signature verification. */
+typedef struct ctmr_stash_out {     /* caller-allocated; HOST buffers */
+    uint8_t* buf; uint64_t cap;     /* the serialized stash */
+    uint64_t bytes;                 /* written; on CTMR_E_BATCH_TOO_LARGE the bytes needed */
+    uint8_t* crl_status;            /* [n_crls] CTMR_CRL_*, as ctmr_revoked_known; may be NULL */
+    uint32_t issuers;               /* issuers covered (the cascade's rule) */
+    uint32_t stash_issuers;         /* issuer units written */
+    uint64_t revoked;               /* key records in R (the cascade's |R| for this batch and now) */
+    uint64_t in_filter;             /* of them: the filter answers revoked */
+    uint64_t in_stashes;            /* of the rest: an earlier stash lists their (issuer, serial) */
+    uint64_t serials;               /* (issuer, serial) entries written */
+} ctmr_stash_out;
+int ctmr_revoked_stash(ctmr_ctx* ctx, const ctmr_crl_batch* batch, int64_t now_unix_sec,
+                       const uint8_t* filter, uint64_t filter_bytes,
+                       const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out);
+
 /* ---- device-resident entry points ---------------------------------------------------------- */
 /* Same path with every buffer already in HBM on ctx's device (benchmarks, multi-GPU orchestration,
  * hosts that receive entries by GPUDirect).  `stream` is a cudaStream_t passed as void*; NULL =
@@ -504,6 +558,10 @@ int ctmr_group_revoked_known(ctmr_group* g, const ctmr_crl_batch* batch, ctmr_cr
  * and copied back to every member before the members test their own records.  No atomic crosses a GPU. */
 int ctmr_group_revoked_cascade(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* salt,
                                uint32_t salt_len, ctmr_cascade_out* out);
+/* ctmr_revoked_stash over every shard, the same bytes as one ctx: the cascade's mark and split on every member, each
+ * member queries the filter for its own R records, and the host merges the candidates. */
+int ctmr_group_revoked_stash(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter,
+                             uint64_t filter_bytes, const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out);
 
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the

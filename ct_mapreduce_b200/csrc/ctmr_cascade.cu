@@ -570,18 +570,12 @@ bool cascade_front(Cascade& cs, const ctmr_crl_batch* b, const std::vector<uint3
         });
 
     // mark: every member's shard against each chunk's set, or a peer rank's against each round's union set
-    const CrlSetVisit mark = [&](ctmr_ctx* c, const CrlSetSlot* set, uint64_t mask) -> int {
-        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set, mask, c->cascade->revoked);
+    const CrlSetVisit mark = [&](ctmr_ctx* c, const CrlSet& set) -> int {
+        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set.slots, set.mask,
+                                                                    c->cascade->revoked);
         return launched(c);
     };
-    bool going = peer ? crl_peer_each_set(c0, b, issuer, row, mark, crl_status, local) : !local.code;
-    if (!peer && going) {
-        ctmr_ctx* at = c0;
-        const int rc = crl_each_set(m, W, b, issuer, mark, crl_status, &at);
-        local.fail(at, rc);
-        going = rc == CTMR_OK;
-    }
-    if (!going) return false;
+    if (!crl_each_set(m, W, peer, b, issuer, row, mark, crl_status, local)) return false;
 
     // coverage: every CRL of an issuer in the batch is CTMR_CRL_OK
     std::vector<uint32_t> sb(2 * IW, 0);  // seen, then bad
@@ -636,17 +630,17 @@ bool cascade_front(Cascade& cs, const ctmr_crl_batch* b, const std::vector<uint3
 //   checks    one ctx or a group: the arguments and crl_prepare, and a failure returns at once.  A peer rank: the same
 //             checks and every allocation of the call, carried in agreement 1 with the rank's chunk count; then one more
 //             mailbox word, a hash of (now, salt), which must equal rank 0's.
-//   mark      one ctx or a group: member 0 builds each chunk's set, and every member marks its shard against its copy of
-//             it (crl_each_set).  A peer rank: the steps and rounds of the collective ctmr_revoked_known
-//             (crl_peer_each_set); in each round the rank marks its shard against the union set of every rank's valid
+//   mark      one call, crl_each_set, which takes the form.  One ctx or a group: member 0 builds each chunk's set, and
+//             every member marks its shard against its copy of it.  A peer rank: the steps and rounds of the collective
+//             ctmr_revoked_known; in each round the rank marks its shard against the union set of every rank's valid
 //             records of the round.
 //   coverage  seen and bad bitmaps over dense indices from the CRLs' statuses (peer ranks: each from its own CRLs, then
 //             OR-reduced over the ranks); covered = seen & ~bad
 //   counts    |R|, |S| and |F_l| are sums over the members, or mailbox sums over the ranks
 //   merge     each member inserts its own include list into partial bits; a group's member 0 pulls them, ORs them
 //             (cascade_or) and copies the merged level back; peer ranks OR-reduce them on every rank (cascade_peer_or)
-//   finish    one ctx or a group: the cap check.  A peer rank: the streams drained and a final agreement, which makes a
-//             failure on any rank every rank's, and then a cap too small on any rank every rank's CTMR_E_BATCH_TOO_LARGE.
+//   finish    one ctx or a group: the cap check.  A peer rank: crl_peer_finish, whose final agreement makes a failure on
+//             any rank every rank's, and then a cap too small on any rank every rank's CTMR_E_BATCH_TOO_LARGE.
 // The OR all-reduce goes through the parity-0 region of source `rank` on every rank, 16 X words a slice: the rank's words
 // of the slice into that region on every rank, a barrier, the OR of the world regions into the rank's bits, a barrier.
 // One ctx or a group stops at its first failure.  A peer rank that failed after agreement 1 does no more work, but every
@@ -666,7 +660,7 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
     rc = salt_len > kMaxSalt ? fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: salt_len > 32")
              : salt_len && !salt ? fail(c0, CTMR_E_INVALID, "ctmr_revoked_cascade: NULL salt")
                                  : CTMR_OK;
-    if (rc == CTMR_OK) rc = peer ? crl_peer_prepare(c0, b, out, call, issuer, &n_chunks) : crl_prepare(c0, b, out, call, issuer);
+    if (rc == CTMR_OK) rc = crl_prepare(c0, b, out, call, issuer, &n_chunks);
     if (rc == CTMR_OK && peer) rc = cascade_ensure(c0, 0, 2 * IW, false);
     if (rc == CTMR_OK) rc = refresh_digests(c0);
     if (peer && (rc = peer_agree(c0, rc, n_chunks, row, call, "collective call failed")) == CTMR_OK)  // agreement 1
@@ -754,20 +748,12 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
     build();
 
     const bool short_cap = img.size() > out->cap || !out->buf;
-    if (peer) {
-        const cudaStream_t drain[] = {c0->crl->copy_stream, c0->stream};
-        drain_streams(c0, drain, 2);  // no upload may read the caller's data after the call
-        if (!local.code && (rc = ctmr_check_device(c0, nullptr))) local.fail(c0, rc);  // a barrier that timed out
-        if (local.code) c0->err = local.err;
-        rc = peer_agree(c0, local.code, short_cap ? 1 : 0, row, call, "collective call failed");  // the final agreement
-        if (rc) return rc;
-    } else {
-        if (local.code) {
-            if (g) g->err = local.err;  // the failing member's text is the group's
-            return local.code;
-        }
-        row[0] = short_cap;  // as the only rank
+    rc = peer ? crl_peer_finish(c0, local, short_cap ? 1 : 0, row, call) : local.code;
+    if (rc) {
+        if (g) g->err = local.err;  // the failing member's text is the group's
+        return rc;
     }
+    if (!peer) row[0] = short_cap;  // as the only rank
     out->bytes = img.size();
     const uint32_t world = peer ? c0->st.peer.world : 1, me = peer ? c0->px.rank : 0;
     for (uint32_t r = 0; r < world; ++r)
@@ -924,12 +910,13 @@ int revoked_stash(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
     int rc = set_device(c0);
     if (rc) return group_fail(g, c0, rc);
     std::vector<uint32_t> issuer;
+    uint64_t n_chunks = 0;  // a peer rank's: the stash is refused there
     StashFilter f;
     std::unordered_set<std::string> listed;
     const char* bad = !filter && filter_bytes ? "NULL filter" : !stashes && stash_bytes ? "NULL stashes" : nullptr;
     if (!bad) bad = stash_filter(filter, filter_bytes, f);
     if (!bad) bad = stash_parse(stashes, stash_bytes, listed);
-    rc = bad ? fail(c0, CTMR_E_INVALID, std::string(call) + bad) : crl_prepare(c0, b, out, call, issuer);
+    rc = bad ? fail(c0, CTMR_E_INVALID, std::string(call) + bad) : crl_prepare(c0, b, out, call, issuer, &n_chunks);
     if (rc == CTMR_OK) rc = refresh_digests(c0);
     if (rc) return group_fail(g, c0, rc);
 

@@ -708,34 +708,6 @@ int crl_set_copy(ctmr_ctx* c0, ctmr_ctx* c, uint64_t slots) {
     return CTMR_OK;
 }
 
-// The other members' part of a group's join: each scans its own table against a bulk copy of member 0's set, and member 0
-// merges the answers.  Synchronous; no atomics cross GPUs.
-int crl_scan_members(ctmr_ctx* const* m, uint32_t W, uint64_t slots, ctmr_group* g) {
-    ctmr_ctx* c0 = m[0];
-    CrlState* s0 = c0->crl.get();
-    CU(c0, cudaStreamSynchronize(c0->stream));
-    for (uint32_t r = 1; r < W; ++r) {
-        ctmr_ctx* c = m[r];
-        CU(c, cudaSetDevice(c->device));
-        const int rc = crl_set_copy(c0, c, slots);
-        if (rc) return group_fail(g, c, rc);
-        CrlState* s = c->crl.get();
-        CU(c, cudaMemsetAsync(s->set_hour, 0x7f, slots * sizeof(int32_t), c->stream));
-        CU(c, cudaMemsetAsync(s->set_count, 0, slots * sizeof(uint32_t), c->stream));
-        const uint64_t n_slots = c->st.table_mask + 1;
-        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, n_slots, s->set, slots - 1, s->set_hour, s->set_count);
-        CU(c, cudaGetLastError());
-        CU(c, cudaMemcpyPeerAsync(s0->recv_hour, c0->device, s->set_hour, c->device, slots * sizeof(int32_t), c->stream));
-        CU(c, cudaMemcpyPeerAsync(s0->recv_count, c0->device, s->set_count, c->device, slots * sizeof(uint32_t), c->stream));
-        CU(c, cudaStreamSynchronize(c->stream));
-        CU(c0, cudaSetDevice(c0->device));
-        crl_merge_kernel<<<grid(slots, 256), 256, 0, c0->stream>>>(s0->set_hour, s0->set_count, s0->recv_hour, s0->recv_count, slots);
-        CU(c0, cudaGetLastError());
-        CU(c0, cudaStreamSynchronize(c0->stream));
-    }
-    return CTMR_OK;
-}
-
 // The split of chunk `ch` in stage[st] on the ctx's stream, up to the compaction: *ne = the chunk's entries (epos, ecrl)
 int crl_split(ctmr_ctx* c, const CrlChunk& ch, int st, uint32_t* ne_out) {
     CrlState* s = c->crl.get();
@@ -831,69 +803,35 @@ EntryOut entry_out(CrlState* s) {
     return EntryOut{s->eserial_off, s->eserial_len, s->ereason, s->estatus, s->eknown, s->erevoked, s->ehour, s->eslot, s->esets};
 }
 
+// the per-entry outputs of a parsed chunk's ne entries, on c's stream
+int crl_entries(ctmr_ctx* c, int st, uint32_t ne) {
+    CrlState* s = c->crl.get();
+    crl_entry_kernel<<<grid(ne, 256), 256, 0, c->stream>>>(s->stage[st], s->desc[st], s->res, s->epos, s->ecrl, ne, entry_out(s));
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
+}
+
 // The entries of the chunk in stage[st] (ne of them, ne > 0) parsed, and the set of their (issuer, serial) pairs built on
-// c's stream, with its hour and count answers reset; *slots = the set's slots (its whole allocation: every member of a
-// group probes with the same mask).  `recv`: a group's member 0 also receives the other members' answers.
+// c's stream; *slots = the set's slots (its whole allocation: every member of a group probes with the same mask).
+// `recv`: a group's member 0 also receives the other members' answers.
 int crl_set_build(ctmr_ctx* c, int st, uint32_t ne, bool recv, uint64_t* slots) {
     CrlState* s = c->crl.get();
-    const cudaStream_t q = c->stream;
-    crl_entry_kernel<<<grid(ne, 256), 256, 0, q>>>(s->stage[st], s->desc[st], s->res, s->epos, s->ecrl, ne, entry_out(s));
-    CU(c, cudaGetLastError());
+    int rc = crl_entries(c, st, ne);
+    if (rc) return rc;
     uint64_t n = 64;
     while (n < 2ull * ne) n <<= 1;
-    const int rc = crl_set_ensure(c, n, recv);
-    if (rc) return rc;
+    if ((rc = crl_set_ensure(c, n, recv))) return rc;
     n = s->set_cap;
-    CU(c, cudaMemsetAsync(s->set, 0, n * sizeof(CrlSetSlot), q));
-    CU(c, cudaMemsetAsync(s->set_hour, 0x7f, n * sizeof(int32_t), q));
-    CU(c, cudaMemsetAsync(s->set_count, 0, n * sizeof(uint32_t), q));
-    crl_set_insert_kernel<<<grid(ne, 256), 256, 0, q>>>(s->stage[st], s->desc[st], s->res, s->ecrl, s->eserial_off, s->eserial_len,
-                                                       s->estatus, ne, s->set, n - 1, s->eslot);
+    CU(c, cudaMemsetAsync(s->set, 0, n * sizeof(CrlSetSlot), c->stream));
+    crl_set_insert_kernel<<<grid(ne, 256), 256, 0, c->stream>>>(s->stage[st], s->desc[st], s->res, s->ecrl, s->eserial_off, s->eserial_len,
+                                                                 s->estatus, ne, s->set, n - 1, s->eslot);
     CU(c, cudaGetLastError());
     *slots = n;
     return CTMR_OK;
 }
 
-// One chunk on member 0 (`c`): split, parse, join (every member's table), copy back.  *base: entries placed so far; with
-// `count_only` (the caller's entry_cap is already exceeded) only the count advances.
-int crl_chunk(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, ctmr_crl_out* out, const CrlChunk& ch, int st, uint64_t* base,
-              bool* count_only) {
-    ctmr_ctx* c = m[0];
-    CrlState* s = c->crl.get();
-    cudaStream_t q = c->stream;
-    uint32_t ne = 0;
-    int rc = crl_split(c, ch, st, &ne);
-    if (rc) return rc;
-    if (*count_only || *base + ne > out->entry_cap) {
-        *count_only = true;
-        *base += ne;
-        CU(c, cudaEventRecord(s->consumed[st], q));
-        return CTMR_OK;
-    }
-    const EntryOut eo = entry_out(s);
-    if (ne) {
-        uint64_t slots = 0;
-        rc = crl_set_build(c, st, ne, W > 1, &slots);
-        if (rc) return group_fail(g, c, rc);
-        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->set, slots - 1, s->set_hour, s->set_count);
-        CU(c, cudaGetLastError());
-        if (W > 1) {
-            rc = crl_scan_members(m, W, slots, g);
-            if (rc) return rc;
-        }
-        crl_finish_kernel<<<grid(ne, 256), 256, 0, q>>>(s->eslot, s->set_hour, s->set_count, ne, eo);
-        CU(c, cudaGetLastError());
-    }
-    CU(c, cudaEventRecord(s->consumed[st], q));
-    // per-entry outputs straight into the caller's arrays
-    rc = crl_copy_back(c, out, ch, *base, ne);
-    if (rc) return rc;
-    *base += ne;
-    return CTMR_OK;
-}
-
 // The checks every call makes before any work: the arguments, and each CRL inside data and no larger than a chunk
-int crl_check_batch(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const std::string& call = "ctmr_revoked_known: ") {
+int crl_check_batch(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const std::string& call) {
     if (!b || !out) return fail(c, CTMR_E_INVALID, call + "NULL batch or output");
     if (b->n_crls && (!b->data || !b->crl_off || !b->crl_len || !b->issuer_digest))
         return fail(c, CTMR_E_INVALID, call + "NULL input array");
@@ -960,26 +898,87 @@ int crl_for_chunks(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint3
     return rc;
 }
 
-// the call on member 0 of `W` members (W == 1: one ctx)
-int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, ctmr_crl_out* out) {
-    ctmr_ctx* c = m[0];
-    CU(c, cudaSetDevice(c->device));
-    int rc = crl_check_batch(c, b, out);
-    if (rc) return group_fail(g, c, rc);
-    out->n_entries = 0;
-    if (b->n_crls == 0) return CTMR_OK;
-    std::vector<uint32_t> issuer;
-    rc = crl_issuers(c, b, issuer);
-    if (rc) return group_fail(g, c, rc);
-    uint64_t base = 0;
-    bool count_only = false;
-    rc = crl_for_chunks(c, b, issuer, [&](const CrlChunk& ch, int st) { return crl_chunk(m, W, g, out, ch, st, &base, &count_only); });
-    if (rc) return group_fail(g, c, rc);
-    out->n_entries = base;
-    if (count_only)
-        return group_fail(g, c, fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: entry_cap " + std::to_string(out->entry_cap) + " < " +
-                                                               std::to_string(base) + " entries"));
+// the CTMR_CRL_* of chunk ch's CRLs, parsed on c, into status[ch.lo, ch.hi); waits for c's stream
+int crl_read_status(ctmr_ctx* c, const CrlChunk& ch, std::vector<uint8_t>& status) {
+    const uint32_t n = (uint32_t)(ch.hi - ch.lo);
+    std::vector<CrlRes> res(n);
+    CU(c, cudaMemcpyAsync(res.data(), c->crl->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    for (uint32_t k = 0; k < n; ++k) status[ch.lo + k] = (uint8_t)res[k].status;
     return CTMR_OK;
+}
+
+// What a call does with each chunk of its batch, in both forms' drivers (crl_group_chunks, crl_peer_steps):
+// ctmr_revoked_known joins the entries and gathers their answers, ctmr_revoked_cascade marks every shard.
+struct CrlActions {
+    std::function<bool(uint32_t ne)> take;  // the chunk parsed with ne entries: are they joined (false: only counted)
+    CrlSetVisit visit;     // a shard against a set: a member's copy of the chunk's set, or a peer rank's union set of a round
+    bool answers = false;  // each joined entry's answer is gathered from the visits' hour and count arrays
+    std::function<int(const CrlChunk& ch, uint32_t ne)> done;  // after chunk ch (ne entries), its last read of the stage issued
+};
+
+// The answers of one ctx or a group, after every member's visit: each other member's (hour, count) into member 0's
+// recv_* and merged there, one member at a time in member order, then each entry's answer.  On error *at names the
+// member that failed.
+int crl_group_answers(ctmr_ctx* const* m, uint32_t W, uint64_t slots, uint32_t ne, ctmr_ctx** at) {
+    ctmr_ctx* c0 = m[0];
+    CrlState* s0 = c0->crl.get();
+    for (uint32_t r = 1; r < W; ++r) {
+        ctmr_ctx* c = *at = m[r];
+        CU(c, cudaSetDevice(c->device));
+        CU(c, cudaMemcpyPeerAsync(s0->recv_hour, c0->device, c->crl->set_hour, c->device, slots * sizeof(int32_t), c->stream));
+        CU(c, cudaMemcpyPeerAsync(s0->recv_count, c0->device, c->crl->set_count, c->device, slots * sizeof(uint32_t), c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        *at = c0;
+        CU(c0, cudaSetDevice(c0->device));
+        crl_merge_kernel<<<grid(slots, 256), 256, 0, c0->stream>>>(s0->set_hour, s0->set_count, s0->recv_hour, s0->recv_count, slots);
+        CU(c0, cudaGetLastError());
+        CU(c0, cudaStreamSynchronize(c0->stream));
+    }
+    crl_finish_kernel<<<grid(ne, 256), 256, 0, c0->stream>>>(s0->eslot, s0->set_hour, s0->set_count, ne, entry_out(s0));
+    CU(c0, cudaGetLastError());
+    return CTMR_OK;
+}
+
+// One ctx or a group of W members: member 0 parses each chunk and builds the set of the entries it takes, every other
+// member gets a bulk copy of the set (cudaMemcpyPeerAsync), and each member visits its copy on its own stream; with
+// answers, crl_group_answers follows.  Synchronous; no upload outlives it.  The first failure goes to `local` and stops
+// the call; false: it failed (here, or before).  No atomic crosses a GPU.
+bool crl_group_chunks(ctmr_ctx* const* m, uint32_t W, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlActions& a,
+                      PeerLocal& local) {
+    if (local.code) return false;
+    if (b->n_crls == 0) return true;
+    ctmr_ctx *c0 = m[0], *at = c0;
+    const int rc = crl_for_chunks(c0, b, issuer, [&](const CrlChunk& ch, int st) -> int {
+        uint32_t ne = 0;
+        uint64_t slots = 0;
+        int rc2 = crl_split(c0, ch, st, &ne);
+        const bool sets = rc2 == CTMR_OK && a.take(ne) && ne;
+        if (sets) rc2 = crl_set_build(c0, st, ne, a.answers && W > 1, &slots);
+        if (rc2) return rc2;
+        CU(c0, cudaEventRecord(c0->crl->consumed[st], c0->stream));
+        if (sets) {
+            if (W > 1) CU(c0, cudaStreamSynchronize(c0->stream));  // the other members copy member 0's set
+            for (uint32_t r = 0; r < W; ++r) {
+                ctmr_ctx* c = at = m[r];
+                CU(c, cudaSetDevice(c->device));
+                if (r && (rc2 = crl_set_copy(c0, c, slots))) return rc2;
+                CrlState* s = c->crl.get();
+                if ((rc2 = a.visit(c, CrlSet{s->set, slots - 1, s->set_hour, s->set_count}))) return rc2;
+            }
+            for (uint32_t r = W; r-- > 1;) {  // the next chunk rewrites member 0's set
+                ctmr_ctx* c = at = m[r];
+                CU(c, cudaSetDevice(c->device));
+                CU(c, cudaStreamSynchronize(c->stream));
+            }
+            at = c0;
+            CU(c0, cudaSetDevice(c0->device));
+            if (a.answers && (rc2 = crl_group_answers(m, W, slots, ne, &at))) return rc2;
+        }
+        return a.done(ch, ne);
+    });
+    local.fail(at, rc);
+    return rc == CTMR_OK;
 }
 
 // ---- one process per GPU: the collective call on a ctx attached to peers (include/ctmr.h states the rules) -----------
@@ -996,14 +995,6 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
 // only after its own pull of round j (stream order), and every owner's reads and answers of round j came before the
 // second barrier of round j, which the source has passed.  A final agreement makes any later failure every rank's.
 
-// the per-entry outputs of a parsed chunk's ne entries
-int crl_peer_entries(ctmr_ctx* c, int st, uint32_t ne) {
-    CrlState* s = c->crl.get();
-    crl_entry_kernel<<<grid(ne, 256), 256, 0, c->stream>>>(s->stage[st], s->desc[st], s->res, s->epos, s->ecrl, ne, entry_out(s));
-    CU(c, cudaGetLastError());
-    return CTMR_OK;
-}
-
 // entries [lo, lo + n) of the chunk in stage[st] as records, sent to every rank with the count (n == 0: the count only)
 int crl_peer_send(ctmr_ctx* c, int st, uint64_t lo, uint64_t n) {
     CrlState* s = c->crl.get();
@@ -1017,51 +1008,26 @@ int crl_peer_send(ctmr_ctx* c, int st, uint64_t lo, uint64_t n) {
     return CTMR_OK;
 }
 
-// The union set of a round's valid records (agreed.n[s] from source s, `total` of them, at most `most` from one source),
-// cleared and filled on c's stream; *slots = its slots
-int crl_union_build(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uint64_t total, uint64_t* slots) {
+// the owner's part of a round: the round's valid records (agreed.n[s] from source s, `total` of them, at most `most` from
+// one source) into the union set, the call's visit of the own shard, and with answers each record's answer in place
+int crl_peer_owner(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uint64_t total, const CrlActions& a) {
     CrlState* s = c->crl.get();
-    *slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
-    CU(c, cudaMemsetAsync(s->union_set, 0, *slots * sizeof(CrlSetSlot), c->stream));
-    crl_union_insert_kernel<<<dim3(grid(most, 256), c->px.world), 256, 0, c->stream>>>(c->px, agreed, s->union_set, *slots - 1, c->in_slot);
-    CU(c, cudaGetLastError());
-    return CTMR_OK;
-}
-
-// the owner's part of a round: the union set, then every record's answer from the own shard
-int crl_peer_owner(ctmr_ctx* c, const CrlRoundCounts& agreed, uint64_t most, uint64_t total) {
-    CrlState* s = c->crl.get();
-    const cudaStream_t q = c->stream;
-    uint64_t slots = 0;
-    const int rc = crl_union_build(c, agreed, most, total, &slots);
-    if (rc) return rc;
-    CU(c, cudaMemsetAsync(s->union_hour, 0x7f, slots * sizeof(int32_t), q));
-    CU(c, cudaMemsetAsync(s->union_count, 0, slots * sizeof(uint32_t), q));
-    crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, q>>>(c->st.table, c->st.table_mask + 1, s->union_set, slots - 1, s->union_hour,
-                                                          s->union_count);
-    CU(c, cudaGetLastError());
     const dim3 g(grid(most, 256), c->px.world);
-    crl_peer_answer_kernel<<<g, 256, 0, q>>>(c->px, agreed, c->in_slot, s->union_hour, s->union_count);
+    const uint64_t slots = pow2_at_least(2 * total > 64 ? 2 * total : 64);  // <= union_cap: total <= world X
+    CU(c, cudaMemsetAsync(s->union_set, 0, slots * sizeof(CrlSetSlot), c->stream));
+    crl_union_insert_kernel<<<g, 256, 0, c->stream>>>(c->px, agreed, s->union_set, slots - 1, c->in_slot);
+    CU(c, cudaGetLastError());
+    const int rc = a.visit(c, CrlSet{s->union_set, slots - 1, s->union_hour, s->union_count});
+    if (rc || !a.answers) return rc;
+    crl_peer_answer_kernel<<<g, 256, 0, c->stream>>>(c->px, agreed, c->in_slot, s->union_hour, s->union_count);
     CU(c, cudaGetLastError());
     return CTMR_OK;
 }
 
-// What a collective call does around the shared step and round driver (crl_peer_steps): ctmr_revoked_known answers
-// each rank's entries and pulls the answers back, ctmr_revoked_cascade marks its shard against each round's union set.
-struct CrlPeerActions {
-    std::function<bool(uint32_t ne)> send;  // the rank's chunk parsed with ne entries: does it send them (false: it only serves)
-    // the owner's part of a round, between its two barriers: agreed.n[s] records from source s, `total` in all, at most
-    // `most` from one source
-    std::function<int(const CrlRoundCounts& agreed, uint64_t most, uint64_t total)> owner;
-    std::function<int(uint64_t lo, uint64_t mine)> pull;  // after a round in which the rank sent entries [lo, lo + mine); may be empty
-    // after the rounds of the rank's own chunk `ch` (ne entries, parsed in stage[st]), whose last read of the stage is issued
-    std::function<int(const CrlChunk& ch, int st, uint32_t ne)> done;
-};
-
-// Round j of a step whose sent entries are row[0..world), this rank's chunk in stage[st].  `work` false (this rank
-// failed): nothing but the two barriers, which every rank issues whatever happens, so that a failure never leaves another
-// rank waiting.
-int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int st, const CrlPeerActions& a) {
+// Round j of a step whose sent entries are row[0..world), this rank's chunk in stage[st]; with answers, the rank pulls
+// the answers to the entries it sent.  `work` false (this rank failed): nothing but the two barriers, which every rank
+// issues whatever happens, so that a failure never leaves another rank waiting.
+int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int st, const CrlActions& a) {
     const uint64_t X = c->px.X, lo = j * X;
     const auto in_round = [&](uint64_t n) -> uint64_t { return n > lo ? std::min(X, n - lo) : 0; };
     CrlRoundCounts agreed{};
@@ -1075,18 +1041,22 @@ int crl_peer_round(ctmr_ctx* c, const uint64_t* row, uint64_t j, bool work, int 
     int rc = work ? crl_peer_send(c, st, lo, mine) : CTMR_OK;
     int brc = peer_barrier(c, CH_CRL, c->stream);
     if (rc == CTMR_OK) rc = brc;
-    if (rc == CTMR_OK && work && total) rc = a.owner(agreed, most, total);
+    if (rc == CTMR_OK && work && total) rc = crl_peer_owner(c, agreed, most, total, a);
     brc = peer_barrier(c, CH_CRL, c->stream);
     if (rc == CTMR_OK) rc = brc;
-    if (rc == CTMR_OK && work && mine && a.pull) rc = a.pull(lo, mine);
-    return rc;
+    if (rc || !work || !mine || !a.answers) return rc;
+    CrlState* s = c->crl.get();
+    crl_peer_pull_kernel<<<grid(mine, 256), 256, 0, c->stream>>>(c->px, mine, lo, s->eknown, s->ehour, s->esets);
+    CU(c, cudaGetLastError());
+    return CTMR_OK;
 }
 
-// The steps after agreement 1 (row: every rank's chunk count), up to the final agreement, which the caller makes after
-// draining the streams.  A failure of this rank goes to `local`; false: a rank's failure stopped the steps early (every
-// rank saw it in the same agreement 2), and the ranks go straight to the final agreement.
-bool crl_peer_steps(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const std::vector<CrlChunk>& chunks,
-                    uint64_t* row, const CrlPeerActions& a, PeerLocal& local) {
+// A peer rank's steps after agreement 1 (row: every rank's chunk count), up to the final agreement (crl_peer_finish).  A
+// failure of this rank goes to `local`; false: a rank's failure stopped the steps early (every rank saw it in the same
+// agreement 2), and the ranks go straight to the final agreement.
+bool crl_peer_steps(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlActions& a,
+                    PeerLocal& local) {
+    const std::vector<CrlChunk> chunks = crl_cut(c, b);
     const uint32_t W = c->st.peer.world;
     uint64_t steps = 0;
     for (uint32_t r = 0; r < W; ++r) steps = std::max(steps, row[r]);
@@ -1101,8 +1071,8 @@ bool crl_peer_steps(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint
         if (mine) {
             rc = k + 1 < chunks.size() ? crl_upload(c, b, issuer, chunks[k + 1], st ^ 1) : CTMR_OK;
             if (rc == CTMR_OK) rc = crl_split(c, chunks[k], st, &ne);
-            if (rc == CTMR_OK && a.send(ne) && ne) {
-                rc = crl_peer_entries(c, st, ne);
+            if (rc == CTMR_OK && a.take(ne) && ne) {
+                rc = crl_entries(c, st, ne);
                 send = ne;
             }
             if (rc) local.fail(c, rc);
@@ -1122,131 +1092,107 @@ bool crl_peer_steps(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint
             local.fail(c, fail(c, CTMR_E_CUDA, "cudaEventRecord failed"));
             continue;
         }
-        if ((rc = a.done(chunks[k], st, ne))) local.fail(c, rc);
+        if ((rc = a.done(chunks[k], ne))) local.fail(c, rc);
     }
     return true;
 }
 
-// this rank's part of the collective call
-int revoked_known_peer(ctmr_ctx* c, const ctmr_crl_batch* b, ctmr_crl_out* out) {
-    CU(c, cudaSetDevice(c->device));
-    if (out) out->n_entries = 0;
+// every chunk of the batch through the form's driver: one ctx or a group, or a peer rank after agreement 1
+bool crl_chunks(ctmr_ctx* const* m, uint32_t W, bool peer, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row,
+                const CrlActions& a, PeerLocal& local) {
+    return peer ? crl_peer_steps(m[0], b, issuer, row, a, local) : crl_group_chunks(m, W, b, issuer, a, local);
+}
+
+// ---- the call ---------------------------------------------------------------------------------------------------------
+// One driver answers the call on the members this process holds: a group's W members, one ctx (W == 1), or one rank of
+// a group of processes (W == 1; the call is collective, include/ctmr.h states the rules).  Only these steps differ:
+//   checks   one ctx or a group: a failure returns at once, and n_entries is 0 once the checks pass.  A peer rank:
+//            n_entries is 0 first; the checks and every buffer of the call travel in agreement 1 with its chunk count.
+//   answers  one ctx or a group: crl_group_answers.  A peer rank: each owner answers the records it received in a round
+//            (crl_peer_answer), and each source pulls its records' answers from every owner (crl_peer_pull).
+//   finish   one ctx or a group: its first failure, with the failing member's text.  A peer rank: crl_peer_finish.
+// The entry_cap rule holds in every form: once the entries do not fit, later chunks are only counted, and a peer rank
+// still answers the other ranks' records.
+int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, ctmr_crl_out* out) {
+    ctmr_ctx* c0 = m[0];
+    const bool peer = peer_call(c0);
+    const char* call = "ctmr_revoked_known: ";
+    CU(c0, cudaSetDevice(c0->device));
+    if (peer && out) out->n_entries = 0;
     std::vector<uint32_t> issuer;
-    std::vector<CrlChunk> chunks;
-    // everything that can fail before any work, allocations included, so that it travels in agreement 1
-    int rc = crl_check_batch(c, b, out);
-    if (rc == CTMR_OK) rc = crl_issuers(c, b, issuer);
-    if (rc == CTMR_OK) rc = crl_ensure(c);
-    if (rc == CTMR_OK) rc = crl_peer_ensure(c);
-    if (rc == CTMR_OK) chunks = crl_cut(c, b);
-    uint64_t row[kMaxWorld] = {};
-    rc = peer_agree(c, rc, chunks.size(), row, "ctmr_revoked_known: ", "collective call failed");  // agreement 1
-    if (rc) return rc;
-    CrlState* s = c->crl.get();
-    uint64_t base = 0;
-    bool count_only = false;  // entry_cap is exceeded: the rank still answers the others' records, and sends none of its own
-    PeerLocal local;          // this rank's error after agreement 1: it does no more work, and the ranks stop at the next agreement
-    CrlPeerActions a;
-    a.send = [&](uint32_t ne) {
+    uint64_t n_chunks = 0, row[kMaxWorld] = {};
+    int rc = crl_prepare(c0, b, out, call, issuer, &n_chunks);
+    if (peer) rc = peer_agree(c0, rc, n_chunks, row, call, "collective call failed");  // agreement 1
+    if (rc) return group_fail(g, c0, rc);
+    out->n_entries = 0;
+    uint64_t base = 0;  // entries placed so far
+    bool count_only = false;
+    PeerLocal local;
+    CrlActions a;
+    a.take = [&](uint32_t ne) {
         if (count_only || base + ne > out->entry_cap) count_only = true;
         return !count_only;
     };
-    a.owner = [&](const CrlRoundCounts& agreed, uint64_t most, uint64_t total) { return crl_peer_owner(c, agreed, most, total); };
-    a.pull = [&](uint64_t lo, uint64_t mine) -> int {
-        crl_peer_pull_kernel<<<grid(mine, 256), 256, 0, c->stream>>>(c->px, mine, lo, s->eknown, s->ehour, s->esets);
+    a.visit = [](ctmr_ctx* c, const CrlSet& set) -> int {  // every key whose pair is in the set takes the lowest hour and counts
+        CU(c, cudaMemsetAsync(set.hour, 0x7f, (set.mask + 1) * sizeof(int32_t), c->stream));
+        CU(c, cudaMemsetAsync(set.count, 0, (set.mask + 1) * sizeof(uint32_t), c->stream));
+        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, set.slots, set.mask, set.hour,
+                                                                          set.count);
         CU(c, cudaGetLastError());
         return CTMR_OK;
     };
-    a.done = [&](const CrlChunk& ch, int, uint32_t ne) {
-        const int rc2 = count_only ? CTMR_OK : crl_copy_back(c, out, ch, base, ne);
+    a.answers = true;
+    a.done = [&](const CrlChunk& ch, uint32_t ne) {  // per-entry outputs straight into the caller's arrays
+        const int rc2 = count_only ? CTMR_OK : crl_copy_back(c0, out, ch, base, ne);
         base += ne;
         return rc2;
     };
-    crl_peer_steps(c, b, issuer, chunks, row, a, local);
-    const cudaStream_t drain[] = {s->copy_stream, c->stream};
-    drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
-    if (!local.code && (rc = ctmr_check_device(c, nullptr))) local.fail(c, rc);  // a barrier of a round that timed out
-    if (local.code) c->err = local.err;
-    rc = peer_agree(c, local.code, 0, row, "ctmr_revoked_known: ", "collective call failed");
-    if (rc) return rc;
+    crl_chunks(m, W, peer, b, issuer, row, a, local);
+    rc = peer ? crl_peer_finish(c0, local, 0, row, call) : local.code;
+    if (rc) {
+        if (g) g->err = local.err;  // the failing member's text is the group's
+        return rc;
+    }
     out->n_entries = base;
     if (count_only)
-        return fail(c, CTMR_E_BATCH_TOO_LARGE, "ctmr_revoked_known: entry_cap " + std::to_string(out->entry_cap) + " < " + std::to_string(base) +
-                                                   " entries");
-    return CTMR_OK;
-}
-
-// the CTMR_CRL_* of chunk ch's CRLs, parsed on c, into status[ch.lo, ch.hi); waits for c's stream
-int crl_read_status(ctmr_ctx* c, const CrlChunk& ch, std::vector<uint8_t>& status) {
-    const uint32_t n = (uint32_t)(ch.hi - ch.lo);
-    std::vector<CrlRes> res(n);
-    CU(c, cudaMemcpyAsync(res.data(), c->crl->res, n * sizeof(CrlRes), cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    for (uint32_t k = 0; k < n; ++k) status[ch.lo + k] = (uint8_t)res[k].status;
+        return group_fail(g, c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, std::string(call) + "entry_cap " + std::to_string(out->entry_cap) + " < " +
+                                                               std::to_string(base) + " entries"));
     return CTMR_OK;
 }
 
 }  // namespace
 
-// ---- the chunk path as ctmr_revoked_cascade uses it (ctmr_cascade.cu) -------------------------------------------------
+// ---- the chunk path as ctmr_revoked_cascade and ctmr_revoked_stash use it (ctmr_cascade.cu) ---------------------------
 namespace ctmr_host {
 
-int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer) {
+int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
+                uint64_t* n_chunks) {
+    *n_chunks = 0;
     int rc = crl_check_batch(c, b, out, call);
     if (rc == CTMR_OK) rc = crl_issuers(c, b, issuer);
-    return rc;
-}
-
-int crl_each_set(ctmr_ctx* const* m, uint32_t W, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit,
-                 std::vector<uint8_t>& status, ctmr_ctx** failed) {
-    ctmr_ctx* c0 = *failed = m[0];
-    if (b->n_crls == 0) return CTMR_OK;
-    return crl_for_chunks(c0, b, issuer, [&](const CrlChunk& ch, int st) -> int {
-        uint32_t ne = 0;
-        uint64_t slots = 0;
-        int rc = crl_split(c0, ch, st, &ne);
-        if (rc == CTMR_OK && ne) rc = crl_set_build(c0, st, ne, false, &slots);
-        if (rc) return rc;
-        CU(c0, cudaEventRecord(c0->crl->consumed[st], c0->stream));
-        if ((rc = crl_read_status(c0, ch, status)) || !ne) return rc;
-        for (uint32_t r = 0; r < W; ++r) {
-            ctmr_ctx* c = *failed = m[r];
-            CU(c, cudaSetDevice(c->device));
-            if (r && (rc = crl_set_copy(c0, c, slots))) return rc;
-            if ((rc = visit(c, c->crl->set, slots - 1))) return rc;
-        }
-        for (uint32_t r = W; r-- > 1;) {  // the next chunk rewrites member 0's set
-            ctmr_ctx* c = *failed = m[r];
-            CU(c, cudaSetDevice(c->device));
-            CU(c, cudaStreamSynchronize(c->stream));
-        }
-        *failed = c0;
-        CU(c0, cudaSetDevice(c0->device));
-        return CTMR_OK;
-    });
-}
-
-int crl_peer_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
-                     uint64_t* n_chunks) {
-    *n_chunks = 0;
-    int rc = crl_prepare(c, b, out, call, issuer);
-    if (rc == CTMR_OK) rc = crl_ensure(c);
+    if (rc || !peer_call(c)) return rc;
+    rc = crl_ensure(c);
     if (rc == CTMR_OK) rc = crl_peer_ensure(c);
     if (rc == CTMR_OK) *n_chunks = crl_cut(c, b).size();
     return rc;
 }
 
-bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlSetVisit& visit,
-                       std::vector<uint8_t>& status, PeerLocal& local) {
-    CrlPeerActions a;
-    a.send = [](uint32_t) { return true; };
-    a.owner = [&](const CrlRoundCounts& agreed, uint64_t most, uint64_t total) -> int {
-        uint64_t slots = 0;
-        const int rc = crl_union_build(c, agreed, most, total, &slots);
-        return rc ? rc : visit(c, c->crl->union_set, slots - 1);
-    };
-    a.done = [&](const CrlChunk& ch, int, uint32_t) { return crl_read_status(c, ch, status); };
-    return crl_peer_steps(c, b, issuer, crl_cut(c, b), row, a, local);
+bool crl_each_set(ctmr_ctx* const* m, uint32_t W, bool peer, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row,
+                  const CrlSetVisit& visit, std::vector<uint8_t>& status, PeerLocal& local) {
+    CrlActions a;
+    a.take = [](uint32_t) { return true; };
+    a.visit = visit;
+    a.done = [&](const CrlChunk& ch, uint32_t) { return crl_read_status(m[0], ch, status); };
+    return crl_chunks(m, W, peer, b, issuer, row, a, local);
+}
+
+int crl_peer_finish(ctmr_ctx* c, PeerLocal& local, uint64_t payload, uint64_t* row, const char* call) {
+    const cudaStream_t drain[] = {c->crl->copy_stream, c->stream};
+    drain_streams(c, drain, 2);  // no upload may read the caller's data after the call
+    int rc = CTMR_OK;
+    if (!local.code && (rc = ctmr_check_device(c, nullptr))) local.fail(c, rc);  // a barrier of a round that timed out
+    if (local.code) c->err = local.err;
+    return peer_agree(c, local.code, payload, row, call, "collective call failed");  // the final agreement
 }
 
 }  // namespace ctmr_host
@@ -1256,7 +1202,6 @@ extern "C" {
 int ctmr_revoked_known(ctmr_ctx* c, const ctmr_crl_batch* batch, ctmr_crl_out* out) {
     if (!c) return CTMR_E_INVALID;
     if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_known: a member of a group; use ctmr_group_revoked_known");
-    if (peer_call(c)) return revoked_known_peer(c, batch, out);
     ctmr_ctx* m[1] = {c};
     return revoked_known(m, 1, nullptr, batch, out);
 }

@@ -623,20 +623,9 @@ int reset_tables(ctmr_ctx* c, cudaStream_t s);
 // after the registry was replaced: the host memos of it go, and so do the Chain[0] mirror and the tiles' fingerprints
 int clear_issuer_memos(ctmr_ctx* c);
 
-// ctmr_revoked_cascade's use of the CRL path (ctmr_crl.cu).  crl_prepare: ctmr_revoked_known's checks before any work
-// (`out` is only tested for NULL; `call` opens the error text), then each CRL's dense issuer (CTMR_ISSUER_NONE when the
-// digest is not registered).  crl_each_set, on member 0 of W members (a group, or one ctx): every chunk through the
-// split, the entries and the set of its (issuer, serial) pairs, and status[] gets the CTMR_CRL_* of its CRLs; then each
-// member, its device current, gets visit(member, a copy of the set on its device (member 0: the set), mask) on its
-// stream while the set is intact (a chunk with no entries: no visit).  Synchronous; no upload outlives it.  On error
-// *failed names the member that failed.
-using CrlSetVisit = std::function<int(ctmr_ctx* c, const CrlSetSlot* set, uint64_t mask)>;
-int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer);
-int crl_each_set(ctmr_ctx* const* m, uint32_t W, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, const CrlSetVisit& visit,
-                 std::vector<uint8_t>& status, ctmr_ctx** failed);
-
-// A rank's own failure in a collective call after its first agreement: it does no more work but still meets every barrier
-// and agreement of the call, and the first failure's code and text are kept for the final agreement.
+// A failure of one ctx, a group or a peer rank in a CRL call.  One ctx or a group stops at the first; a peer rank that
+// failed after its first agreement does no more work but still meets every barrier and agreement of the call.  The first
+// failure's code and text are kept (for a peer rank, for the final agreement).
 struct PeerLocal {
     int code = CTMR_OK;
     std::string err;
@@ -647,17 +636,38 @@ struct PeerLocal {
     }
 };
 
-// ctmr_revoked_cascade's collective use of the CRL exchange (ctmr_crl.cu).  crl_peer_prepare: crl_prepare, then the
-// split's and the exchange's buffers and the number of chunks, so that every failure before any work travels in
-// agreement 1.  crl_peer_each_set: after agreement 1 (row: every rank's chunk count), the step and round driver of the
-// collective ctmr_revoked_known; in each round, visit(c, the union set of every rank's valid records of the round, mask)
-// is issued on c's stream between the round's two barriers, and status[] gets the CTMR_CRL_* of the rank's own CRLs.
-// This rank's failures go to `local`; false: a rank's failure stopped the steps, and the ranks go to the final agreement.
-// The caller drains c's streams (the copy stream too) before that agreement.
-int crl_peer_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
-                     uint64_t* n_chunks);
-bool crl_peer_each_set(ctmr_ctx* c, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row, const CrlSetVisit& visit,
-                       std::vector<uint8_t>& status, PeerLocal& local);
+// The CRL path as ctmr_revoked_cascade and ctmr_revoked_stash use it (ctmr_crl.cu, whose ctmr_revoked_known runs the same
+// drivers).  crl_prepare: the checks every CRL call makes before any work (`out` is only tested for NULL; `call` opens the
+// error text), then each CRL's dense issuer (CTMR_ISSUER_NONE when the digest is not registered); on a peer rank
+// (peer_call) also the split's and the exchange's buffers and *n_chunks, the batch's chunk count, so that every failure
+// before any work travels in agreement 1 (*n_chunks is 0 otherwise).
+int crl_prepare(ctmr_ctx* c, const ctmr_crl_batch* b, const void* out, const char* call, std::vector<uint32_t>& issuer,
+                uint64_t* n_chunks);
+
+// A set of (issuer, serial) pairs on a member's device, mask + 1 slots, and per slot the answer arrays a join fills: the
+// lowest hour and the number of sets that hold the pair.
+struct CrlSet {
+    const CrlSetSlot* slots;
+    uint64_t mask;
+    int32_t* hour;
+    uint32_t* count;
+};
+using CrlSetVisit = std::function<int(ctmr_ctx* c, const CrlSet& set)>;
+// crl_each_set: every chunk through the split, its entries and the set of its (issuer, serial) pairs; status[] gets the
+// CTMR_CRL_* of this process's CRLs, and visit(c, set) is issued on c's stream, its device current, while the set is
+// intact.  One ctx or a group (peer false; W members): member 0 builds each chunk's set, and every member visits a copy
+// on its device (a chunk with no entries: no visit); synchronous, and no upload outlives it.  A peer rank (peer true,
+// W == 1), after agreement 1 (row: every rank's chunk count): the steps and rounds of the collective
+// ctmr_revoked_known, and in each round the rank visits the union set of every rank's valid records of the round,
+// between the round's two barriers.  Failures go to `local`; false: the call stops (one ctx or a group failed, or a
+// rank's failure stopped the steps and the ranks go to the final agreement).
+bool crl_each_set(ctmr_ctx* const* m, uint32_t W, bool peer, const ctmr_crl_batch* b, const std::vector<uint32_t>& issuer, uint64_t* row,
+                  const CrlSetVisit& visit, std::vector<uint8_t>& status, PeerLocal& local);
+// crl_peer_finish: a peer rank's end of a CRL call after crl_each_set.  The ctx's copy stream and stream are drained (no
+// upload may read the caller's data afterwards), the device is checked for a barrier that timed out, the text of the
+// rank's first failure is restored, and the final agreement posts `payload` (row: every rank's).  Returns peer_agree's
+// code.
+int crl_peer_finish(ctmr_ctx* c, PeerLocal& local, uint64_t payload, uint64_t* row, const char* call);
 
 // Where a table's live slots go when they are compacted in slot order (launch_evict_compact): the exclusive prefix of the
 // live slots per tile of kCompactTile, on the host and on the device.  host[tiles()] = the live slots of the table.

@@ -133,6 +133,7 @@ static void fill_map_params(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev
             p.route.rank = c->px.rank;
         }
         p.table_mask = c->st.table_mask;
+        p.epoch = c->st.epoch;
         p.error_flag = c->st.error_flag;
         p.slot_of = fused_slot_of;
     }
@@ -649,6 +650,7 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
     CU(nullptr, cudaMemsetAsync(c->small, 0, sizeof(SmallDev), c->stream));
     c->st.slots_used = &c->small->slots_used;
     c->st.error_flag = &c->small->error_flag;
+    c->st.epoch = 1u;  // the tables were just zeroed: empty at any epoch
     {
         uint8_t* self[1] = {c->shared};
         attach_views(c.get(), self, 1, 0);  // a single GPU is a group of one
@@ -967,7 +969,9 @@ int ctmr_reset_device(ctmr_ctx* c, void* stream) {
     CU(c, cudaSetDevice(c->device));
     cudaStream_t s = stream ? (cudaStream_t)stream : c->stream;
     // multi-process group: collective.  Nobody may still be inserting into this shard when it is cleared, and nobody
-    // may insert into it again before it has been cleared.
+    // may insert into it again before it has been cleared.  Every rank advances its epoch here (and a checkpoint load,
+    // also collective, resets every rank), so the ranks' epochs move in lockstep: a cross-GPU string-identity insert stamps
+    // its own epoch, which is the owner's.
     int rc = peer_barrier(c, CH_RESET_A, s);
     if (rc == CTMR_OK) rc = reset_tables(c, s);
     return rc ? rc : peer_barrier(c, CH_RESET_B, s);
@@ -1060,14 +1064,29 @@ uint64_t snap_shard_bytes(ctmr_ctx* c) {
            c->st.max_issuers * sizeof(uint64_t) + CTMR_ST__COUNT * sizeof(uint64_t);
 }
 
+// a snapshot holds the tables in canonical form (ctmr_common.cuh): what they held before epochs, byte for byte.  The
+// slots lie at any alignment in the caller's buffer (after the snapshot header), so each is copied out and back.
+template <class Slot>
+static void canonical_slots(uint8_t* p, uint64_t n, uint32_t epoch) {
+    for (uint64_t i = 0; i < n; ++i, p += sizeof(Slot)) {
+        Slot s;
+        std::memcpy(&s, p, sizeof s);
+        s = canonical_slot(s, slot_state(state_word(s), epoch) == kSlotReady);
+        std::memcpy(p, &s, sizeof s);
+    }
+}
+
 int snap_shard_save(ctmr_ctx* c, uint8_t* p) {
     CU(c, cudaSetDevice(c->device));
     CU(c, cudaDeviceSynchronize());
     const uint64_t t = (c->st.table_mask + 1) * sizeof(KnownSlot), pr = (c->st.pair_mask + 1) * sizeof(PairSlot),
                    m = (c->st.meta_mask + 1) * sizeof(MetaSlot), ic = c->st.max_issuers * sizeof(uint64_t);
-    CU(c, cudaMemcpy(p, c->st.table, t, cudaMemcpyDeviceToHost)); p += t;
-    CU(c, cudaMemcpy(p, c->st.pairs, pr, cudaMemcpyDeviceToHost)); p += pr;
-    CU(c, cudaMemcpy(p, c->st.meta, m, cudaMemcpyDeviceToHost)); p += m;
+    CU(c, cudaMemcpy(p, c->st.table, t, cudaMemcpyDeviceToHost));
+    canonical_slots<KnownSlot>(p, c->st.table_mask + 1, c->st.epoch); p += t;
+    CU(c, cudaMemcpy(p, c->st.pairs, pr, cudaMemcpyDeviceToHost));
+    canonical_slots<PairSlot>(p, c->st.pair_mask + 1, c->st.epoch); p += pr;
+    CU(c, cudaMemcpy(p, c->st.meta, m, cudaMemcpyDeviceToHost));
+    canonical_slots<MetaSlot>(p, c->st.meta_mask + 1, c->st.epoch); p += m;
     CU(c, cudaMemcpy(p, c->st.issuer_counts, ic, cudaMemcpyDeviceToHost)); p += ic;
     CU(c, cudaMemcpy(p, c->st.status_counts, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     return CTMR_OK;
@@ -1083,6 +1102,8 @@ int snap_shard_load(ctmr_ctx* c, const uint8_t* p) {
     CU(c, cudaMemcpy(c->st.meta, p, m, cudaMemcpyHostToDevice)); p += m;
     CU(c, cudaMemcpy(c->st.issuer_counts, p, ic, cudaMemcpyHostToDevice)); p += ic;
     CU(c, cudaMemcpy(c->st.status_counts, p, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    CU(c, launch_stamp_tables(c->st, c->sm_count, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
     return clear_issuer_memos(c);
 }
 
@@ -1095,10 +1116,16 @@ int clear_issuer_memos(ctmr_ctx* c) {
     return CTMR_OK;
 }
 
+// The tables are emptied by advancing the epoch: every slot of the old one is empty from the next launch on (kernels
+// take the epoch by value, so the ones already queued still see theirs).  Only when the 16-bit epoch wraps are they zeroed.
 int reset_tables(ctmr_ctx* c, cudaStream_t s) {
-    CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), s));
-    CU(c, cudaMemsetAsync(c->st.pairs, 0, (c->st.pair_mask + 1) * sizeof(PairSlot), s));
-    CU(c, cudaMemsetAsync(c->st.meta, 0, (c->st.meta_mask + 1) * sizeof(MetaSlot), s));
+    c->st.epoch = next_epoch(c->st.epoch);
+    if (c->st.epoch == 0u) {
+        CU(c, cudaMemsetAsync(c->st.table, 0, (c->st.table_mask + 1) * sizeof(KnownSlot), s));
+        CU(c, cudaMemsetAsync(c->st.pairs, 0, (c->st.pair_mask + 1) * sizeof(PairSlot), s));
+        CU(c, cudaMemsetAsync(c->st.meta, 0, (c->st.meta_mask + 1) * sizeof(MetaSlot), s));
+        c->st.epoch = 1u;
+    }
     CU(c, cudaMemsetAsync(c->st.issuer_counts, 0, c->st.max_issuers * sizeof(unsigned long long), s));
     CU(c, cudaMemsetAsync(c->st.status_counts, 0, CTMR_ST__COUNT * sizeof(unsigned long long), s));
     CU(c, cudaMemsetAsync(&c->small->slots_used, 0, offsetof(SmallDev, cardinality), s));  // slots_used and the error flag
@@ -1311,7 +1338,7 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     }
     CU(c, launch_evict_pairs(c->st, now_unix_sec, c->sm_count, c->stream));  // the expired sets' cardinalities are 0 again
     if (counters[0])
-        CU(c, launch_evict_compact(c->st.table, slots, now_unix_sec, 0, plan.tiles(), plan.dev.get(), keep.get(), (uint32_t*)nullptr, c->stream));
+        CU(c, launch_evict_compact(c->st.table, slots, c->st.epoch, now_unix_sec, 0, plan.tiles(), plan.dev.get(), keep.get(), (uint32_t*)nullptr, c->stream));
     CU(c, cudaMemsetAsync(c->st.table, 0, slots * sizeof(KnownSlot), c->stream));
     CU(c, launch_evict_reinsert(c->st, keep, counters[0], c->st.max_issuers, false, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));

@@ -30,6 +30,7 @@ constexpr uint32_t kNoList = 0xFFFFFFFFu;
 struct CascadeParams {
     const KnownSlot* table;
     uint64_t n_slots;
+    uint32_t epoch;
     const uint8_t* dig;        // [n_issuers][32] by dense index
     const uint32_t* covered;   // bit per dense index
     uint32_t n_issuers;
@@ -40,8 +41,8 @@ struct CascadeParams {
     uint32_t one;              // always 1: sha256_compress's multiplier ptxas cannot fold
 };
 
-__device__ __forceinline__ bool slot_live_ready(uint4 q0, uint4 q1, int64_t now) {
-    return (q0.z & 3u) == 2u && (int64_t)(int32_t)q1.x * 3600 > now;
+__device__ __forceinline__ bool slot_live_ready(uint4 q0, uint4 q1, uint32_t epoch, int64_t now) {
+    return slot_state(((uint64_t)q0.w << 32) | q0.z, epoch) == kSlotReady && (int64_t)(int32_t)q1.x * 3600 > now;
 }
 
 __device__ __forceinline__ bool issuer_covered(const CascadeParams& p, uint32_t issuer) {
@@ -123,12 +124,12 @@ __device__ __forceinline__ void append(uint32_t slot, uint32_t* list, uint64_t c
 }
 
 // per chunk: every live ready key whose (issuer, serial) is in the set marks its slot revoked
-__global__ void __launch_bounds__(256) cascade_mark_kernel(const KnownSlot* __restrict__ table, uint64_t n_slots, int64_t now,
+__global__ void __launch_bounds__(256) cascade_mark_kernel(const KnownSlot* __restrict__ table, uint64_t n_slots, uint32_t epoch, int64_t now,
                                                            const CrlSetSlot* __restrict__ set, uint64_t mask, uint32_t* revoked) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_slots; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint4* sp = reinterpret_cast<const uint4*>(table + i);
         const uint4 q0 = __ldcs(sp), q1 = __ldcs(sp + 1);
-        if (!slot_live_ready(q0, q1, now)) continue;
+        if (!slot_live_ready(q0, q1, epoch, now)) continue;
         const uint4 q2 = __ldcs(sp + 2), q3 = __ldcs(sp + 3);
         const uint32_t w[11] = {q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
         const uint32_t h = pair_hash(w), ready = (h & ~3u) | 2u;
@@ -156,7 +157,7 @@ __global__ void __launch_bounds__(256) cascade_split_kernel(CascadeParams p, con
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n_slots; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint4* sp = reinterpret_cast<const uint4*>(p.table + i);
         const uint4 q0 = __ldcs(sp), q1 = __ldcs(sp + 1);
-        if (!slot_live_ready(q0, q1, p.now) || !issuer_covered(p, q1.y)) continue;
+        if (!slot_live_ready(q0, q1, p.epoch, p.now) || !issuer_covered(p, q1.y)) continue;
         if (__ldg(revoked + (i >> 5)) >> (i & 31u) & 1u) append((uint32_t)i, rlist, cap, counters);
         else ++valid;
     }
@@ -204,7 +205,7 @@ __global__ void __launch_bounds__(kCascadeThreads) cascade_test_table_kernel(Cas
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n_slots; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint4* sp = reinterpret_cast<const uint4*>(p.table + i);
         const uint4 q0 = __ldcs(sp), q1 = __ldcs(sp + 1);
-        if (!slot_live_ready(q0, q1, p.now) || !issuer_covered(p, q1.y)) continue;
+        if (!slot_live_ready(q0, q1, p.epoch, p.now) || !issuer_covered(p, q1.y)) continue;
         if (__ldg(revoked + (i >> 5)) >> (i & 31u) & 1u) continue;
         uint32_t b[12];
         load_body(p.table, i, b);
@@ -390,6 +391,7 @@ struct Cascade {
         CascadeParams q = p;
         q.table = c->st.table;
         q.n_slots = c->st.table_mask + 1;
+        q.epoch = c->st.epoch;
         q.dig = c->cascade->dig;
         q.covered = c->cascade->covered;
         return q;
@@ -571,7 +573,7 @@ bool cascade_front(Cascade& cs, const ctmr_crl_batch* b, const std::vector<uint3
 
     // mark: every member's shard against each chunk's set, or a peer rank's against each round's union set
     const CrlSetVisit mark = [&](ctmr_ctx* c, const CrlSet& set) -> int {
-        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, now, set.slots, set.mask,
+        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, c->st.epoch, now, set.slots, set.mask,
                                                                     c->cascade->revoked);
         return launched(c);
     };

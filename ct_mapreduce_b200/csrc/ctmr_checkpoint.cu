@@ -50,7 +50,7 @@ int save_records(ctmr_ctx* c, const Slot* table, uint64_t n_slots, const Compact
         while (t1 < plan.tiles() && base[t1 + 1] - base[t0] <= cap) ++t1;
         const uint64_t n = base[t1] - base[t0];
         if (!n) continue;
-        CU(c, launch_evict_compact(table, n_slots, kEveryKey, t0, t1, plan.dev.get(), stage, (uint32_t*)nullptr, c->stream));
+        CU(c, launch_evict_compact(table, n_slots, c->st.epoch, kEveryKey, t0, t1, plan.dev.get(), stage, (uint32_t*)nullptr, c->stream));
         CU(c, cudaMemcpyAsync(dst + base[t0] * sizeof(Slot), stage, n * sizeof(Slot), cudaMemcpyDeviceToHost, c->stream));
         CU(c, cudaStreamSynchronize(c->stream));
     }

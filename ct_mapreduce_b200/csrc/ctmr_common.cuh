@@ -17,12 +17,83 @@ __device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned lon
     return *reinterpret_cast<const volatile unsigned long long*>(p);
 }
 
-__device__ __forceinline__ uint64_t key_hash(const uint32_t (&b)[12]) {
+__device__ __host__ __forceinline__ uint64_t key_hash(const uint32_t (&b)[12]) {
     uint64_t h = 0x9E3779B97F4A7C15ull;
 #pragma unroll
     for (int i = 0; i < 12; i += 2) h = mix64(h ^ (((uint64_t)b[i + 1] << 32) | b[i])) + 0x632BE59BD9B4E019ull * (i + 1);
     return h;
 }
+
+// ------------------------------------------------------------------------------------------------
+// table epochs.  ctmr_reset_device empties the known-certificate, pair and string-identity tables by advancing the ctx's
+// epoch (DeviceState::epoch, 1..kEpochMax) instead of clearing gigabytes: a slot is live only if its state is non-zero AND
+// it carries the current epoch; every other slot is empty, and an insert may claim it.  Zeroed memory is empty at any epoch.
+//   KnownSlot.tag:                  epoch in bits 48..63 | key_hash bits 2..47 | state in bits 0..1
+//   PairSlot.pad / MetaSlot.pad:    epoch in bits 48..63 | state in bits 0..1
+// The state is pending (claimed, being written) or ready (published by a release store).  Snapshots and checkpoints hold
+// slots in their canonical form, which carries no epoch: a KnownSlot tag of the full key_hash with the ready state, a zero
+// pad, and all-zero bytes for an empty slot.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kEpochMax = 0xFFFFu;
+constexpr uint32_t kSlotPending = 1u, kSlotReady = 2u;
+constexpr uint64_t kTagHashBits = 0x0000FFFFFFFFFFFCull;
+
+// the state word of a slot: `h` = the key's key_hash for a KnownSlot tag, 0 for a pad word
+__device__ __host__ __forceinline__ uint64_t slot_word(uint32_t epoch, uint32_t state, uint64_t h = 0) {
+    return ((uint64_t)epoch << 48) | (h & kTagHashBits) | state;
+}
+// the state of a slot at `epoch`: 0 (empty) unless the word carries that epoch
+__device__ __host__ __forceinline__ uint32_t slot_state(uint64_t w, uint32_t epoch) {
+    return (uint32_t)(w >> 48) == epoch ? (uint32_t)w & 3u : 0u;
+}
+__device__ __host__ __forceinline__ bool tag_hash_eq(uint64_t tag, uint64_t h) { return ((tag ^ h) & kTagHashBits) == 0ull; }
+// the canonical tag of a ready key (what the tables held before epochs, and what snapshots and checkpoints store)
+__device__ __host__ __forceinline__ uint64_t canonical_tag(const uint32_t (&body)[12]) { return (key_hash(body) & ~3ull) | kSlotReady; }
+// the epoch after a reset; 0: the epoch wraps, the tables must be zeroed and the next epoch is 1
+__device__ __host__ __forceinline__ uint32_t next_epoch(uint32_t epoch) { return epoch < kEpochMax ? epoch + 1u : 0u; }
+
+// a live slot in canonical form; `live` = false: all zero
+__device__ __host__ __forceinline__ KnownSlot canonical_slot(const KnownSlot& s, bool live) {
+    KnownSlot o{};
+    if (live) {
+        o = s;
+        o.tag = canonical_tag(s.body);
+    }
+    return o;
+}
+__device__ __host__ __forceinline__ PairSlot canonical_slot(const PairSlot& s, bool live) {
+    PairSlot o{};
+    if (live) {
+        o = s;
+        o.pad = 0ull;
+    }
+    return o;
+}
+__device__ __host__ __forceinline__ MetaSlot canonical_slot(const MetaSlot& s, bool live) {
+    MetaSlot o{};
+    if (live) {
+        o = s;
+        o.pad = 0ull;
+    }
+    return o;
+}
+__device__ __host__ __forceinline__ uint64_t state_word(const KnownSlot& s) { return s.tag; }
+__device__ __host__ __forceinline__ uint64_t state_word(const PairSlot& s) { return s.pad; }
+__device__ __host__ __forceinline__ uint64_t state_word(const MetaSlot& s) { return s.pad; }
+__device__ __host__ __forceinline__ unsigned long long& state_word(KnownSlot& s) { return s.tag; }
+__device__ __host__ __forceinline__ unsigned long long& state_word(PairSlot& s) { return s.pad; }
+__device__ __host__ __forceinline__ unsigned long long& state_word(MetaSlot& s) { return s.pad; }
+// a state word moved from epoch `from` to epoch `to` (ranks agreeing on one epoch at ctmr_peer_attach): a slot live at
+// `from` is live at `to`, any other word is left as it is (a ctx's slots never carry an epoch above its own)
+__device__ __host__ __forceinline__ uint64_t restamp_word(uint64_t w, uint32_t from, uint32_t to) {
+    return slot_state(w, from) == kSlotReady ? slot_word(to, kSlotReady, w) : w;
+}
+// a canonical slot as live at `epoch` (a snapshot's slots on their way in): ready if canonical form calls it live, else empty
+__device__ __host__ __forceinline__ void stamp_slot(KnownSlot& s, uint32_t epoch) {
+    s.tag = (s.tag & 3ull) == kSlotReady ? slot_word(epoch, kSlotReady, s.tag) : 0ull;
+}
+__device__ __host__ __forceinline__ void stamp_slot(PairSlot& s, uint32_t epoch) { s.pad = s.key != 0ull ? slot_word(epoch, kSlotReady) : 0ull; }
+__device__ __host__ __forceinline__ void stamp_slot(MetaSlot& s, uint32_t epoch) { s.pad = s.h1 != 0ull ? slot_word(epoch, kSlotReady) : 0ull; }
 
 // Scope of the table atomics: device scope on a single GPU, system scope once peers' tables are addressed
 // over NVLink (the atomic is performed at the owner's L2 either way; the scope decides what it is ordered with).
@@ -57,31 +128,39 @@ template <bool SYS>
 __device__ __forceinline__ uint4 ld_slot_u4(const uint4* p) { return SYS ? __ldcv(p) : __ldcg(p); }
 __device__ __forceinline__ uint4 ld_cv_u4(const uint4* p) { return __ldcv(p); }
 
-// Find-or-insert of a 48-byte key body; lowest global index wins through an atomic max on ~index.  An empty slot is
-// claimed by an optimistic CAS (the tag read is the CAS's return value), the key bytes are published by a release
-// store of the ready tag.  Returns the slot, or 0xFFFFFFFF when the table is full (error flag set).  Shared by
-// K_insert and by K_map's fused insert; SYS = system scope (only the string-identity table is touched across GPUs).
+// Find-or-insert of a 48-byte key body; lowest global index wins through an atomic max on ~index.  A slot empty at
+// `epoch` (zero, or left by an earlier epoch) is claimed by a CAS from the tag observed to pending; the claimer writes
+// the key bytes and inv_first, then publishes them by a release store of the ready tag (a slot of an earlier epoch may
+// hold a larger ~index, so inv_first is stored, not max'ed, and before the release).  Equal keys act only once they see
+// ready.  Returns the slot, or 0xFFFFFFFF when the table is full (error flag set).  Shared by K_insert and by K_map's
+// fused insert; SYS = system scope (only the string-identity table is touched across GPUs).
 template <bool SYS>
-__device__ __forceinline__ uint32_t known_insert(KnownSlot* __restrict__ table, uint64_t table_mask, int* error_flag,
+__device__ __forceinline__ uint32_t known_insert(KnownSlot* __restrict__ table, uint64_t table_mask, uint32_t epoch, int* error_flag,
                                                  const uint32_t (&body)[12], unsigned long long inv_idx) {
     const uint64_t h = key_hash(body);
-    const unsigned long long tag_ready = (h & ~3ull) | 2ull, tag_pending = (h & ~3ull) | 1ull;
+    const unsigned long long tag_ready = slot_word(epoch, kSlotReady, h), tag_pending = slot_word(epoch, kSlotPending, h);
     uint64_t pos = (h >> 7) & table_mask;
     uint32_t probes = 0;
     for (;;) {
         KnownSlot* sl = table + pos;
-        unsigned long long t = tab_cas<SYS>(&sl->tag, 0ull, tag_pending);
-        if (t == 0ull) {  // claimed: publish the key bytes, then flip to ready
+        unsigned long long t = ld_volatile_u64(&sl->tag);  // relaxed: an acquire here would invalidate the SM's L1 per probe
+        if (slot_state(t, epoch) == 0u) {
+            const unsigned long long seen = t;
+            t = tab_cas<SYS>(&sl->tag, seen, tag_pending);
+            if (t != seen) continue;  // another thread claimed the slot first: look at it again
             uint4* bp = reinterpret_cast<uint4*>(sl->body);
             bp[0] = make_uint4(body[0], body[1], body[2], body[3]);
             bp[1] = make_uint4(body[4], body[5], body[6], body[7]);
             bp[2] = make_uint4(body[8], body[9], body[10], body[11]);
+            sl->inv_first = inv_idx;
             tab_store_release<SYS>(&sl->tag, tag_ready);
-            tab_max<SYS>(&sl->inv_first, inv_idx);
             return (uint32_t)pos;
         }
-        if ((t & ~3ull) == (h & ~3ull)) {
-            while ((t & 3ull) == 1ull) t = tab_load_acquire<SYS>(&sl->tag);  // another thread is publishing this slot
+        if (tag_hash_eq(t, h)) {
+            // the key bytes are read only after an acquire of the ready tag: a relaxed read of ready does not order them,
+            // and a slot of the last epoch may hold an equal key
+            do t = tab_load_acquire<SYS>(&sl->tag);  // pending: another thread is publishing this slot
+            while (slot_state(t, epoch) == kSlotPending);
             const uint4* bp = reinterpret_cast<const uint4*>(sl->body);
             const uint4 b0 = ld_slot_u4<SYS>(bp), b1 = ld_slot_u4<SYS>(bp + 1), b2 = ld_slot_u4<SYS>(bp + 2);
             const bool same = b0.x == body[0] && b0.y == body[1] && b0.z == body[2] && b0.w == body[3] && b1.x == body[4] &&

@@ -391,13 +391,13 @@ __global__ void __launch_bounds__(256) crl_set_insert_kernel(const uint8_t* __re
 }
 
 // one pass over the table: every ready key probes the set with its (issuer, serial); a hit records the key's hour
-__global__ void __launch_bounds__(256) crl_known_scan_kernel(const KnownSlot* __restrict__ table, uint64_t n_slots,
+__global__ void __launch_bounds__(256) crl_known_scan_kernel(const KnownSlot* __restrict__ table, uint64_t n_slots, uint32_t epoch,
                                                              const CrlSetSlot* __restrict__ set, uint64_t mask, int32_t* hour,
                                                              uint32_t* count) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_slots; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint4* sp = reinterpret_cast<const uint4*>(table + i);
         const uint4 q0 = __ldcs(sp), q1 = __ldcs(sp + 1), q2 = __ldcs(sp + 2), q3 = __ldcs(sp + 3);
-        if ((q0.z & 3u) != 2u) continue;  // tag's low word: ready
+        if (slot_state(((uint64_t)q0.w << 32) | q0.z, epoch) != kSlotReady) continue;
         const uint32_t w[11] = {q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
         const uint32_t h = pair_hash(w), ready = (h & ~3u) | 2u;
         uint64_t pos = h & mask;
@@ -1136,7 +1136,7 @@ int revoked_known(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
     a.visit = [](ctmr_ctx* c, const CrlSet& set) -> int {  // every key whose pair is in the set takes the lowest hour and counts
         CU(c, cudaMemsetAsync(set.hour, 0x7f, (set.mask + 1) * sizeof(int32_t), c->stream));
         CU(c, cudaMemsetAsync(set.count, 0, (set.mask + 1) * sizeof(uint32_t), c->stream));
-        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, set.slots, set.mask, set.hour,
+        crl_known_scan_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->st.table, c->st.table_mask + 1, c->st.epoch, set.slots, set.mask, set.hour,
                                                                           set.count);
         CU(c, cudaGetLastError());
         return CTMR_OK;

@@ -23,6 +23,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "ctmr_common.cuh"
 #include "ctmr_device.cuh"
 #include "ctmr_kernels.cuh"
 
@@ -684,7 +685,7 @@ int compact_plan(ctmr_ctx* c, const Slot* table, uint64_t n_slots, int64_t now_s
     std::vector<uint32_t> h(tiles);
     CU(c, alloc(counts, tiles));
     CU(c, alloc(p.dev, tiles + 1));
-    CU(c, launch_evict_compact(table, n_slots, now_sec, 0, tiles, (const unsigned long long*)nullptr, (Slot*)nullptr, counts.get(), c->stream));
+    CU(c, launch_evict_compact(table, n_slots, c->st.epoch, now_sec, 0, tiles, (const unsigned long long*)nullptr, (Slot*)nullptr, counts.get(), c->stream));
     CU(c, cudaMemcpyAsync(h.data(), counts, tiles * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     p.host.assign(tiles + 1, 0);

@@ -24,25 +24,25 @@ static_assert(sizeof(FilterCfg) == 16 + 66 + 446, "FilterCfg layout");
 // known-certificate slot: 64 bytes = two 32-byte sectors
 struct __align__(16) KnownSlot {
     unsigned long long inv_first;  // ~(lowest global entry index seen for this key); 0 = none yet
-    unsigned long long tag;        // 0 empty | (hash & ~3)|1 pending | (hash & ~3)|2 ready
+    unsigned long long tag;        // epoch | hash bits | state (slot_word, ctmr_common.cuh)
     uint32_t body[12];             // exp_hour, issuer, {serial_len, serial[39]}
 };
 static_assert(sizeof(KnownSlot) == 64, "KnownSlot layout");
 
 struct __align__(16) PairSlot {   // one per Redis set "serials::<expDate>::<issuer>" ever written
-    unsigned long long key;        // ((issuer << 32) | (uint32)exp_hour) + 1; 0 = empty
+    unsigned long long key;        // ((issuer << 32) | (uint32)exp_hour) + 1
     unsigned long long inv_first;  // ~(lowest index among was-unknown entries of this (issuer, hour))
     unsigned long long count;      // SetCardinality of the set: unique serials inserted and not yet expired
-    unsigned long long pad;
+    unsigned long long pad;        // epoch | state (slot_word, ctmr_common.cuh); 0 in a snapshot or checkpoint
 };
 static_assert(sizeof(PairSlot) == 32, "PairSlot layout");
 
 
 struct __align__(16) MetaSlot {      // IssuerMetadata string sets: identity = two independent 64-bit hashes
-    unsigned long long h1;           // 0 = empty
-    unsigned long long h2;           // 0 = not yet published
+    unsigned long long h1;
+    unsigned long long h2;
     unsigned long long inv_first;    // ~(lowest index among new certificates carrying this string)
-    unsigned long long pad;
+    unsigned long long pad;          // epoch | state, as PairSlot.pad
 };
 
 // Multi-GPU (SURVEY.md §8(e)): every set "serials::<expDate>::<issuer>" has ONE owner GPU
@@ -144,6 +144,7 @@ struct DeviceState {
     int* error_flag;                    // [1]: 0 ok, CTMR_E_TABLE_FULL...
     MetaSlot* meta;                     // (issuer, kind, bytes) first-seen table
     uint64_t meta_mask;
+    uint32_t epoch;                     // the tables' current epoch (ctmr_common.cuh): slots of other epochs are empty
 };
 
 struct MapParams {
@@ -176,6 +177,7 @@ struct MapParams {
     KnownSlot* table;
     RouteOut route;
     uint64_t table_mask;
+    uint32_t epoch;
     int* error_flag;
     uint32_t* slot_of;
     FilterCfg filter;
@@ -217,13 +219,18 @@ cudaError_t launch_issuer_prepare(const uint8_t* blob, const uint64_t* offsets, 
                                   uint8_t* ok, cudaStream_t s);
 cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, int sm_count, cudaStream_t s);
 cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters /* [2] */, int sm_count, cudaStream_t s);
-// Ordered compaction of a table's live slots (KnownSlot: ready and hour * 3600 > now_sec; PairSlot / MetaSlot: occupied),
-// over tiles [t0, t1) of kCompactTile slots.  counts != NULL: counts[b - t0] = live slots of tile b.  Otherwise tile b's live
-// slots go to keep[base[b] - base[t0] ...] in slot order (base = exclusive prefix of the counts over every tile).
+// Ordered compaction of a table's live slots at `epoch` (KnownSlot: ready and hour * 3600 > now_sec; PairSlot / MetaSlot:
+// ready), over tiles [t0, t1) of kCompactTile slots.  counts != NULL: counts[b - t0] = live slots of tile b.  Otherwise tile
+// b's live slots go to keep[base[b] - base[t0] ...] in slot order and in canonical form (base = exclusive prefix of the
+// counts over every tile).
 constexpr uint32_t kCompactTile = 4096;
 template <class Slot>
-cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, int64_t now_sec, uint64_t t0, uint64_t t1,
+cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, uint32_t epoch, int64_t now_sec, uint64_t t0, uint64_t t1,
                                  const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s);
+// a snapshot's canonical slots, just copied into the tables, as live at st.epoch (ctmr_common.cuh stamp_slot)
+cudaError_t launch_stamp_tables(const DeviceState& st, int sm_count, cudaStream_t s);
+// the slots live at epoch `from` as live at `to` (ctmr_common.cuh restamp_word)
+cudaError_t launch_restamp_tables(const DeviceState& st, uint32_t from, uint32_t to, int sm_count, cudaStream_t s);
 // Inserts n key records again (eviction's survivors, a checkpoint's keys): only those this rank owns under st.peer, each
 // checked first (issuer < n_issuers, serial length, ready tag; else the error flag is CTMR_E_INVALID); count: add each
 // inserted key to the per-issuer histogram.

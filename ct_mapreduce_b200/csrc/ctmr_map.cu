@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(256, 6) map_light_kernel(const __grid_constant
             if (p.slot_of) {
                 const uint32_t owner = (valid && p.route.world > 1u) ? key_owner((int32_t)body[0], body[1], p.route.world) : p.route.rank;
                 const bool remote = valid && owner != p.route.rank;
-                p.slot_of[e] = (valid && !remote) ? known_insert<false>(p.table, p.table_mask, p.error_flag, body, ~gi) : 0xFFFFFFFFu;
+                p.slot_of[e] = (valid && !remote) ? known_insert<false>(p.table, p.table_mask, p.epoch, p.error_flag, body, ~gi) : 0xFFFFFFFFu;
                 route_append(p.route, remote, owner, kr, (uint32_t)e);
             }
         }
@@ -355,7 +355,7 @@ __global__ void __launch_bounds__(StreamCfg::kWarps * 32, StreamCfg::kCtasPerSm)
                         const uint2 k3 = *reinterpret_cast<const uint2*>(reinterpret_cast<const uint32_t*>(kr) + 12);
                         const uint32_t body[12] = {(uint32_t)(int32_t)exp_hour, issuer, k1.x, k1.y, k1.z, k1.w,
                                                    k2.x, k2.y, k2.z, k2.w, k3.x, k3.y};
-                        slot = known_insert<false>(p.table, p.table_mask, p.error_flag, body, ~gi);
+                        slot = known_insert<false>(p.table, p.table_mask, p.epoch, p.error_flag, body, ~gi);
                     }
                     p.slot_of[e] = slot;
                     route_append(p.route, remote, owner, kr, (uint32_t)e);  // keys owned elsewhere: into the owner's inbox over NVLink

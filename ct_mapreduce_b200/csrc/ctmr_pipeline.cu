@@ -597,6 +597,7 @@ struct PeerHandle {
     cudaIpcMemHandle_t mem, xchg;
     uint64_t table_slots, pair_slots, meta_slots, total, X;
     uint32_t max_issuers, world;
+    uint32_t epoch, pad;  // the rank's table epoch at export (ctmr_common.cuh)
 };
 static_assert(sizeof(PeerHandle) <= CTMR_PEER_HANDLE_BYTES, "peer handle size");
 }  // namespace
@@ -624,6 +625,7 @@ int ctmr_peer_export(ctmr_ctx* c, uint32_t world, uint8_t handle_out[CTMR_PEER_H
     h.meta_slots = c->st.meta_mask + 1;
     h.total = c->lay.total;
     h.max_issuers = c->st.max_issuers;
+    h.epoch = c->st.epoch;
     std::memset(handle_out, 0, CTMR_PEER_HANDLE_BYTES);
     std::memcpy(handle_out, &h, sizeof h);
     return CTMR_OK;
@@ -637,6 +639,11 @@ int ctmr_peer_attach(ctmr_ctx* c, uint32_t rank, uint32_t world, const uint8_t* 
     if (!c->xchg || c->exported_world != world) return fail(c, CTMR_E_INVALID, "call ctmr_peer_export(ctx, world, ...) with this group size first");
     uint8_t *bases[kMaxWorld] = {}, *xb[kMaxWorld] = {};
     IpcMap base_maps[kMaxWorld], xchg_maps[kMaxWorld];  // into the ctx once every rank's region is open
+    // The ranks' table epochs must be one: a cross-GPU string-identity insert stamps the inserting rank's epoch into the
+    // owner's table, and each rank would read the other's slots as empty.  A rank that reset its tables or loaded a
+    // checkpoint on its own before attaching is ahead; every rank moves to the highest epoch of the handles (the same on
+    // every rank), its live slots with it.  From then on every reset is collective and the epochs stay in lockstep.
+    uint32_t epoch = 0;
     for (uint32_t r = 0; r < world; ++r) {
         PeerHandle h;
         std::memcpy(&h, handles + (size_t)r * CTMR_PEER_HANDLE_BYTES, sizeof h);
@@ -644,6 +651,9 @@ int ctmr_peer_attach(ctmr_ctx* c, uint32_t rank, uint32_t world, const uint8_t* 
         if (h.table_slots != c->st.table_mask + 1 || h.pair_slots != c->st.pair_mask + 1 || h.meta_slots != c->st.meta_mask + 1 ||
             h.max_issuers != c->st.max_issuers || h.total != c->lay.total || h.X != c->X || h.world != world)
             return fail(c, CTMR_E_INVALID, "rank " + std::to_string(r) + " was created with different capacities (or exported for another group size)");
+        if (r == rank && h.epoch != c->st.epoch)
+            return fail(c, CTMR_E_INVALID, "the tables were reset or loaded since ctmr_peer_export: export again");
+        epoch = h.epoch > epoch ? h.epoch : epoch;
         if (r == rank) {
             bases[r] = c->shared;
             xb[r] = c->xchg;
@@ -657,6 +667,11 @@ int ctmr_peer_attach(ctmr_ctx* c, uint32_t rank, uint32_t world, const uint8_t* 
         }
         bases[r] = base_maps[r];
         xb[r] = xchg_maps[r];
+    }
+    if (epoch != c->st.epoch) {  // done before this rank enters any collective call, whose barriers order the peers' inserts after it
+        CU(c, launch_restamp_tables(c->st, c->st.epoch, epoch, c->sm_count, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        c->st.epoch = epoch;
     }
     std::swap(c->ipc_base, base_maps);
     std::swap(c->ipc_xchg, xchg_maps);

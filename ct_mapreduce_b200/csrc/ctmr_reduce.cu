@@ -21,7 +21,7 @@ __device__ __forceinline__ void insert_one(const DeviceState& st, const ctmr_key
     }
     const unsigned long long inv_idx = ~(((unsigned long long)q0.y << 32) | q0.x);
     const uint32_t body[12] = {q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y};
-    slot_of[j] = known_insert<false>(st.table, st.table_mask, st.error_flag, body, inv_idx);
+    slot_of[j] = known_insert<false>(st.table, st.table_mask, st.epoch, st.error_flag, body, inv_idx);
 }
 
 __global__ void __launch_bounds__(256) insert_kernel(DeviceState st, const ctmr_key* __restrict__ keys, uint64_t m,
@@ -30,14 +30,32 @@ __global__ void __launch_bounds__(256) insert_kernel(DeviceState st, const ctmr_
     if (j < m) insert_one(st, keys, j, slot_of);
 }
 
+// Find-or-insert of an (issuer, hour) key.  The pad word carries the slot's epoch and state (ctmr_common.cuh): the same key
+// recurs after every reset, so a key word left by an earlier epoch cannot tell whether the slot is live.  The claimer
+// writes key, inv_first and count = 0 while the slot is pending; equal keys act (max, add) only once they see it ready.
 template <bool SYS>
-__device__ __forceinline__ uint32_t pair_insert(PairSlot* __restrict__ pairs, uint64_t pair_mask, int* error_flag,
+__device__ __forceinline__ uint32_t pair_insert(PairSlot* __restrict__ pairs, uint64_t pair_mask, uint32_t epoch, int* error_flag,
                                                 unsigned long long pk, unsigned long long inv_idx) {
     uint64_t pos = mix64(pk) & pair_mask;
     for (uint32_t probes = 0;; ++probes) {
-        unsigned long long cur = tab_cas<SYS>(&pairs[pos].key, 0ull, pk);  // 64-bit key: one CAS claims and identifies
-        if (cur == 0ull || cur == pk) {
-            tab_max<SYS>(&pairs[pos].inv_first, inv_idx);
+        PairSlot* sl = pairs + pos;
+        unsigned long long w = ld_volatile_u64(&sl->pad);
+        while (slot_state(w, epoch) == 0u) {
+            const unsigned long long seen = w;
+            w = tab_cas<SYS>(&sl->pad, seen, slot_word(epoch, kSlotPending));
+            if (w != seen) continue;  // another thread claimed the slot first
+            sl->key = pk;
+            sl->inv_first = inv_idx;
+            sl->count = 0ull;
+            tab_store_release<SYS>(&sl->pad, slot_word(epoch, kSlotReady));
+            return (uint32_t)pos;
+        }
+        // the key is read only after an acquire of the ready word (a relaxed read of ready does not order it, and the slot
+        // may hold the same key from the last epoch); pending: another thread is publishing the slot
+        do w = tab_load_acquire<SYS>(&sl->pad);
+        while (slot_state(w, epoch) == kSlotPending);
+        if (ld_volatile_u64(&sl->key) == pk) {
+            tab_max<SYS>(&sl->inv_first, inv_idx);
             return (uint32_t)pos;
         }
         pos = (pos + 1) & pair_mask;
@@ -78,7 +96,7 @@ __device__ __forceinline__ void resolve_one(const DeviceState& st, const ctmr_ke
         // the set's (issuer, exp_hour) slot: first-seen index + cardinality
         const unsigned long long pk = ((((unsigned long long)issuer) << 32) | (uint32_t)hour) + 1ull;
         const uint32_t same_set = __match_any_sync(umask, pk);
-        ps = pair_insert<false>(st.pairs, st.pair_mask, st.error_flag, pk, inv_idx);
+        ps = pair_insert<false>(st.pairs, st.pair_mask, st.epoch, st.error_flag, pk, inv_idx);
         if (ps != 0xFFFFFFFFu && (threadIdx.x & 31u) == (uint32_t)__ffs(same_set) - 1u)
             tab_add<false>(&st.pairs[ps].count, (unsigned long long)__popc(same_set));
     }
@@ -185,19 +203,33 @@ __device__ inline void hash_bytes(const uint8_t* __restrict__ p, uint32_t len, u
 // owner of a string identity: by its first hash (any rank may meet any issuer's strings)
 __device__ __forceinline__ uint32_t meta_owner(uint64_t h1, uint32_t world) { return world > 1u ? (uint32_t)((h1 >> 40) % world) : 0u; }
 
+// The pad word carries the slot's epoch and state, as in pair_insert: the claimer writes h1, h2 and inv_first while the
+// slot is pending.  A cross-GPU insert (SYS) stamps the inserting rank's epoch, which is the owner's: every reset is
+// collective (ctmr_reset_device).
 template <bool SYS>
-__device__ inline uint32_t meta_insert_at(MetaSlot* __restrict__ meta, uint64_t meta_mask, int* error_flag, uint64_t h1, uint64_t h2,
-                                          unsigned long long inv_idx) {
+__device__ inline uint32_t meta_insert_at(MetaSlot* __restrict__ meta, uint64_t meta_mask, uint32_t epoch, int* error_flag, uint64_t h1,
+                                          uint64_t h2, unsigned long long inv_idx) {
     uint64_t pos = (h1 >> 5) & meta_mask;
     for (uint32_t probes = 0; probes < 4096u; ++probes) {
         MetaSlot* sl = meta + pos;
-        unsigned long long c1 = tab_cas<SYS>(&sl->h1, 0ull, (unsigned long long)h1);
-        if (c1 == 0ull || c1 == h1) {
-            unsigned long long c2 = tab_cas<SYS>(&sl->h2, 0ull, (unsigned long long)h2);  // first writer publishes; equal strings write equal values
-            if (c2 == 0ull || c2 == h2) {
-                tab_max<SYS>(&sl->inv_first, inv_idx);
-                return (uint32_t)pos;
-            }
+        unsigned long long w = ld_volatile_u64(&sl->pad);
+        while (slot_state(w, epoch) == 0u) {
+            const unsigned long long seen = w;
+            w = tab_cas<SYS>(&sl->pad, seen, slot_word(epoch, kSlotPending));
+            if (w != seen) continue;  // another thread claimed the slot first
+            sl->h1 = h1;
+            sl->h2 = h2;
+            sl->inv_first = inv_idx;
+            tab_store_release<SYS>(&sl->pad, slot_word(epoch, kSlotReady));
+            return (uint32_t)pos;
+        }
+        // the key is read only after an acquire of the ready word (a relaxed read of ready does not order it, and the slot
+        // may hold the same key from the last epoch); pending: another thread is publishing the slot
+        do w = tab_load_acquire<SYS>(&sl->pad);
+        while (slot_state(w, epoch) == kSlotPending);
+        if (ld_volatile_u64(&sl->h1) == h1 && ld_volatile_u64(&sl->h2) == h2) {
+            tab_max<SYS>(&sl->inv_first, inv_idx);
+            return (uint32_t)pos;
         }
         pos = (pos + 1) & meta_mask;
     }
@@ -207,9 +239,9 @@ __device__ inline uint32_t meta_insert_at(MetaSlot* __restrict__ meta, uint64_t 
 
 // returns (owner << 28) | slot (the table has at most 2^26 slots), 0xFFFFFFFF on failure
 __device__ inline uint32_t meta_insert(const DeviceState& st, uint64_t h1, uint64_t h2, unsigned long long inv_idx) {
-    if (st.peer.world <= 1u) return meta_insert_at<false>(st.meta, st.meta_mask, st.error_flag, h1, h2, inv_idx);
+    if (st.peer.world <= 1u) return meta_insert_at<false>(st.meta, st.meta_mask, st.epoch, st.error_flag, h1, h2, inv_idx);
     const uint32_t owner = meta_owner(h1, st.peer.world);
-    const uint32_t pos = meta_insert_at<true>(st.peer.meta[owner], st.meta_mask, st.error_flag, h1, h2, inv_idx);
+    const uint32_t pos = meta_insert_at<true>(st.peer.meta[owner], st.meta_mask, st.epoch, st.error_flag, h1, h2, inv_idx);
     return pos == 0xFFFFFFFFu ? pos : ((owner << 28) | pos);
 }
 __device__ __forceinline__ unsigned long long meta_first(const DeviceState& st, uint32_t packed) {
@@ -360,9 +392,8 @@ __global__ void cardinality_kernel(DeviceState st, int32_t hour, uint32_t issuer
     uint64_t pos = mix64(pk) & st.pair_mask;
     unsigned long long v = 0;
     for (uint32_t probes = 0; probes <= 4096u; ++probes) {
-        const unsigned long long cur = ld_volatile_u64(&pairs[pos].key);
-        if (cur == 0ull) break;
-        if (cur == pk) {
+        if (slot_state(ld_volatile_u64(&pairs[pos].pad), st.epoch) == 0u) break;
+        if (ld_volatile_u64(&pairs[pos].key) == pk) {
             v = ld_volatile_u64(&pairs[pos].count);
             break;
         }
@@ -374,7 +405,7 @@ __global__ void cardinality_kernel(DeviceState st, int32_t hour, uint32_t issuer
 __global__ void __launch_bounds__(256) table_count_kernel(DeviceState st, unsigned long long* out) {
     unsigned int local = 0;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= st.table_mask; i += (uint64_t)gridDim.x * blockDim.x)
-        local += (st.table[i].tag & 3ull) == 2ull;
+        local += slot_state(st.table[i].tag, st.epoch) == kSlotReady;
     local = __reduce_add_sync(0xffffffffu, local);
     if ((threadIdx.x & 31) == 0 && local) atomicAdd(out, (unsigned long long)local);
 }
@@ -385,7 +416,7 @@ __global__ void __launch_bounds__(256) evict_count_kernel(DeviceState st, int64_
     unsigned int live = 0, dead = 0;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= st.table_mask; i += (uint64_t)gridDim.x * blockDim.x) {
         const KnownSlot& sl = st.table[i];
-        if ((sl.tag & 3ull) != 2ull) continue;
+        if (slot_state(sl.tag, st.epoch) != kSlotReady) continue;
         const int64_t hour = (int32_t)sl.body[0];
         if (hour * 3600 <= now_sec) {
             ++dead;
@@ -407,14 +438,14 @@ __global__ void __launch_bounds__(256) evict_count_kernel(DeviceState st, int64_
 // with counts set, counts[b] = its live slots; otherwise it writes them from keep[base[t0 + b] - base[t0]] on, in slot
 // order (a ballot per warp and a scan over the CTA's eight warps per row of 256 slots).  Two runs over the same state
 // write the same bytes.
-__device__ __forceinline__ bool slot_live(const KnownSlot& sl, int64_t now_sec) {
-    return (sl.tag & 3ull) == 2ull && (int64_t)(int32_t)sl.body[0] * 3600 > now_sec;
+__device__ __forceinline__ bool slot_live(const KnownSlot& sl, uint32_t epoch, int64_t now_sec) {
+    return slot_state(sl.tag, epoch) == kSlotReady && (int64_t)(int32_t)sl.body[0] * 3600 > now_sec;
 }
-__device__ __forceinline__ bool slot_live(const PairSlot& sl, int64_t) { return sl.key != 0ull; }
-__device__ __forceinline__ bool slot_live(const MetaSlot& sl, int64_t) { return sl.h1 != 0ull; }
+__device__ __forceinline__ bool slot_live(const PairSlot& sl, uint32_t epoch, int64_t) { return slot_state(sl.pad, epoch) == kSlotReady; }
+__device__ __forceinline__ bool slot_live(const MetaSlot& sl, uint32_t epoch, int64_t) { return slot_state(sl.pad, epoch) == kSlotReady; }
 
 template <class Slot>
-__global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restrict__ table, uint64_t n_slots, int64_t now_sec, uint64_t t0,
+__global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restrict__ table, uint64_t n_slots, uint32_t epoch, int64_t now_sec, uint64_t t0,
                                                             const unsigned long long* __restrict__ base, Slot* __restrict__ keep,
                                                             uint32_t* __restrict__ counts) {
     __shared__ uint32_t warp_n[8];
@@ -424,7 +455,7 @@ __global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restri
     uint32_t total = 0;
     for (uint32_t row = 0; row < kCompactTile / 256u; ++row) {
         const uint64_t i = tile * kCompactTile + row * 256u + threadIdx.x;
-        const bool live = i < n_slots && slot_live(table[i], now_sec);
+        const bool live = i < n_slots && slot_live(table[i], epoch, now_sec);
         const uint32_t ball = __ballot_sync(0xffffffffu, live);
         if (lane == 0) warp_n[warp] = __popc(ball);
         __syncthreads();
@@ -434,7 +465,7 @@ __global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restri
             before += w < warp ? warp_n[w] : 0u;
             row_n += warp_n[w];
         }
-        if (live && !counts) keep[out + before + __popc(ball & ((1u << lane) - 1u))] = table[i];
+        if (live && !counts) keep[out + before + __popc(ball & ((1u << lane) - 1u))] = canonical_slot(table[i], true);
         out += row_n;
         total += row_n;
         __syncthreads();  // warp_n is rewritten by the next row
@@ -443,7 +474,7 @@ __global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restri
 }
 
 // pass 3 (after the table has been cleared), and a checkpoint's records on their way in: linear probing leaves no holes
-// only if every record is inserted again.  A record whose owner under this rank's world is another rank is skipped
+// only if every record is inserted again.  The records are canonical (no epoch): a ready one has state 2 in its tag.  A record whose owner under this rank's world is another rank is skipped
 // (eviction: a rank only ever holds keys it owns).  Every index a record carries is checked before it is used: an
 // issuer >= n_issuers, a serial longer than CTMR_MAX_SERIAL or a slot that is not ready raises CTMR_E_INVALID.  count:
 // the inserted keys go into the per-issuer histogram (a checkpoint carries no histogram).
@@ -460,7 +491,7 @@ __global__ void __launch_bounds__(256) evict_reinsert_kernel(DeviceState st, con
     uint32_t body[12];
 #pragma unroll
     for (int k = 0; k < 12; ++k) body[k] = sl.body[k];
-    if (known_insert<false>(st.table, st.table_mask, st.error_flag, body, sl.inv_first) != 0xFFFFFFFFu && count)
+    if (known_insert<false>(st.table, st.table_mask, st.epoch, st.error_flag, body, sl.inv_first) != 0xFFFFFFFFu && count)
         atomicAdd(st.issuer_counts + sl.body[1], 1ull);
 }
 
@@ -476,7 +507,7 @@ __global__ void __launch_bounds__(256) ckpt_pairs_kernel(DeviceState st, const P
     const uint32_t issuer = (uint32_t)((p.key - 1ull) >> 32);
     const int32_t hour = (int32_t)(uint32_t)(p.key - 1ull);
     if (st.peer.world > 1u && key_owner(hour, issuer, st.peer.world) != st.peer.rank) return;
-    const uint32_t ps = pair_insert<false>(st.pairs, st.pair_mask, st.error_flag, p.key, p.inv_first);
+    const uint32_t ps = pair_insert<false>(st.pairs, st.pair_mask, st.epoch, st.error_flag, p.key, p.inv_first);
     if (ps != 0xFFFFFFFFu && p.count) tab_add<false>(&st.pairs[ps].count, p.count);
 }
 
@@ -490,7 +521,7 @@ __global__ void __launch_bounds__(256) ckpt_meta_kernel(DeviceState st, const Me
         return;
     }
     if (meta_owner(m.h1, st.peer.world) != (st.peer.world > 1u ? st.peer.rank : 0u)) return;
-    meta_insert_at<false>(st.meta, st.meta_mask, st.error_flag, m.h1, m.h2, m.inv_first);
+    meta_insert_at<false>(st.meta, st.meta_mask, st.epoch, st.error_flag, m.h1, m.h2, m.inv_first);
 }
 
 cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters, int sm_count, cudaStream_t s) {
@@ -498,18 +529,41 @@ cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned 
     return cudaGetLastError();
 }
 template <class Slot>
-cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, int64_t now_sec, uint64_t t0, uint64_t t1,
+cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, uint32_t epoch, int64_t now_sec, uint64_t t0, uint64_t t1,
                                  const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s) {
     if (t1 <= t0) return cudaSuccess;
-    evict_compact_kernel<Slot><<<(unsigned)(t1 - t0), 256, 0, s>>>(table, n_slots, now_sec, t0, base, keep, counts);
+    evict_compact_kernel<Slot><<<(unsigned)(t1 - t0), 256, 0, s>>>(table, n_slots, epoch, now_sec, t0, base, keep, counts);
     return cudaGetLastError();
 }
-template cudaError_t launch_evict_compact<KnownSlot>(const KnownSlot*, uint64_t, int64_t, uint64_t, uint64_t, const unsigned long long*,
-                                                     KnownSlot*, uint32_t*, cudaStream_t);
-template cudaError_t launch_evict_compact<PairSlot>(const PairSlot*, uint64_t, int64_t, uint64_t, uint64_t, const unsigned long long*,
-                                                    PairSlot*, uint32_t*, cudaStream_t);
-template cudaError_t launch_evict_compact<MetaSlot>(const MetaSlot*, uint64_t, int64_t, uint64_t, uint64_t, const unsigned long long*,
-                                                    MetaSlot*, uint32_t*, cudaStream_t);
+template cudaError_t launch_evict_compact<KnownSlot>(const KnownSlot*, uint64_t, uint32_t, int64_t, uint64_t, uint64_t,
+                                                     const unsigned long long*, KnownSlot*, uint32_t*, cudaStream_t);
+template cudaError_t launch_evict_compact<PairSlot>(const PairSlot*, uint64_t, uint32_t, int64_t, uint64_t, uint64_t,
+                                                    const unsigned long long*, PairSlot*, uint32_t*, cudaStream_t);
+template cudaError_t launch_evict_compact<MetaSlot>(const MetaSlot*, uint64_t, uint32_t, int64_t, uint64_t, uint64_t,
+                                                    const unsigned long long*, MetaSlot*, uint32_t*, cudaStream_t);
+
+template <class Slot>
+__global__ void __launch_bounds__(256) stamp_kernel(Slot* __restrict__ table, uint64_t n_slots, uint32_t epoch) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_slots; i += (uint64_t)gridDim.x * blockDim.x)
+        stamp_slot(table[i], epoch);
+}
+template <class Slot>
+__global__ void __launch_bounds__(256) restamp_kernel(Slot* __restrict__ table, uint64_t n_slots, uint32_t from, uint32_t to) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_slots; i += (uint64_t)gridDim.x * blockDim.x)
+        state_word(table[i]) = restamp_word(state_word(table[i]), from, to);
+}
+cudaError_t launch_restamp_tables(const DeviceState& st, uint32_t from, uint32_t to, int sm_count, cudaStream_t s) {
+    restamp_kernel<<<sm_count * 8, 256, 0, s>>>(st.table, st.table_mask + 1, from, to);
+    restamp_kernel<<<sm_count * 4, 256, 0, s>>>(st.pairs, st.pair_mask + 1, from, to);
+    restamp_kernel<<<sm_count * 4, 256, 0, s>>>(st.meta, st.meta_mask + 1, from, to);
+    return cudaGetLastError();
+}
+cudaError_t launch_stamp_tables(const DeviceState& st, int sm_count, cudaStream_t s) {
+    stamp_kernel<<<sm_count * 8, 256, 0, s>>>(st.table, st.table_mask + 1, st.epoch);
+    stamp_kernel<<<sm_count * 4, 256, 0, s>>>(st.pairs, st.pair_mask + 1, st.epoch);
+    stamp_kernel<<<sm_count * 4, 256, 0, s>>>(st.meta, st.meta_mask + 1, st.epoch);
+    return cudaGetLastError();
+}
 cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, uint64_t n, uint32_t n_issuers, bool count, cudaStream_t s) {
     if (n == 0) return cudaSuccess;
     evict_reinsert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(st, keep, n, n_issuers, count);
@@ -541,8 +595,8 @@ cudaError_t launch_cardinality(const DeviceState& st, int32_t hour, uint32_t iss
 // reference, storage/issuermetadata.go:95-108) stays.
 __global__ void __launch_bounds__(256) evict_pairs_kernel(DeviceState st, int64_t now_sec) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i <= st.pair_mask; i += (uint64_t)gridDim.x * blockDim.x) {
+        if (slot_state(st.pairs[i].pad, st.epoch) != kSlotReady) continue;
         const unsigned long long k = st.pairs[i].key;
-        if (k == 0ull) continue;
         const int64_t hour = (int32_t)(uint32_t)(k - 1ull);
         if (hour * 3600 <= now_sec) st.pairs[i].count = 0ull;
     }

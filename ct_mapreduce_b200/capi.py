@@ -54,6 +54,14 @@ EXPORTS = [
     "ctmr_revoked_cascade", "ctmr_group_revoked_cascade",   # CRLite's filter cascade of the covered issuers
     "ctmr_revoked_stash", "ctmr_group_revoked_stash",   # CRLite's stash: what a published filter and its stashes miss
 ]
+# the calls with a ctmr_group_<name> form beside ctmr_<name>
+GROUP_TWINS = (
+    "destroy", "last_error", "process_batch", "issuer_counts", "set_cardinality", "status_counters", "table_stats",
+    "preload_known", "evict_expired", "snapshot_size", "snapshot_save", "snapshot_load", "checkpoint_size", "checkpoint_save",
+    "checkpoint_load", "process_raw", "process_raw_tree", "process_raw_trees", "process_raw_bodies", "process_raw_bodies_tree",
+    "process_raw_bodies_trees", "process_tiles", "process_tiles_tree", "process_tiles_trees", "register_chain_certs",
+    "revoked_known", "revoked_cascade", "revoked_stash",
+)
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
 
@@ -258,53 +266,26 @@ def load():
     L.ctmr_synth_raw_pages_host.argtypes = [C.POINTER(SynthCfg), u64, u64, u32, vp, u64, vp, vp, vp, vp]
     L.ctmr_synth_raw_pages_host.restype = u64
     L.ctmr_process_raw.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut)]
-    L.ctmr_group_process_raw.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut)]
     L.ctmr_frontend_profile_last.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(u64)]
     L.ctmr_process_tiles.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut)]
-    L.ctmr_group_process_tiles.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut)]
     L.ctmr_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_tiles_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
     L.ctmr_process_raw_tree.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), C.POINTER(Tree)]
     L.ctmr_process_tiles_tree.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), C.POINTER(Tree)]
     L.ctmr_process_raw_trees.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), vp, vp, u32]
     L.ctmr_process_tiles_trees.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), vp, vp, u32]
-    L.ctmr_group_process_raw_tree.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), C.POINTER(Tree)]
-    L.ctmr_group_process_tiles_tree.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), C.POINTER(Tree)]
-    L.ctmr_group_process_raw_trees.argtypes = [vp, C.POINTER(RawBatch), C.POINTER(RawOut), vp, vp, u32]
-    L.ctmr_group_process_tiles_trees.argtypes = [vp, C.POINTER(TileBatch), C.POINTER(TileOut), vp, vp, u32]
     L.ctmr_process_raw_bodies.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut)]
-    L.ctmr_group_process_raw_bodies.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut)]
     L.ctmr_bodies_profile_last.argtypes = [vp, C.POINTER(C.c_float)]
     L.ctmr_process_raw_bodies_tree.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, C.POINTER(Tree)]
     L.ctmr_process_raw_bodies_trees.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, vp, vp, u32]
-    L.ctmr_group_process_raw_bodies_tree.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, C.POINTER(Tree)]
-    L.ctmr_group_process_raw_bodies_trees.argtypes = [vp, C.POINTER(BodyBatch), C.POINTER(BodyOut), vp, vp, vp, u32]
-    L.ctmr_group_register_chain_certs.argtypes = [vp, vp, vp, u32, vp, vp]
     L.ctmr_synth_tiles_host.argtypes = [C.POINTER(SynthCfg), u64, u64, vp, vp, u64, vp, vp]
     L.ctmr_synth_tiles_host.restype = u64
     L.ctmr_group_create.argtypes = [C.POINTER(Config), vp, u32, C.POINTER(vp)]
-    L.ctmr_group_destroy.argtypes = [vp]
-    L.ctmr_group_destroy.restype = None
-    L.ctmr_group_last_error.argtypes = [vp]
-    L.ctmr_group_last_error.restype = C.c_char_p
     L.ctmr_group_size.argtypes = [vp]
     L.ctmr_group_size.restype = u32
     L.ctmr_group_member.argtypes = [vp, u32]
     L.ctmr_group_member.restype = vp
-    L.ctmr_group_process_batch.argtypes = [vp, vp, vp, u64, vp, vp, u32, vp, i64, C.POINTER(Out)]
-    L.ctmr_group_issuer_counts.argtypes = [vp, vp, vp, C.POINTER(C.c_size_t)]
-    L.ctmr_group_set_cardinality.argtypes = [vp, i64, vp, C.POINTER(u64)]
-    L.ctmr_group_status_counters.argtypes = [vp, vp]
-    L.ctmr_group_table_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
-    L.ctmr_group_preload_known.argtypes = [vp, i64, vp, vp, vp, u64]
-    L.ctmr_group_evict_expired.argtypes = [vp, i64, C.POINTER(u64)]
     L.ctmr_group_reset.argtypes = [vp]
-    L.ctmr_group_snapshot_size.argtypes = [vp, C.POINTER(u64)]
-    L.ctmr_group_snapshot_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
-    L.ctmr_group_snapshot_load.argtypes = [vp, vp, u64]
-    L.ctmr_group_checkpoint_size.argtypes = [vp, C.POINTER(u64)]
-    L.ctmr_group_checkpoint_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
-    L.ctmr_group_checkpoint_load.argtypes = [vp, vp, vp, u32]
     L.ctmr_peer_export.argtypes = [vp, u32, vp]
     L.ctmr_peer_attach.argtypes = [vp, u32, u32, vp]
     L.ctmr_peer_barrier_device.argtypes = [vp, vp]
@@ -316,11 +297,12 @@ def load():
     L.ctmr_peer_frontend_stopped.argtypes = [vp, C.POINTER(u32)]
     L.ctmr_next_index.argtypes = [vp, C.POINTER(u64)]
     L.ctmr_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
-    L.ctmr_group_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
     L.ctmr_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
-    L.ctmr_group_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
     L.ctmr_revoked_stash.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u64, vp, u64, C.POINTER(StashOut)]
-    L.ctmr_group_revoked_stash.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u64, vp, u64, C.POINTER(StashOut)]
+    # a group's form of a call takes the group handle where the ctx form takes the ctx, and otherwise the same arguments
+    for name in GROUP_TWINS:
+        g, c = getattr(L, "ctmr_group_" + name), getattr(L, "ctmr_" + name)
+        g.argtypes, g.restype = c.argtypes, c.restype
     for name in EXPORTS:
         getattr(L, name)  # every symbol include/ctmr.h declares must resolve
     _lib = L

@@ -14,6 +14,11 @@ int fail(ctmr_ctx* ctx, int code, const std::string& msg) {
     return code;
 }
 
+int group_fail(ctmr_group* g, ctmr_ctx* c, int rc) {
+    if (g && c) g->err = c->err;
+    return rc;
+}
+
 uint64_t pow2_at_least(uint64_t v) {
     uint64_t p = 1;
     while (p < v) p <<= 1;
@@ -977,6 +982,23 @@ int ctmr_reset_device(ctmr_ctx* c, void* stream) {
     return rc ? rc : peer_barrier(c, CH_RESET_B, s);
 }
 
+int ctmr_group_reset(ctmr_group* g) {
+    return on_group(g, [](ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed) -> int {
+        for (uint32_t r = 0; r < W; ++r) {  // nobody may still be inserting into a shard when it is cleared
+            cudaSetDevice(m[r]->device);
+            cudaDeviceSynchronize();
+        }
+        for (uint32_t r = 0; r < W; ++r) {
+            ctmr_ctx* c = m[r];
+            *failed = c;
+            const int rc = ctmr_reset_device(c, nullptr);
+            if (rc) return rc;
+            if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(c, CTMR_E_CUDA, "reset failed");
+        }
+        return CTMR_OK;
+    });
+}
+
 // Reads AND clears the sticky device-side failure flag: one failed batch does not poison the ctx.
 int ctmr_check_device(ctmr_ctx* c, void* stream) {
     if (!c) return CTMR_E_INVALID;
@@ -999,113 +1021,38 @@ int ctmr_check_device(ctmr_ctx* c, void* stream) {
     }
 }
 
-// ------------------------------------------------------------------------------------------------ warm start / checkpoint
-}  // extern "C"
-
-namespace ctmr_host {
-// Seeds keys with the indices first_index .. first_index + n - 1 (the caller keeps them below every later batch
-// index).  Inserts go to the set's owner, so in a group any member can run it; not collective: the group is quiescent.
-int preload_impl(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32], const uint8_t* serial_blob, const uint64_t* serial_offsets,
-                 uint64_t n, uint64_t first_index) {
-    if (exp_hour > INT32_MAX || exp_hour < INT32_MIN) return fail(c, CTMR_E_INVALID, "exp_hour out of range");
+// ------------------------------------------------------------------------------------------------ tooling
+int ctmr_sha256_ceiling_device(ctmr_ctx* c, uint32_t iters, uint32_t rolled, uint32_t ctas_per_sm, float* ms_out,
+                               uint64_t* blocks_out) {
+    if (!c || !iters || !ctas_per_sm || ctas_per_sm > 8) return fail(c, CTMR_E_INVALID, "bad argument");
     CU(c, cudaSetDevice(c->device));
-    uint32_t issuer = 0;
-    bool found = false;
-    int rc = lookup_digest(c, digest, true, &issuer, &found);  // the issuer may be unknown so far (state written by an earlier process)
-    if (rc) return rc;
-    if (!n) return CTMR_OK;
-    if (c->st.peer.world > 1) {
-        const uint32_t owner = key_owner((int32_t)exp_hour, issuer, c->st.peer.world);
-        if (owner != c->st.peer.rank)
-            return fail(c, CTMR_E_INVALID, "this set is owned by rank " + std::to_string(owner) + " of the group: preload it there");
-    }
-    std::vector<ctmr_key> keys(n);
-    for (uint64_t i = 0; i < n; ++i) {
-        const uint64_t len = serial_offsets[i + 1] - serial_offsets[i];
-        if (serial_offsets[i + 1] < serial_offsets[i] || len == 0 || len > CTMR_MAX_SERIAL)
-            return fail(c, CTMR_E_INVALID, "preloaded serial empty or longer than CTMR_MAX_SERIAL");
-        std::memset(&keys[i], 0, sizeof(ctmr_key));
-        keys[i].index = first_index + i;
-        keys[i].exp_hour = (int32_t)exp_hour;
-        keys[i].issuer = issuer;
-        keys[i].serial_len = (uint8_t)len;
-        std::memcpy(keys[i].serial, serial_blob + serial_offsets[i], len);
-        keys[i].valid = 1;
-    }
-    rc = ensure_scratch(c, n);
-    if (rc) return rc;
-    CU(c, cudaMemcpyAsync(c->keys_scratch, keys.data(), n * sizeof(ctmr_key), cudaMemcpyHostToDevice, c->stream));
-    rc = reduce_on(c, c->keys_scratch, n, c->slot_scratch, c->pair_scratch, c->bits_scratch, c->bits_scratch + n, c->stream);
-    if (rc) return rc;
-    CU(c, cudaStreamSynchronize(c->stream));
-    return ctmr_check_device(c, nullptr);
-}
-}  // namespace ctmr_host
-
-extern "C" {
-
-int ctmr_preload_known(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32], const uint8_t* serial_blob,
-                       const uint64_t* serial_offsets, uint64_t n) {
-    if (!c || !digest || (n && (!serial_blob || !serial_offsets))) return fail(c, CTMR_E_INVALID, "bad argument");
-    if (c->group) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_preload_known");
-    // key records with the indices next_index .. BELOW every later batch index: preloaded keys always win "first seen"
-    int rc = preload_impl(c, exp_hour, digest, serial_blob, serial_offsets, n, c->next_index);
-    if (rc == CTMR_OK) c->next_index += n;
-    return rc;
-}
-
-}  // extern "C"
-
-namespace ctmr_host {
-
-// one shard's tables and histograms, in a fixed order (device <-> host)
-uint64_t snap_shard_bytes(ctmr_ctx* c) {
-    return (c->st.table_mask + 1) * sizeof(KnownSlot) + (c->st.pair_mask + 1) * sizeof(PairSlot) + (c->st.meta_mask + 1) * sizeof(MetaSlot) +
-           c->st.max_issuers * sizeof(uint64_t) + CTMR_ST__COUNT * sizeof(uint64_t);
-}
-
-// a snapshot holds the tables in canonical form (ctmr_common.cuh): what they held before epochs, byte for byte.  The
-// slots lie at any alignment in the caller's buffer (after the snapshot header), so each is copied out and back.
-template <class Slot>
-static void canonical_slots(uint8_t* p, uint64_t n, uint32_t epoch) {
-    for (uint64_t i = 0; i < n; ++i, p += sizeof(Slot)) {
-        Slot s;
-        std::memcpy(&s, p, sizeof s);
-        s = canonical_slot(s, slot_state(state_word(s), epoch) == kSlotReady);
-        std::memcpy(p, &s, sizeof s);
-    }
-}
-
-int snap_shard_save(ctmr_ctx* c, uint8_t* p) {
-    CU(c, cudaSetDevice(c->device));
-    CU(c, cudaDeviceSynchronize());
-    const uint64_t t = (c->st.table_mask + 1) * sizeof(KnownSlot), pr = (c->st.pair_mask + 1) * sizeof(PairSlot),
-                   m = (c->st.meta_mask + 1) * sizeof(MetaSlot), ic = c->st.max_issuers * sizeof(uint64_t);
-    CU(c, cudaMemcpy(p, c->st.table, t, cudaMemcpyDeviceToHost));
-    canonical_slots<KnownSlot>(p, c->st.table_mask + 1, c->st.epoch); p += t;
-    CU(c, cudaMemcpy(p, c->st.pairs, pr, cudaMemcpyDeviceToHost));
-    canonical_slots<PairSlot>(p, c->st.pair_mask + 1, c->st.epoch); p += pr;
-    CU(c, cudaMemcpy(p, c->st.meta, m, cudaMemcpyDeviceToHost));
-    canonical_slots<MetaSlot>(p, c->st.meta_mask + 1, c->st.epoch); p += m;
-    CU(c, cudaMemcpy(p, c->st.issuer_counts, ic, cudaMemcpyDeviceToHost)); p += ic;
-    CU(c, cudaMemcpy(p, c->st.status_counts, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    Event e0, e1;
+    CU(c, create(e0, cudaEventDefault));
+    CU(c, create(e1, cudaEventDefault));
+    uint32_t* sink = &c->small->sha_sink;
+    CU(c, launch_sha_ceiling(iters / 8 + 1, (int)rolled, (int)ctas_per_sm, c->sm_count, sink, c->stream));  // warm-up
+    CU(c, cudaEventRecord(e0, c->stream));
+    CU(c, launch_sha_ceiling(iters, (int)rolled, (int)ctas_per_sm, c->sm_count, sink, c->stream));
+    CU(c, cudaEventRecord(e1, c->stream));
+    CU(c, cudaEventSynchronize(e1));
+    float ms = 0.f;
+    CU(c, cudaEventElapsedTime(&ms, e0, e1));
+    if (ms_out) *ms_out = ms;
+    if (blocks_out) *blocks_out = (uint64_t)c->sm_count * ctas_per_sm * 256ull * iters;
     return CTMR_OK;
 }
 
-int snap_shard_load(ctmr_ctx* c, const uint8_t* p) {
-    CU(c, cudaSetDevice(c->device));
-    CU(c, cudaDeviceSynchronize());
-    const uint64_t t = (c->st.table_mask + 1) * sizeof(KnownSlot), pr = (c->st.pair_mask + 1) * sizeof(PairSlot),
-                   m = (c->st.meta_mask + 1) * sizeof(MetaSlot), ic = c->st.max_issuers * sizeof(uint64_t);
-    CU(c, cudaMemcpy(c->st.table, p, t, cudaMemcpyHostToDevice)); p += t;
-    CU(c, cudaMemcpy(c->st.pairs, p, pr, cudaMemcpyHostToDevice)); p += pr;
-    CU(c, cudaMemcpy(c->st.meta, p, m, cudaMemcpyHostToDevice)); p += m;
-    CU(c, cudaMemcpy(c->st.issuer_counts, p, ic, cudaMemcpyHostToDevice)); p += ic;
-    CU(c, cudaMemcpy(c->st.status_counts, p, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyHostToDevice));
-    CU(c, launch_stamp_tables(c->st, c->sm_count, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    return clear_issuer_memos(c);
+int ctmr_frontend_profile_last(ctmr_ctx* c, float* frontend_ms, float* path_ms, uint64_t* frontend_launches) {
+    if (!c || !c->fe) return fail(c, CTMR_E_INVALID, "no ctmr_process_raw / ctmr_process_tiles call to report");
+    if (frontend_ms) *frontend_ms = c->fe->fe_ms;
+    if (path_ms) *path_ms = c->fe->path_ms;
+    if (frontend_launches) *frontend_launches = c->fe->launches;
+    return CTMR_OK;
 }
+
+}  // extern "C"
+
+namespace ctmr_host {
 
 int clear_issuer_memos(ctmr_ctx* c) {
     // host memos: the DER memo is rebuilt lazily, the digest memos come back from the device registry
@@ -1162,119 +1109,241 @@ int snap_registry_restore(ctmr_ctx* c, const uint8_t* digests, uint64_t n, const
 }  // namespace ctmr_host
 
 namespace {
-struct SnapHeader {
-    char magic[8];  // "CTMRSNP3"
-    uint64_t table_slots, pair_slots, meta_slots, max_issuers, n_issuers, next_index;
-};
-}  // namespace
 
-extern "C" {
+// The table calls: one body over the members m[0..W) a handle drives, body(m, W, next_index, failed, arguments...).  A
+// ctx passes itself (on_ctx; on a group member that is its own shard), a group every member (on_group); next_index is
+// the handle's.  On error *failed names the member whose last error says why.
 
-int ctmr_snapshot_size(ctmr_ctx* c, uint64_t* bytes) {
-    if (!c || !bytes) return fail(c, CTMR_E_INVALID, "bad argument");
-    if (c->st.peer.world > 1) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_snapshot_* (the shards share one issuer registry)");
+// Seeds keys with the indices *next_index .. *next_index + n - 1, below every later batch index, so that preloaded keys
+// always win "first seen".  The issuer is looked up on m[0] (the registry is the group's) and the keys go to the set's
+// owner: on a group the owning member, on a peer rank only the rank itself.  Not collective: the group is quiescent.
+int preload_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed, int64_t exp_hour, const uint8_t* digest,
+                    const uint8_t* serial_blob, const uint64_t* serial_offsets, uint64_t n) {
+    ctmr_ctx* c = m[0];
+    *failed = c;
+    if (!digest || (n && (!serial_blob || !serial_offsets))) return fail(c, CTMR_E_INVALID, "bad argument");
+    if (exp_hour > INT32_MAX || exp_hour < INT32_MIN) return fail(c, CTMR_E_INVALID, "exp_hour out of range");
     CU(c, cudaSetDevice(c->device));
-    int rc = refresh_digests(c);
+    uint32_t issuer = 0;
+    bool found = false;
+    int rc = lookup_digest(c, digest, true, &issuer, &found);  // the issuer may be unknown so far (state written by an earlier process)
     if (rc) return rc;
-    *bytes = sizeof(SnapHeader) + snap_shard_bytes(c) + c->digests.size() * 32;
+    if (!n) return CTMR_OK;
+    if (W > 1) {
+        c = m[key_owner((int32_t)exp_hour, issuer, W)];
+        *failed = c;
+        CU(c, cudaSetDevice(c->device));
+    } else if (c->st.peer.world > 1) {
+        const uint32_t owner = key_owner((int32_t)exp_hour, issuer, c->st.peer.world);
+        if (owner != c->st.peer.rank)
+            return fail(c, CTMR_E_INVALID, "this set is owned by rank " + std::to_string(owner) + " of the group: preload it there");
+    }
+    const uint64_t first_index = *next_index;
+    std::vector<ctmr_key> keys(n);
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint64_t len = serial_offsets[i + 1] - serial_offsets[i];
+        if (serial_offsets[i + 1] < serial_offsets[i] || len == 0 || len > CTMR_MAX_SERIAL)
+            return fail(c, CTMR_E_INVALID, "preloaded serial empty or longer than CTMR_MAX_SERIAL");
+        std::memset(&keys[i], 0, sizeof(ctmr_key));
+        keys[i].index = first_index + i;
+        keys[i].exp_hour = (int32_t)exp_hour;
+        keys[i].issuer = issuer;
+        keys[i].serial_len = (uint8_t)len;
+        std::memcpy(keys[i].serial, serial_blob + serial_offsets[i], len);
+        keys[i].valid = 1;
+    }
+    rc = ensure_scratch(c, n);
+    if (rc) return rc;
+    CU(c, cudaMemcpyAsync(c->keys_scratch, keys.data(), n * sizeof(ctmr_key), cudaMemcpyHostToDevice, c->stream));
+    rc = reduce_on(c, c->keys_scratch, n, c->slot_scratch, c->pair_scratch, c->bits_scratch, c->bits_scratch + n, c->stream);
+    if (rc) return rc;
+    CU(c, cudaStreamSynchronize(c->stream));
+    rc = ctmr_check_device(c, nullptr);
+    if (rc == CTMR_OK) *next_index += n;
+    return rc;
+}
+
+// one shard's tables and histograms, in a fixed order (device <-> host)
+uint64_t snap_shard_bytes(ctmr_ctx* c) {
+    return (c->st.table_mask + 1) * sizeof(KnownSlot) + (c->st.pair_mask + 1) * sizeof(PairSlot) + (c->st.meta_mask + 1) * sizeof(MetaSlot) +
+           c->st.max_issuers * sizeof(uint64_t) + CTMR_ST__COUNT * sizeof(uint64_t);
+}
+
+// a snapshot holds the tables in canonical form (ctmr_common.cuh): what they held before epochs, byte for byte.  The
+// slots lie at any alignment in the caller's buffer (after the snapshot header), so each is copied out and back.
+template <class Slot>
+static void canonical_slots(uint8_t* p, uint64_t n, uint32_t epoch) {
+    for (uint64_t i = 0; i < n; ++i, p += sizeof(Slot)) {
+        Slot s;
+        std::memcpy(&s, p, sizeof s);
+        s = canonical_slot(s, slot_state(state_word(s), epoch) == kSlotReady);
+        std::memcpy(p, &s, sizeof s);
+    }
+}
+
+int snap_shard_save(ctmr_ctx* c, uint8_t* p) {
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaDeviceSynchronize());
+    const uint64_t t = (c->st.table_mask + 1) * sizeof(KnownSlot), pr = (c->st.pair_mask + 1) * sizeof(PairSlot),
+                   m = (c->st.meta_mask + 1) * sizeof(MetaSlot), ic = c->st.max_issuers * sizeof(uint64_t);
+    CU(c, cudaMemcpy(p, c->st.table, t, cudaMemcpyDeviceToHost));
+    canonical_slots<KnownSlot>(p, c->st.table_mask + 1, c->st.epoch); p += t;
+    CU(c, cudaMemcpy(p, c->st.pairs, pr, cudaMemcpyDeviceToHost));
+    canonical_slots<PairSlot>(p, c->st.pair_mask + 1, c->st.epoch); p += pr;
+    CU(c, cudaMemcpy(p, c->st.meta, m, cudaMemcpyDeviceToHost));
+    canonical_slots<MetaSlot>(p, c->st.meta_mask + 1, c->st.epoch); p += m;
+    CU(c, cudaMemcpy(p, c->st.issuer_counts, ic, cudaMemcpyDeviceToHost)); p += ic;
+    CU(c, cudaMemcpy(p, c->st.status_counts, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     return CTMR_OK;
 }
 
-int ctmr_snapshot_save(ctmr_ctx* c, uint8_t* buf, uint64_t cap, uint64_t* written) {
-    uint64_t need = 0;
-    int rc = ctmr_snapshot_size(c, &need);
-    if (rc) return rc;
-    if (!buf || cap < need) return fail(c, CTMR_E_INVALID, "snapshot buffer too small");
+int snap_shard_load(ctmr_ctx* c, const uint8_t* p) {
+    CU(c, cudaSetDevice(c->device));
+    CU(c, cudaDeviceSynchronize());
+    const uint64_t t = (c->st.table_mask + 1) * sizeof(KnownSlot), pr = (c->st.pair_mask + 1) * sizeof(PairSlot),
+                   m = (c->st.meta_mask + 1) * sizeof(MetaSlot), ic = c->st.max_issuers * sizeof(uint64_t);
+    CU(c, cudaMemcpy(c->st.table, p, t, cudaMemcpyHostToDevice)); p += t;
+    CU(c, cudaMemcpy(c->st.pairs, p, pr, cudaMemcpyHostToDevice)); p += pr;
+    CU(c, cudaMemcpy(c->st.meta, p, m, cudaMemcpyHostToDevice)); p += m;
+    CU(c, cudaMemcpy(c->st.issuer_counts, p, ic, cudaMemcpyHostToDevice)); p += ic;
+    CU(c, cudaMemcpy(c->st.status_counts, p, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyHostToDevice));
+    CU(c, launch_stamp_tables(c->st, c->sm_count, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return clear_issuer_memos(c);
+}
+
+// A snapshot of members m[0..W): the header, every member's shard in member order, then the registry's digests.  A
+// ctx's (CTMRSNP3) and a group's (CTMRGRP1) headers differ in their first three words: a group's names its size, so that
+// it loads only into a group of the same shape (the owner of a set depends on the group size).
+struct SnapHeader {
+    char magic[8];
+    uint64_t shape[3];  // CTMRSNP3: table, pair and meta slots; CTMRGRP1: members, shard bytes, table slots
+    uint64_t max_issuers, n_issuers, next_index;
+};
+
+SnapHeader snap_header(ctmr_ctx** m, uint32_t W, bool group) {
+    const DeviceState& st = m[0]->st;
     SnapHeader h{};
-    std::memcpy(h.magic, "CTMRSNP3", 8);
-    h.table_slots = c->st.table_mask + 1;
-    h.pair_slots = c->st.pair_mask + 1;
-    h.meta_slots = c->st.meta_mask + 1;
-    h.max_issuers = c->st.max_issuers;
-    h.n_issuers = c->digests.size();
-    h.next_index = c->next_index;
+    std::memcpy(h.magic, group ? "CTMRGRP1" : "CTMRSNP3", 8);
+    if (group) {
+        h.shape[0] = W;
+        h.shape[1] = snap_shard_bytes(m[0]);
+        h.shape[2] = st.table_mask + 1;
+    } else {
+        h.shape[0] = st.table_mask + 1;
+        h.shape[1] = st.pair_mask + 1;
+        h.shape[2] = st.meta_mask + 1;
+    }
+    h.max_issuers = st.max_issuers;
+    return h;
+}
+
+// group: the snapshot of a whole group; otherwise of one ctx, which must not share its registry with other shards
+int snapshot_size_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, bool group, uint64_t* bytes) {
+    ctmr_ctx* c0 = m[0];
+    *failed = c0;
+    if (!bytes) return fail(c0, CTMR_E_INVALID, "bad argument");
+    if (!group && c0->st.peer.world > 1)
+        return fail(c0, CTMR_E_INVALID, "member of a group: use ctmr_group_snapshot_* (the shards share one issuer registry)");
+    CU(c0, cudaSetDevice(c0->device));
+    const int rc = refresh_digests(c0);
+    if (rc) return rc;
+    *bytes = sizeof(SnapHeader) + W * snap_shard_bytes(c0) + c0->digests.size() * 32;
+    return CTMR_OK;
+}
+
+int snapshot_save_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed, bool group, uint8_t* buf, uint64_t cap,
+                          uint64_t* written) {
+    uint64_t need = 0;
+    int rc = snapshot_size_members(m, W, next_index, failed, group, &need);
+    if (rc) return rc;
+    ctmr_ctx* c0 = m[0];
+    if (!buf || cap < need) return fail(c0, CTMR_E_INVALID, "snapshot buffer too small");
+    SnapHeader h = snap_header(m, W, group);
+    h.n_issuers = c0->digests.size();
+    h.next_index = *next_index;
     uint8_t* p = buf;
     std::memcpy(p, &h, sizeof h); p += sizeof h;
-    rc = snap_shard_save(c, p);
-    if (rc) return rc;
-    p += snap_shard_bytes(c);
-    for (const auto& d : c->digests) { std::memcpy(p, d.data(), 32); p += 32; }
+    for (uint32_t r = 0; r < W; ++r) {
+        *failed = m[r];
+        rc = snap_shard_save(m[r], p);
+        if (rc) return rc;
+        p += snap_shard_bytes(m[r]);
+    }
+    for (const auto& d : c0->digests) { std::memcpy(p, d.data(), 32); p += 32; }
     if (written) *written = (uint64_t)(p - buf);
     return CTMR_OK;
 }
 
-int ctmr_snapshot_load(ctmr_ctx* c, const uint8_t* buf, uint64_t bytes) {
-    if (!c || !buf || bytes < sizeof(SnapHeader)) return fail(c, CTMR_E_INVALID, "bad snapshot");
+int snapshot_load_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed, bool group, const uint8_t* buf,
+                          uint64_t bytes) {
+    ctmr_ctx* c0 = m[0];
+    *failed = c0;
     SnapHeader h;
+    if (!buf || bytes < sizeof h) return fail(c0, CTMR_E_INVALID, "bad snapshot");
     std::memcpy(&h, buf, sizeof h);
-    if (std::memcmp(h.magic, "CTMRSNP3", 8) != 0) return fail(c, CTMR_E_INVALID, "not a ctmr snapshot");
-    if (h.table_slots != c->st.table_mask + 1 || h.pair_slots != c->st.pair_mask + 1 || h.meta_slots != c->st.meta_mask + 1 ||
-        h.max_issuers != c->st.max_issuers)
-        return fail(c, CTMR_E_INVALID, "snapshot was taken with different capacities (table / pairs / max_issuers)");
-    if (bytes < sizeof h + snap_shard_bytes(c) + h.n_issuers * 32 || h.n_issuers > h.max_issuers) return fail(c, CTMR_E_INVALID, "truncated snapshot");
-    if (c->st.peer.world > 1) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_snapshot_*");
+    const SnapHeader want = snap_header(m, W, group);
+    if (std::memcmp(h.magic, want.magic, 8) != 0) return fail(c0, CTMR_E_INVALID, group ? "not a ctmr group snapshot" : "not a ctmr snapshot");
+    const bool too_many = h.n_issuers > h.max_issuers;
+    if (std::memcmp(h.shape, want.shape, sizeof h.shape) != 0 || h.max_issuers != want.max_issuers || (group && too_many))
+        return fail(c0, CTMR_E_INVALID, group ? "snapshot was taken by a group of another size or with other capacities"
+                                              : "snapshot was taken with different capacities (table / pairs / max_issuers)");
+    if (bytes < sizeof h + W * snap_shard_bytes(c0) + h.n_issuers * 32 || too_many) return fail(c0, CTMR_E_INVALID, "truncated snapshot");
+    if (!group && c0->st.peer.world > 1) return fail(c0, CTMR_E_INVALID, "member of a group: use ctmr_group_snapshot_*");
     RegistryUpload u;
-    int rc = snap_registry_alloc(c, h.n_issuers, u);
+    int rc = snap_registry_alloc(c0, h.n_issuers, u);
     if (rc) return rc;
-    rc = snap_shard_load(c, buf + sizeof h);
-    if (rc) return rc;
-    c->next_index = h.next_index;
-    return snap_registry_restore(c, buf + sizeof h + snap_shard_bytes(c), h.n_issuers, u);
-}
-
-// ------------------------------------------------------------------------------------------------ tooling
-int ctmr_sha256_ceiling_device(ctmr_ctx* c, uint32_t iters, uint32_t rolled, uint32_t ctas_per_sm, float* ms_out,
-                               uint64_t* blocks_out) {
-    if (!c || !iters || !ctas_per_sm || ctas_per_sm > 8) return fail(c, CTMR_E_INVALID, "bad argument");
-    CU(c, cudaSetDevice(c->device));
-    Event e0, e1;
-    CU(c, create(e0, cudaEventDefault));
-    CU(c, create(e1, cudaEventDefault));
-    uint32_t* sink = &c->small->sha_sink;
-    CU(c, launch_sha_ceiling(iters / 8 + 1, (int)rolled, (int)ctas_per_sm, c->sm_count, sink, c->stream));  // warm-up
-    CU(c, cudaEventRecord(e0, c->stream));
-    CU(c, launch_sha_ceiling(iters, (int)rolled, (int)ctas_per_sm, c->sm_count, sink, c->stream));
-    CU(c, cudaEventRecord(e1, c->stream));
-    CU(c, cudaEventSynchronize(e1));
-    float ms = 0.f;
-    CU(c, cudaEventElapsedTime(&ms, e0, e1));
-    if (ms_out) *ms_out = ms;
-    if (blocks_out) *blocks_out = (uint64_t)c->sm_count * ctas_per_sm * 256ull * iters;
-    return CTMR_OK;
-}
-
-// ------------------------------------------------------------------------------------------------ read side
-int ctmr_issuer_counts(ctmr_ctx* c, uint8_t* digests, uint64_t* counts, size_t* n) {
-    if (!c || !n) return fail(c, CTMR_E_INVALID, "bad argument");
-    CU(c, cudaSetDevice(c->device));
-    {
-        int rc0 = refresh_digests(c);  // issuers another rank of the group registered count too (with 0 here)
-        if (rc0) return rc0;
+    const uint8_t* p = buf + sizeof h;
+    for (uint32_t r = 0; r < W; ++r) {
+        *failed = m[r];
+        rc = snap_shard_load(m[r], p);
+        if (rc) return rc;
+        p += snap_shard_bytes(m[r]);
     }
-    const size_t have = c->digests.size(), cap = *n;
-    const size_t take = have < cap ? have : cap;
-    if (take) {
-        if (counts) {
-            CU(c, cudaMemcpyAsync(counts, c->st.issuer_counts, take * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-            CU(c, cudaStreamSynchronize(c->stream));
+    *failed = c0;
+    *next_index = h.next_index;
+    return snap_registry_restore(c0, p, h.n_issuers, u);
+}
+
+// Every shard counts the keys of the sets it owns (the owner resolves its own entries and its inbox records, receives the
+// preloads and evicts its sets), so each member's counts are exact and their sum is the group's count.
+int issuer_counts_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, uint8_t* digests, uint64_t* counts, size_t* n) {
+    *failed = m[0];
+    if (!n) return fail(m[0], CTMR_E_INVALID, "bad argument");
+    const size_t cap = *n;
+    std::vector<uint64_t> part(W > 1 && counts ? cap : 0);
+    size_t take = 0;
+    for (uint32_t r = 0; r < W; ++r) {
+        ctmr_ctx* c = m[r];
+        *failed = c;
+        CU(c, cudaSetDevice(c->device));
+        const int rc = refresh_digests(c);  // issuers another rank of the group registered count too (with 0 here)
+        if (rc) return rc;
+        const size_t k = std::min(c->digests.size(), cap);
+        if (r == 0) {
+            take = k;
+            for (size_t i = 0; digests && i < k; ++i) std::memcpy(digests + 32 * i, c->digests[i].data(), 32);
         }
-        if (digests)
-            for (size_t i = 0; i < take; ++i) std::memcpy(digests + 32 * i, c->digests[i].data(), 32);
+        if (!counts || !k) continue;
+        CU(c, cudaMemcpyAsync(r ? part.data() : counts, c->st.issuer_counts, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        for (size_t i = 0; r && i < std::min(k, take); ++i) counts[i] += part[i];
     }
     *n = take;
     return CTMR_OK;
 }
 
-int ctmr_set_cardinality(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32], uint64_t* out) {
-    if (!c || !digest || !out) return fail(c, CTMR_E_INVALID, "bad argument");
+// one probe of the set's (issuer, hour) slot at its owner, which may be another GPU of the group: through m[0]
+int set_cardinality_members(ctmr_ctx** m, uint32_t, uint64_t*, ctmr_ctx** failed, int64_t exp_hour, const uint8_t* digest, uint64_t* out) {
+    ctmr_ctx* c = m[0];
+    *failed = c;
+    if (!digest || !out) return fail(c, CTMR_E_INVALID, "bad argument");
     CU(c, cudaSetDevice(c->device));
     *out = 0;
     uint32_t issuer = 0;
     bool found = false;
-    int rc = lookup_digest(c, digest, false, &issuer, &found);
-    if (rc) return rc;
-    if (!found || exp_hour > INT32_MAX || exp_hour < INT32_MIN) return CTMR_OK;
-    // one probe of the set's (issuer, hour) slot at its owner -- which may be another GPU of the group
+    const int rc = lookup_digest(c, digest, false, &issuer, &found);
+    if (rc || !found || exp_hour > INT32_MAX || exp_hour < INT32_MIN) return rc;
     CU(c, launch_cardinality(c->st, (int32_t)exp_hour, issuer, &c->small->cardinality, c->stream));
     unsigned long long v = 0;
     CU(c, cudaMemcpyAsync(&v, &c->small->cardinality, sizeof v, cudaMemcpyDeviceToHost, c->stream));
@@ -1283,31 +1352,44 @@ int ctmr_set_cardinality(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32]
     return CTMR_OK;
 }
 
-int ctmr_status_counters(ctmr_ctx* c, uint64_t out[CTMR_ST__COUNT]) {
-    if (!c || !out) return fail(c, CTMR_E_INVALID, "bad argument");
-    CU(c, cudaSetDevice(c->device));
-    CU(c, cudaMemcpyAsync(out, c->st.status_counts, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
+int status_counters_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, uint64_t* out) {
+    *failed = m[0];
+    if (!out) return fail(m[0], CTMR_E_INVALID, "bad argument");
+    uint64_t part[CTMR_ST__COUNT];
+    for (uint32_t r = 0; r < W; ++r) {
+        ctmr_ctx* c = m[r];
+        *failed = c;
+        CU(c, cudaSetDevice(c->device));
+        CU(c, cudaMemcpyAsync(r ? part : out, c->st.status_counts, CTMR_ST__COUNT * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        for (int i = 0; r && i < CTMR_ST__COUNT; ++i) out[i] += part[i];
+    }
     return CTMR_OK;
 }
 
-int ctmr_table_stats(ctmr_ctx* c, uint64_t* used, uint64_t* capacity) {
-    if (!c) return CTMR_E_INVALID;
-    CU(c, cudaSetDevice(c->device));
-    unsigned long long u = 0;
-    CU(c, cudaMemsetAsync(&c->small->table_count, 0, sizeof(unsigned long long), c->stream));
-    CU(c, launch_table_count(c->st, &c->small->table_count, c->sm_count, c->stream));
-    CU(c, cudaMemcpyAsync(&u, &c->small->table_count, sizeof u, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
+int table_stats_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, uint64_t* used, uint64_t* capacity) {
+    uint64_t u = 0, cp = 0;
+    for (uint32_t r = 0; r < W; ++r) {
+        ctmr_ctx* c = m[r];
+        *failed = c;
+        CU(c, cudaSetDevice(c->device));
+        unsigned long long v = 0;
+        CU(c, cudaMemsetAsync(&c->small->table_count, 0, sizeof(unsigned long long), c->stream));
+        CU(c, launch_table_count(c->st, &c->small->table_count, c->sm_count, c->stream));
+        CU(c, cudaMemcpyAsync(&v, &c->small->table_count, sizeof v, cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        u += v;
+        cp += c->st.table_mask + 1;
+    }
     if (used) *used = u;
-    if (capacity) *capacity = c->st.table_mask + 1;
+    if (capacity) *capacity = cp;
     return CTMR_OK;
 }
 
 // Redis TTLs firing (SURVEY §8(f)-4): every set "serials::<expDate>::<issuer>" carries EXPIREAT(expDate)
-// (storage/knowncertificates.go:44-47,98-104), so at `now` the sets with expDate <= now no longer exist.
-int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out) {
-    if (!c) return CTMR_E_INVALID;
+// (storage/knowncertificates.go:44-47,98-104), so at `now` the sets with expDate <= now no longer exist.  One shard: the
+// expired keys it holds go, *evicted their number.
+int evict_shard(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted) {
     CU(c, cudaSetDevice(c->device));
     CU(c, cudaDeviceSynchronize());
     unsigned long long counters[2] = {0, 0};
@@ -1320,7 +1402,7 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     CU(c, launch_evict_count(c->st, now_unix_sec, dev, c->sm_count, c->stream));
     CU(c, cudaMemcpyAsync(counters, dev, sizeof counters, cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
-    if (evicted_out) *evicted_out = counters[1];
+    *evicted = counters[1];
     if (counters[1] == 0) return CTMR_OK;
     // open addressing with linear probing: taking slots out would cut probe chains, so the survivors are
     // compacted aside, the table is cleared and they are inserted again (first-seen indices preserved)
@@ -1345,12 +1427,69 @@ int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out)
     return ctmr_check_device(c, nullptr);
 }
 
-int ctmr_frontend_profile_last(ctmr_ctx* c, float* frontend_ms, float* path_ms, uint64_t* frontend_launches) {
-    if (!c || !c->fe) return fail(c, CTMR_E_INVALID, "no ctmr_process_raw / ctmr_process_tiles call to report");
-    if (frontend_ms) *frontend_ms = c->fe->fe_ms;
-    if (path_ms) *path_ms = c->fe->path_ms;
-    if (frontend_launches) *frontend_launches = c->fe->launches;
+// every shard drops the expired sets it owns
+int evict_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, int64_t now_unix_sec, uint64_t* evicted_out) {
+    uint64_t total = 0;
+    for (uint32_t r = 0; r < W; ++r) {
+        *failed = m[r];
+        uint64_t e = 0;
+        const int rc = evict_shard(m[r], now_unix_sec, &e);
+        if (rc) return rc;
+        total += e;
+    }
+    if (evicted_out) *evicted_out = total;
     return CTMR_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ctmr_preload_known(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32], const uint8_t* serial_blob,
+                       const uint64_t* serial_offsets, uint64_t n) {
+    if (c && c->group) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_preload_known");
+    return on_ctx(c, preload_members, exp_hour, digest, serial_blob, serial_offsets, n);
+}
+int ctmr_snapshot_size(ctmr_ctx* c, uint64_t* bytes) { return on_ctx(c, snapshot_size_members, false, bytes); }
+int ctmr_snapshot_save(ctmr_ctx* c, uint8_t* buf, uint64_t cap, uint64_t* written) {
+    return on_ctx(c, snapshot_save_members, false, buf, cap, written);
+}
+int ctmr_snapshot_load(ctmr_ctx* c, const uint8_t* buf, uint64_t bytes) { return on_ctx(c, snapshot_load_members, false, buf, bytes); }
+int ctmr_issuer_counts(ctmr_ctx* c, uint8_t* digests, uint64_t* counts, size_t* n) {
+    return on_ctx(c, issuer_counts_members, digests, counts, n);
+}
+int ctmr_set_cardinality(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32], uint64_t* out) {
+    return on_ctx(c, set_cardinality_members, exp_hour, digest, out);
+}
+int ctmr_status_counters(ctmr_ctx* c, uint64_t out[CTMR_ST__COUNT]) { return on_ctx(c, status_counters_members, out); }
+int ctmr_table_stats(ctmr_ctx* c, uint64_t* used, uint64_t* capacity) { return on_ctx(c, table_stats_members, used, capacity); }
+int ctmr_evict_expired(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted_out) {
+    return on_ctx(c, evict_members, now_unix_sec, evicted_out);
+}
+
+int ctmr_group_preload_known(ctmr_group* g, int64_t exp_hour, const uint8_t issuer_digest[32], const uint8_t* serial_blob,
+                             const uint64_t* serial_offsets, uint64_t n) {
+    return on_group(g, preload_members, exp_hour, issuer_digest, serial_blob, serial_offsets, n);
+}
+int ctmr_group_snapshot_size(ctmr_group* g, uint64_t* bytes) { return on_group(g, snapshot_size_members, true, bytes); }
+int ctmr_group_snapshot_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written) {
+    return on_group(g, snapshot_save_members, true, buf, cap, written);
+}
+int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes) {
+    return on_group(g, snapshot_load_members, true, buf, bytes);
+}
+int ctmr_group_issuer_counts(ctmr_group* g, uint8_t* digests, uint64_t* counts, size_t* n) {
+    return on_group(g, issuer_counts_members, digests, counts, n);
+}
+int ctmr_group_set_cardinality(ctmr_group* g, int64_t exp_hour, const uint8_t issuer_digest[32], uint64_t* count_out) {
+    return on_group(g, set_cardinality_members, exp_hour, issuer_digest, count_out);
+}
+int ctmr_group_status_counters(ctmr_group* g, uint64_t out[CTMR_ST__COUNT]) { return on_group(g, status_counters_members, out); }
+int ctmr_group_table_stats(ctmr_group* g, uint64_t* slots_used, uint64_t* capacity) {
+    return on_group(g, table_stats_members, slots_used, capacity);
+}
+int ctmr_group_evict_expired(ctmr_group* g, int64_t now_unix_sec, uint64_t* evicted_out) {
+    return on_group(g, evict_members, now_unix_sec, evicted_out);
 }
 
 }  // extern "C"

@@ -334,28 +334,26 @@ int ctmr_checkpoint_load(ctmr_ctx* c, const uint8_t* const* parts, const uint64_
 }
 
 int ctmr_group_checkpoint_size(ctmr_group* g, uint64_t* bytes) {
-    if (!g || g->m.empty() || !bytes) return CTMR_E_INVALID;
-    ctmr_ctx* failed = nullptr;
-    const int rc = save_members(g->m.data(), (uint32_t)g->m.size(), 0, 1, g->next_index, nullptr, 0, bytes, &failed);
-    return rc ? group_fail(g, failed ? failed : g->m[0], rc) : rc;
+    return on_group(g, [=](ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed) {
+        if (!bytes) return fail(m[0], CTMR_E_INVALID, "bad argument");
+        return save_members(m, W, 0, 1, *next_index, nullptr, 0, bytes, failed);
+    });
 }
 
 int ctmr_group_checkpoint_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    if (!buf) return group_fail(g, g->m[0], fail(g->m[0], CTMR_E_INVALID, "bad argument"));
-    uint64_t need = 0;
-    ctmr_ctx* failed = nullptr;
-    const int rc = save_members(g->m.data(), (uint32_t)g->m.size(), 0, 1, g->next_index, buf, cap, &need, &failed);
-    if (rc) return group_fail(g, failed ? failed : g->m[0], rc);
-    if (written) *written = need;
-    return CTMR_OK;
+    return on_group(g, [=](ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed) {
+        if (!buf) return fail(m[0], CTMR_E_INVALID, "bad argument");
+        uint64_t need = 0;
+        const int rc = save_members(m, W, 0, 1, *next_index, buf, cap, &need, failed);
+        if (rc == CTMR_OK && written) *written = need;
+        return rc;
+    });
 }
 
 int ctmr_group_checkpoint_load(ctmr_group* g, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    ctmr_ctx* failed = nullptr;
-    const int rc = load_members(g->m.data(), (uint32_t)g->m.size(), parts, part_bytes, n_parts, &g->next_index, &failed);
-    return rc ? group_fail(g, failed ? failed : g->m[0], rc) : rc;
+    return on_group(g, [=](ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed) {
+        return load_members(m, W, parts, part_bytes, n_parts, next_index, failed);
+    });
 }
 
 }  // extern "C"

@@ -1,9 +1,10 @@
 // ctmr_ctx.cuh -- internal: the context behind the opaque ctmr_ctx of include/ctmr.h, shared by the translation
 // units that implement the C ABI (ctmr_api.cu: lifecycle, issuers, the steps of a round and run_round, which sequences
-// one round of the key exchange for all three callers, the ranks' barriers and mailbox, device entry points, read side,
-// front end plumbing;
+// one round of the key exchange for all three callers, the ranks' barriers and mailbox, device entry points, the table
+// calls of a ctx and a group (read side, preload, eviction, snapshots), front end plumbing;
 // ctmr_pipeline.cu: the host-buffer batch pipeline on one GPU, on a group of GPUs, and across processes, and the copy of
-// a round's outputs to the host; ctmr_frontend_api.cu: the wire-format front end on one GPU and on a group).
+// a round's outputs to the host, the group's lifecycle and the peer attach; ctmr_frontend_api.cu: the wire-format front
+// end on one GPU and on a group).
 //
 // Ownership: the ctx owns everything it allocates, through the handles below and std::unique_ptr, so deleting the ctx
 // releases it all.  The parts built on first use (the pipeline stages, ctmr_process_device's streams and events, the
@@ -581,6 +582,22 @@ inline void drain_streams(ctmr_ctx* c, const cudaStream_t* s, int n) {
     c->err = keep;
 }
 int group_fail(ctmr_group* g, ctmr_ctx* c, int rc);   // c's error becomes g's last error (when both are given); returns rc
+// A call through the body a ctx and a group share, body(m, W, next_index, &failed, args...) over the members m[0..W):
+// on_ctx passes the ctx alone (a NULL ctx: CTMR_E_INVALID), on_group every member of the group, whose last error becomes
+// that of the member the body names (member 0 when none) on failure (a NULL or empty group: bare CTMR_E_INVALID).
+template <class Body, class... Args>
+int on_ctx(ctmr_ctx* c, Body body, Args... args) {
+    if (!c) return fail(nullptr, CTMR_E_INVALID, "bad argument");
+    ctmr_ctx* failed = nullptr;
+    return body(&c, 1u, &c->next_index, &failed, args...);
+}
+template <class Body, class... Args>
+int on_group(ctmr_group* g, Body body, Args... args) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    ctmr_ctx* failed = nullptr;
+    const int rc = body(g->m.data(), (uint32_t)g->m.size(), &g->next_index, &failed, args...);
+    return rc ? group_fail(g, failed ? failed : g->m[0], rc) : rc;
+}
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise
@@ -597,14 +614,9 @@ int peer_agree(ctmr_ctx* c, int mine, uint64_t payload, uint64_t* row, const cha
 int refresh_digests(ctmr_ctx* c);                                   // host memo <- device registry
 int lookup_digest(ctmr_ctx* c, const uint8_t digest[32], bool insert, uint32_t* idx_out, bool* found);
 int upload_issuer_map(ctmr_ctx* c, const uint32_t* dense, uint32_t n);
-int preload_impl(ctmr_ctx* c, int64_t exp_hour, const uint8_t digest[32], const uint8_t* serial_blob, const uint64_t* serial_offsets,
-                 uint64_t n, uint64_t first_index);
 int ensure_stages(ctmr_ctx* c);
-// snapshot pieces (ctmr_api.cu): one shard's tables + histograms, and the registry of the group (rank 0's region)
-uint64_t snap_shard_bytes(ctmr_ctx* c);
-int snap_shard_save(ctmr_ctx* c, uint8_t* p);
-int snap_shard_load(ctmr_ctx* c, const uint8_t* p);
-// a snapshot's issuer digests on their way into the registry: allocated before a load overwrites anything
+// a snapshot's or checkpoint's issuer digests on their way into the registry of the group (rank 0's region): allocated
+// before a load overwrites anything (ctmr_api.cu)
 struct RegistryUpload {
     DevBuf<uint8_t> digests;
     DevBuf<uint32_t> idx;

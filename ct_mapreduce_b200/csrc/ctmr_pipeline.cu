@@ -1,5 +1,7 @@
 // ctmr_pipeline.cu -- the host-buffer batch of include/ctmr.h on one GPU, on a group of GPUs driven by one process
-// (ctmr_group_*: what a Go host calls), and on one GPU of a multi-process group (ctmr_peer_*: one process per GPU).
+// (ctmr_group_*: what a Go host calls), and on one GPU of a multi-process group (ctmr_peer_*: one process per GPU); and
+// the handles of those groups: a group's create, destroy and accessors, a rank's export and attach.  The table calls of
+// a group share their bodies with a ctx's, in ctmr_api.cu.
 //
 // One pipeline serves all three.  A batch is cut into ROUNDS; in a round every member GPU takes one slice of at
 // most `stage_entries` entries and runs, on the stream of the round's stage (three stages rotate, so H2D, kernels
@@ -98,11 +100,6 @@ int copy_out(ctmr_ctx* c, const ctmr_dev_out& d, uint64_t cnt, const ctmr_out* o
     CU(c, d2h_rows(out->first_issuer_dn, d.first_issuer_dn, lo, cnt, s));
     CU(c, d2h_rows(out->first_crldp, d.first_crldp, lo, cnt, s));
     return CTMR_OK;
-}
-
-int group_fail(ctmr_group* g, ctmr_ctx* c, int rc) {
-    if (g && c) g->err = c->err;
-    return rc;
 }
 
 }  // namespace ctmr_host
@@ -251,9 +248,9 @@ void drain(ctmr_ctx** m, uint32_t W) {
     }
 }
 
-int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, const uint8_t* blob, const uint64_t* offsets, uint64_t n,
-                          const uint8_t* issuer_blob, const uint64_t* issuer_offsets, uint32_t n_issuers, const uint32_t* issuer_idx,
-                          int64_t now_unix_ns, ctmr_out* out, ctmr_ctx** failed) {
+int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed, const uint8_t* blob, const uint64_t* offsets,
+                          uint64_t n, const uint8_t* issuer_blob, const uint64_t* issuer_offsets, uint32_t n_issuers,
+                          const uint32_t* issuer_idx, int64_t now_unix_ns, ctmr_out* out) {
     ctmr_ctx* c0 = m[0];
     *failed = c0;
     if (!out || (n && (!blob || !offsets))) return fail(c0, CTMR_E_INVALID, "bad argument");
@@ -341,8 +338,8 @@ int ctmr_process_batch(ctmr_ctx* c, const uint8_t* blob, const uint64_t* offsets
     if (!c) return CTMR_E_INVALID;
     if (c->group) return fail(c, CTMR_E_INVALID, "member of a group: use ctmr_group_process_batch");
     ctmr_ctx* failed = nullptr;
-    return process_batch_members(&c, 1, &c->next_index, blob, offsets, n, issuer_blob, issuer_offsets, n_issuers, issuer_idx, now_unix_ns,
-                                 out, &failed);
+    return process_batch_members(&c, 1, &c->next_index, &failed, blob, offsets, n, issuer_blob, issuer_offsets, n_issuers, issuer_idx,
+                                 now_unix_ns, out);
 }
 
 // ------------------------------------------------------------------------------------------------ one process, several GPUs
@@ -414,181 +411,9 @@ ctmr_ctx* ctmr_group_member(ctmr_group* g, uint32_t rank) { return g && rank < g
 int ctmr_group_process_batch(ctmr_group* g, const uint8_t* blob, const uint64_t* offsets, uint64_t n, const uint8_t* issuer_blob,
                              const uint64_t* issuer_offsets, uint32_t n_issuers, const uint32_t* issuer_idx, int64_t now_unix_ns,
                              ctmr_out* out) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    ctmr_ctx* failed = nullptr;
-    const int rc = process_batch_members(g->m.data(), (uint32_t)g->m.size(), &g->next_index, blob, offsets, n, issuer_blob, issuer_offsets,
-                                         n_issuers, issuer_idx, now_unix_ns, out, &failed);
-    return rc ? group_fail(g, failed ? failed : g->m[0], rc) : rc;
+    return on_group(g, process_batch_members, blob, offsets, n, issuer_blob, issuer_offsets, n_issuers, issuer_idx, now_unix_ns, out);
 }
 
-int ctmr_group_issuer_counts(ctmr_group* g, uint8_t* digests, uint64_t* counts, size_t* n) {
-    if (!g || g->m.empty() || !n) return CTMR_E_INVALID;
-    const size_t cap = *n;
-    std::vector<uint64_t> part(cap ? cap : 1);
-    size_t take = 0;
-    for (size_t r = 0; r < g->m.size(); ++r) {
-        size_t k = cap;
-        const int rc = ctmr_issuer_counts(g->m[r], r == 0 ? digests : nullptr, part.data(), &k);
-        if (rc) return group_fail(g, g->m[r], rc);
-        if (r == 0) {
-            take = k;
-            if (counts) std::copy(part.begin(), part.begin() + k, counts);
-        } else if (counts) {
-            // every shard counts the keys of the sets it owns (the owner resolves its own entries and its inbox records,
-            // receives the preloads and evicts its sets), so each part is exact and the sum is the group's count
-            for (size_t i = 0; i < std::min(k, take); ++i) counts[i] += part[i];
-        }
-    }
-    *n = take;
-    return CTMR_OK;
-}
-
-int ctmr_group_set_cardinality(ctmr_group* g, int64_t exp_hour, const uint8_t issuer_digest[32], uint64_t* count_out) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    const int rc = ctmr_set_cardinality(g->m[0], exp_hour, issuer_digest, count_out);  // probes the owner's slot over peer memory
-    return rc ? group_fail(g, g->m[0], rc) : rc;
-}
-
-int ctmr_group_status_counters(ctmr_group* g, uint64_t out[CTMR_ST__COUNT]) {
-    if (!g || g->m.empty() || !out) return CTMR_E_INVALID;
-    uint64_t part[CTMR_ST__COUNT];
-    std::fill(out, out + CTMR_ST__COUNT, 0);
-    for (ctmr_ctx* c : g->m) {
-        const int rc = ctmr_status_counters(c, part);
-        if (rc) return group_fail(g, c, rc);
-        for (int i = 0; i < CTMR_ST__COUNT; ++i) out[i] += part[i];
-    }
-    return CTMR_OK;
-}
-
-int ctmr_group_table_stats(ctmr_group* g, uint64_t* slots_used, uint64_t* capacity) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    uint64_t u = 0, cp = 0;
-    for (ctmr_ctx* c : g->m) {
-        uint64_t a = 0, b = 0;
-        const int rc = ctmr_table_stats(c, &a, &b);
-        if (rc) return group_fail(g, c, rc);
-        u += a;
-        cp += b;
-    }
-    if (slots_used) *slots_used = u;
-    if (capacity) *capacity = cp;
-    return CTMR_OK;
-}
-
-int ctmr_group_preload_known(ctmr_group* g, int64_t exp_hour, const uint8_t issuer_digest[32], const uint8_t* serial_blob,
-                             const uint64_t* serial_offsets, uint64_t n) {
-    if (!g || g->m.empty() || !issuer_digest || (n && (!serial_blob || !serial_offsets))) return CTMR_E_INVALID;
-    // the set's owner shard receives the serials (every table operation is local to the owner)
-    uint32_t issuer = 0;
-    bool found = false;
-    cudaSetDevice(g->m[0]->device);
-    int rc = lookup_digest(g->m[0], issuer_digest, true, &issuer, &found);
-    if (rc) return group_fail(g, g->m[0], rc);
-    if (exp_hour > INT32_MAX || exp_hour < INT32_MIN) return group_fail(g, g->m[0], fail(g->m[0], CTMR_E_INVALID, "exp_hour out of range"));
-    ctmr_ctx* owner = g->m[key_owner((int32_t)exp_hour, issuer, (uint32_t)g->m.size())];
-    rc = preload_impl(owner, exp_hour, issuer_digest, serial_blob, serial_offsets, n, g->next_index);
-    if (rc) return group_fail(g, owner, rc);
-    g->next_index += n;
-    return CTMR_OK;
-}
-
-int ctmr_group_evict_expired(ctmr_group* g, int64_t now_unix_sec, uint64_t* evicted_out) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    uint64_t total = 0;
-    for (ctmr_ctx* c : g->m) {  // every shard drops the expired sets it owns
-        uint64_t e = 0;
-        const int rc = ctmr_evict_expired(c, now_unix_sec, &e);
-        if (rc) return group_fail(g, c, rc);
-        total += e;
-    }
-    if (evicted_out) *evicted_out = total;
-    return CTMR_OK;
-}
-
-// Snapshot of a whole group: every shard's tables and histograms + the one issuer registry + the group's next index.
-namespace {
-struct GroupSnapHeader {
-    char magic[8];  // "CTMRGRP1"
-    uint64_t members, shard_bytes, table_slots, max_issuers, n_issuers, next_index;
-};
-}  // namespace
-
-int ctmr_group_snapshot_size(ctmr_group* g, uint64_t* bytes) {
-    if (!g || g->m.empty() || !bytes) return CTMR_E_INVALID;
-    ctmr_ctx* c0 = g->m[0];
-    cudaSetDevice(c0->device);
-    const int rc = refresh_digests(c0);
-    if (rc) return group_fail(g, c0, rc);
-    *bytes = sizeof(GroupSnapHeader) + g->m.size() * snap_shard_bytes(c0) + c0->digests.size() * 32;
-    return CTMR_OK;
-}
-
-int ctmr_group_snapshot_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written) {
-    uint64_t need = 0;
-    int rc = ctmr_group_snapshot_size(g, &need);
-    if (rc) return rc;
-    ctmr_ctx* c0 = g->m[0];
-    if (!buf || cap < need) return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "snapshot buffer too small"));
-    GroupSnapHeader h{};
-    std::memcpy(h.magic, "CTMRGRP1", 8);
-    h.members = g->m.size();
-    h.shard_bytes = snap_shard_bytes(c0);
-    h.table_slots = c0->st.table_mask + 1;
-    h.max_issuers = c0->st.max_issuers;
-    h.n_issuers = c0->digests.size();
-    h.next_index = g->next_index;
-    uint8_t* p = buf;
-    std::memcpy(p, &h, sizeof h); p += sizeof h;
-    for (ctmr_ctx* c : g->m) {
-        rc = snap_shard_save(c, p);
-        if (rc) return group_fail(g, c, rc);
-        p += h.shard_bytes;
-    }
-    for (const auto& d : c0->digests) { std::memcpy(p, d.data(), 32); p += 32; }
-    if (written) *written = (uint64_t)(p - buf);
-    return CTMR_OK;
-}
-
-int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    ctmr_ctx* c0 = g->m[0];
-    GroupSnapHeader h;
-    if (!buf || bytes < sizeof h) return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "bad snapshot"));
-    std::memcpy(&h, buf, sizeof h);
-    if (std::memcmp(h.magic, "CTMRGRP1", 8) != 0) return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "not a ctmr group snapshot"));
-    // the owner of a set depends on the group size: a snapshot only fits a group of the same shape
-    if (h.members != g->m.size() || h.shard_bytes != snap_shard_bytes(c0) || h.table_slots != c0->st.table_mask + 1 ||
-        h.max_issuers != c0->st.max_issuers || h.n_issuers > h.max_issuers)
-        return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "snapshot was taken by a group of another size or with other capacities"));
-    if (bytes < sizeof h + h.members * h.shard_bytes + h.n_issuers * 32) return group_fail(g, c0, fail(c0, CTMR_E_INVALID, "truncated snapshot"));
-    RegistryUpload u;
-    if (const int rc = snap_registry_alloc(c0, h.n_issuers, u)) return group_fail(g, c0, rc);
-    const uint8_t* p = buf + sizeof h;
-    for (ctmr_ctx* c : g->m) {
-        const int rc = snap_shard_load(c, p);
-        if (rc) return group_fail(g, c, rc);
-        p += h.shard_bytes;
-    }
-    const int rc = snap_registry_restore(c0, p, h.n_issuers, u);
-    if (rc) return group_fail(g, c0, rc);
-    g->next_index = h.next_index;
-    return CTMR_OK;
-}
-
-int ctmr_group_reset(ctmr_group* g) {
-    if (!g || g->m.empty()) return CTMR_E_INVALID;
-    for (ctmr_ctx* c : g->m) {
-        cudaSetDevice(c->device);
-        cudaDeviceSynchronize();
-    }
-    for (ctmr_ctx* c : g->m) {
-        int rc = ctmr_reset_device(c, nullptr);
-        if (rc) return group_fail(g, c, rc);
-        if (cudaStreamSynchronize(c->stream) != cudaSuccess) return group_fail(g, c, fail(c, CTMR_E_CUDA, "reset failed"));
-    }
-    return CTMR_OK;
-}
 
 // ------------------------------------------------------------------------------------------------ one process per GPU
 namespace {

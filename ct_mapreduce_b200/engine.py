@@ -58,7 +58,8 @@ class BatchResult:
 
 
 class KnownCertificatesView:
-    """Read side of storage.KnownCertificates for one (expDate, issuer) (knowncertificates.go:57-63)."""
+    """Read side of storage.KnownCertificates for one (expDate, issuer) (knowncertificates.go:57-63), on a ctx or a
+    group."""
 
     def __init__(self, db: "GpuCertDatabase", exp_hour: int, issuer_digest: bytes):
         self._db, self.exp_hour, self.issuer_digest = db, int(exp_hour), bytes(issuer_digest)
@@ -66,7 +67,7 @@ class KnownCertificatesView:
     def count(self) -> int:
         out = C.c_uint64(0)
         d = (C.c_uint8 * 32).from_buffer_copy(self.issuer_digest)
-        self._db._check(self._db._lib.ctmr_set_cardinality(self._db._h, self.exp_hour, d, C.byref(out)))
+        self._db._check(self._db._c("set_cardinality")(self._db._h, self.exp_hour, d, C.byref(out)))
         return out.value
 
 
@@ -120,6 +121,37 @@ def _pack(ders):
     offsets = np.zeros(len(ders) + 1, np.uint64)
     offsets[1:] = np.cumsum([len(d) for d in ders], dtype=np.uint64)
     return np.frombuffer(b"".join(ders) or b"\0", np.uint8).copy(), offsets
+
+
+def _config(table_capacity: int, issuer_cn_filter: bytes | str, log_expired_entries: bool, flags: int, max_issuers: int,
+            max_batch_entries: int, max_batch_bytes: int, pair_capacity_log2: int, meta_capacity_log2: int,
+            max_round_entries: int = 0, device: int = 0) -> "capi.Config":
+    """ctmr_config of a ctx or a group (whose create sets each member's device)"""
+    if isinstance(issuer_cn_filter, str):
+        issuer_cn_filter = issuer_cn_filter.encode()
+    cfg = capi.Config()
+    cfg.struct_size = C.sizeof(capi.Config)
+    cfg.device = device
+    cfg.table_capacity, cfg.max_batch_entries, cfg.max_batch_bytes = table_capacity, max_batch_entries, max_batch_bytes
+    cfg.max_issuers, cfg.pair_capacity_log2, cfg.meta_capacity_log2 = max_issuers, pair_capacity_log2, meta_capacity_log2
+    cfg.max_round_entries = max_round_entries
+    cfg.issuer_cn_filter = bytes(issuer_cn_filter)
+    cfg.issuer_cn_filter_len = len(issuer_cn_filter)
+    cfg.log_expired_entries, cfg.flags = int(bool(log_expired_entries)), flags
+    return cfg
+
+
+def _at(a, e0: int = 0, per: int = 1):
+    """address of row e0 of a (rows of `per` elements), or None"""
+    return None if a is None else capi.ptr(a) + e0 * per * a.itemsize
+
+
+def _path_out(p: BatchResult, want_sha: bool, want_meta: bool, e0: int = 0) -> "capi.Out":
+    """ctmr_out over p's arrays from entry e0 on: sha256 with want_sha, the string-identity arrays with want_meta"""
+    meta = [_at(p.issuer_name_off, e0), _at(p.issuer_name_len, e0), _at(p.crldp_off, e0), _at(p.crldp_len, e0),
+            _at(p.first_issuer_dn, e0), _at(p.first_crldp, e0)] if want_meta else [None] * 6
+    return capi.Out(_at(p.status, e0), _at(p.sha256, e0, 32) if want_sha else None, _at(p.exp_hour, e0), _at(p.serial_off, e0),
+                    _at(p.serial_len, e0), _at(p.was_unknown, e0), _at(p.first_issuer_hour, e0), *meta)
 
 
 def _attach_pem(o: "capi.Out", res: BatchResult, n: int, der_bytes: int):
@@ -281,6 +313,7 @@ class GpuCertDatabase:
     """One ctmr_ctx = one GPU's share of the known-certificate state."""
 
     _peers = False   # attached to peers in other processes (peer_attach): the front end is collective
+    _form = "ctmr_"  # prefix of the C entry points that take this handle (a group's: ctmr_group_)
 
     def __init__(self, device: int = 0, table_capacity: int = 1 << 22, issuer_cn_filter: bytes | str = b"",
                  log_expired_entries: bool = False, flags: int = 0, max_issuers: int = 0, max_batch_entries: int = 0,
@@ -291,23 +324,8 @@ class GpuCertDatabase:
             self._h, self.device, self.flags, self._owned = _adopt, device, flags, False
             return
         self._owned = True
-        if isinstance(issuer_cn_filter, str):
-            issuer_cn_filter = issuer_cn_filter.encode()
-        self._filter = bytes(issuer_cn_filter)
-        cfg = capi.Config()
-        cfg.struct_size = C.sizeof(capi.Config)
-        cfg.device = device
-        cfg.table_capacity = table_capacity
-        cfg.max_batch_entries = max_batch_entries
-        cfg.max_batch_bytes = max_batch_bytes
-        cfg.max_issuers = max_issuers
-        cfg.pair_capacity_log2 = pair_capacity_log2
-        cfg.meta_capacity_log2 = meta_capacity_log2
-        cfg.max_round_entries = max_round_entries
-        cfg.issuer_cn_filter = self._filter
-        cfg.issuer_cn_filter_len = len(self._filter)
-        cfg.log_expired_entries = int(bool(log_expired_entries))
-        cfg.flags = flags
+        cfg = _config(table_capacity, issuer_cn_filter, log_expired_entries, flags, max_issuers, max_batch_entries,
+                      max_batch_bytes, pair_capacity_log2, meta_capacity_log2, max_round_entries, device)
         h = C.c_void_p()
         rc = self._lib.ctmr_create(C.byref(cfg), C.byref(h))
         if rc != 0:
@@ -317,9 +335,18 @@ class GpuCertDatabase:
         self.flags = flags
 
     # ------------------------------------------------------------------ plumbing
+    def _c(self, name: str):
+        """the C entry point `name` in this handle's form: ctmr_<name>, or ctmr_group_<name> on a group"""
+        return getattr(self._lib, self._form + name)
+
+    @property
+    def _registry(self) -> "GpuCertDatabase":
+        """the ctx whose handle reaches the issuer registry: this one (a group's member 0)"""
+        return self
+
     def _check(self, rc: int):
         if rc != 0:
-            raise CtmrError(rc, (self._lib.ctmr_last_error(self._h) or b"").decode())
+            raise CtmrError(rc, (self._c("last_error")(self._h) or b"").decode())
 
     def close(self):
         if getattr(self, "_h", None):
@@ -350,12 +377,14 @@ class GpuCertDatabase:
         issuer_offsets = np.ascontiguousarray(issuer_offsets, np.uint64)
         n = issuer_offsets.size - 1
         out = np.zeros(max(n, 1), np.uint32)
-        self._check(self._lib.ctmr_register_issuers(self._h, capi.ptr(issuer_blob), capi.ptr(issuer_offsets), n, capi.ptr(out)))
+        reg = self._registry
+        reg._check(self._lib.ctmr_register_issuers(reg._h, capi.ptr(issuer_blob), capi.ptr(issuer_offsets), n, capi.ptr(out)))
         return out[:n]
 
     def issuer_digest(self, dense_idx: int) -> bytes:
         d = (C.c_uint8 * 32)()
-        self._check(self._lib.ctmr_issuer_digest(self._h, dense_idx, d))
+        reg = self._registry
+        reg._check(self._lib.ctmr_issuer_digest(reg._h, dense_idx, d))
         return bytes(d)
 
     # ------------------------------------------------------------------ the hot path, host buffers
@@ -380,21 +409,14 @@ class GpuCertDatabase:
             out.issuer_name_off, out.issuer_name_len = np.zeros(n, np.uint32), np.zeros(n, np.uint32)
             out.crldp_off, out.crldp_len = np.zeros(n, np.uint32), np.zeros(n, np.uint32)
             out.first_issuer_dn, out.first_crldp = np.zeros(n, np.uint8), np.zeros(n, np.uint8)
-        o = capi.Out(capi.ptr(out.status), capi.ptr(out.sha256) if want_sha else None, capi.ptr(out.exp_hour),
-                     capi.ptr(out.serial_off), capi.ptr(out.serial_len), capi.ptr(out.was_unknown),
-                     capi.ptr(out.first_issuer_hour),
-                     *([capi.ptr(out.issuer_name_off), capi.ptr(out.issuer_name_len), capi.ptr(out.crldp_off),
-                        capi.ptr(out.crldp_len), capi.ptr(out.first_issuer_dn), capi.ptr(out.first_crldp)] if want_meta else [None] * 6))
+        o = _path_out(out, want_sha, want_meta)
         if want_pem:
             _attach_pem(o, out, n, int(blob.size))
-        self._check(self._process_batch_fn()(self._h, capi.ptr(blob), capi.ptr(offsets), n,
+        self._check(self._c("process_batch")(self._h, capi.ptr(blob), capi.ptr(offsets), n,
                                              capi.ptr(issuer_blob) if n_iss else None,
                                              capi.ptr(issuer_offsets) if n_iss else None, n_iss,
                                              capi.ptr(issuer_idx), now_unix_ns, C.byref(o)))
         return out
-
-    def _process_batch_fn(self):
-        return self._lib.ctmr_process_batch
 
     # ------------------------------------------------------------------ CT wire-format front end (include/ctmr_frontend.h)
     def store_raw_entries(self, text, leaf_off, leaf_len, extra_off, extra_len, now_unix_ns: int, want_sha: bool = True,
@@ -417,10 +439,7 @@ class GpuCertDatabase:
         r = RawBatchResult(n, want_sha, want_meta)
         p = r.path
         o = capi.RawOut()
-        o.path = capi.Out(capi.ptr(p.status), capi.ptr(p.sha256) if want_sha else None, capi.ptr(p.exp_hour), capi.ptr(p.serial_off),
-                          capi.ptr(p.serial_len), capi.ptr(p.was_unknown), capi.ptr(p.first_issuer_hour),
-                          *([capi.ptr(p.issuer_name_off), capi.ptr(p.issuer_name_len), capi.ptr(p.crldp_off), capi.ptr(p.crldp_len),
-                             capi.ptr(p.first_issuer_dn), capi.ptr(p.first_crldp)] if want_meta else [None] * 6))
+        o.path = _path_out(p, want_sha, want_meta)
         for name in ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_src", "leaf_off", "leaf_len"):
             setattr(o, name, capi.ptr(getattr(r, name)))
         if want_pem:
@@ -429,26 +448,17 @@ class GpuCertDatabase:
                           n, now_unix_ns)
         if trees is not None:
             arr = _trees_to_c(trees)
-            self._check(self._process_raw_trees_fn()(self._h, C.byref(b), C.byref(o), capi.ptr(log) if n else None,
+            self._check(self._c("process_raw_trees")(self._h, C.byref(b), C.byref(o), capi.ptr(log) if n else None,
                                                      arr if trees else None, len(trees)))
             r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
             return r
         if tree is None:
-            self._check(self._process_raw_fn()(self._h, C.byref(b), C.byref(o)))
+            self._check(self._c("process_raw")(self._h, C.byref(b), C.byref(o)))
             return r
         ct = tree.to_c()
-        self._check(self._process_raw_tree_fn()(self._h, C.byref(b), C.byref(o), C.byref(ct)))
+        self._check(self._c("process_raw_tree")(self._h, C.byref(b), C.byref(o), C.byref(ct)))
         r.tree = LogTree.from_c(ct)
         return r
-
-    def _process_raw_fn(self):
-        return self._lib.ctmr_process_raw
-
-    def _process_raw_tree_fn(self):
-        return self._lib.ctmr_process_raw_tree
-
-    def _process_raw_trees_fn(self):
-        return self._lib.ctmr_process_raw_trees
 
     def store_raw_bodies(self, text, body_off, body_len, body_max, now_unix_ns: int, want_sha: bool = True, want_meta: bool = False,
                          want_pem: bool = False, tree: LogTree | None = None, trees=None, body_log=None,
@@ -478,10 +488,7 @@ class GpuCertDatabase:
         r = BodiesResult(cap, nb, want_sha, want_meta)
         p = r.path
         o = capi.BodyOut()
-        o.raw.path = capi.Out(capi.ptr(p.status), capi.ptr(p.sha256) if want_sha else None, capi.ptr(p.exp_hour), capi.ptr(p.serial_off),
-                              capi.ptr(p.serial_len), capi.ptr(p.was_unknown), capi.ptr(p.first_issuer_hour),
-                              *([capi.ptr(p.issuer_name_off), capi.ptr(p.issuer_name_len), capi.ptr(p.crldp_off), capi.ptr(p.crldp_len),
-                                 capi.ptr(p.first_issuer_dn), capi.ptr(p.first_crldp)] if want_meta else [None] * 6))
+        o.raw.path = _path_out(p, want_sha, want_meta)
         for name in ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_src", "leaf_off", "leaf_len"):
             setattr(o.raw, name, capi.ptr(getattr(r, name)))
         for name in ("body_status", "body_first", "body_entries", "leaf_input_off", "leaf_input_len", "extra_data_off",
@@ -493,26 +500,17 @@ class GpuCertDatabase:
         starts = capi.ptr(start) if start is not None and nb else None
         if trees is not None:
             arr = _trees_to_c(trees)
-            self._check(self._process_raw_bodies_trees_fn()(self._h, C.byref(b), C.byref(o), capi.ptr(log) if log is not None and nb else None,
+            self._check(self._c("process_raw_bodies_trees")(self._h, C.byref(b), C.byref(o), capi.ptr(log) if log is not None and nb else None,
                                                             starts, arr if trees else None, len(trees)))
             r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
         elif tree is not None:
             ct = tree.to_c()
-            self._check(self._process_raw_bodies_tree_fn()(self._h, C.byref(b), C.byref(o), starts, C.byref(ct)))
+            self._check(self._c("process_raw_bodies_tree")(self._h, C.byref(b), C.byref(o), starts, C.byref(ct)))
             r.tree = LogTree.from_c(ct)
         else:
-            self._check(self._process_raw_bodies_fn()(self._h, C.byref(b), C.byref(o)))
+            self._check(self._c("process_raw_bodies")(self._h, C.byref(b), C.byref(o)))
         r.trim(int(o.n_entries))
         return r
-
-    def _process_raw_bodies_fn(self):
-        return self._lib.ctmr_process_raw_bodies
-
-    def _process_raw_bodies_tree_fn(self):
-        return self._lib.ctmr_process_raw_bodies_tree
-
-    def _process_raw_bodies_trees_fn(self):
-        return self._lib.ctmr_process_raw_bodies_trees
 
     def bodies_profile_last(self) -> float:
         """Milliseconds of the JSON kernels in the last store_raw_bodies call, part of frontend_ms."""
@@ -529,21 +527,9 @@ class GpuCertDatabase:
         n = offsets.size - 1
         dense = np.zeros(max(n, 1), np.uint32)
         fps = np.zeros((max(n, 1), 32), np.uint8)
-        self._check(self._register_chain_fn()(self._h, capi.ptr(blob) if blob.size else None, capi.ptr(offsets), n, capi.ptr(dense),
-                                              capi.ptr(fps)))
+        self._check(self._c("register_chain_certs")(self._h, capi.ptr(blob) if blob.size else None, capi.ptr(offsets), n,
+                                                    capi.ptr(dense), capi.ptr(fps)))
         return dense[:n], fps[:n]
-
-    def _register_chain_fn(self):
-        return self._lib.ctmr_register_chain_certs
-
-    def _process_tiles_fn(self):
-        return self._lib.ctmr_process_tiles
-
-    def _process_tiles_tree_fn(self):
-        return self._lib.ctmr_process_tiles_tree
-
-    def _process_tiles_trees_fn(self):
-        return self._lib.ctmr_process_tiles_trees
 
     def store_tiles(self, data, tile_off, tile_len, tile_index, tile_width, now_unix_ns: int, want_sha: bool = True,
                     want_meta: bool = False, want_pem: bool = False, want_leaf_hash: bool = False, missing_cap: int = 256,
@@ -579,20 +565,13 @@ class GpuCertDatabase:
         t0, pem_base = 0, 0
         while True:
             e0 = int(ent[t0])
-
-            def at(a, per=1):
-                return None if a is None else capi.ptr(a) + e0 * per * a.itemsize
-
             o = capi.TileOut()
-            o.path = capi.Out(at(p.status), at(p.sha256, 32) if want_sha else None, at(p.exp_hour), at(p.serial_off),
-                              at(p.serial_len), at(p.was_unknown), at(p.first_issuer_hour),
-                              *([at(p.issuer_name_off), at(p.issuer_name_len), at(p.crldp_off), at(p.crldp_len),
-                                 at(p.first_issuer_dn), at(p.first_crldp)] if want_meta else [None] * 6))
+            o.path = _path_out(p, want_sha, want_meta, e0)
             if want_pem:
-                o.path.pem, o.path.pem_cap, o.path.pem_off = capi.ptr(p.pem) + pem_base, p.pem.size - pem_base, at(p.pem_off)
+                o.path.pem, o.path.pem_cap, o.path.pem_off = capi.ptr(p.pem) + pem_base, p.pem.size - pem_base, _at(p.pem_off, e0)
             for name in ("entry_status", "entry_type", "timestamp_ms", "issuer", "leaf_index", "leaf_off", "leaf_len"):
-                setattr(o, name, at(getattr(r, name)))
-            o.leaf_hash = at(r.leaf_hash, 32)
+                setattr(o, name, _at(getattr(r, name), e0))
+            o.leaf_hash = _at(r.leaf_hash, e0, 32)
             o.tile_status = capi.ptr(r.tile_status) + t0
             o.missing_fp, o.missing_cap = capi.ptr(miss), missing_cap
             b = capi.TileBatch(capi.ptr(data), data.size, capi.ptr(tile_off) + 8 * t0, capi.ptr(tile_len) + 4 * t0,
@@ -605,14 +584,14 @@ class GpuCertDatabase:
                         rest = np.flatnonzero(tlog[t0:] == d)
                         if rest.size and arr[d].size < 256 * int(tile_index[t0 + rest[0]]):
                             tlog[t0 + rest] = capi.NO_TREE
-                rc = self._process_tiles_trees_fn()(self._h, C.byref(b), C.byref(o), capi.ptr(tlog) + 4 * t0 if nt else None,
+                rc = self._c("process_tiles_trees")(self._h, C.byref(b), C.byref(o), capi.ptr(tlog) + 4 * t0 if nt else None,
                                                     arr if trees else None, len(trees))
                 if rc in (0, capi.E_UNKNOWN_ISSUER):
                     r.trees = [LogTree.from_c(arr[d]) for d in range(len(trees))]
             elif ct is None:
-                rc = self._process_tiles_fn()(self._h, C.byref(b), C.byref(o))
+                rc = self._c("process_tiles")(self._h, C.byref(b), C.byref(o))
             else:  # written back on success and at the stop: the resumed call continues this tree
-                rc = self._process_tiles_tree_fn()(self._h, C.byref(b), C.byref(o), C.byref(ct))
+                rc = self._c("process_tiles_tree")(self._h, C.byref(b), C.byref(o), C.byref(ct))
                 if rc in (0, capi.E_UNKNOWN_ISSUER):
                     r.tree = LogTree.from_c(ct)
             done = int(o.tiles_done)
@@ -625,7 +604,7 @@ class GpuCertDatabase:
             r.missing = [miss[k].tobytes() for k in range(o.n_missing)] if rc == capi.E_UNKNOWN_ISSUER else []
             if rc != capi.E_UNKNOWN_ISSUER:
                 if rc and fetch is not None:   # the others' resumed calls wait for this rank too
-                    err = CtmrError(rc, (self._lib.ctmr_last_error(self._h) or b"").decode())
+                    err = CtmrError(rc, (self._c("last_error")(self._h) or b"").decode())
                     self._join_resumes()
                     raise err
                 self._check(rc)
@@ -747,29 +726,21 @@ class GpuCertDatabase:
     def preload_known(self, exp_hour: int, issuer_digest: bytes, serials):
         """Seed one "serials::<expDate>::<issuer>" set (e.g. KnownCertificates.Known() read back from Redis)."""
         serials = [bytes(x) for x in serials]
-        offs = np.zeros(len(serials) + 1, np.uint64)
-        offs[1:] = np.cumsum([len(x) for x in serials], dtype=np.uint64)
-        blob = np.frombuffer(b"".join(serials) or b"\0", np.uint8).copy()
+        blob, offs = _pack(serials)
         d = (C.c_uint8 * 32).from_buffer_copy(issuer_digest)
-        self._check(self._lib.ctmr_preload_known(self._h, exp_hour, d, capi.ptr(blob), capi.ptr(offs), len(serials)))
+        self._check(self._c("preload_known")(self._h, exp_hour, d, capi.ptr(blob), capi.ptr(offs), len(serials)))
 
     def snapshot(self) -> np.ndarray:
         need = C.c_uint64(0)
-        self._check(self._lib.ctmr_snapshot_size(self._h, C.byref(need)))
+        self._check(self._c("snapshot_size")(self._h, C.byref(need)))
         buf = np.empty(need.value, np.uint8)
         wrote = C.c_uint64(0)
-        self._check(self._lib.ctmr_snapshot_save(self._h, capi.ptr(buf), buf.size, C.byref(wrote)))
+        self._check(self._c("snapshot_save")(self._h, capi.ptr(buf), buf.size, C.byref(wrote)))
         return buf[:wrote.value]
 
     def restore(self, snap: np.ndarray):
         snap = np.ascontiguousarray(snap, np.uint8)
-        self._check(self._lib.ctmr_snapshot_load(self._h, capi.ptr(snap), snap.size))
-
-    def _checkpoint_fns(self):
-        return self._lib.ctmr_checkpoint_size, self._lib.ctmr_checkpoint_save, self._lib.ctmr_checkpoint_load
-
-    def _revoked_known_fn(self):
-        return self._lib.ctmr_revoked_known
+        self._check(self._c("snapshot_load")(self._h, capi.ptr(snap), snap.size))
 
     def revoked_known(self, crls, issuer_digests, entry_cap: int | None = None) -> RevokedResult:
         """Which revoked serials of these CRLs are known certificates (ctmr_revoked_known).  `crls`: a list of DER CRLs,
@@ -779,13 +750,13 @@ class GpuCertDatabase:
         On a db attached to peers the call is collective: every rank calls it with its own CRLs (an empty list will do)
         and gets the answers for its own CRLs against every rank's shard.  A rank whose arguments are refused here
         still makes the call, with no batch, so that the other ranks return CTMR_E_PEER_FAILED, and then raises."""
-        with self._peer_refusal(lambda: self._revoked_known_fn()(self._h, None, None)):
+        with self._peer_refusal(lambda: self._c("revoked_known")(self._h, None, None)):
             b, keep = _crl_batch(crls, issuer_digests)
             lens = keep[2]
             cap = int(lens.sum()) // capi.CRL_MIN_ENTRY if entry_cap is None else int(entry_cap)
             res = RevokedResult(int(b.n_crls), cap)
             o = res.to_c()
-        rc = self._revoked_known_fn()(self._h, C.byref(b), C.byref(o))
+        rc = self._c("revoked_known")(self._h, C.byref(b), C.byref(o))
         res.n_entries = int(o.n_entries)
         try:
             self._check(rc)
@@ -794,9 +765,6 @@ class GpuCertDatabase:
             raise
         res.trim(int(o.n_entries))
         return res
-
-    def _revoked_cascade_fn(self):
-        return self._lib.ctmr_revoked_cascade
 
     _cascade_bytes = 0   # size of the last cascade this db built: the next call's first buffer holds twice that
 
@@ -815,7 +783,7 @@ class GpuCertDatabase:
         CRLs.  A buffer too small on any rank is too small on every rank, so every rank builds it the second time together.
         A rank whose arguments are refused here still makes the call, with no batch, so that the other ranks return
         CTMR_E_PEER_FAILED, and then raises."""
-        fn = self._revoked_cascade_fn()
+        fn = self._c("revoked_cascade")
         with self._peer_refusal(lambda: fn(self._h, None, 0, None, 0, None)):
             b, keep = _crl_batch(crls, issuer_digests)
             salt = bytes(salt)
@@ -834,9 +802,6 @@ class GpuCertDatabase:
         self._cascade_bytes = int(o.bytes)
         return CascadeResult(buf[:o.bytes].tobytes(), status[:b.n_crls].copy(), o)
 
-    def _revoked_stash_fn(self):
-        return self._lib.ctmr_revoked_stash
-
     _stash_bytes = 0   # size of the last stash this db computed: the next call's first buffer holds twice that
 
     def revoked_stash(self, crls, issuer_digests, now_unix_sec: int, filter: bytes, stashes: bytes = b"",
@@ -848,7 +813,7 @@ class GpuCertDatabase:
         and .serials.  The output buffer holds `cap` bytes; by default 1 MiB, or twice the last stash this db computed if
         that is more.  A larger stash is computed twice: the first call only reports its size.  Not on a db attached to
         peers (CTMR_E_INVALID on every rank)."""
-        fn = self._revoked_stash_fn()
+        fn = self._c("revoked_stash")
         b, keep = _crl_batch(crls, issuer_digests)
         filter, stashes = bytes(filter), bytes(stashes)
         fbuf = (C.c_uint8 * max(len(filter), 1)).from_buffer_copy(filter or b"\0")
@@ -870,12 +835,11 @@ class GpuCertDatabase:
     def checkpoint(self) -> np.ndarray:
         """This db's part of a portable checkpoint (ctmr_checkpoint_save): loads into any table size, group size or number
         of ranks.  On a db attached to peers it is collective, and every rank returns its own part."""
-        size, save, _ = self._checkpoint_fns()
         need = C.c_uint64(0)
-        self._check(size(self._h, C.byref(need)))
+        self._check(self._c("checkpoint_size")(self._h, C.byref(need)))
         buf = np.empty(max(need.value, 1), np.uint8)
         wrote = C.c_uint64(0)
-        self._check(save(self._h, capi.ptr(buf), buf.size, C.byref(wrote)))
+        self._check(self._c("checkpoint_save")(self._h, capi.ptr(buf), buf.size, C.byref(wrote)))
         return buf[:wrote.value]
 
     def load_checkpoint(self, parts):
@@ -886,13 +850,13 @@ class GpuCertDatabase:
         parts = [np.ascontiguousarray(p, np.uint8) for p in parts]
         ptrs = (C.c_void_p * max(len(parts), 1))(*[p.ctypes.data for p in parts])
         sizes = (C.c_uint64 * max(len(parts), 1))(*[p.size for p in parts])
-        self._check(self._checkpoint_fns()[2](self._h, ptrs, sizes, len(parts)))
+        self._check(self._c("checkpoint_load")(self._h, ptrs, sizes, len(parts)))
 
     def evict_expired(self, now_unix_sec: int) -> int:
         """Apply the Redis TTLs (EXPIREAT(expDate) on every serials:: set, knowncertificates.go:98-104): sets with
         expDate <= now vanish.  Returns the number of serials dropped."""
         n = C.c_uint64(0)
-        self._check(self._lib.ctmr_evict_expired(self._h, int(now_unix_sec), C.byref(n)))
+        self._check(self._c("evict_expired")(self._h, int(now_unix_sec), C.byref(n)))
         return int(n.value)
 
     # ------------------------------------------------------------------ reducers' read side
@@ -901,21 +865,21 @@ class GpuCertDatabase:
 
     def issuer_counts(self) -> dict:
         """{Issuer.ID digest (32 bytes): number of unique certificates} for every registered issuer."""
-        n = C.c_size_t(self._lib.ctmr_issuer_count(self._h))
+        n = C.c_size_t(self._lib.ctmr_issuer_count(self._registry._h))
         cap = max(int(n.value), 1)
         dig = np.zeros((cap, 32), np.uint8)
         cnt = np.zeros(cap, np.uint64)
-        self._check(self._lib.ctmr_issuer_counts(self._h, capi.ptr(dig), capi.ptr(cnt), C.byref(n)))
+        self._check(self._c("issuer_counts")(self._h, capi.ptr(dig), capi.ptr(cnt), C.byref(n)))
         return {bytes(dig[i]): int(cnt[i]) for i in range(n.value)}
 
     def status_counters(self) -> np.ndarray:
         out = np.zeros(capi.ST_COUNT, np.uint64)
-        self._check(self._lib.ctmr_status_counters(self._h, capi.ptr(out)))
+        self._check(self._c("status_counters")(self._h, capi.ptr(out)))
         return out
 
     def table_stats(self):
         used, cap = C.c_uint64(0), C.c_uint64(0)
-        self._check(self._lib.ctmr_table_stats(self._h, C.byref(used), C.byref(cap)))
+        self._check(self._c("table_stats")(self._h, C.byref(used), C.byref(cap)))
         return used.value, cap.value
 
 
@@ -924,19 +888,14 @@ class GpuCertGroup(GpuCertDatabase):
     StartDatabaseThreads (cmd/ct-fetch/ct-fetch.go:140-145).  Same methods, globally exact results: every set
     "serials::<expDate>::<issuer>" lives on one owner GPU and the map kernels insert into it over NVLink."""
 
+    _form = "ctmr_group_"
+
     def __init__(self, devices, table_capacity: int = 1 << 22, issuer_cn_filter: bytes | str = b"", log_expired_entries: bool = False,
                  flags: int = 0, max_issuers: int = 0, max_batch_entries: int = 0, max_batch_bytes: int = 0,
                  pair_capacity_log2: int = 0, meta_capacity_log2: int = 0):
         self._lib = capi.load()
-        if isinstance(issuer_cn_filter, str):
-            issuer_cn_filter = issuer_cn_filter.encode()
-        self._filter = bytes(issuer_cn_filter)
-        cfg = capi.Config()
-        cfg.struct_size = C.sizeof(capi.Config)
-        cfg.table_capacity, cfg.max_batch_entries, cfg.max_batch_bytes = table_capacity, max_batch_entries, max_batch_bytes
-        cfg.max_issuers, cfg.pair_capacity_log2, cfg.meta_capacity_log2 = max_issuers, pair_capacity_log2, meta_capacity_log2
-        cfg.issuer_cn_filter, cfg.issuer_cn_filter_len = self._filter, len(self._filter)
-        cfg.log_expired_entries, cfg.flags = int(bool(log_expired_entries)), flags
+        cfg = _config(table_capacity, issuer_cn_filter, log_expired_entries, flags, max_issuers, max_batch_entries,
+                      max_batch_bytes, pair_capacity_log2, meta_capacity_log2)
         devs = (C.c_int32 * len(devices))(*devices)
         h = C.c_void_p()
         rc = self._lib.ctmr_group_create(C.byref(cfg), devs, len(devices), C.byref(h))
@@ -947,9 +906,9 @@ class GpuCertGroup(GpuCertDatabase):
         self.members = [GpuCertDatabase(device=devices[r], flags=flags, _adopt=C.c_void_p(self._lib.ctmr_group_member(h, r)))
                         for r in range(len(devices))]
 
-    def _check(self, rc: int):
-        if rc != 0:
-            raise CtmrError(rc, (self._lib.ctmr_group_last_error(self._h) or b"").decode())
+    @property
+    def _registry(self) -> GpuCertDatabase:
+        return self.members[0]   # the registry is the group's, in member 0's memory
 
     def close(self):
         if getattr(self, "_h", None):
@@ -957,36 +916,6 @@ class GpuCertGroup(GpuCertDatabase):
                 m._h = None
             self._lib.ctmr_group_destroy(self._h)
             self._h = None
-
-    def _process_batch_fn(self):
-        return self._lib.ctmr_group_process_batch
-
-    def _process_raw_fn(self):
-        return self._lib.ctmr_group_process_raw
-
-    def _process_raw_bodies_fn(self):
-        return self._lib.ctmr_group_process_raw_bodies
-
-    def _process_raw_bodies_tree_fn(self):
-        return self._lib.ctmr_group_process_raw_bodies_tree
-
-    def _process_raw_bodies_trees_fn(self):
-        return self._lib.ctmr_group_process_raw_bodies_trees
-
-    def _process_tiles_fn(self):
-        return self._lib.ctmr_group_process_tiles
-
-    def _process_raw_tree_fn(self):
-        return self._lib.ctmr_group_process_raw_tree
-
-    def _process_raw_trees_fn(self):
-        return self._lib.ctmr_group_process_raw_trees
-
-    def _process_tiles_tree_fn(self):
-        return self._lib.ctmr_group_process_tiles_tree
-
-    def _process_tiles_trees_fn(self):
-        return self._lib.ctmr_group_process_tiles_trees
 
     def store_raw_entries(self, *a, tree=None, trees=None, **k):
         if tree is not None or trees is not None:
@@ -1019,83 +948,8 @@ class GpuCertGroup(GpuCertDatabase):
         fetch-and-resume loop and per-log resume rule as GpuCertDatabase.store_tiles"""
         return GpuCertDatabase.store_tiles(self, *a, fetch=fetch, tree=tree, trees=trees, tile_log=tile_log, **k)
 
-    def _register_chain_fn(self):
-        return self._lib.ctmr_group_register_chain_certs
-
-    def register_issuers(self, issuer_blob, issuer_offsets):
-        return self.members[0].register_issuers(issuer_blob, issuer_offsets)   # the registry is the group's
-
-    def issuer_digest(self, dense_idx: int) -> bytes:
-        return self.members[0].issuer_digest(dense_idx)
-
-    def preload_known(self, exp_hour: int, issuer_digest: bytes, serials):
-        serials = [bytes(x) for x in serials]
-        offs = np.zeros(len(serials) + 1, np.uint64)
-        offs[1:] = np.cumsum([len(x) for x in serials], dtype=np.uint64)
-        blob = np.frombuffer(b"".join(serials) or b"\0", np.uint8).copy()
-        d = (C.c_uint8 * 32).from_buffer_copy(issuer_digest)
-        self._check(self._lib.ctmr_group_preload_known(self._h, exp_hour, d, capi.ptr(blob), capi.ptr(offs), len(serials)))
-
-    def evict_expired(self, now_unix_sec: int) -> int:
-        n = C.c_uint64(0)
-        self._check(self._lib.ctmr_group_evict_expired(self._h, int(now_unix_sec), C.byref(n)))
-        return int(n.value)
-
     def reset(self):
         self._check(self._lib.ctmr_group_reset(self._h))
-
-    def snapshot(self) -> np.ndarray:
-        need = C.c_uint64(0)
-        self._check(self._lib.ctmr_group_snapshot_size(self._h, C.byref(need)))
-        buf = np.empty(need.value, np.uint8)
-        wrote = C.c_uint64(0)
-        self._check(self._lib.ctmr_group_snapshot_save(self._h, capi.ptr(buf), buf.size, C.byref(wrote)))
-        return buf[:wrote.value]
-
-    def restore(self, snap: np.ndarray):
-        snap = np.ascontiguousarray(snap, np.uint8)
-        self._check(self._lib.ctmr_group_snapshot_load(self._h, capi.ptr(snap), snap.size))
-
-    def _checkpoint_fns(self):
-        return self._lib.ctmr_group_checkpoint_size, self._lib.ctmr_group_checkpoint_save, self._lib.ctmr_group_checkpoint_load
-
-    def _revoked_known_fn(self):
-        return self._lib.ctmr_group_revoked_known
-
-    def _revoked_cascade_fn(self):
-        return self._lib.ctmr_group_revoked_cascade
-
-    def _revoked_stash_fn(self):
-        return self._lib.ctmr_group_revoked_stash
-
-    def get_known_certificates(self, exp_hour: int, issuer_digest: bytes):
-        grp = self
-
-        class _View:
-            def count(self_inner) -> int:
-                out = C.c_uint64(0)
-                d = (C.c_uint8 * 32).from_buffer_copy(bytes(issuer_digest))
-                grp._check(grp._lib.ctmr_group_set_cardinality(grp._h, int(exp_hour), d, C.byref(out)))
-                return out.value
-        return _View()
-
-    def issuer_counts(self) -> dict:
-        n = C.c_size_t(self._lib.ctmr_issuer_count(self.members[0]._h))
-        cap = max(int(n.value), 1)
-        dig = np.zeros((cap, 32), np.uint8)
-        cnt = np.zeros(cap, np.uint64)
-        self._check(self._lib.ctmr_group_issuer_counts(self._h, capi.ptr(dig), capi.ptr(cnt), C.byref(n)))
-        return {bytes(dig[i]): int(cnt[i]) for i in range(n.value)}
-
-    def status_counters(self) -> np.ndarray:
-        out = np.zeros(capi.ST_COUNT, np.uint64)
-        self._check(self._lib.ctmr_group_status_counters(self._h, capi.ptr(out)))
-        return out
-
-    def table_stats(self):
-        used, cap = C.c_uint64(0), C.c_uint64(0)
-        self._check(self._lib.ctmr_group_table_stats(self._h, C.byref(used), C.byref(cap)))
-        return used.value, cap.value
 
     def _single_ctx_only(self, *a, **k):
         raise CtmrError(capi.E_INVALID, "this entry point takes one ctx: use group.members[r] (read side) or the group's own methods")

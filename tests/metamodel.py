@@ -9,8 +9,8 @@ Mirrors, and must change with:
                     meta_insert_at (home slot (h1 >> 5) & mask, linear probing), meta_owner ((h1 >> 40) % world)
   ctmr_device.cuh   mix64
   ctmr_kernels.cuh  MetaSlot {h1, h2, inv_first, pad} (32 bytes)
-  ctmr_api.cu       SnapHeader ("CTMRSNP3" + six u64), then table, pairs, meta, issuer counts, status counts, digests
-  ctmr_pipeline.cu  GroupSnapHeader ("CTMRGRP1", members, shard_bytes, ...), then one shard per member in order
+  ctmr_api.cu       SnapHeader ("CTMRSNP3" + six u64), then table, pairs, meta, issuer counts, status counts, digests;
+                    a group's ("CTMRGRP1", members, shard_bytes, ...), then one shard per member in order
 """
 from __future__ import annotations
 

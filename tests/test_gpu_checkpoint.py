@@ -234,11 +234,11 @@ def test_failures_leave_the_stated_target(eng, ora):
                 assert code(lambda: t.load_checkpoint(parts)) == capi.E_INVALID, name
                 assert before == (t.issuer_counts(), t.table_stats(), t.status_counters().tolist()), name
             # a NULL part
-            fns = t._checkpoint_fns()
+            load = t._c("checkpoint_load")
             ptrs = (C.c_void_p * 2)(ck.ctypes.data, None)
             sizes = (C.c_uint64 * 2)(ck.size, ck.size)
-            assert fns[2](t._h, ptrs, sizes, 2) == capi.E_INVALID
-            assert fns[2](t._h, None, None, 0) == capi.E_INVALID
+            assert load(t._h, ptrs, sizes, 2) == capi.E_INVALID
+            assert load(t._h, None, None, 0) == capi.E_INVALID
             assert before == (t.issuer_counts(), t.table_stats(), t.status_counters().tolist())
             # the two parts of a two-part checkpoint load in any order: the same state as the one part
             t.load_checkpoint(two[::-1])
@@ -291,7 +291,7 @@ def test_failures_leave_the_stated_target(eng, ora):
     # a member of a group is refused
     with eng.GpuCertGroup([0, 0], **kw) as g:
         m = g.members[0]
-        assert m._checkpoint_fns()[2](m._h, (C.c_void_p * 1)(ck.ctypes.data), (C.c_uint64 * 1)(ck.size), 1) == capi.E_INVALID
+        assert m._c("checkpoint_load")(m._h, (C.c_void_p * 1)(ck.ctypes.data), (C.c_uint64 * 1)(ck.size), 1) == capi.E_INVALID
         need = C.c_uint64(0)
         assert m._lib.ctmr_checkpoint_size(m._h, C.byref(need)) == capi.E_INVALID
     assert nxt == part["next_index"]

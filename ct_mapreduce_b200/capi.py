@@ -20,6 +20,8 @@ ISSUER_NONE = 0xFFFFFFFF
 ISSUER_BAD = 0xFFFFFFFE
 F_NO_FINGERPRINT = 1
 E_INVALID = -1
+E_CUDA = -2
+E_NOMEM = -3
 E_TABLE_FULL = -4
 E_TOO_MANY_ISSUERS = -5
 E_NO_DEVICE = -6
@@ -53,6 +55,7 @@ EXPORTS = [
     "ctmr_revoked_known", "ctmr_group_revoked_known",   # CRLs joined with the known-certificate sets
     "ctmr_revoked_cascade", "ctmr_group_revoked_cascade",   # CRLite's filter cascade of the covered issuers
     "ctmr_revoked_stash", "ctmr_group_revoked_stash",   # CRLite's stash: what a published filter and its stashes miss
+    "ctmr_resize", "ctmr_group_resize", "ctmr_table_occupancy", "ctmr_group_table_occupancy",   # the tables in other sizes
 ]
 # the calls with a ctmr_group_<name> form beside ctmr_<name>
 GROUP_TWINS = (
@@ -60,7 +63,7 @@ GROUP_TWINS = (
     "preload_known", "evict_expired", "snapshot_size", "snapshot_save", "snapshot_load", "checkpoint_size", "checkpoint_save",
     "checkpoint_load", "process_raw", "process_raw_tree", "process_raw_trees", "process_raw_bodies", "process_raw_bodies_tree",
     "process_raw_bodies_trees", "process_tiles", "process_tiles_tree", "process_tiles_trees", "register_chain_certs",
-    "revoked_known", "revoked_cascade", "revoked_stash",
+    "revoked_known", "revoked_cascade", "revoked_stash", "resize", "table_occupancy",
 )
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -255,6 +258,8 @@ def load():
     L.ctmr_checkpoint_size.argtypes = [vp, C.POINTER(u64)]
     L.ctmr_checkpoint_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
     L.ctmr_checkpoint_load.argtypes = [vp, vp, vp, u32]
+    L.ctmr_resize.argtypes = [vp, u64, u32, u32]
+    L.ctmr_table_occupancy.argtypes = [vp, vp, vp]
     L.ctmr_evict_expired.argtypes = [vp, i64, C.POINTER(u64)]
     L.ctmr_sha256_ceiling_device.argtypes = [vp, u32, u32, u32, C.POINTER(C.c_float), C.POINTER(u64)]
     L.ctmr_profile_last.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float)]

@@ -56,6 +56,9 @@ int build_filter(const ctmr_config* cfg, FilterCfg& f) {
     return 0;
 }
 
+}  // namespace
+namespace ctmr_host {
+
 SharedLayout make_layout(uint64_t table_slots, uint64_t pair_slots, uint64_t meta_slots, uint32_t max_issuers) {
     SharedLayout l;
     auto take = [&](size_t bytes) {
@@ -76,8 +79,14 @@ SharedLayout make_layout(uint64_t table_slots, uint64_t pair_slots, uint64_t met
     return l;
 }
 
-}  // namespace
-namespace ctmr_host {
+void point_at_region(ctmr_ctx* c) {
+    c->st.table = reinterpret_cast<KnownSlot*>(c->shared + c->lay.table);
+    c->st.pairs = reinterpret_cast<PairSlot*>(c->shared + c->lay.pairs);
+    c->st.meta = reinterpret_cast<MetaSlot*>(c->shared + c->lay.meta);
+    c->st.issuer_counts = reinterpret_cast<unsigned long long*>(c->shared + c->lay.issuer_counts);
+    c->st.status_counts = reinterpret_cast<unsigned long long*>(c->shared + c->lay.status_counts);
+}
+
 int ensure_scratch(ctmr_ctx* c, uint64_t n) {
     if (n <= c->scratch_cap) return CTMR_OK;
     CU(c, cudaDeviceSynchronize());
@@ -646,11 +655,7 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
     c->lay = make_layout(cap, c->st.pair_mask + 1, c->st.meta_mask + 1, c->st.max_issuers);
     CU(nullptr, alloc(c->shared, c->lay.total));
     CU(nullptr, cudaMemsetAsync(c->shared, 0, c->lay.total, c->stream));
-    c->st.table = reinterpret_cast<KnownSlot*>(c->shared + c->lay.table);
-    c->st.pairs = reinterpret_cast<PairSlot*>(c->shared + c->lay.pairs);
-    c->st.meta = reinterpret_cast<MetaSlot*>(c->shared + c->lay.meta);
-    c->st.issuer_counts = reinterpret_cast<unsigned long long*>(c->shared + c->lay.issuer_counts);
-    c->st.status_counts = reinterpret_cast<unsigned long long*>(c->shared + c->lay.status_counts);
+    point_at_region(c.get());
     CU(nullptr, alloc(c->small, 1));
     CU(nullptr, cudaMemsetAsync(c->small, 0, sizeof(SmallDev), c->stream));
     c->st.slots_used = &c->small->slots_used;

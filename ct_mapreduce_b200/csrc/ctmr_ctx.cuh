@@ -4,7 +4,7 @@
 // calls of a ctx and a group (read side, preload, eviction, snapshots), front end plumbing;
 // ctmr_pipeline.cu: the host-buffer batch pipeline on one GPU, on a group of GPUs, and across processes, and the copy of
 // a round's outputs to the host, the group's lifecycle and the peer attach; ctmr_frontend_api.cu: the wire-format front
-// end on one GPU and on a group).
+// end on one GPU and on a group; ctmr_resize.cu: the tables of a ctx or a group in other sizes).
 //
 // Ownership: the ctx owns everything it allocates, through the handles below and std::unique_ptr, so deleting the ctx
 // releases it all.  The parts built on first use (the pipeline stages, ctmr_process_device's streams and events, the
@@ -395,6 +395,8 @@ struct SmallDev {
     uint32_t sha_sink;               // ctmr_sha256_ceiling_device's sink
     alignas(16) uint8_t digest[32];  // lookup_digest: one digest to register
     uint32_t idx;                    //   and its index
+    int resize_error;                // ctmr_resize's rehash: its own flag, so that a failed resize leaves error_flag as it was
+    unsigned long long occupancy[3]; // ctmr_table_occupancy's counts: known, pair, meta
 };
 
 }  // namespace ctmr_host
@@ -453,6 +455,7 @@ struct ctmr_ctx {
     DevBuf<uint8_t> xchg;
     uint64_t X = 0, cfg_round_entries = 0;
     uint32_t exported_world = 0;            // ctmr_peer_export was called for a group of this size (the views follow at attach)
+    bool ipc_exported = false;              // ctmr_peer_export was called: the region is behind a CUDA IPC handle (no resize)
     PeerExchange px{};
     DevBuf<unsigned long long> cursors;     // [kParities][kMaxWorld] records appended per owner (local)
     DevBuf<uint32_t> rev;                   // [kParities][world][X] inbox position -> entry
@@ -598,6 +601,11 @@ int on_group(ctmr_group* g, Body body, Args... args) {
     const int rc = body(g->m.data(), (uint32_t)g->m.size(), &g->next_index, &failed, args...);
     return rc ? group_fail(g, failed ? failed : g->m[0], rc) : rc;
 }
+// the sections of a shared region for these capacities: the tables come last, so every section before SharedLayout::meta
+// depends on max_issuers alone (ctmr_resize copies that prefix byte for byte)
+SharedLayout make_layout(uint64_t table_slots, uint64_t pair_slots, uint64_t meta_slots, uint32_t max_issuers);
+// st.table, pairs, meta, issuer_counts and status_counts -> their sections of c->shared under c->lay
+void point_at_region(ctmr_ctx* c);
 // views of the shared regions `bases[0..world)` (this rank's own among them) -> st.peer, pf, reg
 void attach_views(ctmr_ctx* c, uint8_t* const* bases, uint32_t world, uint32_t rank);
 int peer_barrier(ctmr_ctx* c, uint32_t channel, cudaStream_t s);   // PEER_IPC only; no-op otherwise

@@ -240,6 +240,14 @@ cudaError_t launch_ckpt_pairs(const DeviceState& st, const PairSlot* rec, uint64
 cudaError_t launch_ckpt_meta(const DeviceState& st, const MetaSlot* rec, uint64_t n, cudaStream_t s);
 cudaError_t launch_cardinality(const DeviceState& st, int32_t exp_hour, uint32_t issuer, unsigned long long* out,
                                cudaStream_t s);
+// ctmr_resize: one pass over an old table of n_old slots, each slot ready at `epoch` inserted into the tables of `to` (its
+// masks, epoch and error flag) with the batch path's inserts.  KnownSlot: the keys also rebuild to.issuer_counts, which
+// must hold zero before.  A table too small raises the table's *_TABLE_FULL in to.error_flag.
+template <class Slot>
+cudaError_t launch_rehash(const Slot* old, uint64_t n_old, uint32_t epoch, const DeviceState& to, int sm_count, cudaStream_t s);
+// *out += the slots of table[0..n) ready at `epoch`
+template <class Slot>
+cudaError_t launch_live_count(const Slot* table, uint64_t n, uint32_t epoch, unsigned long long* out, int sm_count, cudaStream_t s);
 
 // ---- CT wire-format front end (ctmr_frontend.cu, include/ctmr_frontend.h) ------------------------
 #define CTMR_ISSUER_UNRESOLVED 0xFFFFFFFDu  // internal: Chain[0] present, dense index not looked up yet

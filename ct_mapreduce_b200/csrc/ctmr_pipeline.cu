@@ -453,6 +453,7 @@ int ctmr_peer_export(ctmr_ctx* c, uint32_t world, uint8_t handle_out[CTMR_PEER_H
     h.epoch = c->st.epoch;
     std::memset(handle_out, 0, CTMR_PEER_HANDLE_BYTES);
     std::memcpy(handle_out, &h, sizeof h);
+    c->ipc_exported = true;
     return CTMR_OK;
 }
 

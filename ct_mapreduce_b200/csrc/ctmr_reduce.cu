@@ -1,6 +1,9 @@
 // ctmr_reduce.cu -- the reduce half: known-certificate table insert / resolve, (issuer, hour) first-seen,
 // IssuerMetadata string identities, issuer preparation, set cardinality, the owner / source passes of the multi-GPU key
-// exchange, the issuer registry, the cross-process barrier and the histogram merge.
+// exchange, the issuer registry, the cross-process barrier and the histogram merge, and the rehash of ctmr_resize.
+#include <algorithm>
+#include <type_traits>
+
 #include "ctmr_common.cuh"
 
 namespace ctmr {
@@ -584,6 +587,92 @@ cudaError_t launch_table_count(const DeviceState& st, unsigned long long* out, i
     table_count_kernel<<<sm_count * 8, 256, 0, s>>>(st, out);
     return cudaGetLastError();
 }
+
+// ---- resize (ctmr_resize): the slots ready at the current epoch into tables of another size ----------------------------
+// One slot in 16-byte streaming loads: the old table is read once and never again.
+template <class Slot>
+__device__ __forceinline__ Slot ld_slot_once(const Slot* p) {
+    static_assert(sizeof(Slot) % 16 == 0, "slots are whole 16-byte vectors");
+    union {
+        uint4 v[sizeof(Slot) / 16];
+        Slot s;
+    } u;
+#pragma unroll
+    for (int k = 0; k < (int)(sizeof(Slot) / 16); ++k) u.v[k] = __ldcs(reinterpret_cast<const uint4*>(p) + k);
+    return u.s;
+}
+
+// A record into the new tables with the insert of the batch path; returns the issuer whose histogram entry the record
+// adds to (a known key that went in), else 0xFFFFFFFF.  A pair keeps its first-seen index and its count (an evicted set's
+// 0 included); a string identity its first-seen index.  Every record is unique in its table, so the claimer of a slot is
+// the only writer of its count.
+__device__ __forceinline__ uint32_t rehash_one(const DeviceState& to, const KnownSlot& sl) {
+    uint32_t body[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) body[k] = sl.body[k];
+    return known_insert<false>(to.table, to.table_mask, to.epoch, to.error_flag, body, sl.inv_first) != 0xFFFFFFFFu ? sl.body[1] : 0xFFFFFFFFu;
+}
+__device__ __forceinline__ uint32_t rehash_one(const DeviceState& to, const PairSlot& p) {
+    const uint32_t ps = pair_insert<false>(to.pairs, to.pair_mask, to.epoch, to.error_flag, p.key, p.inv_first);
+    if (ps != 0xFFFFFFFFu) to.pairs[ps].count = p.count;
+    return 0xFFFFFFFFu;
+}
+__device__ __forceinline__ uint32_t rehash_one(const DeviceState& to, const MetaSlot& m) {
+    meta_insert_at<false>(to.meta, to.meta_mask, to.epoch, to.error_flag, m.h1, m.h2, m.inv_first);
+    return 0xFFFFFFFFu;
+}
+
+// Grid-stride over the old table in warp-wide steps (every lane of a warp takes part in each step's histogram vote).  The
+// known keys rebuild to.issuer_counts, one atomic per distinct issuer of a warp's step, as a checkpoint load rebuilds it.
+template <class Slot>
+__global__ void __launch_bounds__(256) rehash_kernel(const Slot* __restrict__ old, uint64_t n_old, uint32_t epoch, DeviceState to) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n_old; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t issuer = 0xFFFFFFFFu;
+        if (i < n_old) {
+            const Slot sl = ld_slot_once(old + i);
+            if (slot_state(state_word(sl), epoch) == kSlotReady) issuer = rehash_one(to, sl);
+        }
+        if constexpr (std::is_same<Slot, KnownSlot>::value) {
+            const bool counted = issuer < to.max_issuers;
+            const uint32_t mask = __ballot_sync(0xffffffffu, counted);
+            if (counted) {
+                const uint32_t peers = __match_any_sync(mask, issuer);
+                if (lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(to.issuer_counts + issuer, (unsigned long long)__popc(peers));
+            }
+        }
+    }
+}
+
+template <class Slot>
+__global__ void __launch_bounds__(256) live_count_kernel(const Slot* __restrict__ table, uint64_t n, uint32_t epoch, unsigned long long* out) {
+    unsigned int local = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+        local += slot_state(state_word(table[i]), epoch) == kSlotReady;
+    local = __reduce_add_sync(0xffffffffu, local);
+    if ((threadIdx.x & 31) == 0 && local) atomicAdd(out, (unsigned long long)local);
+}
+
+template <class Slot>
+cudaError_t launch_rehash(const Slot* old, uint64_t n_old, uint32_t epoch, const DeviceState& to, int sm_count, cudaStream_t s) {
+    const uint64_t blocks = std::min<uint64_t>((n_old + 255) / 256, (uint64_t)sm_count * 8);
+    if (blocks) rehash_kernel<Slot><<<(unsigned)blocks, 256, 0, s>>>(old, n_old, epoch, to);
+    return cudaGetLastError();
+}
+template <class Slot>
+cudaError_t launch_live_count(const Slot* table, uint64_t n, uint32_t epoch, unsigned long long* out, int sm_count, cudaStream_t s) {
+    const uint64_t blocks = std::min<uint64_t>((n + 255) / 256, (uint64_t)sm_count * 8);
+    if (blocks) live_count_kernel<Slot><<<(unsigned)blocks, 256, 0, s>>>(table, n, epoch, out);
+    return cudaGetLastError();
+}
+template cudaError_t launch_rehash<KnownSlot>(const KnownSlot*, uint64_t, uint32_t, const DeviceState&, int, cudaStream_t);
+template cudaError_t launch_rehash<PairSlot>(const PairSlot*, uint64_t, uint32_t, const DeviceState&, int, cudaStream_t);
+template cudaError_t launch_rehash<MetaSlot>(const MetaSlot*, uint64_t, uint32_t, const DeviceState&, int, cudaStream_t);
+template cudaError_t launch_live_count<KnownSlot>(const KnownSlot*, uint64_t, uint32_t, unsigned long long*, int, cudaStream_t);
+template cudaError_t launch_live_count<PairSlot>(const PairSlot*, uint64_t, uint32_t, unsigned long long*, int, cudaStream_t);
+template cudaError_t launch_live_count<MetaSlot>(const MetaSlot*, uint64_t, uint32_t, unsigned long long*, int, cudaStream_t);
 
 cudaError_t launch_cardinality(const DeviceState& st, int32_t hour, uint32_t issuer, unsigned long long* out,
                                cudaStream_t s) {

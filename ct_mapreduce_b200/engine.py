@@ -882,6 +882,22 @@ class GpuCertDatabase:
         self._check(self._c("table_stats")(self._h, C.byref(used), C.byref(cap)))
         return used.value, cap.value
 
+    def resize(self, table_capacity: int | None = None, pair_capacity_log2: int | None = None,
+               meta_capacity_log2: int | None = None):
+        """The known-certificate, (issuer, expDate) and string-identity tables in other sizes, rehashed on the device
+        (ctmr_resize): afterwards every call answers as a db created with these capacities and loaded from a checkpoint
+        taken just before; the registry, the chain certificates and the fingerprints stay.  None keeps a table's size.
+        All or nothing: on failure (E_NOMEM, a *_TABLE_FULL for a target too small) the db is unchanged.  Not on a db
+        exported to peers (E_INVALID on every rank, without a collective call)."""
+        self._check(self._c("resize")(self._h, int(table_capacity or 0), int(pair_capacity_log2 or 0), int(meta_capacity_log2 or 0)))
+
+    def table_occupancy(self):
+        """((used known, pair, meta), (capacity known, pair, meta)): live slots and slots of the three tables
+        (ctmr_table_occupancy; a group's are sums over its shards)."""
+        used, cap = (C.c_uint64 * 3)(), (C.c_uint64 * 3)()
+        self._check(self._c("table_occupancy")(self._h, used, cap))
+        return tuple(int(v) for v in used), tuple(int(v) for v in cap)
+
 
 class GpuCertGroup(GpuCertDatabase):
     """Several GPUs of one box behind ONE handle (ctmr_group_*): what the Go host calls in place of the worker pool of

@@ -513,6 +513,34 @@ func (d *DB) LoadCheckpoint(parts ...[]byte) error {
 	return d.err(C.ctmr_checkpoint_load(d.h, &ptrs[0], &sizes[0], C.uint32_t(n)), "ctmr_checkpoint_load")
 }
 
+// Resize rehashes the known-certificate, (issuer, expDate) and string-identity tables into the given sizes on the
+// device (ctmr_resize / ctmr_group_resize); 0 keeps a table's size.  Afterwards the DB answers as one created with these
+// capacities and loaded from a checkpoint taken just before, with its registered chain certificates kept.  All or
+// nothing: on failure (CTMR_E_NOMEM, a *_TABLE_FULL for a target too small) the DB is unchanged.  A DB exported to peers
+// is refused; resize it before PeerExport, or move the state through Checkpoint / LoadCheckpoint.
+func (d *DB) Resize(tableCapacity uint64, pairLog2, metaLog2 uint32) error {
+	if d.g != nil {
+		return d.err(C.ctmr_group_resize(d.g, C.uint64_t(tableCapacity), C.uint32_t(pairLog2), C.uint32_t(metaLog2)), "ctmr_group_resize")
+	}
+	return d.err(C.ctmr_resize(d.h, C.uint64_t(tableCapacity), C.uint32_t(pairLog2), C.uint32_t(metaLog2)), "ctmr_resize")
+}
+
+// TableOccupancy returns the live slots and the slots of the known-certificate, (issuer, expDate) and string-identity
+// tables, in that order (a group: sums over its shards).  Watch it to resize before a batch fails with *_TABLE_FULL.
+func (d *DB) TableOccupancy() (used, capacity [3]uint64, err error) {
+	var u, c [3]C.uint64_t
+	var rc C.int
+	if d.g != nil {
+		rc = C.ctmr_group_table_occupancy(d.g, &u[0], &c[0])
+	} else {
+		rc = C.ctmr_table_occupancy(d.h, &u[0], &c[0])
+	}
+	for k := range u {
+		used[k], capacity[k] = uint64(u[k]), uint64(c[k])
+	}
+	return used, capacity, d.err(rc, "ctmr_table_occupancy")
+}
+
 func HostAlloc(n int) unsafe.Pointer { return C.ctmr_host_alloc(C.size_t(n)) }
 func HostFree(p unsafe.Pointer)      { C.ctmr_host_free(p) }
 

@@ -226,6 +226,47 @@ int ctmr_checkpoint_size(ctmr_ctx* ctx, uint64_t* bytes);
 int ctmr_checkpoint_save(ctmr_ctx* ctx, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_checkpoint_load(ctmr_ctx* ctx, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
 
+/* ---- resize ------------------------------------------------------------------------------------------------------- */
+/* The known-certificate, (issuer, expDate) and string-identity tables in other sizes, rehashed on the device: what
+ * checkpoint save, destroy, create, checkpoint load and registering the chain certificates again would do, without
+ * leaving the GPU.  0 keeps a table's current size; table_capacity is rounded up to a power of two as in ctmr_create.
+ *
+ * Equivalence.  After ctmr_resize(ctx, T, P, M) returns CTMR_OK, every later call returns exactly what it would return on
+ * a ctx created with capacities (T, P, M) and the same other config, loaded with ctmr_checkpoint_load from a
+ * ctmr_checkpoint_save taken just before the resize: every ctmr_out field, the front-end calls, ctmr_issuer_counts,
+ * ctmr_set_cardinality, ctmr_status_counters, ctmr_next_index, ctmr_revoked_known, the cascade and the stash.  Checkpoint
+ * records (parsed and sorted) are equal; slot order, and so the checkpoint bytes, may differ.
+ * Kept state.  Everything else stays as it was: the issuer registry (same dense indices), the registered chain
+ * certificates, the Chain[0] mirror, the tiles' fingerprint table and the staging buffers.  Unlike the checkpoint route,
+ * nothing is registered again.
+ * Records.  A resize carries what a checkpoint carries: the ready known-certificate slots of the current epoch with their
+ * first-seen index, every occupied (issuer, expDate) slot (an evicted set's, count 0, included) and every occupied
+ * string-identity slot.  Slots left by earlier epochs (ctmr_reset_device) are empty and are not carried.  The per-issuer
+ * counts are rebuilt from the keys, as a checkpoint load rebuilds them.
+ * Shrinking is allowed.  A target too small for its records fails with the table's own CTMR_E_TABLE_FULL,
+ * CTMR_E_PAIR_TABLE_FULL or CTMR_E_META_TABLE_FULL.
+ * All or nothing.  On any failure (CTMR_E_NOMEM for the new tables, a *_TABLE_FULL, a CUDA error) the ctx or every member
+ * of the group is left exactly as it was: the same tables, a checkpoint byte-equal to the one before, usable; the rehash
+ * raises no flag that ctmr_check_device would report later.
+ * Peak memory.  The old and the new tables exist together; a group builds every member's new tables before it frees any
+ * old ones, so the peak on a device is old plus new for every member on it.  A shape that does not fit is CTMR_E_NOMEM
+ * with nothing changed: move the state through ctmr_checkpoint_save / ctmr_checkpoint_load instead, which holds it in
+ * host memory between the two tables.
+ * Refusals (CTMR_E_INVALID, nothing touched): a NULL ctx; a member ctx of a group (use ctmr_group_resize); table_capacity
+ * above 2^32 - 16 slots once rounded, pair_capacity_log2 above 32, meta_capacity_log2 above 26 (ctmr_create's limits);
+ * a ctx on which ctmr_peer_export was called.  Its whole shared region, tables included, is behind a CUDA IPC handle whose
+ * size the other ranks check at ctmr_peer_attach, and the table size must be the same on every rank: a rank resizes
+ * before it exports, and ranks attached to each other resize through the checkpoint route.  The refusal comes before any
+ * barrier, so no rank waits for it.
+ * Not collective and not automatic: a full table still fails its batch with *_TABLE_FULL.  Watch ctmr_table_occupancy and
+ * resize, or resize after a *_TABLE_FULL and replay the batch (safe by ctmr_process_batch's replay rule).
+ * Cost: one pass over each old table and one scattered insert per record (DESIGN.md §3 "Resize"). */
+int ctmr_resize(ctmr_ctx* ctx, uint64_t table_capacity, uint32_t pair_capacity_log2, uint32_t meta_capacity_log2);
+/* used (live slots of the current epoch) and capacity (slots) of the three tables, in the order known-certificate,
+ * (issuer, expDate), string identities; either array may be NULL.  One count pass per table.  A member ctx of a group
+ * reports its own shard; ctmr_group_table_occupancy sums over the members. */
+int ctmr_table_occupancy(ctmr_ctx* ctx, uint64_t used[3], uint64_t capacity[3]);
+
 /* ---- revoked known certificates (CRLite's join of CRLs with the serials:: sets) ------------------- */
 /* Which revoked serials of an issuer's CRLs are known certificates, and in which "serials::<expDate>::<issuer>" set
  * (storage/knowncertificates.go:28-55)?  A CRL entry carries no expiry, so the set cannot be named; the call parses the
@@ -550,6 +591,10 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
 int ctmr_group_checkpoint_size(ctmr_group* g, uint64_t* bytes);
 int ctmr_group_checkpoint_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_group_checkpoint_load(ctmr_group* g, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
+/* ctmr_resize of every shard, all or nothing: each member's tables get the given size (0 keeps it), every member's new
+ * tables are built and rehashed before any old ones go, and a failure of one member leaves every member unchanged */
+int ctmr_group_resize(ctmr_group* g, uint64_t table_capacity, uint32_t pair_capacity_log2, uint32_t meta_capacity_log2);
+int ctmr_group_table_occupancy(ctmr_group* g, uint64_t used[3], uint64_t capacity[3]);   /* summed over the shards */
 /* ctmr_revoked_known over every shard: member 0 parses the CRLs and builds the set of (issuer, serial) pairs, each member
  * scans its own table against a bulk copy of it, and member 0 merges the answers (lowest hour, sum of sets). */
 int ctmr_group_revoked_known(ctmr_group* g, const ctmr_crl_batch* batch, ctmr_crl_out* out);

@@ -128,23 +128,36 @@ template <bool SYS>
 __device__ __forceinline__ uint4 ld_slot_u4(const uint4* p) { return SYS ? __ldcv(p) : __ldcg(p); }
 __device__ __forceinline__ uint4 ld_cv_u4(const uint4* p) { return __ldcv(p); }
 
+// The probe rule of the three tables (known-certificate, (issuer, hour) pair, string identity), all open addressing with
+// linear probing (DESIGN.md §3 "Probe rule"):
+//   finding  a find-or-insert or a lookup walks from the home slot until it meets its key or a slot empty at the current
+//            epoch.  Its only bound is the table size, so it finds every record the table holds, however far from home.
+//   placing  a NEW record of the batch path or of a preload goes at most kProbeLimit slots past its home slot; the empty
+//            slot the walk ended at lies further, or there is none: the table's *_TABLE_FULL.
+//   again    a record the state already holds, placed again (eviction's reinsert, the resize rehash, a checkpoint load),
+//            may go anywhere in the table (limit = the table's mask): the order of those inserts decides how far each
+//            record lands, so no survivor is lost to a limit and a state always fits tables of its own size.
+constexpr uint64_t kProbeLimit = 4096;
+
 // Find-or-insert of a 48-byte key body; lowest global index wins through an atomic max on ~index.  A slot empty at
 // `epoch` (zero, or left by an earlier epoch) is claimed by a CAS from the tag observed to pending; the claimer writes
 // the key bytes and inv_first, then publishes them by a release store of the ready tag (a slot of an earlier epoch may
 // hold a larger ~index, so inv_first is stored, not max'ed, and before the release).  Equal keys act only once they see
-// ready.  Returns the slot, or 0xFFFFFFFF when the table is full (error flag set).  Shared by K_insert and by K_map's
+// ready.  `limit`: how far past its home a new key may be placed (kProbeLimit, or the table's mask for a key placed
+// again).  Returns the slot, or 0xFFFFFFFF when the table is full (error flag set).  Shared by K_insert and by K_map's
 // fused insert; SYS = system scope (only the string-identity table is touched across GPUs).
 template <bool SYS>
 __device__ __forceinline__ uint32_t known_insert(KnownSlot* __restrict__ table, uint64_t table_mask, uint32_t epoch, int* error_flag,
-                                                 const uint32_t (&body)[12], unsigned long long inv_idx) {
+                                                 const uint32_t (&body)[12], unsigned long long inv_idx, uint64_t limit = kProbeLimit) {
     const uint64_t h = key_hash(body);
     const unsigned long long tag_ready = slot_word(epoch, kSlotReady, h), tag_pending = slot_word(epoch, kSlotPending, h);
     uint64_t pos = (h >> 7) & table_mask;
-    uint32_t probes = 0;
+    uint64_t probes = 0;  // distance of pos from the home slot
     for (;;) {
         KnownSlot* sl = table + pos;
         unsigned long long t = ld_volatile_u64(&sl->tag);  // relaxed: an acquire here would invalidate the SM's L1 per probe
         if (slot_state(t, epoch) == 0u) {
+            if (probes > limit) break;  // the key is not in the table, and its place would lie past the limit
             const unsigned long long seen = t;
             t = tab_cas<SYS>(&sl->tag, seen, tag_pending);
             if (t != seen) continue;  // another thread claimed the slot first: look at it again
@@ -172,11 +185,10 @@ __device__ __forceinline__ uint32_t known_insert(KnownSlot* __restrict__ table, 
             }
         }
         pos = (pos + 1) & table_mask;
-        if (++probes > 4096u) {  // table effectively full
-            atomicExch(error_flag, CTMR_E_TABLE_FULL);
-            return 0xFFFFFFFFu;
-        }
+        if (++probes > table_mask) break;  // every slot holds another key
     }
+    atomicExch(error_flag, CTMR_E_TABLE_FULL);
+    return 0xFFFFFFFFu;
 }
 
 // a CRL join's (issuer, serial) pair exactly as words 1..11 of a KnownSlot body: issuer, then {serial_len, serial[39]}

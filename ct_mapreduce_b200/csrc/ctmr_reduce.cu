@@ -36,14 +36,15 @@ __global__ void __launch_bounds__(256) insert_kernel(DeviceState st, const ctmr_
 // Find-or-insert of an (issuer, hour) key.  The pad word carries the slot's epoch and state (ctmr_common.cuh): the same key
 // recurs after every reset, so a key word left by an earlier epoch cannot tell whether the slot is live.  The claimer
 // writes key, inv_first and count = 0 while the slot is pending; equal keys act (max, add) only once they see it ready.
+// `limit` and the probe rule as for known_insert (ctmr_common.cuh).
 template <bool SYS>
 __device__ __forceinline__ uint32_t pair_insert(PairSlot* __restrict__ pairs, uint64_t pair_mask, uint32_t epoch, int* error_flag,
-                                                unsigned long long pk, unsigned long long inv_idx) {
+                                                unsigned long long pk, unsigned long long inv_idx, uint64_t limit = kProbeLimit) {
     uint64_t pos = mix64(pk) & pair_mask;
-    for (uint32_t probes = 0;; ++probes) {
+    for (uint64_t probes = 0; probes <= pair_mask; ++probes) {
         PairSlot* sl = pairs + pos;
         unsigned long long w = ld_volatile_u64(&sl->pad);
-        while (slot_state(w, epoch) == 0u) {
+        while (slot_state(w, epoch) == 0u && probes <= limit) {
             const unsigned long long seen = w;
             w = tab_cas<SYS>(&sl->pad, seen, slot_word(epoch, kSlotPending));
             if (w != seen) continue;  // another thread claimed the slot first
@@ -53,6 +54,7 @@ __device__ __forceinline__ uint32_t pair_insert(PairSlot* __restrict__ pairs, ui
             tab_store_release<SYS>(&sl->pad, slot_word(epoch, kSlotReady));
             return (uint32_t)pos;
         }
+        if (slot_state(w, epoch) == 0u) break;  // the key is not in the table, and its place would lie past the limit
         // the key is read only after an acquire of the ready word (a relaxed read of ready does not order it, and the slot
         // may hold the same key from the last epoch); pending: another thread is publishing the slot
         do w = tab_load_acquire<SYS>(&sl->pad);
@@ -62,11 +64,9 @@ __device__ __forceinline__ uint32_t pair_insert(PairSlot* __restrict__ pairs, ui
             return (uint32_t)pos;
         }
         pos = (pos + 1) & pair_mask;
-        if (probes > 4096u) {
-            atomicExch(error_flag, CTMR_E_PAIR_TABLE_FULL);
-            return 0xFFFFFFFFu;
-        }
     }
+    atomicExch(error_flag, CTMR_E_PAIR_TABLE_FULL);
+    return 0xFFFFFFFFu;
 }
 
 // `in` lanes hold record j; every lane of the warp takes part in the aggregation
@@ -208,15 +208,15 @@ __device__ __forceinline__ uint32_t meta_owner(uint64_t h1, uint32_t world) { re
 
 // The pad word carries the slot's epoch and state, as in pair_insert: the claimer writes h1, h2 and inv_first while the
 // slot is pending.  A cross-GPU insert (SYS) stamps the inserting rank's epoch, which is the owner's: every reset is
-// collective (ctmr_reset_device).
+// collective (ctmr_reset_device).  `limit` and the probe rule as for known_insert (ctmr_common.cuh).
 template <bool SYS>
 __device__ inline uint32_t meta_insert_at(MetaSlot* __restrict__ meta, uint64_t meta_mask, uint32_t epoch, int* error_flag, uint64_t h1,
-                                          uint64_t h2, unsigned long long inv_idx) {
+                                          uint64_t h2, unsigned long long inv_idx, uint64_t limit = kProbeLimit) {
     uint64_t pos = (h1 >> 5) & meta_mask;
-    for (uint32_t probes = 0; probes < 4096u; ++probes) {
+    for (uint64_t probes = 0; probes <= meta_mask; ++probes) {
         MetaSlot* sl = meta + pos;
         unsigned long long w = ld_volatile_u64(&sl->pad);
-        while (slot_state(w, epoch) == 0u) {
+        while (slot_state(w, epoch) == 0u && probes <= limit) {
             const unsigned long long seen = w;
             w = tab_cas<SYS>(&sl->pad, seen, slot_word(epoch, kSlotPending));
             if (w != seen) continue;  // another thread claimed the slot first
@@ -226,6 +226,7 @@ __device__ inline uint32_t meta_insert_at(MetaSlot* __restrict__ meta, uint64_t 
             tab_store_release<SYS>(&sl->pad, slot_word(epoch, kSlotReady));
             return (uint32_t)pos;
         }
+        if (slot_state(w, epoch) == 0u) break;  // the identity is not in the table, and its place would lie past the limit
         // the key is read only after an acquire of the ready word (a relaxed read of ready does not order it, and the slot
         // may hold the same key from the last epoch); pending: another thread is publishing the slot
         do w = tab_load_acquire<SYS>(&sl->pad);
@@ -394,7 +395,7 @@ __global__ void cardinality_kernel(DeviceState st, int32_t hour, uint32_t issuer
     const PairSlot* pairs = st.peer.pairs[st.peer.world > 1u ? key_owner(hour, issuer, st.peer.world) : 0u];
     uint64_t pos = mix64(pk) & st.pair_mask;
     unsigned long long v = 0;
-    for (uint32_t probes = 0; probes <= 4096u; ++probes) {
+    for (uint64_t probes = 0; probes <= st.pair_mask; ++probes) {  // to the key or an empty slot (the probe rule, ctmr_common.cuh)
         if (slot_state(ld_volatile_u64(&pairs[pos].pad), st.epoch) == 0u) break;
         if (ld_volatile_u64(&pairs[pos].key) == pk) {
             v = ld_volatile_u64(&pairs[pos].count);
@@ -477,8 +478,10 @@ __global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restri
 }
 
 // pass 3 (after the table has been cleared), and a checkpoint's records on their way in: linear probing leaves no holes
-// only if every record is inserted again.  The records are canonical (no epoch): a ready one has state 2 in its tag.  A record whose owner under this rank's world is another rank is skipped
-// (eviction: a rank only ever holds keys it owns).  Every index a record carries is checked before it is used: an
+// only if every record is inserted again.  Records placed again, bounded by the table size alone (the probe rule,
+// ctmr_common.cuh): this order may place a survivor further from home than the batch path did.  The records are
+// canonical (no epoch): a ready one has state 2 in its tag.  A record whose owner under this rank's world is another rank
+// is skipped (eviction: a rank only ever holds keys it owns).  Every index a record carries is checked before it is used: an
 // issuer >= n_issuers, a serial longer than CTMR_MAX_SERIAL or a slot that is not ready raises CTMR_E_INVALID.  count:
 // the inserted keys go into the per-issuer histogram (a checkpoint carries no histogram).
 __global__ void __launch_bounds__(256) evict_reinsert_kernel(DeviceState st, const KnownSlot* __restrict__ keep, uint64_t n,
@@ -494,7 +497,7 @@ __global__ void __launch_bounds__(256) evict_reinsert_kernel(DeviceState st, con
     uint32_t body[12];
 #pragma unroll
     for (int k = 0; k < 12; ++k) body[k] = sl.body[k];
-    if (known_insert<false>(st.table, st.table_mask, st.epoch, st.error_flag, body, sl.inv_first) != 0xFFFFFFFFu && count)
+    if (known_insert<false>(st.table, st.table_mask, st.epoch, st.error_flag, body, sl.inv_first, st.table_mask) != 0xFFFFFFFFu && count)
         atomicAdd(st.issuer_counts + sl.body[1], 1ull);
 }
 
@@ -510,7 +513,7 @@ __global__ void __launch_bounds__(256) ckpt_pairs_kernel(DeviceState st, const P
     const uint32_t issuer = (uint32_t)((p.key - 1ull) >> 32);
     const int32_t hour = (int32_t)(uint32_t)(p.key - 1ull);
     if (st.peer.world > 1u && key_owner(hour, issuer, st.peer.world) != st.peer.rank) return;
-    const uint32_t ps = pair_insert<false>(st.pairs, st.pair_mask, st.epoch, st.error_flag, p.key, p.inv_first);
+    const uint32_t ps = pair_insert<false>(st.pairs, st.pair_mask, st.epoch, st.error_flag, p.key, p.inv_first, st.pair_mask);
     if (ps != 0xFFFFFFFFu && p.count) tab_add<false>(&st.pairs[ps].count, p.count);
 }
 
@@ -524,7 +527,7 @@ __global__ void __launch_bounds__(256) ckpt_meta_kernel(DeviceState st, const Me
         return;
     }
     if (meta_owner(m.h1, st.peer.world) != (st.peer.world > 1u ? st.peer.rank : 0u)) return;
-    meta_insert_at<false>(st.meta, st.meta_mask, st.epoch, st.error_flag, m.h1, m.h2, m.inv_first);
+    meta_insert_at<false>(st.meta, st.meta_mask, st.epoch, st.error_flag, m.h1, m.h2, m.inv_first, st.meta_mask);
 }
 
 cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters, int sm_count, cudaStream_t s) {
@@ -602,7 +605,8 @@ __device__ __forceinline__ Slot ld_slot_once(const Slot* p) {
     return u.s;
 }
 
-// A record into the new tables with the insert of the batch path; returns the issuer whose histogram entry the record
+// A record into the new tables with the insert of the batch path, bounded by the new table's size alone (a record placed
+// again, ctmr_common.cuh); returns the issuer whose histogram entry the record
 // adds to (a known key that went in), else 0xFFFFFFFF.  A pair keeps its first-seen index and its count (an evicted set's
 // 0 included); a string identity its first-seen index.  Every record is unique in its table, so the claimer of a slot is
 // the only writer of its count.
@@ -610,15 +614,16 @@ __device__ __forceinline__ uint32_t rehash_one(const DeviceState& to, const Know
     uint32_t body[12];
 #pragma unroll
     for (int k = 0; k < 12; ++k) body[k] = sl.body[k];
-    return known_insert<false>(to.table, to.table_mask, to.epoch, to.error_flag, body, sl.inv_first) != 0xFFFFFFFFu ? sl.body[1] : 0xFFFFFFFFu;
+    return known_insert<false>(to.table, to.table_mask, to.epoch, to.error_flag, body, sl.inv_first, to.table_mask) != 0xFFFFFFFFu ? sl.body[1]
+                                                                                                                      : 0xFFFFFFFFu;
 }
 __device__ __forceinline__ uint32_t rehash_one(const DeviceState& to, const PairSlot& p) {
-    const uint32_t ps = pair_insert<false>(to.pairs, to.pair_mask, to.epoch, to.error_flag, p.key, p.inv_first);
+    const uint32_t ps = pair_insert<false>(to.pairs, to.pair_mask, to.epoch, to.error_flag, p.key, p.inv_first, to.pair_mask);
     if (ps != 0xFFFFFFFFu) to.pairs[ps].count = p.count;
     return 0xFFFFFFFFu;
 }
 __device__ __forceinline__ uint32_t rehash_one(const DeviceState& to, const MetaSlot& m) {
-    meta_insert_at<false>(to.meta, to.meta_mask, to.epoch, to.error_flag, m.h1, m.h2, m.inv_first);
+    meta_insert_at<false>(to.meta, to.meta_mask, to.epoch, to.error_flag, m.h1, m.h2, m.inv_first, to.meta_mask);
     return 0xFFFFFFFFu;
 }
 

@@ -47,6 +47,10 @@ enum {
     CTMR_E_INVALID = -1,          /* bad argument */
     CTMR_E_CUDA = -2,             /* CUDA runtime error (text in ctmr_last_error) */
     CTMR_E_NOMEM = -3,            /* host or device allocation failed */
+    /* The *_TABLE_FULL codes.  The batch path and preloads place a new record at most 4096 slots (kProbeLimit) past its
+     * home slot, and fail with the table's code when the nearest free slot lies further.  Finding a record the table
+     * holds has no such limit, and eviction, ctmr_resize and checkpoint loads place records again anywhere in the
+     * table: they fail only when it has no free slot (DESIGN.md §3 "Probe rule"). */
     CTMR_E_TABLE_FULL = -4,       /* known-certificate table exhausted (cf. Redis OOM, rediscache.go:61-63) */
     CTMR_E_TOO_MANY_ISSUERS = -5, /* more distinct issuers than config.max_issuers */
     CTMR_E_NO_DEVICE = -6,        /* no usable CUDA device: the product path has no CPU fallback */

@@ -9,6 +9,7 @@ Mirrors, and must change with:
                     (issuer, hour)), evict_pairs_kernel (an expired set's count is 0 again, its first-seen index stays)
   ctmr_map.cu       the key body: (u32)(i32)exp_hour, dense issuer, then {serial_len, serial[39]} packed little-endian
   ctmr_api.cu       SnapHeader (8-byte magic + six u64) followed by the table, then the pair table
+The probe rule the chains follow (how far a record may lie past its home) is tests/probe_model.py's.
 """
 from __future__ import annotations
 
@@ -120,9 +121,14 @@ def decode_snapshot(snap: np.ndarray):
     return table, pairs
 
 
-def check_table(snap, model: KeyModel, used: int | None = None, owner=None):
+def check_table(snap, model: KeyModel, used: int | None = None, owner=None, limit="probe"):
     """Every ready slot against the model; returns the number of slots checked.  `snap` is a ctx snapshot or one shard's
-    decoded (table, pairs); owner = (key_owner, world, rank): every key and pair must be one the shard owns."""
+    decoded (table, pairs); owner = (key_owner, world, rank): every key and pair must be one the shard owns.  Every key
+    and pair lies on an unbroken chain from its home slot, at most `limit` slots past it: by default the probe limit of
+    the batch path (probe_model.PROBE_LIMIT); None for a state whose records were placed again (eviction, resize,
+    checkpoint load), which the table size alone bounds."""
+    import probe_model as P
+    limit = P.PROBE_LIMIT if limit == "probe" else limit
     table, pairs = snap if isinstance(snap, tuple) else decode_snapshot(snap)
     mask = table.size - 1
     tags = table["tag"]
@@ -130,6 +136,7 @@ def check_table(snap, model: KeyModel, used: int | None = None, owner=None):
     assert not ((tags != 0) & ~ready).any(), "a slot was left pending"
     occupied = tags != 0
     seen = set()
+    homes = []
     for pos in np.nonzero(ready)[0]:
         body = tuple(int(x) for x in table["body"][pos])
         h = key_hash(body)
@@ -140,11 +147,9 @@ def check_table(snap, model: KeyModel, used: int | None = None, owner=None):
         assert body not in seen, ("key stored twice", body)
         seen.add(body)
         assert (~int(table["inv_first"][pos])) & M64 == model.first[body], ("first index", pos)
-        home = home_slot(h, mask)
-        s = home
-        while s != pos:  # the probe chain from the home slot has no hole (linear probing, wraps past the last slot)
-            assert occupied[s], ("hole in the probe chain", home, s, pos)
-            s = (s + 1) & mask
+        homes.append(home_slot(h, mask))
+    # the probe chain from the home slot has no hole (linear probing, wraps past the last slot)
+    P.check_chains(np.nonzero(ready)[0], homes, occupied, limit, "key")
     assert len(seen) == len(model.first), ("keys missing from the table", len(model.first) - len(seen))
     if used is not None:
         assert used == len(seen)
@@ -152,6 +157,7 @@ def check_table(snap, model: KeyModel, used: int | None = None, owner=None):
     got = {}
     pmask = pairs.size - 1
     pkeys = pairs["key"]
+    phomes = []
     for pos in np.nonzero(pkeys != 0)[0]:
         p = pairs[pos]
         k = int(p["key"]) - 1
@@ -162,11 +168,8 @@ def check_table(snap, model: KeyModel, used: int | None = None, owner=None):
         got[hk] = int(p["count"])
         assert hk in model.pair_first, ("pair slot of a set no new certificate opened", pos, hk)
         assert (~int(p["inv_first"])) & M64 == model.pair_first[hk], ("pair first index", pos, hk)
-        home = int(mix64(int(p["key"])) & pmask)
-        s = home
-        while s != pos:  # no hole between the pair's home slot and its slot
-            assert pkeys[s] != 0, ("hole in the pair probe chain", home, s, pos)
-            s = (s + 1) & pmask
+        phomes.append(int(mix64(int(p["key"])) & pmask))
+    P.check_chains(np.nonzero(pkeys != 0)[0], phomes, pkeys != 0, limit, "pair")  # no hole between home and slot
     for k, v in got.items():
         assert v == want.get(k, 0), ("pair count", k, v, want.get(k, 0))
     assert set(want) <= set(got)

@@ -6,7 +6,8 @@ slot against a model built from the oracle's per-entry outputs.
 Mirrors, and must change with:
   ctmr_reduce.cu    hash_bytes (little-endian 8-byte words, the last one zero padded; h1 = mix64(a ^ len) | 1,
                     h2 = mix64(b + len) | 1), the seed (dense_issuer << 8) | kind (1 issuer Name, 2 cRLDistributionPoints),
-                    meta_insert_at (home slot (h1 >> 5) & mask, linear probing), meta_owner ((h1 >> 40) % world)
+                    meta_insert_at (home slot (h1 >> 5) & mask, linear probing with tests/probe_model.py's rule),
+                    meta_owner ((h1 >> 40) % world)
   ctmr_device.cuh   mix64
   ctmr_kernels.cuh  MetaSlot {h1, h2, inv_first, pad} (32 bytes)
   ctmr_api.cu       SnapHeader ("CTMRSNP3" + six u64), then table, pairs, meta, issuer counts, status counts, digests;
@@ -209,13 +210,17 @@ def decode_group_snapshot(snap: np.ndarray, pair_slots: int, meta_slots: int) ->
     return out
 
 
-def check_meta(meta: np.ndarray, model: MetaModel, world: int = 1, rank: int = 0) -> int:
-    """Every occupied slot of one shard's string-identity table against the model; returns the slots checked."""
+def check_meta(meta: np.ndarray, model: MetaModel, world: int = 1, rank: int = 0, limit="probe") -> int:
+    """Every occupied slot of one shard's string-identity table against the model; returns the slots checked.  Every
+    identity lies on an unbroken chain at most `limit` slots past its home (keymodel.check_table's `limit`)."""
+    import probe_model as P
+    limit = P.PROBE_LIMIT if limit == "probe" else limit
     by_hash = model.hashes()
     mask = meta.size - 1
     h1s, h2s = meta["h1"], meta["h2"]
     occupied = h1s != 0
     seen = set()
+    homes = []
     for pos in np.nonzero(occupied)[0]:
         h1, h2 = int(h1s[pos]), int(h2s[pos])
         assert h2 != 0, ("a slot was left unpublished", pos)
@@ -225,11 +230,9 @@ def check_meta(meta: np.ndarray, model: MetaModel, world: int = 1, rank: int = 0
         assert k not in seen, ("identity stored twice", k)
         seen.add(k)
         assert (~int(meta["inv_first"][pos])) & M64 == model.first[k], ("first index", pos, k[:2])
-        home = home_slot(h1, mask)
-        s = home
-        while s != pos:  # linear probing leaves no hole between the home slot and the slot; wraps past the last slot
-            assert occupied[s], ("hole in the probe chain", home, s, pos)
-            s = (s + 1) & mask
+        homes.append(home_slot(h1, mask))
+    # linear probing leaves no hole between the home slot and the slot; wraps past the last slot
+    P.check_chains(np.nonzero(occupied)[0], homes, occupied, limit, "string identity")
     mine = sum(1 for h in by_hash if meta_owner(h[0], world) == rank)
     assert len(seen) == mine, ("identities missing from the table", mine - len(seen))
     return len(seen)

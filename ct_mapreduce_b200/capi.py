@@ -55,6 +55,7 @@ EXPORTS = [
     "ctmr_revoked_known", "ctmr_group_revoked_known",   # CRLs joined with the known-certificate sets
     "ctmr_revoked_cascade", "ctmr_group_revoked_cascade",   # CRLite's filter cascade of the covered issuers
     "ctmr_revoked_stash", "ctmr_group_revoked_stash",   # CRLite's stash: what a published filter and its stashes miss
+    "ctmr_revoked_verify", "ctmr_group_revoked_verify",   # a published filter and its stashes checked against the table
     "ctmr_resize", "ctmr_group_resize", "ctmr_table_occupancy", "ctmr_group_table_occupancy",   # the tables in other sizes
 ]
 # the calls with a ctmr_group_<name> form beside ctmr_<name>
@@ -63,7 +64,7 @@ GROUP_TWINS = (
     "preload_known", "evict_expired", "snapshot_size", "snapshot_save", "snapshot_load", "checkpoint_size", "checkpoint_save",
     "checkpoint_load", "process_raw", "process_raw_tree", "process_raw_trees", "process_raw_bodies", "process_raw_bodies_tree",
     "process_raw_bodies_trees", "process_tiles", "process_tiles_tree", "process_tiles_trees", "register_chain_certs",
-    "revoked_known", "revoked_cascade", "revoked_stash", "resize", "table_occupancy",
+    "revoked_known", "revoked_cascade", "revoked_stash", "revoked_verify", "resize", "table_occupancy",
 )
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -193,6 +194,26 @@ class StashOut(C.Structure):
                 ("in_stashes", C.c_uint64), ("serials", C.c_uint64)]
 
 
+class VerifyCounts(C.Structure):
+    """ctmr_verify_counts (include/ctmr.h)."""
+    _fields_ = [("revoked", C.c_uint64), ("missed", C.c_uint64), ("valid", C.c_uint64), ("blocked", C.c_uint64)]
+
+
+MAX_SERIAL = 39   # CTMR_MAX_SERIAL
+
+
+class VerifyMiss(C.Structure):
+    """ctmr_verify_miss (include/ctmr.h)."""
+    _fields_ = [("digest", C.c_uint8 * 32), ("exp_hour", C.c_int64), ("first_index", C.c_uint64), ("serial_len", C.c_uint8),
+                ("serial", C.c_uint8 * MAX_SERIAL), ("blocked", C.c_uint8), ("pad", C.c_uint8 * 7)]
+
+
+class VerifyOut(C.Structure):
+    """ctmr_verify_out (include/ctmr.h)."""
+    _fields_ = [("crl_status", C.c_void_p), ("issuers", C.c_uint32), ("levels", C.c_uint32), ("before", VerifyCounts),
+                ("since", VerifyCounts), ("list", C.c_void_p), ("list_cap", C.c_uint64), ("n_list", C.c_uint64)]
+
+
 class SynthCfg(C.Structure):
     """ctmr_synth_cfg (csrc/ctmr_synth.h): the synthetic CT corpus of SURVEY.md §8(d)."""
     _fields_ = [
@@ -304,6 +325,7 @@ def load():
     L.ctmr_revoked_known.argtypes = [vp, C.POINTER(CrlBatch), C.POINTER(CrlOut)]
     L.ctmr_revoked_cascade.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u32, C.POINTER(CascadeOut)]
     L.ctmr_revoked_stash.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u64, vp, u64, C.POINTER(StashOut)]
+    L.ctmr_revoked_verify.argtypes = [vp, C.POINTER(CrlBatch), C.c_int64, vp, u64, vp, u64, u64, C.POINTER(VerifyOut)]
     # a group's form of a call takes the group handle where the ctx form takes the ctx, and otherwise the same arguments
     for name in GROUP_TWINS:
         g, c = getattr(L, "ctmr_group_" + name), getattr(L, "ctmr_" + name)

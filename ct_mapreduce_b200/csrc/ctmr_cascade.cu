@@ -12,9 +12,15 @@
 // The host reads one count per level, sizes the next level and reads each finished level back.
 // ctmr_revoked_stash / ctmr_group_revoked_stash share the work up to the split (cascade_front), then
 //   stash_query      thread per R record: the published filter's query; the records it misses go to the host
+// ctmr_revoked_verify / ctmr_group_revoked_verify share cascade_front too, mark the stashes' set with cascade_mark, then
+//   verify_table     grid-stride over the table, one hash per lane per step: the filter's query of every covered live
+//                    record the stashes do not list; counts, and the slots of the records answered wrongly
+//   verify_gather    thread per listed record: the slot, for the host
 #include <algorithm>
 #include <cmath>
+#include <initializer_list>
 #include <string>
+#include <unordered_map>
 #include <unordered_set>
 
 #include "ctmr_common.cuh"
@@ -236,10 +242,51 @@ __global__ void __launch_bounds__(256) cascade_peer_or_kernel(PeerExchange px, u
     bits[j] = v;
 }
 
-// ctmr_revoked_stash, thread per record of the R list: the published filter's query (p: its salt; levels[l]: level l + 1's
-// first word in `words`, m and k).  The message is built once and only its level byte changes between levels.  A record
-// the filter calls revoked is counted in counters[1]; the key body words 1..11 of any other go to `bodies`, which holds
-// n of them, at counters[0].
+// The published filter's query of the key whose message msg holds, one hash at a time (p: the filter's salt; levels[l]:
+// level l + 1's first word in `words`, m and k).  The message is built once and only its level byte changes between
+// levels.  A walk is at (l, i, lv): function i of level l + 1, lv = levels[l].
+struct FilterWalk {
+    uint32_t l, i;
+    StashLevel lv;
+
+    __device__ __forceinline__ void start(const CascadeParams& p, CascadeMsg& msg, const StashLevel* __restrict__ levels) {
+        l = i = 0;
+        lv = levels[0];
+        msg.put(p.salt_len + 4u, 1u);
+    }
+
+    // the walk's next hash; true when the key is answered, with *revoked
+    __device__ __forceinline__ bool step(const CascadeParams& p, CascadeMsg& msg, const uint32_t* __restrict__ words,
+                                         const StashLevel* __restrict__ levels, uint32_t n_levels, bool* revoked) {
+        const uint32_t b = msg.hash(p, i) % lv.m;
+        if (!(__ldg(words + lv.word + (b >> 5)) >> (b & 31u) & 1u)) {  // stopped at level l + 1: revoked iff that is even
+            *revoked = l & 1u;
+            return true;
+        }
+        if (++i < lv.k) return false;
+        i = 0;
+        if (++l == n_levels) {  // contained in all: revoked iff n_levels is odd
+            *revoked = n_levels & 1u;
+            return true;
+        }
+        lv = levels[l];
+        msg.put(p.salt_len + 4u, l + 1u);
+        return false;
+    }
+};
+
+__device__ __forceinline__ bool filter_revoked(const CascadeParams& p, CascadeMsg& msg, const uint32_t* __restrict__ words,
+                                               const StashLevel* __restrict__ levels, uint32_t n_levels) {
+    FilterWalk w;
+    w.start(p, msg, levels);
+    bool revoked = false;
+    while (!w.step(p, msg, words, levels, n_levels, &revoked)) {
+    }
+    return revoked;
+}
+
+// ctmr_revoked_stash, thread per record of the R list: the published filter's query.  A record the filter calls revoked
+// is counted in counters[1]; the key body words 1..11 of any other go to `bodies`, which holds n of them, at counters[0].
 __global__ void __launch_bounds__(kCascadeThreads) stash_query_kernel(CascadeParams p, const uint32_t* __restrict__ list, uint64_t n,
                                                                       const uint32_t* __restrict__ words, const StashLevel* __restrict__ levels,
                                                                       uint32_t n_levels, uint32_t* bodies, unsigned long long* counters) {
@@ -250,22 +297,124 @@ __global__ void __launch_bounds__(kCascadeThreads) stash_query_kernel(CascadePar
     load_body(p.table, list[t], b);
     CascadeMsg msg{smem + threadIdx.x, 0u};
     msg.build(p, b);
-    uint32_t l = 0;
-    for (; l < n_levels; ++l) {
-        const StashLevel lv = levels[l];
-        p.m = lv.m;
-        p.k = lv.k;
-        msg.put(p.salt_len + 4u, l + 1u);
-        if (!contains(p, msg, words + lv.word)) break;
-    }
-    // stopped at level l + 1: revoked iff that number is even; contained in all: iff n_levels is odd
-    if (l < n_levels ? (l & 1u) : (n_levels & 1u)) {
+    if (filter_revoked(p, msg, words, levels, n_levels)) {
         atomicAdd(counters + 1, 1ull);
         return;
     }
     uint32_t* o = bodies + 11ull * atomicAdd(counters, 1ull);
 #pragma unroll
     for (int j = 0; j < 11; ++j) o[j] = b[1 + j];
+}
+
+// ctmr_revoked_verify: the filter and the verify call's inputs of a member
+struct VerifyArgs {
+    const uint32_t* revoked;  // slot bits: R
+    const uint32_t* listed;   // slot bits: a stash lists the slot's pair
+    const uint32_t* words;
+    const StashLevel* levels;
+    uint32_t n_levels;
+    uint64_t covered_below;
+    uint32_t* list;           // slots of the listed records [cap]
+    uint64_t cap;
+    unsigned long long* counters;  // [9]
+};
+
+__device__ __forceinline__ bool slot_bit(const uint32_t* __restrict__ bits, uint32_t i) { return __ldg(bits + (i >> 5)) >> (i & 31u) & 1u; }
+
+// The answer `ans` of the covered live record in `slot`: its count into the block's counters and, when it is listed,
+// its slot into the list
+__device__ __forceinline__ void verify_finish(const CascadeParams& p, const VerifyArgs& a, uint32_t slot, bool ans,
+                                              unsigned long long* counts) {
+    const bool rev = slot_bit(a.revoked, slot);
+    const bool before = ~__ldg(&p.table[slot].inv_first) < a.covered_below;
+    atomicAdd(counts + (before ? 0u : 4u) + (rev ? (ans ? 0u : 1u) : (ans ? 3u : 2u)), 1ull);
+    if (before && rev != ans) append(slot, a.list, a.cap, a.counters + 8);
+}
+
+constexpr uint32_t kVerifyBlocksPerSm = 4;  // 64 registers, no spills (DESIGN.md "Revoked verify")
+
+// One pass over the table, scheduled by hash rather than by record.  Each lane holds one covered live record and its
+// place in the filter walk (FilterWalk), and every step of the loop computes one SHA-256 per lane.  A lane
+// whose record is answered (a clear bit, or every level walked) takes the next record from its warp's queue in shared
+// memory at the next step; the warp refills the queue 32 slots at a time whenever it holds fewer records than idle
+// lanes.  So a lane never waits for the longest walk of its warp, and the R records, whose walks are the long ones, cost
+// their own hashes only.  Records a stash lists are answered revoked at the scan, with no hash.  counters[0..8) += the
+// counts, counters[8]: records listed (past cap only the count advances).
+__global__ void __launch_bounds__(kCascadeThreads, kVerifyBlocksPerSm) verify_table_kernel(CascadeParams p, VerifyArgs a) {
+    __shared__ uint32_t smem[32 * kCascadeThreads];
+    __shared__ uint32_t queue[kCascadeThreads / 32][64];
+    __shared__ unsigned long long counts[8];
+    if (threadIdx.x < 8u) counts[threadIdx.x] = 0;
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31u, lower = (1u << lane) - 1u;
+    uint32_t* q = queue[threadIdx.x >> 5];
+    CascadeMsg msg{smem + threadIdx.x, 0u};
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    uint64_t base = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u);
+    uint32_t nq = 0, slot = 0;
+    bool have = false;
+    FilterWalk walk{};
+    for (;;) {
+        const uint32_t idle = __ballot_sync(0xffffffffu, !have);
+        const uint32_t want = __popc(idle);
+        while (nq < want && base < p.n_slots) {  // nq < 64 afterwards
+            const uint64_t s = base + lane;
+            bool cand = false;
+            if (s < p.n_slots) {
+                const uint4* sp = reinterpret_cast<const uint4*>(p.table + s);
+                const uint4 q0 = __ldg(sp), q1 = __ldg(sp + 1);  // the body is read again soon: no evict-first hint
+                cand = slot_live_ready(q0, q1, p.epoch, p.now) && issuer_covered(p, q1.y);
+                if (cand && slot_bit(a.listed, (uint32_t)s)) {
+                    verify_finish(p, a, (uint32_t)s, true, counts);
+                    cand = false;
+                }
+            }
+            const uint32_t bal = __ballot_sync(0xffffffffu, cand);
+            if (cand) q[nq + __popc(bal & lower)] = (uint32_t)s;
+            nq += __popc(bal);
+            base += stride;
+        }
+        __syncwarp();
+        if (!have) {
+            const uint32_t r = __popc(idle & lower);
+            if (r < nq) {
+                slot = q[nq - 1u - r];
+                have = true;
+                uint32_t b[12];
+                load_body(p.table, slot, b);
+                msg.build(p, b);
+                walk.start(p, msg, a.levels);
+            }
+        }
+        nq -= min(want, nq);
+        __syncwarp();
+        if (!__any_sync(0xffffffffu, have)) break;  // no record left in the warp's slots
+        bool revoked;
+        if (have && walk.step(p, msg, a.words, a.levels, a.n_levels, &revoked)) {
+            verify_finish(p, a, slot, revoked, counts);
+            have = false;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < 8u && counts[threadIdx.x]) atomicAdd(a.counters + threadIdx.x, counts[threadIdx.x]);
+}
+
+// thread per listed record: the whole slot, its tag replaced by 1 for an S record and 0 for an R record
+__global__ void __launch_bounds__(256) verify_gather_kernel(const KnownSlot* __restrict__ table, const uint32_t* __restrict__ list, uint64_t n,
+                                                            const uint32_t* __restrict__ revoked, KnownSlot* out) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const uint32_t s = list[t];
+    KnownSlot r = table[s];
+    r.tag = slot_bit(revoked, s) ? 0ull : 1ull;
+    out[t] = r;
+}
+
+// One process per GPU, a slice of the list exchange: records [0, n) of the rank's listed records into its region on
+// every rank (grid (n * 4 / 256, world); posted stores, the barrier after publishes them)
+__global__ void __launch_bounds__(256) verify_peer_send_kernel(PeerExchange px, const uint4* __restrict__ recs, uint64_t n) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < 4 * n) reinterpret_cast<uint4*>(px.inbox[blockIdx.y] + (uint64_t)px.rank * px.X)[j] = recs[j];
 }
 
 inline unsigned grid(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
@@ -500,8 +649,8 @@ int cascade_peer_or(ctmr_ctx* c, uint32_t* bits, uint64_t words, bool work) {
 }
 
 // One mailbox exchange of this rank's payload, or of its failure.  false: some rank failed (every rank reads the same
-// row and goes to the final agreement); else *sum = the sum of the payloads.
-bool peer_sum(ctmr_ctx* c, PeerLocal& local, uint64_t mine, uint64_t* sum) {
+// row and goes to the final agreement); else *sum = the sum of the payloads, and row_out (if given) every rank's.
+bool peer_sum(ctmr_ctx* c, PeerLocal& local, uint64_t mine, uint64_t* sum, uint64_t* row_out = nullptr) {
     uint64_t row[kMaxWorld] = {};
     const int rc = peer_mailbox(c, peer_word(local.code, mine), row);
     if (rc) {
@@ -512,26 +661,30 @@ bool peer_sum(ctmr_ctx* c, PeerLocal& local, uint64_t mine, uint64_t* sum) {
     if (peer_row_failed(row, W) < W) return false;
     *sum = 0;
     for (uint32_t r = 0; r < W; ++r) *sum += row[r];
+    if (row_out) std::copy(row, row + W, row_out);
     return true;
 }
 
-// now and salt define R, S and every bit, so every rank's must be rank 0's: one mailbox word each, 63 bits of FNV-1a over
-// (now, salt_len, salt)
-int peer_same_args(ctmr_ctx* c, int64_t now, const uint8_t* salt, uint32_t salt_len) {
+struct ByteSpan {
+    const void* p;
+    uint64_t n;
+};
+
+// The arguments that define the outputs (`what` names them) must be rank 0's on every rank: one mailbox word each, 63
+// bits of FNV-1a over the spans' bytes back to back
+int peer_same_args(ctmr_ctx* c, std::initializer_list<ByteSpan> args, const char* call, const char* what) {
     uint64_t h = 14695981039346656037ull;
-    const auto put = [&](uint8_t v) { h = (h ^ v) * 1099511628211ull; };
-    for (int i = 0; i < 8; ++i) put((uint8_t)((uint64_t)now >> (8 * i)));
-    put((uint8_t)salt_len);
-    for (uint32_t j = 0; j < salt_len; ++j) put(salt[j]);
+    for (const ByteSpan& s : args)
+        for (uint64_t j = 0; j < s.n; ++j) h = (h ^ static_cast<const uint8_t*>(s.p)[j]) * 1099511628211ull;
     h >>= 1;
     uint64_t row[kMaxWorld] = {};
     int rc = peer_mailbox(c, h, row);
     if (rc == CTMR_OK) rc = ctmr_check_device(c, nullptr);  // a barrier that timed out
     if (rc) return rc;
-    if (h != row[0]) return fail(c, CTMR_E_INVALID, "ctmr_revoked_cascade: now_unix_sec or salt differs from rank 0's");
+    if (h != row[0]) return fail(c, CTMR_E_INVALID, std::string(call) + what + " differs from rank 0's");
     for (uint32_t r = 1; r < c->st.peer.world; ++r)
         if (row[r] != row[0])
-            return fail(c, CTMR_E_PEER_FAILED, "ctmr_revoked_cascade: rank " + std::to_string(r) + "'s now_unix_sec or salt differs from rank 0's");
+            return fail(c, CTMR_E_PEER_FAILED, std::string(call) + "rank " + std::to_string(r) + "'s " + what + " differs from rank 0's");
     return CTMR_OK;
 }
 
@@ -665,8 +818,10 @@ int revoked_cascade(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_cr
     if (rc == CTMR_OK) rc = crl_prepare(c0, b, out, call, issuer, &n_chunks);
     if (rc == CTMR_OK && peer) rc = cascade_ensure(c0, 0, 2 * IW, false);
     if (rc == CTMR_OK) rc = refresh_digests(c0);
-    if (peer && (rc = peer_agree(c0, rc, n_chunks, row, call, "collective call failed")) == CTMR_OK)  // agreement 1
-        rc = peer_same_args(c0, now, salt, salt_len);
+    if (peer && (rc = peer_agree(c0, rc, n_chunks, row, call, "collective call failed")) == CTMR_OK) {  // agreement 1
+        const uint8_t sl = (uint8_t)salt_len;
+        rc = peer_same_args(c0, {{&now, 8}, {&sl, 1}, {salt, salt_len}}, call, "now_unix_sec or salt");
+    }
     if (rc) return group_fail(g, c0, rc);
 
     Cascade cs{m, W, peer};
@@ -981,6 +1136,263 @@ int revoked_stash(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_
     return CTMR_OK;
 }
 
+// ---- the verify -----------------------------------------------------------------------------------------------------
+// all or nothing, like cascade_ensure: the listed bits and the counters, a set of set_slots slots and room for `records`
+// listed records
+int verify_ensure(ctmr_ctx* c, uint64_t set_slots, uint64_t records) {
+    const uint64_t slot_words = (c->st.table_mask + 1 + 31) / 32;
+    VerifyState* have = c->verify.get();
+    const bool base = !have || have->slot_words < slot_words;
+    const bool st = !have || have->set_cap < set_slots;
+    const bool rs = !have || have->rec_cap < records;
+    if (!base && !st && !rs) return CTMR_OK;
+    DevBuf<uint32_t> listed;
+    DevBuf<unsigned long long> counters;
+    DevBuf<CrlSetSlot> set;
+    DevBuf<KnownSlot> recs;
+    if (base) {
+        CU(c, alloc(listed, slot_words));
+        CU(c, alloc(counters, 9));
+    }
+    if (st) CU(c, alloc(set, std::max<uint64_t>(set_slots, 1)));
+    if (rs) CU(c, alloc(recs, std::max<uint64_t>(records, 1)));
+    if (!have) {
+        c->verify.reset(new (std::nothrow) VerifyState());
+        if (!c->verify) return fail(c, CTMR_E_NOMEM, "host allocation failed");
+    }
+    VerifyState* s = c->verify.get();
+    if (base) {
+        s->listed = std::move(listed);
+        s->counters = std::move(counters);
+        s->slot_words = slot_words;
+    }
+    if (st) {
+        s->set = std::move(set);
+        s->set_cap = std::max<uint64_t>(set_slots, 1);
+    }
+    if (rs) {
+        s->recs = std::move(recs);
+        s->rec_cap = std::max<uint64_t>(records, 1);
+    }
+    return CTMR_OK;
+}
+
+// The stashes' pairs as the slots of a CrlSet (the join's key words, pair_hash, linear probing, at least twice the
+// pairs' slots): every listed (digest || serial) whose digest is registered and whose serial a key can hold.  Empty when
+// there is none.
+std::vector<CrlSetSlot> verify_stash_set(const std::vector<std::array<uint8_t, 32>>& digests, const std::unordered_set<std::string>& listed) {
+    std::unordered_map<std::string, uint32_t> dense;
+    for (uint32_t i = 0; i < digests.size(); ++i) dense.emplace(std::string(reinterpret_cast<const char*>(digests[i].data()), 32), i);
+    std::vector<std::array<uint32_t, 11>> keys;
+    for (const std::string& x : listed) {
+        const auto it = dense.find(x.substr(0, 32));
+        if (x.size() - 32 > CTMR_MAX_SERIAL || it == dense.end()) continue;  // never matches
+        std::array<uint32_t, 11> w{};
+        w[0] = it->second;
+        uint8_t* sb = reinterpret_cast<uint8_t*>(w.data() + 1);  // serial_len, then the serial, zero padded
+        sb[0] = (uint8_t)(x.size() - 32);
+        std::memcpy(sb + 1, x.data() + 32, x.size() - 32);
+        keys.push_back(w);
+    }
+    if (keys.empty()) return {};
+    uint64_t n = 64;
+    while (n < 2 * keys.size()) n <<= 1;
+    std::vector<CrlSetSlot> set(n, CrlSetSlot{});
+    for (const auto& k : keys) {
+        uint32_t w[11];
+        std::copy(k.begin(), k.end(), w);
+        const uint32_t h = pair_hash(w);
+        uint64_t pos = h & (n - 1);
+        while (set[pos].tag) pos = (pos + 1) & (n - 1);  // the pairs are distinct
+        set[pos].tag = (h & ~3u) | 2u;
+        std::copy(w, w + 11, set[pos].key);
+    }
+    return set;
+}
+
+// member r's verify after cascade_front: the stashes' set marked into the listed bits, the pass over the shard (run
+// again with longer lists when its listed records outgrew them), counts[0..8) = its counts, and its listed records
+// gathered into VerifyState::recs and appended to `recs`
+int verify_member(Cascade& cs, uint32_t r, const StashFilter& f, const std::vector<CrlSetSlot>& set, uint64_t covered_below,
+                  uint64_t* counts, std::vector<KnownSlot>& recs) {
+    ctmr_ctx* c = cs.m[r];
+    CU(c, cudaSetDevice(c->device));
+    int rc = stash_ensure(c, f.words.size(), f.levels.size(), 0);
+    if (rc == CTMR_OK) rc = verify_ensure(c, set.size(), 0);
+    if (rc) return rc;
+    StashState* s = c->stash.get();
+    VerifyState* v = c->verify.get();
+    CascadeState* cst = c->cascade.get();
+    const CascadeParams q = cs.params(c);
+    CU(c, cudaMemcpyAsync(s->words, f.words.data(), f.words.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(s->levels, f.levels.data(), f.levels.size() * sizeof(StashLevel), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaMemsetAsync(v->listed, 0, v->slot_words * 4, c->stream));
+    if (!set.empty()) {
+        CU(c, cudaMemcpyAsync(v->set, set.data(), set.size() * sizeof(CrlSetSlot), cudaMemcpyHostToDevice, c->stream));
+        cascade_mark_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(q.table, q.n_slots, q.epoch, q.now, v->set, set.size() - 1, v->listed);
+        CU(c, cudaGetLastError());
+    }
+    unsigned long long h[9] = {};
+    for (;;) {
+        const VerifyArgs a{cst->revoked, v->listed, s->words, s->levels, (uint32_t)f.levels.size(), covered_below, cst->list[1], cst->list_cap,
+                           v->counters};
+        CU(c, cudaMemsetAsync(v->counters, 0, sizeof(h), c->stream));
+        verify_table_kernel<<<c->sm_count * kVerifyBlocksPerSm, kCascadeThreads, 0, c->stream>>>(q, a);
+        CU(c, cudaGetLastError());
+        CU(c, cudaMemcpyAsync(h, v->counters, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        if (h[8] <= cst->list_cap) break;
+        if ((rc = cascade_ensure(c, h[8], 0, false))) return rc;
+    }
+    std::copy(h, h + 8, counts);
+    if (h[8] == 0) return CTMR_OK;
+    if ((rc = verify_ensure(c, 0, h[8]))) return rc;
+    verify_gather_kernel<<<grid(h[8], 256), 256, 0, c->stream>>>(q.table, cst->list[1], h[8], cst->revoked, v->recs);
+    CU(c, cudaGetLastError());
+    const size_t at = recs.size();
+    recs.resize(at + h[8]);
+    CU(c, cudaMemcpyAsync(recs.data() + at, v->recs, h[8] * sizeof(KnownSlot), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    return CTMR_OK;
+}
+
+// Peer ranks: every other rank's listed records (n[s] of rank s, agreed) appended to `recs`, slice by slice through the
+// parity-0 regions: the rank's X records of the slice into its region on every rank, a barrier, the other ranks' regions
+// to the host, a barrier.  `work` false (this rank failed): the barriers only.
+int verify_peer_gather(ctmr_ctx* c, const uint64_t* n, std::vector<KnownSlot>& recs, bool work) {
+    const PeerExchange& px = c->px;
+    uint64_t most = 0;
+    for (uint32_t r = 0; r < px.world; ++r) most = std::max(most, n[r]);
+    int rc = CTMR_OK;
+    for (uint64_t lo = 0; lo < most; lo += px.X) {
+        work = work && rc == CTMR_OK;
+        if (work && n[px.rank] > lo) {
+            const uint64_t k = std::min(px.X, n[px.rank] - lo);
+            verify_peer_send_kernel<<<dim3(grid(4 * k, 256), px.world), 256, 0, c->stream>>>(
+                px, reinterpret_cast<const uint4*>(c->verify->recs.get() + lo), k);
+            rc = launched(c);
+        }
+        int brc = peer_barrier(c, CH_CRL, c->stream);  // every region of the slice has landed
+        if (rc == CTMR_OK) rc = brc;
+        if (rc == CTMR_OK && work)
+            rc = [&]() -> int {
+                for (uint32_t s = 0; s < px.world; ++s) {
+                    if (s == px.rank || n[s] <= lo) continue;
+                    const uint64_t k = std::min(px.X, n[s] - lo);
+                    const size_t at = recs.size();
+                    recs.resize(at + k);
+                    CU(c, cudaMemcpyAsync(recs.data() + at, px.inbox[px.rank] + (uint64_t)s * px.X, k * sizeof(KnownSlot), cudaMemcpyDeviceToHost,
+                                          c->stream));
+                }
+                CU(c, cudaStreamSynchronize(c->stream));
+                return CTMR_OK;
+            }();
+        brc = peer_barrier(c, CH_CRL, c->stream);  // every rank has read the slice: the regions are free again
+        if (rc == CTMR_OK) rc = brc;
+    }
+    return rc;
+}
+
+// One driver for one ctx, a group and one rank of a group of processes, in revoked_cascade's phases: its checks (with the
+// stash's checks of the filter and the stashes) and agreements (the hash covers now, covered_below, the filter and the
+// stashes), cascade_front, then every member's verify_member.  The counts are sums over the members, or mailbox sums
+// over the ranks; the listed records are every member's, or every rank's after verify_peer_gather, and every rank sorts
+// the same union.  The finish is the cascade's, with the list cap in place of the byte cap.
+int revoked_verify(ctmr_ctx* const* m, uint32_t W, ctmr_group* g, const ctmr_crl_batch* b, int64_t now, const uint8_t* filter,
+                   uint64_t filter_bytes, const uint8_t* stashes, uint64_t stash_bytes, uint64_t covered_below, ctmr_verify_out* out) {
+    ctmr_ctx* c0 = m[0];
+    const bool peer = peer_call(c0);
+    const char* call = "ctmr_revoked_verify: ";
+    int rc = set_device(c0);
+    if (rc) return group_fail(g, c0, rc);
+    if (peer && out) out->n_list = 0;
+    const uint64_t IW = c0->st.max_issuers / 32 + 1;  // words of the seen bitmap, and of the bad one after it
+    std::vector<uint32_t> issuer;
+    uint64_t n_chunks = 0, row[kMaxWorld] = {};
+    StashFilter f;
+    std::unordered_set<std::string> listed;
+    const char* bad = !filter && filter_bytes ? "NULL filter" : !stashes && stash_bytes ? "NULL stashes" : nullptr;
+    if (!bad) bad = stash_filter(filter, filter_bytes, f);
+    if (!bad) bad = stash_parse(stashes, stash_bytes, listed);
+    rc = bad ? fail(c0, CTMR_E_INVALID, std::string(call) + bad) : crl_prepare(c0, b, out, call, issuer, &n_chunks);
+    if (rc == CTMR_OK && peer) rc = cascade_ensure(c0, 0, 2 * IW, false);
+    if (rc == CTMR_OK) rc = refresh_digests(c0);
+    if (peer && (rc = peer_agree(c0, rc, n_chunks, row, call, "collective call failed")) == CTMR_OK)  // agreement 1
+        rc = peer_same_args(c0, {{&now, 8}, {&covered_below, 8}, {&filter_bytes, 8}, {filter, filter_bytes}, {&stash_bytes, 8}, {stashes, stash_bytes}},
+                            call, "now_unix_sec, covered_below, filter or stashes");
+    if (rc) return group_fail(g, c0, rc);
+
+    Cascade cs{m, W, peer};
+    cs.p.n_issuers = (uint32_t)c0->digests.size();
+    cs.p.salt_len = f.salt_len;
+    cs.p.now = now;
+    for (uint32_t j = 0; j < f.salt_len; ++j) cs.p.salt[j >> 2] |= (uint32_t)f.salt[j] << (8 * (j & 3));
+    cs.p.one = 1;
+    cs.ml.assign(W, MemberLevel{});
+    PeerLocal& local = cs.local;
+    std::vector<uint8_t> crl_status(b->n_crls, CTMR_CRL_OK);
+    uint32_t n_covered = 0;
+    uint64_t counts[8] = {};
+    std::vector<KnownSlot> recs;
+    const auto verify = [&]() {  // every return is one that all peer ranks take together, to the finish
+        if (!cascade_front(cs, b, issuer, row, crl_status, &n_covered)) return;
+        const std::vector<CrlSetSlot> set = verify_stash_set(c0->digests, listed);
+        std::vector<uint64_t> mc(8 * W, 0);
+        for (uint32_t r = 0; r < W; ++r) cs.run(m[r], [&] { return verify_member(cs, r, f, set, covered_below, &mc[8 * r], recs); });
+        if (!peer) {
+            for (uint32_t j = 0; j < 8 * W; ++j) counts[j & 7] += mc[j];
+            return;
+        }
+        for (uint32_t j = 0; j < 8; ++j)
+            if (!peer_sum(c0, local, mc[j], &counts[j])) return;
+        uint64_t total = 0, n[kMaxWorld] = {};
+        if (!peer_sum(c0, local, recs.size(), &total, n)) return;
+        local.fail(c0, verify_peer_gather(c0, n, recs, !local.code));
+    };
+    verify();
+
+    const uint64_t n_list = recs.size();
+    const bool short_cap = n_list > out->list_cap || (!out->list && n_list);
+    rc = peer ? crl_peer_finish(c0, local, short_cap ? 1 : 0, row, call) : local.code;
+    if (rc) {
+        if (g) g->err = local.err;  // the failing member's text is the group's
+        return rc;
+    }
+    if (!peer) row[0] = short_cap;  // as the only rank
+    out->n_list = n_list;
+    const uint32_t world = peer ? c0->st.peer.world : 1, me = peer ? c0->px.rank : 0;
+    for (uint32_t r = 0; r < world; ++r)
+        if (row[r])
+            return group_fail(g, c0, fail(c0, CTMR_E_BATCH_TOO_LARGE, r == me ? "ctmr_revoked_verify: list_cap " + std::to_string(out->list_cap) + " < " + std::to_string(n_list) + " records"
+                                                                             : "ctmr_revoked_verify: rank " + std::to_string(r) + "'s list_cap < " + std::to_string(n_list) + " records"));
+    std::vector<ctmr_verify_miss> list(n_list);
+    for (uint64_t i = 0; i < n_list; ++i) {
+        const KnownSlot& k = recs[i];
+        const uint8_t* kb = reinterpret_cast<const uint8_t*>(k.body);  // exp_hour, issuer, serial_len, serial
+        ctmr_verify_miss& e = list[i];
+        std::memset(&e, 0, sizeof(e));
+        std::memcpy(e.digest, c0->digests[k.body[1]].data(), 32);
+        e.exp_hour = (int32_t)k.body[0];
+        e.first_index = ~k.inv_first;
+        e.serial_len = kb[8];
+        std::memcpy(e.serial, kb + 9, CTMR_MAX_SERIAL);
+        e.blocked = (uint8_t)k.tag;
+    }
+    std::sort(list.begin(), list.end(), [](const ctmr_verify_miss& a, const ctmr_verify_miss& z) {
+        if (const int d = std::memcmp(a.digest, z.digest, 32)) return d < 0;
+        if (const int s = std::memcmp(a.serial, z.serial, std::min(a.serial_len, z.serial_len))) return s < 0;
+        if (a.serial_len != z.serial_len) return a.serial_len < z.serial_len;
+        return a.exp_hour < z.exp_hour;
+    });
+    if (n_list) std::memcpy(out->list, list.data(), n_list * sizeof(ctmr_verify_miss));
+    if (out->crl_status) std::memcpy(out->crl_status, crl_status.data(), crl_status.size());
+    out->issuers = n_covered;
+    out->levels = (uint32_t)f.levels.size();
+    out->before = ctmr_verify_counts{counts[0], counts[1], counts[2], counts[3]};
+    out->since = ctmr_verify_counts{counts[4], counts[5], counts[6], counts[7]};
+    return CTMR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1014,6 +1426,23 @@ int ctmr_group_revoked_stash(ctmr_group* g, const ctmr_crl_batch* batch, int64_t
                              const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out) {
     if (!g || g->m.empty()) return CTMR_E_INVALID;
     const int rc = revoked_stash(g->m.data(), (uint32_t)g->m.size(), g, batch, now_unix_sec, filter, filter_bytes, stashes, stash_bytes, out);
+    cudaSetDevice(g->m[0]->device);
+    return rc;
+}
+
+int ctmr_revoked_verify(ctmr_ctx* c, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter, uint64_t filter_bytes,
+                        const uint8_t* stashes, uint64_t stash_bytes, uint64_t covered_below, ctmr_verify_out* out) {
+    if (!c) return CTMR_E_INVALID;
+    if (c->group) return fail(c, CTMR_E_INVALID, "ctmr_revoked_verify: a member of a group; use ctmr_group_revoked_verify");
+    ctmr_ctx* m[1] = {c};
+    return revoked_verify(m, 1, nullptr, batch, now_unix_sec, filter, filter_bytes, stashes, stash_bytes, covered_below, out);
+}
+
+int ctmr_group_revoked_verify(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter, uint64_t filter_bytes,
+                              const uint8_t* stashes, uint64_t stash_bytes, uint64_t covered_below, ctmr_verify_out* out) {
+    if (!g || g->m.empty()) return CTMR_E_INVALID;
+    const int rc = revoked_verify(g->m.data(), (uint32_t)g->m.size(), g, batch, now_unix_sec, filter, filter_bytes, stashes, stash_bytes,
+                                  covered_below, out);
     cudaSetDevice(g->m[0]->device);
     return rc;
 }

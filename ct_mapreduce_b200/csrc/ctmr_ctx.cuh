@@ -385,6 +385,19 @@ struct StashState {
     DevBuf<uint32_t> bodies;             // [body_cap][11]: issuer, serial_len, serial[39]
 };
 
+// ctmr_revoked_verify (ctmr_cascade.cu): one bit per table slot (listed: a stash lists the slot's pair), the stashes' set,
+// the counts and the listed records read back (the filter is StashState's, the slots of the listed records go to the
+// cascade's list 1).  Built on first use and grown, all or nothing.
+struct VerifyState {
+    uint64_t slot_words = 0;
+    DevBuf<uint32_t> listed;              // [slot_words]
+    DevBuf<unsigned long long> counters;  // [9]: before and since (revoked, missed, valid, blocked), then records listed
+    uint64_t set_cap = 0;
+    DevBuf<CrlSetSlot> set;               // [set_cap]
+    uint64_t rec_cap = 0;
+    DevBuf<KnownSlot> recs;               // [rec_cap]: the listed records, tag 1 for an S record, 0 for an R record
+};
+
 // the ctx's private device words (one allocation)
 struct SmallDev {
     unsigned long long slots_used;   // DeviceState::slots_used points here (no kernel reads it)
@@ -485,7 +498,8 @@ struct ctmr_ctx {
     uint32_t fe_peer_stopped = 0;  // ranks that stopped (tiles) in the last collective front-end call
     std::unique_ptr<CrlState> crl;  // ctmr_revoked_known (ctmr_crl.cu)
     std::unique_ptr<CascadeState> cascade;  // ctmr_revoked_cascade (ctmr_cascade.cu)
-    std::unique_ptr<StashState> stash;      // ctmr_revoked_stash (ctmr_cascade.cu)
+    std::unique_ptr<StashState> stash;      // ctmr_revoked_stash and ctmr_revoked_verify (ctmr_cascade.cu)
+    std::unique_ptr<VerifyState> verify;    // ctmr_revoked_verify (ctmr_cascade.cu)
     std::string err;
 };
 

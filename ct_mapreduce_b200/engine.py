@@ -16,6 +16,8 @@ points, and exposes the results under the reference's names:
                                           certificates, built on the GPU next to the table
     GpuCertDatabase.revoked_stash      <- CRLite's stash: the revoked known certificates a published filter and the
                                           stashes since it miss
+    GpuCertDatabase.revoked_verify     <- filter-cascade's verify(include, exclude) of a published filter and its
+                                          stashes, with the table's revoked and valid known certificates
 
 All arithmetic happens in the CUDA kernels; nothing here parses, hashes or de-duplicates.
 """
@@ -281,6 +283,28 @@ class StashResult:
         self.crl_status = crl_status
         self.issuers, self.stash_issuers = int(o.issuers), int(o.stash_issuers)
         self.revoked, self.in_filter, self.in_stashes, self.serials = int(o.revoked), int(o.in_filter), int(o.in_stashes), int(o.serials)
+
+
+MISS_DTYPE = np.dtype([("digest", "u1", 32), ("exp_hour", "<i8"), ("first_index", "<u8"), ("serial_len", "u1"),
+                       ("serial", "u1", capi.MAX_SERIAL), ("blocked", "u1"), ("pad", "u1", 7)])   # ctmr_verify_miss
+
+
+class VerifyResult:
+    """Outputs of ctmr_revoked_verify (include/ctmr.h ctmr_verify_out): each CRL's status, the covered issuers, the
+    filter's levels, the counts of the records first seen before covered_below (.before) and of the others (.since), each
+    a dict of revoked, missed, valid and blocked, and .list, a MISS_DTYPE array of the `before` records answered wrongly
+    in the header's order."""
+
+    def __init__(self, crl_status: np.ndarray, o, lst: np.ndarray):
+        self.crl_status = crl_status
+        self.issuers, self.levels = int(o.issuers), int(o.levels)
+        self.before, self.since = ({f: int(getattr(c, f)) for f, _ in capi.VerifyCounts._fields_} for c in (o.before, o.since))
+        self.list = lst
+
+    def entries(self) -> list:
+        """the list as (digest, serial, exp_hour, first_index, blocked) tuples"""
+        return [(r["digest"].tobytes(), r["serial"][:r["serial_len"]].tobytes(), int(r["exp_hour"]), int(r["first_index"]),
+                 bool(r["blocked"])) for r in self.list]
 
 
 def _crl_batch(crls, issuer_digests):
@@ -831,6 +855,42 @@ class GpuCertDatabase:
         self._check(rc)
         self._stash_bytes = int(o.bytes)
         return StashResult(buf[:o.bytes].tobytes(), status[:b.n_crls].copy(), o)
+
+    _verify_records = 0   # records the last verify of this db listed: the next call's first list holds twice that
+
+    def revoked_verify(self, crls, issuer_digests, now_unix_sec: int, filter: bytes, stashes: bytes = b"",
+                       covered_below: int = 2**64 - 1, cap: int | None = None) -> VerifyResult:
+        """A published `filter`, with `stashes` (every stash published since it, back to back), checked against the table
+        (ctmr_revoked_verify): every live known certificate of the covered issuers, revoked by these CRLs or not, is queried,
+        and counted in .before when it was first seen at a global index below covered_below (ctmr_next_index when the
+        filter was built), in .since otherwise.  `crls` and `issuer_digests` as for revoked_cascade.  Read-only.  The list
+        holds `cap` records; by default 4096, or twice the last list this db returned if that is more.  A longer list is
+        computed twice: the first call only reports its length.
+        On a db attached to peers the call is collective: every rank calls it with its own CRLs (an empty list will do) and
+        the same now_unix_sec, filter, stashes and covered_below, and every rank gets the same counts and list.  A rank
+        whose arguments are refused here still makes the call, with no batch, so that the other ranks return
+        CTMR_E_PEER_FAILED, and then raises."""
+        fn = self._c("revoked_verify")
+        with self._peer_refusal(lambda: fn(self._h, None, 0, None, 0, None, 0, 0, None)):
+            b, keep = _crl_batch(crls, issuer_digests)
+            filter, stashes = bytes(filter), bytes(stashes)
+            fbuf = (C.c_uint8 * max(len(filter), 1)).from_buffer_copy(filter or b"\0")
+            sbuf = (C.c_uint8 * max(len(stashes), 1)).from_buffer_copy(stashes or b"\0")
+            status = np.zeros(max(int(b.n_crls), 1), np.uint8)
+            size = int(cap) if cap is not None else max(4096, 2 * self._verify_records)
+            now_unix_sec, covered_below = int(now_unix_sec), int(covered_below)
+
+        def call(n):
+            lst = np.zeros(max(n, 1), MISS_DTYPE)
+            o = capi.VerifyOut(capi.ptr(status), 0, 0, capi.VerifyCounts(), capi.VerifyCounts(), capi.ptr(lst), n, 0)
+            return fn(self._h, C.byref(b), now_unix_sec, fbuf, len(filter), sbuf, len(stashes), covered_below, C.byref(o)), o, lst
+
+        rc, o, lst = call(size)
+        if rc == capi.E_BATCH_TOO_LARGE and o.n_list:  # longer than the list: again into one of the length it reported
+            rc, o, lst = call(int(o.n_list))
+        self._check(rc)
+        self._verify_records = int(o.n_list)
+        return VerifyResult(status[:b.n_crls].copy(), o, lst[:o.n_list].copy())
 
     def checkpoint(self) -> np.ndarray:
         """This db's part of a portable checkpoint (ctmr_checkpoint_save): loads into any table size, group size or number

@@ -162,6 +162,39 @@ type Stash struct {
 	Serials      uint64  // (issuer, serial) entries written
 }
 
+// cCRLBatch copies crls and their issuer IDs (at least one per CRL) into C memory as one ctmr_crl_batch: the batch
+// holds pointers, so it cannot point into Go memory.  free releases all of it.
+func cCRLBatch(crls [][]byte, issuerIDs [][32]byte) (*C.ctmr_crl_batch, func()) {
+	n := len(crls)
+	total := 0
+	for _, c := range crls {
+		total += len(c)
+	}
+	data := C.malloc(C.size_t(total + 1))
+	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
+	lens := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
+	dig := C.malloc(C.size_t(32*n + 32))
+	flat := unsafe.Slice((*byte)(data), total+1)
+	o := 0
+	for i, c := range crls {
+		copy(flat[o:], c)
+		offs[i], lens[i] = C.uint64_t(o), C.uint64_t(len(c))
+		copy(unsafe.Slice((*byte)(dig), 32*n)[32*i:], issuerIDs[i][:])
+		o += len(c)
+	}
+	b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
+	b.data, b.data_bytes = (*C.uint8_t)(data), C.uint64_t(total)
+	b.crl_off, b.crl_len = &offs[0], &lens[0]
+	b.issuer_digest, b.n_crls = (*C.uint8_t)(dig), C.uint64_t(n)
+	return b, func() {
+		C.free(unsafe.Pointer(b))
+		C.free(dig)
+		C.free(unsafe.Pointer(&lens[0]))
+		C.free(unsafe.Pointer(&offs[0]))
+		C.free(data)
+	}
+}
+
 // RevokedCascade builds the filter cascade of the covered issuers' live known certificates on the GPU: the revoked
 // ones included, every other one excluded.  crls and issuerIDs as for RevokedKnown, verified CRLs only; salt is at most
 // 32 bytes.  Read-only.  The output buffer holds 16 MiB, or twice the DB's last cascade if that is more; a larger cascade
@@ -176,31 +209,8 @@ func (d *DB) RevokedCascade(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int6
 		err := fmt.Errorf("RevokedCascade: %d issuer IDs for %d CRLs", len(issuerIDs), n)
 		return nil, d.peerRefuseWith(err, func() { C.ctmr_revoked_cascade(d.h, nil, 0, nil, 0, nil) })
 	}
-	total := 0
-	for _, c := range crls {
-		total += len(c)
-	}
-	data := C.malloc(C.size_t(total + 1))
-	defer C.free(data)
-	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
-	lens := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
-	dig := C.malloc(C.size_t(32*n + 32))
-	defer C.free(unsafe.Pointer(&offs[0]))
-	defer C.free(unsafe.Pointer(&lens[0]))
-	defer C.free(dig)
-	flat := unsafe.Slice((*byte)(data), total+1)
-	o := 0
-	for i, c := range crls {
-		copy(flat[o:], c)
-		offs[i], lens[i] = C.uint64_t(o), C.uint64_t(len(c))
-		copy(unsafe.Slice((*byte)(dig), 32*n)[32*i:], issuerIDs[i][:])
-		o += len(c)
-	}
-	b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
-	defer C.free(unsafe.Pointer(b))
-	b.data, b.data_bytes = (*C.uint8_t)(data), C.uint64_t(total)
-	b.crl_off, b.crl_len = &offs[0], &lens[0]
-	b.issuer_digest, b.n_crls = (*C.uint8_t)(dig), C.uint64_t(n)
+	b, free := cCRLBatch(crls, issuerIDs)
+	defer free()
 	cs := C.malloc(C.size_t(len(salt) + 1))
 	defer C.free(cs)
 	copy(unsafe.Slice((*byte)(cs), len(salt)+1), salt)
@@ -252,31 +262,8 @@ func (d *DB) RevokedStash(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int64,
 	if len(issuerIDs) < n {
 		return nil, fmt.Errorf("RevokedStash: %d issuer IDs for %d CRLs", len(issuerIDs), n)
 	}
-	total := 0
-	for _, c := range crls {
-		total += len(c)
-	}
-	data := C.malloc(C.size_t(total + 1))
-	defer C.free(data)
-	offs := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
-	lens := (*[1 << 30]C.uint64_t)(C.malloc(C.size_t(8*n + 8)))[: n+1 : n+1]
-	dig := C.malloc(C.size_t(32*n + 32))
-	defer C.free(unsafe.Pointer(&offs[0]))
-	defer C.free(unsafe.Pointer(&lens[0]))
-	defer C.free(dig)
-	flat := unsafe.Slice((*byte)(data), total+1)
-	o := 0
-	for i, c := range crls {
-		copy(flat[o:], c)
-		offs[i], lens[i] = C.uint64_t(o), C.uint64_t(len(c))
-		copy(unsafe.Slice((*byte)(dig), 32*n)[32*i:], issuerIDs[i][:])
-		o += len(c)
-	}
-	b := (*C.ctmr_crl_batch)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_crl_batch{}))))
-	defer C.free(unsafe.Pointer(b))
-	b.data, b.data_bytes = (*C.uint8_t)(data), C.uint64_t(total)
-	b.crl_off, b.crl_len = &offs[0], &lens[0]
-	b.issuer_digest, b.n_crls = (*C.uint8_t)(dig), C.uint64_t(n)
+	b, free := cCRLBatch(crls, issuerIDs)
+	defer free()
 	cf := C.malloc(C.size_t(len(filter) + 1))
 	defer C.free(cf)
 	copy(unsafe.Slice((*byte)(cf), len(filter)+1), filter)
@@ -323,4 +310,103 @@ func (d *DB) RevokedStash(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int64,
 		InStashes:    uint64(out.in_stashes),
 		Serials:      uint64(out.serials),
 	}, nil
+}
+
+// VerifyCounts are key records of the covered issuers, counted as RevokedCascade counts them.
+type VerifyCounts struct {
+	Revoked uint64 // in R, answered revoked
+	Missed  uint64 // in R, answered not revoked
+	Valid   uint64 // in S, answered not revoked
+	Blocked uint64 // in S, answered revoked
+}
+
+// VerifyMiss is one key record the filter and the stashes answer wrongly.
+type VerifyMiss struct {
+	IssuerID   [32]byte
+	ExpHour    int64
+	FirstIndex uint64 // the record's first-seen global index
+	Serial     []byte
+	Blocked    bool   // an S record answered revoked; false: an R record answered not revoked
+}
+
+// Verify is what RevokedVerify reports (include/ctmr.h "CRLite verify" states the rules).
+type Verify struct {
+	CRLStatus []uint8      // per CRL, CTMR_CRL_*
+	Issuers   uint32       // issuers covered (RevokedCascade's rule)
+	Levels    uint32       // levels of the filter
+	Before    VerifyCounts // records first seen at a global index below coveredBelow
+	Since     VerifyCounts // the others
+	List      []VerifyMiss // the Before records answered wrongly, by issuer ID, serial and hour
+}
+
+// RevokedVerify checks a published filter, with every stash published since it (back to back; may be empty), against
+// the table on the GPU: every live known certificate of the covered issuers, revoked by these CRLs or not, is queried.
+// coveredBelow is DB.NextIndex read when the filter was built (math.MaxUint64: every record counts in Before).  crls and
+// issuerIDs as for RevokedCascade.  Read-only.  The list holds 4096 records, or twice the DB's last list if that is
+// more; a longer list is computed twice (the first call only reports its length).  On a DB attached to peers the call
+// is collective: every rank calls it with its own CRLs (none will do) and the same nowUnixSec, filter, stashes and
+// coveredBelow, and every rank gets the same counts and list.  A rank whose arguments are refused here still makes the
+// call, with no batch, so that the other ranks fail instead of waiting.
+func (d *DB) RevokedVerify(crls [][]byte, issuerIDs [][32]byte, nowUnixSec int64, filter, stashes []byte, coveredBelow uint64) (*Verify, error) {
+	n := len(crls)
+	if len(issuerIDs) < n {
+		err := fmt.Errorf("RevokedVerify: %d issuer IDs for %d CRLs", len(issuerIDs), n)
+		return nil, d.peerRefuseWith(err, func() { C.ctmr_revoked_verify(d.h, nil, 0, nil, 0, nil, 0, 0, nil) })
+	}
+	b, free := cCRLBatch(crls, issuerIDs)
+	defer free()
+	cf := C.malloc(C.size_t(len(filter) + 1))
+	defer C.free(cf)
+	copy(unsafe.Slice((*byte)(cf), len(filter)+1), filter)
+	cst := C.malloc(C.size_t(len(stashes) + 1))
+	defer C.free(cst)
+	copy(unsafe.Slice((*byte)(cst), len(stashes)+1), stashes)
+	status := C.calloc(C.size_t(n+1), 1)
+	defer C.free(status)
+	out := (*C.ctmr_verify_out)(C.calloc(1, C.size_t(unsafe.Sizeof(C.ctmr_verify_out{}))))
+	defer C.free(unsafe.Pointer(out))
+	call := func() C.int {
+		f, fn := (*C.uint8_t)(cf), C.uint64_t(len(filter))
+		s, sn := (*C.uint8_t)(cst), C.uint64_t(len(stashes))
+		if d.g != nil {
+			return C.ctmr_group_revoked_verify(d.g, b, C.int64_t(nowUnixSec), f, fn, s, sn, C.uint64_t(coveredBelow), out)
+		}
+		return C.ctmr_revoked_verify(d.h, b, C.int64_t(nowUnixSec), f, fn, s, sn, C.uint64_t(coveredBelow), out)
+	}
+	size := uint64(4096)
+	if 2*d.verifyList > size {
+		size = 2 * d.verifyList
+	}
+	rec := C.size_t(unsafe.Sizeof(C.ctmr_verify_miss{}))
+	list := C.malloc(C.size_t(size) * rec) // a longer list is computed again into one of the length it reported
+	out.list, out.list_cap, out.crl_status = (*C.ctmr_verify_miss)(list), C.uint64_t(size), (*C.uint8_t)(status)
+	rc := call()
+	if rc == C.CTMR_E_BATCH_TOO_LARGE && out.n_list > 0 {
+		C.free(list)
+		list = C.malloc(C.size_t(out.n_list) * rec)
+		out.list, out.list_cap = (*C.ctmr_verify_miss)(list), out.n_list
+		rc = call()
+	}
+	defer C.free(list)
+	if err := d.err(rc, "ctmr_revoked_verify"); err != nil {
+		return nil, err
+	}
+	d.verifyList = uint64(out.n_list)
+	counts := func(c C.ctmr_verify_counts) VerifyCounts {
+		return VerifyCounts{uint64(c.revoked), uint64(c.missed), uint64(c.valid), uint64(c.blocked)}
+	}
+	v := &Verify{
+		CRLStatus: C.GoBytes(status, C.int(n)),
+		Issuers:   uint32(out.issuers),
+		Levels:    uint32(out.levels),
+		Before:    counts(out.before),
+		Since:     counts(out.since),
+	}
+	for _, m := range unsafe.Slice((*C.ctmr_verify_miss)(list), int(out.n_list)) {
+		e := VerifyMiss{ExpHour: int64(m.exp_hour), FirstIndex: uint64(m.first_index), Blocked: m.blocked != 0}
+		copy(e.IssuerID[:], C.GoBytes(unsafe.Pointer(&m.digest[0]), 32))
+		e.Serial = C.GoBytes(unsafe.Pointer(&m.serial[0]), C.int(m.serial_len))
+		v.List = append(v.List, e)
+	}
+	return v, nil
 }

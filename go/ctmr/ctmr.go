@@ -64,6 +64,7 @@ type DB struct {
 	peer         bool   // attached to the DBs of other processes (PeerAttach): the batch calls and the front end are collective
 	cascadeBytes uint64 // size of the last RevokedCascade: the next call's first buffer holds twice that
 	stashBytes   uint64 // size of the last RevokedStash: the next call's first buffer holds twice that
+	verifyList   uint64 // records the last RevokedVerify listed: the next call's first list holds twice that
 }
 
 func New(c Config) (*DB, error) {

@@ -487,6 +487,71 @@ int ctmr_revoked_stash(ctmr_ctx* ctx, const ctmr_crl_batch* batch, int64_t now_u
                        const uint8_t* filter, uint64_t filter_bytes,
                        const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out);
 
+/* ---- CRLite verify (a published filter and its stashes checked against the table) --------------------------------- */
+/* Checks a filter, with the stashes published since it, against the table before it is published or while it is in
+ * use: every live record of a covered issuer is queried, and only the records answered wrongly reach the host
+ * (DESIGN.md "Revoked verify").  Filter.verify(include, exclude) of Mozilla's filter-cascade, with R and S from the table.
+ *
+ * Sets.  Covered issuers, live records, R and S are ctmr_revoked_cascade's for the same batch and now_unix_sec.  Records
+ * of issuers that are not covered are neither verified nor counted.
+ *
+ * Answer.  x = digest || serial.  A record is ANSWERED REVOKED when the query rule above, with the filter's own salt,
+ * says revoked, or when any stash in `stashes` lists (digest, serial) (the stash layout above; `stashes` may be empty).
+ * Counts are key records: a serial under two hours is two records, each with its own first index.
+ *
+ * Age.  A record is counted in `before` when its first-seen global index is below covered_below, and in `since`
+ * otherwise.  The index is the one the table keeps per key (eviction, resize and checkpoint loads keep it; preloads take
+ * indices from next_index).  Pass ctmr_next_index, read when the filter was built, to tell the records the filter was
+ * built over from the ones that arrived later; UINT64_MAX puts every record in `before`.
+ *
+ * List.  Every `before` record that is missed or blocked, ordered by digest bytes, then serial (ascending bytes, a prefix
+ * before any longer serial), then exp_hour.  That triple is unique per key record, so the output is deterministic: it
+ * depends neither on slot order, shard count nor thread order.  If list_cap is too small, or list is NULL while records
+ * are to be listed, the call returns CTMR_E_BATCH_TOO_LARGE and writes n_list and nothing else (ctmr_revoked_known's
+ * entry_cap rule).
+ *
+ * Checks before any work, each CTMR_E_INVALID: ctmr_revoked_stash's checks of the filter (including k <= 64) and of the
+ * stashes, ctmr_revoked_cascade's (a NULL batch or output, a CRL outside data or larger than a chunk).  Stash entries of
+ * unregistered digests or longer than CTMR_MAX_SERIAL are accepted and never match.  Read-only, like the other CRL calls.
+ * A member ctx of a group is refused with CTMR_E_INVALID (use ctmr_group_revoked_verify).  Cost: the cascade's mark and
+ * split, one more mark pass for the stashes, and one pass over the table that hashes the covered live records the
+ * stashes do not list (DESIGN.md "Revoked verify").
+ *
+ * On a ctx attached to peers (world > 1) the call is COLLECTIVE and follows ctmr_revoked_cascade's peer rules: every rank
+ * passes its own CRLs (possibly none) and the same now_unix_sec, covered_below, filter and stashes.  Counts and list are
+ * identical on every rank: what one ctx holding every rank's table gives for the CRLs of all ranks in rank order;
+ * crl_status covers the rank's own CRLs.  A rank whose now_unix_sec, covered_below, filter or stashes differ from rank
+ * 0's returns CTMR_E_INVALID and the others CTMR_E_PEER_FAILED, before any work.  A list_cap too small on any rank is
+ * CTMR_E_BATCH_TOO_LARGE on every rank, each writing only n_list; later failures are every rank's.
+ * Out of scope: un-revocations in stashes; which issuers the old filter covered (the issuers covered now are verified). */
+typedef struct ctmr_verify_counts {  /* key records, counted as the cascade counts them */
+    uint64_t revoked;                /* in R, answered revoked */
+    uint64_t missed;                 /* in R, answered not revoked */
+    uint64_t valid;                  /* in S, answered not revoked */
+    uint64_t blocked;                /* in S, answered revoked */
+} ctmr_verify_counts;
+typedef struct ctmr_verify_miss {    /* one listed key record: 96 bytes */
+    uint8_t  digest[32];             /* Issuer.ID() digest */
+    int64_t  exp_hour;
+    uint64_t first_index;            /* the record's first-seen global index */
+    uint8_t  serial_len;
+    uint8_t  serial[CTMR_MAX_SERIAL]; /* zero padded */
+    uint8_t  blocked;                /* 0: an R record answered not revoked; 1: an S record answered revoked */
+    uint8_t  pad[7];
+} ctmr_verify_miss;
+typedef struct ctmr_verify_out {     /* caller-allocated; HOST buffers */
+    uint8_t* crl_status;             /* [n_crls] CTMR_CRL_*, as ctmr_revoked_known; may be NULL */
+    uint32_t issuers;                /* covered (the cascade's rule) */
+    uint32_t levels;                 /* levels of the filter */
+    ctmr_verify_counts before;       /* records first seen at a global index < covered_below */
+    ctmr_verify_counts since;        /* the others */
+    ctmr_verify_miss* list; uint64_t list_cap;
+    uint64_t n_list;                 /* written; on CTMR_E_BATCH_TOO_LARGE the count needed */
+} ctmr_verify_out;
+int ctmr_revoked_verify(ctmr_ctx* ctx, const ctmr_crl_batch* batch, int64_t now_unix_sec,
+                        const uint8_t* filter, uint64_t filter_bytes, const uint8_t* stashes, uint64_t stash_bytes,
+                        uint64_t covered_below, ctmr_verify_out* out);
+
 /* ---- device-resident entry points ---------------------------------------------------------- */
 /* Same path with every buffer already in HBM on ctx's device (benchmarks, multi-GPU orchestration,
  * hosts that receive entries by GPUDirect).  `stream` is a cudaStream_t passed as void*; NULL =
@@ -611,6 +676,11 @@ int ctmr_group_revoked_cascade(ctmr_group* g, const ctmr_crl_batch* batch, int64
  * member queries the filter for its own R records, and the host merges the candidates. */
 int ctmr_group_revoked_stash(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter,
                              uint64_t filter_bytes, const uint8_t* stashes, uint64_t stash_bytes, ctmr_stash_out* out);
+/* ctmr_revoked_verify over every shard, the same counts and list as one ctx: the cascade's mark and split and the
+ * stashes' mark on every member, each member verifies its own shard, and the host sums the counts and merges the lists. */
+int ctmr_group_revoked_verify(ctmr_group* g, const ctmr_crl_batch* batch, int64_t now_unix_sec, const uint8_t* filter,
+                              uint64_t filter_bytes, const uint8_t* stashes, uint64_t stash_bytes, uint64_t covered_below,
+                              ctmr_verify_out* out);
 
 /* ---- several GPUs, one PROCESS PER GPU (torchrun-style launches; SURVEY.md §8(e)) ------------------------------ */
 /* Every rank creates its ctx with the same capacities, exports a handle, gathers all handles by whatever means the

@@ -34,6 +34,7 @@ EXPORTS = [
     "ctmr_process_device", "ctmr_read_histogram_device",
     "ctmr_check_device", "ctmr_reset_device", "ctmr_profile_last", "ctmr_preload_known", "ctmr_snapshot_size",
     "ctmr_snapshot_save", "ctmr_snapshot_load", "ctmr_checkpoint_size", "ctmr_checkpoint_save", "ctmr_checkpoint_load",
+    "ctmr_checkpoint_delta_size", "ctmr_checkpoint_delta_save", "ctmr_checkpoint_apply",
     "ctmr_evict_expired", "ctmr_sha256_ceiling_device", "ctmr_synth_offsets_device", "ctmr_synth_write_device", "ctmr_synth_truth_device", "ctmr_synth_issuers_host", "ctmr_synth_raw_pages_host",
     "ctmr_synth_tiles_host",
     "ctmr_process_raw", "ctmr_group_process_raw", "ctmr_frontend_profile_last",  # include/ctmr_frontend.h
@@ -49,6 +50,7 @@ EXPORTS = [
     "ctmr_group_table_stats", "ctmr_group_preload_known", "ctmr_group_evict_expired", "ctmr_group_reset",
     "ctmr_group_snapshot_size", "ctmr_group_snapshot_save", "ctmr_group_snapshot_load",
     "ctmr_group_checkpoint_size", "ctmr_group_checkpoint_save", "ctmr_group_checkpoint_load",
+    "ctmr_group_checkpoint_delta_size", "ctmr_group_checkpoint_delta_save", "ctmr_group_checkpoint_apply",
     "ctmr_peer_export", "ctmr_peer_attach", "ctmr_peer_barrier_device", "ctmr_peer_allreduce_histogram_device",
     "ctmr_bind_host_to_device", "ctmr_peer_rounds", "ctmr_peer_round_entries", "ctmr_peer_frontend_stopped",
     "ctmr_next_index",
@@ -65,6 +67,7 @@ GROUP_TWINS = (
     "checkpoint_load", "process_raw", "process_raw_tree", "process_raw_trees", "process_raw_bodies", "process_raw_bodies_tree",
     "process_raw_bodies_trees", "process_tiles", "process_tiles_tree", "process_tiles_trees", "register_chain_certs",
     "revoked_known", "revoked_cascade", "revoked_stash", "revoked_verify", "resize", "table_occupancy",
+    "checkpoint_delta_size", "checkpoint_delta_save", "checkpoint_apply",
 )
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -279,6 +282,9 @@ def load():
     L.ctmr_checkpoint_size.argtypes = [vp, C.POINTER(u64)]
     L.ctmr_checkpoint_save.argtypes = [vp, vp, u64, C.POINTER(u64)]
     L.ctmr_checkpoint_load.argtypes = [vp, vp, vp, u32]
+    L.ctmr_checkpoint_delta_size.argtypes = [vp, u64, C.POINTER(u64)]
+    L.ctmr_checkpoint_delta_save.argtypes = [vp, u64, vp, u64, C.POINTER(u64)]
+    L.ctmr_checkpoint_apply.argtypes = [vp, vp, vp, u32]
     L.ctmr_resize.argtypes = [vp, u64, u32, u32]
     L.ctmr_table_occupancy.argtypes = [vp, vp, vp]
     L.ctmr_evict_expired.argtypes = [vp, i64, C.POINTER(u64)]

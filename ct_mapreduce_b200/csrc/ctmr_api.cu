@@ -984,11 +984,12 @@ int ctmr_reset_device(ctmr_ctx* c, void* stream) {
     // its own epoch, which is the owner's.
     int rc = peer_barrier(c, CH_RESET_A, s);
     if (rc == CTMR_OK) rc = reset_tables(c, s);
+    delta_floor_at(c, c->next_index);  // a member of a group: ctmr_group_reset sets member 0's at the group's index
     return rc ? rc : peer_barrier(c, CH_RESET_B, s);
 }
 
 int ctmr_group_reset(ctmr_group* g) {
-    return on_group(g, [](ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed) -> int {
+    return on_group(g, [](ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed) -> int {
         for (uint32_t r = 0; r < W; ++r) {  // nobody may still be inserting into a shard when it is cleared
             cudaSetDevice(m[r]->device);
             cudaDeviceSynchronize();
@@ -997,6 +998,7 @@ int ctmr_group_reset(ctmr_group* g) {
             ctmr_ctx* c = m[r];
             *failed = c;
             const int rc = ctmr_reset_device(c, nullptr);
+            delta_floor_at(m[0], *next_index);  // after the member's own
             if (rc) return rc;
             if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(c, CTMR_E_CUDA, "reset failed");
         }
@@ -1307,6 +1309,7 @@ int snapshot_load_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_c
     }
     *failed = c0;
     *next_index = h.next_index;
+    delta_floor_at(c0, *next_index);
     return snap_registry_restore(c0, p, h.n_issuers, u);
 }
 
@@ -1391,6 +1394,10 @@ int table_stats_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, 
     return CTMR_OK;
 }
 
+}  // namespace
+
+namespace ctmr_host {
+
 // Redis TTLs firing (SURVEY §8(f)-4): every set "serials::<expDate>::<issuer>" carries EXPIREAT(expDate)
 // (storage/knowncertificates.go:44-47,98-104), so at `now` the sets with expDate <= now no longer exist.  One shard: the
 // expired keys it holds go, *evicted their number.
@@ -1432,8 +1439,12 @@ int evict_shard(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted) {
     return ctmr_check_device(c, nullptr);
 }
 
+}  // namespace ctmr_host
+
+namespace {
+
 // every shard drops the expired sets it owns
-int evict_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, int64_t now_unix_sec, uint64_t* evicted_out) {
+int evict_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** failed, int64_t now_unix_sec, uint64_t* evicted_out) {
     uint64_t total = 0;
     for (uint32_t r = 0; r < W; ++r) {
         *failed = m[r];
@@ -1442,6 +1453,7 @@ int evict_members(ctmr_ctx** m, uint32_t W, uint64_t*, ctmr_ctx** failed, int64_
         if (rc) return rc;
         total += e;
     }
+    note_eviction(m[0], *next_index, now_unix_sec);
     if (evicted_out) *evicted_out = total;
     return CTMR_OK;
 }

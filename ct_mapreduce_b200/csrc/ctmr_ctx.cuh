@@ -454,6 +454,12 @@ struct ctmr_ctx {
     DeviceState st{};
     FilterCfg filter{};
     uint64_t next_index = 0;
+    // delta checkpoints (ctmr_checkpoint.cu), kept by the ctx, by member 0 of a group and by every peer rank: the next
+    // index at the last call that removed records other than by eviction (a reset or a load), and the evictions since,
+    // as (next index at the call, now) with the indices rising and the nows falling, so that the first mark at or above
+    // an index holds the highest now passed from that index on
+    uint64_t delta_floor = 0;
+    std::vector<std::pair<uint64_t, int64_t>> evict_marks;
     uint64_t stage_entries = 0, stage_bytes = 0;
     std::unique_ptr<Stage[]> stages;  // [kStages], ensure_stages
     // shared region + the views of every rank's region (a single GPU is a group of one)
@@ -657,6 +663,24 @@ int ensure_device_path(ctmr_ctx* c, uint64_t n);   // what ctmr_process_device n
 int reset_tables(ctmr_ctx* c, cudaStream_t s);
 // after the registry was replaced: the host memos of it go, and so do the Chain[0] mirror and the tiles' fingerprints
 int clear_issuer_memos(ctmr_ctx* c);
+// one shard's TTL eviction at now_unix_sec (ctmr_evict_expired), *evicted its expired keys
+int evict_shard(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted);
+// the delta state of the ctx that holds it (member 0 of a group): records were removed other than by eviction, and the
+// state stands at next_index; an eviction at now_unix_sec while the state stood at next_index; the highest now of an
+// eviction from `since` on (INT64_MIN when none)
+inline void delta_floor_at(ctmr_ctx* c, uint64_t next_index) {
+    c->delta_floor = next_index;
+    c->evict_marks.clear();
+}
+inline void note_eviction(ctmr_ctx* c, uint64_t next_index, int64_t now_unix_sec) {
+    while (!c->evict_marks.empty() && c->evict_marks.back().second <= now_unix_sec) c->evict_marks.pop_back();
+    c->evict_marks.emplace_back(next_index, now_unix_sec);
+}
+inline int64_t evicted_since(const ctmr_ctx* c, uint64_t since) {
+    for (const auto& mk : c->evict_marks)
+        if (mk.first >= since) return mk.second;
+    return INT64_MIN;
+}
 
 // A failure of one ctx, a group or a peer rank in a CRL call.  One ctx or a group stops at the first; a peer rank that
 // failed after its first agreement does no more work but still meets every barrier and agreement of the call.  The first
@@ -713,13 +737,14 @@ struct CompactPlan {
     uint64_t live() const { return host.empty() ? 0 : host.back(); }
 };
 template <class Slot>
-int compact_plan(ctmr_ctx* c, const Slot* table, uint64_t n_slots, int64_t now_sec, CompactPlan& p) {
+int compact_plan(ctmr_ctx* c, const Slot* table, uint64_t n_slots, int64_t now_sec, CompactPlan& p, uint64_t since = 0) {
     const uint64_t tiles = (n_slots + kCompactTile - 1) / kCompactTile;
     DevBuf<uint32_t> counts;
     std::vector<uint32_t> h(tiles);
     CU(c, alloc(counts, tiles));
     CU(c, alloc(p.dev, tiles + 1));
-    CU(c, launch_evict_compact(table, n_slots, c->st.epoch, now_sec, 0, tiles, (const unsigned long long*)nullptr, (Slot*)nullptr, counts.get(), c->stream));
+    CU(c, launch_evict_compact(table, n_slots, c->st.epoch, now_sec, 0, tiles, (const unsigned long long*)nullptr, (Slot*)nullptr, counts.get(), c->stream,
+                               since));
     CU(c, cudaMemcpyAsync(h.data(), counts, tiles * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CU(c, cudaStreamSynchronize(c->stream));
     p.host.assign(tiles + 1, 0);

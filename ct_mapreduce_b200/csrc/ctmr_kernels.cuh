@@ -222,11 +222,11 @@ cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned 
 // Ordered compaction of a table's live slots at `epoch` (KnownSlot: ready and hour * 3600 > now_sec; PairSlot / MetaSlot:
 // ready), over tiles [t0, t1) of kCompactTile slots.  counts != NULL: counts[b - t0] = live slots of tile b.  Otherwise tile
 // b's live slots go to keep[base[b] - base[t0] ...] in slot order and in canonical form (base = exclusive prefix of the
-// counts over every tile).
+// counts over every tile).  since > 0: only the slots whose first-seen index is at or above it (a delta checkpoint).
 constexpr uint32_t kCompactTile = 4096;
 template <class Slot>
 cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, uint32_t epoch, int64_t now_sec, uint64_t t0, uint64_t t1,
-                                 const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s);
+                                 const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s, uint64_t since = 0);
 // a snapshot's canonical slots, just copied into the tables, as live at st.epoch (ctmr_common.cuh stamp_slot)
 cudaError_t launch_stamp_tables(const DeviceState& st, int sm_count, cudaStream_t s);
 // the slots live at epoch `from` as live at `to` (ctmr_common.cuh restamp_word)
@@ -238,6 +238,9 @@ cudaError_t launch_evict_reinsert(const DeviceState& st, const KnownSlot* keep, 
 // a checkpoint's pair records and string identities into this rank's tables (owner-filtered, checked the same way)
 cudaError_t launch_ckpt_pairs(const DeviceState& st, const PairSlot* rec, uint64_t n, uint32_t n_issuers, cudaStream_t s);
 cudaError_t launch_ckpt_meta(const DeviceState& st, const MetaSlot* rec, uint64_t n, cudaStream_t s);
+// a delta checkpoint's apply: the per-issuer histogram and every pair count of this rank rebuilt from its ready keys (a
+// key whose (issuer, hour) slot is missing raises CTMR_E_INVALID)
+cudaError_t launch_recount(const DeviceState& st, int sm_count, cudaStream_t s);
 cudaError_t launch_cardinality(const DeviceState& st, int32_t exp_hour, uint32_t issuer, unsigned long long* out,
                                cudaStream_t s);
 // ctmr_resize: one pass over an old table of n_old slots, each slot ready at `epoch` inserted into the tables of `to` (its

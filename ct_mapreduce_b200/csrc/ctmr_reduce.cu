@@ -442,16 +442,21 @@ __global__ void __launch_bounds__(256) evict_count_kernel(DeviceState st, int64_
 // with counts set, counts[b] = its live slots; otherwise it writes them from keep[base[t0 + b] - base[t0]] on, in slot
 // order (a ballot per warp and a scan over the CTA's eight warps per row of 256 slots).  Two runs over the same state
 // write the same bytes.
-__device__ __forceinline__ bool slot_live(const KnownSlot& sl, uint32_t epoch, int64_t now_sec) {
-    return slot_state(sl.tag, epoch) == kSlotReady && (int64_t)(int32_t)sl.body[0] * 3600 > now_sec;
+// since > 0 (a delta checkpoint) also asks for a first-seen index at or above `since` (inv_first = ~index)
+__device__ __forceinline__ bool slot_live(const KnownSlot& sl, uint32_t epoch, int64_t now_sec, uint64_t since) {
+    return slot_state(sl.tag, epoch) == kSlotReady && (int64_t)(int32_t)sl.body[0] * 3600 > now_sec && ~sl.inv_first >= since;
 }
-__device__ __forceinline__ bool slot_live(const PairSlot& sl, uint32_t epoch, int64_t) { return slot_state(sl.pad, epoch) == kSlotReady; }
-__device__ __forceinline__ bool slot_live(const MetaSlot& sl, uint32_t epoch, int64_t) { return slot_state(sl.pad, epoch) == kSlotReady; }
+__device__ __forceinline__ bool slot_live(const PairSlot& sl, uint32_t epoch, int64_t, uint64_t since) {
+    return slot_state(sl.pad, epoch) == kSlotReady && ~sl.inv_first >= since;
+}
+__device__ __forceinline__ bool slot_live(const MetaSlot& sl, uint32_t epoch, int64_t, uint64_t since) {
+    return slot_state(sl.pad, epoch) == kSlotReady && ~sl.inv_first >= since;
+}
 
 template <class Slot>
 __global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restrict__ table, uint64_t n_slots, uint32_t epoch, int64_t now_sec, uint64_t t0,
                                                             const unsigned long long* __restrict__ base, Slot* __restrict__ keep,
-                                                            uint32_t* __restrict__ counts) {
+                                                            uint32_t* __restrict__ counts, uint64_t since) {
     __shared__ uint32_t warp_n[8];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint64_t tile = t0 + blockIdx.x;
@@ -459,7 +464,7 @@ __global__ void __launch_bounds__(256) evict_compact_kernel(const Slot* __restri
     uint32_t total = 0;
     for (uint32_t row = 0; row < kCompactTile / 256u; ++row) {
         const uint64_t i = tile * kCompactTile + row * 256u + threadIdx.x;
-        const bool live = i < n_slots && slot_live(table[i], epoch, now_sec);
+        const bool live = i < n_slots && slot_live(table[i], epoch, now_sec, since);
         const uint32_t ball = __ballot_sync(0xffffffffu, live);
         if (lane == 0) warp_n[warp] = __popc(ball);
         __syncthreads();
@@ -530,23 +535,74 @@ __global__ void __launch_bounds__(256) ckpt_meta_kernel(DeviceState st, const Me
     meta_insert_at<false>(st.meta, st.meta_mask, st.epoch, st.error_flag, m.h1, m.h2, m.inv_first, st.meta_mask);
 }
 
+// A delta checkpoint's apply: every (issuer, hour) count and the per-issuer histogram again, from the ready keys alone (the
+// delta carries no old pair, whose count changed).  Pass 1 zeroes the pair counts; pass 2 adds each key to its issuer and
+// to its set's slot, found with the cardinality lookup's probe (a key and its set have one owner, so the slot is local).
+// A key whose set is missing raises CTMR_E_INVALID.  One atomic per distinct issuer / set per warp.
+__global__ void __launch_bounds__(256) recount_zero_kernel(PairSlot* __restrict__ pairs, uint64_t n) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) pairs[i].count = 0ull;
+}
+__global__ void __launch_bounds__(256) recount_kernel(DeviceState st) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    const uint64_t end = (st.table_mask + 1 + stride - 1) / stride * stride;  // every lane runs the same trips: the warp votes stay whole
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+        bool live = false;
+        uint32_t issuer = 0;
+        unsigned long long pk = 0;
+        if (i <= st.table_mask) {
+            const KnownSlot& sl = st.table[i];
+            live = slot_state(sl.tag, st.epoch) == kSlotReady && sl.body[1] < st.max_issuers;
+            issuer = sl.body[1];
+            pk = ((((unsigned long long)issuer) << 32) | sl.body[0]) + 1ull;
+        }
+        const uint32_t lmask = __ballot_sync(0xffffffffu, live);
+        if (!live) continue;
+        const uint32_t lane = threadIdx.x & 31u;
+        const uint32_t same_issuer = __match_any_sync(lmask, issuer);
+        if (lane == (uint32_t)__ffs(same_issuer) - 1u) atomicAdd(st.issuer_counts + issuer, (unsigned long long)__popc(same_issuer));
+        const uint32_t same_set = __match_any_sync(lmask, pk);
+        if (lane != (uint32_t)__ffs(same_set) - 1u) continue;
+        uint64_t pos = mix64(pk) & st.pair_mask;
+        bool found = false;
+        for (uint64_t probes = 0; probes <= st.pair_mask; ++probes) {  // to the key or an empty slot (the probe rule, ctmr_common.cuh)
+            const PairSlot& p = st.pairs[pos];
+            if (slot_state(p.pad, st.epoch) == 0u) break;
+            if (p.key == pk) {
+                atomicAdd(&st.pairs[pos].count, (unsigned long long)__popc(same_set));
+                found = true;
+                break;
+            }
+            pos = (pos + 1) & st.pair_mask;
+        }
+        if (!found) atomicExch(st.error_flag, CTMR_E_INVALID);
+    }
+}
+
+cudaError_t launch_recount(const DeviceState& st, int sm_count, cudaStream_t s) {
+    cudaError_t e = cudaMemsetAsync(st.issuer_counts, 0, st.max_issuers * sizeof(unsigned long long), s);
+    if (e != cudaSuccess) return e;
+    recount_zero_kernel<<<sm_count * 4, 256, 0, s>>>(st.pairs, st.pair_mask + 1);
+    recount_kernel<<<sm_count * 8, 256, 0, s>>>(st);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_evict_count(const DeviceState& st, int64_t now_sec, unsigned long long* counters, int sm_count, cudaStream_t s) {
     evict_count_kernel<<<sm_count * 8, 256, 0, s>>>(st, now_sec, counters);
     return cudaGetLastError();
 }
 template <class Slot>
 cudaError_t launch_evict_compact(const Slot* table, uint64_t n_slots, uint32_t epoch, int64_t now_sec, uint64_t t0, uint64_t t1,
-                                 const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s) {
+                                 const unsigned long long* base, Slot* keep, uint32_t* counts, cudaStream_t s, uint64_t since) {
     if (t1 <= t0) return cudaSuccess;
-    evict_compact_kernel<Slot><<<(unsigned)(t1 - t0), 256, 0, s>>>(table, n_slots, epoch, now_sec, t0, base, keep, counts);
+    evict_compact_kernel<Slot><<<(unsigned)(t1 - t0), 256, 0, s>>>(table, n_slots, epoch, now_sec, t0, base, keep, counts, since);
     return cudaGetLastError();
 }
 template cudaError_t launch_evict_compact<KnownSlot>(const KnownSlot*, uint64_t, uint32_t, int64_t, uint64_t, uint64_t,
-                                                     const unsigned long long*, KnownSlot*, uint32_t*, cudaStream_t);
+                                                     const unsigned long long*, KnownSlot*, uint32_t*, cudaStream_t, uint64_t);
 template cudaError_t launch_evict_compact<PairSlot>(const PairSlot*, uint64_t, uint32_t, int64_t, uint64_t, uint64_t,
-                                                    const unsigned long long*, PairSlot*, uint32_t*, cudaStream_t);
+                                                    const unsigned long long*, PairSlot*, uint32_t*, cudaStream_t, uint64_t);
 template cudaError_t launch_evict_compact<MetaSlot>(const MetaSlot*, uint64_t, uint32_t, int64_t, uint64_t, uint64_t,
-                                                    const unsigned long long*, MetaSlot*, uint32_t*, cudaStream_t);
+                                                    const unsigned long long*, MetaSlot*, uint32_t*, cudaStream_t, uint64_t);
 
 template <class Slot>
 __global__ void __launch_bounds__(256) stamp_kernel(Slot* __restrict__ table, uint64_t n_slots, uint32_t epoch) {

@@ -905,12 +905,32 @@ class GpuCertDatabase:
     def load_checkpoint(self, parts):
         """Replace the state with a checkpoint: `parts` = every part of it (a list of arrays, any order) or its one part.
         Collective on a db attached to peers."""
+        self._parts_call("checkpoint_load", parts)
+
+    def _parts_call(self, name, parts):
         if isinstance(parts, np.ndarray):
             parts = [parts]
         parts = [np.ascontiguousarray(p, np.uint8) for p in parts]
         ptrs = (C.c_void_p * max(len(parts), 1))(*[p.ctypes.data for p in parts])
         sizes = (C.c_uint64 * max(len(parts), 1))(*[p.size for p in parts])
-        self._check(self._c("checkpoint_load")(self._h, ptrs, sizes, len(parts)))
+        self._check(self._c(name)(self._h, ptrs, sizes, len(parts)))
+
+    def checkpoint_delta(self, since: int) -> np.ndarray:
+        """This db's part of a delta checkpoint (ctmr_checkpoint_delta_save): the records first seen at or above `since`,
+        the next index kept with an earlier checkpoint or delta, with the whole registry and the status counters.
+        Collective on a db attached to peers."""
+        need = C.c_uint64(0)
+        self._check(self._c("checkpoint_delta_size")(self._h, int(since), C.byref(need)))
+        buf = np.empty(max(need.value, 1), np.uint8)
+        wrote = C.c_uint64(0)
+        self._check(self._c("checkpoint_delta_save")(self._h, int(since), capi.ptr(buf), buf.size, C.byref(wrote)))
+        return buf[:wrote.value]
+
+    def apply_checkpoint_delta(self, parts):
+        """Put a delta checkpoint on top of the state (ctmr_checkpoint_apply): `parts` = every part of it (a list of
+        arrays, any order) or its one part.  The state must stand at the delta's `since`.  Collective on a db attached
+        to peers."""
+        self._parts_call("checkpoint_apply", parts)
 
     def evict_expired(self, now_unix_sec: int) -> int:
         """Apply the Redis TTLs (EXPIREAT(expDate) on every serials:: set, knowncertificates.go:98-104): sets with

@@ -24,6 +24,7 @@ package ctmr
 import "C"
 
 import (
+	"encoding/binary"
 	"fmt"
 	"runtime"
 	"unsafe"
@@ -487,9 +488,74 @@ func (d *DB) Checkpoint() ([]byte, error) {
 	return buf[:int(wrote)], d.err(rc, "ctmr_checkpoint_save")
 }
 
-// LoadCheckpoint replaces the state with a checkpoint: every part of it, in any order.  The parts' addresses go to the
-// library in a C-allocated table, and the parts are pinned for the call (cgo's rule on Go pointers in C memory).
+// LoadCheckpoint replaces the state with a checkpoint: every part of it, in any order.
 func (d *DB) LoadCheckpoint(parts ...[]byte) error {
+	return withParts(parts, func(ptrs **C.uint8_t, sizes *C.uint64_t, n C.uint32_t) error {
+		if d.g != nil {
+			return d.err(C.ctmr_group_checkpoint_load(d.g, ptrs, sizes, n), "ctmr_group_checkpoint_load")
+		}
+		return d.err(C.ctmr_checkpoint_load(d.h, ptrs, sizes, n), "ctmr_checkpoint_load")
+	})
+}
+
+// CheckpointDelta returns this DB's part of a delta checkpoint (ctmr_checkpoint_delta_save): the records first seen at
+// or above since, the next index kept with the previous checkpoint or delta (NextIndex at that save, or PartNextIndex of its part).  A DB attached to
+// peers saves its own part, collectively.  Refused when since lies past the next index or before the last reset or
+// load: take a full Checkpoint there.
+func (d *DB) CheckpointDelta(since uint64) ([]byte, error) {
+	var need, wrote C.uint64_t
+	var rc C.int
+	if d.g != nil {
+		rc = C.ctmr_group_checkpoint_delta_size(d.g, C.uint64_t(since), &need)
+	} else {
+		rc = C.ctmr_checkpoint_delta_size(d.h, C.uint64_t(since), &need)
+	}
+	if err := d.err(rc, "ctmr_checkpoint_delta_size"); err != nil {
+		return nil, err
+	}
+	buf := make([]byte, int(need)+1) // never empty: &buf[0] is valid
+	if d.g != nil {
+		rc = C.ctmr_group_checkpoint_delta_save(d.g, C.uint64_t(since), (*C.uint8_t)(unsafe.Pointer(&buf[0])), need, &wrote)
+	} else {
+		rc = C.ctmr_checkpoint_delta_save(d.h, C.uint64_t(since), (*C.uint8_t)(unsafe.Pointer(&buf[0])), need, &wrote)
+	}
+	return buf[:int(wrote)], d.err(rc, "ctmr_checkpoint_delta_save")
+}
+
+// ApplyCheckpointDelta puts a delta checkpoint on top of the state (ctmr_checkpoint_apply): every part of it, in any
+// order.  The state must stand at the delta's since: the base checkpoint loaded and the earlier deltas applied in order.
+func (d *DB) ApplyCheckpointDelta(parts ...[]byte) error {
+	return withParts(parts, func(ptrs **C.uint8_t, sizes *C.uint64_t, n C.uint32_t) error {
+		if d.g != nil {
+			return d.err(C.ctmr_group_checkpoint_apply(d.g, ptrs, sizes, n), "ctmr_group_checkpoint_apply")
+		}
+		return d.err(C.ctmr_checkpoint_apply(d.h, ptrs, sizes, n), "ctmr_checkpoint_apply")
+	})
+}
+
+// NextIndex is the global index the next entry stored takes (ctmr_next_index).  One ctx only: a group has no index of
+// its own to read; use PartNextIndex of its last checkpoint or delta part.
+func (d *DB) NextIndex() (uint64, error) {
+	if d.g != nil {
+		return 0, fmt.Errorf("a group has no ctmr_next_index: use PartNextIndex")
+	}
+	var n C.uint64_t
+	err := d.err(C.ctmr_next_index(d.h, &n), "ctmr_next_index")
+	return uint64(n), err
+}
+
+// PartNextIndex is the next index a checkpoint or delta part was saved at: the since of the next delta.  Both headers
+// keep it as the little-endian uint64 at byte 24.
+func PartNextIndex(part []byte) (uint64, error) {
+	if len(part) < 128 {
+		return 0, fmt.Errorf("truncated checkpoint part")
+	}
+	return binary.LittleEndian.Uint64(part[24:32]), nil
+}
+
+// withParts calls call with the parts' addresses and sizes in C-allocated tables, the parts pinned for the call (cgo's
+// rule on Go pointers in C memory).
+func withParts(parts [][]byte, call func(ptrs **C.uint8_t, sizes *C.uint64_t, n C.uint32_t) error) error {
 	if len(parts) == 0 {
 		return fmt.Errorf("no checkpoint parts")
 	}
@@ -508,10 +574,7 @@ func (d *DB) LoadCheckpoint(parts ...[]byte) error {
 		ptrs[i] = (*C.uint8_t)(unsafe.Pointer(&p[0]))
 		sizes[i] = C.uint64_t(len(p))
 	}
-	if d.g != nil {
-		return d.err(C.ctmr_group_checkpoint_load(d.g, &ptrs[0], &sizes[0], C.uint32_t(n)), "ctmr_group_checkpoint_load")
-	}
-	return d.err(C.ctmr_checkpoint_load(d.h, &ptrs[0], &sizes[0], C.uint32_t(n)), "ctmr_checkpoint_load")
+	return call(&ptrs[0], &sizes[0], C.uint32_t(n))
 }
 
 // Resize rehashes the known-certificate, (issuer, expDate) and string-identity tables into the given sizes on the

@@ -230,6 +230,52 @@ int ctmr_checkpoint_size(ctmr_ctx* ctx, uint64_t* bytes);
 int ctmr_checkpoint_save(ctmr_ctx* ctx, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_checkpoint_load(ctmr_ctx* ctx, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
 
+/* ---- delta checkpoint --------------------------------------------------------------------------------------------- */
+/* The records added since an earlier checkpoint, and their application on top of the state that checkpoint gave.  Every
+ * record keeps its first-seen index (eviction, resize and loads keep it), so the records added since a checkpoint taken
+ * at next index N are the live ones first seen at or above N.  A delta save reads the whole table on the device and
+ * copies only those records to the host.  HOST buffers.
+ *
+ * Part layout: the checkpoint's, with its own 128-byte header -- magic "CTMRDLT1", u16 part index, u16 part count,
+ * u32 n_issuers, u64 since, u64 next_index, i64 evict_now, u64 status counters [CTMR_ST__COUNT] of this part (totals,
+ * not increments), u64 keys, pairs, string identities -- then the WHOLE registry [n_issuers][32] in dense-index order,
+ * the ready key slots, the (issuer, hour) slots and the string identities whose first-seen index is >= since (64, 32
+ * and 32 B as in a checkpoint).  Bytes = 128 + 32 n_issuers + 64 keys + 32 (pairs + strings).  evict_now is the highest
+ * now_unix_sec passed to ctmr_evict_expired while the state stood at next index >= since (INT64_MIN: none); an
+ * eviction before `since` is already in the state the delta goes on, and repeating it would drop the keys stored after
+ * it.  A ctx or a group saves one part; a rank attached to peers saves its own, collectively, as ctmr_checkpoint_save.
+ * Two saves of one state with the same since are byte-equal.  In both headers the next index is the u64 at byte 24, so
+ * the since of the next delta can be read from the last part saved (a group has no ctmr_next_index).  Deltas follow the
+ * handle's next index: ctmr_map_device / ctmr_process_device take their indices from the caller and do not move it.
+ *
+ * Save refusals (CTMR_E_INVALID, nothing written): since > next index; since below the DELTA FLOOR, the next index at
+ * the last call that removed records other than by eviction (ctmr_reset_device / ctmr_group_reset, ctmr_snapshot_load,
+ * ctmr_checkpoint_load, and a failed ctmr_checkpoint_apply, which leaves a reset state).  A delta cannot express a
+ * reset: take a full checkpoint there.  ctmr_resize and a successful apply keep every record and its index, and do not
+ * move the floor.
+ *
+ * Apply puts one delta (every part of it, any order) on top of the target's state; the target may have any shape and
+ * capacities.  Every check runs before anything changes: magic and truncation, part count and indices, the same since,
+ * next index and registry in every part, the target's next index == since (deltas go on in order, with no gap), the
+ * target's registry a prefix of the delta's, the registry within max_issuers.  Then: the new digests are registered in
+ * order (digest i keeps index i); if evict_now (the highest over the parts) is above every eviction the target made at
+ * its current index, every member evicts at evict_now; the records go in as a load puts them (each member / rank keeps
+ * the ones it owns); every (issuer, hour) count and the per-issuer histogram are rebuilt from the live keys; the status
+ * counters (on member 0 / rank 0) and the next index become the delta's.  The Chain[0] mirror and the fingerprints stay.
+ * Failures: a failed check (CTMR_E_INVALID; CTMR_E_TOO_MANY_ISSUERS) changes nothing; CTMR_E_*TABLE_FULL or a record out
+ * of range during the inserts leaves the target as after a reset, with the delta's registry: resize, then replay the
+ * base checkpoint and its deltas.  On peer ranks apply is collective with ctmr_checkpoint_load's two agreements.
+ *
+ * The contract: a full checkpoint C0 at next index N0, deltas D1 (since N0) ... Dk (since N(k-1)) saved later, with any
+ * calls between them (batches, front-end calls, preloads, evictions, resizes).  ctmr_checkpoint_load(C0) and
+ * ctmr_checkpoint_apply(D1) ... (Dk) into any shape give every later call the result that loading a full checkpoint
+ * taken at Dk's point gives in that shape: every ctmr_out field and front-end output, ctmr_issuer_counts,
+ * ctmr_set_cardinality, ctmr_status_counters, ctmr_next_index and the CRL calls; the checkpoint records, parsed and
+ * sorted, are equal.  A member ctx of an in-process group is refused: use ctmr_group_checkpoint_*. */
+int ctmr_checkpoint_delta_size(ctmr_ctx* ctx, uint64_t since, uint64_t* bytes);
+int ctmr_checkpoint_delta_save(ctmr_ctx* ctx, uint64_t since, uint8_t* buf, uint64_t cap, uint64_t* written);
+int ctmr_checkpoint_apply(ctmr_ctx* ctx, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
+
 /* ---- resize ------------------------------------------------------------------------------------------------------- */
 /* The known-certificate, (issuer, expDate) and string-identity tables in other sizes, rehashed on the device: what
  * checkpoint save, destroy, create, checkpoint load and registering the chain certificates again would do, without
@@ -660,6 +706,11 @@ int ctmr_group_snapshot_load(ctmr_group* g, const uint8_t* buf, uint64_t bytes);
 int ctmr_group_checkpoint_size(ctmr_group* g, uint64_t* bytes);
 int ctmr_group_checkpoint_save(ctmr_group* g, uint8_t* buf, uint64_t cap, uint64_t* written);
 int ctmr_group_checkpoint_load(ctmr_group* g, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
+/* delta checkpoint of the whole group (one part; member 0 holds the delta floor and the evictions), and a delta applied
+ * onto it (ctmr_checkpoint_delta_*, ctmr_checkpoint_apply) */
+int ctmr_group_checkpoint_delta_size(ctmr_group* g, uint64_t since, uint64_t* bytes);
+int ctmr_group_checkpoint_delta_save(ctmr_group* g, uint64_t since, uint8_t* buf, uint64_t cap, uint64_t* written);
+int ctmr_group_checkpoint_apply(ctmr_group* g, const uint8_t* const* parts, const uint64_t* part_bytes, uint32_t n_parts);
 /* ctmr_resize of every shard, all or nothing: each member's tables get the given size (0 keeps it), every member's new
  * tables are built and rehashed before any old ones go, and a failure of one member leaves every member unchanged */
 int ctmr_group_resize(ctmr_group* g, uint64_t table_capacity, uint32_t pair_capacity_log2, uint32_t meta_capacity_log2);

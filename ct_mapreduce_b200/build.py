@@ -15,7 +15,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libctmr.so")
-SOURCES = ["ctmr_map.cu", "ctmr_reduce.cu", "ctmr_api.cu", "ctmr_checkpoint.cu", "ctmr_resize.cu", "ctmr_pipeline.cu", "ctmr_frontend.cu", "ctmr_frontend_api.cu", "ctmr_tiles.cu", "ctmr_merkle.cu", "ctmr_json.cu", "ctmr_crl.cu", "ctmr_cascade.cu", "ctmr_synth_kernels.cu", "ctmr_synth_pages.cu"]
+SOURCES = ["ctmr_map.cu", "ctmr_reduce.cu", "ctmr_api.cu", "ctmr_checkpoint.cu", "ctmr_resize.cu", "ctmr_rollback.cu", "ctmr_pipeline.cu", "ctmr_frontend.cu", "ctmr_frontend_api.cu", "ctmr_tiles.cu", "ctmr_merkle.cu", "ctmr_json.cu", "ctmr_crl.cu", "ctmr_cascade.cu", "ctmr_synth_kernels.cu", "ctmr_synth_pages.cu"]
 DEPS = SOURCES + ["ctmr_ctx.cuh", "ctmr_kernels.cuh", "ctmr_common.cuh", "ctmr_stream.cuh", "ctmr_device.cuh", "ctmr_synth.h",
                   "ctmr_synth_ecpoints.inc",
                   os.path.join("..", "..", "include", "ctmr.h"), os.path.join("..", "..", "include", "ctmr_frontend.h")]

@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(HERE, "libctmr.so")
 # per-entry status (include/ctmr.h CTMR_ST_*)
 ST_OK, ST_PARSE_ERR, ST_FILTER_CA, ST_FILTER_EXPIRED, ST_FILTER_CN, ST_NO_ISSUER, ST_ISSUER_PARSE_ERR, ST_SERIAL_TOO_LONG = range(8)
 ST_COUNT = 8
+ROLLBACK_MARKS = 4096   # CTMR_ROLLBACK_MARKS: the call starts a handle keeps for ctmr_rollback
 ISSUER_NONE = 0xFFFFFFFF
 ISSUER_BAD = 0xFFFFFFFE
 F_NO_FINGERPRINT = 1
@@ -59,6 +60,7 @@ EXPORTS = [
     "ctmr_revoked_stash", "ctmr_group_revoked_stash",   # CRLite's stash: what a published filter and its stashes miss
     "ctmr_revoked_verify", "ctmr_group_revoked_verify",   # a published filter and its stashes checked against the table
     "ctmr_resize", "ctmr_group_resize", "ctmr_table_occupancy", "ctmr_group_table_occupancy",   # the tables in other sizes
+    "ctmr_rollback", "ctmr_group_rollback",   # the state back to the start of an earlier call
 ]
 # the calls with a ctmr_group_<name> form beside ctmr_<name>
 GROUP_TWINS = (
@@ -67,7 +69,7 @@ GROUP_TWINS = (
     "checkpoint_load", "process_raw", "process_raw_tree", "process_raw_trees", "process_raw_bodies", "process_raw_bodies_tree",
     "process_raw_bodies_trees", "process_tiles", "process_tiles_tree", "process_tiles_trees", "register_chain_certs",
     "revoked_known", "revoked_cascade", "revoked_stash", "revoked_verify", "resize", "table_occupancy",
-    "checkpoint_delta_size", "checkpoint_delta_save", "checkpoint_apply",
+    "checkpoint_delta_size", "checkpoint_delta_save", "checkpoint_apply", "rollback",
 )
 PEER_HANDLE_BYTES = 256
 PEER_ROUNDS = 8   # default; peer_rounds() asks the library (environment override)
@@ -286,6 +288,7 @@ def load():
     L.ctmr_checkpoint_delta_save.argtypes = [vp, u64, vp, u64, C.POINTER(u64)]
     L.ctmr_checkpoint_apply.argtypes = [vp, vp, vp, u32]
     L.ctmr_resize.argtypes = [vp, u64, u32, u32]
+    L.ctmr_rollback.argtypes = [vp, u64]
     L.ctmr_table_occupancy.argtypes = [vp, vp, vp]
     L.ctmr_evict_expired.argtypes = [vp, i64, C.POINTER(u64)]
     L.ctmr_sha256_ceiling_device.argtypes = [vp, u32, u32, u32, C.POINTER(C.c_float), C.POINTER(u64)]

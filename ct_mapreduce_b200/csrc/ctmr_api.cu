@@ -658,6 +658,9 @@ int ctmr_create(const ctmr_config* cfg, ctmr_ctx** out) {
     point_at_region(c.get());
     CU(nullptr, alloc(c->small, 1));
     CU(nullptr, cudaMemsetAsync(c->small, 0, sizeof(SmallDev), c->stream));
+    CU(nullptr, alloc(c->mark_status, (size_t)CTMR_ROLLBACK_MARKS * CTMR_ST__COUNT));
+    CU(nullptr, create(c->mark_taken));
+    c->mark_index.assign(CTMR_ROLLBACK_MARKS, 0);
     c->st.slots_used = &c->small->slots_used;
     c->st.error_flag = &c->small->error_flag;
     c->st.epoch = 1u;  // the tables were just zeroed: empty at any epoch
@@ -867,7 +870,10 @@ int ctmr_reduce_device(ctmr_ctx* c, const ctmr_key* keys, uint64_t m, uint8_t* w
                      first ? first : c->bits_scratch + m, s);
 }
 
-int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, void* stream) {
+}  // extern "C"
+
+namespace ctmr_host {
+int process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, void* stream, bool mark) {
     if (!c || !b || !o) return fail(c, CTMR_E_INVALID, "bad argument");
     if (b->n && (!b->blob || !b->offsets)) return fail(c, CTMR_E_INVALID, "null batch buffers");
     CU(c, cudaSetDevice(c->device));
@@ -892,6 +898,10 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     const uint64_t per_round = device_round_entries(b->n, (uint32_t)nsub);
     if (coll && per_round > c->px.X)
         return fail(c, CTMR_E_BATCH_TOO_LARGE, "entries per round exceed the key-exchange regions: raise config.max_round_entries to ceil(n / ctmr_peer_rounds())");
+    if (mark) {
+        rc = note_call_start(&c, 1, c->next_index, user);
+        if (rc) return rc;
+    }
     ctmr_dev_out all = *o;  // the outputs the rounds write, scratch where the caller asks for none
     if (!all.keys) all.keys = c->keys_scratch;
     if (!all.was_unknown) all.was_unknown = c->bits_scratch;
@@ -939,6 +949,15 @@ int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out
     CU(c, cudaStreamWaitEvent(user, dp.ev_join_a, 0));
     CU(c, cudaStreamWaitEvent(user, dp.ev_join_b, 0));
     return CTMR_OK;
+}
+}  // namespace ctmr_host
+
+extern "C" {
+
+// the public entry takes a rollback mark at the handle's next index; a member of a group has no index of its own (the
+// group's calls mark the group's), and the front end's chunks run inside a call that took its mark already
+int ctmr_process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, void* stream) {
+    return process_device(c, b, o, stream, c && !c->group);
 }
 
 uint32_t ctmr_peer_rounds(void) { return peer_rounds(); }
@@ -1145,6 +1164,8 @@ int preload_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_ctx** f
         if (owner != c->st.peer.rank)
             return fail(c, CTMR_E_INVALID, "this set is owned by rank " + std::to_string(owner) + " of the group: preload it there");
     }
+    rc = note_call_start(m, W, *next_index);
+    if (rc) return rc;
     const uint64_t first_index = *next_index;
     std::vector<ctmr_key> keys(n);
     for (uint64_t i = 0; i < n; ++i) {

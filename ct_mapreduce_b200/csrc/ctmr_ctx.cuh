@@ -460,6 +460,14 @@ struct ctmr_ctx {
     // an index holds the highest now passed from that index on
     uint64_t delta_floor = 0;
     std::vector<std::pair<uint64_t, int64_t>> evict_marks;
+    // rollback marks (ctmr_rollback.cu): the starts of the last CTMR_ROLLBACK_MARKS entry-taking calls.  Mark k (counted
+    // from the last clear) lives in slot k % CTMR_ROLLBACK_MARKS: its next index on the ctx that holds the delta state,
+    // the status counters at the call's start on every member (copied on the device by the call's stream).
+    std::vector<uint64_t> mark_index;        // [CTMR_ROLLBACK_MARKS]
+    uint64_t marks = 0;                      // marks taken since the last clear; the indices rise
+    uint64_t marks_lo = 0;                   // the marks held are marks_lo .. marks - 1 (their slots not overwritten)
+    DevBuf<unsigned long long> mark_status;  // [CTMR_ROLLBACK_MARKS][CTMR_ST__COUNT]
+    Event mark_taken;                        // recorded after the last mark's copy
     uint64_t stage_entries = 0, stage_bytes = 0;
     std::unique_ptr<Stage[]> stages;  // [kStages], ensure_stages
     // shared region + the views of every rank's region (a single GPU is a group of one)
@@ -671,7 +679,15 @@ int evict_shard(ctmr_ctx* c, int64_t now_unix_sec, uint64_t* evicted);
 inline void delta_floor_at(ctmr_ctx* c, uint64_t next_index) {
     c->delta_floor = next_index;
     c->evict_marks.clear();
+    c->marks = c->marks_lo = 0;  // no rollback reaches across it either
 }
+// A rollback mark for the members m[0..W) of a call that starts at next_index (ctmr_rollback.cu): each member's status
+// counters copied into its ring on the stream `s` (NULL: the member's own stream), then mark_taken recorded there.  A
+// call that starts where the newest mark stands keeps that mark (an earlier call at this index may have changed the
+// state already).  No host wait.
+int note_call_start(ctmr_ctx** m, uint32_t W, uint64_t next_index, cudaStream_t s = nullptr);
+// ctmr_process_device; mark: take the call's rollback mark (the public entry on a handle with an index of its own)
+int process_device(ctmr_ctx* c, const ctmr_dev_batch* b, const ctmr_dev_out* o, void* stream, bool mark);
 inline void note_eviction(ctmr_ctx* c, uint64_t next_index, int64_t now_unix_sec) {
     while (!c->evict_marks.empty() && c->evict_marks.back().second <= now_unix_sec) c->evict_marks.pop_back();
     c->evict_marks.emplace_back(next_index, now_unix_sec);

@@ -1264,7 +1264,7 @@ int count_chunks(ctmr_ctx* c, const Format& fm, uint64_t* chunks) {
 int run_path(ctmr_ctx** m, uint32_t W, uint64_t k, Chunk* cur, bool meta, const PeerCall& pc, ctmr_ctx** failed) {
     if (W == 1 && !pc.on) {
         *failed = m[0];
-        return cur[0].db.n ? ctmr_process_device(m[0], &cur[0].db, &cur[0].dout, m[0]->stream) : CTMR_OK;
+        return cur[0].db.n ? process_device(m[0], &cur[0].db, &cur[0].dout, m[0]->stream, false) : CTMR_OK;
     }
     const int parity = (int)(k % kParities);
     RoundMember rm[kMaxWorld];
@@ -1486,7 +1486,8 @@ template <class Format>
 int front_end_call(ctmr_ctx** m, uint32_t W, uint64_t* next_index, Format fm, const TreeArgs* tree, ctmr_group* g) {
     ctmr_ctx* failed = nullptr;
     PeerCall pc;  // a collective call takes pc.span indices once the ranks agreed, whatever happens after
-    const int rc = process_members(m, W, next_index, fm, tree, pc, &failed);
+    int rc = note_call_start(m, W, *next_index);  // on each member's stream, which runs the path
+    if (rc == CTMR_OK) rc = process_members(m, W, next_index, fm, tree, pc, &failed);
     *next_index += pc.on ? pc.span : rc == CTMR_OK ? fm.entries() : fm.done;
     for (uint32_t r = 0; r < W; ++r) {
         if (m[r]->fe && m[r]->fe->tree) {

@@ -268,6 +268,10 @@ int process_batch_members(ctmr_ctx** m, uint32_t W, uint64_t* next_index, ctmr_c
         if (rc) return rc;
     }
     *failed = c0;
+    rc = note_call_start(m, W, *next_index);
+    if (rc) return rc;
+    for (uint32_t r = 0; r < W; ++r)  // the mark's copy before any round's kernels
+        for (int k = 0; k < kStages; ++k) CU(m[r], cudaStreamWaitEvent(m[r]->stages[k].stream, m[r]->mark_taken, 0));
     // issuers of this batch -> dense indices (GPU work only for certificates never seen before); the registry is
     // shared by the group, so member 0's answer holds for every member
     std::vector<const uint32_t*> map_dev(W, nullptr);

@@ -971,6 +971,15 @@ class GpuCertDatabase:
         exported to peers (E_INVALID on every rank, without a collective call)."""
         self._check(self._c("resize")(self._h, int(table_capacity or 0), int(pair_capacity_log2 or 0), int(meta_capacity_log2 or 0)))
 
+    def rollback(self, next_index: int):
+        """Take the state back to the start of an earlier entry-taking call (ctmr_rollback): every record first seen at or
+        above `next_index` goes, the counts follow the remaining keys, the status counters are those at that call's start
+        and the next index is `next_index`.  It must be the next index at the start of one of the last
+        capi.ROLLBACK_MARKS batch, front-end, device or preload calls, at or above the last reset or load (E_INVALID
+        otherwise, with nothing touched); the current next index does nothing.  The registry and the chain certificates
+        stay; restore your trees yourself.  Collective on a db attached to peers."""
+        self._check(self._c("rollback")(self._h, int(next_index)))
+
     def table_occupancy(self):
         """((used known, pair, meta), (capacity known, pair, meta)): live slots and slots of the three tables
         (ctmr_table_occupancy; a group's are sums over its shards)."""

@@ -25,6 +25,7 @@ import "C"
 
 import (
 	"encoding/binary"
+	"errors"
 	"fmt"
 	"runtime"
 	"unsafe"
@@ -587,6 +588,31 @@ func (d *DB) Resize(tableCapacity uint64, pairLog2, metaLog2 uint32) error {
 		return d.err(C.ctmr_group_resize(d.g, C.uint64_t(tableCapacity), C.uint32_t(pairLog2), C.uint32_t(metaLog2)), "ctmr_group_resize")
 	}
 	return d.err(C.ctmr_resize(d.h, C.uint64_t(tableCapacity), C.uint32_t(pairLog2), C.uint32_t(metaLog2)), "ctmr_resize")
+}
+
+// ErrNoMark is the error Rollback returns (wrapped, with the library's text) when the target is not the start of one of
+// the last CTMR_ROLLBACK_MARKS entry-taking calls, lies above the next index or below the last reset or load: nothing was
+// touched.  Load a checkpoint instead.  These are the only CTMR_E_INVALID refusals a DB can meet: the library's others
+// (a NULL handle, a member ctx of a group) concern handles a DB never holds.
+var ErrNoMark = errors.New("ctmr: no rollback mark at that index")
+
+// Rollback takes the device state back to the start of an earlier entry-taking call (ctmr_rollback /
+// ctmr_group_rollback): the records first seen at or above nextIndex go, the counts follow the remaining keys, the status
+// counters are those at that call's start and the next index is nextIndex.  Then run the call again with the same
+// indices: its outputs are a clean run's.  The registry and the chain certificates stay; restore the trees yourself.
+// Collective on a DB attached to peers.
+func (d *DB) Rollback(nextIndex uint64) error {
+	var rc C.int
+	what := "ctmr_rollback"
+	if d.g != nil {
+		rc, what = C.ctmr_group_rollback(d.g, C.uint64_t(nextIndex)), "ctmr_group_rollback"
+	} else {
+		rc = C.ctmr_rollback(d.h, C.uint64_t(nextIndex))
+	}
+	if rc == C.CTMR_E_INVALID {
+		return fmt.Errorf("%w: %v", ErrNoMark, d.err(rc, what))
+	}
+	return d.err(rc, what)
 }
 
 // TableOccupancy returns the live slots and the slots of the known-certificate, (issuer, expDate) and string-identity

@@ -157,7 +157,8 @@ uint32_t ctmr_issuer_count(ctmr_ctx* ctx);
  * copies the requested outputs back; synchronous.
  * After a failure (rc != 0) the outputs are undefined and part of the batch may already be in the tables; the
  * call's entry indices are consumed either way, so replaying the batch is safe in the reference's own sense
- * (idempotent replays, SURVEY §5): entries that were inserted read as known, never as unknown twice. */
+ * (idempotent replays, SURVEY §5): entries that were inserted read as known, never as unknown twice.  A replay does
+ * not issue the write-back of those entries: ctmr_rollback to the call's start first (see "rollback"). */
 int ctmr_process_batch(ctmr_ctx* ctx, const uint8_t* blob, const uint64_t* offsets /* [n+1] */, uint64_t n,
                        const uint8_t* issuer_blob, const uint64_t* issuer_offsets /* [n_issuers+1] */,
                        uint32_t n_issuers, const uint32_t* issuer_idx /* [n] */, int64_t now_unix_ns,
@@ -316,6 +317,52 @@ int ctmr_resize(ctmr_ctx* ctx, uint64_t table_capacity, uint32_t pair_capacity_l
  * (issuer, expDate), string identities; either array may be NULL.  One count pass per table.  A member ctx of a group
  * reports its own shard; ctmr_group_table_occupancy sums over the members. */
 int ctmr_table_occupancy(ctmr_ctx* ctx, uint64_t used[3], uint64_t capacity[3]);
+
+/* ---- rollback ----------------------------------------------------------------------------------------------------- */
+/* Takes the device state back to the start of an earlier entry-taking call, so that "undo that call, run it again" gives
+ * exactly the outputs of a clean run: the same was_unknown bits, the same write-back and the same indices.  Use it after a
+ * failed batch (part of it may already be in the tables: its entries would read as known on a replay, and their
+ * SetInsert and PEM write would never be issued) and when a tree root does not match the log's STH.
+ *
+ * Semantics.  After ctmr_rollback(ctx, N) returns CTMR_OK the ctx is in exactly the state a checkpoint taken when the
+ * next index was N would load to, followed by ctmr_evict_expired(now) with the highest now evicted since N:
+ *   - every key, (issuer, expDate) and string-identity slot whose first-seen index is >= N is gone; every other slot is
+ *     unchanged, its first-seen index included;
+ *   - every (issuer, expDate) count and the per-issuer histogram equal those of the remaining live keys;
+ *   - the status counters equal their values at the start of the call that began at N;
+ *   - the next index is N.
+ * Not indexed, so kept: the issuer registry, the registered chain certificates, the Chain[0] mirror and the caller's
+ * ctmr_tree structs (keep a copy of the trees from before the call and restore it).
+ *
+ * Valid targets.  N is the next index at the start of an entry-taking call of this ctx or group, failed calls included:
+ * ctmr_process_batch, every front-end call (ctmr_frontend.h), ctmr_process_device and ctmr_preload_known.  Each call
+ * start is a MARK: its next index and the status counters, copied on the device on the call's stream (no host wait).
+ * The ctx keeps the last CTMR_ROLLBACK_MARKS marks; calls that start at the same index keep the first one's.
+ * ctmr_process_device takes its indices from the caller and does not move the handle's next index, so its mark is at
+ * the handle's next index: a rollback to it undoes the device call (its records at or above that index, its status
+ * counts) only once a later host-buffer, front-end or preload call has moved the index past it.  A caller of the device
+ * path alone reaches no earlier state this way (N == the next index does nothing); it keeps its own checkpoints.  The
+ * chunks of a front-end call and a group's members take no mark of their own.
+ * N == the current next index is valid and does nothing.  Refusals (CTMR_E_INVALID, nothing touched): N above the next
+ * index, N not a mark, N below the delta floor (see "delta checkpoint"), a mark that has dropped out of the ring, a NULL
+ * ctx, a member ctx of a group (use ctmr_group_rollback).  A reset, ctmr_snapshot_load and ctmr_checkpoint_load (and a
+ * failed ctmr_checkpoint_apply) clear the marks as they move the delta floor; ctmr_resize keeps them.  Afterwards the
+ * marks above N are gone, the eviction history at or above N counts as made at N (a later delta's evict_now stays
+ * right), and the delta floor is unchanged.
+ * Group.  The group's next index is the one checked; each member restores its own shard and status counters.
+ * Peer ranks (ctmr_peer_attach, world > 1): COLLECTIVE.  The ranks agree on their checks first (every rank needs a mark
+ * at N; a rank whose check fails returns its error, the others CTMR_E_PEER_FAILED, nothing changes); each rank then
+ * rolls its own shard back, and a final agreement makes a failure on one rank every rank's.
+ * Failures.  Every check comes before any work.  Among them, after waiting for the device, the error flag of each
+ * member is read and cleared as ctmr_check_device does: a flag raised by an earlier call that nobody checked (an
+ * asynchronous ctmr_process_device) is returned as that call's failure, with nothing rolled back; call again.  The
+ * deletion works in place: a CUDA error after it started leaves that member's tables undefined and raises its error
+ * flag (ctmr_check_device reports it), as eviction does; load a checkpoint.  On peer ranks the ranks whose own deletion
+ * succeeded stand at N (next index, marks, tables) even when another rank's failed and they return CTMR_E_PEER_FAILED.
+ * Cost: one pass over each table, then per cluster of occupied slots that holds a removed record, one walk over the
+ * cluster from its first removed slot (DESIGN.md §3 "Rollback"). */
+#define CTMR_ROLLBACK_MARKS 4096u
+int ctmr_rollback(ctmr_ctx* ctx, uint64_t next_index);
 
 /* ---- revoked known certificates (CRLite's join of CRLs with the serials:: sets) ------------------- */
 /* Which revoked serials of an issuer's CRLs are known certificates, and in which "serials::<expDate>::<issuer>" set
@@ -715,6 +762,8 @@ int ctmr_group_checkpoint_apply(ctmr_group* g, const uint8_t* const* parts, cons
  * tables are built and rehashed before any old ones go, and a failure of one member leaves every member unchanged */
 int ctmr_group_resize(ctmr_group* g, uint64_t table_capacity, uint32_t pair_capacity_log2, uint32_t meta_capacity_log2);
 int ctmr_group_table_occupancy(ctmr_group* g, uint64_t used[3], uint64_t capacity[3]);   /* summed over the shards */
+/* ctmr_rollback of the group to its own next index N: every member's shard and status counters back to the mark at N */
+int ctmr_group_rollback(ctmr_group* g, uint64_t next_index);
 /* ctmr_revoked_known over every shard: member 0 parses the CRLs and builds the set of (issuer, serial) pairs, each member
  * scans its own table against a bulk copy of it, and member 0 merges the answers (lowest hour, sum of sets). */
 int ctmr_group_revoked_known(ctmr_group* g, const ctmr_crl_batch* batch, ctmr_crl_out* out);
